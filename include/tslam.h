@@ -45,7 +45,7 @@ const char* tslam_last_error(void);
 int tslam_device_count(void);
 /* ABI version of this header (tests check the library agrees). */
 int tslam_abi_version(void);
-#define TSLAM_ABI_VERSION 3
+#define TSLAM_ABI_VERSION 4
 
 /* ----------------------------------------------------------------------------
  * TSDF map  (DenseTSDF, dense_tsdf.py)
@@ -284,6 +284,25 @@ int tslam_esdf_update2(tslam_tsdf_t* m, int32_t submap, int32_t mode, int32_t* s
 /* ESDF of observed voxels: idx int32[cap,3], esdf f32[cap] (DEVICE). Synchronises. */
 int tslam_esdf_gather(tslam_tsdf_t* m, int32_t submap, int64_t cap, int32_t* idx, float* esdf, int64_t* n_out,
                       void* stream);
+/* Reading the field.  Both calls answer from the field as of the last tslam_esdf_update* of `submap`: integrating
+ * more frames does not change their answers until the next update, and voxels of blocks allocated since then count
+ * as unknown.  Both return TSLAM_E_INVALID when no update has completed, when the last update was for another
+ * submap, or when a reset, load (scatter), fusion or ghost import has happened since.  Neither synchronises.
+ *
+ * Batched distance and gradient queries (what Voxblox answers for planners).  xyz f32[n,3] (DEVICE) are points in
+ * the submap's own map frame - voxel i is centred at i*voxel_scale, no submap base pose is applied - like the other
+ * planner queries.  Per point: dist f32[n] = trilinear interpolation of the ESDF over the 8 voxels around the point,
+ * grad f32[n,3] = the exact partial derivatives of that interpolant (m/m), valid u8[n] = 1 when it is defined.
+ * Undefined (valid 0, dist and grad NaN): a non-finite coordinate, a corner outside the volume, a corner that was
+ * unobserved at the last update or whose TSDF was NaN.  n == 0 is a no-op. */
+int tslam_esdf_query(tslam_tsdf_t* m, int32_t submap, int64_t n, const float* xyz, float* dist, float* grad,
+                     uint8_t* valid, void* stream);
+/* cvt_ESDF_to_voxels_slice (dense_esdf.py:498-509): the voxels of `submap` that were observed at the last update
+ * and whose uncentred index k + Nz/2 lies strictly within 0.5 of _index = (z + map_size_z/2)/voxel_scale (f32),
+ * appended to xyz f32[cap,3] / val f32[cap] (ESDF) at *count_dev (DEVICE int32 counter, incremented; rows beyond
+ * cap are counted but not written).  Positions as tslam_tsdf_extract_slice. */
+int tslam_esdf_extract_slice(tslam_tsdf_t* m, int32_t submap, float z, int64_t cap, float* xyz, float* val,
+                             int32_t* count_dev, void* stream);
 
 /* ----------------------------------------------------------------------------
  * Octomap = per-voxel hit counter  (Octomap, taichi_octomap.py)

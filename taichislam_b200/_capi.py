@@ -16,7 +16,7 @@ E_INVALID, E_CUDA, E_POOL_FULL, E_CAPACITY, E_NOGPU = -1, -2, -3, -4, -5
 MEM_DEVICE, MEM_HOST = 0, 1
 F_COMMIT = 1
 MAX_BATCH = 64
-ABI_VERSION = 3
+ABI_VERSION = 4
 
 
 class TslamError(RuntimeError):
@@ -111,6 +111,8 @@ SIGNATURES = {
     "tslam_esdf_update": (C.c_int, [_vp, _i32, C.POINTER(_i32), _vp]),
     "tslam_esdf_update2": (C.c_int, [_vp, _i32, _i32, _vp, _vp]),
     "tslam_esdf_gather": (C.c_int, [_vp, _i32, _i64, _vp, _vp, C.POINTER(_i64), _vp]),
+    "tslam_esdf_query": (C.c_int, [_vp, _i32, _i64, _vp, _vp, _vp, _vp, _vp]),
+    "tslam_esdf_extract_slice": (C.c_int, [_vp, _i32, _f32, _i64, _vp, _vp, _vp, _vp]),
     "tslam_octo_create": (C.c_int, [C.POINTER(OctoConfig), C.POINTER(_vp)]),
     "tslam_octo_destroy": (C.c_int, [_vp]),
     "tslam_octo_reset": (C.c_int, [_vp, _vp]),

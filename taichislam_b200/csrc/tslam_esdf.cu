@@ -55,6 +55,7 @@ struct EsAux {
   int* repoch;   // [max_blocks] raise wave: last raise sweep in which the block gained suspects
   int* rchanged; // [ES_MAX_SWEEPS+2]
   int* counts;   // [4] changed voxels, suspect voxels, re-initialised blocks, (spare)
+  int* nb_seen;  // [1] blocks in the pool when the last update ran (blocks are bump-allocated: higher indices are newer)
 };
 __device__ __forceinline__ unsigned char es_class(bool obs, float t, float gamma) {
   if (!obs) return ES_UNOBS;
@@ -66,6 +67,7 @@ __device__ __forceinline__ float es_sgn(float v) { return (float)((0.0f < v) - (
 
 __global__ void __launch_bounds__(256) k_esdf_init(TsGrid g, EsAux aux, int submap, float gamma, float far_v) {
   const int nb = min(*g.n_blocks, g.max_blocks);
+  if (blockIdx.x == 0 && threadIdx.x == 0) *aux.nb_seen = nb;
   for (int b = blockIdx.x; b < nb; b += gridDim.x) {
     int s, bx, by, bz;
     ts_unpack_key(g.block_key[b], s, bx, by, bz);
@@ -92,6 +94,7 @@ __global__ void __launch_bounds__(256) k_esdf_init(TsGrid g, EsAux aux, int subm
 // neighbour table of every block of the submap + epochs reset; the voxel state is left alone
 __global__ void __launch_bounds__(256) k_esdf_prepare(TsGrid g, EsAux aux, int submap) {
   const int nb = min(*g.n_blocks, g.max_blocks);
+  if (blockIdx.x == 0 && threadIdx.x == 0) *aux.nb_seen = nb;
   const int w = (blockIdx.x * 256 + threadIdx.x) >> 5, lane = threadIdx.x & 31, nw = (gridDim.x * 256) >> 5;
   for (int b = w; b < nb; b += nw) {
     int s, bx, by, bz;
@@ -396,6 +399,7 @@ static EsAux es_aux(tslam_tsdf* m) {
   aux.changed = aux.repoch + nb;
   aux.rchanged = aux.changed + (ES_MAX_SWEEPS + 2);
   aux.counts = aux.rchanged + (ES_MAX_SWEEPS + 2);
+  aux.nb_seen = aux.counts + 4;  // (inside the 8-int counts area; cleared with it at the start of every update)
   aux.cls = (unsigned char*)(aux.counts + 8);
   return aux;
 }
@@ -482,5 +486,155 @@ extern "C" int tslam_esdf_gather(tslam_tsdf_t* m, int32_t submap, int64_t cap, i
   TS_CUDA(cudaStreamSynchronize(st));
   *n_out = (int64_t)v;
   if ((int64_t)v > cap) { ts_set_error("esdf gather: capacity"); return TSLAM_E_CAPACITY; }
+  return TSLAM_OK;
+}
+
+// ---- reading the field: batched queries and the slice export ----------------------------------------------------
+// Both answer from the field as of the last update of the submap: the class byte that update left (not the live obs
+// plane) and only the blocks the update saw.  A block allocated later has a pool index >= *nb_seen (bump allocation;
+// a reset, which recycles the pool, forces the next update to be a full one and refuses queries until then).
+__device__ __forceinline__ int esq_block(const TsGrid& g, int submap, int nb_seen, int bx, int by, int bz) {
+  const int b = ts_find(g, ts_pack_key(submap, bx, by, bz));
+  return (b >= 0 && b < nb_seen && !g.ghost[b]) ? b : -1;
+}
+// lerp(a, b, t) = a + t*(b - a), rounded step by step (never contracted to an FMA): tests/esdf_query_reference.py
+__device__ __forceinline__ float esq_lerp(float a, float b, float t) { return __fadd_rn(a, __fmul_rn(t, __fsub_rn(b, a))); }
+
+// Trilinear interpolation of the ESDF over the 8 voxels around each point (voxel i centred at i*vs, submap-local frame)
+// and the exact partial derivatives of that interpolant.  One thread per point; each distinct corner block is looked
+// up once (the corner cube spans 2, 4 or 8 blocks only where i0 & 15 == 15 on some axis).  Invalid (NaN, valid = 0):
+// a non-finite coordinate, a corner outside the volume, a corner in an absent / ghost / newer block, a corner that was
+// unobserved or INERT at the last update.
+__global__ void __launch_bounds__(256) k_esdf_query(TsGrid g, EsAux aux, int submap, long long n, const float* __restrict__ xyz,
+                                                     float vs, float* __restrict__ dist, float* __restrict__ grad,
+                                                     uint8_t* __restrict__ valid) {
+  const int nb_seen = *aux.nb_seen;
+  const float lo = (float)(-g.hN), hi = (float)(g.N - g.hN - 1), loz = (float)(-g.hNz), hiz = (float)(g.Nz - g.hNz - 1);
+  const float qnan = __int_as_float(0x7fc00000);
+  for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < n; q += (long long)gridDim.x * blockDim.x) {
+    const float ux = __fdiv_rn(xyz[3 * q], vs), uy = __fdiv_rn(xyz[3 * q + 1], vs), uz = __fdiv_rn(xyz[3 * q + 2], vs);
+    // both corners i0, i0 + 1 inside the volume <=> lo <= u < hi.  NaN and +-inf fail the test, so no out-of-range
+    // value reaches the float -> int conversion below.
+    bool ok = ux >= lo && ux < hi && uy >= lo && uy < hi && uz >= loz && uz < hiz;
+    float d = qnan, gx = qnan, gy = qnan, gz = qnan;
+    if (ok) {
+      const int i0 = (int)floorf(ux), j0 = (int)floorf(uy), k0 = (int)floorf(uz);
+      const float fx = __fsub_rn(ux, (float)i0), fy = __fsub_rn(uy, (float)j0), fz = __fsub_rn(uz, (float)k0);
+      const bool sx = (i0 & TS_BMASK) == TS_BMASK, sy = (j0 & TS_BMASK) == TS_BMASK, sz = (k0 & TS_BMASK) == TS_BMASK;
+      const int x0 = i0 >> TS_BSHIFT, y0 = j0 >> TS_BSHIFT, z0 = k0 >> TS_BSHIFT;
+      // b[dx*4 + dy*2 + dz]: block of corner (i0+dx, j0+dy, k0+dz); a corner that shares its block with a lower one reuses it
+      int b[8];
+      b[0] = esq_block(g, submap, nb_seen, x0, y0, z0);
+      b[1] = sz ? esq_block(g, submap, nb_seen, x0, y0, z0 + 1) : b[0];
+      b[2] = sy ? esq_block(g, submap, nb_seen, x0, y0 + 1, z0) : b[0];
+      b[3] = sy ? (sz ? esq_block(g, submap, nb_seen, x0, y0 + 1, z0 + 1) : b[2]) : b[1];
+      b[4] = sx ? esq_block(g, submap, nb_seen, x0 + 1, y0, z0) : b[0];
+      b[5] = sx ? (sz ? esq_block(g, submap, nb_seen, x0 + 1, y0, z0 + 1) : b[4]) : b[1];
+      b[6] = sx ? (sy ? esq_block(g, submap, nb_seen, x0 + 1, y0 + 1, z0) : b[4]) : b[2];
+      b[7] = sx ? (sy ? (sz ? esq_block(g, submap, nb_seen, x0 + 1, y0 + 1, z0 + 1) : b[6]) : b[5]) : b[3];
+      float e[8];
+#pragma unroll
+      for (int c = 0; c < 8; c++) {
+        ok &= b[c] >= 0;
+        e[c] = 0.0f;
+      }
+      if (ok) {
+#pragma unroll
+        for (int c = 0; c < 8; c++) {
+          const size_t off = (size_t)b[c] * TS_B3 + ts_voxel_off(i0 + (c >> 2), j0 + ((c >> 1) & 1), k0 + (c & 1));
+          const unsigned char cl = aux.cls[off] & ES_CLS;
+          ok &= cl == ES_FIXED || cl == ES_POS || cl == ES_NEG;
+          e[c] = g.esdf[off];
+        }
+      }
+      if (ok) {
+        // dist: along x, then y, then z
+        const float c00 = esq_lerp(e[0], e[4], fx), c01 = esq_lerp(e[1], e[5], fx);
+        const float c10 = esq_lerp(e[2], e[6], fx), c11 = esq_lerp(e[3], e[7], fx);
+        d = esq_lerp(esq_lerp(c00, c10, fy), esq_lerp(c01, c11, fy), fz);
+        // d/dx: the four x-differences along y, then z
+        const float ax00 = __fsub_rn(e[4], e[0]), ax01 = __fsub_rn(e[5], e[1]), ax10 = __fsub_rn(e[6], e[2]), ax11 = __fsub_rn(e[7], e[3]);
+        gx = __fdiv_rn(esq_lerp(esq_lerp(ax00, ax10, fy), esq_lerp(ax01, ax11, fy), fz), vs);
+        // d/dy: the four y-differences along x, then z
+        const float ay00 = __fsub_rn(e[2], e[0]), ay01 = __fsub_rn(e[3], e[1]), ay10 = __fsub_rn(e[6], e[4]), ay11 = __fsub_rn(e[7], e[5]);
+        gy = __fdiv_rn(esq_lerp(esq_lerp(ay00, ay10, fx), esq_lerp(ay01, ay11, fx), fz), vs);
+        // d/dz: the four z-differences along x, then y
+        const float az00 = __fsub_rn(e[1], e[0]), az01 = __fsub_rn(e[3], e[2]), az10 = __fsub_rn(e[5], e[4]), az11 = __fsub_rn(e[7], e[6]);
+        gz = __fdiv_rn(esq_lerp(esq_lerp(az00, az10, fx), esq_lerp(az01, az11, fx), fy), vs);
+      } else {
+        d = gx = gy = gz = qnan;
+      }
+    }
+    dist[q] = d;
+    grad[3 * q] = gx; grad[3 * q + 1] = gy; grad[3 * q + 2] = gz;
+    valid[q] = ok ? 1 : 0;
+  }
+}
+
+// cvt_ESDF_to_voxels_slice (dense_esdf.py:498-509): the voxels known at the last update whose uncentred index k + Nz/2
+// lies strictly between _index - 0.5 and _index + 0.5 (bounds from the host), with ESDF value and position.  The
+// reference's struct-for also visits the unobserved cells of active blocks (ESDF 0): those are not exported here.
+__global__ void __launch_bounds__(256) k_esdf_extract_slice(TsGrid g, EsAux aux, int submap, int global_map, const float* pR,
+                                                             const float* pT, float vs, float k_lo, float k_hi, long long cap,
+                                                             float* xyz, float* val, int* counter) {
+  const int nb = min(*aux.nb_seen, g.max_blocks);
+  for (int b = blockIdx.x; b < nb; b += gridDim.x) {
+    int s, bx, by, bz;
+    ts_unpack_key(g.block_key[b], s, bx, by, bz);
+    if (s != submap || g.ghost[b]) continue;  // (uniform per CTA)
+    const size_t base = (size_t)b * TS_B3;
+    for (int v = threadIdx.x; v < TS_B3; v += blockDim.x) {
+      const int k = bz * TS_B + (v & 15);
+      const float ku = (float)(k + g.hNz);
+      const bool want = (aux.cls[base + v] & ES_CLS) != ES_UNOBS && k_lo < ku && ku < k_hi;
+      const int row = warp_append_i32(want, counter);
+      if (want && row < cap) {
+        float x, y, z;
+        voxel_xyz(g, global_map, pR, pT, s, bx * TS_B + (v >> 8), by * TS_B + ((v >> 4) & 15), k, vs, x, y, z);
+        xyz[3 * (size_t)row] = x; xyz[3 * (size_t)row + 1] = y; xyz[3 * (size_t)row + 2] = z;
+        val[row] = g.esdf[base + v];
+      }
+    }
+  }
+}
+
+// the field of `submap` can be read: an update has completed, for that submap, and nothing has invalidated its state
+static int es_readable(tslam_tsdf* m, int32_t submap, const char* what) {
+  if (!m->g.esdf) { ts_set_error("%s: no ESDF has been computed (tslam_esdf_update has not run)", what); return TSLAM_E_INVALID; }
+  if (m->esdf_full_needed) {
+    ts_set_error("%s: the map was reset, bulk-loaded or fused since the last completed tslam_esdf_update", what);
+    return TSLAM_E_INVALID;
+  }
+  if (m->esdf_submap != submap) {
+    ts_set_error("%s: the last tslam_esdf_update was for submap %d, not %d", what, m->esdf_submap, submap);
+    return TSLAM_E_INVALID;
+  }
+  return TSLAM_OK;
+}
+
+extern "C" int tslam_esdf_query(tslam_tsdf_t* m, int32_t submap, int64_t n, const float* xyz, float* dist, float* grad,
+                                uint8_t* valid, void* stream) {
+  if (!m || n < 0 || (n && (!xyz || !dist || !grad || !valid))) return TSLAM_E_INVALID;
+  int rc = es_readable(m, submap, "tslam_esdf_query");
+  if (rc || n == 0) return rc;
+  long long blocks = (n + 255) / 256;
+  if (blocks > (long long)m->sm_count * 16) blocks = (long long)m->sm_count * 16;
+  k_esdf_query<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(m->g, es_aux(m), submap, n, xyz, m->in.vs, dist, grad, valid);
+  TS_LAUNCH_CHECK(m);
+  return TSLAM_OK;
+}
+
+extern "C" int tslam_esdf_extract_slice(tslam_tsdf_t* m, int32_t submap, float z, int64_t cap, float* xyz, float* val,
+                                        int32_t* count_dev, void* stream) {
+  if (!m || cap < 0 || !xyz || !val || !count_dev) return TSLAM_E_INVALID;
+  int rc = es_readable(m, submap, "tslam_esdf_extract_slice");
+  if (rc) return rc;
+  // _index = (z + map_size_z/2) / voxel_scale in f32 (dense_esdf.py:504), map_size_z = voxel_scale * Nz
+  const float msz = (float)(m->cfg.voxel_scale * (double)m->cfg.Nz);
+  const float index = (z + msz / 2.0f) / m->in.vs;
+  k_esdf_extract_slice<<<m->sm_count * 4, 256, 0, (cudaStream_t)stream>>>(m->g, es_aux(m), submap, m->cfg.is_global_map, m->pose_R,
+                                                                          m->pose_T, m->in.vs, index - 0.5f, index + 0.5f, cap, xyz,
+                                                                          val, count_dev);
+  TS_LAUNCH_CHECK(m);
   return TSLAM_OK;
 }

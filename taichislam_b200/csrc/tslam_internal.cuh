@@ -184,6 +184,30 @@ __device__ __forceinline__ float div_vs(float x, float vs, float rvs) {
   return __fmaf_rn(e, rvs, q0);
 }
 
+// warp-aggregated append to an int32 row counter: the row of this lane, or -1 when it does not want one
+__device__ __forceinline__ int warp_append_i32(bool want, int* counter) {
+  const unsigned m = __ballot_sync(0xffffffffu, want);
+  if (!m) return -1;
+  const int lane = threadIdx.x & 31;
+  const int leader = __ffs(m) - 1;
+  int base = 0;
+  if (lane == leader) base = atomicAdd(counter, __popc(m));
+  base = __shfl_sync(0xffffffffu, base, leader);
+  return want ? base + __popc(m & ((1u << lane) - 1)) : -1;
+}
+
+// position of voxel (i, j, k) of submap s as the exporters write it (tslam_tsdf.cu, tslam_esdf.cu)
+__device__ __forceinline__ void voxel_xyz(const TsGrid& g, bool global_map, const float* pR, const float* pT, int s, int i, int j,
+                                          int k, float vs, float& x, float& y, float& z) {
+  const float lx = (float)i * vs, ly = (float)j * vs, lz = (float)k * vs;  // ijk_to_xyz mapping_common.py:221-223
+  if (global_map) { x = lx; y = ly; z = lz; return; }                      // i_j_k_to_xyz
+  const float* R = pR + 9 * s;                                             // submap_i_j_k_to_xyz :229-232
+  const float* T = pT + 3 * s;
+  x = ((R[0] * lx + R[1] * ly) + R[2] * lz) + T[0];
+  y = ((R[3] * lx + R[4] * ly) + R[5] * lz) + T[1];
+  z = ((R[6] * lx + R[7] * ly) + R[8] * lz) + T[2];
+}
+
 __device__ __forceinline__ void red_add_f32x2(float2* addr, float a, float b) {
   // one 8-byte vector reduction without return value: REDG.E.ADD.F32x2 (sm_90+).  Spelled in PTX because
   // atomicAdd(float2*) was lowered to ATOMG (response sector per update) inside the divergent march loop.

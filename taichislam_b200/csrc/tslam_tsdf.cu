@@ -1502,17 +1502,6 @@ __device__ __forceinline__ long long warp_append(bool want, unsigned long long* 
   base = __shfl_sync(0xffffffffu, base, leader);
   return want ? (long long)(base + __popc(m & ((1u << lane) - 1))) : -1;
 }
-__device__ __forceinline__ int warp_append_i32(bool want, int* counter) {
-  const unsigned m = __ballot_sync(0xffffffffu, want);
-  if (!m) return -1;
-  const int lane = threadIdx.x & 31;
-  const int leader = __ffs(m) - 1;
-  int base = 0;
-  if (lane == leader) base = atomicAdd(counter, __popc(m));
-  base = __shfl_sync(0xffffffffu, base, leader);
-  return want ? base + __popc(m & ((1u << lane) - 1)) : -1;
-}
-
 __global__ void __launch_bounds__(256) k_gather(TsGrid g, int submap, long long cap, int32_t* idx, float* tsdf, float* wts,
                                                  int8_t* occ, float* color, unsigned long long* counter) {
   const int nb = min(*g.n_blocks, g.max_blocks);
@@ -1617,17 +1606,6 @@ extern "C" int tslam_tsdf_scatter2(tslam_tsdf_t* m, int32_t submap, int64_t n, c
 // ---------------------------------------------------------------------------
 // exporters  (dense_tsdf.py:339-385)
 // ---------------------------------------------------------------------------
-__device__ __forceinline__ void voxel_xyz(const TsGrid& g, bool global_map, const float* pR, const float* pT, int s, int i, int j,
-                                          int k, float vs, float& x, float& y, float& z) {
-  const float lx = (float)i * vs, ly = (float)j * vs, lz = (float)k * vs;  // ijk_to_xyz mapping_common.py:221-223
-  if (global_map) { x = lx; y = ly; z = lz; return; }                      // i_j_k_to_xyz
-  const float* R = pR + 9 * s;                                             // submap_i_j_k_to_xyz :229-232
-  const float* T = pT + 3 * s;
-  x = ((R[0] * lx + R[1] * ly) + R[2] * lz) + T[0];
-  y = ((R[3] * lx + R[4] * ly) + R[5] * lz) + T[1];
-  z = ((R[6] * lx + R[7] * ly) + R[8] * lz) + T[2];
-}
-
 __global__ void __launch_bounds__(256) k_extract_surface(TsGrid g, int submap, int global_map, const float* pR, const float* pT,
                                                           float vs, float thres, float fl, float ce, const float* cmap,
                                                           long long cap, float* xyz, float* rgb, int* counter) {

@@ -90,6 +90,8 @@ class DenseTSDF(BaseMap):
         self.export_color = Field(torch.full((n, 3), 0.5, dtype=torch.float32, device=dev), fl)
         self.export_TSDF = Field(torch.zeros(n, dtype=torch.float32, device=dev), fl)
         self.export_TSDF_xyz = Field(torch.full((n, 3), -100000.0, dtype=torch.float32, device=dev), fl)
+        self.export_ESDF = Field(torch.zeros(n, dtype=torch.float32, device=dev), fl)  # dense_esdf.py ESDF slice export
+        self.export_ESDF_xyz = Field(torch.full((n, 3), -100000.0, dtype=torch.float32, device=dev), fl)
 
     def _on_intrinsics(self):
         self._flush()
@@ -340,3 +342,28 @@ class DenseTSDF(BaseMap):
 
     def get_voxels_ESDF(self):
         return self._h.esdf_gather(self._active())
+
+    def esdf_query(self, xyz, update=True):
+        """Interpolated ESDF and its gradient at points [n,3] of the active submap's map frame (what Voxblox, which
+        dense_esdf.py:1 implements, answers for planners): (dist, grad, valid), torch CUDA tensors for a torch tensor,
+        numpy arrays for a numpy array.  update=True first brings the field up to date (incremental esdf_update);
+        update=False answers from the field as of the last update."""
+        self._flush()
+        if update:
+            self._h.esdf_update(self._active())
+        return self._h.esdf_query(xyz, submap=self._active())
+
+    def cvt_ESDF_to_voxels_slice(self, z):
+        """dense_esdf.py:498-509, after bringing the field up to date: the ESDF voxels of the slice at height z into
+        export_ESDF / export_ESDF_xyz, their number into num_export_ESDF_particles.  Only voxels observed at the update
+        are exported (the reference's struct-for also visits unobserved cells of active blocks, ESDF 0)."""
+        self._flush()
+        s = self._active()
+        self._h.esdf_update(s)
+        self.num_export_ESDF_particles.t.zero_()
+        self._h.esdf_extract_slice(s, z, self.export_ESDF_xyz.t, self.export_ESDF.t, self.num_export_ESDF_particles.t)
+
+    def get_voxels_ESDF_slice(self, z):
+        """dense_esdf.py:569-571."""
+        self.cvt_ESDF_to_voxels_slice(z)
+        return self.export_ESDF_xyz.to_numpy(), self.export_ESDF.to_numpy()

@@ -292,6 +292,42 @@ class TsdfHandle:
         k = int(n.value)
         return idx[:k].cpu().numpy(), e[:k].cpu().numpy()
 
+    def esdf_query(self, xyz, submap=0):
+        """Trilinear ESDF and its exact gradient at points [n,3] of the submap's map frame, as of the last esdf_update of
+        `submap`: (dist f32[n], grad f32[n,3], valid bool[n]); dist and grad are NaN where valid is False.
+        A torch CUDA tensor in -> torch CUDA tensors out, enqueued on the current stream without a host synchronisation
+        (a planner's torch loop can call it); a numpy array in -> numpy arrays out."""
+        torch = self.torch
+        as_torch = isinstance(xyz, torch.Tensor)
+        x = self._dev_f32(xyz).reshape(-1, 3)
+        n = x.shape[0]
+        dist = torch.empty(n, dtype=torch.float32, device=x.device)
+        grad = torch.empty((n, 3), dtype=torch.float32, device=x.device)
+        valid = torch.empty(n, dtype=torch.uint8, device=x.device)
+        capi.check(self.L.tslam_esdf_query(self.h, int(submap), n, capi.tptr(x), capi.tptr(dist), capi.tptr(grad), capi.tptr(valid),
+                                           capi.stream_ptr()))
+        valid = valid.view(torch.bool)  # the kernel writes 0 / 1
+        if as_torch:
+            return dist, grad, valid
+        return dist.cpu().numpy(), grad.cpu().numpy(), valid.cpu().numpy()
+
+    def esdf_extract_slice(self, submap, z, xyz, val, count):
+        """Append the ESDF slice at height z to torch CUDA buffers xyz f32[cap,3] / val f32[cap]; count: int32[1] device counter."""
+        capi.check(self.L.tslam_esdf_extract_slice(self.h, int(submap), float(z), xyz.shape[0], capi.tptr(xyz), capi.tptr(val),
+                                                   capi.tptr(count), capi.stream_ptr()))
+
+    def esdf_slice(self, z, submap=0, cap=1 << 22):
+        """cvt_ESDF_to_voxels_slice (dense_esdf.py:498-509) as of the last esdf_update: (demand, xyz, ESDF) numpy."""
+        torch = self.torch
+        dev = torch.device("cuda", torch.cuda.current_device())
+        xyz = torch.empty((max(cap, 1), 3), dtype=torch.float32, device=dev)
+        val = torch.empty(max(cap, 1), dtype=torch.float32, device=dev)
+        cnt = torch.zeros(1, dtype=torch.int32, device=dev)
+        self.esdf_extract_slice(submap, z, xyz[:cap], val[:cap], cnt)
+        n = int(cnt.item())
+        k = min(n, cap)
+        return n, xyz[:k].cpu().numpy(), val[:k].cpu().numpy()
+
     # -- introspection --------------------------------------------------------------------
     def stats(self, clear=False):
         o = np.zeros(8, np.int64)

@@ -45,7 +45,7 @@ const char* tslam_last_error(void);
 int tslam_device_count(void);
 /* ABI version of this header (tests check the library agrees). */
 int tslam_abi_version(void);
-#define TSLAM_ABI_VERSION 4
+#define TSLAM_ABI_VERSION 5
 
 /* ----------------------------------------------------------------------------
  * TSDF map  (DenseTSDF, dense_tsdf.py)
@@ -255,6 +255,36 @@ int tslam_tsdf_halo_pack2(tslam_tsdf_t* m, const int32_t* tiles3, int32_t rank, 
                           int64_t* keys, float* tw, uint8_t* obs, float* col, void* stream);
 int tslam_tsdf_ghost_unpack2(tslam_tsdf_t* m, int64_t n, const int64_t* keys, const float* tw, const uint8_t* obs, const float* col,
                              void* stream);
+/* Query routing: owner[n] (DEVICE int32) = owner rank of the block that holds the low interpolation corner of each
+ * point xyz f32[n,3] (DEVICE) - the corner tslam_esdf_query starts from, computed by the same f32 expression - or -1
+ * for a point that is not finite or whose low corner lies outside the volume (any rank answers those: invalid). */
+int tslam_tiling_owner_points(tslam_tsdf_t* m, const int32_t* tiles3, int32_t world, int64_t n, const float* xyz, int32_t* owner,
+                              void* stream);
+/* ESDF of the tiled map (DESIGN.md section 6).  Always a full recompute of `submap`, exact: the result is bit-identical
+ * to tslam_esdf_update2 on one map holding every tile.  Run a TSDF halo exchange first (ghosts must carry the current
+ * TSDF), then on every rank:
+ *   tslam_esdf_tiled_begin                  seed owned and ghost blocks, local wave to convergence; ghost blocks are
+ *                                           read-only sources.  Synchronises.
+ *   repeat: tslam_esdf_halo_count / _pack   owned boundary blocks (the TSDF halo's blocks and destinations) whose ESDF
+ *                                           changed since they were last packed - after begin, all of them - into
+ *                                           keys int64[cap] / esdf f32[cap,4096] (DEVICE) grouped by destination;
+ *                                           packing clears the mark.  Synchronises.  TSLAM_E_CAPACITY: saturated,
+ *                                           the blocks that did not fit stay marked.
+ *           exchange (all-to-all), then tslam_esdf_ghost_unpack: overwrite the ESDF of existing ghost blocks (never
+ *                                           allocates).  A key that is not a ghost block of the submap writes nothing
+ *                                           and makes the call return TSLAM_E_INVALID.  Synchronises.
+ *           tslam_esdf_tiled_relax          the wave from the ghosts unpacked since the last relax.  Synchronises.
+ *   until every rank packed 0 blocks;  tslam_esdf_tiled_end.
+ * n_sweeps_out (HOST, may be NULL) as tslam_esdf_update.  Between begin and end tslam_esdf_query / _extract_slice
+ * return TSLAM_E_INVALID; after end tslam_esdf_query also reads corners in ghost blocks (after a plain update they stay
+ * invalid), until the next reset, load, fusion, ghost import or update.  An update after a tiled ESDF is full. */
+int tslam_esdf_tiled_begin(tslam_tsdf_t* m, int32_t submap, int32_t* n_sweeps_out, void* stream);
+int tslam_esdf_halo_count(tslam_tsdf_t* m, const int32_t* tiles3, int32_t rank, int32_t world, int32_t* counts_out, void* stream);
+int tslam_esdf_halo_pack(tslam_tsdf_t* m, const int32_t* tiles3, int32_t rank, int32_t world, const int32_t* counts, int64_t cap,
+                         int64_t* keys, float* esdf, void* stream);
+int tslam_esdf_ghost_unpack(tslam_tsdf_t* m, int64_t n, const int64_t* keys, const float* esdf, void* stream);
+int tslam_esdf_tiled_relax(tslam_tsdf_t* m, int32_t* n_sweeps_out, void* stream);
+int tslam_esdf_tiled_end(tslam_tsdf_t* m);
 
 /* ----------------------------------------------------------------------------
  * Marching cubes  (MarchingCubeMesher, marching_cube_mesher.py)

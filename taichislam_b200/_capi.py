@@ -16,7 +16,7 @@ E_INVALID, E_CUDA, E_POOL_FULL, E_CAPACITY, E_NOGPU = -1, -2, -3, -4, -5
 MEM_DEVICE, MEM_HOST = 0, 1
 F_COMMIT = 1
 MAX_BATCH = 64
-ABI_VERSION = 4
+ABI_VERSION = 5
 
 
 class TslamError(RuntimeError):
@@ -107,6 +107,13 @@ SIGNATURES = {
     "tslam_tsdf_unpack_add2": (C.c_int, [_vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp]),
     "tslam_tsdf_halo_pack2": (C.c_int, [_vp, _vp, _i32, _i32, _vp, _i64, _vp, _vp, _vp, _vp, _vp]),
     "tslam_tsdf_ghost_unpack2": (C.c_int, [_vp, _i64, _vp, _vp, _vp, _vp, _vp]),
+    "tslam_tiling_owner_points": (C.c_int, [_vp, _vp, _i32, _i64, _vp, _vp, _vp]),
+    "tslam_esdf_tiled_begin": (C.c_int, [_vp, _i32, C.POINTER(_i32), _vp]),
+    "tslam_esdf_halo_count": (C.c_int, [_vp, _vp, _i32, _i32, _vp, _vp]),
+    "tslam_esdf_halo_pack": (C.c_int, [_vp, _vp, _i32, _i32, _vp, _i64, _vp, _vp, _vp]),
+    "tslam_esdf_ghost_unpack": (C.c_int, [_vp, _i64, _vp, _vp, _vp]),
+    "tslam_esdf_tiled_relax": (C.c_int, [_vp, C.POINTER(_i32), _vp]),
+    "tslam_esdf_tiled_end": (C.c_int, [_vp]),
     "tslam_mc_generate": (C.c_int, [_vp, _i32, _f32, _i64, _vp, _vp, C.POINTER(_i64), _vp]),
     "tslam_esdf_update": (C.c_int, [_vp, _i32, C.POINTER(_i32), _vp]),
     "tslam_esdf_update2": (C.c_int, [_vp, _i32, _i32, _vp, _vp]),

@@ -244,6 +244,71 @@ __global__ void __launch_bounds__(256) k_ghost_unpack(TsGrid g, long long n, con
   }
 }
 
+// ---- ESDF halo (tiled ESDF, tslam_esdf.cu) ------------------------------------------------------------------------
+// The same boundary blocks as the TSDF halo (halo_dests), those marked as changed since they were last packed.
+__global__ void __launch_bounds__(256) k_esdf_halo_count(TsGrid g, TsTiling t, const int* xmark, int* counts) {
+  const int nb = min(*g.n_blocks, g.max_blocks);
+  for (int b = blockIdx.x * blockDim.x + threadIdx.x; b < nb; b += gridDim.x * blockDim.x) {
+    if (g.ghost[b] || !xmark[b]) continue;
+    int s, bx, by, bz, d[26];
+    ts_unpack_key(g.block_key[b], s, bx, by, bz);
+    if (tile_owner(t, bx, by, bz) != t.rank) continue;
+    const int n = halo_dests(t, bx, by, bz, d);
+    for (int q = 0; q < n; q++) atomicAdd(&counts[d[q]], 1);
+  }
+}
+
+struct EsHaloGroups { int off[24], cnt[24]; };  // slot group of every destination rank (from the caller's counts)
+
+// One CTA per block.  A block whose every copy found a slot inside its group and below cap loses its mark; the others
+// keep it (the host reports TSLAM_E_CAPACITY).
+__global__ void __launch_bounds__(256) k_esdf_halo_pack(TsGrid g, TsTiling t, int* xmark, EsHaloGroups grp, int* cursor, long long cap,
+                                                         long long* keys, float4* esdf_out) {
+  __shared__ long long s_slot[26];
+  __shared__ int s_n;
+  const int nb = min(*g.n_blocks, g.max_blocks);
+  for (int b = blockIdx.x; b < nb; b += gridDim.x) {
+    if (g.ghost[b] || !xmark[b]) continue;  // (uniform per CTA)
+    int s, bx, by, bz;
+    ts_unpack_key(g.block_key[b], s, bx, by, bz);
+    if (tile_owner(t, bx, by, bz) != t.rank) continue;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      int d[26];
+      bool all = true;
+      s_n = halo_dests(t, bx, by, bz, d);
+      for (int q = 0; q < s_n; q++) {
+        const int k = atomicAdd(&cursor[d[q]], 1);
+        long long slot = (long long)grp.off[d[q]] + k;
+        if (k >= grp.cnt[d[q]] || slot >= cap) slot = -1;
+        if (slot >= 0) keys[slot] = (long long)g.block_key[b];
+        all &= slot >= 0;
+        s_slot[q] = slot;
+      }
+      if (all) xmark[b] = 0;
+    }
+    __syncthreads();
+    const int n = s_n;
+    const float4* src = reinterpret_cast<const float4*>(g.esdf + (size_t)b * TS_B3);
+    for (int q = 0; q < n; q++) {
+      const long long slot = s_slot[q];
+      if (slot < 0) continue;
+      for (int v = threadIdx.x; v < TS_B3 / 4; v += blockDim.x) esdf_out[slot * (TS_B3 / 4) + v] = src[v];
+    }
+  }
+}
+
+// owner rank of the block holding each point's low interpolation corner (the corner k_esdf_query starts from), -1 for
+// a point that is not finite or whose low corner lies outside the volume
+__global__ void __launch_bounds__(256) k_owner_points(TsGrid g, TsTiling t, float vs, long long n, const float* __restrict__ xyz,
+                                                       int* __restrict__ owner) {
+  for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < n; q += (long long)gridDim.x * blockDim.x) {
+    float u[3];
+    int c[3];
+    owner[q] = esq_low_corner(g, vs, xyz + 3 * q, u, c) ? tile_owner(t, c[0] >> TS_BSHIFT, c[1] >> TS_BSHIFT, c[2] >> TS_BSHIFT) : -1;
+  }
+}
+
 // ---- C ABI -------------------------------------------------------------------------------------------------------
 // defined in tslam_tsdf.cu
 extern "C" int tslam_tsdf_fuse_pending(tslam_tsdf_t* dst, tslam_tsdf_t* src, void* stream);
@@ -260,6 +325,19 @@ extern "C" int tslam_tiling_owner(tslam_tsdf_t* m, const int32_t* tiles3, int32_
   int rc = fill_tiling(m, tiles3, 0, world, &t);
   if (rc) return rc;
   *owner = tile_owner(t, bx, by, bz);
+  return TSLAM_OK;
+}
+
+extern "C" int tslam_tiling_owner_points(tslam_tsdf_t* m, const int32_t* tiles3, int32_t world, int64_t n, const float* xyz, int32_t* owner,
+                                         void* stream) {
+  if (!m || n < 0 || (n && (!xyz || !owner))) return TSLAM_E_INVALID;
+  TsTiling t;
+  int rc = fill_tiling(m, tiles3, 0, world, &t);
+  if (rc || n == 0) return rc;
+  long long blocks = (n + 255) / 256;
+  if (blocks > (long long)m->sm_count * 16) blocks = (long long)m->sm_count * 16;
+  k_owner_points<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(m->g, t, m->in.vs, n, xyz, owner);
+  TS_LAUNCH_CHECK(m);
   return TSLAM_OK;
 }
 
@@ -406,5 +484,59 @@ extern "C" int tslam_tsdf_ghost_unpack2(tslam_tsdf_t* m, int64_t n, const int64_
   m->esdf_full_needed = 1;
   k_ghost_unpack<<<(int)(n < m->sm_count * 4 ? n : m->sm_count * 4), 256, 0, st>>>(m->g, n, (const long long*)keys, (const float2*)tw, obs, (const float4*)col);
   TS_LAUNCH_CHECK(m);
+  return TSLAM_OK;
+}
+
+// ---- ESDF halo of a tiled ESDF (tslam_esdf_tiled_begin .. _end) ----------------------------------------------------
+static int esdf_halo_open(tslam_tsdf* m, const char* what) {
+  if (!ts_esdf_xmark(m) || m->esdf_tiled != 1 || m->esdf_full_needed) {
+    ts_set_error("%s: no tiled ESDF is in progress (tslam_esdf_tiled_begin, then no reset, load, fusion or ghost import)", what);
+    return TSLAM_E_INVALID;
+  }
+  return TSLAM_OK;
+}
+
+extern "C" int tslam_esdf_halo_count(tslam_tsdf_t* m, const int32_t* tiles3, int32_t rank, int32_t world, int32_t* counts_out, void* stream) {
+  if (!m || !counts_out || world > 24) return TSLAM_E_INVALID;
+  TsTiling t;
+  int rc = fill_tiling(m, tiles3, rank, world, &t);
+  if (rc) return rc;
+  rc = esdf_halo_open(m, "tslam_esdf_halo_count");
+  if (rc) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  int* d = m->scratch_i + 16;
+  TS_CUDA(cudaMemsetAsync(d, 0, 48 * sizeof(int), st));
+  k_esdf_halo_count<<<m->sm_count * 2, 256, 0, st>>>(m->g, t, ts_esdf_xmark(m), d);
+  TS_LAUNCH_CHECK(m);
+  TS_CUDA(cudaMemcpyAsync(counts_out, d, world * sizeof(int), cudaMemcpyDeviceToHost, st));
+  TS_CUDA(cudaStreamSynchronize(st));
+  return TSLAM_OK;
+}
+
+extern "C" int tslam_esdf_halo_pack(tslam_tsdf_t* m, const int32_t* tiles3, int32_t rank, int32_t world, const int32_t* counts, int64_t cap,
+                                    int64_t* keys, float* esdf, void* stream) {
+  if (!m || !counts || world > 24 || cap < 0 || (cap && (!keys || !esdf))) return TSLAM_E_INVALID;
+  TsTiling t;
+  int rc = fill_tiling(m, tiles3, rank, world, &t);
+  if (rc) return rc;
+  rc = esdf_halo_open(m, "tslam_esdf_halo_pack");
+  if (rc) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  EsHaloGroups grp;
+  const int tot = scan_counts(counts, world, grp.off);
+  for (int r = 0; r < world; r++) grp.cnt[r] = counts[r] < 0 ? 0 : counts[r];
+  int* d_cur = m->scratch_i + 40;
+  TS_CUDA(cudaMemsetAsync(d_cur, 0, 24 * sizeof(int), st));
+  k_esdf_halo_pack<<<m->sm_count * 4, 256, 0, st>>>(m->g, t, ts_esdf_xmark(m), grp, d_cur, cap, (long long*)keys, (float4*)esdf);
+  TS_LAUNCH_CHECK(m);
+  int h_cur[24];
+  TS_CUDA(cudaMemcpyAsync(h_cur, d_cur, world * sizeof(int), cudaMemcpyDeviceToHost, st));
+  TS_CUDA(cudaStreamSynchronize(st));
+  bool over = tot > cap;
+  for (int r = 0; r < world; r++) over |= h_cur[r] > grp.cnt[r];
+  if (over) {
+    ts_set_error("esdf halo pack: capacity (buffers saturated; the blocks that did not fit stay marked)");
+    return TSLAM_E_CAPACITY;
+  }
   return TSLAM_OK;
 }

@@ -56,6 +56,7 @@ struct EsAux {
   int* rchanged; // [ES_MAX_SWEEPS+2]
   int* counts;   // [4] changed voxels, suspect voxels, re-initialised blocks, (spare)
   int* nb_seen;  // [1] blocks in the pool when the last update ran (blocks are bump-allocated: higher indices are newer)
+  int* xmark;    // [max_blocks] tiled ESDF: owned block changed since last packed / ghost block unpacked since last relax
 };
 __device__ __forceinline__ unsigned char es_class(bool obs, float t, float gamma) {
   if (!obs) return ES_UNOBS;
@@ -65,6 +66,9 @@ __device__ __forceinline__ unsigned char es_class(bool obs, float t, float gamma
 __device__ __forceinline__ int es_tidx(int lx, int ly, int lz) { return ((lx + 1) * ES_T + (ly + 1)) * ES_T + (lz + 1); }
 __device__ __forceinline__ float es_sgn(float v) { return (float)((0.0f < v) - (v < 0.0f)); }
 
+// TILED (tslam_esdf_tiled_begin): ghost blocks are seeded like owned ones, and every owned block of the submap is
+// marked for the first ESDF halo pack.
+template <bool TILED>
 __global__ void __launch_bounds__(256) k_esdf_init(TsGrid g, EsAux aux, int submap, float gamma, float far_v) {
   const int nb = min(*g.n_blocks, g.max_blocks);
   if (blockIdx.x == 0 && threadIdx.x == 0) *aux.nb_seen = nb;
@@ -72,6 +76,7 @@ __global__ void __launch_bounds__(256) k_esdf_init(TsGrid g, EsAux aux, int subm
     int s, bx, by, bz;
     ts_unpack_key(g.block_key[b], s, bx, by, bz);
     if (threadIdx.x == 0) aux.epoch[b] = (s == submap) ? 0 : -1000000;
+    if (TILED && threadIdx.x == 0) aux.xmark[b] = (s == submap && !g.ghost[b]) ? 1 : 0;
     if (s != submap) continue;
     if (threadIdx.x < 27) {
       const int dx = threadIdx.x / 9 - 1, dy = (threadIdx.x / 3) % 3 - 1, dz = threadIdx.x % 3 - 1;
@@ -267,6 +272,9 @@ struct EsTile {
 };
 
 
+// TILED: ghost blocks are read-only sources - never relaxed, but their epochs wake their owned neighbours - and an
+// owned block that changes is marked for the next ESDF halo pack.  Otherwise every block of the submap is relaxed.
+template <bool TILED>
 __global__ void __launch_bounds__(256) k_esdf_sweep(TsGrid g, EsAux aux, int submap, int sweep, float gamma, float vs) {
   __shared__ EsTile tile;
   if (sweep > 1 && aux.changed[sweep - 1] == 0) return;  // already converged: nothing to do
@@ -277,6 +285,7 @@ __global__ void __launch_bounds__(256) k_esdf_sweep(TsGrid g, EsAux aux, int sub
     if (threadIdx.x == 0) { tile.active = 0; tile.any_write = 0; }
     __syncthreads();
     if (aux.epoch[b] < -1) continue;  // block of another submap (uniform per CTA)
+    if (TILED && g.ghost[b]) continue;  // the owner's values: a source only
     if (threadIdx.x < 27) {
       const int n = aux.nbr[b * 27 + threadIdx.x];
       tile.nbr[threadIdx.x] = n;
@@ -348,8 +357,46 @@ __global__ void __launch_bounds__(256) k_esdf_sweep(TsGrid g, EsAux aux, int sub
         __threadfence();
         aux.epoch[b] = sweep;
         aux.changed[sweep] = 1;
+        if (TILED) aux.xmark[b] = 1;
       }
     }
+  }
+}
+
+// ---- tiled ESDF (tslam_esdf_tiled_*) ----------------------------------------------------------------------------
+// Start of a relax: only the ghosts unpacked since the last relax are wave sources (epoch 0); every other block of the
+// submap waits for the wave (epoch -1).  The marks of owned blocks (changed since last packed) are kept.
+__global__ void __launch_bounds__(256) k_esdf_rearm(TsGrid g, EsAux aux) {
+  const int nb = min(*aux.nb_seen, g.max_blocks);
+  for (int b = blockIdx.x * blockDim.x + threadIdx.x; b < nb; b += gridDim.x * blockDim.x) {
+    if (aux.epoch[b] < -1) continue;  // block of another submap
+    const bool src = g.ghost[b] && aux.xmark[b];
+    aux.epoch[b] = src ? 0 : -1;
+    if (g.ghost[b]) aux.xmark[b] = 0;
+  }
+}
+
+// One CTA per received block: overwrite the ESDF plane of an existing ghost block of the submap and mark it as a
+// source of the next relax.  A key that is absent, owned, of another submap or newer than the update is counted in
+// *bad and nothing is written for it.
+__global__ void __launch_bounds__(256) k_esdf_ghost_unpack(TsGrid g, EsAux aux, long long n, const long long* keys, const float4* esdf_in,
+                                                            int* bad) {
+  __shared__ int s_blk;
+  const int nb_seen = *aux.nb_seen;
+  for (long long q = blockIdx.x; q < n; q += gridDim.x) {
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      int b = ts_find(g, (unsigned long long)keys[q]);
+      if (b >= nb_seen || (b >= 0 && (!g.ghost[b] || aux.epoch[b] < -1))) b = -1;
+      if (b < 0) atomicAdd(bad, 1);
+      s_blk = b;
+    }
+    __syncthreads();
+    const int blk = s_blk;
+    if (blk < 0) continue;
+    float4* dst = reinterpret_cast<float4*>(g.esdf + (size_t)blk * TS_B3);
+    for (int v = threadIdx.x; v < TS_B3 / 4; v += blockDim.x) dst[v] = esdf_in[q * (TS_B3 / 4) + v];
+    if (threadIdx.x == 0) aux.xmark[blk] = 1;
   }
 }
 
@@ -385,8 +432,8 @@ static int es_alloc(tslam_tsdf* m) {
   const size_t nb = (size_t)m->g.max_blocks;
   TS_CUDA(cudaMalloc(&m->g.esdf, nb * TS_B3 * 4));
   TS_CUDA(cudaMemset(m->g.esdf, 0, nb * TS_B3 * 4));
-  TS_CUDA(cudaMalloc(&m->esdf_aux, (nb * 29 + 2 * (ES_MAX_SWEEPS + 2) + 8) * 4 + nb * TS_B3));
-  TS_CUDA(cudaMemset(m->esdf_aux, 0, (nb * 29 + 2 * (ES_MAX_SWEEPS + 2) + 8) * 4 + nb * TS_B3));
+  TS_CUDA(cudaMalloc(&m->esdf_aux, (nb * 30 + 2 * (ES_MAX_SWEEPS + 2) + 8) * 4 + nb * TS_B3));
+  TS_CUDA(cudaMemset(m->esdf_aux, 0, (nb * 30 + 2 * (ES_MAX_SWEEPS + 2) + 8) * 4 + nb * TS_B3));
   m->esdf_full_needed = 1;
   return TSLAM_OK;
 }
@@ -401,8 +448,10 @@ static EsAux es_aux(tslam_tsdf* m) {
   aux.counts = aux.rchanged + (ES_MAX_SWEEPS + 2);
   aux.nb_seen = aux.counts + 4;  // (inside the 8-int counts area; cleared with it at the start of every update)
   aux.cls = (unsigned char*)(aux.counts + 8);
+  aux.xmark = (int*)(aux.cls + nb * TS_B3);
   return aux;
 }
+int* ts_esdf_xmark(tslam_tsdf* m) { return m->esdf_aux ? es_aux(m).xmark : nullptr; }
 
 // One wave (raise or lower) to convergence: sweeps are enqueued in groups, a sweep whose predecessor changed nothing
 // returns at once; the host reads ONE flag per group.  Returns the number of sweeps that did something + 1.
@@ -438,13 +487,15 @@ extern "C" int tslam_esdf_update2(tslam_tsdf_t* m, int32_t submap, int32_t mode,
   EsAux aux = es_aux(m);
   const float gamma = (float)m->cfg.voxel_scale;     // dense_esdf.py:40
   const float far_v = (float)m->cfg.max_ray_length;  // dense_esdf.py:324
-  const bool full = mode == 1 || m->esdf_full_needed || m->esdf_submap != submap;
+  // (the state a tiled ESDF leaves - ghosts holding their owners' values - is no base for an incremental update)
+  const bool full = mode == 1 || m->esdf_full_needed || m->esdf_submap != submap || m->esdf_tiled != 0;
   int h_counts[4] = {0, 0, 0, 0}, n_lower = 0, n_raise = 0;
+  m->esdf_tiled = 0;
   TS_CUDA(cudaMemsetAsync(aux.changed, 0, (2 * (ES_MAX_SWEEPS + 2) + 8) * 4, st));  // changed, rchanged, counts
   if (full) {
-    k_esdf_init<<<m->sm_count * 4, 256, 0, st>>>(m->g, aux, submap, gamma, far_v);
+    k_esdf_init<false><<<m->sm_count * 4, 256, 0, st>>>(m->g, aux, submap, gamma, far_v);
     TS_LAUNCH_CHECK(m);
-    rc = es_wave(m, st, aux.changed, ES_GROUP, [&](int k) { k_esdf_sweep<<<m->sm_count * 4, 256, 0, st>>>(m->g, aux, submap, k, gamma, m->in.vs); }, &n_lower);
+    rc = es_wave(m, st, aux.changed, ES_GROUP, [&](int k) { k_esdf_sweep<false><<<m->sm_count * 4, 256, 0, st>>>(m->g, aux, submap, k, gamma, m->in.vs); }, &n_lower);
     if (rc) return rc;
   } else {
     k_esdf_prepare<<<m->sm_count * 2, 256, 0, st>>>(m->g, aux, submap);
@@ -455,7 +506,7 @@ extern "C" int tslam_esdf_update2(tslam_tsdf_t* m, int32_t submap, int32_t mode,
     if (rc) return rc;
     k_esdf_reinit<<<m->sm_count * 4, 256, 0, st>>>(m->g, aux, gamma, far_v);
     TS_LAUNCH_CHECK(m);
-    rc = es_wave(m, st, aux.changed, 4, [&](int k) { k_esdf_sweep<<<m->sm_count * 4, 256, 0, st>>>(m->g, aux, submap, k, gamma, m->in.vs); }, &n_lower);
+    rc = es_wave(m, st, aux.changed, 4, [&](int k) { k_esdf_sweep<false><<<m->sm_count * 4, 256, 0, st>>>(m->g, aux, submap, k, gamma, m->in.vs); }, &n_lower);
     if (rc) return rc;
     TS_CUDA(cudaMemcpy(h_counts, aux.counts, 16, cudaMemcpyDeviceToHost));
   }
@@ -470,6 +521,87 @@ extern "C" int tslam_esdf_update(tslam_tsdf_t* m, int32_t submap, int32_t* n_swe
   int rc = tslam_esdf_update2(m, submap, 0, st4, stream);
   if (n_sweeps_out) *n_sweeps_out = st4[0];
   return rc;
+}
+
+// ---- tiled ESDF: begin -> (ESDF halo pack -> exchange -> ghost unpack -> relax)* -> end --------------------------
+// The exchange loop between begin and end is driven by the host layer (taichislam_b200/distributed.py); the ESDF halo
+// pack lives with the other halo code in tslam_dist.cu.  Every value is an attainable upper bound at every step, so
+// the loop ends at the single map's least fixed point (DESIGN.md section 6).
+static int es_tiled_open(tslam_tsdf* m, const char* what) {
+  if (!m->g.esdf || m->esdf_tiled != 1 || m->esdf_full_needed) {
+    ts_set_error("%s: no tiled ESDF is in progress (tslam_esdf_tiled_begin, then no reset, load, fusion or ghost import)", what);
+    return TSLAM_E_INVALID;
+  }
+  return TSLAM_OK;
+}
+
+extern "C" int tslam_esdf_tiled_begin(tslam_tsdf_t* m, int32_t submap, int32_t* n_sweeps_out, void* stream) {
+  if (!m) return TSLAM_E_INVALID;
+  cudaStream_t st = (cudaStream_t)stream;
+  int rc = ts_flush_pending(m, st);
+  if (rc) return rc;
+  rc = es_alloc(m);
+  if (rc) return rc;
+  EsAux aux = es_aux(m);
+  const float gamma = (float)m->cfg.voxel_scale, far_v = (float)m->cfg.max_ray_length;
+  int n_lower = 0;
+  m->esdf_tiled = 1;
+  TS_CUDA(cudaMemsetAsync(aux.changed, 0, (2 * (ES_MAX_SWEEPS + 2) + 8) * 4, st));
+  k_esdf_init<true><<<m->sm_count * 4, 256, 0, st>>>(m->g, aux, submap, gamma, far_v);
+  TS_LAUNCH_CHECK(m);
+  rc = es_wave(m, st, aux.changed, ES_GROUP, [&](int k) { k_esdf_sweep<true><<<m->sm_count * 4, 256, 0, st>>>(m->g, aux, submap, k, gamma, m->in.vs); }, &n_lower);
+  if (rc) return rc;
+  m->esdf_full_needed = 0;
+  m->esdf_submap = submap;
+  if (n_sweeps_out) *n_sweeps_out = n_lower;
+  return TSLAM_OK;
+}
+
+extern "C" int tslam_esdf_ghost_unpack(tslam_tsdf_t* m, int64_t n, const int64_t* keys, const float* esdf, void* stream) {
+  if (!m || n < 0 || (n && (!keys || !esdf))) return TSLAM_E_INVALID;
+  int rc = es_tiled_open(m, "tslam_esdf_ghost_unpack");
+  if (rc || n == 0) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  int* bad = m->scratch_i + 12;
+  TS_CUDA(cudaMemsetAsync(bad, 0, 4, st));
+  k_esdf_ghost_unpack<<<(int)(n < m->sm_count * 4 ? n : m->sm_count * 4), 256, 0, st>>>(m->g, es_aux(m), n, (const long long*)keys,
+                                                                                         (const float4*)esdf, bad);
+  TS_LAUNCH_CHECK(m);
+  int h_bad = 0;
+  TS_CUDA(cudaMemcpyAsync(&h_bad, bad, 4, cudaMemcpyDeviceToHost, st));
+  TS_CUDA(cudaStreamSynchronize(st));
+  if (h_bad) {
+    ts_set_error("tslam_esdf_ghost_unpack: %d of %lld keys are not ghost blocks of submap %d (nothing written for them)", h_bad, (long long)n,
+                 m->esdf_submap);
+    return TSLAM_E_INVALID;
+  }
+  return TSLAM_OK;
+}
+
+extern "C" int tslam_esdf_tiled_relax(tslam_tsdf_t* m, int32_t* n_sweeps_out, void* stream) {
+  if (!m) return TSLAM_E_INVALID;
+  int rc = es_tiled_open(m, "tslam_esdf_tiled_relax");
+  if (rc) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  EsAux aux = es_aux(m);
+  const int submap = m->esdf_submap;
+  const float gamma = (float)m->cfg.voxel_scale;
+  int n_lower = 0;
+  TS_CUDA(cudaMemsetAsync(aux.changed, 0, (ES_MAX_SWEEPS + 2) * 4, st));
+  k_esdf_rearm<<<m->sm_count * 2, 256, 0, st>>>(m->g, aux);
+  TS_LAUNCH_CHECK(m);
+  rc = es_wave(m, st, aux.changed, 4, [&](int k) { k_esdf_sweep<true><<<m->sm_count * 4, 256, 0, st>>>(m->g, aux, submap, k, gamma, m->in.vs); }, &n_lower);
+  if (rc) return rc;
+  if (n_sweeps_out) *n_sweeps_out = n_lower;
+  return TSLAM_OK;
+}
+
+extern "C" int tslam_esdf_tiled_end(tslam_tsdf_t* m) {
+  if (!m) return TSLAM_E_INVALID;
+  int rc = es_tiled_open(m, "tslam_esdf_tiled_end");
+  if (rc) return rc;
+  m->esdf_tiled = 2;
+  return TSLAM_OK;
 }
 
 extern "C" int tslam_esdf_gather(tslam_tsdf_t* m, int32_t submap, int64_t cap, int32_t* idx, float* esdf, int64_t* n_out,
@@ -493,9 +625,10 @@ extern "C" int tslam_esdf_gather(tslam_tsdf_t* m, int32_t submap, int64_t cap, i
 // Both answer from the field as of the last update of the submap: the class byte that update left (not the live obs
 // plane) and only the blocks the update saw.  A block allocated later has a pool index >= *nb_seen (bump allocation;
 // a reset, which recycles the pool, forces the next update to be a full one and refuses queries until then).
-__device__ __forceinline__ int esq_block(const TsGrid& g, int submap, int nb_seen, int bx, int by, int bz) {
+// (ghost blocks count only after a completed tiled ESDF: they then hold their owners' final values)
+__device__ __forceinline__ int esq_block(const TsGrid& g, int submap, int nb_seen, bool ghosts, int bx, int by, int bz) {
   const int b = ts_find(g, ts_pack_key(submap, bx, by, bz));
-  return (b >= 0 && b < nb_seen && !g.ghost[b]) ? b : -1;
+  return (b >= 0 && b < nb_seen && (ghosts || !g.ghost[b])) ? b : -1;
 }
 // lerp(a, b, t) = a + t*(b - a), rounded step by step (never contracted to an FMA): tests/esdf_query_reference.py
 __device__ __forceinline__ float esq_lerp(float a, float b, float t) { return __fadd_rn(a, __fmul_rn(t, __fsub_rn(b, a))); }
@@ -503,35 +636,34 @@ __device__ __forceinline__ float esq_lerp(float a, float b, float t) { return __
 // Trilinear interpolation of the ESDF over the 8 voxels around each point (voxel i centred at i*vs, submap-local frame)
 // and the exact partial derivatives of that interpolant.  One thread per point; each distinct corner block is looked
 // up once (the corner cube spans 2, 4 or 8 blocks only where i0 & 15 == 15 on some axis).  Invalid (NaN, valid = 0):
-// a non-finite coordinate, a corner outside the volume, a corner in an absent / ghost / newer block, a corner that was
-// unobserved or INERT at the last update.
-__global__ void __launch_bounds__(256) k_esdf_query(TsGrid g, EsAux aux, int submap, long long n, const float* __restrict__ xyz,
+// a non-finite coordinate, a corner outside the volume, a corner in an absent / newer block, a corner in a ghost block
+// (unless `ghosts`: the field is a completed tiled ESDF), a corner that was unobserved or INERT at the last update.
+__global__ void __launch_bounds__(256) k_esdf_query(TsGrid g, EsAux aux, int submap, bool ghosts, long long n, const float* __restrict__ xyz,
                                                      float vs, float* __restrict__ dist, float* __restrict__ grad,
                                                      uint8_t* __restrict__ valid) {
   const int nb_seen = *aux.nb_seen;
-  const float lo = (float)(-g.hN), hi = (float)(g.N - g.hN - 1), loz = (float)(-g.hNz), hiz = (float)(g.Nz - g.hNz - 1);
   const float qnan = __int_as_float(0x7fc00000);
   for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < n; q += (long long)gridDim.x * blockDim.x) {
-    const float ux = __fdiv_rn(xyz[3 * q], vs), uy = __fdiv_rn(xyz[3 * q + 1], vs), uz = __fdiv_rn(xyz[3 * q + 2], vs);
-    // both corners i0, i0 + 1 inside the volume <=> lo <= u < hi.  NaN and +-inf fail the test, so no out-of-range
-    // value reaches the float -> int conversion below.
-    bool ok = ux >= lo && ux < hi && uy >= lo && uy < hi && uz >= loz && uz < hiz;
+    // both corners i0, i0 + 1 inside the volume: the low corner and i0 < N - hN - 1 per axis
+    float u[3];
+    int c0[3];
+    bool ok = esq_low_corner(g, vs, xyz + 3 * q, u, c0) && c0[0] < g.N - g.hN - 1 && c0[1] < g.N - g.hN - 1 && c0[2] < g.Nz - g.hNz - 1;
     float d = qnan, gx = qnan, gy = qnan, gz = qnan;
     if (ok) {
-      const int i0 = (int)floorf(ux), j0 = (int)floorf(uy), k0 = (int)floorf(uz);
-      const float fx = __fsub_rn(ux, (float)i0), fy = __fsub_rn(uy, (float)j0), fz = __fsub_rn(uz, (float)k0);
+      const int i0 = c0[0], j0 = c0[1], k0 = c0[2];
+      const float fx = __fsub_rn(u[0], (float)i0), fy = __fsub_rn(u[1], (float)j0), fz = __fsub_rn(u[2], (float)k0);
       const bool sx = (i0 & TS_BMASK) == TS_BMASK, sy = (j0 & TS_BMASK) == TS_BMASK, sz = (k0 & TS_BMASK) == TS_BMASK;
       const int x0 = i0 >> TS_BSHIFT, y0 = j0 >> TS_BSHIFT, z0 = k0 >> TS_BSHIFT;
       // b[dx*4 + dy*2 + dz]: block of corner (i0+dx, j0+dy, k0+dz); a corner that shares its block with a lower one reuses it
       int b[8];
-      b[0] = esq_block(g, submap, nb_seen, x0, y0, z0);
-      b[1] = sz ? esq_block(g, submap, nb_seen, x0, y0, z0 + 1) : b[0];
-      b[2] = sy ? esq_block(g, submap, nb_seen, x0, y0 + 1, z0) : b[0];
-      b[3] = sy ? (sz ? esq_block(g, submap, nb_seen, x0, y0 + 1, z0 + 1) : b[2]) : b[1];
-      b[4] = sx ? esq_block(g, submap, nb_seen, x0 + 1, y0, z0) : b[0];
-      b[5] = sx ? (sz ? esq_block(g, submap, nb_seen, x0 + 1, y0, z0 + 1) : b[4]) : b[1];
-      b[6] = sx ? (sy ? esq_block(g, submap, nb_seen, x0 + 1, y0 + 1, z0) : b[4]) : b[2];
-      b[7] = sx ? (sy ? (sz ? esq_block(g, submap, nb_seen, x0 + 1, y0 + 1, z0 + 1) : b[6]) : b[5]) : b[3];
+      b[0] = esq_block(g, submap, nb_seen, ghosts, x0, y0, z0);
+      b[1] = sz ? esq_block(g, submap, nb_seen, ghosts, x0, y0, z0 + 1) : b[0];
+      b[2] = sy ? esq_block(g, submap, nb_seen, ghosts, x0, y0 + 1, z0) : b[0];
+      b[3] = sy ? (sz ? esq_block(g, submap, nb_seen, ghosts, x0, y0 + 1, z0 + 1) : b[2]) : b[1];
+      b[4] = sx ? esq_block(g, submap, nb_seen, ghosts, x0 + 1, y0, z0) : b[0];
+      b[5] = sx ? (sz ? esq_block(g, submap, nb_seen, ghosts, x0 + 1, y0, z0 + 1) : b[4]) : b[1];
+      b[6] = sx ? (sy ? esq_block(g, submap, nb_seen, ghosts, x0 + 1, y0 + 1, z0) : b[4]) : b[2];
+      b[7] = sx ? (sy ? (sz ? esq_block(g, submap, nb_seen, ghosts, x0 + 1, y0 + 1, z0 + 1) : b[6]) : b[5]) : b[3];
       float e[8];
 #pragma unroll
       for (int c = 0; c < 8; c++) {
@@ -609,6 +741,10 @@ static int es_readable(tslam_tsdf* m, int32_t submap, const char* what) {
     ts_set_error("%s: the last tslam_esdf_update was for submap %d, not %d", what, m->esdf_submap, submap);
     return TSLAM_E_INVALID;
   }
+  if (m->esdf_tiled == 1) {
+    ts_set_error("%s: a tiled ESDF is in progress (tslam_esdf_tiled_begin without tslam_esdf_tiled_end)", what);
+    return TSLAM_E_INVALID;
+  }
   return TSLAM_OK;
 }
 
@@ -619,7 +755,8 @@ extern "C" int tslam_esdf_query(tslam_tsdf_t* m, int32_t submap, int64_t n, cons
   if (rc || n == 0) return rc;
   long long blocks = (n + 255) / 256;
   if (blocks > (long long)m->sm_count * 16) blocks = (long long)m->sm_count * 16;
-  k_esdf_query<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(m->g, es_aux(m), submap, n, xyz, m->in.vs, dist, grad, valid);
+  k_esdf_query<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(m->g, es_aux(m), submap, m->esdf_tiled == 2, n, xyz, m->in.vs, dist,
+                                                               grad, valid);
   TS_LAUNCH_CHECK(m);
   return TSLAM_OK;
 }

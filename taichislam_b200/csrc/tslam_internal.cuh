@@ -196,6 +196,18 @@ __device__ __forceinline__ int warp_append_i32(bool want, int* counter) {
   return want ? base + __popc(m & ((1u << lane) - 1)) : -1;
 }
 
+// Low interpolation corner of an ESDF query point (k_esdf_query, and k_owner_points which routes the points of a tiled
+// map to the rank that answers them): u = x / vs per axis, correctly rounded, c = floor(u).  False when a coordinate
+// is not finite or the corner lies outside the volume; NaN and +-inf fail the range test, so no out-of-range value
+// reaches the float -> int conversion.
+__device__ __forceinline__ bool esq_low_corner(const TsGrid& g, float vs, const float* p, float u[3], int c[3]) {
+  u[0] = __fdiv_rn(p[0], vs); u[1] = __fdiv_rn(p[1], vs); u[2] = __fdiv_rn(p[2], vs);
+  const bool ok = u[0] >= (float)(-g.hN) && u[0] < (float)(g.N - g.hN) && u[1] >= (float)(-g.hN) && u[1] < (float)(g.N - g.hN) &&
+                  u[2] >= (float)(-g.hNz) && u[2] < (float)(g.Nz - g.hNz);
+  if (ok) { c[0] = (int)floorf(u[0]); c[1] = (int)floorf(u[1]); c[2] = (int)floorf(u[2]); }
+  return ok;
+}
+
 // position of voxel (i, j, k) of submap s as the exporters write it (tslam_tsdf.cu, tslam_esdf.cu)
 __device__ __forceinline__ void voxel_xyz(const TsGrid& g, bool global_map, const float* pR, const float* pT, int s, int i, int j,
                                           int k, float vs, float& x, float& y, float& z) {
@@ -390,6 +402,7 @@ struct tslam_tsdf {
   int* scratch_i;      // small device scratch (counters for gather etc.)
   void* esdf_aux;      // ESDF: neighbour table, epochs, per-sweep change flags, class bytes (allocated with g.esdf)
   int esdf_full_needed, esdf_submap;  // the next update recomputes everything (first use, reset, bulk load) / submap of the kept state
+  int esdf_tiled;      // tiled ESDF (tslam_esdf_tiled_*): 0 = none (plain update), 1 = begun, exchange in progress, 2 = ended
   void* mc_scratch;    // marching cubes: per-block triangle counts / offsets (allocated on first use)
   long long launches;
   int n_integrate_calls;
@@ -490,6 +503,9 @@ int ts_cuda_fail(cudaError_t e, const char* what);
 int ts_flush_pending(tslam_tsdf* m, cudaStream_t st);   // commit if anything is pending
 int ts_check_deferred(tslam_tsdf* m);                    // read + translate device error flags (synchronises)
 int ts_check_deferred_async(tslam_tsdf* m, cudaStream_t st);  // same, after the work queued on st
+// tslam_esdf.cu: per-block exchange mark of the tiled ESDF ([max_blocks]; owned block: ESDF changed since it was last
+// packed, ghost block: ESDF unpacked since the last relax), or NULL before the first ESDF update
+int* ts_esdf_xmark(tslam_tsdf* m);
 // tslam_march.cu: block-binned ray march of the rays listed in m->ray_list (replaces k_raymarch<false>)
 int ts_march_alloc(tslam_tsdf* m);
 void ts_march_free(tslam_tsdf* m);

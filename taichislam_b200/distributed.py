@@ -166,6 +166,8 @@ class TiledGlobalMap:
         self._tiles_c = (C.c_int32 * 3)(*self.tiles)
         self.cuts = None
         self.last_exchange = {}
+        self._halo_current = False  # ghosts carry the TSDF of the last fusion (exchange_halo ran since)
+        self.esdf_submap = 0
 
     # ---- helpers ----------------------------------------------------------------------------------------
     def _L(self):
@@ -236,6 +238,7 @@ class TiledGlobalMap:
         capi.check(L.tslam_tsdf_commit_fused(h, st))
         torch.cuda.current_stream().synchronize()  # received buffers must outlive the kernels
         self.last_exchange["fusion_blocks_received"] = n_recv
+        self._halo_current = False
 
     def fuse_submaps_tiled(self, submaps):
         """fuse_submaps (dense_tsdf.py:312-318) with the result tiled over the ranks.  `submaps` = this rank's
@@ -281,6 +284,7 @@ class TiledGlobalMap:
         capi.check(L.tslam_tsdf_ghost_unpack2(h, n_recv, capi.tptr(bufs[0]), capi.tptr(bufs[1]), capi.tptr(bufs[2]), capi.tptr(col), st))
         torch.cuda.current_stream().synchronize()
         self.last_exchange["halo_blocks_received"] = n_recv
+        self._halo_current = True
 
     def exchange_halo(self):
         import torch
@@ -302,6 +306,157 @@ class TiledGlobalMap:
         allv, counts = all_gather_ragged(self.dist, v, self.world)
         alln, _ = all_gather_ragged(self.dist, nrm, self.world)
         return allv, alln, [c // 3 for c in counts]
+
+
+    # ---- ESDF, phase by phase (csrc/tslam_esdf.cu: tslam_esdf_tiled_*) -------------------------------------------
+    # The tiled ESDF is a full recompute: begin seeds owned and ghost blocks and runs the local wave with the ghosts as
+    # read-only sources; then rounds of (pack the boundary blocks that changed -> all-to-all -> unpack into the
+    # neighbours' ghosts -> relax from them) until no rank packs anything.  The result is bit-identical to one map
+    # holding every tile (DESIGN.md section 6).
+    def esdf_begin(self, submap=0):
+        self.esdf_submap = int(submap)
+        return self.m._h.esdf_tiled_begin(submap)
+
+    def esdf_halo_pack(self):
+        """Owned boundary blocks whose ESDF changed since they were last packed -> (send counts, (keys, esdf))."""
+        import torch
+        from . import _capi as capi
+        L, h, st = self._L(), self._h(), capi.stream_ptr()
+        dev = torch.device("cuda", torch.cuda.current_device())
+        send = np.zeros(self.world, np.int32)
+        capi.check(L.tslam_esdf_halo_count(h, self._tiles_c, self.rank, self.world, capi.np_ptr(send), st))
+        n_send = int(send.sum())
+        keys = torch.empty(max(n_send, 1), dtype=torch.int64, device=dev)
+        esdf = torch.empty((max(n_send, 1), 4096), dtype=torch.float32, device=dev)
+        capi.check(L.tslam_esdf_halo_pack(h, self._tiles_c, self.rank, self.world, capi.np_ptr(send), n_send, capi.tptr(keys),
+                                          capi.tptr(esdf), st))
+        self.last_exchange["esdf_blocks_sent"] = self.last_exchange.get("esdf_blocks_sent", 0) + n_send
+        return send, (keys[:n_send], esdf[:n_send])
+
+    def esdf_halo_unpack(self, bufs):
+        import torch
+        self.m._h.esdf_ghost_unpack(bufs[0], bufs[1])
+        torch.cuda.current_stream().synchronize()
+
+    def esdf_relax(self):
+        return self.m._h.esdf_tiled_relax()
+
+    def esdf_end(self):
+        self.m._h.esdf_tiled_end()
+
+    def esdf_update(self, submap=0, max_rounds=1024):
+        """Tiled ESDF of `submap` on every rank (collective) -> dict(rounds, sweeps, blocks_sent, bytes_sent) of this
+        rank; rounds = exchange rounds in which some rank sent a block.  Runs a TSDF halo exchange first unless one
+        has run since the last fusion.  Raises after `max_rounds` rounds."""
+        import torch
+        dev = torch.device("cuda", torch.cuda.current_device())
+        if not self._halo_current:
+            self.exchange_halo()
+        self.last_exchange["esdf_blocks_sent"] = 0
+        sweeps = self.esdf_begin(submap)
+        rounds = 0
+        while True:
+            send, bufs = self.esdf_halo_pack()
+            tot = torch.tensor([int(send.sum())], dtype=torch.int64, device=dev)
+            self.dist.all_reduce(tot)
+            if int(tot.item()) == 0:
+                break
+            rounds += 1
+            if rounds > max_rounds:
+                raise RuntimeError(f"tiled ESDF: still exchanging after {max_rounds} rounds")
+            recv = exchange_counts(self.dist, send, dev)
+            self.esdf_halo_unpack(tuple(exchange_rows(self.dist, b, send, recv) for b in bufs))
+            sweeps += self.esdf_relax()
+        self.esdf_end()
+        return _esdf_stats(rounds, sweeps, self.last_exchange["esdf_blocks_sent"])
+
+    def _query_dest(self, xyz):
+        """Points f32[n,3] on the device and the rank that answers each: the owner of the block holding its low
+        interpolation corner; this rank for points no tile holds (they come out invalid anywhere)."""
+        import torch
+        from . import _capi as capi
+        x = self.m._h._dev_f32(xyz).reshape(-1, 3)
+        owner = torch.empty(x.shape[0], dtype=torch.int32, device=x.device)
+        capi.check(self._L().tslam_tiling_owner_points(self._h(), self._tiles_c, self.world, x.shape[0], capi.tptr(x), capi.tptr(owner),
+                                                       capi.stream_ptr()))
+        return x, torch.where(owner < 0, torch.full_like(owner, self.rank), owner).long()
+
+    def _esdf_answer(self, pts):
+        """tslam_esdf_query on points routed here -> (dist|grad f32[n,4], valid u8[n])."""
+        import torch
+        from . import _capi as capi
+        n = pts.shape[0]
+        dg = torch.empty((n, 4), dtype=torch.float32, device=pts.device)
+        dist = torch.empty(n, dtype=torch.float32, device=pts.device)
+        grad = torch.empty((n, 3), dtype=torch.float32, device=pts.device)
+        valid = torch.empty(n, dtype=torch.uint8, device=pts.device)
+        capi.check(self._L().tslam_esdf_query(self._h(), self.esdf_submap, n, capi.tptr(pts), capi.tptr(dist), capi.tptr(grad),
+                                              capi.tptr(valid), capi.stream_ptr()))
+        dg[:, 0] = dist
+        dg[:, 1:] = grad
+        return dg, valid
+
+    def esdf_query(self, xyz):
+        """Trilinear ESDF and gradient (TsdfHandle.esdf_query) at this rank's points, answered by the ranks that own
+        them (collective: every rank calls it, with any points).  Returns (dist, grad, valid) in the caller's order:
+        torch CUDA tensors for a torch tensor, numpy arrays for numpy."""
+        import torch
+        as_torch = isinstance(xyz, torch.Tensor)
+        x, dest = self._query_dest(xyz)
+        dg, valid = routed_answers(self.dist, x, dest, self.world, self._esdf_answer)
+        return _query_result(dg, valid, as_torch)
+
+    def esdf_slice_local(self, z):
+        """This rank's part of the ESDF slice at height z: (xyz f32[n,3], ESDF f32[n]) torch CUDA tensors."""
+        import torch
+        dev = torch.device("cuda", torch.cuda.current_device())
+        _, xyz, val = self.m._h.esdf_slice(z, submap=self.esdf_submap)
+        return torch.from_numpy(xyz).to(dev), torch.from_numpy(val).to(dev)
+
+    def esdf_slice_all_gather(self, z):
+        """cvt_ESDF_to_voxels_slice of the whole tiled map on every rank: (xyz, ESDF) torch CUDA tensors."""
+        xyz, val = self.esdf_slice_local(z)
+        allx, _ = all_gather_ragged(self.dist, xyz, self.world)
+        allv, _ = all_gather_ragged(self.dist, val, self.world)
+        return allx, allv
+
+
+def _esdf_stats(rounds, sweeps, blocks):
+    return dict(rounds=int(rounds), sweeps=int(sweeps), blocks_sent=int(blocks), bytes_sent=int(blocks) * (8 + 4096 * 4))
+
+
+def _query_result(dg, valid, as_torch):
+    import torch
+    dist, grad, valid = dg[:, 0].contiguous(), dg[:, 1:].contiguous(), valid.view(torch.bool)
+    if as_torch:
+        return dist, grad, valid
+    return dist.cpu().numpy(), grad.cpu().numpy(), valid.cpu().numpy()
+
+
+def route_order(dest, world):
+    """Rows addressed to ranks dest (int64 tensor [n]): the stable order that groups them by destination, and the
+    rows per destination."""
+    import torch
+    order = torch.argsort(dest, stable=True)
+    counts = torch.bincount(dest, minlength=world).cpu().numpy().astype(np.int64)
+    return order, counts
+
+
+def route_restore(order, rows):
+    """Undo route_order: rows[i] belongs to caller row order[i]."""
+    import torch
+    out = torch.empty_like(rows)
+    out[order] = rows
+    return out
+
+
+def routed_answers(dist, rows, dest, world, answer):
+    """Send row i to rank dest[i] (all-to-all), answer there with answer(rows) -> tuple of tensors with one row per
+    row, send the answers back: the answers in the caller's row order."""
+    order, send = route_order(dest, world)
+    recv = exchange_counts(dist, send, rows.device)
+    got = exchange_rows(dist, rows[order], send, recv)
+    return tuple(route_restore(order, exchange_rows(dist, a, recv, send)) for a in answer(got))
 
 
 def run_local_fusion(tiled, submaps):
@@ -328,3 +483,44 @@ def run_local_mesh(tiled, meshers, step=1):
     import torch
     vs, ns = zip(*[t.local_mesh(m, step) for t, m in zip(tiled, meshers)])
     return torch.cat(vs, 0), torch.cat(ns, 0), [int(v.shape[0]) // 3 for v in vs]
+
+
+def run_local_esdf(tiled, submap=0, max_rounds=1024):
+    """TiledGlobalMap.esdf_update on `world` virtual ranks in one process; the statistics are summed over the ranks."""
+    world = len(tiled)
+    if not all(t._halo_current for t in tiled):
+        packed = [t.halo_pack() for t in tiled]
+        routed, _ = _route([p[1] for p in packed], [p[0] for p in packed], world)
+        for t, bufs in zip(tiled, routed):
+            t.halo_unpack(bufs)
+    sweeps = sum(t.esdf_begin(submap) for t in tiled)
+    rounds = blocks = 0
+    while True:
+        packed = [t.esdf_halo_pack() for t in tiled]
+        n = sum(int(p[0].sum()) for p in packed)
+        if n == 0:
+            break
+        rounds += 1
+        blocks += n
+        if rounds > max_rounds:
+            raise RuntimeError(f"tiled ESDF: still exchanging after {max_rounds} rounds")
+        routed, _ = _route([p[1] for p in packed], [p[0] for p in packed], world)
+        for t, bufs in zip(tiled, routed):
+            t.esdf_halo_unpack(bufs)
+        sweeps += sum(t.esdf_relax() for t in tiled)
+    for t in tiled:
+        t.esdf_end()
+    return _esdf_stats(rounds, sweeps, blocks)
+
+
+def run_local_esdf_query(tiled, xyz_per_rank):
+    """TiledGlobalMap.esdf_query on `world` virtual ranks: [(dist, grad, valid)] per rank, in each caller's order."""
+    import torch
+    world = len(tiled)
+    plans = [t._query_dest(x) for t, x in zip(tiled, xyz_per_rank)]
+    orders, sends = zip(*[route_order(dest, world) for _, dest in plans])
+    routed, rcounts = _route([(x[o],) for (x, _), o in zip(plans, orders)], sends, world)
+    answers = [t._esdf_answer(pts[0]) for t, pts in zip(tiled, routed)]
+    back, _ = _route(answers, rcounts, world)
+    return [_query_result(route_restore(o, b[0]), route_restore(o, b[1]), isinstance(x, torch.Tensor))
+            for o, b, x in zip(orders, back, xyz_per_rank)]

@@ -280,6 +280,27 @@ class TsdfHandle:
         capi.check(self.L.tslam_esdf_update2(self.h, int(submap), 1 if full else 0, capi.np_ptr(st), capi.stream_ptr()))
         return dict(lower_sweeps=int(st[0]), raise_sweeps=int(st[1]), changed=int(st[2]), suspect=int(st[3]))
 
+    # -- ESDF of a tiled global map (the exchange between the phases is taichislam_b200.distributed's) ----------
+    def esdf_tiled_begin(self, submap=0):
+        """Seed owned and ghost blocks, run the local wave with ghosts as read-only sources -> sweeps."""
+        sw = C.c_int32(0)
+        capi.check(self.L.tslam_esdf_tiled_begin(self.h, int(submap), C.byref(sw), capi.stream_ptr()))
+        return int(sw.value)
+
+    def esdf_ghost_unpack(self, keys, esdf):
+        """Overwrite the ESDF of existing ghost blocks: keys int64[n], esdf f32[n,4096] torch CUDA tensors."""
+        n = int(keys.shape[0])
+        capi.check(self.L.tslam_esdf_ghost_unpack(self.h, n, capi.tptr(keys), capi.tptr(esdf), capi.stream_ptr()))
+
+    def esdf_tiled_relax(self):
+        """The wave from the ghosts unpacked since the last relax -> sweeps."""
+        sw = C.c_int32(0)
+        capi.check(self.L.tslam_esdf_tiled_relax(self.h, C.byref(sw), capi.stream_ptr()))
+        return int(sw.value)
+
+    def esdf_tiled_end(self):
+        capi.check(self.L.tslam_esdf_tiled_end(self.h))
+
     def esdf_gather(self, submap=0):
         torch = self.torch
         cap = self.count_active(submap)

@@ -6,12 +6,24 @@
 64 submaps (20 frames of the S2 scene each, base poses on an 8x8 grid, 6 m pitch), integrated submap-sharded
 (rank r owns submaps r, r+W, ...), fused into a 2048^3 x 0.05 m global volume tiled over the ranks (2x2x2 for 8):
 foreign blocks travel in one NCCL all-to-all, the boundary layer is exchanged as ghost blocks, marching cubes runs
-locally and the triangle soup is all-gathered.  Prints one JSON line on rank 0."""
+locally and the triangle soup is all-gathered.  Then the tiled ESDF of the fused map (exchange rounds of boundary-block
+ESDF until no rank sends) and routed ESDF queries (2^20 uniform points per rank, answered by the owning ranks).
+Prints one JSON line on rank 0, with the GPU model and its power limit beside the figures."""
 import json, os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
 import torch
 import torch.distributed as dist
+
+
+def _power_limit(dev):
+    """Enforced power limit of the GPU in W (read only), or None where NVML cannot say."""
+    try:
+        import pynvml
+        pynvml.nvmlInit()
+        return pynvml.nvmlDeviceGetEnforcedPowerLimit(pynvml.nvmlDeviceGetHandleByIndex(dev)) / 1000.0
+    except Exception:
+        return None
 
 
 def main():
@@ -59,6 +71,22 @@ def main():
     torch.cuda.synchronize(); dist.barrier()
     t_mesh = time.perf_counter() - t0
     x.update(tiled.last_exchange)
+    t0 = time.perf_counter()
+    es = tiled.esdf_update()  # (the mesh's halo exchange is current: no TSDF halo inside)
+    torch.cuda.synchronize(); dist.barrier()
+    t_esdf = time.perf_counter() - t0
+    rng = np.random.default_rng(rank)
+    pts = torch.from_numpy(rng.uniform([-51.2, -51.2, -2.0], [51.2, 51.2, 6.0], size=(1 << 20, 3)).astype(np.float32)).cuda()
+    tiled.esdf_query(pts)  # warm
+    torch.cuda.synchronize(); dist.barrier()
+    t0 = time.perf_counter()
+    reps = 5
+    for _ in range(reps):
+        dq, gq, vq = tiled.esdf_query(pts)
+    torch.cuda.synchronize(); dist.barrier()
+    t_query = (time.perf_counter() - t0) / reps
+    esx = torch.tensor([es["blocks_sent"], es["bytes_sent"], int(vq.sum().item())], dtype=torch.float64, device="cuda")
+    dist.all_reduce(esx)
     own = torch.tensor([glo.count_active(), sum(sub._h.count_active(s) for s in mine), x["fusion_blocks_sent"], x.get("halo_blocks_sent", 0),
                         glo._h.stats()["n_blocks"]], dtype=torch.float64, device="cuda")
     dist.all_reduce(own)
@@ -68,7 +96,11 @@ def main():
                           "fuse_ms": 1e3 * t_fuse, "source_voxels": int(own[1].item()), "global_voxels": int(own[0].item()),
                           "fusion_blocks_exchanged": int(own[2].item()), "fusion_exchange_MB": own[2].item() * (8 + 4096 * 10) / 1e6,
                           "halo_blocks_exchanged": int(own[3].item()), "mesh_ms_incl_halo_and_allgather": 1e3 * t_mesh,
-                          "triangles": int(sum(counts)), "triangles_per_rank": counts, "global_blocks": int(own[4].item())}))
+                          "triangles": int(sum(counts)), "triangles_per_rank": counts, "global_blocks": int(own[4].item()),
+                          "esdf_ms": 1e3 * t_esdf, "esdf_rounds": es["rounds"], "esdf_halo_blocks": int(esx[0].item()),
+                          "esdf_halo_MB": esx[1].item() / 1e6, "query_points_per_rank": 1 << 20, "query_ms": 1e3 * t_query,
+                          "query_Gpoints_per_s": world * (1 << 20) / t_query / 1e9, "query_valid": int(esx[2].item()),
+                          "gpu": torch.cuda.get_device_name(local), "power_limit_W": _power_limit(local)}))
     dist.destroy_process_group()
 
 

@@ -45,7 +45,7 @@ const char* tslam_last_error(void);
 int tslam_device_count(void);
 /* ABI version of this header (tests check the library agrees). */
 int tslam_abi_version(void);
-#define TSLAM_ABI_VERSION 5
+#define TSLAM_ABI_VERSION 6
 
 /* ----------------------------------------------------------------------------
  * TSDF map  (DenseTSDF, dense_tsdf.py)
@@ -260,6 +260,28 @@ int tslam_tsdf_ghost_unpack2(tslam_tsdf_t* m, int64_t n, const int64_t* keys, co
  * for a point that is not finite or whose low corner lies outside the volume (any rank answers those: invalid). */
 int tslam_tiling_owner_points(tslam_tsdf_t* m, const int32_t* tiles3, int32_t world, int64_t n, const float* xyz, int32_t* owner,
                               void* stream);
+/* Planner queries of the tiled map (DESIGN.md section 6).  Every answer is bit-identical to the same query on one map
+ * holding every tile; the host layer routes the points / rays (TiledGlobalMap.raycast, is_pos_occupy, ...).
+ * tslam_tiling_owner_cells: owner[n] (DEVICE int32) = owner rank of the block holding the cell round(x / vs) of each
+ * point xyz f32[n,3] (DEVICE) - the cell tslam_tsdf_query_points / _query_near_occupy read, by the same f32 expression -
+ * or -1 for a cell outside the volume (it reads occupied and unobserved on any rank). */
+int tslam_tiling_owner_cells(tslam_tsdf_t* m, const int32_t* tiles3, int32_t world, int64_t n, const float* xyz, int32_t* owner,
+                             void* stream);
+/* One round of tslam_tsdf_raycast on a tiled map.  ray f32[n,8] (DEVICE, in/out) = pos[3], dir[3], max_dist, next
+ * sample j (int32 bits; 0 for a new ray).  Marches each ray from sample j while the sample's cell lies in a block this
+ * rank owns (ghosts are not read).  A ray that reaches a block of another rank gets dest[i] = that rank and its j
+ * written back into row i; route the row there and call again.  A ray that hits, leaves the volume or runs out of
+ * steps (int)(max_dist / vs) gets dest[i] = -1 and the answer of tslam_tsdf_raycast in row i of hit u8[n] /
+ * xyz_out f32[n,3] / len_out f32[n]; those rows are untouched for a handed-over ray.  A batch is done after at most
+ * tx+ty+tz-2 hand-over rounds (DESIGN.md section 6).  Does not synchronise. */
+int tslam_tsdf_raycast_tiled(tslam_tsdf_t* m, const int32_t* tiles3, int32_t rank, int32_t world, int32_t submap, int64_t n, float* ray,
+                             int32_t* dest, uint8_t* hit, float* xyz_out, float* len_out, void* stream);
+/* tslam_tsdf_query_near_occupy that also reads ghost blocks, for points routed to the owner of their centre cell
+ * (tslam_tiling_owner_cells).  The answer is exact when the ghosts carry the current TSDF - a halo exchange after the
+ * last fusion, which the host layer runs first - and voxel is in [0, 16]: the window then stays within the blocks next
+ * to the centre cell's block, all of which the halo brings.  TSLAM_E_INVALID for voxel outside [0, 16]. */
+int tslam_tsdf_query_near_occupy_tiled(tslam_tsdf_t* m, int32_t submap, int64_t n, const float* xyz, int32_t voxel, uint8_t* out,
+                                       void* stream);
 /* ESDF of the tiled map (DESIGN.md section 6).  Always a full recompute of `submap`, exact: the result is bit-identical
  * to tslam_esdf_update2 on one map holding every tile.  Run a TSDF halo exchange first (ghosts must carry the current
  * TSDF), then on every rank:

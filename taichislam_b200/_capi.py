@@ -16,7 +16,7 @@ E_INVALID, E_CUDA, E_POOL_FULL, E_CAPACITY, E_NOGPU = -1, -2, -3, -4, -5
 MEM_DEVICE, MEM_HOST = 0, 1
 F_COMMIT = 1
 MAX_BATCH = 64
-ABI_VERSION = 5
+ABI_VERSION = 6
 
 
 class TslamError(RuntimeError):
@@ -108,6 +108,9 @@ SIGNATURES = {
     "tslam_tsdf_halo_pack2": (C.c_int, [_vp, _vp, _i32, _i32, _vp, _i64, _vp, _vp, _vp, _vp, _vp]),
     "tslam_tsdf_ghost_unpack2": (C.c_int, [_vp, _i64, _vp, _vp, _vp, _vp, _vp]),
     "tslam_tiling_owner_points": (C.c_int, [_vp, _vp, _i32, _i64, _vp, _vp, _vp]),
+    "tslam_tiling_owner_cells": (C.c_int, [_vp, _vp, _i32, _i64, _vp, _vp, _vp]),
+    "tslam_tsdf_raycast_tiled": (C.c_int, [_vp, _vp, _i32, _i32, _i32, _i64, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "tslam_tsdf_query_near_occupy_tiled": (C.c_int, [_vp, _i32, _i64, _vp, _i32, _vp, _vp]),
     "tslam_esdf_tiled_begin": (C.c_int, [_vp, _i32, C.POINTER(_i32), _vp]),
     "tslam_esdf_halo_count": (C.c_int, [_vp, _vp, _i32, _i32, _vp, _vp]),
     "tslam_esdf_halo_pack": (C.c_int, [_vp, _vp, _i32, _i32, _vp, _i64, _vp, _vp, _vp]),

@@ -309,6 +309,58 @@ __global__ void __launch_bounds__(256) k_owner_points(TsGrid g, TsTiling t, floa
   }
 }
 
+// ---- planner queries of a tiled map (tslam_query.cu) ---------------------------------------------------------------
+// owner rank of the block holding each point's cell round(x / vs) - the cell tsdf_probe reads, by the same helper -
+// or -1 for a cell outside the volume (it reads occupied and unobserved on any rank)
+__global__ void __launch_bounds__(256) k_owner_cells(TsGrid g, TsTiling t, float vs, long long n, const float* __restrict__ xyz,
+                                                      int* __restrict__ owner) {
+  for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < n; q += (long long)gridDim.x * blockDim.x) {
+    int c[3];
+    owner[q] = ts_query_cell(g, xyz[3 * q], xyz[3 * q + 1], xyz[3 * q + 2], vs, c) ? tile_owner(t, c[0] >> TS_BSHIFT, c[1] >> TS_BSHIFT, c[2] >> TS_BSHIFT)
+                                                                                   : -1;
+  }
+}
+
+// One round of BaseMap.raycast (mapping_common.py:165-178) on a tiled map, one lane per ray row f32[8] = pos, dir,
+// max_dist, next sample j (int32 bits).  Sample j is a function of (pos, dir, j) alone, computed by the expressions of
+// k_tsdf_raycast, so a ray that stops at sample j here and continues at j on another rank visits the same cells with
+// the same bits as one uninterrupted march.  The march runs while the sample's cell lies in a block this rank owns;
+// ghosts are not read.  A sample in a foreign block hands the ray over: dest = its owner, j written back.  A hit, a
+// sample outside the volume (occupied on any rank) or the last step ends the ray here: dest = -1 and the answer of
+// k_tsdf_raycast in row i of hit / xyz_out / len_out (for a miss: the last sample's position and length).
+__global__ void __launch_bounds__(256) k_tsdf_raycast_tiled(TsGrid g, TsTiling t, int s, long long n, float* __restrict__ ray, float vs,
+                                                             float thres, int* __restrict__ dest, uint8_t* hit, float* xyz_out, float* len_out) {
+  for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < n; q += (long long)gridDim.x * blockDim.x) {
+    float* r = ray + 8 * q;
+    const float px = r[0], py = r[1], pz = r[2];
+    const float dx = r[3], dy = r[4], dz = r[5];
+    const int steps = (int)(r[6] / vs);  // as k_tsdf_raycast
+    int j = __float_as_int(r[7]), to = -1;
+    float x = 0.f, y = 0.f, z = 0.f, len = 0.f;
+    bool succ = false;
+    for (; j < steps; j++) {
+      len = (float)j * vs;
+      x = dx * len + px; y = dy * len + py; z = dz * len + pz;
+      int c[3];
+      if (!ts_query_cell(g, x, y, z, vs, c)) { succ = true; break; }  // outside the volume: TSDF 0 on every rank
+      const int o = tile_owner(t, c[0] >> TS_BSHIFT, c[1] >> TS_BSHIFT, c[2] >> TS_BSHIFT);
+      if (o != t.rank) { to = o; break; }
+      float tv = 0.0f;
+      int ob = 0;
+      ts_query_read<false>(g, s, c, tv, ob);
+      if (tv < thres) { succ = true; break; }
+    }
+    dest[q] = to;
+    if (to >= 0) {
+      r[7] = __int_as_float(j);
+      continue;
+    }
+    hit[q] = succ ? 1 : 0;
+    xyz_out[3 * q] = x; xyz_out[3 * q + 1] = y; xyz_out[3 * q + 2] = z;
+    len_out[q] = len;
+  }
+}
+
 // ---- C ABI -------------------------------------------------------------------------------------------------------
 // defined in tslam_tsdf.cu
 extern "C" int tslam_tsdf_fuse_pending(tslam_tsdf_t* dst, tslam_tsdf_t* src, void* stream);
@@ -337,6 +389,37 @@ extern "C" int tslam_tiling_owner_points(tslam_tsdf_t* m, const int32_t* tiles3,
   long long blocks = (n + 255) / 256;
   if (blocks > (long long)m->sm_count * 16) blocks = (long long)m->sm_count * 16;
   k_owner_points<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(m->g, t, m->in.vs, n, xyz, owner);
+  TS_LAUNCH_CHECK(m);
+  return TSLAM_OK;
+}
+
+static int lanes_grid(long long n, int sm) {
+  const long long b = (n + 255) / 256;
+  return (int)(b < (long long)sm * 16 ? b : (long long)sm * 16);
+}
+
+extern "C" int tslam_tiling_owner_cells(tslam_tsdf_t* m, const int32_t* tiles3, int32_t world, int64_t n, const float* xyz, int32_t* owner,
+                                        void* stream) {
+  if (!m || n < 0 || (n && (!xyz || !owner))) return TSLAM_E_INVALID;
+  TsTiling t;
+  int rc = fill_tiling(m, tiles3, 0, world, &t);
+  if (rc || n == 0) return rc;
+  k_owner_cells<<<lanes_grid(n, m->sm_count), 256, 0, (cudaStream_t)stream>>>(m->g, t, m->in.vs, n, xyz, owner);
+  TS_LAUNCH_CHECK(m);
+  return TSLAM_OK;
+}
+
+extern "C" int tslam_tsdf_raycast_tiled(tslam_tsdf_t* m, const int32_t* tiles3, int32_t rank, int32_t world, int32_t submap, int64_t n,
+                                        float* ray, int32_t* dest, uint8_t* hit, float* xyz_out, float* len_out, void* stream) {
+  if (!m || n < 0 || (n && (!ray || !dest || !hit || !xyz_out || !len_out))) return TSLAM_E_INVALID;
+  TsTiling t;
+  int rc = fill_tiling(m, tiles3, rank, world, &t);
+  if (rc || n == 0) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  rc = ts_flush_pending(m, st);
+  if (rc) return rc;
+  k_tsdf_raycast_tiled<<<lanes_grid(n, m->sm_count), 256, 0, st>>>(m->g, t, submap, n, ray, m->in.vs, (float)(m->cfg.voxel_scale * 1.8), dest,
+                                                                   hit, xyz_out, len_out);
   TS_LAUNCH_CHECK(m);
   return TSLAM_OK;
 }

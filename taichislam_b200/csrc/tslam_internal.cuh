@@ -208,6 +208,28 @@ __device__ __forceinline__ bool esq_low_corner(const TsGrid& g, float vs, const 
   return ok;
 }
 
+// Cell of a planner-query point (sxyz_to_ijk, mapping_common.py:257-261): c = (int)roundf(x / vs) per axis, and whether
+// it lies in the volume.  The probe of the planner queries (tslam_query.cu), the tiled ray march and the routing of
+// point queries (k_tsdf_raycast_tiled, k_owner_cells) share this one expression, so a point is routed to the rank that
+// owns the cell the probe reads.  A NaN coordinate converts to index 0 and +-inf saturates (out of the volume), in all
+// of them alike.
+__device__ __forceinline__ bool ts_query_cell(const TsGrid& g, float x, float y, float z, float vs, int c[3]) {
+  c[0] = (int)roundf(x / vs); c[1] = (int)roundf(y / vs); c[2] = (int)roundf(z / vs);
+  return ts_in_bounds(g, c[0], c[1], c[2]);
+}
+
+// TSDF and observed byte of in-volume cell c of submap s as the planner queries read them: a block that is absent reads
+// (0, 0), i.e. occupied and unobserved, and so does a ghost block unless Ghosts.
+template <bool Ghosts>
+__device__ __forceinline__ void ts_query_read(const TsGrid& g, int s, const int c[3], float& t, int& o) {
+  const int blk = ts_find(g, ts_pack_key(s, c[0] >> TS_BSHIFT, c[1] >> TS_BSHIFT, c[2] >> TS_BSHIFT));
+  if (blk >= 0 && (Ghosts || !g.ghost[blk])) {
+    const size_t off = (size_t)blk * TS_B3 + ts_voxel_off(c[0], c[1], c[2]);
+    t = g.tw[off].x;
+    o = g.obs[off];
+  }
+}
+
 // position of voxel (i, j, k) of submap s as the exporters write it (tslam_tsdf.cu, tslam_esdf.cu)
 __device__ __forceinline__ void voxel_xyz(const TsGrid& g, bool global_map, const float* pR, const float* pT, int s, int i, int j,
                                           int k, float vs, float& x, float& y, float& z) {

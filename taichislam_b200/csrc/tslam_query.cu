@@ -7,18 +7,13 @@ __device__ __forceinline__ int q_iround(float x) { return (int)roundf(x); }
 
 // DenseTSDF.is_occupy (dense_tsdf.py:152-155): TSDF[sijk] < tsdf_surface_thres - no observed test, and an
 // inactive cell reads 0, so unobserved space counts as occupied.  is_unobserved (:148-150): observed == 0.
+// Ghost blocks read as inactive unless Ghosts (the near-occupancy query of a tiled map, whose ghosts are current).
+template <bool Ghosts = false>
 __device__ __forceinline__ void tsdf_probe(const TsGrid& g, int s, float x, float y, float z, float vs, float thres, bool& occ, bool& unobs) {
-  const int i = q_iround(x / vs), j = q_iround(y / vs), k = q_iround(z / vs);  // sxyz_to_ijk mapping_common.py:257-261
+  int c[3];
   float t = 0.0f;
   int o = 0;
-  if (ts_in_bounds(g, i, j, k)) {
-    const int blk = ts_find(g, ts_pack_key(s, i >> TS_BSHIFT, j >> TS_BSHIFT, k >> TS_BSHIFT));
-    if (blk >= 0 && !g.ghost[blk]) {
-      const size_t off = (size_t)blk * TS_B3 + ts_voxel_off(i, j, k);
-      t = g.tw[off].x;
-      o = g.obs[off];
-    }
-  }
+  if (ts_query_cell(g, x, y, z, vs, c)) ts_query_read<Ghosts>(g, s, c, t, o);  // sxyz_to_ijk mapping_common.py:257-261
   occ = t < thres;
   unobs = o == 0;
 }
@@ -32,7 +27,10 @@ __global__ void __launch_bounds__(256) k_tsdf_query_points(TsGrid g, int s, long
   }
 }
 
-// is_near_pos_occupy (mapping_common.py:193-204): any occupied cell in [-voxel, voxel)^3 around the point's cell
+// is_near_pos_occupy (mapping_common.py:193-204): any occupied cell in [-voxel, voxel)^3 around the point's cell.
+// Ghosts: ghost blocks are read like owned ones (a tiled map after a halo exchange, voxel <= 16: the window stays in
+// the 3^3 blocks around the centre cell's block, and the halo carries every one of them that lies in a foreign tile).
+template <bool Ghosts>
 __global__ void __launch_bounds__(256) k_tsdf_query_near(TsGrid g, int s, long long n, const float* __restrict__ xyz, float vs, float thres,
                                                           int voxel, uint8_t* out) {
   for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < n; q += (long long)gridDim.x * blockDim.x) {
@@ -42,7 +40,7 @@ __global__ void __launch_bounds__(256) k_tsdf_query_near(TsGrid g, int s, long l
       for (int j = -voxel; j < voxel && !any; j++)
         for (int k = -voxel; k < voxel && !any; k++) {
           bool occ, un;
-          tsdf_probe(g, s, (float)(i0 + i) * vs, (float)(j0 + j) * vs, (float)(k0 + k) * vs, vs, thres, occ, un);
+          tsdf_probe<Ghosts>(g, s, (float)(i0 + i) * vs, (float)(j0 + j) * vs, (float)(k0 + k) * vs, vs, thres, occ, un);
           // (probe re-rounds (i0+i)*vs/vs; exact for |index| < 2^22)
           any = occ;
         }
@@ -127,7 +125,22 @@ extern "C" int tslam_tsdf_query_near_occupy(tslam_tsdf_t* m, int32_t submap, int
   cudaStream_t st = (cudaStream_t)stream;
   int rc = ts_flush_pending(m, st);
   if (rc) return rc;
-  k_tsdf_query_near<<<grid_for(n, m->sm_count), 256, 0, st>>>(m->g, submap, n, xyz, m->in.vs, (float)(m->cfg.voxel_scale * 1.8), voxel, out);
+  k_tsdf_query_near<false><<<grid_for(n, m->sm_count), 256, 0, st>>>(m->g, submap, n, xyz, m->in.vs, (float)(m->cfg.voxel_scale * 1.8), voxel, out);
+  TS_LAUNCH_CHECK(m);
+  return TSLAM_OK;
+}
+extern "C" int tslam_tsdf_query_near_occupy_tiled(tslam_tsdf_t* m, int32_t submap, int64_t n, const float* xyz, int32_t voxel, uint8_t* out,
+                                                  void* stream) {
+  if (!m || n < 0 || (n && (!xyz || !out))) return TSLAM_E_INVALID;
+  if (voxel < 0 || voxel > TS_B) {
+    ts_set_error("tslam_tsdf_query_near_occupy_tiled: voxel %d outside [0, %d] (the halo holds one block)", voxel, TS_B);
+    return TSLAM_E_INVALID;
+  }
+  if (n == 0) return TSLAM_OK;
+  cudaStream_t st = (cudaStream_t)stream;
+  int rc = ts_flush_pending(m, st);
+  if (rc) return rc;
+  k_tsdf_query_near<true><<<grid_for(n, m->sm_count), 256, 0, st>>>(m->g, submap, n, xyz, m->in.vs, (float)(m->cfg.voxel_scale * 1.8), voxel, out);
   TS_LAUNCH_CHECK(m);
   return TSLAM_OK;
 }

@@ -168,6 +168,7 @@ class TiledGlobalMap:
         self.last_exchange = {}
         self._halo_current = False  # ghosts carry the TSDF of the last fusion (exchange_halo ran since)
         self.esdf_submap = 0
+        self.last_query = {}  # raycast: dict(rounds, rays_forwarded) of the last batch
 
     # ---- helpers ----------------------------------------------------------------------------------------
     def _L(self):
@@ -420,6 +421,115 @@ class TiledGlobalMap:
         allv, _ = all_gather_ragged(self.dist, val, self.world)
         return allx, allv
 
+    # ---- planner queries: BaseMap's surface (mapping_common.py:165-204) on the tiled map ---------------------------
+    # Collectives: every rank calls them, with any points (an empty batch included); the answers come back in the
+    # caller's order and are bit-identical to the same call on one DenseTSDF holding every tile (DESIGN.md section 6).
+    # TopoGraphGen(tiled) therefore works unchanged when every rank runs the same TopoGraphGen in lockstep: its host
+    # code is deterministic numpy, so the ranks issue identical calls.
+    @property
+    def voxel_scale(self):
+        return self.m.voxel_scale
+
+    def ray_round_bound(self):
+        """Hand-over rounds a raycast batch can need: one into the tile of the first sample, then one per tile change,
+        at most tiles - 1 per axis because the tile of a ray's samples is monotone on each axis."""
+        return sum(self.tiles) - 2
+
+    def _ray_rows(self, pos, dir, max_dist):
+        """Rays f32[n,8] (pos, dir, max_dist, next sample 0) and their tags row * world + rank (int64[n])."""
+        import torch
+        p = self.m._h._dev_f32(pos).reshape(-1, 3)
+        d = self.m._h._dev_f32(dir).reshape(-1, 3)
+        rays = torch.zeros((p.shape[0], 8), dtype=torch.float32, device=p.device)  # (j = 0: int32 0 has the bits of 0.0f)
+        rays[:, :3] = p
+        rays[:, 3:6] = d
+        rays[:, 6] = float(max_dist)
+        return rays, torch.arange(p.shape[0], dtype=torch.int64, device=p.device) * self.world + self.rank
+
+    def _march(self, rays):
+        """One round of tslam_tsdf_raycast_tiled on the rays held here -> (dest int64[n], answer f32[n,5] = hit,
+        xyz, len; meaningful where dest < 0)."""
+        import torch
+        from . import _capi as capi
+        n, dev = rays.shape[0], rays.device
+        dest = torch.empty(n, dtype=torch.int32, device=dev)
+        hit = torch.empty(n, dtype=torch.uint8, device=dev)
+        xyz = torch.empty((n, 3), dtype=torch.float32, device=dev)
+        ln = torch.empty(n, dtype=torch.float32, device=dev)
+        capi.check(self._L().tslam_tsdf_raycast_tiled(self._h(), self._tiles_c, self.rank, self.world, self.m._active(), n, capi.tptr(rays),
+                                                      capi.tptr(dest), capi.tptr(hit), capi.tptr(xyz), capi.tptr(ln), capi.stream_ptr()))
+        return dest.long(), torch.cat([hit.float()[:, None], xyz, ln[:, None]], 1)
+
+    def _cell_dest(self, xyz):
+        """Points f32[n,3] on the device and the rank that answers each: the owner of the block holding its cell; this
+        rank for cells outside the volume (occupied and unobserved anywhere)."""
+        import torch
+        from . import _capi as capi
+        x = self.m._h._dev_f32(xyz).reshape(-1, 3)
+        owner = torch.empty(x.shape[0], dtype=torch.int32, device=x.device)
+        capi.check(self._L().tslam_tiling_owner_cells(self._h(), self._tiles_c, self.world, x.shape[0], capi.tptr(x), capi.tptr(owner),
+                                                      capi.stream_ptr()))
+        return x, torch.where(owner < 0, torch.full_like(owner, self.rank), owner).long()
+
+    def _points_answer(self, pts):
+        """tslam_tsdf_query_points on points routed here -> (flags u8[n],)."""
+        import torch
+        from . import _capi as capi
+        f = torch.empty(pts.shape[0], dtype=torch.uint8, device=pts.device)
+        capi.check(self._L().tslam_tsdf_query_points(self._h(), self.m._active(), pts.shape[0], capi.tptr(pts), capi.tptr(f), capi.stream_ptr()))
+        return (f,)
+
+    def _near_answer(self, pts, voxel):
+        """tslam_tsdf_query_near_occupy_tiled (reads ghosts) on points routed here -> (u8[n],)."""
+        import torch
+        from . import _capi as capi
+        f = torch.empty(pts.shape[0], dtype=torch.uint8, device=pts.device)
+        capi.check(self._L().tslam_tsdf_query_near_occupy_tiled(self._h(), self.m._active(), pts.shape[0], capi.tptr(pts), int(voxel), capi.tptr(f),
+                                                                capi.stream_ptr()))
+        return (f,)
+
+    def raycast(self, pos, dir, max_dist):
+        """BaseMap.raycast: (succ, last position, length) per ray, each ray marched by the ranks whose tiles it crosses.
+        self.last_query = dict(rounds, rays_forwarded) (summed over the ranks)."""
+        from .mapping.mapping_common import BaseMap
+        p, single = BaseMap._as_batch(pos)
+        d, _ = BaseMap._as_batch(dir)
+        rays, tags = self._ray_rows(p, d, max_dist)
+        (ans,), self.last_query = raycast_rounds(_DistRouter(self.dist, self.world, rays.device), [self._march], [rays], [tags], self.world,
+                                                 self.ray_round_bound())
+        return _ray_result(ans, single)
+
+    def _query_points(self, xyz):
+        x, dest = self._cell_dest(xyz)
+        (f,) = routed_answers(self.dist, x, dest, self.world, self._points_answer)
+        f = f.cpu().numpy()
+        return (f & 1).astype(bool), (f & 2).astype(bool)
+
+    def is_pos_occupy(self, xyz):
+        from .mapping.mapping_common import BaseMap
+        p, single = BaseMap._as_batch(xyz)
+        r = self._query_points(p)[0]
+        return bool(r[0]) if single else r
+
+    def is_pos_unobserved(self, xyz):
+        from .mapping.mapping_common import BaseMap
+        p, single = BaseMap._as_batch(xyz)
+        r = self._query_points(p)[1]
+        return bool(r[0]) if single else r
+
+    def is_near_pos_occupy(self, xyz, voxel):
+        """Answered by the owner of the centre cell, reading its ghosts: runs a TSDF halo exchange first unless one
+        has run since the last fusion.  voxel must lie in [0, 16] (the halo is one block deep)."""
+        from .mapping.mapping_common import BaseMap
+        voxel = _near_voxel(voxel)
+        p, single = BaseMap._as_batch(xyz)
+        if not self._halo_current:
+            self.exchange_halo()
+        x, dest = self._cell_dest(p)
+        (f,) = routed_answers(self.dist, x, dest, self.world, lambda pts: self._near_answer(pts, voxel))
+        r = f.cpu().numpy().astype(bool)
+        return bool(r[0]) if single else r
+
 
 def _esdf_stats(rounds, sweeps, blocks):
     return dict(rounds=int(rounds), sweeps=int(sweeps), blocks_sent=int(blocks), bytes_sent=int(blocks) * (8 + 4096 * 4))
@@ -457,6 +567,95 @@ def routed_answers(dist, rows, dest, world, answer):
     recv = exchange_counts(dist, send, rows.device)
     got = exchange_rows(dist, rows[order], send, recv)
     return tuple(route_restore(order, exchange_rows(dist, a, recv, send)) for a in answer(got))
+
+
+class _DistRouter:
+    """The ranks of a torch.distributed group, one per process: raycast_rounds sees a list of one local rank."""
+
+    def __init__(self, dist, world, device):
+        self.dist, self.world, self.device = dist, int(world), device
+
+    def total(self, counts):
+        import torch
+        t = torch.tensor([int(sum(counts))], dtype=torch.int64, device=self.device)
+        self.dist.all_reduce(t)
+        return int(t.item())
+
+    def route(self, bufs, dests):
+        """bufs[0] = tuple of tensors, row i addressed to rank dests[0][i] -> [tuple of the rows received]."""
+        order, send = route_order(dests[0], self.world)
+        recv = exchange_counts(self.dist, send, self.device)
+        return [tuple(exchange_rows(self.dist, b[order], send, recv) for b in bufs[0])]
+
+
+class _LocalRouter:
+    """`world` virtual ranks in one process (LocalGroup): the all-to-all is _route's slicing."""
+
+    def __init__(self, world):
+        self.world = int(world)
+
+    def total(self, counts):
+        return int(sum(counts))
+
+    def route(self, bufs, dests):
+        orders, sends = zip(*[route_order(d, self.world) for d in dests])
+        routed, _ = _route([tuple(b[o] for b in bb) for bb, o in zip(bufs, orders)], sends, self.world)
+        return routed
+
+
+def raycast_rounds(router, marches, rays, tags, world, bound):
+    """The hand-over loop of a routed raycast over the local ranks k of `router` (one per process with NCCL / gloo,
+    all of them for LocalGroup).  rays[k] f32[n,8] and tags[k] int64[n] (row * world + origin rank) are rank k's
+    rays; marches[k](rays) -> (dest int64[n], answer f32[n,5]) marches them as far as rank k's tile goes (dest -1:
+    finished, with its answer).  Rounds: march, count the handed-over rays over all ranks, stop at 0, route them to
+    their dest.  Raises past `bound` rounds, which the tile monotonicity of a ray rules out (DESIGN.md section 6).
+    Finally every answer goes home in one exchange.  Returns ([answer f32[n_k,5] in rank k's row order], dict(rounds,
+    rays_forwarded) summed over the ranks)."""
+    import torch
+    n0 = [int(r.shape[0]) for r in rays]
+    rays, tags = list(rays), list(tags)
+    fin_tags, fin_ans = [[] for _ in rays], [[] for _ in rays]
+    rounds = forwarded = 0
+    while True:
+        dests = []
+        for k, march in enumerate(marches):
+            dest, ans = march(rays[k])
+            done = dest < 0
+            fin_tags[k].append(tags[k][done])
+            fin_ans[k].append(ans[done])
+            rays[k], tags[k] = rays[k][~done], tags[k][~done]
+            dests.append(dest[~done])
+        n = router.total([int(d.shape[0]) for d in dests])
+        if n == 0:
+            break
+        rounds += 1
+        if rounds > bound:
+            raise RuntimeError(f"tiled raycast: rays still handed over after {bound} rounds (the bound of a tiling {world} wide)")
+        forwarded += n
+        got = router.route([(r, t) for r, t in zip(rays, tags)], dests)
+        rays, tags = [g[0] for g in got], [g[1] for g in got]
+    tags = [torch.cat(t) for t in fin_tags]
+    home = router.route([(torch.cat(a), t) for a, t in zip(fin_ans, tags)], [t % world for t in tags])
+    out = []
+    for n, (ans, tag) in zip(n0, home):
+        o = torch.empty((n, 5), dtype=ans.dtype, device=ans.device)
+        o[tag // world] = ans
+        out.append(o)
+    return out, dict(rounds=rounds, rays_forwarded=forwarded)
+
+
+def _ray_result(ans, single):
+    """answer f32[n,5] of raycast_rounds -> BaseMap.raycast's (succ, xyz, len)."""
+    a = ans.cpu().numpy()
+    succ, xyz, ln = a[:, 0] > 0, np.ascontiguousarray(a[:, 1:4]), np.ascontiguousarray(a[:, 4])
+    return (bool(succ[0]), xyz[0], float(ln[0])) if single else (succ, xyz, ln)
+
+
+def _near_voxel(voxel):
+    voxel = int(voxel)
+    if not 0 <= voxel <= 16:
+        raise ValueError(f"is_near_pos_occupy on a tiled map: voxel {voxel} outside [0, 16] (the halo is one 16^3 block deep)")
+    return voxel
 
 
 def run_local_fusion(tiled, submaps):
@@ -524,3 +723,87 @@ def run_local_esdf_query(tiled, xyz_per_rank):
     back, _ = _route(answers, rcounts, world)
     return [_query_result(route_restore(o, b[0]), route_restore(o, b[1]), isinstance(x, torch.Tensor))
             for o, b, x in zip(orders, back, xyz_per_rank)]
+
+
+def run_local_raycast(tiled, rays_per_rank):
+    """TiledGlobalMap.raycast on `world` virtual ranks: rays_per_rank[r] = (pos, dir, max_dist) of rank r ->
+    [(succ, xyz, len)] per rank in each caller's order; every tiled[r].last_query = dict(rounds, rays_forwarded)."""
+    from .mapping.mapping_common import BaseMap
+    world = len(tiled)
+    rows = [t._ray_rows(BaseMap._as_batch(p)[0], BaseMap._as_batch(d)[0], m) for t, (p, d, m) in zip(tiled, rays_per_rank)]
+    ans, st = raycast_rounds(_LocalRouter(world), [t._march for t in tiled], [r[0] for r in rows], [r[1] for r in rows], world,
+                             tiled[0].ray_round_bound())
+    for t in tiled:
+        t.last_query = dict(st)
+    return [_ray_result(a, False) for a in ans]
+
+
+def _run_local_routed(tiled, xyz_per_rank, answer):
+    """Points of every virtual rank routed to the owners of their cells, answered there by answer(t, pts) -> (u8[n],),
+    and sent back: [u8 numpy array] per rank in each caller's order."""
+    world = len(tiled)
+    plans = [t._cell_dest(x) for t, x in zip(tiled, xyz_per_rank)]
+    orders, sends = zip(*[route_order(dest, world) for _, dest in plans])
+    routed, rcounts = _route([(x[o],) for (x, _), o in zip(plans, orders)], sends, world)
+    back, _ = _route([answer(t, pts[0]) for t, pts in zip(tiled, routed)], rcounts, world)
+    return [route_restore(o, b[0]).cpu().numpy() for o, b in zip(orders, back)]
+
+
+def run_local_query_points(tiled, xyz_per_rank):
+    """is_pos_occupy / is_pos_unobserved on `world` virtual ranks -> [(occupied, unobserved)] per rank."""
+    f = _run_local_routed(tiled, xyz_per_rank, lambda t, pts: t._points_answer(pts))
+    return [((a & 1).astype(bool), (a & 2).astype(bool)) for a in f]
+
+
+def run_local_near_occupy(tiled, xyz_per_rank, voxel):
+    """is_near_pos_occupy on `world` virtual ranks (halo exchange first unless current) -> [bool array] per rank."""
+    voxel = _near_voxel(voxel)
+    world = len(tiled)
+    if not all(t._halo_current for t in tiled):
+        packed = [t.halo_pack() for t in tiled]
+        routed, _ = _route([p[1] for p in packed], [p[0] for p in packed], world)
+        for t, bufs in zip(tiled, routed):
+            t.halo_unpack(bufs)
+    return [a.astype(bool) for a in _run_local_routed(tiled, xyz_per_rank, lambda t, pts: t._near_answer(pts, voxel))]
+
+
+class LocalGroupMap:
+    """BaseMap's planner-query surface over the `world` virtual ranks of a LocalGroup (tiled[r] = rank r's
+    TiledGlobalMap), so that TopoGraphGen runs on a tiled map on one GPU.  Every query is asked by virtual rank
+    `asker`; the other ranks take part with empty batches, as ranks with nothing to ask do under NCCL."""
+
+    def __init__(self, tiled, asker=0):
+        self.tiled, self.asker = list(tiled), int(asker)
+        self.voxel_scale = self.tiled[0].voxel_scale
+        self.last_query = {}
+
+    def _per_rank(self, a):
+        empty = np.zeros((0, 3), np.float32)
+        return [a if r == self.asker else empty for r in range(len(self.tiled))]
+
+    def raycast(self, pos, dir, max_dist):
+        from .mapping.mapping_common import BaseMap
+        p, single = BaseMap._as_batch(pos)
+        d, _ = BaseMap._as_batch(dir)
+        out = run_local_raycast(self.tiled, [(a, b, max_dist) for a, b in zip(self._per_rank(p), self._per_rank(d))])[self.asker]
+        self.last_query = dict(self.tiled[0].last_query)
+        succ, xyz, ln = out
+        return (bool(succ[0]), xyz[0], float(ln[0])) if single else out
+
+    def _points(self, xyz, bit):
+        from .mapping.mapping_common import BaseMap
+        p, single = BaseMap._as_batch(xyz)
+        r = run_local_query_points(self.tiled, self._per_rank(p))[self.asker][bit]
+        return bool(r[0]) if single else r
+
+    def is_pos_occupy(self, xyz):
+        return self._points(xyz, 0)
+
+    def is_pos_unobserved(self, xyz):
+        return self._points(xyz, 1)
+
+    def is_near_pos_occupy(self, xyz, voxel):
+        from .mapping.mapping_common import BaseMap
+        p, single = BaseMap._as_batch(xyz)
+        r = run_local_near_occupy(self.tiled, self._per_rank(p), voxel)[self.asker]
+        return bool(r[0]) if single else r

@@ -7,7 +7,9 @@
 (rank r owns submaps r, r+W, ...), fused into a 2048^3 x 0.05 m global volume tiled over the ranks (2x2x2 for 8):
 foreign blocks travel in one NCCL all-to-all, the boundary layer is exchanged as ghost blocks, marching cubes runs
 locally and the triangle soup is all-gathered.  Then the tiled ESDF of the fused map (exchange rounds of boundary-block
-ESDF until no rank sends) and routed ESDF queries (2^20 uniform points per rank, answered by the owning ranks).
+ESDF until no rank sends) and routed ESDF queries (2^20 uniform points per rank, answered by the owning ranks), a
+routed raycast (2^16 rays per rank, 4 m, handed across tile seams; rounds and forwarded rays reported beside the
+time) and one TopoGraphGen run on the tiled map, all ranks in lockstep.
 Prints one JSON line on rank 0, with the GPU model and its power limit beside the figures."""
 import json, os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -85,6 +87,24 @@ def main():
         dq, gq, vq = tiled.esdf_query(pts)
     torch.cuda.synchronize(); dist.barrier()
     t_query = (time.perf_counter() - t0) / reps
+    # routed raycast: 2^16 rays per rank from uniform origins in the surveyed slab, 4 m long, handed across tile seams
+    rp = rng.uniform([-48.0, -48.0, -1.0], [48.0, 48.0, 4.0], size=(1 << 16, 3)).astype(np.float32)
+    rd = rng.normal(size=(1 << 16, 3)).astype(np.float32)
+    rd /= np.linalg.norm(rd, axis=1, keepdims=True)
+    tiled.raycast(rp, rd, 4.0)  # warm
+    torch.cuda.synchronize(); dist.barrier()
+    t0 = time.perf_counter()
+    tiled.raycast(rp, rd, 4.0)
+    torch.cuda.synchronize(); dist.barrier()
+    t_ray = time.perf_counter() - t0
+    rq = dict(tiled.last_query)
+    # one TopoGraphGen run on the tiled map, every rank in lockstep (its queries are collectives)
+    from taichi_slam.mapping import TopoGraphGen
+    topo = TopoGraphGen(tiled)
+    t0 = time.perf_counter()
+    n_nodes = topo.generate_topo_graph(np.array([0.0, 0.0, 1.0]), max_nodes=20)
+    torch.cuda.synchronize(); dist.barrier()
+    t_topo = time.perf_counter() - t0
     esx = torch.tensor([es["blocks_sent"], es["bytes_sent"], int(vq.sum().item())], dtype=torch.float64, device="cuda")
     dist.all_reduce(esx)
     own = torch.tensor([glo.count_active(), sum(sub._h.count_active(s) for s in mine), x["fusion_blocks_sent"], x.get("halo_blocks_sent", 0),
@@ -100,6 +120,8 @@ def main():
                           "esdf_ms": 1e3 * t_esdf, "esdf_rounds": es["rounds"], "esdf_halo_blocks": int(esx[0].item()),
                           "esdf_halo_MB": esx[1].item() / 1e6, "query_points_per_rank": 1 << 20, "query_ms": 1e3 * t_query,
                           "query_Gpoints_per_s": world * (1 << 20) / t_query / 1e9, "query_valid": int(esx[2].item()),
+                          "raycast_rays_per_rank": 1 << 16, "raycast_ms": 1e3 * t_ray, "raycast_rounds": rq["rounds"],
+                          "raycast_rays_forwarded": rq["rays_forwarded"], "topo_ms": 1e3 * t_topo, "topo_nodes": int(n_nodes),
                           "gpu": torch.cuda.get_device_name(local), "power_limit_W": _power_limit(local)}))
     dist.destroy_process_group()
 

@@ -320,6 +320,27 @@ int tslam_mc_generate(tslam_tsdf_t* m, int32_t step, float tsdf_surface_thres, i
  * colors f32[3*cap_tri,3] DEVICE or NULL. */
 int tslam_mc_generate2(tslam_tsdf_t* m, int32_t step, float tsdf_surface_thres, int64_t cap_tri, float* verts, float* normals,
                        float* colors, int64_t* n_tri_out, void* stream);
+/* Incremental mesh of one map (step 1 only).  The cache keeps the mesh of its last update on the device and, on the next
+ * update, remeshes only the blocks whose output a commit or ghost import since then could have changed; the rest of the
+ * mesh is copied.  tslam_mesh_update has the output contract of tslam_mc_generate2(m, 1, ...): the same *n_tri_out
+ * (demand), the same first min(demand, cap_tri) triangles bit for bit, the same TSLAM_E_CAPACITY and deferred
+ * TSLAM_E_POOL_FULL.  It rebuilds fully on the first call, after a reset, load (scatter), fusion or fusion exchange of
+ * the map, and when thres or the colour mode (colors NULL or not) changes.  stats4 (HOST, may be NULL) = pool blocks,
+ * stamped blocks, touched blocks, remeshed blocks (a full rebuild: 0 stamped and touched, every block remeshed).
+ * Synchronises.  A cache belongs to its map and must be destroyed before it. */
+typedef struct tslam_mesh tslam_mesh_t;
+int tslam_mesh_create(tslam_tsdf_t* m, tslam_mesh_t** out);
+int tslam_mesh_destroy(tslam_mesh_t* c);
+int tslam_mesh_update(tslam_mesh_t* c, float tsdf_surface_thres, int64_t cap_tri, float* verts, float* normals, float* colors,
+                      int64_t* n_tri_out, int32_t* stats4, void* stream);
+/* The blocks remeshed by the last update, in pool order: blk4 int32[cap,4] = submap, bx, by, bz; first_tri int64[cap] and
+ * n_tri int32[cap] = their range in the update's output (demand numbering: a range may reach past a saturated cap_tri)
+ * (all DEVICE).  n_tri 0: the block's mesh is now empty.  The list is a superset of the blocks whose triangles changed.
+ * *full_out (HOST, may be NULL) = 1 after a full rebuild: every block is listed and the consumer drops what it kept.
+ * *n_out (HOST) = blocks; rows beyond cap are not written (TSLAM_E_CAPACITY).  TSLAM_E_INVALID before the first
+ * completed update.  Synchronises. */
+int tslam_mesh_updated_blocks(tslam_mesh_t* c, int64_t cap, int32_t* blk4, int64_t* first_tri, int32_t* n_tri, int64_t* n_out,
+                              int32_t* full_out, void* stream);
 
 /* ----------------------------------------------------------------------------
  * ESDF  (DenseSDF.propogate_esdf semantics, dense_esdf.py:228-333; see DESIGN.md)

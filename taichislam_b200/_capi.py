@@ -118,6 +118,10 @@ SIGNATURES = {
     "tslam_esdf_tiled_relax": (C.c_int, [_vp, C.POINTER(_i32), _vp]),
     "tslam_esdf_tiled_end": (C.c_int, [_vp]),
     "tslam_mc_generate": (C.c_int, [_vp, _i32, _f32, _i64, _vp, _vp, C.POINTER(_i64), _vp]),
+    "tslam_mesh_create": (C.c_int, [_vp, C.POINTER(_vp)]),
+    "tslam_mesh_destroy": (C.c_int, [_vp]),
+    "tslam_mesh_update": (C.c_int, [_vp, _f32, _i64, _vp, _vp, _vp, C.POINTER(_i64), _vp, _vp]),
+    "tslam_mesh_updated_blocks": (C.c_int, [_vp, _i64, _vp, _vp, _vp, C.POINTER(_i64), C.POINTER(_i32), _vp]),
     "tslam_esdf_update": (C.c_int, [_vp, _i32, C.POINTER(_i32), _vp]),
     "tslam_esdf_update2": (C.c_int, [_vp, _i32, _i32, _vp, _vp]),
     "tslam_esdf_gather": (C.c_int, [_vp, _i32, _i64, _vp, _vp, C.POINTER(_i64), _vp]),

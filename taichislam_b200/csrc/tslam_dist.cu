@@ -224,13 +224,14 @@ __global__ void __launch_bounds__(256) k_halo_pack(TsGrid g, TsTiling t, const i
 }
 
 __global__ void __launch_bounds__(256) k_ghost_unpack(TsGrid g, long long n, const long long* keys, const float2* tw_in,
-                                                       const uint8_t* obs_in, const float4* col_in) {
+                                                       const uint8_t* obs_in, const float4* col_in, unsigned long long* stamp,
+                                                       unsigned long long seq) {
   __shared__ int s_blk;
   for (long long q = blockIdx.x; q < n; q += gridDim.x) {
     __syncthreads();
     if (threadIdx.x == 0) {
       s_blk = ts_get_or_alloc(g, (unsigned long long)keys[q]);
-      if (s_blk >= 0) g.ghost[s_blk] = 1;
+      if (s_blk >= 0) { g.ghost[s_blk] = 1; stamp[s_blk] = seq; }
     }
     __syncthreads();
     const int blk = s_blk;
@@ -492,6 +493,7 @@ extern "C" int tslam_tsdf_foreign_pack2(tslam_tsdf_t* m, const int32_t* tiles3, 
   int* d_cur = m->scratch_i + 40;
   TS_CUDA(cudaMemcpyAsync(d_off, h_off, world * sizeof(int), cudaMemcpyHostToDevice, st));
   TS_CUDA(cudaMemsetAsync(d_cur, 0, 24 * sizeof(int), st));
+  m->mesh_epoch++;  // the packed blocks' obs / col planes are cleared without a stamp
   k_foreign_pack<<<m->sm_count * 4, 256, 0, st>>>(m->g, t, d_off, d_cur, cap, (long long*)keys, (float2*)acc, obs, occ, (float4*)col);
   TS_LAUNCH_CHECK(m);
   TS_CUDA(cudaStreamSynchronize(st));  // h_off is on the stack
@@ -508,6 +510,7 @@ extern "C" int tslam_tsdf_unpack_add2(tslam_tsdf_t* m, int64_t n, const int64_t*
   if (col && !m->g.col) { ts_set_error("colour plane given to an untextured map"); return TSLAM_E_INVALID; }
   if (n == 0) return TSLAM_OK;
   cudaStream_t st = (cudaStream_t)stream;
+  m->mesh_epoch++;  // obs / col change before the fused commit stamps the blocks
   k_unpack_add<<<(int)(n < m->sm_count * 4 ? n : m->sm_count * 4), 256, 0, st>>>(m->g, n, (const long long*)keys, (const float2*)acc, obs, occ, (const float4*)col);
   TS_LAUNCH_CHECK(m);
   return TSLAM_OK;
@@ -565,7 +568,9 @@ extern "C" int tslam_tsdf_ghost_unpack2(tslam_tsdf_t* m, int64_t n, const int64_
   if (n == 0) return TSLAM_OK;
   cudaStream_t st = (cudaStream_t)stream;
   m->esdf_full_needed = 1;
-  k_ghost_unpack<<<(int)(n < m->sm_count * 4 ? n : m->sm_count * 4), 256, 0, st>>>(m->g, n, (const long long*)keys, (const float2*)tw, obs, (const float4*)col);
+  const unsigned long long seq = ++m->commit_seq;  // the imported ghosts are stamped like committed blocks (incremental mesh)
+  k_ghost_unpack<<<(int)(n < m->sm_count * 4 ? n : m->sm_count * 4), 256, 0, st>>>(m->g, n, (const long long*)keys, (const float2*)tw, obs, (const float4*)col,
+                                                                                  m->blk_stamp, seq);
   TS_LAUNCH_CHECK(m);
   return TSLAM_OK;
 }

@@ -426,6 +426,13 @@ struct tslam_tsdf {
   int esdf_full_needed, esdf_submap;  // the next update recomputes everything (first use, reset, bulk load) / submap of the kept state
   int esdf_tiled;      // tiled ESDF (tslam_esdf_tiled_*): 0 = none (plain update), 1 = begun, exchange in progress, 2 = ended
   void* mc_scratch;    // marching cubes: per-block triangle counts / offsets (allocated on first use)
+  // Change tracking for the incremental mesh (tslam_mesh_*, tslam_mc.cu).  Every commit (k_commit / k_commit_tma) and
+  // every ghost import (k_ghost_unpack) takes the next commit_seq and stores it in blk_stamp[] of each block it writes;
+  // every other writer of the tw / obs / col planes, and whatever recycles pool slots, bumps mesh_epoch instead
+  // (DESIGN.md section 4 lists them).
+  unsigned long long* blk_stamp;  // [max_blocks] commit_seq of the last commit / ghost import that wrote the block
+  unsigned long long commit_seq;
+  unsigned long long mesh_epoch;
   long long launches;
   int n_integrate_calls;
   int profiling;

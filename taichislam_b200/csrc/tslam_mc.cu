@@ -108,33 +108,57 @@ __device__ __forceinline__ int mc_cube_index(const McTile& tile, int lx, int ly,
   return any_unobs ? -1 : cube;
 }
 
-// pass 1: triangles per block
-__global__ void __launch_bounds__(256) k_mc_count(TsGrid g, float thres, unsigned int* blk_tris) {
+// Whether block b holds an observed voxel with TSDF < 0 (NaN and -0 are not < 0, as in mc_cube_index): a cell can only
+// emit a triangle when one of its corners is such a voxel.  Read straight from the planes; CTA-uniform result.
+__device__ __forceinline__ bool mc_block_neg(const TsGrid& g, int b) {
+  const size_t base = (size_t)b * TS_B3;
+  int neg = 0;
+  for (int v = threadIdx.x; v < TS_B3; v += blockDim.x) neg |= (g.obs[base + v] != 0 && g.tw[base + v].x < 0.0f);
+  return __syncthreads_or(neg) != 0;
+}
+
+// pass 1: triangles per block.  List = false: every block of the pool (tslam_mc_generate2).  List = true: the blocks
+// list[0 .. *n_list) (the incremental mesh), which also stores mc_block_neg of each listed block in neg[].
+template <bool List>
+__global__ void __launch_bounds__(256) k_mc_count(TsGrid g, float thres, unsigned int* blk_tris, const int* list, const int* n_list,
+                                                   uint8_t* neg) {
   __shared__ McTile tile;
   __shared__ unsigned int warp_sum[8];
-  const int nb = min(*g.n_blocks, g.max_blocks);
-  for (int b = blockIdx.x; b < nb; b += gridDim.x) {
+  const int nb = List ? *n_list : min(*g.n_blocks, g.max_blocks);
+  for (int q = blockIdx.x; q < nb; q += gridDim.x) {
+    const int b = List ? list[q] : q;
     int s, bx, by, bz;
     ts_unpack_key(g.block_key[b], s, bx, by, bz);
     if (g.ghost[b]) {  // halo copy: its cells belong to the owning rank
+      if (List) {      // (its voxels are corners of the owned cells next to it)
+        const bool ng = mc_block_neg(g, b);
+        if (threadIdx.x == 0) neg[b] = ng;
+      }
       if (threadIdx.x == 0) blk_tris[b] = 0;
       continue;
     }
     __syncthreads();
     mc_stage(g, tile, s, bx, by, bz);
     unsigned int n = 0;
+    int ng = 0;
     for (int v = threadIdx.x; v < TS_B3; v += blockDim.x) {
       float val[8];
       const int cube = mc_cube_index(tile, v >> 8, (v >> 4) & 15, v & 15, thres, val);
       if (cube >= 0) n += c_mc_ntri[cube];
+      if (List) {
+        const int c = mc_tidx(v >> 8, (v >> 4) & 15, v & 15);
+        ng |= (tile.o[c] != 0 && tile.t[c] < 0.0f);
+      }
     }
     for (int o = 16; o > 0; o >>= 1) n += __shfl_xor_sync(0xffffffffu, n, o);
     if ((threadIdx.x & 31) == 0) warp_sum[threadIdx.x >> 5] = n;
-    __syncthreads();
+    if (List) ng = __syncthreads_or(ng);
+    else __syncthreads();
     if (threadIdx.x == 0) {
       unsigned int t = 0;
       for (int w = 0; w < 8; w++) t += warp_sum[w];
       blk_tris[b] = t;
+      if (List) neg[b] = ng != 0;
     }
   }
 }
@@ -263,17 +287,20 @@ __device__ __forceinline__ void mc_emit_list(const TsGrid& g, const McTile& tile
   }
 }
 
+// List as k_mc_count: every block of the pool, or the blocks list[0 .. *n_list).
+template <bool List>
 __global__ void __launch_bounds__(256) k_mc_emit(TsGrid g, float thres, float vs, const unsigned int* blk_tris,
                                                   const unsigned long long* blk_off, long long cap_tri, float* verts, float* normals,
-                                                  float* colors) {
+                                                  float* colors, const int* list, const int* n_list) {
   __shared__ McTile tile;
   __shared__ unsigned int warp_sum[8];
   __shared__ unsigned int run_base;
   __shared__ unsigned int cell_vc[MC_LIST], cell_off[MC_LIST];  // voxel << 8 | cube index; first output triangle (relative to the block's)
   __shared__ int n_cell;
-  const int nb = min(*g.n_blocks, g.max_blocks);
+  const int nb = List ? *n_list : min(*g.n_blocks, g.max_blocks);
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  for (int b = blockIdx.x; b < nb; b += gridDim.x) {
+  for (int q = blockIdx.x; q < nb; q += gridDim.x) {
+    const int b = List ? list[q] : q;
     if (blk_tris[b] == 0) continue;
     int s, bx, by, bz;
     ts_unpack_key(g.block_key[b], s, bx, by, bz);
@@ -426,11 +453,12 @@ extern "C" int tslam_mc_generate2(tslam_tsdf_t* m, int32_t step, float thres, in
     if (!m->mc_scratch) TS_CUDA(cudaMalloc(&m->mc_scratch, (size_t)m->g.max_blocks * 12));  // persistent: per-block counts + offsets
     unsigned long long* blk_off = (unsigned long long*)m->mc_scratch;
     unsigned int* blk_tris = (unsigned int*)(blk_off + m->g.max_blocks);
-    k_mc_count<<<m->sm_count * 4, 256, 0, st>>>(m->g, thres, blk_tris);
+    k_mc_count<false><<<m->sm_count * 4, 256, 0, st>>>(m->g, thres, blk_tris, nullptr, nullptr, nullptr);
     TS_LAUNCH_CHECK(m);
     k_mc_scan<<<1, 1024, 0, st>>>(m->g.n_blocks, m->g.max_blocks, blk_tris, blk_off, d_total);
     TS_LAUNCH_CHECK(m);
-    k_mc_emit<<<m->sm_count * 4, 256, 0, st>>>(m->g, thres, m->in.vs, blk_tris, blk_off, cap_tri, verts, normals, colors);
+    k_mc_emit<false><<<m->sm_count * 4, 256, 0, st>>>(m->g, thres, m->in.vs, blk_tris, blk_off, cap_tri, verts, normals, colors, nullptr,
+                                                      nullptr);
     TS_LAUNCH_CHECK(m);
     TS_CUDA(cudaMemcpyAsync(&total, d_total, 8, cudaMemcpyDeviceToHost, st));
     TS_CUDA(cudaStreamSynchronize(st));
@@ -446,6 +474,370 @@ extern "C" int tslam_mc_generate2(tslam_tsdf_t* m, int32_t step, float thres, in
   if (rc) return rc;
   if ((int64_t)total > cap_tri) {
     ts_set_error("marching cubes: %lld triangles > capacity %lld (output saturated)", (long long)total, (long long)cap_tri);
+    return TSLAM_E_CAPACITY;
+  }
+  return TSLAM_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Incremental mesh (tslam_mesh_*): the step-1 mesh of one map kept on the device, remeshing only the blocks a commit
+// could have changed.  Output bit-identical to tslam_mc_generate2(step = 1); the dependency argument is in DESIGN.md
+// section 4.  Blocks keep the pool order of the two-pass mesh: block b's triangles sit at off[b] .. off[b] + cnt[b].
+// ---------------------------------------------------------------------------------------------------------------------
+struct McCtl {
+  unsigned long long total;  // triangles of the new mesh (k_mc_scan)
+  int n_stamp, n_touch, n_dirty, nb;
+};
+
+struct tslam_mesh {
+  tslam_tsdf* m;
+  unsigned int* cnt;            // [max_blocks] triangles per block of the kept mesh
+  unsigned long long* off[2];   // [max_blocks] first triangle per block, one array per mesh buffer
+  uint8_t* neg;                 // [max_blocks] mc_block_neg at the last update
+  uint8_t* neg_now;             // [max_blocks] mc_block_neg now (stamped blocks only, written by k_mesh_touch)
+  int* touch_flag;              // [max_blocks] block is on touch_list (cleared again by k_mesh_dirty)
+  int* stamp_list;              // [max_blocks]
+  int* touch_list;              // [max_blocks]
+  int* dirty_list;              // [max_blocks] blocks remeshed by this update
+  unsigned int* mark;           // [max_blocks] number of the last update that remeshed the block
+  McCtl* ctl;
+  float* buf[2];                // mesh buffers: verts | normals [| colours], planes of cap[i] * 9 floats
+  long long cap[2];
+  int cur;                      // buffer (and offsets) of the kept mesh
+  int valid;                    // an update completed and the kept state describes the map
+  int colored, full, nb;
+  long long total;              // triangles of the kept mesh
+  float thres;
+  unsigned long long seq, epoch;
+  unsigned int upd;             // updates so far
+};
+
+static inline float* mc_plane(tslam_mesh* c, int i, int p) { return c->buf[i] + (size_t)p * (size_t)c->cap[i] * 9; }
+
+// step 0 (incremental): list the blocks stamped since the last update.  Blocks allocated since then (b >= nb_last)
+// had no triangles and no negative voxel.
+__global__ void __launch_bounds__(256) k_mesh_stamped(TsGrid g, const unsigned long long* stamp, unsigned long long seq, int nb_last,
+                                                       unsigned int* cnt, uint8_t* neg, int* stamp_list, McCtl* ctl) {
+  const int nb = min(*g.n_blocks, g.max_blocks);
+  if (blockIdx.x == 0 && threadIdx.x == 0) ctl->nb = nb;
+  const int stride = gridDim.x * blockDim.x;
+  const int iters = (nb + stride - 1) / stride;
+  for (int it = 0; it < iters; ++it) {  // uniform trip count: the append below is warp-collective
+    const int b = it * stride + blockIdx.x * blockDim.x + threadIdx.x;
+    bool want = false;
+    if (b < nb) {
+      if (b >= nb_last) { cnt[b] = 0; neg[b] = 0; }
+      want = stamp[b] > seq;
+    }
+    const int row = warp_append_i32(want, &ctl->n_stamp);
+    if (want) stamp_list[row] = b;
+  }
+}
+
+// full rebuild: every block is listed
+__global__ void __launch_bounds__(256) k_mesh_all(TsGrid g, int* dirty_list, McCtl* ctl) {
+  const int nb = min(*g.n_blocks, g.max_blocks);
+  if (blockIdx.x == 0 && threadIdx.x == 0) { ctl->nb = nb; ctl->n_dirty = nb; }
+  for (int b = blockIdx.x * blockDim.x + threadIdx.x; b < nb; b += gridDim.x * blockDim.x) dirty_list[b] = b;
+}
+
+// mark, kernel A: one CTA per stamped block S.  neg_now[S], then every existing block of S's 27-neighbourhood is
+// touched (its mesh reads S), each listed once.
+__global__ void __launch_bounds__(256) k_mesh_touch(TsGrid g, const int* stamp_list, uint8_t* neg_now, int* touch_flag, int* touch_list,
+                                                     McCtl* ctl) {
+  const int n = ctl->n_stamp;
+  for (int q = blockIdx.x; q < n; q += gridDim.x) {
+    const int b = stamp_list[q];
+    const bool ng = mc_block_neg(g, b);
+    if (threadIdx.x < 32) {
+      if (threadIdx.x == 0) neg_now[b] = ng;
+      int s, bx, by, bz;
+      ts_unpack_key(g.block_key[b], s, bx, by, bz);
+      int nbk = -1;
+      if (threadIdx.x < 27)  // the keys mc_stage looks up, wrapped the same way
+        nbk = ts_find(g, ts_pack_key(s, bx + (int)threadIdx.x / 9 - 1, by + ((int)threadIdx.x / 3) % 3 - 1, bz + (int)threadIdx.x % 3 - 1));
+      const bool want = nbk >= 0 && atomicExch(&touch_flag[nbk], 1) == 0;
+      const int row = warp_append_i32(want, &ctl->n_touch);
+      if (want) touch_list[row] = nbk;
+    }
+  }
+}
+
+// mark, kernel B: one lane per touched block B.  Dirty iff some block M of B + {0,1}^3 had or has a negative observed
+// voxel (neg_then(M) || neg_now(M); neg_now = neg_then unless M is stamped).
+__global__ void __launch_bounds__(256) k_mesh_dirty(TsGrid g, const unsigned long long* stamp, unsigned long long seq, const uint8_t* neg,
+                                                     const uint8_t* neg_now, int* touch_flag, const int* touch_list, int* dirty_list,
+                                                     unsigned int* mark, unsigned int upd, McCtl* ctl) {
+  const int n = ctl->n_touch;
+  const int stride = gridDim.x * blockDim.x;
+  const int iters = (n + stride - 1) / stride;
+  for (int it = 0; it < iters; ++it) {
+    const int i = it * stride + blockIdx.x * blockDim.x + threadIdx.x;
+    bool want = false;
+    int b = -1;
+    if (i < n) {
+      b = touch_list[i];
+      touch_flag[b] = 0;
+      int s, bx, by, bz;
+      ts_unpack_key(g.block_key[b], s, bx, by, bz);
+      for (int d = 0; d < 8 && !want; d++) {
+        const int mb = ts_find(g, ts_pack_key(s, bx + (d >> 2), by + ((d >> 1) & 1), bz + (d & 1)));
+        if (mb >= 0) want = neg[mb] || (stamp[mb] > seq && neg_now[mb]);
+      }
+      if (want) mark[b] = upd;
+    }
+    const int row = warp_append_i32(want, &ctl->n_dirty);
+    if (want) dirty_list[row] = b;
+  }
+}
+
+// n floats src -> dst by one CTA: 16-byte loads from the source's first aligned word on, 16-byte stores when the
+// destination shares that alignment, else four 4-byte stores
+__device__ __forceinline__ void mc_copy_range(const float* __restrict__ src, float* __restrict__ dst, size_t n) {
+  const size_t head = min((size_t)((4 - (((uintptr_t)src >> 2) & 3)) & 3), n);
+  if (threadIdx.x < head) dst[threadIdx.x] = src[threadIdx.x];
+  const size_t nv = (n - head) >> 2;
+  const float4* s4 = reinterpret_cast<const float4*>(src + head);
+  float* d = dst + head;
+  if ((((uintptr_t)d) & 15) == 0) {
+    float4* d4 = reinterpret_cast<float4*>(d);
+    for (size_t i = threadIdx.x; i < nv; i += blockDim.x) d4[i] = s4[i];
+  } else {
+    for (size_t i = threadIdx.x; i < nv; i += blockDim.x) {
+      const float4 v = s4[i];
+      d[4 * i] = v.x; d[4 * i + 1] = v.y; d[4 * i + 2] = v.z; d[4 * i + 3] = v.w;
+    }
+  }
+  for (size_t i = head + 4 * nv + threadIdx.x; i < n; i += blockDim.x) dst[i] = src[i];
+}
+
+// clean blocks with triangles: their range moves from the kept mesh to the new offsets, one CTA per block
+struct McPlanes { const float* src[3]; float* dst[3]; int n; };
+__global__ void __launch_bounds__(256) k_mesh_copy(int nb_last, const unsigned int* cnt, const unsigned int* mark, unsigned int upd,
+                                                    const unsigned long long* off_old, const unsigned long long* off_new, McPlanes p) {
+  for (int b = blockIdx.x; b < nb_last; b += gridDim.x) {
+    const unsigned int n = cnt[b];
+    if (n == 0 || mark[b] == upd) continue;
+    const size_t so = (size_t)off_old[b] * 9, dn = (size_t)off_new[b] * 9;
+#pragma unroll
+    for (int k = 0; k < 3; k++)  // (constant indices: the planes stay in the parameter space, no local copy)
+      if (k < p.n) mc_copy_range(p.src[k] + so, p.dst[k] + dn, (size_t)n * 9);
+  }
+}
+
+// the remeshed blocks in pool order (single CTA, ordered compaction): keys, first triangle, triangle count
+__global__ void __launch_bounds__(1024) k_mesh_updated(TsGrid g, int nb, int full, const unsigned int* mark, unsigned int upd, const unsigned int* cnt,
+                                                        const unsigned long long* off, long long cap, int* blk4, long long* first, int* ntri,
+                                                        long long* n_out) {
+  __shared__ int wsum[32];
+  __shared__ long long carry;
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  if (threadIdx.x == 0) carry = 0;
+  __syncthreads();
+  for (int base = 0; base < nb; base += 1024) {
+    const int b = base + threadIdx.x;
+    const bool want = b < nb && (full || mark[b] == upd);
+    const unsigned m = __ballot_sync(0xffffffffu, want);
+    if (lane == 0) wsum[wid] = __popc(m);
+    __syncthreads();
+    int woff = 0, tot = 0;
+    for (int w = 0; w < 32; w++) {
+      const int x = wsum[w];
+      if (w < wid) woff += x;
+      tot += x;
+    }
+    const long long row = carry + woff + __popc(m & ((1u << lane) - 1));
+    if (want && row < cap) {
+      int s, bx, by, bz;
+      ts_unpack_key(g.block_key[b], s, bx, by, bz);
+      blk4[4 * row] = s; blk4[4 * row + 1] = bx; blk4[4 * row + 2] = by; blk4[4 * row + 3] = bz;
+      first[row] = (long long)off[b];
+      ntri[row] = (int)cnt[b];
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) carry += tot;
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) *n_out = carry;
+}
+
+static void mc_mesh_free_bufs(tslam_mesh* c) {
+  for (int i = 0; i < 2; i++) {
+    if (c->buf[i]) cudaFree(c->buf[i]);
+    c->buf[i] = nullptr;
+    c->cap[i] = 0;
+  }
+}
+
+extern "C" int tslam_mesh_create(tslam_tsdf_t* m, tslam_mesh_t** out) {
+  if (!m || !out) return TSLAM_E_INVALID;
+  *out = nullptr;
+  tslam_mesh* c = new tslam_mesh();
+  memset(c, 0, sizeof(*c));
+  c->m = m;
+  const size_t mb = (size_t)m->g.max_blocks;
+  int rc = TSLAM_OK;
+  auto alloc = [&](void** p, size_t bytes) {
+    if (rc) return;
+    if (cudaMalloc(p, bytes) != cudaSuccess || cudaMemset(*p, 0, bytes) != cudaSuccess) rc = ts_cuda_fail(cudaGetLastError(), "tslam_mesh_create");
+  };
+  alloc((void**)&c->cnt, mb * 4);
+  alloc((void**)&c->off[0], mb * 8);
+  alloc((void**)&c->off[1], mb * 8);
+  alloc((void**)&c->neg, mb);
+  alloc((void**)&c->neg_now, mb);
+  alloc((void**)&c->touch_flag, mb * 4);
+  alloc((void**)&c->stamp_list, mb * 4);
+  alloc((void**)&c->touch_list, mb * 4);
+  alloc((void**)&c->dirty_list, mb * 4);
+  alloc((void**)&c->mark, mb * 4);
+  alloc((void**)&c->ctl, sizeof(McCtl));
+  if (rc) { tslam_mesh_destroy(c); return rc; }
+  *out = c;
+  return TSLAM_OK;
+}
+
+extern "C" int tslam_mesh_destroy(tslam_mesh_t* c) {
+  if (!c) return TSLAM_OK;
+  cudaDeviceSynchronize();
+  void* p[] = {c->cnt, c->off[0], c->off[1], c->neg, c->neg_now, c->touch_flag, c->stamp_list, c->touch_list, c->dirty_list, c->mark, c->ctl};
+  for (void* q : p)
+    if (q) cudaFree(q);
+  mc_mesh_free_bufs(c);
+  delete c;
+  return TSLAM_OK;
+}
+
+extern "C" int tslam_mesh_update(tslam_mesh_t* c, float thres, int64_t cap_tri, float* verts, float* normals, float* colors,
+                                 int64_t* n_tri_out, int32_t* stats4, void* stream) {
+  if (!c || !verts || !normals || !n_tri_out || cap_tri < 0) return TSLAM_E_INVALID;
+  tslam_tsdf* m = c->m;
+  cudaStream_t st = (cudaStream_t)stream;
+  int rc = mc_upload_tables();
+  if (rc) return rc;
+  rc = ts_flush_pending(m, st);
+  if (rc) return rc;
+  const int colored = colors != nullptr;
+  const bool full = !c->valid || c->epoch != m->mesh_epoch || memcmp(&c->thres, &thres, sizeof(float)) != 0 || c->colored != colored;
+  c->valid = 0;  // until this update completes
+  if (c->colored != colored) {
+    TS_CUDA(cudaStreamSynchronize(st));
+    mc_mesh_free_bufs(c);  // a different number of planes
+    c->colored = colored;
+  }
+  const unsigned long long seq = m->commit_seq;  // stamps above this are seen by the next update
+  const unsigned int upd = ++c->upd;
+  McCtl h;
+  memset(&h, 0, sizeof(h));
+  int out = c->cur;
+  int nb_now = 0;
+  // Nothing committed or imported since the last update: no block is stamped, none is remeshed, and the kept mesh is the
+  // answer.  Blocks allocated since hold no triangles; c->nb stays, so the next pass initialises them.
+  const bool unchanged = !full && seq == c->seq;
+  if (unchanged) {
+    h.total = (unsigned long long)c->total;
+    TS_CUDA(cudaMemcpyAsync(&nb_now, m->g.n_blocks, 4, cudaMemcpyDeviceToHost, st));  // (statistics only; read after the sync below)
+  } else {
+    const int grid = m->sm_count * 4;
+    TS_CUDA(cudaMemsetAsync(c->ctl, 0, sizeof(McCtl), st));
+    if (full) {
+      TS_CUDA(cudaMemsetAsync(c->touch_flag, 0, (size_t)m->g.max_blocks * 4, st));
+      k_mesh_all<<<grid, 256, 0, st>>>(m->g, c->dirty_list, c->ctl);
+      TS_LAUNCH_CHECK(m);
+    } else {
+      k_mesh_stamped<<<grid, 256, 0, st>>>(m->g, m->blk_stamp, c->seq, c->nb, c->cnt, c->neg, c->stamp_list, c->ctl);
+      TS_LAUNCH_CHECK(m);
+      k_mesh_touch<<<grid, 256, 0, st>>>(m->g, c->stamp_list, c->neg_now, c->touch_flag, c->touch_list, c->ctl);
+      TS_LAUNCH_CHECK(m);
+      k_mesh_dirty<<<grid, 256, 0, st>>>(m->g, m->blk_stamp, c->seq, c->neg, c->neg_now, c->touch_flag, c->touch_list, c->dirty_list,
+                                         c->mark, upd, c->ctl);
+      TS_LAUNCH_CHECK(m);
+    }
+    const int nxt = c->cur ^ 1;
+    k_mc_count<true><<<grid, 256, 0, st>>>(m->g, thres, c->cnt, c->dirty_list, &c->ctl->n_dirty, c->neg);
+    TS_LAUNCH_CHECK(m);
+    k_mc_scan<<<1, 1024, 0, st>>>(m->g.n_blocks, m->g.max_blocks, c->cnt, c->off[nxt], &c->ctl->total);
+    TS_LAUNCH_CHECK(m);
+    TS_CUDA(cudaMemcpyAsync(&h, c->ctl, sizeof(McCtl), cudaMemcpyDeviceToHost, st));
+    TS_CUDA(cudaStreamSynchronize(st));
+    nb_now = h.nb;
+    if (h.n_dirty > 0) {
+      // (no block remeshed: nothing moved, the kept mesh and its offsets stay as they are - blocks allocated since hold
+      // no triangles)
+      const long long total = (long long)h.total;
+      const int planes = colored ? 3 : 2;
+      if (total > c->cap[nxt]) {
+        if (c->buf[nxt]) TS_CUDA(cudaFree(c->buf[nxt]));
+        c->buf[nxt] = nullptr;
+        c->cap[nxt] = 0;
+        const long long want = total + total / 4 + 1024;
+        TS_CUDA(cudaMalloc(&c->buf[nxt], (size_t)want * 9 * sizeof(float) * planes));
+        c->cap[nxt] = want;
+      }
+      k_mc_emit<true><<<grid, 256, 0, st>>>(m->g, thres, m->in.vs, c->cnt, c->off[nxt], c->cap[nxt], mc_plane(c, nxt, 0), mc_plane(c, nxt, 1),
+                                            colored ? mc_plane(c, nxt, 2) : nullptr, c->dirty_list, &c->ctl->n_dirty);
+      TS_LAUNCH_CHECK(m);
+      if (!full && c->nb > 0) {
+        McPlanes p;
+        p.n = planes;
+        for (int k = 0; k < 3; k++) {
+          p.src[k] = k < planes ? mc_plane(c, c->cur, k) : nullptr;
+          p.dst[k] = k < planes ? mc_plane(c, nxt, k) : nullptr;
+        }
+        k_mesh_copy<<<grid, 256, 0, st>>>(c->nb, c->cnt, c->mark, upd, c->off[c->cur], c->off[nxt], p);
+        TS_LAUNCH_CHECK(m);
+      }
+      out = nxt;
+    }
+  }
+  // one tail for both: the output contract of tslam_mc_generate2(step = 1)
+  const long long total = (long long)h.total;
+  const long long n_out = total < cap_tri ? total : (long long)cap_tri;
+  if (n_out > 0) {
+    const size_t bytes = (size_t)n_out * 9 * sizeof(float);
+    TS_CUDA(cudaMemcpyAsync(verts, mc_plane(c, out, 0), bytes, cudaMemcpyDeviceToDevice, st));
+    TS_CUDA(cudaMemcpyAsync(normals, mc_plane(c, out, 1), bytes, cudaMemcpyDeviceToDevice, st));
+    if (colored) TS_CUDA(cudaMemcpyAsync(colors, mc_plane(c, out, 2), bytes, cudaMemcpyDeviceToDevice, st));
+  }
+  TS_CUDA(cudaStreamSynchronize(st));
+  c->cur = out;
+  c->seq = seq;
+  c->epoch = m->mesh_epoch;
+  c->thres = thres;
+  if (!unchanged) c->nb = h.nb;
+  c->total = total;
+  c->full = full;
+  c->valid = 1;
+  if (stats4) {
+    stats4[0] = nb_now < m->g.max_blocks ? nb_now : m->g.max_blocks;
+    stats4[1] = h.n_stamp; stats4[2] = h.n_touch; stats4[3] = h.n_dirty;
+  }
+  *n_tri_out = (int64_t)total;
+  rc = ts_check_deferred(m);  // as tslam_mc_generate2
+  if (rc) return rc;
+  if (total > cap_tri) {
+    ts_set_error("marching cubes: %lld triangles > capacity %lld (output saturated)", total, (long long)cap_tri);
+    return TSLAM_E_CAPACITY;
+  }
+  return TSLAM_OK;
+}
+
+extern "C" int tslam_mesh_updated_blocks(tslam_mesh_t* c, int64_t cap, int32_t* blk4, int64_t* first_tri, int32_t* n_tri, int64_t* n_out,
+                                         int32_t* full_out, void* stream) {
+  if (!c || !n_out || cap < 0 || (cap > 0 && (!blk4 || !first_tri || !n_tri))) return TSLAM_E_INVALID;
+  if (!c->valid) { ts_set_error("tslam_mesh_updated_blocks: no completed update"); return TSLAM_E_INVALID; }
+  tslam_tsdf* m = c->m;
+  cudaStream_t st = (cudaStream_t)stream;
+  long long* d_n = (long long*)&c->ctl->total;  // (the update's scratch word, free between updates)
+  k_mesh_updated<<<1, 1024, 0, st>>>(m->g, c->nb, c->full, c->mark, c->upd, c->cnt, c->off[c->cur], cap, blk4, (long long*)first_tri, n_tri, d_n);
+  TS_LAUNCH_CHECK(m);
+  long long n = 0;
+  TS_CUDA(cudaMemcpyAsync(&n, d_n, 8, cudaMemcpyDeviceToHost, st));
+  TS_CUDA(cudaStreamSynchronize(st));
+  *n_out = (int64_t)n;
+  if (full_out) *full_out = c->full;
+  if (n > cap) {
+    ts_set_error("tslam_mesh_updated_blocks: %lld blocks > capacity %lld (output saturated)", n, (long long)cap);
     return TSLAM_E_CAPACITY;
   }
   return TSLAM_OK;

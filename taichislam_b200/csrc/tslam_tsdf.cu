@@ -501,7 +501,7 @@ __global__ void __launch_bounds__(RM_THREADS, 2) k_raymarch(const __grid_constan
 // (dense_tsdf.py:264-267 applied once per voxel per batch).  One CTA per block,
 // fully coalesced float2 streams.  clamp=0 is the fusion variant (:274-278).
 // ---------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) k_commit(TsGrid g, int clamp, int fused_obs) {
+__global__ void __launch_bounds__(256) k_commit(TsGrid g, int clamp, int fused_obs, unsigned long long* stamp, unsigned long long seq) {
   const int nd = *g.n_dirty;
   for (int q = blockIdx.x; q < nd; q += gridDim.x) {
     const int blk = g.dirty_list[q];
@@ -535,7 +535,7 @@ __global__ void __launch_bounds__(256) k_commit(TsGrid g, int clamp, int fused_o
         }
       }
     }
-    if (threadIdx.x == 0) { g.dirty_flag[blk] = 0; g.esdf_dirty[blk] = 1; }
+    if (threadIdx.x == 0) { g.dirty_flag[blk] = 0; g.esdf_dirty[blk] = 1; stamp[blk] = seq; }
   }
 }
 // ---------------------------------------------------------------------------
@@ -576,7 +576,7 @@ __device__ __forceinline__ void bulk_s2g(void* dst_gmem, const void* src_smem, u
   asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(dst_gmem), "r"(smem_u32(src_smem)), "r"(bytes) : "memory");
 }
 
-__global__ void __launch_bounds__(256) k_commit_tma(TsGrid g, int clamp, int fused_obs) {
+__global__ void __launch_bounds__(256) k_commit_tma(TsGrid g, int clamp, int fused_obs, unsigned long long* stamp, unsigned long long seq) {
   extern __shared__ __align__(128) unsigned char cm_smem[];
   float2* s_acc = reinterpret_cast<float2*>(cm_smem);
   float2* s_tw = reinterpret_cast<float2*>(cm_smem + CM_PLANE_BYTES);
@@ -623,6 +623,7 @@ __global__ void __launch_bounds__(256) k_commit_tma(TsGrid g, int clamp, int fus
       asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");  // smem may be overwritten by the next block's loads
       g.dirty_flag[blk] = 0;
       g.esdf_dirty[blk] = 1;
+      stamp[blk] = seq;
     }
     __syncthreads();
   }
@@ -766,6 +767,8 @@ extern "C" int tslam_tsdf_create(const tslam_tsdf_config_t* cfg, tslam_tsdf_t** 
   TS_CUDA(cudaMemset(g.dirty_flag, 0, (size_t)g.max_blocks * 4));
   TS_CUDA(cudaMalloc(&g.esdf_dirty, (size_t)g.max_blocks * 4));
   TS_CUDA(cudaMemset(g.esdf_dirty, 0, (size_t)g.max_blocks * 4));
+  TS_CUDA(cudaMalloc(&m->blk_stamp, (size_t)g.max_blocks * 8));
+  TS_CUDA(cudaMemset(m->blk_stamp, 0, (size_t)g.max_blocks * 8));
   TS_CUDA(cudaMalloc(&m->scratch_i, 64 * sizeof(int)));
   TS_CUDA(cudaMemset(m->scratch_i, 0, 64 * sizeof(int)));
   g.n_blocks = m->scratch_i + 0;
@@ -879,7 +882,7 @@ extern "C" int tslam_tsdf_destroy(tslam_tsdf_t* m) {
   if (g.col) cudaFree(g.col);
   if (m->tex_stage) cudaFree(m->tex_stage);
   if (m->rgb_stage) cudaFree(m->rgb_stage);
-  cudaFree(g.ghost); cudaFree(g.dirty_flag); cudaFree(g.esdf_dirty); cudaFree(g.dirty_list); cudaFree(m->scratch_i);
+  cudaFree(g.ghost); cudaFree(g.dirty_flag); cudaFree(g.esdf_dirty); cudaFree(m->blk_stamp); cudaFree(g.dirty_list); cudaFree(m->scratch_i);
   cudaFree(m->buckets); cudaFree(m->bidx); cudaFree(m->ray_list); cudaFree(m->depth_stage); cudaFree(m->points_stage);
   cudaStreamDestroy(m->copy_stream);
   if (m->h_ring) cudaFreeHost(m->h_ring);
@@ -898,6 +901,7 @@ extern "C" int tslam_tsdf_reset(tslam_tsdf_t* m, void* stream) {
   int nb = 0;
   m->n_integrate_calls = 0;  // pending sums are discarded with the blocks
   m->esdf_full_needed = 1;   // ... and the ESDF state
+  m->mesh_epoch++;           // ... and the incremental mesh (planes cleared and pool slots recycled without stamps)
   m->q_n = 0;                // ... and so are queued frames
   m->q_gathered = 0;
   TS_CUDA(cudaMemcpyAsync(&nb, g.n_blocks, 4, cudaMemcpyDeviceToHost, st));
@@ -950,8 +954,9 @@ static int ts_launch_commit(tslam_tsdf* m, cudaStream_t st, int clamp, int fused
   TS_LAUNCH_CHECK(m);
   static const bool plain_env = getenv("TSLAM_COMMIT_PLAIN") != nullptr;  // A/B switch for the non-TMA variant
   const bool plain = plain_env || m->g.col != nullptr;  // textured maps: the per-thread variant also folds the colours
-  if (plain) k_commit<<<grid, 256, 0, st>>>(m->g, clamp, fused);
-  else k_commit_tma<<<m->sm_count * 3, 256, CM_SMEM, st>>>(m->g, clamp, fused);
+  const unsigned long long seq = ++m->commit_seq;        // stamp of every block this commit writes (incremental mesh)
+  if (plain) k_commit<<<grid, 256, 0, st>>>(m->g, clamp, fused, m->blk_stamp, seq);
+  else k_commit_tma<<<m->sm_count * 3, 256, CM_SMEM, st>>>(m->g, clamp, fused, m->blk_stamp, seq);
   TS_LAUNCH_CHECK(m);
   k_reset_counters<<<1, 1, 0, st>>>(m->g.n_dirty, nullptr);
   TS_LAUNCH_CHECK(m);
@@ -1598,6 +1603,7 @@ extern "C" int tslam_tsdf_scatter2(tslam_tsdf_t* m, int32_t submap, int64_t n, c
   int grid = (int)((n + 255) / 256);
   if (grid > m->sm_count * 32) grid = m->sm_count * 32;
   m->esdf_full_needed = 1;  // bulk load: values change without a commit
+  m->mesh_epoch++;          // (same for the incremental mesh)
   k_scatter<<<grid, 256, 0, st>>>(m->g, submap, n, idx, tsdf, w, occ, color);
   TS_LAUNCH_CHECK(m);
   return TSLAM_OK;

@@ -1,0 +1,62 @@
+"""MeshCache - the incremental marching-cubes mesh of one map (tslam_mesh_*, include/tslam.h).
+
+update() gives what tslam_mc_generate2(step=1) gives, bit for bit, while remeshing only the blocks a commit since the
+previous update could have changed.  Outputs are torch CUDA tensors written on the current stream.
+"""
+import ctypes as C
+
+from . import _capi as capi
+
+
+class MeshCache:
+    def __init__(self, handle):
+        """handle: the TsdfHandle of the map.  The cache keeps it alive: a cache must go before its map."""
+        self.map = handle
+        self.L = handle.L
+        h = C.c_void_p()
+        capi.check(self.L.tslam_mesh_create(handle.h, C.byref(h)))
+        self.h = h
+        self.stats = (0, 0, 0, 0)
+
+    def close(self):
+        if getattr(self, "h", None):
+            self.L.tslam_mesh_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def update_into(self, thres, cap_tri, verts, normals, colors=None):
+        """Mesh into caller tensors verts / normals (/ colors) f32 [3*cap_tri, 3].  Returns (demand, rc); rc is 0 or
+        TSLAM_E_CAPACITY (outputs saturated at cap_tri), anything else raises.  self.stats = (blocks, stamped,
+        touched, remeshed)."""
+        n = C.c_int64(0)
+        st = (C.c_int32 * 4)()
+        rc = self.L.tslam_mesh_update(self.h, float(thres), int(cap_tri), capi.tptr(verts), capi.tptr(normals), capi.tptr(colors),
+                                      C.byref(n), st, capi.stream_ptr())
+        if rc != capi.E_CAPACITY:
+            capi.check(rc)
+        self.stats = tuple(int(x) for x in st)
+        return int(n.value), rc
+
+    def updated_blocks(self):
+        """The blocks remeshed by the last update, in pool order: dict(blocks int32 [n,4] (submap, bx, by, bz),
+        first_tri int64 [n], n_tri int32 [n], full).  A superset of the blocks whose triangles changed; n_tri 0 means
+        the block's mesh is now empty; full = the last update rebuilt everything (drop what was kept)."""
+        import torch
+        dev = torch.device("cuda", torch.cuda.current_device())
+        n, full = C.c_int64(0), C.c_int32(0)
+        rc = self.L.tslam_mesh_updated_blocks(self.h, 0, None, None, None, C.byref(n), C.byref(full), capi.stream_ptr())
+        if rc != capi.E_CAPACITY:  # (the count alone: capacity 0)
+            capi.check(rc)
+        k = int(n.value)
+        blk = torch.empty((max(k, 1), 4), dtype=torch.int32, device=dev)
+        first = torch.empty(max(k, 1), dtype=torch.int64, device=dev)
+        cnt = torch.empty(max(k, 1), dtype=torch.int32, device=dev)
+        rc = self.L.tslam_mesh_updated_blocks(self.h, k, capi.tptr(blk), capi.tptr(first), capi.tptr(cnt), C.byref(n), C.byref(full),
+                                              capi.stream_ptr())
+        capi.check(rc)
+        return dict(blocks=blk[:k], first_tri=first[:k], n_tri=cnt[:k], full=bool(full.value))

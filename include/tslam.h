@@ -437,6 +437,32 @@ int tslam_octo_raycast(tslam_octo_t* m, int32_t submap, int64_t n, const float* 
 int tslam_octo_sync(tslam_octo_t* m, void* stream);
 int64_t tslam_octo_launch_count(tslam_octo_t* m);
 
+/* ----------------------------------------------------------------------------
+ * Log-odds occupancy (OctoMap's probabilistic model; DESIGN.md section 7).  Log-odds are Q10 integers,
+ * l = round_half_away(logit(p) * 1024); with OctoMap's defaults l_hit = 868, l_miss = -415, l_min = -2048, l_max = 3595,
+ * l_occ = 0.  A voxel is unknown until its first update and occupied iff known and L > l_occ.  Each integrate call is one
+ * frame: a ray from the sensor position T3 to every endpoint; the end cell gets one hit update, every other cell of the
+ * 6-connected voxel path one miss update (a hit wins), L <- clamp(L + l, l_min, l_max) once per voxel and frame.  Depth
+ * pixels beyond max_ray_length (points beyond it in range |R p|) are cut there and give misses only.  The mode is fixed
+ * for the map's life; integrate / extract / query / raycast / fuse follow it.  Extra memory: 128 B per pool block (the
+ * per-frame hit / miss marks) + 8 B per pool block + 16 B per ray record.
+ * --------------------------------------------------------------------------*/
+typedef struct tslam_octo_logodds {
+  int32_t l_hit, l_miss, l_min, l_max, l_occ;  /* need l_miss < 0 < l_hit, l_min <= 0 <= l_max, l_occ in [l_min, l_max] */
+} tslam_octo_logodds_t;
+int tslam_octo_create_logodds(const tslam_octo_config_t* cfg, const tslam_octo_logodds_t* lp, tslam_octo_t** out);
+/* is_near_pos_occupy (mapping_common.py:193-204) for both modes: out[q] = 1 iff a cell of [-voxel, voxel)^3 around the
+ * cell of xyz[q] is occupied.  xyz / out DEVICE. */
+int tslam_octo_query_near_occupy(tslam_octo_t* m, int32_t submap, int64_t n, const float* xyz, int32_t voxel, uint8_t* out,
+                                 void* stream);
+/* every known voxel of `submap` of a log-odds map: idx int32[cap,3], L int32[cap], color f32[cap,3] or NULL (DEVICE).
+ * Synchronises. */
+int tslam_octo_gather_logodds(tslam_octo_t* m, int32_t submap, int64_t cap, int32_t* idx, int32_t* L, float* color,
+                              int64_t* n_out, void* stream);
+/* out4 = rays cast, miss-cell visits inside the volume, hit voxels, voxels updated, summed over the frames since the
+ * last clear (zeros for a hit counter).  Synchronises the device. */
+int tslam_octo_get_stats(tslam_octo_t* m, int64_t* out4, int clear);
+
 #ifdef __cplusplus
 }
 #endif

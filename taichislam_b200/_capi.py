@@ -36,6 +36,10 @@ class TsdfConfig(C.Structure):
                 ("max_image_pixels", C.c_int32), ("max_points", C.c_int32), ("texture_enabled", C.c_int32)]
 
 
+class OctoLogodds(C.Structure):
+    _fields_ = [("l_hit", C.c_int32), ("l_miss", C.c_int32), ("l_min", C.c_int32), ("l_max", C.c_int32), ("l_occ", C.c_int32)]
+
+
 class OctoConfig(C.Structure):
     _fields_ = [("voxel_scale", C.c_double), ("N", C.c_int32), ("Nz", C.c_int32), ("K", C.c_int32),
                 ("max_ray_length", C.c_double), ("min_ray_length", C.c_double),
@@ -144,6 +148,10 @@ SIGNATURES = {
     "tslam_octo_extract2": (C.c_int, [_vp, _i32, _i32, _i64, _vp, _vp, _vp, _vp]),
     "tslam_octo_sync": (C.c_int, [_vp, _vp]),
     "tslam_octo_launch_count": (_i64, [_vp]),
+    "tslam_octo_create_logodds": (C.c_int, [C.POINTER(OctoConfig), C.POINTER(OctoLogodds), C.POINTER(_vp)]),
+    "tslam_octo_query_near_occupy": (C.c_int, [_vp, _i32, _i64, _vp, _i32, _vp, _vp]),
+    "tslam_octo_gather_logodds": (C.c_int, [_vp, _i32, _i64, _vp, _vp, _vp, C.POINTER(_i64), _vp]),
+    "tslam_octo_get_stats": (C.c_int, [_vp, _vp, C.c_int]),
 }
 
 _lib = None

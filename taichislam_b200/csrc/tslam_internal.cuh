@@ -477,6 +477,23 @@ struct OcGrid {
 __device__ __forceinline__ int oc_voxel_off(int i, int j, int k) {
   return (((i & OC_BMASK) << OC_BSHIFT) | (j & OC_BMASK)) << OC_BSHIFT | (k & OC_BMASK);
 }
+// Log-odds occupancy (tslam_octo_create_logodds, DESIGN.md section 7): the cnt plane holds w = (L << 1) | 1 for a
+// known voxel and 0 for an unknown one, so a zeroed block reads unknown.  L is Q10 fixed point, clamped to
+// [l_min, l_max] after every update.
+__host__ __device__ __forceinline__ bool lo_known(unsigned int w) { return (w & 1u) != 0; }
+__host__ __device__ __forceinline__ int lo_val(unsigned int w) { return (int)w >> 1; }
+__host__ __device__ __forceinline__ unsigned int lo_word(int L) { return ((unsigned int)L << 1) | 1u; }
+#define OC_MARK_WORDS 32  // mark words per block: 0..15 hit bits, 16..31 miss bits of its 512 voxels (128 B per block)
+struct OcLo {             // per-frame workspace of a log-odds map (allocated in log-odds mode only)
+  uint32_t* mark;         // [max_blocks * 32] hit / miss bits of the frame, cleared by k_octo_lo_apply
+  int* touched_flag;      // [max_blocks] 1 = the block is on the touched list of this frame
+  int* touched;           // [max_blocks] blocks touched by the frame, in first-touch order
+  int* ctr;               // [0] ray records, [1] touched blocks of the frame
+  float4* rays;           // [ray_cap] ray endpoint (map frame, metres); w = 1 clipped (misses only), 0 ends in a hit
+  unsigned long long* stats;  // [4] rays cast, in-volume miss-cell visits, hit voxels, voxels updated
+  float min_ray, max_ray; // f32(min_ray_length), f32(max_ray_length)
+  int l_hit, l_miss, l_min, l_max, l_occ;
+};
 struct tslam_octo {
   tslam_octo_config_t cfg;
   OcGrid g;
@@ -491,6 +508,9 @@ struct tslam_octo {
   int* scratch_i;
   long long launches;
   int sm_count;
+  int logodds;            // 1 = log-odds occupancy (fixed at creation), 0 = hit counter
+  OcLo lo;
+  int ray_cap;            // ray records per frame: max(max_image_pixels, max_points)
 };
 
 // 64-bit max without a return value: RED.E.MAX.64 (atomicMax(unsigned long long*) with an unused result was lowered

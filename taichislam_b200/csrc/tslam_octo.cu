@@ -73,6 +73,8 @@ __device__ __forceinline__ long long oc_warp_append(bool want, unsigned long lon
   return want ? (long long)(base + __popc(m & ((1u << lane) - 1))) : -1;
 }
 
+// LO: gather the known voxels of a log-odds map, count[row] = their L (int32 bits)
+template <bool LO>
 __global__ void __launch_bounds__(256) k_octo_gather(OcGrid g, int submap, long long cap, int32_t* idx, unsigned int* count,
                                                       float* color, unsigned long long* counter) {
   const int nb = min(*g.n_blocks, g.max_blocks);
@@ -89,14 +91,14 @@ __global__ void __launch_bounds__(256) k_octo_gather(OcGrid g, int submap, long 
       v = (int)(e & 511);
       ts_unpack_key(g.block_key[b], s, bx, by, bz);
       c = g.cnt[e];
-      want = (s == submap) && c > 0;
+      want = (s == submap) && (LO ? lo_known(c) : c > 0);
     }
     const long long row = oc_warp_append(want, counter);
     if (want && row < cap) {
       idx[3 * row] = bx * OC_B + (v >> 6);
       idx[3 * row + 1] = by * OC_B + ((v >> 3) & 7);
       idx[3 * row + 2] = bz * OC_B + (v & 7);
-      count[row] = c;
+      count[row] = LO ? (unsigned int)lo_val(c) : c;
       if (color) {
         if (g.cw) oc_word_to_rgb(g.cw[e], color + 3 * row);
         else color[3 * row] = color[3 * row + 1] = color[3 * row + 2] = 0.0f;
@@ -151,6 +153,48 @@ __global__ void __launch_bounds__(256) k_octo_extract(OcGrid g, int submap, int 
   }
 }
 
+// the same LoD export on a log-odds map: the group's corner voxel is known and L > l_occ
+__global__ void __launch_bounds__(256) k_octo_lo_extract(OcGrid g, int submap, int group, int l_occ, const float* pR, const float* pT,
+                                                       float vs, long long cap, float* xyz, float* rgb, int* counter) {
+  const int nb = min(*g.n_blocks, g.max_blocks);
+  const long long total = (long long)nb * OC_B3;
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  const long long iters = (total + stride - 1) / stride;
+  for (long long it = 0; it < iters; ++it) {
+    const long long e = it * stride + (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    bool want = false;
+    int i = 0, j = 0, k = 0, s = 0;
+    if (e < total) {
+      const int b = (int)(e >> 9);
+      const int v = (int)(e & 511);
+      int bx, by, bz;
+      ts_unpack_key(g.block_key[b], s, bx, by, bz);
+      i = bx * OC_B + (v >> 6); j = by * OC_B + ((v >> 3) & 7); k = bz * OC_B + (v & 7);
+      const unsigned int c = g.cnt[e];
+      const bool aligned = ((i + g.hN) % group == 0) && ((j + g.hN) % group == 0) && ((k + g.hNz) % group == 0);
+      want = (s == submap) && lo_known(c) && aligned && lo_val(c) > l_occ;
+    }
+    const unsigned m = __ballot_sync(0xffffffffu, want);
+    int row = -1;
+    if (m) {
+      const int lane = threadIdx.x & 31, leader = __ffs(m) - 1;
+      int base = 0;
+      if (lane == leader) base = atomicAdd(counter, __popc(m));
+      base = __shfl_sync(0xffffffffu, base, leader);
+      row = base + __popc(m & ((1u << lane) - 1));
+    }
+    if (want && row < cap) {
+      const float lx = (float)i * vs, ly = (float)j * vs, lz = (float)k * vs;  // sijk_to_xyz mapping_common.py:234-238
+      const float* R = pR + 9 * s;
+      const float* T = pT + 3 * s;
+      xyz[3 * (size_t)row] = ((R[0] * lx + R[1] * ly) + R[2] * lz) + T[0];
+      xyz[3 * (size_t)row + 1] = ((R[3] * lx + R[4] * ly) + R[5] * lz) + T[1];
+      xyz[3 * (size_t)row + 2] = ((R[6] * lx + R[7] * ly) + R[8] * lz) + T[2];
+      if (rgb && g.cw) oc_word_to_rgb(g.cw[e], rgb + 3 * (size_t)row);  // export_color[index] = color[sijk] (:101-102)
+    }
+  }
+}
+
 // fuse_submaps_kernel (taichi_octomap.py:171-189)
 __global__ void __launch_bounds__(256) k_octo_fuse(OcGrid dst, OcGrid src, float thres, const float* pR, const float* pT, float vs) {
   const int nb = min(*src.n_blocks, src.max_blocks);
@@ -174,13 +218,233 @@ __global__ void __launch_bounds__(256) k_octo_fuse(OcGrid dst, OcGrid src, float
 }
 
 // ---------------------------------------------------------------------------
+// Log-odds occupancy (DESIGN.md section 7, "Log-odds Octomap").  One integrate call = one frame = four steps:
+//   1. k_octo_lo_depth / k_octo_lo_points: one thread per sampled pixel / point.  Unproject, filter, clip at
+//      max_ray_length, append a ray record, set the hit bit of the end cell (unless clipped) and raise its colour word.
+//   2. k_octo_lo_walk: one lane per ray walks the 6-connected voxel path origin cell -> end cell and sets the miss bit
+//      of every in-volume cell before the end cell (and of the end cell of a clipped ray).
+//   3. k_octo_lo_apply: one CTA per block the frame touched: L <- clamp(L + (hit ? l_hit : l_miss)) for every marked
+//      voxel, so a voxel is updated once per frame and a hit wins over a miss; the marks are cleared.
+// ---------------------------------------------------------------------------
+
+// first touch of a block in this frame: put it on the touched list
+__device__ __forceinline__ void lo_touch(const OcLo& lo, int blk) {
+  if (lo.touched_flag[blk] == 0 && atomicExch(&lo.touched_flag[blk], 1) == 0) lo.touched[atomicAdd(&lo.ctr[1], 1)] = blk;
+}
+// test-then-set: every ray starts in the few cells around the sensor, an unconditional atomic would serialise on them
+__device__ __forceinline__ void lo_mark(const OcLo& lo, int blk, int v, bool hit) {
+  uint32_t* w = lo.mark + (size_t)blk * OC_MARK_WORDS + (hit ? 0 : 16) + (v >> 5);
+  const uint32_t bit = 1u << (v & 31);
+  if (!(*(volatile uint32_t*)w & bit)) atomicOr(w, bit);
+}
+
+// append the ray record of a valid sample; an endpoint that is not clipped marks its cell as a hit
+__device__ __forceinline__ void lo_emit(const OcGrid& g, const OcLo& lo, int s, float vs, bool valid, bool clipped, float px, float py,
+                                        float pz, unsigned long long cw) {
+  const int row = warp_append_i32(valid, &lo.ctr[0]);
+  if (!valid) return;
+  lo.rays[row] = make_float4(px, py, pz, clipped ? 1.0f : 0.0f);
+  if (clipped) return;
+  const int i = oc_iroundf(px / vs), j = oc_iroundf(py / vs), k = oc_iroundf(pz / vs);
+  if (!ts_in_bounds(g, i, j, k)) return;
+  const int blk = ts_get_or_alloc(g, ts_pack_key(s, i >> OC_BSHIFT, j >> OC_BSHIFT, k >> OC_BSHIFT));
+  if (blk < 0) return;
+  lo_touch(lo, blk);
+  const int v = oc_voxel_off(i, j, k);
+  lo_mark(lo, blk, v, true);
+  if (cw) ts_red_max_u64(&g.cw[(size_t)blk * OC_B3 + v], cw);
+}
+
+__global__ void __launch_bounds__(256) k_octo_lo_depth(OcGrid g, OcLo lo, const uint16_t* __restrict__ depth, int h, int w, int hh, int ww,
+                                                        TsFrame fr, TsIntrin in, const uint8_t* __restrict__ tex, int th, int tw) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  bool valid = false, clipped = false;
+  float px = 0.0f, py = 0.0f, pz = 0.0f;
+  unsigned long long cw = 0ull;
+  if (t < hh * ww) {
+    const int jj = t / ww, ii = t - jj * ww;
+    const int j = jj * in.step, i = ii * in.step;
+    const uint16_t d = depth[(size_t)j * w + i];
+    const float df = (float)d;
+    if (d != 0 && !(df < in.dmin_mm)) {
+      valid = true;
+      clipped = df > in.dmax_mm;
+      const float dep = clipped ? lo.max_ray : df / 1000.0f;  // a far pixel is cut at depth max_ray_length
+      const float x = ((float)i - in.cx) * dep / in.fx;
+      const float y = ((float)j - in.cy) * dep / in.fy;
+      px = ((fr.R[0] * x + fr.R[1] * y) + fr.R[2] * dep) + fr.T[0];
+      py = ((fr.R[3] * x + fr.R[4] * y) + fr.R[5] * dep) + fr.T[1];
+      pz = ((fr.R[6] * x + fr.R[7] * y) + fr.R[8] * dep) + fr.T[2];
+      if (tex && !clipped) {
+        int ti, tj;
+        const uint8_t zero3[3] = {0, 0, 0};
+        cw = oc_color_word(fr.seq, ts_color_pixel(in, i, j, th, tw, ti, tj) ? tex + ((size_t)tj * tw + ti) * 3 : zero3);
+      }
+    }
+  }
+  lo_emit(g, lo, fr.submap, in.vs, valid, clipped, px, py, pz, cw);
+}
+
+__global__ void __launch_bounds__(256) k_octo_lo_points(OcGrid g, OcLo lo, const float* __restrict__ xyz, int n, TsFrame fr, float vs,
+                                                         const uint8_t* __restrict__ rgb) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  bool valid = false, clipped = false;
+  float px = 0.0f, py = 0.0f, pz = 0.0f;
+  unsigned long long cw = 0ull;
+  if (t < n) {
+    const float x = xyz[3 * (size_t)t], y = xyz[3 * (size_t)t + 1], z = xyz[3 * (size_t)t + 2];
+    float rx = (fr.R[0] * x + fr.R[1] * y) + fr.R[2] * z;
+    float ry = (fr.R[3] * x + fr.R[4] * y) + fr.R[5] * z;
+    float rz = (fr.R[6] * x + fr.R[7] * y) + fr.R[8] * z;
+    const float r = sqrtf((rx * rx + ry * ry) + rz * rz);  // range from the sensor
+    valid = r >= lo.min_ray && r < INFINITY;
+    clipped = r > lo.max_ray;
+    if (clipped) {
+      const float sc = lo.max_ray / r;
+      rx = rx * sc; ry = ry * sc; rz = rz * sc;
+    }
+    px = rx + fr.T[0]; py = ry + fr.T[1]; pz = rz + fr.T[2];
+    if (rgb && valid && !clipped) cw = oc_color_word(fr.seq, rgb + 3 * (size_t)t);
+  }
+  lo_emit(g, lo, fr.submap, vs, valid, clipped, px, py, pz, cw);
+}
+
+// Amanatides-Woo in voxel units: p0 = origin / vs, p1 = endpoint / vs, cells c = round_half_away(p).  The k-th boundary
+// crossing of axis a is at t = ((c_a + 0.5 s_a) - p0_a) * (1 / (p1_a - p0_a)), recomputed from the current cell (no
+// accumulated increments); each step takes the axis with the smallest t among those with steps left, ties to the
+// lower axis.  The step counts |c1 - c0| per axis are integers, so the path always has |c1 - c0|_1 + 1 cells.
+__global__ void __launch_bounds__(256) k_octo_lo_walk(OcGrid g, OcLo lo, int s, float vs, float ox, float oy, float oz) {
+  const int n = lo.ctr[0];
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t == 0) atomicAdd(&lo.stats[0], (unsigned long long)n);
+  unsigned int visits = 0;
+  if (t < n) {
+    const float4 r = lo.rays[t];
+    const float p0x = ox / vs, p0y = oy / vs, p0z = oz / vs;
+    const float p1x = r.x / vs, p1y = r.y / vs, p1z = r.z / vs;
+    int cx = oc_iroundf(p0x), cy = oc_iroundf(p0y), cz = oc_iroundf(p0z);
+    const int ex = oc_iroundf(p1x), ey = oc_iroundf(p1y), ez = oc_iroundf(p1z);
+    int lx = abs(ex - cx), ly = abs(ey - cy), lz = abs(ez - cz);
+    const int sx = ex > cx ? 1 : -1, sy = ey > cy ? 1 : -1, sz = ez > cz ? 1 : -1;
+    const float hx = 0.5f * (float)sx, hy = 0.5f * (float)sy, hz = 0.5f * (float)sz;
+    const float ix = lx ? 1.0f / (p1x - p0x) : 0.0f, iy = ly ? 1.0f / (p1y - p0y) : 0.0f, iz = lz ? 1.0f / (p1z - p0z) : 0.0f;
+    float tx = (((float)cx + hx) - p0x) * ix, ty = (((float)cy + hy) - p0y) * iy, tz = (((float)cz + hz) - p0z) * iz;
+    const bool clipped = r.w != 0.0f;
+    unsigned long long ckey = ~0ull;
+    int cblk = -1;
+    for (int left = lx + ly + lz;; --left) {
+      if ((left > 0 || clipped) && ts_in_bounds(g, cx, cy, cz)) {
+        ++visits;
+        const unsigned long long key = ts_pack_key(s, cx >> OC_BSHIFT, cy >> OC_BSHIFT, cz >> OC_BSHIFT);
+        if (key != ckey) {  // hash probe only when the walk enters another block
+          ckey = key;
+          cblk = ts_get_or_alloc(g, key);
+          if (cblk >= 0) lo_touch(lo, cblk);
+        }
+        if (cblk >= 0) lo_mark(lo, cblk, oc_voxel_off(cx, cy, cz), false);
+      }
+      if (left == 0) break;
+      int a = 3;
+      float tb = 0.0f;
+      if (lx > 0) { a = 0; tb = tx; }
+      if (ly > 0 && (a == 3 || ty < tb)) { a = 1; tb = ty; }
+      if (lz > 0 && (a == 3 || tz < tb)) a = 2;
+      if (a == 0) { cx += sx; --lx; tx = (((float)cx + hx) - p0x) * ix; }
+      else if (a == 1) { cy += sy; --ly; ty = (((float)cy + hy) - p0y) * iy; }
+      else { cz += sz; --lz; tz = (((float)cz + hz) - p0z) * iz; }
+    }
+  }
+  for (int o = 16; o > 0; o >>= 1) visits += __shfl_xor_sync(0xffffffffu, visits, o);
+  if ((threadIdx.x & 31) == 0 && visits) atomicAdd(&lo.stats[1], (unsigned long long)visits);
+}
+
+// one CTA (128 threads, 4 voxels each) per touched block
+__global__ void __launch_bounds__(128) k_octo_lo_apply(OcGrid g, OcLo lo) {
+  __shared__ uint32_t mk[OC_MARK_WORDS];
+  __shared__ unsigned int n_hit, n_upd;
+  const int nt = lo.ctr[1];
+  if (threadIdx.x == 0) { n_hit = 0; n_upd = 0; }
+  for (int q = blockIdx.x; q < nt; q += gridDim.x) {
+    const int blk = lo.touched[q];
+    __syncthreads();  // the previous block's marks are consumed
+    if (threadIdx.x < OC_MARK_WORDS) {
+      uint32_t* w = lo.mark + (size_t)blk * OC_MARK_WORDS + threadIdx.x;
+      mk[threadIdx.x] = *w;
+      *w = 0u;
+    }
+    if (threadIdx.x == 0) lo.touched_flag[blk] = 0;
+    __syncthreads();
+    unsigned int h = 0, u = 0;
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+      const int v = threadIdx.x + 128 * r;
+      const bool hit = (mk[v >> 5] >> (v & 31)) & 1u;
+      const bool miss = (mk[16 + (v >> 5)] >> (v & 31)) & 1u;
+      if (!(hit || miss)) continue;
+      unsigned int* p = g.cnt + (size_t)blk * OC_B3 + v;
+      const unsigned int w = *p;
+      const int L = (lo_known(w) ? lo_val(w) : 0) + (hit ? lo.l_hit : lo.l_miss);
+      *p = lo_word(min(max(L, lo.l_min), lo.l_max));
+      h += hit;
+      ++u;
+    }
+    if (h) atomicAdd(&n_hit, h);
+    if (u) atomicAdd(&n_upd, u);
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    if (n_hit) atomicAdd(&lo.stats[2], (unsigned long long)n_hit);
+    if (n_upd) atomicAdd(&lo.stats[3], (unsigned long long)n_upd);
+  }
+}
+
+// Fusion of log-odds maps: every known source voxel adds its L to the nearest target voxel (placement as k_octo_fuse).
+// The target word collects (sum L) << 1 by additions of L << 1 and gets its known bit by an OR, so the result does not
+// depend on the order; k_octo_lo_clamp clamps every target voxel once when all sums are in.
+__global__ void __launch_bounds__(256) k_octo_lo_fuse(OcGrid dst, OcGrid src, const float* pR, const float* pT, float vs) {
+  const int nb = min(*src.n_blocks, src.max_blocks);
+  const long long total = (long long)nb * OC_B3;
+  for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
+    const unsigned int c = src.cnt[e];
+    if (!lo_known(c)) continue;
+    const int b = (int)(e >> 9), v = (int)(e & 511);
+    int s, bx, by, bz;
+    ts_unpack_key(src.block_key[b], s, bx, by, bz);
+    const float lx = (float)(bx * OC_B + (v >> 6)) * vs, ly = (float)(by * OC_B + ((v >> 3) & 7)) * vs,
+                lz = (float)(bz * OC_B + (v & 7)) * vs;
+    const float* R = pR + 9 * s;
+    const float* T = pT + 3 * s;
+    const float x = ((R[0] * lx + R[1] * ly) + R[2] * lz) + T[0];
+    const float y = ((R[3] * lx + R[4] * ly) + R[5] * lz) + T[1];
+    const float z = ((R[6] * lx + R[7] * ly) + R[8] * lz) + T[2];
+    const int i = oc_iroundf(x / vs), j = oc_iroundf(y / vs), k = oc_iroundf(z / vs);
+    if (!ts_in_bounds(dst, i, j, k)) continue;
+    const int blk = ts_get_or_alloc(dst, ts_pack_key(0, i >> OC_BSHIFT, j >> OC_BSHIFT, k >> OC_BSHIFT));
+    if (blk < 0) continue;
+    const size_t o = (size_t)blk * OC_B3 + oc_voxel_off(i, j, k);
+    red_add_u32(&dst.cnt[o], (unsigned int)lo_val(c) << 1);
+    atomicOr(&dst.cnt[o], 1u);
+    const unsigned long long cw = (dst.cw && src.cw) ? src.cw[e] : 0ull;
+    if (cw) ts_red_max_u64(&dst.cw[o], cw);
+  }
+}
+__global__ void __launch_bounds__(256) k_octo_lo_clamp(OcGrid g, int l_min, int l_max) {
+  const int nb = min(*g.n_blocks, g.max_blocks);
+  const long long total = (long long)nb * OC_B3;
+  for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
+    const unsigned int c = g.cnt[e];
+    if (lo_known(c)) g.cnt[e] = lo_word(min(max(lo_val(c), l_min), l_max));
+  }
+}
+
+// ---------------------------------------------------------------------------
 static size_t oc_next_pow2(size_t v) {
   size_t p = 1;
   while (p < v) p <<= 1;
   return p;
 }
 
-extern "C" int tslam_octo_create(const tslam_octo_config_t* cfg, tslam_octo_t** out) {
+static int oc_create(const tslam_octo_config_t* cfg, const tslam_octo_logodds_t* lp, tslam_octo_t** out) {
   if (!cfg || !out) return TSLAM_E_INVALID;
   *out = nullptr;
   if (cfg->voxel_scale <= 0 || cfg->N <= 0 || cfg->Nz <= 0 || cfg->N > 8192 || cfg->Nz > 8192 || cfg->recast_step <= 0) {
@@ -239,9 +503,39 @@ extern "C" int tslam_octo_create(const tslam_octo_config_t* cfg, tslam_octo_t** 
   TS_CUDA(cudaMalloc(&m->pose_T, (size_t)m->cfg.max_submaps * 12));
   TS_CUDA(cudaMemset(m->pose_R, 0, (size_t)m->cfg.max_submaps * 36));
   TS_CUDA(cudaMemset(m->pose_T, 0, (size_t)m->cfg.max_submaps * 12));
+  if (lp) {  // log-odds workspace: mark plane 128 B + touched flag / list 8 B per pool block, 16 B per ray record
+    m->logodds = 1;
+    OcLo& lo = m->lo;
+    lo.l_hit = lp->l_hit; lo.l_miss = lp->l_miss; lo.l_min = lp->l_min; lo.l_max = lp->l_max; lo.l_occ = lp->l_occ;
+    lo.min_ray = (float)cfg->min_ray_length;
+    lo.max_ray = (float)cfg->max_ray_length;
+    m->ray_cap = m->cfg.max_image_pixels > m->cfg.max_points ? m->cfg.max_image_pixels : m->cfg.max_points;
+    TS_CUDA(cudaMalloc(&lo.mark, (size_t)g.max_blocks * OC_MARK_WORDS * 4));
+    TS_CUDA(cudaMemset(lo.mark, 0, (size_t)g.max_blocks * OC_MARK_WORDS * 4));
+    TS_CUDA(cudaMalloc(&lo.touched_flag, (size_t)g.max_blocks * 4));
+    TS_CUDA(cudaMemset(lo.touched_flag, 0, (size_t)g.max_blocks * 4));
+    TS_CUDA(cudaMalloc(&lo.touched, (size_t)g.max_blocks * 4));
+    TS_CUDA(cudaMalloc(&lo.rays, (size_t)m->ray_cap * 16));
+    lo.ctr = m->scratch_i + 16;
+    TS_CUDA(cudaMalloc(&lo.stats, 4 * 8));
+    TS_CUDA(cudaMemset(lo.stats, 0, 4 * 8));
+  }
   TS_CUDA(cudaDeviceSynchronize());
   *out = m;
   return TSLAM_OK;
+}
+
+extern "C" int tslam_octo_create(const tslam_octo_config_t* cfg, tslam_octo_t** out) { return oc_create(cfg, nullptr, out); }
+
+extern "C" int tslam_octo_create_logodds(const tslam_octo_config_t* cfg, const tslam_octo_logodds_t* lp, tslam_octo_t** out) {
+  if (!lp || !out) return TSLAM_E_INVALID;
+  *out = nullptr;
+  if (!(lp->l_min <= 0 && 0 <= lp->l_max && lp->l_min < lp->l_max && lp->l_miss < 0 && lp->l_hit > 0 && lp->l_min >= -(1 << 24) &&
+        lp->l_max <= (1 << 24) && lp->l_occ >= lp->l_min && lp->l_occ <= lp->l_max)) {
+    ts_set_error("invalid log-odds parameters: need l_miss < 0 < l_hit, l_min <= 0 <= l_max within +-2^24, l_occ in [l_min, l_max]");
+    return TSLAM_E_INVALID;
+  }
+  return oc_create(cfg, lp, out);
 }
 
 extern "C" int tslam_octo_destroy(tslam_octo_t* m) {
@@ -251,6 +545,9 @@ extern "C" int tslam_octo_destroy(tslam_octo_t* m) {
   if (m->g.cw) cudaFree(m->g.cw);
   if (m->tex_stage) cudaFree(m->tex_stage);
   cudaFree(m->depth_stage); cudaFree(m->points_stage); cudaFree(m->pose_R); cudaFree(m->pose_T);
+  if (m->logodds) {
+    cudaFree(m->lo.mark); cudaFree(m->lo.touched_flag); cudaFree(m->lo.touched); cudaFree(m->lo.rays); cudaFree(m->lo.stats);
+  }
   delete m;
   return TSLAM_OK;
 }
@@ -296,6 +593,17 @@ static void oc_fill_frame(tslam_octo* m, TsFrame& fr, const float* R9, const flo
   fr.seq = m->frame_seq;
 }
 
+// steps 2 and 3 of a log-odds frame; n_max bounds the ray records the endpoint kernel wrote
+static int oc_lo_finish(tslam_octo* m, const TsFrame& fr, int n_max, cudaStream_t st) {
+  k_octo_lo_walk<<<(n_max + 255) / 256, 256, 0, st>>>(m->g, m->lo, fr.submap, m->in.vs, fr.T[0], fr.T[1], fr.T[2]);
+  m->launches++;
+  TS_CUDA(cudaGetLastError());
+  k_octo_lo_apply<<<m->sm_count * 16, 128, 0, st>>>(m->g, m->lo);
+  m->launches++;
+  TS_CUDA(cudaGetLastError());
+  return TSLAM_OK;
+}
+
 static int oc_deferred(tslam_octo* m) {
   int err = 0;
   TS_CUDA(cudaMemcpy(&err, m->g.err, 4, cudaMemcpyDeviceToHost));
@@ -331,6 +639,14 @@ extern "C" int tslam_octo_integrate_points_rgb(tslam_octo_t* m, const float* xyz
   }
   TsFrame fr;
   oc_fill_frame(m, fr, R9, T3, submap);
+  if (m->logodds) {
+    if (n > m->ray_cap) { ts_set_error("n=%d exceeds the ray records of a log-odds map (%d)", n, m->ray_cap); return TSLAM_E_INVALID; }
+    TS_CUDA(cudaMemsetAsync(m->lo.ctr, 0, 8, st));
+    k_octo_lo_points<<<(n + 255) / 256, 256, 0, st>>>(m->g, m->lo, src, n, fr, m->in.vs, csrc);
+    m->launches++;
+    TS_CUDA(cudaGetLastError());
+    return oc_lo_finish(m, fr, n, st);
+  }
   k_octo_points<<<(n + 255) / 256, 256, 0, st>>>(m->g, src, n, fr, m->in.vs, csrc);
   m->launches++;
   TS_CUDA(cudaGetLastError());
@@ -365,23 +681,25 @@ extern "C" int tslam_octo_integrate_depth_tex(tslam_octo_t* m, const uint16_t* d
   }
   TsFrame fr;
   oc_fill_frame(m, fr, R9, T3, submap);
+  if (m->logodds) {
+    TS_CUDA(cudaMemsetAsync(m->lo.ctr, 0, 8, st));
+    k_octo_lo_depth<<<(hh * ww + 255) / 256, 256, 0, st>>>(m->g, m->lo, src, h, w, hh, ww, fr, m->in, tsrc, th, tw);
+    m->launches++;
+    TS_CUDA(cudaGetLastError());
+    return oc_lo_finish(m, fr, hh * ww, st);
+  }
   k_octo_depth<<<(hh * ww + 255) / 256, 256, 0, st>>>(m->g, src, h, w, hh, ww, fr, m->in, tsrc, th, tw);
   m->launches++;
   TS_CUDA(cudaGetLastError());
   return TSLAM_OK;
 }
 
-extern "C" int tslam_octo_gather(tslam_octo_t* m, int32_t submap, int64_t cap, int32_t* idx, uint32_t* count, int64_t* n_out,
-                                 void* stream) {
-  return tslam_octo_gather2(m, submap, cap, idx, count, nullptr, n_out, stream);
-}
-extern "C" int tslam_octo_gather2(tslam_octo_t* m, int32_t submap, int64_t cap, int32_t* idx, uint32_t* count, float* color,
-                                  int64_t* n_out, void* stream) {
-  if (!m || !n_out) return TSLAM_E_INVALID;
-  cudaStream_t st = (cudaStream_t)stream;
+template <bool LO>
+static int oc_gather(tslam_octo* m, int32_t submap, int64_t cap, int32_t* idx, uint32_t* count, float* color, int64_t* n_out,
+                     cudaStream_t st) {
   unsigned long long* ctr = (unsigned long long*)(m->scratch_i + 8);
   TS_CUDA(cudaMemsetAsync(ctr, 0, 8, st));
-  k_octo_gather<<<m->sm_count * 8, 256, 0, st>>>(m->g, submap, cap, idx, count, color, ctr);
+  k_octo_gather<LO><<<m->sm_count * 8, 256, 0, st>>>(m->g, submap, cap, idx, count, color, ctr);
   m->launches++;
   TS_CUDA(cudaGetLastError());
   unsigned long long v = 0;
@@ -392,6 +710,23 @@ extern "C" int tslam_octo_gather2(tslam_octo_t* m, int32_t submap, int64_t cap, 
   if (rc) return rc;
   if ((int64_t)v > cap) { ts_set_error("octo gather: %lld voxels > capacity %lld", (long long)v, (long long)cap); return TSLAM_E_CAPACITY; }
   return TSLAM_OK;
+}
+
+extern "C" int tslam_octo_gather(tslam_octo_t* m, int32_t submap, int64_t cap, int32_t* idx, uint32_t* count, int64_t* n_out,
+                                 void* stream) {
+  return tslam_octo_gather2(m, submap, cap, idx, count, nullptr, n_out, stream);
+}
+extern "C" int tslam_octo_gather2(tslam_octo_t* m, int32_t submap, int64_t cap, int32_t* idx, uint32_t* count, float* color,
+                                  int64_t* n_out, void* stream) {
+  if (!m || !n_out) return TSLAM_E_INVALID;
+  if (m->logodds) { ts_set_error("tslam_octo_gather*: the map holds log-odds, read it with tslam_octo_gather_logodds"); return TSLAM_E_INVALID; }
+  return oc_gather<false>(m, submap, cap, idx, count, color, n_out, (cudaStream_t)stream);
+}
+extern "C" int tslam_octo_gather_logodds(tslam_octo_t* m, int32_t submap, int64_t cap, int32_t* idx, int32_t* L, float* color,
+                                         int64_t* n_out, void* stream) {
+  if (!m || !n_out) return TSLAM_E_INVALID;
+  if (!m->logodds) { ts_set_error("tslam_octo_gather_logodds: the map is a hit counter"); return TSLAM_E_INVALID; }
+  return oc_gather<true>(m, submap, cap, idx, (uint32_t*)L, color, n_out, (cudaStream_t)stream);
 }
 
 extern "C" int tslam_octo_extract(tslam_octo_t* m, int32_t submap, int32_t level, int64_t cap, float* xyz, int32_t* count_dev,
@@ -405,8 +740,12 @@ extern "C" int tslam_octo_extract2(tslam_octo_t* m, int32_t submap, int32_t leve
   long long group = 1;
   for (int l = 1; l < level; l++) group *= m->cfg.K;
   if (group > (1 << 20)) group = 1 << 20;
-  k_octo_extract<<<m->sm_count * 8, 256, 0, st>>>(m->g, submap, (int)group, (float)m->cfg.min_occupy_thres, m->pose_R, m->pose_T,
-                                                  m->in.vs, cap, xyz, rgb, count_dev);
+  if (m->logodds)
+    k_octo_lo_extract<<<m->sm_count * 8, 256, 0, st>>>(m->g, submap, (int)group, m->lo.l_occ, m->pose_R, m->pose_T, m->in.vs, cap, xyz,
+                                                       rgb, count_dev);
+  else
+    k_octo_extract<<<m->sm_count * 8, 256, 0, st>>>(m->g, submap, (int)group, (float)m->cfg.min_occupy_thres, m->pose_R, m->pose_T,
+                                                    m->in.vs, cap, xyz, rgb, count_dev);
   m->launches++;
   TS_CUDA(cudaGetLastError());
   return TSLAM_OK;
@@ -414,9 +753,19 @@ extern "C" int tslam_octo_extract2(tslam_octo_t* m, int32_t submap, int32_t leve
 
 extern "C" int tslam_octo_fuse(tslam_octo_t* dst, tslam_octo_t* src, void* stream) {
   if (!dst || !src || dst == src) return TSLAM_E_INVALID;
+  if (dst->logodds != src->logodds) { ts_set_error("tslam_octo_fuse: a log-odds map and a hit counter cannot be fused"); return TSLAM_E_INVALID; }
   int rc = tslam_octo_reset(dst, stream);  // taichi_octomap.py:195-196
   if (rc) return rc;
   cudaStream_t st = (cudaStream_t)stream;
+  if (dst->logodds) {
+    k_octo_lo_fuse<<<dst->sm_count * 8, 256, 0, st>>>(dst->g, src->g, dst->pose_R, dst->pose_T, dst->in.vs);
+    dst->launches++;
+    TS_CUDA(cudaGetLastError());
+    k_octo_lo_clamp<<<dst->sm_count * 8, 256, 0, st>>>(dst->g, dst->lo.l_min, dst->lo.l_max);
+    dst->launches++;
+    TS_CUDA(cudaGetLastError());
+    return TSLAM_OK;
+  }
   k_octo_fuse<<<dst->sm_count * 8, 256, 0, st>>>(dst->g, src->g, (float)dst->cfg.min_occupy_thres, dst->pose_R, dst->pose_T,
                                                  dst->in.vs);
   dst->launches++;
@@ -430,3 +779,12 @@ extern "C" int tslam_octo_sync(tslam_octo_t* m, void* stream) {
   return oc_deferred(m);
 }
 extern "C" int64_t tslam_octo_launch_count(tslam_octo_t* m) { return m ? m->launches : 0; }
+
+extern "C" int tslam_octo_get_stats(tslam_octo_t* m, int64_t* out4, int clear) {
+  if (!m || !out4) return TSLAM_E_INVALID;
+  if (!m->logodds) { for (int q = 0; q < 4; q++) out4[q] = 0; return TSLAM_OK; }
+  TS_CUDA(cudaDeviceSynchronize());
+  TS_CUDA(cudaMemcpy(out4, m->lo.stats, 32, cudaMemcpyDeviceToHost));
+  if (clear) TS_CUDA(cudaMemset(m->lo.stats, 0, 32));
+  return TSLAM_OK;
+}

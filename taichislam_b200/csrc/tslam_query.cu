@@ -104,6 +104,65 @@ __global__ void __launch_bounds__(256) k_octo_raycast(OcGrid g, int s, long long
   }
 }
 
+// Word of cell (i, j, k) of submap s of a log-odds map: 0 (unknown) outside the volume and in absent blocks
+__device__ __forceinline__ unsigned int octo_lo_word(const OcGrid& g, int s, int i, int j, int k) {
+  unsigned int c = 0;
+  if (ts_in_bounds(g, i, j, k)) {
+    const int blk = ts_find(g, ts_pack_key(s, i >> OC_BSHIFT, j >> OC_BSHIFT, k >> OC_BSHIFT));
+    if (blk >= 0) c = g.cnt[(size_t)blk * OC_B3 + oc_voxel_off(i, j, k)];
+  }
+  return c;
+}
+// occupied: known and L > l_occ
+__device__ __forceinline__ bool octo_lo_occ(unsigned int c, int l_occ) { return lo_known(c) && lo_val(c) > l_occ; }
+__device__ __forceinline__ unsigned int octo_lo_probe(const OcGrid& g, int s, float x, float y, float z, float vs) {
+  return octo_lo_word(g, s, q_iround(x / vs), q_iround(y / vs), q_iround(z / vs));
+}
+// flags: bit0 occupied, bit1 unknown
+__global__ void __launch_bounds__(256) k_octo_lo_query_points(OcGrid g, int s, long long n, const float* __restrict__ xyz, float vs, int l_occ,
+                                                               uint8_t* flags) {
+  for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < n; q += (long long)gridDim.x * blockDim.x) {
+    const unsigned int c = octo_lo_probe(g, s, xyz[3 * q], xyz[3 * q + 1], xyz[3 * q + 2], vs);
+    flags[q] = (uint8_t)((octo_lo_occ(c, l_occ) ? 1 : 0) | (lo_known(c) ? 0 : 2));
+  }
+}
+// BaseMap.raycast on a log-odds map: stops at the first occupied sample (unknown space is not occupied)
+__global__ void __launch_bounds__(256) k_octo_lo_raycast(OcGrid g, int s, long long n, const float* __restrict__ pos, const float* __restrict__ dir,
+                                                          float max_dist, float vs, int l_occ, uint8_t* hit, float* xyz_out, float* len_out) {
+  for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < n; q += (long long)gridDim.x * blockDim.x) {
+    const float px = pos[3 * q], py = pos[3 * q + 1], pz = pos[3 * q + 2];
+    const float dx = dir[3 * q], dy = dir[3 * q + 1], dz = dir[3 * q + 2];
+    const int steps = (int)(max_dist / vs);
+    float x = 0.f, y = 0.f, z = 0.f, len = 0.f;
+    bool succ = false;
+    for (int j = 0; j < steps; j++) {
+      len = (float)j * vs;
+      x = dx * len + px; y = dy * len + py; z = dz * len + pz;
+      if (octo_lo_occ(octo_lo_probe(g, s, x, y, z, vs), l_occ)) { succ = true; break; }
+    }
+    hit[q] = succ ? 1 : 0;
+    xyz_out[3 * q] = x; xyz_out[3 * q + 1] = y; xyz_out[3 * q + 2] = z;
+    len_out[q] = len;
+  }
+}
+// is_near_pos_occupy (mapping_common.py:193-204) on an Octomap: any occupied cell (i0 + a, j0 + b, k0 + c), a, b, c in
+// [-voxel, voxel), around the point's cell.  LO: log-odds predicate with thres = l_occ; else count > min_occupy_thres.
+template <bool LO>
+__global__ void __launch_bounds__(256) k_octo_query_near(OcGrid g, int s, long long n, const float* __restrict__ xyz, float vs, int thres,
+                                                          int voxel, uint8_t* out) {
+  for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < n; q += (long long)gridDim.x * blockDim.x) {
+    const int i0 = q_iround(xyz[3 * q] / vs), j0 = q_iround(xyz[3 * q + 1] / vs), k0 = q_iround(xyz[3 * q + 2] / vs);
+    bool any = false;
+    for (int i = -voxel; i < voxel && !any; i++)
+      for (int j = -voxel; j < voxel && !any; j++)
+        for (int k = -voxel; k < voxel && !any; k++) {
+          const unsigned int c = octo_lo_word(g, s, i0 + i, j0 + j, k0 + k);
+          any = LO ? octo_lo_occ(c, thres) : (float)c > (float)thres;
+        }
+    out[q] = any ? 1 : 0;
+  }
+}
+
 static int grid_for(long long n, int sm) {
   long long b = (n + 255) / 256;
   return (int)(b < (long long)sm * 16 ? (b > 0 ? b : 1) : (long long)sm * 16);
@@ -159,7 +218,10 @@ extern "C" int tslam_tsdf_raycast(tslam_tsdf_t* m, int32_t submap, int64_t n, co
 extern "C" int tslam_octo_query_points(tslam_octo_t* m, int32_t submap, int64_t n, const float* xyz, uint8_t* flags, void* stream) {
   if (!m || n < 0 || (n && (!xyz || !flags))) return TSLAM_E_INVALID;
   if (n == 0) return TSLAM_OK;
-  k_octo_query_points<<<grid_for(n, m->sm_count), 256, 0, (cudaStream_t)stream>>>(m->g, submap, n, xyz, m->in.vs, (float)m->cfg.min_occupy_thres, flags);
+  if (m->logodds)
+    k_octo_lo_query_points<<<grid_for(n, m->sm_count), 256, 0, (cudaStream_t)stream>>>(m->g, submap, n, xyz, m->in.vs, m->lo.l_occ, flags);
+  else
+    k_octo_query_points<<<grid_for(n, m->sm_count), 256, 0, (cudaStream_t)stream>>>(m->g, submap, n, xyz, m->in.vs, (float)m->cfg.min_occupy_thres, flags);
   m->launches++;
   TS_CUDA(cudaGetLastError());
   return TSLAM_OK;
@@ -168,8 +230,24 @@ extern "C" int tslam_octo_raycast(tslam_octo_t* m, int32_t submap, int64_t n, co
                                   float* xyz_out, float* len_out, void* stream) {
   if (!m || n < 0 || (n && (!pos || !dir || !hit || !xyz_out || !len_out))) return TSLAM_E_INVALID;
   if (n == 0) return TSLAM_OK;
-  k_octo_raycast<<<grid_for(n, m->sm_count), 256, 0, (cudaStream_t)stream>>>(m->g, submap, n, pos, dir, max_dist, m->in.vs,
+  if (m->logodds)
+    k_octo_lo_raycast<<<grid_for(n, m->sm_count), 256, 0, (cudaStream_t)stream>>>(m->g, submap, n, pos, dir, max_dist, m->in.vs, m->lo.l_occ,
+                                                                                hit, xyz_out, len_out);
+  else
+    k_octo_raycast<<<grid_for(n, m->sm_count), 256, 0, (cudaStream_t)stream>>>(m->g, submap, n, pos, dir, max_dist, m->in.vs,
                                                                              (float)m->cfg.min_occupy_thres, hit, xyz_out, len_out);
+  m->launches++;
+  TS_CUDA(cudaGetLastError());
+  return TSLAM_OK;
+}
+extern "C" int tslam_octo_query_near_occupy(tslam_octo_t* m, int32_t submap, int64_t n, const float* xyz, int32_t voxel, uint8_t* out, void* stream) {
+  if (!m || n < 0 || voxel < 0 || (n && (!xyz || !out))) return TSLAM_E_INVALID;
+  if (n == 0) return TSLAM_OK;
+  if (m->logodds)
+    k_octo_query_near<true><<<grid_for(n, m->sm_count), 256, 0, (cudaStream_t)stream>>>(m->g, submap, n, xyz, m->in.vs, m->lo.l_occ, voxel, out);
+  else
+    k_octo_query_near<false><<<grid_for(n, m->sm_count), 256, 0, (cudaStream_t)stream>>>(m->g, submap, n, xyz, m->in.vs, m->cfg.min_occupy_thres,
+                                                                                         voxel, out);
   m->launches++;
   TS_CUDA(cudaGetLastError());
   return TSLAM_OK;

@@ -1,6 +1,9 @@
-"""Octomap - the reference's class surface (taichi_slam/mapping/taichi_octomap.py) on the hit-count
-hash grid of libtslam.so.  The reference "Octomap" is a per-voxel hit counter (occupy += 1 per point,
-:116-119) with a threshold test (:86-88): no ray casting, no log-odds."""
+"""Octomap - the reference's class surface (taichi_slam/mapping/taichi_octomap.py) on the hash grid of libtslam.so.
+
+occupancy_model="hits" (default) is the reference's "Octomap": a per-voxel hit counter (occupy += 1 per point,
+:116-119) with a threshold test (:86-88), no ray casting.  occupancy_model="logodds" is OctoMap's probabilistic model
+(Hornung et al., 2013): each frame casts a ray from the sensor to every measured point, the end voxel gets a hit update
+and every voxel the ray crosses a miss update, in clamped Q10 integer log-odds (DESIGN.md section 7)."""
 import math
 import time
 
@@ -11,11 +14,18 @@ from .field import Field
 from .mapping_common import BaseMap
 
 
+def _q10(p):
+    """Q10 log-odds of probability p: round_half_away(logit(p) * 1024), in f64."""
+    v = math.log(p / (1.0 - p)) * 1024.0
+    return int(math.copysign(math.floor(abs(v) + 0.5), v))
+
+
 class Octomap(BaseMap):
     def __init__(self, map_scale=[10, 10], voxel_scale=0.05, min_occupy_thres=3, texture_enabled=False,
                  min_ray_length=0.3, max_ray_length=3.0, max_disp_particles=1000000, K=2,
                  max_submap_num=1024, disp_ceiling=10.0, disp_floor=-10.0,
-                 is_global_map=False, recast_step=2, color_same_proj=True, max_blocks=0):
+                 is_global_map=False, recast_step=2, color_same_proj=True, max_blocks=0, occupancy_model="hits",
+                 prob_hit=0.7, prob_miss=0.4, prob_min=0.1192, prob_max=0.971, prob_occupied=0.5):
         super(Octomap, self).__init__(voxel_scale)
         import torch
         self._torch = torch
@@ -41,9 +51,20 @@ class Octomap(BaseMap):
         self.recast_step = recast_step
         self.color_same_proj = color_same_proj
         self.color = None  # the colour plane lives inside the library handle (:77-79); read it with _h.gather(color=True)
+        if occupancy_model not in ("hits", "logodds"):
+            raise ValueError(f"occupancy_model must be 'hits' or 'logodds', not {occupancy_model!r}")
+        self.occupancy_model = occupancy_model
+        lo = None
+        if occupancy_model == "logodds":
+            self.prob_hit, self.prob_miss, self.prob_min, self.prob_max = prob_hit, prob_miss, prob_min, prob_max
+            self.prob_occupied = prob_occupied
+            self.l_hit, self.l_miss = _q10(prob_hit), _q10(prob_miss)
+            self.l_min, self.l_max, self.l_occ = _q10(prob_min), _q10(prob_max), _q10(prob_occupied)
+            lo = dict(l_hit=self.l_hit, l_miss=self.l_miss, l_min=self.l_min, l_max=self.l_max, l_occ=self.l_occ)
         self._h = OctoHandle(self.N, self.Nz, K=K, voxel_scale=ctor_voxel_scale, min_occupy_thres=min_occupy_thres,
                              min_ray_length=min_ray_length, max_ray_length=max_ray_length, recast_step=recast_step,
-                             max_submaps=min(max_submap_num, 1024), max_blocks=max_blocks, texture_enabled=texture_enabled)
+                             max_submaps=min(max_submap_num, 1024), max_blocks=max_blocks, texture_enabled=texture_enabled,
+                             logodds=lo)
         if texture_enabled:
             self._h.set_color_intrinsics([1, 0, 0, 0, 1, 0, 0, 0, 1], color_same_proj)
         dev = torch.device("cuda", torch.cuda.current_device())
@@ -57,7 +78,11 @@ class Octomap(BaseMap):
 
     @property
     def occupy(self):
-        """(idx int32[n,3], count uint32[n]) of the active submap - the leaf field of the reference's tree (:75-76)."""
+        """(idx int32[n,3], count uint32[n]) of the active submap - the leaf field of the reference's tree (:75-76).
+        Log-odds maps: (idx, L / 1024 f32[n]) of the known voxels."""
+        if self.occupancy_model == "logodds":
+            idx, L = self._h.gather(self._active())
+            return idx, (L.astype(np.float64) / 1024.0).astype(np.float32)
         return self._h.gather(self._active())
 
     def _flush(self):
@@ -128,13 +153,14 @@ class Octomap(BaseMap):
         return self._h.raycast(pos, dir, max_dist, submap=self._active())
 
     def _query_points(self, xyz):
-        occ = self._h.query_points(xyz, submap=self._active())
-        return occ, np.zeros(len(occ), bool)  # BaseMap.is_unobserved prints "Not implemented" and returns False (:207-209)
+        f = self._h.query_flags(xyz, submap=self._active())
+        # hit counter: BaseMap.is_unobserved prints "Not implemented" and returns False (:207-209), bit1 is always 0
+        return (f & 1).astype(bool), (f & 2).astype(bool)
 
     def _query_near(self, xyz, voxel):
         if int(voxel) <= 0:  # range(-voxel, voxel) is empty (mapping_common.py:198): what TopoGraphGen asks for (:328)
             return np.zeros(len(xyz), bool)
-        raise NotImplementedError("Octomap.is_near_pos_occupy(voxel > 0) has no batched kernel yet")
+        return self._h.query_near(xyz, int(voxel), submap=self._active())
 
     def saveMap(self, path):  # :201-202 (stub in the reference)
         pass

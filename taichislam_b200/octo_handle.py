@@ -9,7 +9,9 @@ from . import _capi as capi
 class OctoHandle:
     def __init__(self, N, Nz, K=2, voxel_scale=0.05, min_occupy_thres=3, min_ray_length=0.3, max_ray_length=3.0,
                  recast_step=2, Kcam=None, max_submaps=1024, max_blocks=0, max_image_pixels=0, max_points=0,
-                 texture_enabled=False):
+                 texture_enabled=False, logodds=None):
+        """logodds: None (hit counter) or a dict l_hit, l_miss, l_min, l_max, l_occ of Q10 log-odds (log-odds occupancy,
+        fixed for the map's life)."""
         capi.require_gpu()
         import torch
         self.torch = torch
@@ -22,7 +24,12 @@ class OctoHandle:
         torch.cuda.init()
         torch.cuda.current_stream()
         h = C.c_void_p()
-        capi.check(L.tslam_octo_create(C.byref(self.cfg), C.byref(h)))
+        self.logodds = dict(logodds) if logodds is not None else None
+        if self.logodds is None:
+            capi.check(L.tslam_octo_create(C.byref(self.cfg), C.byref(h)))
+        else:
+            lp = capi.OctoLogodds(*(int(self.logodds[k]) for k in ("l_hit", "l_miss", "l_min", "l_max", "l_occ")))
+            capi.check(L.tslam_octo_create_logodds(C.byref(self.cfg), C.byref(lp), C.byref(h)))
         self.h, self.L = h, L
         self.N, self.Nz, self.K = N, Nz, K
 
@@ -114,7 +121,28 @@ class OctoHandle:
         k = int(n.value)
         return (idx[:k], cnt[:k], col[:k]) if color else (idx[:k], cnt[:k])
 
+    def gather_logodds_device(self, submap=0, color=False):
+        """(idx int32[n,3], L int32[n][, color f32[n,3]]) of the known voxels of a log-odds map, on the device."""
+        torch = self.torch
+        dev = torch.device("cuda", torch.cuda.current_device())
+        n = C.c_int64(0)
+        rc = self.L.tslam_octo_gather_logodds(self.h, int(submap), 0, None, None, None, C.byref(n), capi.stream_ptr())
+        if rc not in (capi.TSLAM_OK, capi.E_CAPACITY):
+            capi.check(rc)
+        cap = int(n.value)
+        idx = torch.empty((max(cap, 1), 3), dtype=torch.int32, device=dev)
+        lo = torch.empty(max(cap, 1), dtype=torch.int32, device=dev)
+        col = torch.empty((max(cap, 1), 3), dtype=torch.float32, device=dev) if color else None
+        capi.check(self.L.tslam_octo_gather_logodds(self.h, int(submap), cap, capi.tptr(idx), capi.tptr(lo), capi.tptr(col), C.byref(n),
+                                                    capi.stream_ptr()))
+        k = int(n.value)
+        return (idx[:k], lo[:k], col[:k]) if color else (idx[:k], lo[:k])
+
     def gather(self, submap=0, color=False):
+        """Hit counter: (idx, count uint32[, color]).  Log-odds map: (idx, L int32[, color]) of the known voxels."""
+        if self.logodds is not None:
+            r = self.gather_logodds_device(submap, color=color)
+            return tuple(t.cpu().numpy() for t in r)
         r = self.gather_device(submap, color=color)
         out = (r[0].cpu().numpy(), r[1].cpu().numpy().view(np.uint32))
         return out + (r[2].cpu().numpy(),) if color else out
@@ -135,12 +163,35 @@ class OctoHandle:
             return n, xyz[:min(n, cap)].cpu().numpy(), rgb[:min(n, cap)].cpu().numpy()
         return n, xyz[:min(n, cap)].cpu().numpy()
 
-    def query_points(self, xyz, submap=0):
+    def query_flags(self, xyz, submap=0):
+        """uint8 flags per point: bit0 occupied, bit1 unknown (log-odds maps; always 0 for a hit counter)."""
         torch = self.torch
-        x = torch.from_numpy(np.ascontiguousarray(xyz, dtype=np.float32)).cuda()
+        x = torch.from_numpy(np.ascontiguousarray(xyz, dtype=np.float32).reshape(-1, 3)).cuda()
         f = torch.empty(x.shape[0], dtype=torch.uint8, device=x.device)
         capi.check(self.L.tslam_octo_query_points(self.h, int(submap), x.shape[0], capi.tptr(x), capi.tptr(f), capi.stream_ptr()))
-        return f.cpu().numpy().astype(bool)
+        return f.cpu().numpy()
+
+    def query_points(self, xyz, submap=0):
+        """occupied per point; a log-odds map returns (occupied, unknown)."""
+        f = self.query_flags(xyz, submap)
+        if self.logodds is not None:
+            return (f & 1).astype(bool), (f & 2).astype(bool)
+        return f.astype(bool)
+
+    def query_near(self, xyz, voxel, submap=0):
+        """is_near_pos_occupy: any occupied cell in [-voxel, voxel)^3 around each point's cell."""
+        torch = self.torch
+        x = torch.from_numpy(np.ascontiguousarray(xyz, dtype=np.float32).reshape(-1, 3)).cuda()
+        o = torch.empty(x.shape[0], dtype=torch.uint8, device=x.device)
+        capi.check(self.L.tslam_octo_query_near_occupy(self.h, int(submap), x.shape[0], capi.tptr(x), int(voxel), capi.tptr(o),
+                                                       capi.stream_ptr()))
+        return o.cpu().numpy().astype(bool)
+
+    def stats(self, clear=False):
+        """Log-odds counters since the last clear: rays cast, in-volume miss-cell visits, hit voxels, voxels updated."""
+        out = (C.c_int64 * 4)()
+        capi.check(self.L.tslam_octo_get_stats(self.h, out, int(bool(clear))))
+        return dict(zip(("rays", "miss_visits", "hit_voxels", "updated_voxels"), (int(v) for v in out)))
 
     def raycast(self, pos, direction, max_dist, submap=0):
         torch = self.torch

@@ -463,6 +463,29 @@ int tslam_octo_gather_logodds(tslam_octo_t* m, int32_t submap, int64_t cap, int3
  * last clear (zeros for a hit counter).  Synchronises the device. */
 int tslam_octo_get_stats(tslam_octo_t* m, int64_t* out4, int clear);
 
+/* ----------------------------------------------------------------------------
+ * Occupancy ESDF of a log-odds map (DESIGN.md section 7): per submap, a FREE voxel (known, L <= l_occ) holds its 26-
+ * neighbour chamfer distance to the nearest OCC voxel centre (known, L > l_occ), an OCC voxel minus its distance to the
+ * nearest FREE voxel centre, both truncated at D = max_dist; paths run through known voxels only.  Edge costs are
+ * vs * {1, sqrtf(2), sqrtf(3)} in f32 with vs = f32(voxel_scale).  Every call refuses a hit-counter map
+ * (TSLAM_E_INVALID).  State (allocated by the first update): about 2.7 KB per pool block.
+ * --------------------------------------------------------------------------*/
+/* Bring the field of `submap` up to date.  mode 0: incremental when the last update was for the same submap and the
+ * same max_dist (bit for bit) and no reset or fusion came since, else full; mode 1: full.  Either gives the same bits.
+ * max_dist must be finite and > 0.  stats4 (HOST, may be NULL): lower sweeps, raise sweeps (-1 = full), changed voxels,
+ * suspect voxels.  Synchronises. */
+int tslam_octo_esdf_update(tslam_octo_t* m, int32_t submap, float max_dist, int32_t mode, int32_t* stats4, void* stream);
+/* (ijk, ESDF) of every voxel known at the last update: idx int32[cap,3], esdf f32[cap] (DEVICE); n_out = the number of
+ * such voxels (TSLAM_E_CAPACITY when it exceeds cap).  Refused before an update, for another submap than the last
+ * update's, and after a reset or fusion until the next update.  Synchronises. */
+int tslam_octo_esdf_gather(tslam_octo_t* m, int32_t submap, int64_t cap, int32_t* idx, float* esdf, int64_t* n_out, void* stream);
+/* tslam_esdf_query on the occupancy ESDF, as of the last update: trilinear distance and its exact gradient; dist, grad
+ * NaN and valid 0 where a coordinate is not finite or a corner is outside the volume, in a block newer than the update,
+ * or was unknown at the update.  xyz f32[n,3], dist f32[n], grad f32[n,3], valid u8[n] (DEVICE); n == 0 is a no-op.
+ * Refused like tslam_octo_esdf_gather. */
+int tslam_octo_esdf_query(tslam_octo_t* m, int32_t submap, int64_t n, const float* xyz, float* dist, float* grad, uint8_t* valid,
+                          void* stream);
+
 #ifdef __cplusplus
 }
 #endif

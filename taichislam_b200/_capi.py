@@ -152,6 +152,9 @@ SIGNATURES = {
     "tslam_octo_query_near_occupy": (C.c_int, [_vp, _i32, _i64, _vp, _i32, _vp, _vp]),
     "tslam_octo_gather_logodds": (C.c_int, [_vp, _i32, _i64, _vp, _vp, _vp, C.POINTER(_i64), _vp]),
     "tslam_octo_get_stats": (C.c_int, [_vp, _vp, C.c_int]),
+    "tslam_octo_esdf_update": (C.c_int, [_vp, _i32, _f32, _i32, _vp, _vp]),
+    "tslam_octo_esdf_gather": (C.c_int, [_vp, _i32, _i64, _vp, _vp, C.POINTER(_i64), _vp]),
+    "tslam_octo_esdf_query": (C.c_int, [_vp, _i32, _i64, _vp, _vp, _vp, _vp, _vp]),
 }
 
 _lib = None

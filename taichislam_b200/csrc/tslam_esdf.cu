@@ -35,17 +35,12 @@
 // bounds; min/+ relaxation from there converges to the SAME least fixed point as a full recompute - tested
 // bit-for-bit (tests/test_gpu_mc_octo_esdf.py::test_esdf_incremental_equals_full_512).
 #include <cstring>
-#include "tslam_internal.cuh"
+#include "tslam_esdf_common.cuh"
 
 #define ES_T 18
 #define ES_T3 (ES_T * ES_T * ES_T)
-#define ES_GROUP 6       // sweeps enqueued per host synchronisation
-#define ES_MAX_SWEEPS 4096
 
 enum { ES_UNOBS = 0, ES_FIXED = 1, ES_POS = 2, ES_NEG = 3, ES_INERT = 4 };  // INERT: observed, TSDF is NaN
-#define ES_CH 0x40   // class-byte flags of an incremental update: CHANGED (detect) / SUSPECT (raise wave)
-#define ES_SU 0x80
-#define ES_CLS 0x0F
 
 struct EsAux {
   int* nbr;      // [max_blocks*27] neighbour block indices (-1 = absent)
@@ -453,28 +448,6 @@ static EsAux es_aux(tslam_tsdf* m) {
 }
 int* ts_esdf_xmark(tslam_tsdf* m) { return m->esdf_aux ? es_aux(m).xmark : nullptr; }
 
-// One wave (raise or lower) to convergence: sweeps are enqueued in groups, a sweep whose predecessor changed nothing
-// returns at once; the host reads ONE flag per group.  Returns the number of sweeps that did something + 1.
-template <class Launch>
-static int es_wave(tslam_tsdf* m, cudaStream_t st, int* flags, int group, Launch launch, int* n_out) {
-  int sweeps = 0;
-  for (;;) {
-    for (int q = 0; q < group && sweeps < ES_MAX_SWEEPS; q++) { sweeps++; launch(sweeps); TS_LAUNCH_CHECK(m); }
-    int changed = 0;
-    TS_CUDA(cudaMemcpyAsync(&changed, flags + sweeps, 4, cudaMemcpyDeviceToHost, st));
-    TS_CUDA(cudaStreamSynchronize(st));
-    if (!changed || sweeps >= ES_MAX_SWEEPS) break;
-  }
-  if (n_out) {
-    static int h_changed[ES_MAX_SWEEPS + 2];
-    TS_CUDA(cudaMemcpy(h_changed, flags, (size_t)(sweeps + 1) * 4, cudaMemcpyDeviceToHost));
-    int k = 1;
-    while (k <= sweeps && h_changed[k]) k++;
-    *n_out = k;
-  }
-  return TSLAM_OK;
-}
-
 // mode 0 = incremental when the state allows it (same submap as the last update, no reset / bulk load in between),
 // 1 = full recompute.  stats4 (HOST, may be NULL): lower sweeps, raise sweeps, changed voxels, suspect voxels.
 extern "C" int tslam_esdf_update2(tslam_tsdf_t* m, int32_t submap, int32_t mode, int32_t* stats4, void* stream) {
@@ -630,9 +603,6 @@ __device__ __forceinline__ int esq_block(const TsGrid& g, int submap, int nb_see
   const int b = ts_find(g, ts_pack_key(submap, bx, by, bz));
   return (b >= 0 && b < nb_seen && (ghosts || !g.ghost[b])) ? b : -1;
 }
-// lerp(a, b, t) = a + t*(b - a), rounded step by step (never contracted to an FMA): tests/esdf_query_reference.py
-__device__ __forceinline__ float esq_lerp(float a, float b, float t) { return __fadd_rn(a, __fmul_rn(t, __fsub_rn(b, a))); }
-
 // Trilinear interpolation of the ESDF over the 8 voxels around each point (voxel i centred at i*vs, submap-local frame)
 // and the exact partial derivatives of that interpolant.  One thread per point; each distinct corner block is looked
 // up once (the corner cube spans 2, 4 or 8 blocks only where i0 & 15 == 15 on some axis).  Invalid (NaN, valid = 0):
@@ -680,19 +650,7 @@ __global__ void __launch_bounds__(256) k_esdf_query(TsGrid g, EsAux aux, int sub
         }
       }
       if (ok) {
-        // dist: along x, then y, then z
-        const float c00 = esq_lerp(e[0], e[4], fx), c01 = esq_lerp(e[1], e[5], fx);
-        const float c10 = esq_lerp(e[2], e[6], fx), c11 = esq_lerp(e[3], e[7], fx);
-        d = esq_lerp(esq_lerp(c00, c10, fy), esq_lerp(c01, c11, fy), fz);
-        // d/dx: the four x-differences along y, then z
-        const float ax00 = __fsub_rn(e[4], e[0]), ax01 = __fsub_rn(e[5], e[1]), ax10 = __fsub_rn(e[6], e[2]), ax11 = __fsub_rn(e[7], e[3]);
-        gx = __fdiv_rn(esq_lerp(esq_lerp(ax00, ax10, fy), esq_lerp(ax01, ax11, fy), fz), vs);
-        // d/dy: the four y-differences along x, then z
-        const float ay00 = __fsub_rn(e[2], e[0]), ay01 = __fsub_rn(e[3], e[1]), ay10 = __fsub_rn(e[6], e[4]), ay11 = __fsub_rn(e[7], e[5]);
-        gy = __fdiv_rn(esq_lerp(esq_lerp(ay00, ay10, fx), esq_lerp(ay01, ay11, fx), fz), vs);
-        // d/dz: the four z-differences along x, then y
-        const float az00 = __fsub_rn(e[1], e[0]), az01 = __fsub_rn(e[3], e[2]), az10 = __fsub_rn(e[5], e[4]), az11 = __fsub_rn(e[7], e[6]);
-        gz = __fdiv_rn(esq_lerp(esq_lerp(az00, az10, fx), esq_lerp(az01, az11, fx), fy), vs);
+        esq_interp(e, fx, fy, fz, vs, d, gx, gy, gz);
       } else {
         d = gx = gy = gz = qnan;
       }

@@ -196,11 +196,12 @@ __device__ __forceinline__ int warp_append_i32(bool want, int* counter) {
   return want ? base + __popc(m & ((1u << lane) - 1)) : -1;
 }
 
-// Low interpolation corner of an ESDF query point (k_esdf_query, and k_owner_points which routes the points of a tiled
-// map to the rank that answers them): u = x / vs per axis, correctly rounded, c = floor(u).  False when a coordinate
-// is not finite or the corner lies outside the volume; NaN and +-inf fail the range test, so no out-of-range value
-// reaches the float -> int conversion.
-__device__ __forceinline__ bool esq_low_corner(const TsGrid& g, float vs, const float* p, float u[3], int c[3]) {
+// Low interpolation corner of an ESDF query point (k_esdf_query, k_octo_esdf_query, and k_owner_points which routes the
+// points of a tiled map to the rank that answers them): u = x / vs per axis, correctly rounded, c = floor(u).  False
+// when a coordinate is not finite or the corner lies outside the volume; NaN and +-inf fail the range test, so no
+// out-of-range value reaches the float -> int conversion.  G = TsGrid or OcGrid.
+template <class G>
+__device__ __forceinline__ bool esq_low_corner(const G& g, float vs, const float* p, float u[3], int c[3]) {
   u[0] = __fdiv_rn(p[0], vs); u[1] = __fdiv_rn(p[1], vs); u[2] = __fdiv_rn(p[2], vs);
   const bool ok = u[0] >= (float)(-g.hN) && u[0] < (float)(g.N - g.hN) && u[1] >= (float)(-g.hN) && u[1] < (float)(g.N - g.hN) &&
                   u[2] >= (float)(-g.hNz) && u[2] < (float)(g.Nz - g.hNz);
@@ -511,7 +512,14 @@ struct tslam_octo {
   int logodds;            // 1 = log-odds occupancy (fixed at creation), 0 = hit counter
   OcLo lo;
   int ray_cap;            // ray records per frame: max(max_image_pixels, max_points)
+  // occupancy ESDF of a log-odds map (tslam_octo_esdf_*, tslam_octo_esdf.cu), allocated by the first update
+  void* esdf_mem;         // field, class bytes, neighbour table, epochs, change flags
+  int* esdf_dirty;        // [max_blocks] block updated by k_octo_lo_apply since the last ESDF update; NULL until then
+  int esdf_full_needed;   // the next update recomputes everything (reset, fusion); readers refuse until it has run
+  int esdf_submap;        // submap of the kept field
+  float esdf_D;           // truncation distance of the kept field
 };
+int oc_esdf_free(tslam_octo* m);  // tslam_octo_esdf.cu
 
 // 64-bit max without a return value: RED.E.MAX.64 (atomicMax(unsigned long long*) with an unused result was lowered
 // to ATOMG - a response sector per update, seen as 57 M "L2 ATOM sectors" per textured launch in ncu)

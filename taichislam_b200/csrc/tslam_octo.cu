@@ -358,8 +358,10 @@ __global__ void __launch_bounds__(256) k_octo_lo_walk(OcGrid g, OcLo lo, int s, 
   if ((threadIdx.x & 31) == 0 && visits) atomicAdd(&lo.stats[1], (unsigned long long)visits);
 }
 
-// one CTA (128 threads, 4 voxels each) per touched block
-__global__ void __launch_bounds__(128) k_octo_lo_apply(OcGrid g, OcLo lo) {
+// one CTA (128 threads, 4 voxels each) per touched block.  ESDF: an occupancy ESDF exists, and the block is flagged for
+// its next incremental update (esdf_dirty); without one nothing is marked.
+template <bool ESDF>
+__global__ void __launch_bounds__(128) k_octo_lo_apply(OcGrid g, OcLo lo, int* esdf_dirty) {
   __shared__ uint32_t mk[OC_MARK_WORDS];
   __shared__ unsigned int n_hit, n_upd;
   const int nt = lo.ctr[1];
@@ -373,6 +375,7 @@ __global__ void __launch_bounds__(128) k_octo_lo_apply(OcGrid g, OcLo lo) {
       *w = 0u;
     }
     if (threadIdx.x == 0) lo.touched_flag[blk] = 0;
+    if (ESDF && threadIdx.x == 0) esdf_dirty[blk] = 1;
     __syncthreads();
     unsigned int h = 0, u = 0;
 #pragma unroll
@@ -548,6 +551,7 @@ extern "C" int tslam_octo_destroy(tslam_octo_t* m) {
   if (m->logodds) {
     cudaFree(m->lo.mark); cudaFree(m->lo.touched_flag); cudaFree(m->lo.touched); cudaFree(m->lo.rays); cudaFree(m->lo.stats);
   }
+  oc_esdf_free(m);
   delete m;
   return TSLAM_OK;
 }
@@ -563,6 +567,7 @@ extern "C" int tslam_octo_reset(tslam_octo_t* m, void* stream) {
   if (nb) TS_CUDA(cudaMemsetAsync(m->g.cnt, 0, (size_t)nb * OC_B3 * 4, st));
   if (nb && m->g.cw) TS_CUDA(cudaMemsetAsync(m->g.cw, 0, (size_t)nb * OC_B3 * 8, st));
   TS_CUDA(cudaMemsetAsync(m->scratch_i, 0, 4 * 4, st));
+  m->esdf_full_needed = 1;  // pool slots are recycled: the kept ESDF state no longer describes the map
   return TSLAM_OK;
 }
 
@@ -598,7 +603,10 @@ static int oc_lo_finish(tslam_octo* m, const TsFrame& fr, int n_max, cudaStream_
   k_octo_lo_walk<<<(n_max + 255) / 256, 256, 0, st>>>(m->g, m->lo, fr.submap, m->in.vs, fr.T[0], fr.T[1], fr.T[2]);
   m->launches++;
   TS_CUDA(cudaGetLastError());
-  k_octo_lo_apply<<<m->sm_count * 16, 128, 0, st>>>(m->g, m->lo);
+  if (m->esdf_dirty)
+    k_octo_lo_apply<true><<<m->sm_count * 16, 128, 0, st>>>(m->g, m->lo, m->esdf_dirty);
+  else
+    k_octo_lo_apply<false><<<m->sm_count * 16, 128, 0, st>>>(m->g, m->lo, nullptr);
   m->launches++;
   TS_CUDA(cudaGetLastError());
   return TSLAM_OK;

@@ -162,6 +162,33 @@ class Octomap(BaseMap):
             return np.zeros(len(xyz), bool)
         return self._h.query_near(xyz, int(voxel), submap=self._active())
 
+    # occupancy ESDF (log-odds maps only, DESIGN.md section 7): the interface of DenseTSDF's ESDF
+    def _esdf_map(self):
+        if self.occupancy_model != "logodds":
+            raise ValueError("the occupancy ESDF needs Octomap(..., occupancy_model='logodds'): a hit counter cannot tell "
+                             "free space from unknown space")
+
+    def esdf_update(self, max_dist=None):
+        """Bring the ESDF of the active submap up to date (incremental when possible), truncated at max_dist (default
+        max_ray_length, the TSDF ESDF's far value) -> dict(lower_sweeps, raise_sweeps (-1: full), changed, suspect)."""
+        self._esdf_map()
+        self.esdf_max_dist = float(self.max_ray_length if max_dist is None else max_dist)
+        return self._h.esdf_update(self._active(), self.esdf_max_dist)
+
+    def get_voxels_ESDF(self):
+        """(idx int32[n,3], ESDF f32[n]) of the voxels known at the last esdf_update."""
+        self._esdf_map()
+        return self._h.esdf_gather(self._active())
+
+    def esdf_query(self, xyz, update=True):
+        """Interpolated ESDF and its gradient at points [n,3] of the active submap's map frame: (dist, grad, valid), torch
+        CUDA tensors for a torch tensor, numpy arrays for a numpy array.  update=True first brings the field up to date
+        (with the max_dist of the last esdf_update, else max_ray_length); update=False answers as of the last update."""
+        self._esdf_map()
+        if update:
+            self.esdf_update(getattr(self, "esdf_max_dist", None))
+        return self._h.esdf_query(xyz, submap=self._active())
+
     def saveMap(self, path):  # :201-202 (stub in the reference)
         pass
 

@@ -193,6 +193,57 @@ class OctoHandle:
         capi.check(self.L.tslam_octo_get_stats(self.h, out, int(bool(clear))))
         return dict(zip(("rays", "miss_visits", "hit_voxels", "updated_voxels"), (int(v) for v in out)))
 
+    # -- occupancy ESDF of a log-odds map (tslam_octo_esdf_*, DESIGN.md section 7) ------------------------------------
+    def esdf_update(self, submap=0, max_dist=1.0, full=False):
+        """Bring the ESDF of `submap` up to date, truncated at max_dist (incremental unless full, the last update was for
+        another submap or max_dist, or the map was reset or fused) -> dict(lower_sweeps, raise_sweeps (-1: full
+        recompute), changed, suspect)."""
+        st = np.zeros(4, np.int32)
+        capi.check(self.L.tslam_octo_esdf_update(self.h, int(submap), float(max_dist), 1 if full else 0, capi.np_ptr(st),
+                                                 capi.stream_ptr()))
+        return dict(lower_sweeps=int(st[0]), raise_sweeps=int(st[1]), changed=int(st[2]), suspect=int(st[3]))
+
+    def esdf_gather(self, submap=0, as_torch=False):
+        """(idx int32[n,3], ESDF f32[n]) of the voxels known at the last esdf_update: numpy arrays, or torch CUDA tensors
+        with as_torch."""
+        torch = self.torch
+        dev = torch.device("cuda", torch.cuda.current_device())
+        n = C.c_int64(0)
+        rc = self.L.tslam_octo_esdf_gather(self.h, int(submap), 0, None, None, C.byref(n), capi.stream_ptr())
+        if rc not in (capi.TSLAM_OK, capi.E_CAPACITY):
+            capi.check(rc)
+        cap = int(n.value)
+        idx = torch.empty((max(cap, 1), 3), dtype=torch.int32, device=dev)
+        e = torch.empty(max(cap, 1), dtype=torch.float32, device=dev)
+        capi.check(self.L.tslam_octo_esdf_gather(self.h, int(submap), cap, capi.tptr(idx), capi.tptr(e), C.byref(n),
+                                                 capi.stream_ptr()))
+        k = int(n.value)
+        if as_torch:
+            return idx[:k], e[:k]
+        return idx[:k].cpu().numpy(), e[:k].cpu().numpy()
+
+    def esdf_query(self, xyz, submap=0):
+        """Trilinear ESDF and its exact gradient at points [n,3] of the submap's map frame, as of the last esdf_update:
+        (dist f32[n], grad f32[n,3], valid bool[n]); dist and grad are NaN where valid is False.  A torch CUDA tensor in
+        -> torch CUDA tensors out, without a host synchronisation; a numpy array in -> numpy arrays out."""
+        torch = self.torch
+        as_torch = isinstance(xyz, torch.Tensor)
+        if as_torch:
+            x = xyz.to(device=torch.device("cuda", torch.cuda.current_device()), dtype=torch.float32).contiguous()
+        else:
+            x = torch.from_numpy(np.ascontiguousarray(xyz, dtype=np.float32)).cuda()
+        x = x.reshape(-1, 3)
+        n = x.shape[0]
+        dist = torch.empty(n, dtype=torch.float32, device=x.device)
+        grad = torch.empty((n, 3), dtype=torch.float32, device=x.device)
+        valid = torch.empty(n, dtype=torch.uint8, device=x.device)
+        capi.check(self.L.tslam_octo_esdf_query(self.h, int(submap), n, capi.tptr(x), capi.tptr(dist), capi.tptr(grad),
+                                                capi.tptr(valid), capi.stream_ptr()))
+        valid = valid.view(torch.bool)  # the kernel writes 0 / 1
+        if as_torch:
+            return dist, grad, valid
+        return dist.cpu().numpy(), grad.cpu().numpy(), valid.cpu().numpy()
+
     def raycast(self, pos, direction, max_dist, submap=0):
         torch = self.torch
         p = torch.from_numpy(np.ascontiguousarray(pos, dtype=np.float32)).cuda()

@@ -486,6 +486,31 @@ int tslam_octo_esdf_gather(tslam_octo_t* m, int32_t submap, int64_t cap, int32_t
 int tslam_octo_esdf_query(tslam_octo_t* m, int32_t submap, int64_t n, const float* xyz, float* dist, float* grad, uint8_t* valid,
                           void* stream);
 
+/* ----------------------------------------------------------------------------
+ * Frontiers of a log-odds map (DESIGN.md section 7): per submap, a frontier voxel is a FREE cell (known, L <= l_occ)
+ * with at least one 6-neighbour that is inside the volume and UNKNOWN (not known; every cell of an absent block).
+ * Clusters are the 26-connected components of the frontier voxels, labelled by the smallest linear key
+ * ((i+hN)*N + (j+hN))*Nz + (k+hNz) of their voxels and listed in ascending label order.  Every call refuses a
+ * hit-counter map (TSLAM_E_INVALID).  State (allocated by the first update): 84 B per pool block, plus 8 B per
+ * frontier voxel and 156 B per cluster, grown on demand.
+ * --------------------------------------------------------------------------*/
+/* Bring the frontier set of `submap` up to date.  mode 0: incremental (re-examine the blocks updated since the last
+ * update and their face neighbours) when the last update was for the same submap and no reset or fusion came since,
+ * else full; mode 1: full.  Either gives the same frontier set and records.  stats4 (HOST, may be NULL): frontier
+ * voxels, clusters, blocks re-examined, 1 when the update was full.  Synchronises. */
+int tslam_octo_frontier_update(tslam_octo_t* m, int32_t submap, int32_t mode, int32_t* stats4, void* stream);
+/* (ijk, cluster ordinal) of every frontier voxel of the last update: idx int32[cap,3], cluster int32[cap] (DEVICE);
+ * n_out = the number of frontier voxels (TSLAM_E_CAPACITY when it exceeds cap; the first cap rows are written).
+ * Refused before an update, for another submap than the last update's, and after a reset or fusion until the next
+ * update. */
+int tslam_octo_frontier_gather(tslam_octo_t* m, int32_t submap, int64_t cap, int32_t* idx, int32_t* cluster, int64_t* n_out,
+                               void* stream);
+/* The cluster records of the last update in label order, sixteen int64 each (DEVICE rec16[cap,16]): label, voxels,
+ * sum i, sum j, sum k, min i, min j, min k, max i, max j, max k, faces (voxel / UNKNOWN in-volume 6-neighbour pairs),
+ * the sums of the unit offsets towards those neighbours (x, y, z), 0.  n_out = the number of clusters
+ * (TSLAM_E_CAPACITY when it exceeds cap).  Refused like tslam_octo_frontier_gather. */
+int tslam_octo_frontier_clusters(tslam_octo_t* m, int32_t submap, int64_t cap, int64_t* rec16, int64_t* n_out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -155,6 +155,9 @@ SIGNATURES = {
     "tslam_octo_esdf_update": (C.c_int, [_vp, _i32, _f32, _i32, _vp, _vp]),
     "tslam_octo_esdf_gather": (C.c_int, [_vp, _i32, _i64, _vp, _vp, C.POINTER(_i64), _vp]),
     "tslam_octo_esdf_query": (C.c_int, [_vp, _i32, _i64, _vp, _vp, _vp, _vp, _vp]),
+    "tslam_octo_frontier_update": (C.c_int, [_vp, _i32, _i32, _vp, _vp]),
+    "tslam_octo_frontier_gather": (C.c_int, [_vp, _i32, _i64, _vp, _vp, C.POINTER(_i64), _vp]),
+    "tslam_octo_frontier_clusters": (C.c_int, [_vp, _i32, _i64, _vp, C.POINTER(_i64), _vp]),
 }
 
 _lib = None

@@ -518,8 +518,25 @@ struct tslam_octo {
   int esdf_full_needed;   // the next update recomputes everything (reset, fusion); readers refuse until it has run
   int esdf_submap;        // submap of the kept field
   float esdf_D;           // truncation distance of the kept field
+  // frontier tracker of a log-odds map (tslam_octo_frontier_*, tslam_octo_frontier.cu), allocated by the first update
+  void* fr_mem;           // per pool block: frontier mask, dirty and region flags, region list, popcount, offset (84 B)
+  int* fr_dirty;          // [max_blocks] block updated by k_octo_lo_apply since the last frontier update; NULL until then
+  int fr_full_needed;     // the next update recomputes everything (reset, fusion); readers refuse until it has run
+  int fr_submap;          // submap of the kept frontier set
+  int fr_nb;              // pool blocks the last update saw
+  int fr_n, fr_nc;        // frontier voxels and clusters of the last update
+  void* fr_vox;           // per frontier voxel: union-find parent, cluster slot of a root (grown on demand)
+  long long fr_vox_cap;
+  void* fr_clu;           // per cluster: label, record, sort keys / values, ordinal (grown on demand)
+  long long fr_clu_cap;
+  void* fr_tmp;           // CUB scan / sort scratch
+  size_t fr_tmp_bytes;
 };
-int oc_esdf_free(tslam_octo* m);  // tslam_octo_esdf.cu
+int oc_esdf_free(tslam_octo* m);      // tslam_octo_esdf.cu
+int oc_frontier_free(tslam_octo* m);  // tslam_octo_frontier.cu
+// k_octo_lo_apply flags the blocks it updates for these change trackers (tslam_octo.cu)
+#define OC_TRACK_ESDF 1u
+#define OC_TRACK_FRONTIER 2u
 
 // 64-bit max without a return value: RED.E.MAX.64 (atomicMax(unsigned long long*) with an unused result was lowered
 // to ATOMG - a response sector per update, seen as 57 M "L2 ATOM sectors" per textured launch in ncu)

@@ -358,10 +358,11 @@ __global__ void __launch_bounds__(256) k_octo_lo_walk(OcGrid g, OcLo lo, int s, 
   if ((threadIdx.x & 31) == 0 && visits) atomicAdd(&lo.stats[1], (unsigned long long)visits);
 }
 
-// one CTA (128 threads, 4 voxels each) per touched block.  ESDF: an occupancy ESDF exists, and the block is flagged for
-// its next incremental update (esdf_dirty); without one nothing is marked.
-template <bool ESDF>
-__global__ void __launch_bounds__(128) k_octo_lo_apply(OcGrid g, OcLo lo, int* esdf_dirty) {
+// one CTA (128 threads, 4 voxels each) per touched block.  TRACK names the change trackers that exist (OC_TRACK_ESDF:
+// an occupancy ESDF, OC_TRACK_FRONTIER: a frontier tracker); the block is flagged for the next incremental update of
+// each (esdf_dirty, fr_dirty).  Without a tracker nothing is marked.
+template <unsigned TRACK>
+__global__ void __launch_bounds__(128) k_octo_lo_apply(OcGrid g, OcLo lo, int* esdf_dirty, int* fr_dirty) {
   __shared__ uint32_t mk[OC_MARK_WORDS];
   __shared__ unsigned int n_hit, n_upd;
   const int nt = lo.ctr[1];
@@ -375,7 +376,8 @@ __global__ void __launch_bounds__(128) k_octo_lo_apply(OcGrid g, OcLo lo, int* e
       *w = 0u;
     }
     if (threadIdx.x == 0) lo.touched_flag[blk] = 0;
-    if (ESDF && threadIdx.x == 0) esdf_dirty[blk] = 1;
+    if ((TRACK & OC_TRACK_ESDF) && threadIdx.x == 0) esdf_dirty[blk] = 1;
+    if ((TRACK & OC_TRACK_FRONTIER) && threadIdx.x == 0) fr_dirty[blk] = 1;
     __syncthreads();
     unsigned int h = 0, u = 0;
 #pragma unroll
@@ -552,6 +554,7 @@ extern "C" int tslam_octo_destroy(tslam_octo_t* m) {
     cudaFree(m->lo.mark); cudaFree(m->lo.touched_flag); cudaFree(m->lo.touched); cudaFree(m->lo.rays); cudaFree(m->lo.stats);
   }
   oc_esdf_free(m);
+  oc_frontier_free(m);
   delete m;
   return TSLAM_OK;
 }
@@ -568,6 +571,7 @@ extern "C" int tslam_octo_reset(tslam_octo_t* m, void* stream) {
   if (nb && m->g.cw) TS_CUDA(cudaMemsetAsync(m->g.cw, 0, (size_t)nb * OC_B3 * 8, st));
   TS_CUDA(cudaMemsetAsync(m->scratch_i, 0, 4 * 4, st));
   m->esdf_full_needed = 1;  // pool slots are recycled: the kept ESDF state no longer describes the map
+  m->fr_full_needed = 1;    // ... nor the kept frontier set
   return TSLAM_OK;
 }
 
@@ -603,10 +607,16 @@ static int oc_lo_finish(tslam_octo* m, const TsFrame& fr, int n_max, cudaStream_
   k_octo_lo_walk<<<(n_max + 255) / 256, 256, 0, st>>>(m->g, m->lo, fr.submap, m->in.vs, fr.T[0], fr.T[1], fr.T[2]);
   m->launches++;
   TS_CUDA(cudaGetLastError());
-  if (m->esdf_dirty)
-    k_octo_lo_apply<true><<<m->sm_count * 16, 128, 0, st>>>(m->g, m->lo, m->esdf_dirty);
+  const unsigned track = (m->esdf_dirty ? OC_TRACK_ESDF : 0u) | (m->fr_dirty ? OC_TRACK_FRONTIER : 0u);
+  const int grid = m->sm_count * 16;
+  if (track == 0u)
+    k_octo_lo_apply<0u><<<grid, 128, 0, st>>>(m->g, m->lo, nullptr, nullptr);
+  else if (track == OC_TRACK_ESDF)
+    k_octo_lo_apply<OC_TRACK_ESDF><<<grid, 128, 0, st>>>(m->g, m->lo, m->esdf_dirty, nullptr);
+  else if (track == OC_TRACK_FRONTIER)
+    k_octo_lo_apply<OC_TRACK_FRONTIER><<<grid, 128, 0, st>>>(m->g, m->lo, nullptr, m->fr_dirty);
   else
-    k_octo_lo_apply<false><<<m->sm_count * 16, 128, 0, st>>>(m->g, m->lo, nullptr);
+    k_octo_lo_apply<OC_TRACK_ESDF | OC_TRACK_FRONTIER><<<grid, 128, 0, st>>>(m->g, m->lo, m->esdf_dirty, m->fr_dirty);
   m->launches++;
   TS_CUDA(cudaGetLastError());
   return TSLAM_OK;

@@ -189,6 +189,41 @@ class Octomap(BaseMap):
             self.esdf_update(getattr(self, "esdf_max_dist", None))
         return self._h.esdf_query(xyz, submap=self._active())
 
+    # exploration frontiers (log-odds maps only, DESIGN.md section 7): FREE voxels next to in-volume UNKNOWN space
+    def _frontier_map(self):
+        if self.occupancy_model != "logodds":
+            raise ValueError("frontiers need Octomap(..., occupancy_model='logodds'): a hit counter cannot tell free space "
+                             "from unknown space")
+
+    def frontier_update(self, full=False):
+        """Bring the frontier set of the active submap up to date (incremental when possible) -> dict(voxels, clusters,
+        blocks (re-examined), full)."""
+        self._frontier_map()
+        return self._h.frontier_update(self._active(), full=full)
+
+    def get_frontiers(self):
+        """(idx int32[n,3], cluster int32[n]) of the frontier voxels at the last frontier_update; cluster indexes the
+        arrays of get_frontier_clusters(min_voxels=1)."""
+        self._frontier_map()
+        return self._h.frontier_gather(self._active())
+
+    def get_frontier_clusters(self, min_voxels=1):
+        """The frontier clusters of the last frontier_update with at least min_voxels voxels, in label order, as numpy
+        arrays: label, size, faces (voxel / UNKNOWN-neighbour pairs), centroid [n,3], bbox_min / bbox_max [n,3] (cell
+        centres in metres of the submap frame, f64 of cell index * f32(constructor voxel_scale)) and direction [n,3]
+        (the unit mean direction into unknown space, 0 where the offsets cancel)."""
+        self._frontier_map()
+        rec = self._h.frontier_clusters(self._active())
+        rec = rec[rec[:, 1] >= int(min_voxels)]
+        vs = float(np.float32(self._h.cfg.voxel_scale))
+        size = rec[:, 1]
+        d = rec[:, 12:15].astype(np.float64)
+        norm = np.linalg.norm(d, axis=1, keepdims=True)
+        return dict(label=rec[:, 0].copy(), size=size.copy(), faces=rec[:, 11].copy(),
+                    centroid=rec[:, 2:5].astype(np.float64) / np.maximum(size, 1)[:, None] * vs,
+                    bbox_min=rec[:, 5:8].astype(np.float64) * vs, bbox_max=rec[:, 8:11].astype(np.float64) * vs,
+                    direction=np.divide(d, norm, out=np.zeros_like(d), where=norm > 0))
+
     def saveMap(self, path):  # :201-202 (stub in the reference)
         pass
 

@@ -244,6 +244,48 @@ class OctoHandle:
             return dist, grad, valid
         return dist.cpu().numpy(), grad.cpu().numpy(), valid.cpu().numpy()
 
+    # -- frontiers of a log-odds map (tslam_octo_frontier_*, DESIGN.md section 7) --------------------------------------
+    def frontier_update(self, submap=0, full=False):
+        """Bring the frontier set of `submap` up to date (incremental unless full, the last update was for another submap,
+        or the map was reset or fused) -> dict(voxels, clusters, blocks (re-examined), full (bool))."""
+        st = np.zeros(4, np.int32)
+        capi.check(self.L.tslam_octo_frontier_update(self.h, int(submap), 1 if full else 0, capi.np_ptr(st), capi.stream_ptr()))
+        return dict(voxels=int(st[0]), clusters=int(st[1]), blocks=int(st[2]), full=bool(st[3]))
+
+    def frontier_gather(self, submap=0, as_torch=False):
+        """(idx int32[n,3], cluster int32[n]) of the frontier voxels of the last frontier_update; cluster is the ordinal in
+        frontier_clusters.  numpy arrays, or torch CUDA tensors with as_torch."""
+        torch = self.torch
+        dev = torch.device("cuda", torch.cuda.current_device())
+        n = C.c_int64(0)
+        rc = self.L.tslam_octo_frontier_gather(self.h, int(submap), 0, None, None, C.byref(n), capi.stream_ptr())
+        if rc not in (capi.TSLAM_OK, capi.E_CAPACITY):
+            capi.check(rc)
+        cap = int(n.value)
+        idx = torch.empty((max(cap, 1), 3), dtype=torch.int32, device=dev)
+        cl = torch.empty(max(cap, 1), dtype=torch.int32, device=dev)
+        capi.check(self.L.tslam_octo_frontier_gather(self.h, int(submap), cap, capi.tptr(idx), capi.tptr(cl), C.byref(n),
+                                                     capi.stream_ptr()))
+        k = int(n.value)
+        if as_torch:
+            return idx[:k], cl[:k]
+        return idx[:k].cpu().numpy(), cl[:k].cpu().numpy()
+
+    def frontier_clusters(self, submap=0, as_torch=False):
+        """int64[n,16] cluster records of the last frontier_update in label order (label, voxels, sum i / j / k, min i / j
+        / k, max i / j / k, faces, sum of the unit offsets towards UNKNOWN x / y / z, 0)."""
+        torch = self.torch
+        dev = torch.device("cuda", torch.cuda.current_device())
+        n = C.c_int64(0)
+        rc = self.L.tslam_octo_frontier_clusters(self.h, int(submap), 0, None, C.byref(n), capi.stream_ptr())
+        if rc not in (capi.TSLAM_OK, capi.E_CAPACITY):
+            capi.check(rc)
+        cap = int(n.value)
+        rec = torch.empty((max(cap, 1), 16), dtype=torch.int64, device=dev)
+        capi.check(self.L.tslam_octo_frontier_clusters(self.h, int(submap), cap, capi.tptr(rec), C.byref(n), capi.stream_ptr()))
+        k = int(n.value)
+        return rec[:k] if as_torch else rec[:k].cpu().numpy()
+
     def raycast(self, pos, direction, max_dist, submap=0):
         torch = self.torch
         p = torch.from_numpy(np.ascontiguousarray(pos, dtype=np.float32)).cuda()

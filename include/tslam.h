@@ -511,6 +511,35 @@ int tslam_octo_frontier_gather(tslam_octo_t* m, int32_t submap, int64_t cap, int
  * (TSLAM_E_CAPACITY when it exceeds cap).  Refused like tslam_octo_frontier_gather. */
 int tslam_octo_frontier_clusters(tslam_octo_t* m, int32_t submap, int64_t cap, int64_t* rec16, int64_t* n_out, void* stream);
 
+/* ----------------------------------------------------------------------------
+ * Viewpoint gain of a log-odds map (DESIGN.md section 7): what a depth camera would see from each of n candidate views
+ * of `submap`.  A view is a position pos[3] and a row-major rotation R9[9] in the submap's map frame, with the
+ * convention of integrate_depth's R, T (camera x right, y down, z forward).  A view is valid iff its 12 numbers are
+ * finite and its cell round_half_away(pos / voxel_scale) is inside the volume and FREE; an invalid view gets valid = 0
+ * and zero in every output.  Arrays are DEVICE, n == 0 is a no-op.  Neither call changes the map or any tracker state.
+ * Both refuse (TSLAM_E_INVALID) a NULL handle or camera, n < 0, NULL arrays when n > 0, a hit-counter map, fx, fy or
+ * max_range not finite and > 0, non-finite cx or cy, width, height or step not > 0, width / step or height / step
+ * rounding down to 0, and a camera whose farthest ray spans more than 2^22 cells.
+ * --------------------------------------------------------------------------*/
+typedef struct tslam_view_camera {
+  float fx, fy, cx, cy;          /* pinhole intrinsics of the simulated depth camera                        */
+  int32_t width, height, step;   /* image size; rays at pixels (ii * step, jj * step), ii < width / step    */
+  float max_range;               /* every simulated pixel lies beyond it: rays are cut at depth max_range    */
+} tslam_view_camera_t;
+/* Unknown gain: gain[v] (int64) = the number of distinct UNKNOWN cells among the cells the view's rays see - each ray
+ * walks integrate_depth's path of an all-far pixel up to its first OCC cell; out-of-volume cells are skipped.
+ * Asynchronous: a walk that leaves its view's bitmap window (only possible when R is not a rotation) is reported as
+ * TSLAM_E_INVALID by the next synchronising call (tslam_octo_sync). */
+int tslam_octo_view_gain_unknown(tslam_octo_t* m, int32_t submap, int64_t n, const float* pos, const float* R9,
+                                 const tslam_view_camera_t* cam, uint8_t* valid, int64_t* gain, void* stream);
+/* Frontier gain: the frontier voxels of the last tslam_octo_frontier_update inside the view's frustum whose line of sight
+ * from the view crosses FREE cells only (classes as of the call).  per_cluster[v * n_clusters + c] (int32, may be NULL)
+ * counts them per cluster ordinal, total[v] is the row sum.  Also refused where tslam_octo_frontier_gather is, and when
+ * n_clusters differs from the last update's cluster count. */
+int tslam_octo_view_gain_frontier(tslam_octo_t* m, int32_t submap, int64_t n, const float* pos, const float* R9,
+                                  const tslam_view_camera_t* cam, int64_t n_clusters, uint8_t* valid, int32_t* total,
+                                  int32_t* per_cluster, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

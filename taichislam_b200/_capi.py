@@ -49,6 +49,12 @@ class OctoConfig(C.Structure):
                 ("max_image_pixels", C.c_int32), ("max_points", C.c_int32), ("texture_enabled", C.c_int32)]
 
 
+class ViewCamera(C.Structure):
+    """tslam_view_camera_t: the simulated depth camera of the viewpoint-gain calls."""
+    _fields_ = [("fx", C.c_float), ("fy", C.c_float), ("cx", C.c_float), ("cy", C.c_float), ("width", C.c_int32),
+                ("height", C.c_int32), ("step", C.c_int32), ("max_range", C.c_float)]
+
+
 _vp, _i32, _i64, _f32 = C.c_void_p, C.c_int32, C.c_int64, C.c_float
 
 # name -> (restype, argtypes).  Every symbol declared in include/tslam.h appears here
@@ -158,6 +164,8 @@ SIGNATURES = {
     "tslam_octo_frontier_update": (C.c_int, [_vp, _i32, _i32, _vp, _vp]),
     "tslam_octo_frontier_gather": (C.c_int, [_vp, _i32, _i64, _vp, _vp, C.POINTER(_i64), _vp]),
     "tslam_octo_frontier_clusters": (C.c_int, [_vp, _i32, _i64, _vp, C.POINTER(_i64), _vp]),
+    "tslam_octo_view_gain_unknown": (C.c_int, [_vp, _i32, _i64, _vp, _vp, C.POINTER(ViewCamera), _vp, _vp, _vp]),
+    "tslam_octo_view_gain_frontier": (C.c_int, [_vp, _i32, _i64, _vp, _vp, C.POINTER(ViewCamera), _i64, _vp, _vp, _vp, _vp]),
 }
 
 _lib = None

@@ -531,9 +531,55 @@ struct tslam_octo {
   long long fr_clu_cap;
   void* fr_tmp;           // CUB scan / sort scratch
   size_t fr_tmp_bytes;
+  // viewpoint gain (tslam_octo_view_gain_*, tslam_octo_view.cu): per-view bitmaps of a chunk of views, or the frontier
+  // rows of the frontier gain (grown on demand, freed by tslam_octo_destroy)
+  void* vw_mem;
+  size_t vw_bytes;
 };
 int oc_esdf_free(tslam_octo* m);      // tslam_octo_esdf.cu
 int oc_frontier_free(tslam_octo* m);  // tslam_octo_frontier.cu
+int oc_view_free(tslam_octo* m);      // tslam_octo_view.cu
+// tslam_octo_frontier.cu: the frontier set of `submap` can be read (an update for it has completed and no reset or fusion
+// came since; refused like tslam_octo_frontier_gather, the message naming `what`) ...
+int oc_frontier_readable(tslam_octo* m, int32_t submap, const char* what);
+// ... and its m->fr_n rows (ijk, cluster ordinal) into idx[fr_n * 3], cluster[fr_n] (DEVICE), in compact order, on st
+int oc_frontier_rows(tslam_octo* m, int32_t* idx, int32_t* cluster, cudaStream_t st);
+#define OC_ERR_VIEW_WINDOW 16  // g.err: a viewpoint-gain walk left its view's bitmap window (tslam_octo_view.cu)
+
+// Amanatides-Woo traversal of the log-odds map in voxel units (DESIGN.md section 7, "Traversal"): p0 = origin / vs,
+// p1 = endpoint / vs, cells c = round_half_away(p).  The k-th boundary crossing of axis a is at
+// t = ((c_a + 0.5 s_a) - p0_a) * (1 / (p1_a - p0_a)), recomputed from the current cell (no accumulated increments); each
+// step takes the axis with the smallest t among those with steps left, ties to the lower axis.  The step counts
+// |c1 - c0| per axis are integers, so the path always has |c1 - c0|_1 + 1 cells.  The viewpoint-gain kernels walk with
+// it; k_octo_lo_walk (tslam_octo.cu) spells out the same expressions, because calling the helper there changes that
+// kernel's SASS (the step becomes a jump table).  The gain tests check the two paths agree bit for bit.
+struct OcWalk {
+  int cx, cy, cz;   // current cell
+  int lx, ly, lz;   // steps left per axis
+  int sx, sy, sz;   // step direction per axis
+  float p0x, p0y, p0z, hx, hy, hz, ix, iy, iz, tx, ty, tz;
+};
+__device__ __forceinline__ void oc_walk_begin(OcWalk& w, float p0x, float p0y, float p0z, float p1x, float p1y, float p1z) {
+  w.p0x = p0x; w.p0y = p0y; w.p0z = p0z;
+  w.cx = (int)roundf(p0x); w.cy = (int)roundf(p0y); w.cz = (int)roundf(p0z);
+  const int ex = (int)roundf(p1x), ey = (int)roundf(p1y), ez = (int)roundf(p1z);
+  w.lx = abs(ex - w.cx); w.ly = abs(ey - w.cy); w.lz = abs(ez - w.cz);
+  w.sx = ex > w.cx ? 1 : -1; w.sy = ey > w.cy ? 1 : -1; w.sz = ez > w.cz ? 1 : -1;
+  w.hx = 0.5f * (float)w.sx; w.hy = 0.5f * (float)w.sy; w.hz = 0.5f * (float)w.sz;
+  w.ix = w.lx ? 1.0f / (p1x - p0x) : 0.0f; w.iy = w.ly ? 1.0f / (p1y - p0y) : 0.0f; w.iz = w.lz ? 1.0f / (p1z - p0z) : 0.0f;
+  w.tx = (((float)w.cx + w.hx) - p0x) * w.ix; w.ty = (((float)w.cy + w.hy) - p0y) * w.iy; w.tz = (((float)w.cz + w.hz) - p0z) * w.iz;
+}
+// one step to the next cell of the path; only while steps are left (lx + ly + lz > 0)
+__device__ __forceinline__ void oc_walk_step(OcWalk& w) {
+  int a = 3;
+  float tb = 0.0f;
+  if (w.lx > 0) { a = 0; tb = w.tx; }
+  if (w.ly > 0 && (a == 3 || w.ty < tb)) { a = 1; tb = w.ty; }
+  if (w.lz > 0 && (a == 3 || w.tz < tb)) a = 2;
+  if (a == 0) { w.cx += w.sx; --w.lx; w.tx = (((float)w.cx + w.hx) - w.p0x) * w.ix; }
+  else if (a == 1) { w.cy += w.sy; --w.ly; w.ty = (((float)w.cy + w.hy) - w.p0y) * w.iy; }
+  else { w.cz += w.sz; --w.lz; w.tz = (((float)w.cz + w.hz) - w.p0z) * w.iz; }
+}
 // k_octo_lo_apply flags the blocks it updates for these change trackers (tslam_octo.cu)
 #define OC_TRACK_ESDF 1u
 #define OC_TRACK_FRONTIER 2u

@@ -313,6 +313,8 @@ __global__ void __launch_bounds__(256) k_octo_lo_points(OcGrid g, OcLo lo, const
 // crossing of axis a is at t = ((c_a + 0.5 s_a) - p0_a) * (1 / (p1_a - p0_a)), recomputed from the current cell (no
 // accumulated increments); each step takes the axis with the smallest t among those with steps left, ties to the
 // lower axis.  The step counts |c1 - c0| per axis are integers, so the path always has |c1 - c0|_1 + 1 cells.
+// The viewpoint-gain kernels walk the same path through oc_walk_begin / oc_walk_step (tslam_internal.cuh); this kernel
+// keeps its own copy because the helper changes its SASS (a jump table for the step), checked bit for bit instead.
 __global__ void __launch_bounds__(256) k_octo_lo_walk(OcGrid g, OcLo lo, int s, float vs, float ox, float oy, float oz) {
   const int n = lo.ctr[0];
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
@@ -555,6 +557,7 @@ extern "C" int tslam_octo_destroy(tslam_octo_t* m) {
   }
   oc_esdf_free(m);
   oc_frontier_free(m);
+  oc_view_free(m);
   delete m;
   return TSLAM_OK;
 }
@@ -628,6 +631,10 @@ static int oc_deferred(tslam_octo* m) {
   if (err) {
     int zero = 0;
     cudaMemcpy(m->g.err, &zero, 4, cudaMemcpyHostToDevice);
+    if (err == OC_ERR_VIEW_WINDOW) {
+      ts_set_error("octo view gain: a walk left its view's bitmap window (is every view's R a rotation?): gains are invalid");
+      return TSLAM_E_INVALID;
+    }
     ts_set_error("octomap block pool / table exhausted (max_blocks=%d, flags 0x%x): hits were dropped", m->g.max_blocks, err);
     return TSLAM_E_POOL_FULL;
   }

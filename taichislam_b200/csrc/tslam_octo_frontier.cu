@@ -451,6 +451,8 @@ static int of_readable(tslam_octo* m, int32_t submap, const char* what) {
   return TSLAM_OK;
 }
 
+int oc_frontier_readable(tslam_octo* m, int32_t submap, const char* what) { return of_readable(m, submap, what); }
+
 static int of_grid(long long work, int per_cta, int cap) {
   const long long g = (work + per_cta - 1) / per_cta;
   return (int)(g < 1 ? 1 : (g > cap ? cap : g));
@@ -528,6 +530,15 @@ extern "C" int tslam_octo_frontier_update(tslam_octo_t* m, int32_t submap, int32
   m->fr_n = n;
   m->fr_nc = nc;
   if (stats4) { stats4[0] = n; stats4[1] = nc; stats4[2] = region; stats4[3] = full ? 1 : 0; }
+  return TSLAM_OK;
+}
+
+int oc_frontier_rows(tslam_octo* m, int32_t* idx, int32_t* cluster, cudaStream_t st) {
+  if (m->fr_n > 0) {
+    k_octo_frontier_gather<<<of_grid(m->fr_nb, 8, m->sm_count * 16), 256, 0, st>>>(m->g, of_aux(m), of_vox(m), of_clu(m), m->fr_nb,
+                                                                                   m->fr_n, idx, cluster);
+    TS_LAUNCH_CHECK(m);
+  }
   return TSLAM_OK;
 }
 

@@ -224,6 +224,31 @@ class Octomap(BaseMap):
                     bbox_min=rec[:, 5:8].astype(np.float64) * vs, bbox_max=rec[:, 8:11].astype(np.float64) * vs,
                     direction=np.divide(d, norm, out=np.zeros_like(d), where=norm > 0))
 
+    def view_gain(self, pos, R, width, height, step=None, max_range=None, frontier=True, update=True):
+        """What a depth camera would see from n candidate views of the active submap (positions pos [n,3], rotations R
+        [n,3,3] in its map frame, integrate_depth's convention) -> dict(valid, unknown, frontier, frontier_per_cluster):
+        the distinct UNKNOWN voxels an all-far frame would observe, and the frontier voxels in view with a FREE line of
+        sight, in total and per cluster (frontier=False leaves both None).  The camera is the depth intrinsics with a
+        width x height image; step and max_range default to recast_step and max_ray_length.  update=True first runs
+        frontier_update(), so frontiers and classes agree.  Torch CUDA tensors in -> torch tensors out; numpy -> numpy."""
+        if self.occupancy_model != "logodds":
+            raise ValueError("a viewpoint gain needs Octomap(..., occupancy_model='logodds'): a hit counter cannot tell free "
+                             "space from unknown space")
+        if self.K_cam_dep is None:
+            raise ValueError("view_gain needs the depth intrinsics: call set_dep_camera_intrinsic first")
+        K = self.K_cam_dep
+        cam = dict(fx=K[0], fy=K[4], cx=K[2], cy=K[5], width=int(width), height=int(height),
+                   step=int(self.recast_step if step is None else step),
+                   max_range=float(self.max_ray_length if max_range is None else max_range))
+        s = self._active()
+        out = dict(frontier=None, frontier_per_cluster=None)
+        if frontier and update:
+            self.frontier_update()
+        out["valid"], out["unknown"] = self._h.view_gain_unknown(pos, R, cam, submap=s)
+        if frontier:
+            _, out["frontier"], out["frontier_per_cluster"] = self._h.view_gain_frontier(pos, R, cam, submap=s)
+        return out
+
     def saveMap(self, path):  # :201-202 (stub in the reference)
         pass
 

@@ -286,6 +286,70 @@ class OctoHandle:
         k = int(n.value)
         return rec[:k] if as_torch else rec[:k].cpu().numpy()
 
+    # -- viewpoint gain of a log-odds map (tslam_octo_view_gain_*, DESIGN.md section 7) ------------------------------
+    @staticmethod
+    def view_camera(cam):
+        """tslam_view_camera_t from a mapping with fx, fy, cx, cy, width, height, step, max_range."""
+        return capi.ViewCamera(float(cam["fx"]), float(cam["fy"]), float(cam["cx"]), float(cam["cy"]), int(cam["width"]),
+                               int(cam["height"]), int(cam["step"]), float(cam["max_range"]))
+
+    def _views(self, pos, R):
+        """(as_torch, pos f32 [n,3], R f32 [n,9]) as contiguous CUDA tensors"""
+        torch = self.torch
+        as_torch = isinstance(pos, torch.Tensor)
+        dev = torch.device("cuda", torch.cuda.current_device())
+        if as_torch:
+            p = pos.to(device=dev, dtype=torch.float32).reshape(-1, 3).contiguous()
+            r = R.to(device=dev, dtype=torch.float32).reshape(-1, 9).contiguous()
+        else:
+            p = torch.from_numpy(np.ascontiguousarray(np.asarray(pos, np.float32).reshape(-1, 3))).to(dev)
+            r = torch.from_numpy(np.ascontiguousarray(np.asarray(R, np.float32).reshape(-1, 9))).to(dev)
+        assert p.shape[0] == r.shape[0], "pos [n,3] and R [n,3,3] need the same n"
+        return as_torch, p, r
+
+    def view_gain_unknown(self, pos, R, cam, submap=0):
+        """Unknown gain of n views (positions pos [n,3], rotations R [n,3,3], camera `cam` as in view_camera) -> (valid
+        bool[n], gain int64[n]): the distinct UNKNOWN voxels an all-far depth frame from each view would see up to the
+        first occupied voxel of each ray.  Torch CUDA tensors in -> torch tensors out without a host synchronisation (a
+        walk outside its view's window is then reported by the next sync()); numpy in -> numpy out."""
+        torch = self.torch
+        as_torch, p, r = self._views(pos, R)
+        n = p.shape[0]
+        valid = torch.empty(n, dtype=torch.uint8, device=p.device)
+        gain = torch.empty(n, dtype=torch.int64, device=p.device)
+        c = self.view_camera(cam)
+        capi.check(self.L.tslam_octo_view_gain_unknown(self.h, int(submap), n, capi.tptr(p), capi.tptr(r), C.byref(c), capi.tptr(valid),
+                                                       capi.tptr(gain), capi.stream_ptr()))
+        valid = valid.view(torch.bool)
+        if as_torch:
+            return valid, gain
+        self.sync()
+        return valid.cpu().numpy(), gain.cpu().numpy()
+
+    def view_gain_frontier(self, pos, R, cam, submap=0):
+        """Frontier gain of n views against the frontier set of the last frontier_update -> (valid bool[n], total int32[n],
+        per_cluster int32[n, clusters]): the frontier voxels in each view's frustum whose line of sight crosses FREE voxels
+        only, per cluster ordinal (the rows of frontier_clusters).  Torch in -> torch out, numpy in -> numpy out."""
+        torch = self.torch
+        as_torch, p, r = self._views(pos, R)
+        n = p.shape[0]
+        nc = C.c_int64(0)
+        rc = self.L.tslam_octo_frontier_clusters(self.h, int(submap), 0, None, C.byref(nc), capi.stream_ptr())
+        if rc not in (capi.TSLAM_OK, capi.E_CAPACITY):
+            capi.check(rc)
+        nc = int(nc.value)
+        valid = torch.empty(n, dtype=torch.uint8, device=p.device)
+        total = torch.empty(n, dtype=torch.int32, device=p.device)
+        per = torch.empty((n, nc), dtype=torch.int32, device=p.device)
+        c = self.view_camera(cam)
+        capi.check(self.L.tslam_octo_view_gain_frontier(self.h, int(submap), n, capi.tptr(p), capi.tptr(r), C.byref(c), nc,
+                                                        capi.tptr(valid), capi.tptr(total), capi.tptr(per) if nc else None,
+                                                        capi.stream_ptr()))
+        valid = valid.view(torch.bool)
+        if as_torch:
+            return valid, total, per
+        return valid.cpu().numpy(), total.cpu().numpy(), per.cpu().numpy()
+
     def raycast(self, pos, direction, max_dist, submap=0):
         torch = self.torch
         p = torch.from_numpy(np.ascontiguousarray(pos, dtype=np.float32)).cuda()

@@ -540,6 +540,38 @@ int tslam_octo_view_gain_frontier(tslam_octo_t* m, int32_t submap, int64_t n, co
                                   const tslam_view_camera_t* cam, int64_t n_clusters, uint8_t* valid, int32_t* total,
                                   int32_t* per_cluster, void* stream);
 
+/* ----------------------------------------------------------------------------
+ * Travel cost on a log-odds map (DESIGN.md section 7): per submap, as of one update, the geodesic cost G from a start
+ * cell through known free space.  A cell is traversable iff it is inside the volume and FREE (known, L <= l_occ), and,
+ * when clearance > 0, was FREE at the last tslam_octo_esdf_update of the submap, in a block that update saw, with ESDF
+ * value >= clearance.  Steps join 26-neighbours at the ESDF's f32 edge costs vs * {1, sqrtf(2), sqrtf(3)} and are
+ * allowed iff every cell of the box their two cells span is traversable (no corner cutting).  G(start) = 0 when the
+ * start cell round_half_away(start / voxel_scale) is traversable; every other cell holds the least f32 path sum, added
+ * one step at a time; a cell above max_cost is unreachable (+inf).  Every call refuses a hit-counter map and a submap out
+ * of range (TSLAM_E_INVALID).  State (allocated by the first update): 2224 B per pool block.
+ * --------------------------------------------------------------------------*/
+/* Compute the field of `submap` from start3 (HOST, finite).  clearance finite and >= 0 (> 0 needs a readable occupancy
+ * ESDF of the submap whose max_dist is >= clearance); max_cost finite, > 0 and <= 2^22 * vs.  A start that is not
+ * traversable is not an error: start_ok = 0 and nothing is reachable.  stats4 (HOST, may be NULL): reachable cells,
+ * sweeps, traversable cells, start_ok.  A wave still changing after the last sweep is refused, and so are the readers
+ * until the next update.  Synchronises. */
+int tslam_octo_travel_update(tslam_octo_t* m, int32_t submap, const float* start3, float clearance, float max_cost,
+                             int32_t* stats4, void* stream);
+/* (ijk, G) of every reachable cell: idx int32[cap,3], cost f32[cap] (DEVICE); n_out = the number of such cells
+ * (TSLAM_E_CAPACITY when it exceeds cap).  Refused before an update, for another submap than the last update's, and
+ * after a reset or fusion until the next update.  Synchronises. */
+int tslam_octo_travel_gather(tslam_octo_t* m, int32_t submap, int64_t cap, int32_t* idx, float* cost, int64_t* n_out,
+                             void* stream);
+/* cost f32[n] = G of the cell of xyz[n,3] as of the last update; +inf where unreachable, outside the volume, in a block
+ * newer than the update, or not finite (DEVICE, asynchronous, n == 0 a no-op).  Refused like tslam_octo_travel_gather. */
+int tslam_octo_travel_query(tslam_octo_t* m, int32_t submap, int64_t n, const float* xyz, float* cost, void* stream);
+/* Path from the cell of each target xyz[n,3] to the start: cells int32[n,max_len,3] target -> start, each cell's
+ * predecessor being the reachable 26-neighbour with an allowed step and G(h) + c == G(v), smallest G(h), ties to the
+ * first in dx, dy, dz = -1, 0, 1 order (dx outermost); len int32[n] = the full number of cells, 0 when unreachable (only
+ * the first max_len are written).  max_len >= 1.  DEVICE, asynchronous.  Refused like tslam_octo_travel_gather. */
+int tslam_octo_travel_path(tslam_octo_t* m, int32_t submap, int64_t n, const float* xyz, int32_t max_len, int32_t* cells,
+                           int32_t* len, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

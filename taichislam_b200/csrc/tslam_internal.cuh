@@ -535,16 +535,33 @@ struct tslam_octo {
   // rows of the frontier gain (grown on demand, freed by tslam_octo_destroy)
   void* vw_mem;
   size_t vw_bytes;
+  // travel-cost field of a log-odds map (tslam_octo_travel_*, tslam_octo_travel.cu), allocated by the first update
+  void* tr_mem;           // per pool block: cost field, traversable bits, neighbour table, epoch (2224 B)
+  int tr_ready;           // the kept field can be read (an update completed; cleared by reset, fusion, a failed update)
+  int tr_submap;          // submap of the kept field
 };
 int oc_esdf_free(tslam_octo* m);      // tslam_octo_esdf.cu
 int oc_frontier_free(tslam_octo* m);  // tslam_octo_frontier.cu
 int oc_view_free(tslam_octo* m);      // tslam_octo_view.cu
+int oc_travel_free(tslam_octo* m);    // tslam_octo_travel.cu
+// tslam_octo_esdf.cu: the occupancy ESDF of `submap` as of its last update, for the clearance test of the travel-cost
+// field.  Refused like tslam_octo_esdf_gather (the message naming `what`).  A voxel at pool offset o was FREE at that
+// update, in a block it saw, with field value e[o] iff o / 512 < *nb_seen and (cls[o] & cls_mask) == free_cls.
+struct OcEsdfField {
+  const float* e;            // [max_blocks*512] field, in the cnt plane's layout
+  const unsigned char* cls;  // [max_blocks*512] class byte of the update
+  const int* nb_seen;        // DEVICE: pool blocks the update saw
+  float D;                   // its truncation distance
+  unsigned char free_cls, cls_mask;
+};
+int oc_esdf_field(tslam_octo* m, int32_t submap, const char* what, OcEsdfField* f);
 // tslam_octo_frontier.cu: the frontier set of `submap` can be read (an update for it has completed and no reset or fusion
 // came since; refused like tslam_octo_frontier_gather, the message naming `what`) ...
 int oc_frontier_readable(tslam_octo* m, int32_t submap, const char* what);
 // ... and its m->fr_n rows (ijk, cluster ordinal) into idx[fr_n * 3], cluster[fr_n] (DEVICE), in compact order, on st
 int oc_frontier_rows(tslam_octo* m, int32_t* idx, int32_t* cluster, cudaStream_t st);
 #define OC_ERR_VIEW_WINDOW 16  // g.err: a viewpoint-gain walk left its view's bitmap window (tslam_octo_view.cu)
+#define OC_ERR_TRAVEL_PATH 32  // g.err: a travel path found no predecessor (impossible at the field's fixed point; tslam_octo_travel.cu)
 
 // Amanatides-Woo traversal of the log-odds map in voxel units (DESIGN.md section 7, "Traversal"): p0 = origin / vs,
 // p1 = endpoint / vs, cells c = round_half_away(p).  The k-th boundary crossing of axis a is at

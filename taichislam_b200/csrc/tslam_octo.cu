@@ -558,6 +558,7 @@ extern "C" int tslam_octo_destroy(tslam_octo_t* m) {
   oc_esdf_free(m);
   oc_frontier_free(m);
   oc_view_free(m);
+  oc_travel_free(m);
   delete m;
   return TSLAM_OK;
 }
@@ -575,6 +576,7 @@ extern "C" int tslam_octo_reset(tslam_octo_t* m, void* stream) {
   TS_CUDA(cudaMemsetAsync(m->scratch_i, 0, 4 * 4, st));
   m->esdf_full_needed = 1;  // pool slots are recycled: the kept ESDF state no longer describes the map
   m->fr_full_needed = 1;    // ... nor the kept frontier set
+  m->tr_ready = 0;          // ... nor the kept travel-cost field
   return TSLAM_OK;
 }
 
@@ -633,6 +635,10 @@ static int oc_deferred(tslam_octo* m) {
     cudaMemcpy(m->g.err, &zero, 4, cudaMemcpyHostToDevice);
     if (err == OC_ERR_VIEW_WINDOW) {
       ts_set_error("octo view gain: a walk left its view's bitmap window (is every view's R a rotation?): gains are invalid");
+      return TSLAM_E_INVALID;
+    }
+    if (err == OC_ERR_TRAVEL_PATH) {
+      ts_set_error("octo travel path: a cell of the field had no predecessor: paths are invalid");
       return TSLAM_E_INVALID;
     }
     ts_set_error("octomap block pool / table exhausted (max_blocks=%d, flags 0x%x): hits were dropped", m->g.max_blocks, err);

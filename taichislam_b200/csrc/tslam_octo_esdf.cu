@@ -459,6 +459,19 @@ static int oe_readable(tslam_octo* m, int32_t submap, const char* what) {
   return TSLAM_OK;
 }
 
+int oc_esdf_field(tslam_octo* m, int32_t submap, const char* what, OcEsdfField* f) {
+  int rc = oe_readable(m, submap, what);
+  if (rc) return rc;
+  const OeAux a = oe_aux(m);
+  f->e = a.e;
+  f->cls = a.cls;
+  f->nb_seen = a.nb_seen;
+  f->D = m->esdf_D;
+  f->free_cls = OE_FREE;
+  f->cls_mask = ES_CLS;
+  return TSLAM_OK;
+}
+
 // mode 0 = incremental when the state allows it (same submap and D as the last update, no reset / fusion in between),
 // 1 = full recompute.  stats4 (HOST, may be NULL): lower sweeps, raise sweeps (-1 = full), changed voxels, suspect voxels.
 extern "C" int tslam_octo_esdf_update(tslam_octo_t* m, int32_t submap, float max_dist, int32_t mode, int32_t* stats4, void* stream) {

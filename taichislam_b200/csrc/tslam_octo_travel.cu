@@ -1,0 +1,523 @@
+// libtslam.so - travel-cost field of a log-odds Octomap (DESIGN.md section 7, "Travel cost on the log-odds Octomap").
+//
+// Per submap, as of one update.  Classes as the occupancy ESDF defines them: OCC = known and L > l_occ, FREE = known and
+// L <= l_occ, UNKNOWN = not known (every cell of an absent block).  A cell is traversable iff it is inside the volume and
+// FREE, and, when clearance > 0, was FREE at the last occupancy-ESDF update of the submap, in a block that update saw,
+// with ESDF value >= clearance.  A step between 26-neighbours (edge cost c = vs * {1, sqrtf 2, sqrtf 3}, the ESDF's) is
+// allowed iff every cell of the axis-aligned box its two cells span is traversable (no corner cutting).  From the start
+// cell c0 = rha(p / vs), when traversable, G(c0) = 0 and
+//   G(v) = min over allowed steps h -> v of G(h) + c    (f32, one step at a time), values above max_cost dropped (+inf)
+// to the fixed point.  f32 addition is monotone and, below the bound max_cost <= 2^22 vs, G + c > G: the fixed point is
+// unique, equals Dijkstra's answer and does not depend on the schedule (DESIGN.md section 7 gives the argument).
+//
+// The scheme is the occupancy ESDF's lower wave (k_octo_esdf_sweep): a CTA stages its 8^3 block plus a one-voxel halo of
+// G and traversability in shared memory and relaxes it in place to local convergence (values only decrease); sweep k
+// runs the blocks with a neighbour stamped >= k-1, starting from the start's block, and es_wave drives the sweeps.  A
+// step's box lies inside the 3^3 neighbourhood of its target cell, so the step rule never leaves the staged tile.
+//
+// Nothing here writes the map or another tracker's state: no cnt word, mark bit, touched entry, dirty flag or stats
+// counter.
+#include <cmath>
+#include <cstring>
+#include "tslam_esdf_common.cuh"
+
+#define OT_T 10
+#define OT_T3 (OT_T * OT_T * OT_T)
+#define OT_THREADS 128
+#define OT_WORDS 16  // traversable bits per pool block: 512 bits
+
+struct OtAux {
+  float* G;        // [max_blocks*512] the field, +inf where unreachable
+  uint32_t* trav;  // [max_blocks*16] traversable bits of the update: bit (o & 31) of word o >> 5 for voxel offset o
+  int* nbr;        // [max_blocks*27] neighbour block indices of the update (-1 = absent)
+  int* epoch;      // [max_blocks] last sweep in which the block changed (-1: idle, < -1: block of another submap)
+  int* changed;    // [ES_MAX_SWEEPS+2] changed[k] != 0 <=> sweep k changed something
+  int* counts;     // [4] traversable cells, reachable cells, start_ok, (spare)
+  int* nb_seen;    // blocks in the pool when the last update ran (bump allocation: higher indices are newer)
+};
+
+// bit of neighbourhood offset (dx, dy, dz) in a 27-bit mask: dx outermost, the OFFSETS order of the reference
+__host__ __device__ constexpr int ot_bit(int dx, int dy, int dz) { return (dx + 1) * 9 + (dy + 1) * 3 + (dz + 1); }
+
+// The allowed steps into a cell whose 3^3 neighbourhood has traversable mask nm (bit ot_bit): bit ot_bit(d) is set iff
+// every cell of the box spanned by the cell and its neighbour d is traversable.  0 when the cell itself is not.
+__device__ __forceinline__ unsigned ot_allowed(unsigned nm) {
+  if (!((nm >> ot_bit(0, 0, 0)) & 1u)) return 0u;
+  unsigned am = 0u;
+#pragma unroll
+  for (int dx = -1; dx <= 1; dx++)
+#pragma unroll
+    for (int dy = -1; dy <= 1; dy++)
+#pragma unroll
+      for (int dz = -1; dz <= 1; dz++) {
+        if (dx == 0 && dy == 0 && dz == 0) continue;
+        unsigned box = 0u;
+#pragma unroll
+        for (int a = 0; a <= 1; a++)
+#pragma unroll
+          for (int b = 0; b <= 1; b++)
+#pragma unroll
+            for (int c = 0; c <= 1; c++) box |= 1u << ot_bit(a * dx, b * dy, c * dz);
+        if ((nm & box) == box) am |= 1u << ot_bit(dx, dy, dz);
+      }
+  return am;
+}
+
+__device__ __forceinline__ int ot_tidx(int lx, int ly, int lz) { return ((lx + 1) * OT_T + (ly + 1)) * OT_T + (lz + 1); }
+
+// Every block of the submap: traversable bits (with the clearance test against the occupancy ESDF), G = +inf or 0 at
+// c0, the neighbour table, epoch 0 on the start's block when c0 is traversable, idle on the others.  A pool slot
+// recycled after a reset is overwritten like any other, so no old value survives.
+__global__ void __launch_bounds__(OT_THREADS) k_octo_travel_init(OcGrid g, OtAux a, OcEsdfField ef, int submap, int l_occ, float clearance,
+                                                                 int ci, int cj, int ck, int c_in) {
+  __shared__ int s_n, s_start;
+  const int nb = min(*g.n_blocks, g.max_blocks);
+  if (blockIdx.x == 0 && threadIdx.x == 0) *a.nb_seen = nb;
+  const bool clear = clearance > 0.0f;
+  const int enb = clear ? *ef.nb_seen : 0;
+  const float inf = __int_as_float(0x7f800000);
+  for (int b = blockIdx.x; b < nb; b += gridDim.x) {
+    int s, bx, by, bz;
+    ts_unpack_key(g.block_key[b], s, bx, by, bz);
+    if (s != submap) {  // (uniform per CTA)
+      if (threadIdx.x == 0) a.epoch[b] = -1000000;
+      continue;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) { s_n = 0; s_start = 0; }
+    __syncthreads();
+    if (threadIdx.x < 27) {
+      const int dx = threadIdx.x / 9 - 1, dy = (threadIdx.x / 3) % 3 - 1, dz = threadIdx.x % 3 - 1;
+      a.nbr[b * 27 + threadIdx.x] = ts_find(g, ts_pack_key(s, bx + dx, by + dy, bz + dz));
+    }
+    const size_t base = (size_t)b * OC_B3;
+    const bool sblk = c_in && (ci >> OC_BSHIFT) == bx && (cj >> OC_BSHIFT) == by && (ck >> OC_BSHIFT) == bz;
+    int cnt = 0;
+    for (int v = threadIdx.x; v < OC_B3; v += blockDim.x) {
+      const int i = bx * OC_B + (v >> 6), j = by * OC_B + ((v >> 3) & 7), k = bz * OC_B + (v & 7);
+      const unsigned int w = g.cnt[base + v];
+      bool t = ts_in_bounds(g, i, j, k) && lo_known(w) && lo_val(w) <= l_occ;
+      if (t && clear) t = b < enb && (ef.cls[base + v] & ef.cls_mask) == ef.free_cls && ef.e[base + v] >= clearance;
+      const unsigned m = __ballot_sync(0xffffffffu, t);
+      if ((threadIdx.x & 31) == 0) a.trav[(size_t)b * OT_WORDS + (v >> 5)] = m;
+      float gv = inf;
+      if (t && sblk && i == ci && j == cj && k == ck) { gv = 0.0f; s_start = 1; }
+      a.G[base + v] = gv;
+      cnt += t ? 1 : 0;
+    }
+    for (int o = 16; o > 0; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+    if ((threadIdx.x & 31) == 0 && cnt) atomicAdd(&s_n, cnt);
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      a.epoch[b] = s_start ? 0 : -1;
+      if (s_start) a.counts[2] = 1;
+      if (s_n) atomicAdd(&a.counts[0], s_n);
+    }
+  }
+}
+
+struct OtTile {
+  float G[OT_T3];
+  unsigned char t[OT_T3];
+  int nbr[27];
+  int active, changed, any_write;
+};
+
+// block + one-voxel halo into shared memory (absent neighbour blocks read unreachable and not traversable)
+__device__ __forceinline__ void ot_stage(const OtAux& a, OtTile& tile) {
+  for (int c = threadIdx.x; c < OT_T3; c += blockDim.x) {
+    const int lz = c % OT_T - 1, ly = (c / OT_T) % OT_T - 1, lx = c / (OT_T * OT_T) - 1;
+    const int nbk = tile.nbr[(((lx + 8) >> 3) * 3 + ((ly + 8) >> 3)) * 3 + ((lz + 8) >> 3)];
+    float gv = __int_as_float(0x7f800000);
+    unsigned char tv = 0;
+    if (nbk >= 0) {
+      const int off = oc_voxel_off(lx, ly, lz);
+      tv = (unsigned char)((a.trav[(size_t)nbk * OT_WORDS + (off >> 5)] >> (off & 31)) & 1u);
+      gv = *(volatile float*)&a.G[(size_t)nbk * OC_B3 + off];
+    }
+    tile.G[c] = gv;
+    tile.t[c] = tv;
+  }
+}
+
+// One sweep of the wave: relax the blocks the wave front reaches to local convergence
+__global__ void __launch_bounds__(OT_THREADS) k_octo_travel_sweep(OcGrid g, OtAux a, int sweep, float vs, float max_cost) {
+  __shared__ OtTile tile;
+  if (sweep > 1 && a.changed[sweep - 1] == 0) return;  // already converged: nothing to do
+  const int nb = min(*a.nb_seen, g.max_blocks);
+  const float d1 = vs, d2 = sqrtf(2.0f) * vs, d3 = sqrtf(3.0f) * vs;  // the edge costs of k_octo_esdf_sweep
+  for (int b = blockIdx.x; b < nb; b += gridDim.x) {
+    __syncthreads();
+    if (threadIdx.x == 0) { tile.active = 0; tile.any_write = 0; }
+    __syncthreads();
+    if (a.epoch[b] < -1) continue;  // block of another submap (uniform per CTA)
+    if (threadIdx.x < 27) {
+      const int n = a.nbr[b * 27 + threadIdx.x];
+      tile.nbr[threadIdx.x] = n;
+      if (n >= 0 && *(volatile int*)&a.epoch[n] >= sweep - 1) tile.active = 1;  // the wave front reaches this block
+    }
+    __syncthreads();
+    if (!tile.active) continue;
+    ot_stage(a, tile);
+    __syncthreads();
+    // the allowed steps into each of this thread's voxels: traversability is fixed during the wave
+    unsigned am[OC_B3 / OT_THREADS];
+#pragma unroll
+    for (int q = 0; q < OC_B3 / OT_THREADS; q++) {
+      const int v = threadIdx.x + q * OT_THREADS;
+      const int c0 = ot_tidx(v >> 6, (v >> 3) & 7, v & 7);
+      unsigned nm = 0u;
+#pragma unroll
+      for (int dx = -1; dx <= 1; dx++)
+#pragma unroll
+        for (int dy = -1; dy <= 1; dy++)
+#pragma unroll
+          for (int dz = -1; dz <= 1; dz++) nm |= (unsigned)tile.t[c0 + (dx * OT_T + dy) * OT_T + dz] << ot_bit(dx, dy, dz);
+      am[q] = ot_allowed(nm);
+    }
+    // relax to local convergence (values only decrease, so in-place racy updates are safe)
+    for (int iter = 0; iter < 64; ++iter) {
+      if (threadIdx.x == 0) tile.changed = 0;
+      __syncthreads();
+      bool mine = false;
+#pragma unroll
+      for (int q = 0; q < OC_B3 / OT_THREADS; q++) {
+        if (!am[q]) continue;
+        const int v = threadIdx.x + q * OT_THREADS;
+        const int c0 = ot_tidx(v >> 6, (v >> 3) & 7, v & 7);
+        const float cur = tile.G[c0];
+        float best = cur;
+#pragma unroll
+        for (int dx = -1; dx <= 1; dx++)
+#pragma unroll
+          for (int dy = -1; dy <= 1; dy++)
+#pragma unroll
+            for (int dz = -1; dz <= 1; dz++) {
+              const int nz_ = (dx != 0) + (dy != 0) + (dz != 0);
+              if (nz_ == 0 || !((am[q] >> ot_bit(dx, dy, dz)) & 1u)) continue;
+              const float dis = nz_ == 1 ? d1 : (nz_ == 2 ? d2 : d3);
+              const float cand = tile.G[c0 + (dx * OT_T + dy) * OT_T + dz] + dis;
+              if (cand <= max_cost) best = fminf(best, cand);  // (+inf + c is +inf: never kept)
+            }
+        if (best < cur) {
+          tile.G[c0] = best;
+          mine = true;
+        }
+      }
+      if (__any_sync(0xffffffffu, mine) && (threadIdx.x & 31) == 0) tile.changed = 1;
+      __syncthreads();
+      const int ch = tile.changed;
+      if (ch && threadIdx.x == 0) tile.any_write = 1;
+      __syncthreads();
+      if (!ch) break;
+    }
+    if (tile.any_write) {
+      const size_t base = (size_t)b * OC_B3;
+      for (int v = threadIdx.x; v < OC_B3; v += blockDim.x) a.G[base + v] = tile.G[ot_tidx(v >> 6, (v >> 3) & 7, v & 7)];
+      if (threadIdx.x == 0) {
+        __threadfence();
+        a.epoch[b] = sweep;
+        a.changed[sweep] = 1;
+      }
+    }
+  }
+}
+
+// reachable cells of the submap after the wave -> counts[1]
+__global__ void __launch_bounds__(OT_THREADS) k_octo_travel_count(OcGrid g, OtAux a) {
+  __shared__ int s_n;
+  const int nb = min(*a.nb_seen, g.max_blocks);
+  for (int b = blockIdx.x; b < nb; b += gridDim.x) {
+    if (a.epoch[b] < -1) continue;  // (uniform per CTA)
+    __syncthreads();
+    if (threadIdx.x == 0) s_n = 0;
+    __syncthreads();
+    const size_t base = (size_t)b * OC_B3;
+    int cnt = 0;
+    for (int v = threadIdx.x; v < OC_B3; v += blockDim.x) cnt += isfinite(a.G[base + v]) ? 1 : 0;
+    for (int o = 16; o > 0; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+    if ((threadIdx.x & 31) == 0 && cnt) atomicAdd(&s_n, cnt);
+    __syncthreads();
+    if (threadIdx.x == 0 && s_n) atomicAdd(&a.counts[1], s_n);
+  }
+}
+
+// (ijk, G) of every reachable cell, in the blocks the update saw
+__global__ void __launch_bounds__(OT_THREADS) k_octo_travel_gather(OcGrid g, OtAux a, int submap, long long cap, int32_t* idx, float* cost,
+                                                                   unsigned long long* counter) {
+  const int nb = min(*a.nb_seen, g.max_blocks);
+  for (int b = blockIdx.x; b < nb; b += gridDim.x) {
+    int s, bx, by, bz;
+    ts_unpack_key(g.block_key[b], s, bx, by, bz);
+    if (s != submap) continue;  // (uniform per CTA)
+    const size_t base = (size_t)b * OC_B3;
+    for (int v = threadIdx.x; v < OC_B3; v += blockDim.x) {
+      const float gv = a.G[base + v];
+      const bool want = isfinite(gv);
+      const unsigned m = __ballot_sync(0xffffffffu, want);
+      if (!m) continue;
+      const int lane = threadIdx.x & 31, leader = __ffs(m) - 1;
+      unsigned long long rb = 0;
+      if (lane == leader) rb = atomicAdd(counter, (unsigned long long)__popc(m));
+      rb = __shfl_sync(0xffffffffu, rb, leader);
+      const long long row = (long long)(rb + __popc(m & ((1u << lane) - 1)));
+      if (want && row < cap) {
+        idx[3 * row] = bx * OC_B + (v >> 6);
+        idx[3 * row + 1] = by * OC_B + ((v >> 3) & 7);
+        idx[3 * row + 2] = bz * OC_B + (v & 7);
+        cost[row] = gv;
+      }
+    }
+  }
+}
+
+// cell rha(p / vs) of a point, and whether it is inside the volume (false for a non-finite coordinate)
+__device__ __forceinline__ bool ot_cell(const OcGrid& g, float vs, const float* p, int c[3]) {
+  const float u0 = __fdiv_rn(p[0], vs), u1 = __fdiv_rn(p[1], vs), u2 = __fdiv_rn(p[2], vs);
+  if (!(fabsf(u0) < 1e9f && fabsf(u1) < 1e9f && fabsf(u2) < 1e9f)) return false;  // no out-of-range float -> int conversion
+  c[0] = (int)roundf(u0); c[1] = (int)roundf(u1); c[2] = (int)roundf(u2);
+  return ts_in_bounds(g, c[0], c[1], c[2]);
+}
+
+// pool block of cell c in `submap` when the update saw it, else -1
+__device__ __forceinline__ int ot_block(const OcGrid& g, int submap, int nb_seen, const int c[3]) {
+  const int b = ts_find(g, ts_pack_key(submap, c[0] >> OC_BSHIFT, c[1] >> OC_BSHIFT, c[2] >> OC_BSHIFT));
+  return (b >= 0 && b < nb_seen) ? b : -1;
+}
+
+// G of the cell of each point; +inf where unreachable, outside the volume, in a newer block or not finite
+__global__ void __launch_bounds__(256) k_octo_travel_query(OcGrid g, OtAux a, int submap, long long n, const float* __restrict__ xyz, float vs,
+                                                           float* __restrict__ cost) {
+  const int nb_seen = *a.nb_seen;
+  for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < n; q += (long long)gridDim.x * blockDim.x) {
+    int c[3];
+    float gv = __int_as_float(0x7f800000);
+    if (ot_cell(g, vs, xyz + 3 * q, c)) {
+      const int b = ot_block(g, submap, nb_seen, c);
+      if (b >= 0) gv = a.G[(size_t)b * OC_B3 + oc_voxel_off(c[0], c[1], c[2])];
+    }
+    cost[q] = gv;
+  }
+}
+
+// Path from the cell of each target to the start: from the current cell v, the predecessor is the reachable
+// 26-neighbour h with an allowed step and G(h) + c == G(v) exactly, smallest G(h), ties to the first in ot_bit order.
+// One hash probe for the target's block; the walk moves through the update's neighbour table.
+__global__ void __launch_bounds__(256) k_octo_travel_path(OcGrid g, OtAux a, int submap, long long n, const float* __restrict__ xyz, float vs,
+                                                          int max_len, int32_t* __restrict__ cells, int32_t* __restrict__ len) {
+  const int nb_seen = *a.nb_seen;
+  const float d1 = vs, d2 = sqrtf(2.0f) * vs, d3 = sqrtf(3.0f) * vs;
+  const float inf = __int_as_float(0x7f800000);
+  for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < n; q += (long long)gridDim.x * blockDim.x) {
+    int c[3];
+    int L = 0;
+    int b = ot_cell(g, vs, xyz + 3 * q, c) ? ot_block(g, submap, nb_seen, c) : -1;
+    float gv = b >= 0 ? a.G[(size_t)b * OC_B3 + oc_voxel_off(c[0], c[1], c[2])] : inf;
+    int32_t* out = cells + 3 * (size_t)q * max_len;
+    while (gv < inf) {
+      if (L < max_len) { out[3 * L] = c[0]; out[3 * L + 1] = c[1]; out[3 * L + 2] = c[2]; }
+      ++L;
+      if (gv == 0.0f) break;  // the start: the only cell at 0
+      const int bx = c[0] >> OC_BSHIFT, by = c[1] >> OC_BSHIFT, bz = c[2] >> OC_BSHIFT;
+      // traversability of the 3^3 neighbourhood as the update left it, then the costs of the allowed steps only
+      unsigned nm = 0u;
+#pragma unroll
+      for (int e = 0; e < 27; e++) {
+        const int i = c[0] + e / 9 - 1, j = c[1] + (e / 3) % 3 - 1, k = c[2] + e % 3 - 1;
+        const int nb_ = a.nbr[b * 27 + ot_bit((i >> OC_BSHIFT) - bx, (j >> OC_BSHIFT) - by, (k >> OC_BSHIFT) - bz)];
+        const int off = oc_voxel_off(i, j, k);
+        if (nb_ >= 0) nm |= ((a.trav[(size_t)nb_ * OT_WORDS + (off >> 5)] >> (off & 31)) & 1u) << e;
+      }
+      const unsigned am = ot_allowed(nm);
+      int best = -1;
+      float bg = inf;
+#pragma unroll
+      for (int e = 0; e < 27; e++) {
+        if (!((am >> e) & 1u)) continue;  // (never the cell itself)
+        const int dx = e / 9 - 1, dy = (e / 3) % 3 - 1, dz = e % 3 - 1;
+        const int i = c[0] + dx, j = c[1] + dy, k = c[2] + dz;
+        const int nb_ = a.nbr[b * 27 + ot_bit((i >> OC_BSHIFT) - bx, (j >> OC_BSHIFT) - by, (k >> OC_BSHIFT) - bz)];
+        const float hg = a.G[(size_t)nb_ * OC_B3 + oc_voxel_off(i, j, k)];  // (an allowed step's cell is traversable: nb_ >= 0)
+        const int nz_ = (dx != 0) + (dy != 0) + (dz != 0);
+        const float dis = nz_ == 1 ? d1 : (nz_ == 2 ? d2 : d3);
+        if (hg < bg && hg + dis == gv) { best = e; bg = hg; }
+      }
+      if (best < 0) {  // cannot happen at the fixed point: reported by the next tslam_octo_sync, never a silent cut
+        atomicOr(g.err, OC_ERR_TRAVEL_PATH);
+        L = 0;
+        break;
+      }
+      const int i = c[0] + best / 9 - 1, j = c[1] + (best / 3) % 3 - 1, k = c[2] + best % 3 - 1;
+      b = a.nbr[b * 27 + ot_bit((i >> OC_BSHIFT) - bx, (j >> OC_BSHIFT) - by, (k >> OC_BSHIFT) - bz)];
+      c[0] = i; c[1] = j; c[2] = k;
+      gv = bg;
+    }
+    len[q] = L;
+  }
+}
+
+// ---- host side -----------------------------------------------------------------------------------------------------
+// bytes per pool block: field 2048 + traversable bits 64 + neighbour table 108 + epoch 4 = 2224
+static size_t ot_bytes(size_t nb) { return nb * (OC_B3 * 4 + OT_WORDS * 4 + 28 * 4) + ((ES_MAX_SWEEPS + 2) + 8) * 4; }
+
+static OtAux ot_aux(tslam_octo* m) {
+  const size_t nb = (size_t)m->g.max_blocks;
+  OtAux a;
+  a.G = (float*)m->tr_mem;
+  a.trav = (uint32_t*)(a.G + nb * OC_B3);
+  a.nbr = (int*)(a.trav + nb * OT_WORDS);
+  a.epoch = a.nbr + nb * 27;
+  a.changed = a.epoch + nb;
+  a.counts = a.changed + (ES_MAX_SWEEPS + 2);
+  a.nb_seen = a.counts + 4;
+  return a;
+}
+
+int oc_travel_free(tslam_octo* m) {
+  if (m->tr_mem) cudaFree(m->tr_mem);
+  m->tr_mem = nullptr;
+  m->tr_ready = 0;
+  return TSLAM_OK;
+}
+
+// the checks every travel call makes first
+static int ot_check(tslam_octo* m, int32_t submap, const char* what) {
+  if (!m->logodds) {
+    ts_set_error("%s: the map is a hit counter; a travel-cost field needs a log-odds map (tslam_octo_create_logodds)", what);
+    return TSLAM_E_INVALID;
+  }
+  if (submap < 0 || submap >= m->cfg.max_submaps) { ts_set_error("%s: submap %d out of range", what, submap); return TSLAM_E_INVALID; }
+  return TSLAM_OK;
+}
+
+// the field of `submap` can be read: an update has completed, for that submap, and no reset or fusion came after it
+static int ot_readable(tslam_octo* m, int32_t submap, const char* what) {
+  int rc = ot_check(m, submap, what);
+  if (rc) return rc;
+  if (!m->tr_mem) { ts_set_error("%s: no travel-cost field has been computed (tslam_octo_travel_update has not run)", what); return TSLAM_E_INVALID; }
+  if (!m->tr_ready) {
+    ts_set_error("%s: the map was reset or fused, or the last tslam_octo_travel_update failed, since the last completed update", what);
+    return TSLAM_E_INVALID;
+  }
+  if (m->tr_submap != submap) {
+    ts_set_error("%s: the last tslam_octo_travel_update was for submap %d, not %d", what, m->tr_submap, submap);
+    return TSLAM_E_INVALID;
+  }
+  return TSLAM_OK;
+}
+
+extern "C" int tslam_octo_travel_update(tslam_octo_t* m, int32_t submap, const float* start3, float clearance, float max_cost,
+                                        int32_t* stats4, void* stream) {
+  const char* what = "tslam_octo_travel_update";
+  if (!m || !start3) return TSLAM_E_INVALID;
+  int rc = ot_check(m, submap, what);
+  if (rc) return rc;
+  if (!(std::isfinite(start3[0]) && std::isfinite(start3[1]) && std::isfinite(start3[2]))) {
+    ts_set_error("%s: the start must be finite", what);
+    return TSLAM_E_INVALID;
+  }
+  const float vs = m->in.vs;
+  const float cost_limit = std::ldexp(vs, 22);  // keeps G + vs > G for every kept value
+  if (!(std::isfinite(clearance) && clearance >= 0.0f)) {
+    ts_set_error("%s: clearance must be finite and >= 0 (got %g)", what, (double)clearance);
+    return TSLAM_E_INVALID;
+  }
+  if (!(std::isfinite(max_cost) && max_cost > 0.0f && max_cost <= cost_limit)) {
+    ts_set_error("%s: max_cost must be finite, > 0 and <= 2^22 * voxel_scale = %g (got %g)", what, (double)cost_limit, (double)max_cost);
+    return TSLAM_E_INVALID;
+  }
+  OcEsdfField ef;
+  memset(&ef, 0, sizeof(ef));
+  if (clearance > 0.0f) {
+    rc = oc_esdf_field(m, submap, what, &ef);
+    if (rc) return rc;
+    if (clearance > ef.D) {
+      ts_set_error("%s: clearance %g exceeds the occupancy ESDF's max_dist %g", what, (double)clearance, (double)ef.D);
+      return TSLAM_E_INVALID;
+    }
+  }
+  if (!m->tr_mem) {
+    const size_t bytes = ot_bytes((size_t)m->g.max_blocks);
+    TS_CUDA(cudaMalloc(&m->tr_mem, bytes));
+    TS_CUDA(cudaMemset(m->tr_mem, 0, bytes));
+  }
+  // start cell c0 = rha(p / vs), f32 division as the kernels do it
+  int c[3] = {0, 0, 0};
+  bool c_in = true;
+  for (int q = 0; q < 3; q++) {
+    const float u = start3[q] / vs;
+    if (!(std::fabs(u) < 1e9f)) { c_in = false; break; }
+    c[q] = (int)std::round(u);
+  }
+  c_in = c_in && c[0] >= -m->g.hN && c[0] < m->g.N - m->g.hN && c[1] >= -m->g.hN && c[1] < m->g.N - m->g.hN && c[2] >= -m->g.hNz &&
+         c[2] < m->g.Nz - m->g.hNz;
+  cudaStream_t st = (cudaStream_t)stream;
+  OtAux a = ot_aux(m);
+  m->tr_ready = 0;  // until this update has completed
+  TS_CUDA(cudaMemsetAsync(a.changed, 0, ((ES_MAX_SWEEPS + 2) + 4) * 4, st));  // changed, counts
+  const int grid = m->sm_count * 8;
+  k_octo_travel_init<<<grid, OT_THREADS, 0, st>>>(m->g, a, ef, submap, m->lo.l_occ, clearance, c[0], c[1], c[2], c_in ? 1 : 0);
+  TS_LAUNCH_CHECK(m);
+  int sweeps = 0;
+  rc = es_wave(m, st, a.changed, ES_GROUP, [&](int k) { k_octo_travel_sweep<<<grid, OT_THREADS, 0, st>>>(m->g, a, k, vs, max_cost); },
+               &sweeps);
+  if (rc) return rc;
+  if (sweeps > ES_MAX_SWEEPS) {  // the last sweep still changed something: the field is not the fixed point
+    ts_set_error("%s: the wave was still changing after %d sweeps; the field is incomplete and its readers refuse", what, ES_MAX_SWEEPS);
+    return TSLAM_E_INVALID;
+  }
+  k_octo_travel_count<<<grid, OT_THREADS, 0, st>>>(m->g, a);
+  TS_LAUNCH_CHECK(m);
+  int h_counts[4] = {0, 0, 0, 0};
+  TS_CUDA(cudaMemcpyAsync(h_counts, a.counts, 16, cudaMemcpyDeviceToHost, st));
+  TS_CUDA(cudaStreamSynchronize(st));
+  m->tr_ready = 1;
+  m->tr_submap = submap;
+  if (stats4) { stats4[0] = h_counts[1]; stats4[1] = sweeps; stats4[2] = h_counts[0]; stats4[3] = h_counts[2]; }
+  return TSLAM_OK;
+}
+
+extern "C" int tslam_octo_travel_gather(tslam_octo_t* m, int32_t submap, int64_t cap, int32_t* idx, float* cost, int64_t* n_out,
+                                        void* stream) {
+  if (!m || !n_out || cap < 0 || (cap > 0 && (!idx || !cost))) return TSLAM_E_INVALID;
+  int rc = ot_readable(m, submap, "tslam_octo_travel_gather");
+  if (rc) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  unsigned long long* ctr = (unsigned long long*)(m->scratch_i + 8);
+  TS_CUDA(cudaMemsetAsync(ctr, 0, 8, st));
+  k_octo_travel_gather<<<m->sm_count * 8, OT_THREADS, 0, st>>>(m->g, ot_aux(m), submap, cap, idx, cost, ctr);
+  TS_LAUNCH_CHECK(m);
+  unsigned long long v = 0;
+  TS_CUDA(cudaMemcpyAsync(&v, ctr, 8, cudaMemcpyDeviceToHost, st));
+  TS_CUDA(cudaStreamSynchronize(st));
+  *n_out = (int64_t)v;
+  if ((int64_t)v > cap) { ts_set_error("octo travel gather: %lld cells > capacity %lld", (long long)v, (long long)cap); return TSLAM_E_CAPACITY; }
+  return TSLAM_OK;
+}
+
+static int ot_grid(tslam_octo* m, long long n) {
+  long long blocks = (n + 255) / 256;
+  if (blocks > (long long)m->sm_count * 16) blocks = (long long)m->sm_count * 16;
+  return (int)blocks;
+}
+
+extern "C" int tslam_octo_travel_query(tslam_octo_t* m, int32_t submap, int64_t n, const float* xyz, float* cost, void* stream) {
+  if (!m || n < 0 || (n && (!xyz || !cost))) return TSLAM_E_INVALID;
+  int rc = ot_readable(m, submap, "tslam_octo_travel_query");
+  if (rc || n == 0) return rc;
+  k_octo_travel_query<<<ot_grid(m, n), 256, 0, (cudaStream_t)stream>>>(m->g, ot_aux(m), submap, n, xyz, m->in.vs, cost);
+  TS_LAUNCH_CHECK(m);
+  return TSLAM_OK;
+}
+
+extern "C" int tslam_octo_travel_path(tslam_octo_t* m, int32_t submap, int64_t n, const float* xyz, int32_t max_len, int32_t* cells,
+                                      int32_t* len, void* stream) {
+  if (!m || n < 0 || (n && (!xyz || !cells || !len))) return TSLAM_E_INVALID;
+  const char* what = "tslam_octo_travel_path";
+  if (max_len < 1) { ts_set_error("%s: max_len must be >= 1 (got %d)", what, max_len); return TSLAM_E_INVALID; }
+  int rc = ot_readable(m, submap, what);
+  if (rc || n == 0) return rc;
+  k_octo_travel_path<<<ot_grid(m, n), 256, 0, (cudaStream_t)stream>>>(m->g, ot_aux(m), submap, n, xyz, m->in.vs, max_len, cells, len);
+  TS_LAUNCH_CHECK(m);
+  return TSLAM_OK;
+}

@@ -249,6 +249,49 @@ class Octomap(BaseMap):
             _, out["frontier"], out["frontier_per_cluster"] = self._h.view_gain_frontier(pos, R, cam, submap=s)
         return out
 
+    # travel cost through known free space (log-odds maps only, DESIGN.md section 7)
+    def _travel_map(self):
+        if self.occupancy_model != "logodds":
+            raise ValueError("a travel cost needs Octomap(..., occupancy_model='logodds'): a hit counter cannot tell free "
+                             "space from unknown space")
+
+    def travel_update(self, start, clearance=0.0, max_cost=None):
+        """Travel-cost field of the active submap from `start` (metres, map frame) through known free space -> dict(
+        reachable, sweeps, traversable, start_ok).  clearance > 0 keeps to cells at least that far from occupied space:
+        it first runs esdf_update() with the max_dist of the last esdf_update (else max_ray_length) and raises
+        ValueError when clearance exceeds it.  max_cost None: no bound below the limit 2^22 * voxel_scale."""
+        self._travel_map()
+        if float(clearance) > 0.0:
+            d = float(getattr(self, "esdf_max_dist", None) or self.max_ray_length)
+            if np.float32(clearance) > np.float32(d):
+                raise ValueError(f"clearance {clearance} exceeds the ESDF's max_dist {d}: call esdf_update(max_dist) with a "
+                                 "larger max_dist first")
+            self.esdf_update(d)
+        return self._h.travel_update(self._active(), start, clearance, max_cost)
+
+    def travel_cost(self, xyz):
+        """Travel cost of the cells of points [n,3] as of the last travel_update, +inf where unreachable: a torch CUDA
+        tensor for a torch tensor, a numpy array for a numpy array."""
+        self._travel_map()
+        return self._h.travel_query(xyz, submap=self._active())
+
+    def travel_path(self, goal, max_len=4096):
+        """The path of the last travel_update from its start to the cell of `goal` [3] as cell centres in metres (f64 of
+        cell index * f32(constructor voxel_scale)), [n,3] ordered start to goal, or None when the goal is unreachable."""
+        self._travel_map()
+        if isinstance(goal, self._torch.Tensor):
+            goal = goal.detach().cpu().numpy()
+        g = np.asarray(goal, np.float32).reshape(1, 3)
+        cells, n = self._h.travel_path(g, submap=self._active(), max_len=max_len)
+        n = int(n[0])
+        if n == 0:
+            return None
+        if n > max_len:   # the buffer was too small: once more with the reported length
+            cells, n2 = self._h.travel_path(g, submap=self._active(), max_len=n)
+            assert int(n2[0]) == n
+        vs = float(np.float32(self._h.cfg.voxel_scale))
+        return cells[0, :n][::-1].astype(np.float64) * vs
+
     def saveMap(self, path):  # :201-202 (stub in the reference)
         pass
 

@@ -350,6 +350,76 @@ class OctoHandle:
             return valid, total, per
         return valid.cpu().numpy(), total.cpu().numpy(), per.cpu().numpy()
 
+    # -- travel cost on a log-odds map (tslam_octo_travel_*, DESIGN.md section 7) --------------------------------------
+    def travel_limit(self):
+        """The largest max_cost a travel update accepts: 2^22 * f32(voxel_scale)."""
+        return float(np.ldexp(np.float32(self.cfg.voxel_scale), 22))
+
+    def travel_update(self, submap, start, clearance=0.0, max_cost=None):
+        """Travel-cost field of `submap` from `start` (metres, submap frame) through known free space, with `clearance`
+        (> 0: cells whose occupancy ESDF at the last esdf_update is >= clearance) and max_cost (None: the limit
+        2^22 * voxel_scale) -> dict(reachable, sweeps, traversable, start_ok (bool))."""
+        p = capi.f32c(start).reshape(3)
+        st = np.zeros(4, np.int32)
+        mc = self.travel_limit() if max_cost is None else float(max_cost)
+        capi.check(self.L.tslam_octo_travel_update(self.h, int(submap), capi.np_ptr(p), float(clearance), mc, capi.np_ptr(st),
+                                                   capi.stream_ptr()))
+        return dict(reachable=int(st[0]), sweeps=int(st[1]), traversable=int(st[2]), start_ok=bool(st[3]))
+
+    def travel_gather(self, submap=0, as_torch=False):
+        """(idx int32[n,3], cost f32[n]) of the cells reachable at the last travel_update: numpy arrays, or torch CUDA
+        tensors with as_torch."""
+        torch = self.torch
+        dev = torch.device("cuda", torch.cuda.current_device())
+        n = C.c_int64(0)
+        rc = self.L.tslam_octo_travel_gather(self.h, int(submap), 0, None, None, C.byref(n), capi.stream_ptr())
+        if rc not in (capi.TSLAM_OK, capi.E_CAPACITY):
+            capi.check(rc)
+        cap = int(n.value)
+        idx = torch.empty((max(cap, 1), 3), dtype=torch.int32, device=dev)
+        g = torch.empty(max(cap, 1), dtype=torch.float32, device=dev)
+        capi.check(self.L.tslam_octo_travel_gather(self.h, int(submap), cap, capi.tptr(idx), capi.tptr(g), C.byref(n), capi.stream_ptr()))
+        k = int(n.value)
+        if as_torch:
+            return idx[:k], g[:k]
+        return idx[:k].cpu().numpy(), g[:k].cpu().numpy()
+
+    def _points(self, xyz):
+        """(as_torch, contiguous f32 [n,3] CUDA tensor)"""
+        torch = self.torch
+        as_torch = isinstance(xyz, torch.Tensor)
+        if as_torch:
+            x = xyz.to(device=torch.device("cuda", torch.cuda.current_device()), dtype=torch.float32).contiguous()
+        else:
+            x = torch.from_numpy(np.ascontiguousarray(xyz, dtype=np.float32)).cuda()
+        return as_torch, x.reshape(-1, 3)
+
+    def travel_query(self, xyz, submap=0):
+        """Travel cost f32[n] of the cells of points [n,3] as of the last travel_update (+inf where unreachable).  A torch
+        CUDA tensor in -> a torch CUDA tensor out, without a host synchronisation; a numpy array in -> a numpy array out."""
+        torch = self.torch
+        as_torch, x = self._points(xyz)
+        n = x.shape[0]
+        cost = torch.empty(n, dtype=torch.float32, device=x.device)
+        capi.check(self.L.tslam_octo_travel_query(self.h, int(submap), n, capi.tptr(x), capi.tptr(cost), capi.stream_ptr()))
+        return cost if as_torch else cost.cpu().numpy()
+
+    def travel_path(self, xyz, submap=0, max_len=4096):
+        """Paths from the cells of targets [n,3] back to the start of the last travel_update -> (cells int32[n,max_len,3]
+        target -> start, len int32[n]: the full cell count, 0 when unreachable; rows beyond min(len, max_len) are
+        undefined).  Torch in -> torch out without a host synchronisation; numpy in -> numpy out."""
+        torch = self.torch
+        as_torch, x = self._points(xyz)
+        n = x.shape[0]
+        cells = torch.empty((n, int(max_len), 3), dtype=torch.int32, device=x.device)
+        ln = torch.empty(n, dtype=torch.int32, device=x.device)
+        capi.check(self.L.tslam_octo_travel_path(self.h, int(submap), n, capi.tptr(x), int(max_len), capi.tptr(cells), capi.tptr(ln),
+                                                 capi.stream_ptr()))
+        if as_torch:
+            return cells, ln
+        self.sync()
+        return cells.cpu().numpy(), ln.cpu().numpy()
+
     def raycast(self, pos, direction, max_dist, submap=0):
         torch = self.torch
         p = torch.from_numpy(np.ascontiguousarray(pos, dtype=np.float32)).cuda()

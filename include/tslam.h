@@ -572,6 +572,29 @@ int tslam_octo_travel_query(tslam_octo_t* m, int32_t submap, int64_t n, const fl
 int tslam_octo_travel_path(tslam_octo_t* m, int32_t submap, int64_t n, const float* xyz, int32_t max_len, int32_t* cells,
                            int32_t* len, void* stream);
 
+/* Many-source travel costs: S fields of one submap in one update, field s exactly the single-source field from starts[s]
+ * (same traversability, steps, f32 sums and max_cost cut).  G_s(p_t) and G_t(p_s) add the same steps in opposite orders
+ * and may differ in the last bits; nothing symmetrises them.  Under the default max_cost (2^22 * vs) reachability is
+ * symmetric.  The fields are separate from the single-source field: an update of either changes nothing the other's
+ * readers return.  State: 68 B per pool block, plus ~2.1 KB per submap block with a traversable cell (B_t) and ~2 KB per
+ * (block, source) pair, grown on demand and freed by tslam_octo_destroy. */
+#define TSLAM_OCTO_TRAVEL_MAX_STARTS 1024
+/* Compute the fields from starts[n_starts,3] (HOST, finite, 1 <= n_starts <= TSLAM_OCTO_TRAVEL_MAX_STARTS, duplicates
+ * allowed); clearance and max_cost as for tslam_octo_travel_update.  stats2 (HOST, may be NULL): sweeps, traversable
+ * cells; reachable[n_starts] (HOST, may be NULL): reachable cells per start; start_ok[n_starts] (HOST, may be NULL): 1
+ * when the start's cell is traversable, else 0 and its row is all +inf (not an error).  Synchronises. */
+int tslam_octo_travel_multi_update(tslam_octo_t* m, int32_t submap, int32_t n_starts, const float* starts, float clearance,
+                                   float max_cost, int32_t* stats2, int32_t* reachable, uint8_t* start_ok, void* stream);
+/* cost f32[S,n] row-major: cost[s*n + q] = G_s of the cell of xyz[q] as of the last multi update, with the rules of
+ * tslam_octo_travel_query (DEVICE, asynchronous).  Passing the starts as xyz gives the S x S matrix.  Refused before a
+ * multi update, for another submap, after a reset or fusion, and after a failed update. */
+int tslam_octo_travel_multi_query(tslam_octo_t* m, int32_t submap, int64_t n, const float* xyz, float* cost, void* stream);
+/* Path of pair q from the cell of xyz[q] back to starts[source[q]] with the rule and the len / max_len semantics of
+ * tslam_octo_travel_path (DEVICE, asynchronous).  A source outside [0, S) writes len 0 and makes the next
+ * tslam_octo_sync return TSLAM_E_INVALID.  Refused like tslam_octo_travel_multi_query. */
+int tslam_octo_travel_multi_path(tslam_octo_t* m, int32_t submap, int64_t n, const int32_t* source, const float* xyz,
+                                 int32_t max_len, int32_t* cells, int32_t* len, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -539,6 +539,13 @@ struct tslam_octo {
   void* tr_mem;           // per pool block: cost field, traversable bits, neighbour table, epoch (2224 B)
   int tr_ready;           // the kept field can be read (an update completed; cleared by reset, fusion, a failed update)
   int tr_submap;          // submap of the kept field
+  // many-source travel costs (tslam_octo_travel_multi_*), separate from the single-source field
+  void* trm_blk;          // per pool block: traversable bits, compact slot (68 B); change flags, per-source arrays
+  void* trm_mem;          // per compact slot: allowed steps, neighbour table; per (slot, source): field, epoch (grown on demand)
+  size_t trm_bytes;       // bytes of trm_mem
+  int trm_ready;          // the kept fields can be read (an update completed; cleared by reset, fusion, a failed update)
+  int trm_submap;         // submap of the kept fields
+  int trm_S, trm_nt;      // sources and compact slots of the kept fields
 };
 int oc_esdf_free(tslam_octo* m);      // tslam_octo_esdf.cu
 int oc_frontier_free(tslam_octo* m);  // tslam_octo_frontier.cu
@@ -562,6 +569,7 @@ int oc_frontier_readable(tslam_octo* m, int32_t submap, const char* what);
 int oc_frontier_rows(tslam_octo* m, int32_t* idx, int32_t* cluster, cudaStream_t st);
 #define OC_ERR_VIEW_WINDOW 16  // g.err: a viewpoint-gain walk left its view's bitmap window (tslam_octo_view.cu)
 #define OC_ERR_TRAVEL_PATH 32  // g.err: a travel path found no predecessor (impossible at the field's fixed point; tslam_octo_travel.cu)
+#define OC_ERR_TRAVEL_SOURCE 64  // g.err: a many-source travel path named a source outside [0, S) (tslam_octo_travel.cu)
 
 // Amanatides-Woo traversal of the log-odds map in voxel units (DESIGN.md section 7, "Traversal"): p0 = origin / vs,
 // p1 = endpoint / vs, cells c = round_half_away(p).  The k-th boundary crossing of axis a is at

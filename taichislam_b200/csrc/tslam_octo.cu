@@ -577,6 +577,7 @@ extern "C" int tslam_octo_reset(tslam_octo_t* m, void* stream) {
   m->esdf_full_needed = 1;  // pool slots are recycled: the kept ESDF state no longer describes the map
   m->fr_full_needed = 1;    // ... nor the kept frontier set
   m->tr_ready = 0;          // ... nor the kept travel-cost field
+  m->trm_ready = 0;         // ... nor the kept many-source travel-cost fields
   return TSLAM_OK;
 }
 
@@ -639,6 +640,10 @@ static int oc_deferred(tslam_octo* m) {
     }
     if (err == OC_ERR_TRAVEL_PATH) {
       ts_set_error("octo travel path: a cell of the field had no predecessor: paths are invalid");
+      return TSLAM_E_INVALID;
+    }
+    if (err == OC_ERR_TRAVEL_SOURCE) {
+      ts_set_error("octo travel multi path: a source index was outside [0, n_starts): those paths have len 0");
       return TSLAM_E_INVALID;
     }
     ts_set_error("octomap block pool / table exhausted (max_blocks=%d, flags 0x%x): hits were dropped", m->g.max_blocks, err);

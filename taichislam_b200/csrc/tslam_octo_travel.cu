@@ -17,8 +17,10 @@
 //
 // Nothing here writes the map or another tracker's state: no cnt word, mark bit, touched entry, dirty flag or stats
 // counter.
+#include <algorithm>
 #include <cmath>
 #include <cstring>
+#include <vector>
 #include "tslam_esdf_common.cuh"
 
 #define OT_T 10
@@ -377,6 +379,11 @@ int oc_travel_free(tslam_octo* m) {
   if (m->tr_mem) cudaFree(m->tr_mem);
   m->tr_mem = nullptr;
   m->tr_ready = 0;
+  if (m->trm_blk) cudaFree(m->trm_blk);
+  if (m->trm_mem) cudaFree(m->trm_mem);
+  m->trm_blk = m->trm_mem = nullptr;
+  m->trm_bytes = 0;
+  m->trm_ready = 0;
   return TSLAM_OK;
 }
 
@@ -406,6 +413,40 @@ static int ot_readable(tslam_octo* m, int32_t submap, const char* what) {
   return TSLAM_OK;
 }
 
+// the clearance and max_cost checks of every travel update, and the occupancy ESDF the clearance test reads
+static int ot_params(tslam_octo* m, int32_t submap, float clearance, float max_cost, const char* what, OcEsdfField* ef) {
+  const float cost_limit = std::ldexp(m->in.vs, 22);  // keeps G + vs > G for every kept value
+  if (!(std::isfinite(clearance) && clearance >= 0.0f)) {
+    ts_set_error("%s: clearance must be finite and >= 0 (got %g)", what, (double)clearance);
+    return TSLAM_E_INVALID;
+  }
+  if (!(std::isfinite(max_cost) && max_cost > 0.0f && max_cost <= cost_limit)) {
+    ts_set_error("%s: max_cost must be finite, > 0 and <= 2^22 * voxel_scale = %g (got %g)", what, (double)cost_limit, (double)max_cost);
+    return TSLAM_E_INVALID;
+  }
+  memset(ef, 0, sizeof(*ef));
+  if (clearance > 0.0f) {
+    const int rc = oc_esdf_field(m, submap, what, ef);
+    if (rc) return rc;
+    if (clearance > ef->D) {
+      ts_set_error("%s: clearance %g exceeds the occupancy ESDF's max_dist %g", what, (double)clearance, (double)ef->D);
+      return TSLAM_E_INVALID;
+    }
+  }
+  return TSLAM_OK;
+}
+
+// start cell c0 = rha(p / vs) of a finite point, f32 division as the kernels do it; false when outside the volume
+static bool ot_start_cell(const tslam_octo* m, const float* p, int c[3]) {
+  for (int q = 0; q < 3; q++) {
+    const float u = p[q] / m->in.vs;
+    if (!(std::fabs(u) < 1e9f)) return false;
+    c[q] = (int)std::round(u);
+  }
+  return c[0] >= -m->g.hN && c[0] < m->g.N - m->g.hN && c[1] >= -m->g.hN && c[1] < m->g.N - m->g.hN && c[2] >= -m->g.hNz &&
+         c[2] < m->g.Nz - m->g.hNz;
+}
+
 extern "C" int tslam_octo_travel_update(tslam_octo_t* m, int32_t submap, const float* start3, float clearance, float max_cost,
                                         int32_t* stats4, void* stream) {
   const char* what = "tslam_octo_travel_update";
@@ -417,40 +458,16 @@ extern "C" int tslam_octo_travel_update(tslam_octo_t* m, int32_t submap, const f
     return TSLAM_E_INVALID;
   }
   const float vs = m->in.vs;
-  const float cost_limit = std::ldexp(vs, 22);  // keeps G + vs > G for every kept value
-  if (!(std::isfinite(clearance) && clearance >= 0.0f)) {
-    ts_set_error("%s: clearance must be finite and >= 0 (got %g)", what, (double)clearance);
-    return TSLAM_E_INVALID;
-  }
-  if (!(std::isfinite(max_cost) && max_cost > 0.0f && max_cost <= cost_limit)) {
-    ts_set_error("%s: max_cost must be finite, > 0 and <= 2^22 * voxel_scale = %g (got %g)", what, (double)cost_limit, (double)max_cost);
-    return TSLAM_E_INVALID;
-  }
   OcEsdfField ef;
-  memset(&ef, 0, sizeof(ef));
-  if (clearance > 0.0f) {
-    rc = oc_esdf_field(m, submap, what, &ef);
-    if (rc) return rc;
-    if (clearance > ef.D) {
-      ts_set_error("%s: clearance %g exceeds the occupancy ESDF's max_dist %g", what, (double)clearance, (double)ef.D);
-      return TSLAM_E_INVALID;
-    }
-  }
+  rc = ot_params(m, submap, clearance, max_cost, what, &ef);
+  if (rc) return rc;
   if (!m->tr_mem) {
     const size_t bytes = ot_bytes((size_t)m->g.max_blocks);
     TS_CUDA(cudaMalloc(&m->tr_mem, bytes));
     TS_CUDA(cudaMemset(m->tr_mem, 0, bytes));
   }
-  // start cell c0 = rha(p / vs), f32 division as the kernels do it
   int c[3] = {0, 0, 0};
-  bool c_in = true;
-  for (int q = 0; q < 3; q++) {
-    const float u = start3[q] / vs;
-    if (!(std::fabs(u) < 1e9f)) { c_in = false; break; }
-    c[q] = (int)std::round(u);
-  }
-  c_in = c_in && c[0] >= -m->g.hN && c[0] < m->g.N - m->g.hN && c[1] >= -m->g.hN && c[1] < m->g.N - m->g.hN && c[2] >= -m->g.hNz &&
-         c[2] < m->g.Nz - m->g.hNz;
+  const bool c_in = ot_start_cell(m, start3, c);
   cudaStream_t st = (cudaStream_t)stream;
   OtAux a = ot_aux(m);
   m->tr_ready = 0;  // until this update has completed
@@ -518,6 +535,477 @@ extern "C" int tslam_octo_travel_path(tslam_octo_t* m, int32_t submap, int64_t n
   int rc = ot_readable(m, submap, what);
   if (rc || n == 0) return rc;
   k_octo_travel_path<<<ot_grid(m, n), 256, 0, (cudaStream_t)stream>>>(m->g, ot_aux(m), submap, n, xyz, m->in.vs, max_len, cells, len);
+  TS_LAUNCH_CHECK(m);
+  return TSLAM_OK;
+}
+
+// ---- many sources (DESIGN.md section 7, "Many-source travel costs") ------------------------------------------------
+// S fields, one per start, computed in the same launches.  Each field is exactly the single-source field from its start:
+// the same traversability, steps, f32 sums and max_cost cut, and a fixed point that does not depend on the schedule.
+// State scales with the B_t submap blocks that hold a traversable cell (compact slots), not with the pool: per pool
+// block only the traversable bits and the slot; per slot the allowed steps of each voxel (fixed during the wave and the
+// same for every source) and the compact neighbour table; per (slot, source) item the field and an epoch.  Items are
+// numbered t * S + s, so consecutive CTAs of a sweep read the same slot's allowed steps.  The parent's single-source
+// kernels keep their own copies of the traversability test and the relaxation loop: calling the helpers below from them
+// changes their SASS (register allocation in k_octo_travel_init, constant order in k_octo_travel_sweep).
+
+struct OtmAux {
+  uint32_t* trav;  // [max_blocks*16] traversable bits of the update (pool layout)
+  int* slot;       // [max_blocks] compact slot of a block of the update with a traversable cell, else -1
+  int* changed;    // [ES_MAX_SWEEPS+2] changed[k] != 0 <=> sweep k changed something (all sources)
+  int* counts;     // [4] traversable cells, slots (B_t)
+  int* nb_seen;    // blocks in the pool when the last update ran
+  int* start;      // [MAX_STARTS*4] start cell i, j, k, inside the volume
+  int* sitem;      // [MAX_STARTS] item of the start's cell, -1 when it is not traversable
+  int* reach;      // [MAX_STARTS] reachable cells per source
+  int* cblk;       // [B_t] pool block of a slot
+  int* cnbr;       // [B_t*27] compact slots of the 27 neighbour blocks (-1: absent or without a traversable cell)
+  uint32_t* am;    // [B_t*512] allowed steps into each voxel (ot_allowed of its traversable neighbourhood)
+  int* epoch;      // [S*B_t] last sweep in which the item changed (-1: idle)
+  float* G;        // [S*B_t*512] the fields, +inf where unreachable
+  int S, nt;
+};
+
+__device__ __forceinline__ float* otm_field(const OtmAux& a, int t, int s) { return a.G + ((size_t)t * a.S + s) * OC_B3; }
+
+// the traversability test of k_octo_travel_init for cell (i, j, k) with map word w at pool offset o = b * 512 + v
+__device__ __forceinline__ bool ot_traversable(const OcGrid& g, const OcEsdfField& ef, int l_occ, float clearance, bool clear, int enb,
+                                               int b, size_t o, unsigned int w, int i, int j, int k) {
+  bool t = ts_in_bounds(g, i, j, k) && lo_known(w) && lo_val(w) <= l_occ;
+  if (t && clear) t = b < enb && (ef.cls[o] & ef.cls_mask) == ef.free_cls && ef.e[o] >= clearance;
+  return t;
+}
+
+// the relaxation loop of k_octo_travel_sweep: the staged tile in place to local convergence, am[q] the allowed steps into
+// voxel threadIdx.x + q * OT_THREADS; tile.any_write is set when a value changed
+template <class Tile>
+__device__ __forceinline__ void ot_relax(Tile& tile, const unsigned (&am)[OC_B3 / OT_THREADS], float d1, float d2, float d3,
+                                         float max_cost) {
+  for (int iter = 0; iter < 64; ++iter) {
+    if (threadIdx.x == 0) tile.changed = 0;
+    __syncthreads();
+    bool mine = false;
+#pragma unroll
+    for (int q = 0; q < OC_B3 / OT_THREADS; q++) {
+      if (!am[q]) continue;
+      const int v = threadIdx.x + q * OT_THREADS;
+      const int c0 = ot_tidx(v >> 6, (v >> 3) & 7, v & 7);
+      const float cur = tile.G[c0];
+      float best = cur;
+#pragma unroll
+      for (int dx = -1; dx <= 1; dx++)
+#pragma unroll
+        for (int dy = -1; dy <= 1; dy++)
+#pragma unroll
+          for (int dz = -1; dz <= 1; dz++) {
+            const int nz_ = (dx != 0) + (dy != 0) + (dz != 0);
+            if (nz_ == 0 || !((am[q] >> ot_bit(dx, dy, dz)) & 1u)) continue;
+            const float dis = nz_ == 1 ? d1 : (nz_ == 2 ? d2 : d3);
+            const float cand = tile.G[c0 + (dx * OT_T + dy) * OT_T + dz] + dis;
+            if (cand <= max_cost) best = fminf(best, cand);  // (+inf + c is +inf: never kept)
+          }
+      if (best < cur) {
+        tile.G[c0] = best;
+        mine = true;
+      }
+    }
+    if (__any_sync(0xffffffffu, mine) && (threadIdx.x & 31) == 0) tile.changed = 1;
+    __syncthreads();
+    const int ch = tile.changed;
+    if (ch && threadIdx.x == 0) tile.any_write = 1;
+    __syncthreads();
+    if (!ch) break;
+  }
+}
+
+// Every pool block the update sees: traversable bits, and a compact slot for the blocks of the submap with a traversable
+// cell (counts[0] traversable cells, counts[1] slots).  Slots are handed out in any order: the fields do not depend on it.
+__global__ void __launch_bounds__(OT_THREADS) k_octo_travel_multi_classify(OcGrid g, OtmAux a, OcEsdfField ef, int submap, int l_occ,
+                                                                           float clearance) {
+  __shared__ int s_n;
+  const int nb = min(*g.n_blocks, g.max_blocks);
+  if (blockIdx.x == 0 && threadIdx.x == 0) *a.nb_seen = nb;
+  const bool clear = clearance > 0.0f;
+  const int enb = clear ? *ef.nb_seen : 0;
+  for (int b = blockIdx.x; b < nb; b += gridDim.x) {
+    int s, bx, by, bz;
+    ts_unpack_key(g.block_key[b], s, bx, by, bz);
+    if (s != submap) {  // (uniform per CTA)
+      if (threadIdx.x == 0) a.slot[b] = -1;
+      continue;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) s_n = 0;
+    __syncthreads();
+    const size_t base = (size_t)b * OC_B3;
+    int cnt = 0;
+    for (int v = threadIdx.x; v < OC_B3; v += blockDim.x) {
+      const int i = bx * OC_B + (v >> 6), j = by * OC_B + ((v >> 3) & 7), k = bz * OC_B + (v & 7);
+      const bool t = ot_traversable(g, ef, l_occ, clearance, clear, enb, b, base + v, g.cnt[base + v], i, j, k);
+      const unsigned m = __ballot_sync(0xffffffffu, t);
+      if ((threadIdx.x & 31) == 0) a.trav[(size_t)b * OT_WORDS + (v >> 5)] = m;
+      cnt += t ? 1 : 0;
+    }
+    for (int o = 16; o > 0; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+    if ((threadIdx.x & 31) == 0 && cnt) atomicAdd(&s_n, cnt);
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      a.slot[b] = s_n ? atomicAdd(&a.counts[1], 1) : -1;
+      if (s_n) atomicAdd(&a.counts[0], s_n);
+    }
+  }
+}
+
+// Per slot: its pool block, the compact neighbour table, and the allowed steps into each voxel from the traversable bits
+// of its 3^3 block neighbourhood (staged as a 10^3 byte tile, as k_octo_travel_sweep stages them)
+__global__ void __launch_bounds__(OT_THREADS) k_octo_travel_multi_tables(OcGrid g, OtmAux a) {
+  __shared__ unsigned char t_[OT_T3];
+  __shared__ int nbr[27];
+  const int nb = *a.nb_seen;
+  for (int b = blockIdx.x; b < nb; b += gridDim.x) {
+    const int t = a.slot[b];
+    if (t < 0) continue;  // (uniform per CTA)
+    __syncthreads();
+    if (threadIdx.x < 27) {
+      int s, bx, by, bz;
+      ts_unpack_key(g.block_key[b], s, bx, by, bz);
+      const int dx = threadIdx.x / 9 - 1, dy = (threadIdx.x / 3) % 3 - 1, dz = threadIdx.x % 3 - 1;
+      int n = ts_find(g, ts_pack_key(s, bx + dx, by + dy, bz + dz));
+      n = n < nb ? n : -1;
+      nbr[threadIdx.x] = n;
+      a.cnbr[(size_t)t * 27 + threadIdx.x] = n >= 0 ? a.slot[n] : -1;
+      if (threadIdx.x == 0) a.cblk[t] = b;
+    }
+    __syncthreads();
+    for (int c = threadIdx.x; c < OT_T3; c += blockDim.x) {
+      const int lz = c % OT_T - 1, ly = (c / OT_T) % OT_T - 1, lx = c / (OT_T * OT_T) - 1;
+      const int nbk = nbr[(((lx + 8) >> 3) * 3 + ((ly + 8) >> 3)) * 3 + ((lz + 8) >> 3)];
+      const int off = oc_voxel_off(lx, ly, lz);
+      t_[c] = nbk >= 0 ? (unsigned char)((a.trav[(size_t)nbk * OT_WORDS + (off >> 5)] >> (off & 31)) & 1u) : 0;
+    }
+    __syncthreads();
+    for (int v = threadIdx.x; v < OC_B3; v += blockDim.x) {
+      const int c0 = ot_tidx(v >> 6, (v >> 3) & 7, v & 7);
+      unsigned nm = 0u;
+#pragma unroll
+      for (int dx = -1; dx <= 1; dx++)
+#pragma unroll
+        for (int dy = -1; dy <= 1; dy++)
+#pragma unroll
+          for (int dz = -1; dz <= 1; dz++) nm |= (unsigned)t_[c0 + (dx * OT_T + dy) * OT_T + dz] << ot_bit(dx, dy, dz);
+      a.am[(size_t)t * OC_B3 + v] = ot_allowed(nm);
+    }
+  }
+}
+
+// every item: G = +inf, idle
+__global__ void __launch_bounds__(OT_THREADS) k_octo_travel_multi_fill(OtmAux a) {
+  const long long items = (long long)a.S * a.nt;
+  const float inf = __int_as_float(0x7f800000);
+  for (long long it = blockIdx.x; it < items; it += gridDim.x) {
+    float* G = a.G + (size_t)it * OC_B3;
+    for (int v = threadIdx.x; v < OC_B3; v += blockDim.x) G[v] = inf;
+    if (threadIdx.x == 0) a.epoch[it] = -1;
+  }
+}
+
+// one thread per source: G = 0 and epoch 0 at a traversable start cell (its item in sitem), else sitem = -1
+__global__ void k_octo_travel_multi_starts(OcGrid g, OtmAux a, int submap) {
+  const int s = blockIdx.x * blockDim.x + threadIdx.x;
+  if (s >= a.S) return;
+  const int* c = a.start + 4 * s;
+  int item = -1;
+  if (c[3]) {
+    const int b = ot_block(g, submap, *a.nb_seen, c);
+    const int t = b >= 0 ? a.slot[b] : -1;
+    const int off = oc_voxel_off(c[0], c[1], c[2]);
+    if (t >= 0 && ((a.trav[(size_t)b * OT_WORDS + (off >> 5)] >> (off & 31)) & 1u)) {
+      item = t * a.S + s;
+      otm_field(a, t, s)[off] = 0.0f;
+      a.epoch[item] = 0;
+    }
+  }
+  a.sitem[s] = item;
+}
+
+struct OtmTile {
+  float G[OT_T3];
+  int nbr[27];  // neighbour items of the same source (-1: none)
+  int active, changed, any_write;
+};
+
+// One sweep of the S waves: relax the items the wave fronts reach to local convergence.  An item is active when one of
+// its 27 neighbour items of the same source was stamped in the previous sweep or later.
+__global__ void __launch_bounds__(OT_THREADS) k_octo_travel_multi_sweep(OtmAux a, int sweep, float vs, float max_cost) {
+  __shared__ OtmTile tile;
+  if (sweep > 1 && a.changed[sweep - 1] == 0) return;  // already converged: nothing to do
+  const long long items = (long long)a.S * a.nt;
+  const float d1 = vs, d2 = sqrtf(2.0f) * vs, d3 = sqrtf(3.0f) * vs;  // the edge costs of k_octo_esdf_sweep
+  for (long long it = blockIdx.x; it < items; it += gridDim.x) {
+    const int t = (int)(it / a.S), s = (int)(it % a.S);
+    __syncthreads();
+    if (threadIdx.x == 0) { tile.active = 0; tile.any_write = 0; }
+    __syncthreads();
+    if (threadIdx.x < 27) {
+      const int n = a.cnbr[(size_t)t * 27 + threadIdx.x];
+      const int ni = n >= 0 ? n * a.S + s : -1;
+      tile.nbr[threadIdx.x] = ni;
+      if (ni >= 0 && *(volatile int*)&a.epoch[ni] >= sweep - 1) tile.active = 1;
+    }
+    __syncthreads();
+    if (!tile.active) continue;
+    for (int c = threadIdx.x; c < OT_T3; c += blockDim.x) {
+      const int lz = c % OT_T - 1, ly = (c / OT_T) % OT_T - 1, lx = c / (OT_T * OT_T) - 1;
+      const int ni = tile.nbr[(((lx + 8) >> 3) * 3 + ((ly + 8) >> 3)) * 3 + ((lz + 8) >> 3)];
+      tile.G[c] = ni >= 0 ? *(volatile float*)&a.G[(size_t)ni * OC_B3 + oc_voxel_off(lx, ly, lz)] : __int_as_float(0x7f800000);
+    }
+    unsigned am[OC_B3 / OT_THREADS];
+#pragma unroll
+    for (int q = 0; q < OC_B3 / OT_THREADS; q++) am[q] = a.am[(size_t)t * OC_B3 + threadIdx.x + q * OT_THREADS];
+    __syncthreads();
+    ot_relax(tile, am, d1, d2, d3, max_cost);
+    if (tile.any_write) {
+      float* G = a.G + (size_t)it * OC_B3;
+      for (int v = threadIdx.x; v < OC_B3; v += blockDim.x) G[v] = tile.G[ot_tidx(v >> 6, (v >> 3) & 7, v & 7)];
+      if (threadIdx.x == 0) {
+        __threadfence();
+        a.epoch[it] = sweep;
+        a.changed[sweep] = 1;
+      }
+    }
+  }
+}
+
+// reachable cells per source after the waves -> reach[s]
+__global__ void __launch_bounds__(OT_THREADS) k_octo_travel_multi_count(OtmAux a) {
+  __shared__ int s_n;
+  const long long items = (long long)a.S * a.nt;
+  for (long long it = blockIdx.x; it < items; it += gridDim.x) {
+    if (a.epoch[it] < 0) continue;  // never reached: all +inf (uniform per CTA)
+    __syncthreads();
+    if (threadIdx.x == 0) s_n = 0;
+    __syncthreads();
+    int cnt = 0;
+    for (int v = threadIdx.x; v < OC_B3; v += blockDim.x) cnt += isfinite(a.G[(size_t)it * OC_B3 + v]) ? 1 : 0;
+    for (int o = 16; o > 0; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+    if ((threadIdx.x & 31) == 0 && cnt) atomicAdd(&s_n, cnt);
+    __syncthreads();
+    if (threadIdx.x == 0 && s_n) atomicAdd(&a.reach[it % a.S], s_n);
+  }
+}
+
+// slot of the cell of a point in the update's blocks, -1 when outside the volume, not finite, in a newer block or in a
+// block without a traversable cell (whose cells all read +inf)
+__device__ __forceinline__ int otm_slot(const OcGrid& g, const OtmAux& a, int submap, int nb_seen, float vs, const float* p, int c[3]) {
+  if (!ot_cell(g, vs, p, c)) return -1;
+  const int b = ot_block(g, submap, nb_seen, c);
+  return b >= 0 ? a.slot[b] : -1;
+}
+
+// cost[s * n + q] = G_s of the cell of point q: one thread per point, looping over the sources
+__global__ void __launch_bounds__(256) k_octo_travel_multi_query(OcGrid g, OtmAux a, int submap, long long n, const float* __restrict__ xyz,
+                                                                 float vs, float* __restrict__ cost) {
+  const int nb_seen = *a.nb_seen;
+  for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < n; q += (long long)gridDim.x * blockDim.x) {
+    int c[3];
+    const int t = otm_slot(g, a, submap, nb_seen, vs, xyz + 3 * q, c);
+    const int off = t >= 0 ? oc_voxel_off(c[0], c[1], c[2]) : 0;
+    for (int s = 0; s < a.S; s++) cost[(size_t)s * n + q] = t >= 0 ? otm_field(a, t, s)[off] : __int_as_float(0x7f800000);
+  }
+}
+
+// Path from the cell of xyz[q] back to the start of field source[q], with the predecessor rule of k_octo_travel_path
+// (exact f32 equality, smallest G(h), ties in ot_bit order) over the compact slots and their allowed steps.  A source
+// outside [0, S) writes len 0 and sets OC_ERR_TRAVEL_SOURCE, reported by the next tslam_octo_sync.
+__global__ void __launch_bounds__(256) k_octo_travel_multi_path(OcGrid g, OtmAux a, int submap, long long n, const int32_t* __restrict__ source,
+                                                                const float* __restrict__ xyz, float vs, int max_len,
+                                                                int32_t* __restrict__ cells, int32_t* __restrict__ len) {
+  const int nb_seen = *a.nb_seen;
+  const float d1 = vs, d2 = sqrtf(2.0f) * vs, d3 = sqrtf(3.0f) * vs;
+  const float inf = __int_as_float(0x7f800000);
+  for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < n; q += (long long)gridDim.x * blockDim.x) {
+    const int s = source[q];
+    int L = 0;
+    if (s < 0 || s >= a.S) {
+      atomicOr(g.err, OC_ERR_TRAVEL_SOURCE);
+      len[q] = 0;
+      continue;
+    }
+    int c[3];
+    int t = otm_slot(g, a, submap, nb_seen, vs, xyz + 3 * q, c);
+    float gv = t >= 0 ? otm_field(a, t, s)[oc_voxel_off(c[0], c[1], c[2])] : inf;
+    int32_t* out = cells + 3 * (size_t)q * max_len;
+    while (gv < inf) {
+      if (L < max_len) { out[3 * L] = c[0]; out[3 * L + 1] = c[1]; out[3 * L + 2] = c[2]; }
+      ++L;
+      if (gv == 0.0f) break;  // the start: the only cell at 0
+      const int bx = c[0] >> OC_BSHIFT, by = c[1] >> OC_BSHIFT, bz = c[2] >> OC_BSHIFT;
+      const unsigned am = a.am[(size_t)t * OC_B3 + oc_voxel_off(c[0], c[1], c[2])];
+      int best = -1, bt = -1;
+      float bg = inf;
+#pragma unroll
+      for (int e = 0; e < 27; e++) {
+        if (!((am >> e) & 1u)) continue;  // (never the cell itself)
+        const int dx = e / 9 - 1, dy = (e / 3) % 3 - 1, dz = e % 3 - 1;
+        const int i = c[0] + dx, j = c[1] + dy, k = c[2] + dz;
+        const int tn = a.cnbr[(size_t)t * 27 + ot_bit((i >> OC_BSHIFT) - bx, (j >> OC_BSHIFT) - by, (k >> OC_BSHIFT) - bz)];
+        const float hg = otm_field(a, tn, s)[oc_voxel_off(i, j, k)];  // (an allowed step's cell is traversable: tn >= 0)
+        const int nz_ = (dx != 0) + (dy != 0) + (dz != 0);
+        const float dis = nz_ == 1 ? d1 : (nz_ == 2 ? d2 : d3);
+        if (hg < bg && hg + dis == gv) { best = e; bg = hg; bt = tn; }
+      }
+      if (best < 0) {  // cannot happen at the fixed point: reported by the next tslam_octo_sync, never a silent cut
+        atomicOr(g.err, OC_ERR_TRAVEL_PATH);
+        L = 0;
+        break;
+      }
+      c[0] += best / 9 - 1; c[1] += (best / 3) % 3 - 1; c[2] += best % 3 - 1;
+      t = bt;
+      gv = bg;
+    }
+    len[q] = L;
+  }
+}
+
+// per pool block: traversable bits 64 + slot 4 = 68 B; then change flags, counts and the per-source arrays
+static size_t otm_blk_bytes(size_t nb) {
+  return nb * (OT_WORDS * 4 + 4) + ((ES_MAX_SWEEPS + 2) + 8 + TSLAM_OCTO_TRAVEL_MAX_STARTS * 6) * 4;
+}
+// per slot: pool block 4 + neighbour table 108 + allowed steps 2048 = 2160 B; per item: field 2048 + epoch 4 = 2052 B
+static size_t otm_bytes(size_t nt, size_t S) { return nt * (4 + 27 * 4 + OC_B3 * 4) + S * nt * (OC_B3 * 4 + 4); }
+
+static OtmAux otm_aux(tslam_octo* m, int S, int nt) {
+  const size_t nb = (size_t)m->g.max_blocks;
+  OtmAux a;
+  a.trav = (uint32_t*)m->trm_blk;
+  a.slot = (int*)(a.trav + nb * OT_WORDS);
+  a.changed = a.slot + nb;
+  a.counts = a.changed + (ES_MAX_SWEEPS + 2);
+  a.nb_seen = a.counts + 4;
+  a.start = a.counts + 8;
+  a.sitem = a.start + 4 * TSLAM_OCTO_TRAVEL_MAX_STARTS;
+  a.reach = a.sitem + TSLAM_OCTO_TRAVEL_MAX_STARTS;
+  a.am = (uint32_t*)m->trm_mem;  // (the two 2 KB-per-row arrays first: 128-byte aligned rows)
+  a.G = (float*)(a.am + (size_t)nt * OC_B3);
+  a.epoch = (int*)(a.G + (size_t)S * nt * OC_B3);
+  a.cblk = a.epoch + (size_t)S * nt;
+  a.cnbr = a.cblk + nt;
+  a.S = S;
+  a.nt = nt;
+  return a;
+}
+
+static int otm_readable(tslam_octo* m, int32_t submap, const char* what) {
+  int rc = ot_check(m, submap, what);
+  if (rc) return rc;
+  if (!m->trm_ready) {
+    ts_set_error("%s: no completed tslam_octo_travel_multi_update since the map was created, reset or fused, or since the last one "
+                 "failed", what);
+    return TSLAM_E_INVALID;
+  }
+  if (m->trm_submap != submap) {
+    ts_set_error("%s: the last tslam_octo_travel_multi_update was for submap %d, not %d", what, m->trm_submap, submap);
+    return TSLAM_E_INVALID;
+  }
+  return TSLAM_OK;
+}
+
+extern "C" int tslam_octo_travel_multi_update(tslam_octo_t* m, int32_t submap, int32_t n_starts, const float* starts, float clearance,
+                                              float max_cost, int32_t* stats2, int32_t* reachable, uint8_t* start_ok, void* stream) {
+  const char* what = "tslam_octo_travel_multi_update";
+  if (!m || !starts) return TSLAM_E_INVALID;
+  int rc = ot_check(m, submap, what);
+  if (rc) return rc;
+  if (n_starts < 1 || n_starts > TSLAM_OCTO_TRAVEL_MAX_STARTS) {
+    ts_set_error("%s: n_starts must be in [1, %d] (got %d)", what, TSLAM_OCTO_TRAVEL_MAX_STARTS, n_starts);
+    return TSLAM_E_INVALID;
+  }
+  for (int q = 0; q < 3 * n_starts; q++)
+    if (!std::isfinite(starts[q])) {
+      ts_set_error("%s: start %d is not finite", what, q / 3);
+      return TSLAM_E_INVALID;
+    }
+  OcEsdfField ef;
+  rc = ot_params(m, submap, clearance, max_cost, what, &ef);
+  if (rc) return rc;
+  const int S = n_starts;
+  m->trm_ready = 0;  // until this update has completed
+  if (!m->trm_blk) TS_CUDA(cudaMalloc(&m->trm_blk, otm_blk_bytes((size_t)m->g.max_blocks)));
+  std::vector<int> h_start(4 * (size_t)S);
+  for (int s = 0; s < S; s++) h_start[4 * s + 3] = ot_start_cell(m, starts + 3 * s, &h_start[4 * s]) ? 1 : 0;
+  cudaStream_t st = (cudaStream_t)stream;
+  OtmAux a = otm_aux(m, S, 0);
+  TS_CUDA(cudaMemsetAsync(a.changed, 0, ((ES_MAX_SWEEPS + 2) + 4) * 4, st));  // changed, counts
+  TS_CUDA(cudaMemsetAsync(a.reach, 0, (size_t)S * 4, st));
+  TS_CUDA(cudaMemcpyAsync(a.start, h_start.data(), h_start.size() * 4, cudaMemcpyHostToDevice, st));
+  const int grid = m->sm_count * 8;
+  k_octo_travel_multi_classify<<<grid, OT_THREADS, 0, st>>>(m->g, a, ef, submap, m->lo.l_occ, clearance);
+  TS_LAUNCH_CHECK(m);
+  int h_counts[2] = {0, 0};
+  TS_CUDA(cudaMemcpyAsync(h_counts, a.counts, 8, cudaMemcpyDeviceToHost, st));
+  TS_CUDA(cudaStreamSynchronize(st));
+  const int nt = h_counts[1];
+  const size_t bytes = std::max(otm_bytes((size_t)nt, (size_t)S), (size_t)256);
+  if (bytes > m->trm_bytes) {  // grow on demand
+    if (m->trm_mem) cudaFree(m->trm_mem);
+    m->trm_mem = nullptr;
+    m->trm_bytes = 0;
+    TS_CUDA(cudaMalloc(&m->trm_mem, bytes));
+    m->trm_bytes = bytes;
+  }
+  a = otm_aux(m, S, nt);
+  k_octo_travel_multi_tables<<<grid, OT_THREADS, 0, st>>>(m->g, a);
+  TS_LAUNCH_CHECK(m);
+  k_octo_travel_multi_fill<<<m->sm_count * 16, OT_THREADS, 0, st>>>(a);
+  TS_LAUNCH_CHECK(m);
+  k_octo_travel_multi_starts<<<(S + 127) / 128, 128, 0, st>>>(m->g, a, submap);
+  TS_LAUNCH_CHECK(m);
+  const int sgrid = m->sm_count * 16;
+  int sweeps = 0;
+  rc = es_wave(m, st, a.changed, ES_GROUP,
+               [&](int k) { k_octo_travel_multi_sweep<<<sgrid, OT_THREADS, 0, st>>>(a, k, m->in.vs, max_cost); }, &sweeps);
+  if (rc) return rc;
+  if (sweeps > ES_MAX_SWEEPS) {
+    ts_set_error("%s: the waves were still changing after %d sweeps; the fields are incomplete and their readers refuse", what, ES_MAX_SWEEPS);
+    return TSLAM_E_INVALID;
+  }
+  k_octo_travel_multi_count<<<sgrid, OT_THREADS, 0, st>>>(a);
+  TS_LAUNCH_CHECK(m);
+  std::vector<int> h_reach(S), h_item(S);
+  TS_CUDA(cudaMemcpyAsync(h_reach.data(), a.reach, (size_t)S * 4, cudaMemcpyDeviceToHost, st));
+  TS_CUDA(cudaMemcpyAsync(h_item.data(), a.sitem, (size_t)S * 4, cudaMemcpyDeviceToHost, st));
+  TS_CUDA(cudaStreamSynchronize(st));
+  m->trm_ready = 1;
+  m->trm_submap = submap;
+  m->trm_S = S;
+  m->trm_nt = nt;
+  if (stats2) { stats2[0] = sweeps; stats2[1] = h_counts[0]; }
+  for (int s = 0; s < S; s++) {
+    if (reachable) reachable[s] = h_reach[s];
+    if (start_ok) start_ok[s] = h_item[s] >= 0 ? 1 : 0;
+  }
+  return TSLAM_OK;
+}
+
+extern "C" int tslam_octo_travel_multi_query(tslam_octo_t* m, int32_t submap, int64_t n, const float* xyz, float* cost, void* stream) {
+  if (!m || n < 0 || (n && (!xyz || !cost))) return TSLAM_E_INVALID;
+  int rc = otm_readable(m, submap, "tslam_octo_travel_multi_query");
+  if (rc || n == 0) return rc;
+  k_octo_travel_multi_query<<<ot_grid(m, n), 256, 0, (cudaStream_t)stream>>>(m->g, otm_aux(m, m->trm_S, m->trm_nt), submap, n, xyz,
+                                                                             m->in.vs, cost);
+  TS_LAUNCH_CHECK(m);
+  return TSLAM_OK;
+}
+
+extern "C" int tslam_octo_travel_multi_path(tslam_octo_t* m, int32_t submap, int64_t n, const int32_t* source, const float* xyz,
+                                            int32_t max_len, int32_t* cells, int32_t* len, void* stream) {
+  if (!m || n < 0 || (n && (!source || !xyz || !cells || !len))) return TSLAM_E_INVALID;
+  const char* what = "tslam_octo_travel_multi_path";
+  if (max_len < 1) { ts_set_error("%s: max_len must be >= 1 (got %d)", what, max_len); return TSLAM_E_INVALID; }
+  int rc = otm_readable(m, submap, what);
+  if (rc || n == 0) return rc;
+  k_octo_travel_multi_path<<<ot_grid(m, n), 256, 0, (cudaStream_t)stream>>>(m->g, otm_aux(m, m->trm_S, m->trm_nt), submap, n, source, xyz,
+                                                                            m->in.vs, max_len, cells, len);
   TS_LAUNCH_CHECK(m);
   return TSLAM_OK;
 }

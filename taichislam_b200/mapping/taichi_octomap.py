@@ -292,6 +292,47 @@ class Octomap(BaseMap):
         vs = float(np.float32(self._h.cfg.voxel_scale))
         return cells[0, :n][::-1].astype(np.float64) * vs
 
+    def travel_update_multi(self, starts, clearance=0.0, max_cost=None):
+        """Travel-cost fields of the active submap from each of S starts [S,3] (metres, map frame; 1 <= S <= 1024) in one
+        update, row s exactly what travel_update(starts[s]) computes -> dict(sweeps, traversable, reachable int32[S],
+        start_ok bool[S]).  clearance and max_cost as for travel_update (which also runs esdf_update() first)."""
+        self._travel_map()
+        if float(clearance) > 0.0:
+            d = float(getattr(self, "esdf_max_dist", None) or self.max_ray_length)
+            if np.float32(clearance) > np.float32(d):
+                raise ValueError(f"clearance {clearance} exceeds the ESDF's max_dist {d}: call esdf_update(max_dist) with a "
+                                 "larger max_dist first")
+            self.esdf_update(d)
+        return self._h.travel_multi_update(self._active(), starts, clearance, max_cost)
+
+    def travel_cost_multi(self, xyz):
+        """Travel costs [S,n] of the cells of points [n,3] from each start of the last travel_update_multi, +inf where
+        unreachable; travel_cost_multi(starts) is the S x S matrix (not symmetrised: entry [s,t] and [t,s] may differ in
+        the last bits).  A torch CUDA tensor for a torch tensor, a numpy array for a numpy array."""
+        self._travel_map()
+        return self._h.travel_multi_query(xyz, submap=self._active())
+
+    def travel_path_multi(self, source, goal, max_len=4096):
+        """The path from start `source` of the last travel_update_multi to the cell of `goal` [3] as cell centres in
+        metres, [n,3] ordered start to goal, or None when the goal is unreachable from that start."""
+        self._travel_map()
+        if isinstance(goal, self._torch.Tensor):
+            goal = goal.detach().cpu().numpy()
+        g = np.asarray(goal, np.float32).reshape(1, 3)
+        S = getattr(self._h, "_travel_multi_S", 0)
+        if not 0 <= int(source) < S:
+            raise ValueError(f"source {source} is not a start of the last travel_update_multi ({S} starts)")
+        src = np.array([int(source)], np.int32)
+        cells, n = self._h.travel_multi_path(src, g, submap=self._active(), max_len=max_len)
+        n = int(n[0])
+        if n == 0:
+            return None
+        if n > max_len:   # the buffer was too small: once more with the reported length
+            cells, n2 = self._h.travel_multi_path(src, g, submap=self._active(), max_len=n)
+            assert int(n2[0]) == n
+        vs = float(np.float32(self._h.cfg.voxel_scale))
+        return cells[0, :n][::-1].astype(np.float64) * vs
+
     def saveMap(self, path):  # :201-202 (stub in the reference)
         pass
 

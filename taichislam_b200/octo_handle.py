@@ -420,6 +420,53 @@ class OctoHandle:
         self.sync()
         return cells.cpu().numpy(), ln.cpu().numpy()
 
+    def travel_multi_update(self, submap, starts, clearance=0.0, max_cost=None):
+        """Travel-cost fields of `submap` from each of S starts [S,3] (metres, submap frame; 1 <= S <= 1024) in one update,
+        row s exactly the field travel_update(starts[s]) would compute; clearance and max_cost as there -> dict(sweeps,
+        traversable, reachable int32[S], start_ok bool[S])."""
+        p = capi.f32c(starts).reshape(-1, 3)
+        S = p.shape[0]
+        st = np.zeros(2, np.int32)
+        reach = np.zeros(max(S, 1), np.int32)
+        ok = np.zeros(max(S, 1), np.uint8)
+        mc = self.travel_limit() if max_cost is None else float(max_cost)
+        capi.check(self.L.tslam_octo_travel_multi_update(self.h, int(submap), S, capi.np_ptr(p), float(clearance), mc, capi.np_ptr(st),
+                                                         capi.np_ptr(reach), capi.np_ptr(ok), capi.stream_ptr()))
+        self._travel_multi_S = S
+        return dict(sweeps=int(st[0]), traversable=int(st[1]), reachable=reach[:S].copy(), start_ok=ok[:S].astype(bool))
+
+    def travel_multi_query(self, xyz, submap=0):
+        """Travel costs f32[S,n] of the cells of points [n,3] from each start of the last travel_multi_update (+inf where
+        unreachable); the starts themselves give the S x S matrix.  Torch in -> torch out without a host
+        synchronisation; numpy in -> numpy out."""
+        torch = self.torch
+        as_torch, x = self._points(xyz)
+        n = x.shape[0]
+        cost = torch.empty((getattr(self, "_travel_multi_S", 0), n), dtype=torch.float32, device=x.device)
+        capi.check(self.L.tslam_octo_travel_multi_query(self.h, int(submap), n, capi.tptr(x), capi.tptr(cost), capi.stream_ptr()))
+        return cost if as_torch else cost.cpu().numpy()
+
+    def travel_multi_path(self, source, xyz, submap=0, max_len=4096):
+        """Paths of pairs (source[q], xyz[q]) from the cell of the target back to starts[source[q]] of the last
+        travel_multi_update -> (cells int32[n,max_len,3], len int32[n]) as travel_path returns them.  A source outside
+        [0, S) gets len 0 and the next sync() raises.  Torch in -> torch out without a host synchronisation; numpy in ->
+        numpy out."""
+        torch = self.torch
+        as_torch, x = self._points(xyz)
+        n = x.shape[0]
+        if isinstance(source, torch.Tensor):
+            src = source.to(device=x.device, dtype=torch.int32).reshape(-1).contiguous()
+        else:
+            src = torch.from_numpy(np.ascontiguousarray(np.asarray(source, np.int32).reshape(-1))).to(x.device)
+        assert src.shape[0] == n, "source [n] and xyz [n,3] need the same n"
+        cells = torch.empty((n, int(max_len), 3), dtype=torch.int32, device=x.device)
+        ln = torch.empty(n, dtype=torch.int32, device=x.device)
+        capi.check(self.L.tslam_octo_travel_multi_path(self.h, int(submap), n, capi.tptr(src), capi.tptr(x), int(max_len), capi.tptr(cells),
+                                                       capi.tptr(ln), capi.stream_ptr()))
+        if as_torch:
+            return cells, ln
+        return cells.cpu().numpy(), ln.cpu().numpy()
+
     def raycast(self, pos, direction, max_dist, submap=0):
         torch = self.torch
         p = torch.from_numpy(np.ascontiguousarray(pos, dtype=np.float32)).cuda()

@@ -548,7 +548,9 @@ int tslam_octo_view_gain_frontier(tslam_octo_t* m, int32_t submap, int64_t n, co
  * allowed iff every cell of the box their two cells span is traversable (no corner cutting).  G(start) = 0 when the
  * start cell round_half_away(start / voxel_scale) is traversable; every other cell holds the least f32 path sum, added
  * one step at a time; a cell above max_cost is unreachable (+inf).  Every call refuses a hit-counter map and a submap out
- * of range (TSLAM_E_INVALID).  State (allocated by the first update): 2224 B per pool block.
+ * of range (TSLAM_E_INVALID).  The field is the S = 1 case of the many-source fields below, in a state of its own: 68 B
+ * per pool block plus ~4.2 KB per submap block with a traversable cell, allocated by the first update, grown
+ * geometrically and freed by tslam_octo_destroy.
  * --------------------------------------------------------------------------*/
 /* Compute the field of `submap` from start3 (HOST, finite).  clearance finite and >= 0 (> 0 needs a readable occupancy
  * ESDF of the submap whose max_dist is >= clearance); max_cost finite, > 0 and <= 2^22 * vs.  A start that is not
@@ -577,7 +579,7 @@ int tslam_octo_travel_path(tslam_octo_t* m, int32_t submap, int64_t n, const flo
  * and may differ in the last bits; nothing symmetrises them.  Under the default max_cost (2^22 * vs) reachability is
  * symmetric.  The fields are separate from the single-source field: an update of either changes nothing the other's
  * readers return.  State: 68 B per pool block, plus ~2.1 KB per submap block with a traversable cell (B_t) and ~2 KB per
- * (block, source) pair, grown on demand and freed by tslam_octo_destroy. */
+ * (block, source) pair, grown geometrically (at least x2 per growth) and freed by tslam_octo_destroy. */
 #define TSLAM_OCTO_TRAVEL_MAX_STARTS 1024
 /* Compute the fields from starts[n_starts,3] (HOST, finite, 1 <= n_starts <= TSLAM_OCTO_TRAVEL_MAX_STARTS, duplicates
  * allowed); clearance and max_cost as for tslam_octo_travel_update.  stats2 (HOST, may be NULL): sweeps, traversable

@@ -495,6 +495,15 @@ struct OcLo {             // per-frame workspace of a log-odds map (allocated in
   float min_ray, max_ray; // f32(min_ray_length), f32(max_ray_length)
   int l_hit, l_miss, l_min, l_max, l_occ;
 };
+// S travel-cost fields of one submap as of one update (tslam_octo_travel.cu), allocated by the first update
+struct OcTravel {
+  void* blk;      // per pool block: traversable bits, compact slot (68 B); change flags, per-source arrays
+  void* mem;      // per compact slot: allowed steps, neighbour table; per (slot, source): field, epoch (grown geometrically)
+  size_t bytes;   // bytes of mem
+  int ready;      // the kept fields can be read (an update completed; cleared by reset, fusion, a failed update)
+  int submap;     // submap of the kept fields
+  int S, nt;      // sources and compact slots of the kept fields
+};
 struct tslam_octo {
   tslam_octo_config_t cfg;
   OcGrid g;
@@ -535,17 +544,9 @@ struct tslam_octo {
   // rows of the frontier gain (grown on demand, freed by tslam_octo_destroy)
   void* vw_mem;
   size_t vw_bytes;
-  // travel-cost field of a log-odds map (tslam_octo_travel_*, tslam_octo_travel.cu), allocated by the first update
-  void* tr_mem;           // per pool block: cost field, traversable bits, neighbour table, epoch (2224 B)
-  int tr_ready;           // the kept field can be read (an update completed; cleared by reset, fusion, a failed update)
-  int tr_submap;          // submap of the kept field
-  // many-source travel costs (tslam_octo_travel_multi_*), separate from the single-source field
-  void* trm_blk;          // per pool block: traversable bits, compact slot (68 B); change flags, per-source arrays
-  void* trm_mem;          // per compact slot: allowed steps, neighbour table; per (slot, source): field, epoch (grown on demand)
-  size_t trm_bytes;       // bytes of trm_mem
-  int trm_ready;          // the kept fields can be read (an update completed; cleared by reset, fusion, a failed update)
-  int trm_submap;         // submap of the kept fields
-  int trm_S, trm_nt;      // sources and compact slots of the kept fields
+  // travel-cost fields of a log-odds map (tslam_octo_travel_*, tslam_octo_travel.cu): the single-source field
+  // (tslam_octo_travel_update, S = 1) and the many-source fields (tslam_octo_travel_multi_update), kept apart
+  OcTravel tr, trm;
 };
 int oc_esdf_free(tslam_octo* m);      // tslam_octo_esdf.cu
 int oc_frontier_free(tslam_octo* m);  // tslam_octo_frontier.cu

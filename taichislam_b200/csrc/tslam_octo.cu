@@ -576,8 +576,8 @@ extern "C" int tslam_octo_reset(tslam_octo_t* m, void* stream) {
   TS_CUDA(cudaMemsetAsync(m->scratch_i, 0, 4 * 4, st));
   m->esdf_full_needed = 1;  // pool slots are recycled: the kept ESDF state no longer describes the map
   m->fr_full_needed = 1;    // ... nor the kept frontier set
-  m->tr_ready = 0;          // ... nor the kept travel-cost field
-  m->trm_ready = 0;         // ... nor the kept many-source travel-cost fields
+  m->tr.ready = 0;          // ... nor the kept travel-cost fields
+  m->trm.ready = 0;
   return TSLAM_OK;
 }
 

@@ -1,4 +1,5 @@
-// libtslam.so - travel-cost field of a log-odds Octomap (DESIGN.md section 7, "Travel cost on the log-odds Octomap").
+// libtslam.so - travel-cost fields of a log-odds Octomap (DESIGN.md section 7, "Travel cost on the log-odds Octomap" and
+// "Many-source travel costs").
 //
 // Per submap, as of one update.  Classes as the occupancy ESDF defines them: OCC = known and L > l_occ, FREE = known and
 // L <= l_occ, UNKNOWN = not known (every cell of an absent block).  A cell is traversable iff it is inside the volume and
@@ -10,10 +11,13 @@
 // to the fixed point.  f32 addition is monotone and, below the bound max_cost <= 2^22 vs, G + c > G: the fixed point is
 // unique, equals Dijkstra's answer and does not depend on the schedule (DESIGN.md section 7 gives the argument).
 //
-// The scheme is the occupancy ESDF's lower wave (k_octo_esdf_sweep): a CTA stages its 8^3 block plus a one-voxel halo of
-// G and traversability in shared memory and relaxes it in place to local convergence (values only decrease); sweep k
-// runs the blocks with a neighbour stamped >= k-1, starting from the start's block, and es_wave drives the sweeps.  A
-// step's box lies inside the 3^3 neighbourhood of its target cell, so the step rule never leaves the staged tile.
+// One update computes S such fields, one per start, in the same launches.  The single-source API
+// (tslam_octo_travel_update and its readers) is the S = 1 case, kept in a state of its own so that it and the
+// many-source fields never change each other's answers.  The scheme is the occupancy ESDF's lower wave
+// (k_octo_esdf_sweep): a CTA stages one (block, source) item plus a one-voxel halo of G in shared memory and relaxes it
+// in place to local convergence (values only decrease); sweep k runs the items with a neighbour item of the same source
+// stamped >= k-1, starting from the starts' items, and es_wave drives the sweeps.  A step's box lies inside the 3^3
+// neighbourhood of its target cell, so the step rule never leaves the staged tile.
 //
 // Nothing here writes the map or another tracker's state: no cnt word, mark bit, touched entry, dirty flag or stats
 // counter.
@@ -27,16 +31,6 @@
 #define OT_T3 (OT_T * OT_T * OT_T)
 #define OT_THREADS 128
 #define OT_WORDS 16  // traversable bits per pool block: 512 bits
-
-struct OtAux {
-  float* G;        // [max_blocks*512] the field, +inf where unreachable
-  uint32_t* trav;  // [max_blocks*16] traversable bits of the update: bit (o & 31) of word o >> 5 for voxel offset o
-  int* nbr;        // [max_blocks*27] neighbour block indices of the update (-1 = absent)
-  int* epoch;      // [max_blocks] last sweep in which the block changed (-1: idle, < -1: block of another submap)
-  int* changed;    // [ES_MAX_SWEEPS+2] changed[k] != 0 <=> sweep k changed something
-  int* counts;     // [4] traversable cells, reachable cells, start_ok, (spare)
-  int* nb_seen;    // blocks in the pool when the last update ran (bump allocation: higher indices are newer)
-};
 
 // bit of neighbourhood offset (dx, dy, dz) in a 27-bit mask: dx outermost, the OFFSETS order of the reference
 __host__ __device__ constexpr int ot_bit(int dx, int dy, int dz) { return (dx + 1) * 9 + (dy + 1) * 3 + (dz + 1); }
@@ -67,212 +61,6 @@ __device__ __forceinline__ unsigned ot_allowed(unsigned nm) {
 
 __device__ __forceinline__ int ot_tidx(int lx, int ly, int lz) { return ((lx + 1) * OT_T + (ly + 1)) * OT_T + (lz + 1); }
 
-// Every block of the submap: traversable bits (with the clearance test against the occupancy ESDF), G = +inf or 0 at
-// c0, the neighbour table, epoch 0 on the start's block when c0 is traversable, idle on the others.  A pool slot
-// recycled after a reset is overwritten like any other, so no old value survives.
-__global__ void __launch_bounds__(OT_THREADS) k_octo_travel_init(OcGrid g, OtAux a, OcEsdfField ef, int submap, int l_occ, float clearance,
-                                                                 int ci, int cj, int ck, int c_in) {
-  __shared__ int s_n, s_start;
-  const int nb = min(*g.n_blocks, g.max_blocks);
-  if (blockIdx.x == 0 && threadIdx.x == 0) *a.nb_seen = nb;
-  const bool clear = clearance > 0.0f;
-  const int enb = clear ? *ef.nb_seen : 0;
-  const float inf = __int_as_float(0x7f800000);
-  for (int b = blockIdx.x; b < nb; b += gridDim.x) {
-    int s, bx, by, bz;
-    ts_unpack_key(g.block_key[b], s, bx, by, bz);
-    if (s != submap) {  // (uniform per CTA)
-      if (threadIdx.x == 0) a.epoch[b] = -1000000;
-      continue;
-    }
-    __syncthreads();
-    if (threadIdx.x == 0) { s_n = 0; s_start = 0; }
-    __syncthreads();
-    if (threadIdx.x < 27) {
-      const int dx = threadIdx.x / 9 - 1, dy = (threadIdx.x / 3) % 3 - 1, dz = threadIdx.x % 3 - 1;
-      a.nbr[b * 27 + threadIdx.x] = ts_find(g, ts_pack_key(s, bx + dx, by + dy, bz + dz));
-    }
-    const size_t base = (size_t)b * OC_B3;
-    const bool sblk = c_in && (ci >> OC_BSHIFT) == bx && (cj >> OC_BSHIFT) == by && (ck >> OC_BSHIFT) == bz;
-    int cnt = 0;
-    for (int v = threadIdx.x; v < OC_B3; v += blockDim.x) {
-      const int i = bx * OC_B + (v >> 6), j = by * OC_B + ((v >> 3) & 7), k = bz * OC_B + (v & 7);
-      const unsigned int w = g.cnt[base + v];
-      bool t = ts_in_bounds(g, i, j, k) && lo_known(w) && lo_val(w) <= l_occ;
-      if (t && clear) t = b < enb && (ef.cls[base + v] & ef.cls_mask) == ef.free_cls && ef.e[base + v] >= clearance;
-      const unsigned m = __ballot_sync(0xffffffffu, t);
-      if ((threadIdx.x & 31) == 0) a.trav[(size_t)b * OT_WORDS + (v >> 5)] = m;
-      float gv = inf;
-      if (t && sblk && i == ci && j == cj && k == ck) { gv = 0.0f; s_start = 1; }
-      a.G[base + v] = gv;
-      cnt += t ? 1 : 0;
-    }
-    for (int o = 16; o > 0; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
-    if ((threadIdx.x & 31) == 0 && cnt) atomicAdd(&s_n, cnt);
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      a.epoch[b] = s_start ? 0 : -1;
-      if (s_start) a.counts[2] = 1;
-      if (s_n) atomicAdd(&a.counts[0], s_n);
-    }
-  }
-}
-
-struct OtTile {
-  float G[OT_T3];
-  unsigned char t[OT_T3];
-  int nbr[27];
-  int active, changed, any_write;
-};
-
-// block + one-voxel halo into shared memory (absent neighbour blocks read unreachable and not traversable)
-__device__ __forceinline__ void ot_stage(const OtAux& a, OtTile& tile) {
-  for (int c = threadIdx.x; c < OT_T3; c += blockDim.x) {
-    const int lz = c % OT_T - 1, ly = (c / OT_T) % OT_T - 1, lx = c / (OT_T * OT_T) - 1;
-    const int nbk = tile.nbr[(((lx + 8) >> 3) * 3 + ((ly + 8) >> 3)) * 3 + ((lz + 8) >> 3)];
-    float gv = __int_as_float(0x7f800000);
-    unsigned char tv = 0;
-    if (nbk >= 0) {
-      const int off = oc_voxel_off(lx, ly, lz);
-      tv = (unsigned char)((a.trav[(size_t)nbk * OT_WORDS + (off >> 5)] >> (off & 31)) & 1u);
-      gv = *(volatile float*)&a.G[(size_t)nbk * OC_B3 + off];
-    }
-    tile.G[c] = gv;
-    tile.t[c] = tv;
-  }
-}
-
-// One sweep of the wave: relax the blocks the wave front reaches to local convergence
-__global__ void __launch_bounds__(OT_THREADS) k_octo_travel_sweep(OcGrid g, OtAux a, int sweep, float vs, float max_cost) {
-  __shared__ OtTile tile;
-  if (sweep > 1 && a.changed[sweep - 1] == 0) return;  // already converged: nothing to do
-  const int nb = min(*a.nb_seen, g.max_blocks);
-  const float d1 = vs, d2 = sqrtf(2.0f) * vs, d3 = sqrtf(3.0f) * vs;  // the edge costs of k_octo_esdf_sweep
-  for (int b = blockIdx.x; b < nb; b += gridDim.x) {
-    __syncthreads();
-    if (threadIdx.x == 0) { tile.active = 0; tile.any_write = 0; }
-    __syncthreads();
-    if (a.epoch[b] < -1) continue;  // block of another submap (uniform per CTA)
-    if (threadIdx.x < 27) {
-      const int n = a.nbr[b * 27 + threadIdx.x];
-      tile.nbr[threadIdx.x] = n;
-      if (n >= 0 && *(volatile int*)&a.epoch[n] >= sweep - 1) tile.active = 1;  // the wave front reaches this block
-    }
-    __syncthreads();
-    if (!tile.active) continue;
-    ot_stage(a, tile);
-    __syncthreads();
-    // the allowed steps into each of this thread's voxels: traversability is fixed during the wave
-    unsigned am[OC_B3 / OT_THREADS];
-#pragma unroll
-    for (int q = 0; q < OC_B3 / OT_THREADS; q++) {
-      const int v = threadIdx.x + q * OT_THREADS;
-      const int c0 = ot_tidx(v >> 6, (v >> 3) & 7, v & 7);
-      unsigned nm = 0u;
-#pragma unroll
-      for (int dx = -1; dx <= 1; dx++)
-#pragma unroll
-        for (int dy = -1; dy <= 1; dy++)
-#pragma unroll
-          for (int dz = -1; dz <= 1; dz++) nm |= (unsigned)tile.t[c0 + (dx * OT_T + dy) * OT_T + dz] << ot_bit(dx, dy, dz);
-      am[q] = ot_allowed(nm);
-    }
-    // relax to local convergence (values only decrease, so in-place racy updates are safe)
-    for (int iter = 0; iter < 64; ++iter) {
-      if (threadIdx.x == 0) tile.changed = 0;
-      __syncthreads();
-      bool mine = false;
-#pragma unroll
-      for (int q = 0; q < OC_B3 / OT_THREADS; q++) {
-        if (!am[q]) continue;
-        const int v = threadIdx.x + q * OT_THREADS;
-        const int c0 = ot_tidx(v >> 6, (v >> 3) & 7, v & 7);
-        const float cur = tile.G[c0];
-        float best = cur;
-#pragma unroll
-        for (int dx = -1; dx <= 1; dx++)
-#pragma unroll
-          for (int dy = -1; dy <= 1; dy++)
-#pragma unroll
-            for (int dz = -1; dz <= 1; dz++) {
-              const int nz_ = (dx != 0) + (dy != 0) + (dz != 0);
-              if (nz_ == 0 || !((am[q] >> ot_bit(dx, dy, dz)) & 1u)) continue;
-              const float dis = nz_ == 1 ? d1 : (nz_ == 2 ? d2 : d3);
-              const float cand = tile.G[c0 + (dx * OT_T + dy) * OT_T + dz] + dis;
-              if (cand <= max_cost) best = fminf(best, cand);  // (+inf + c is +inf: never kept)
-            }
-        if (best < cur) {
-          tile.G[c0] = best;
-          mine = true;
-        }
-      }
-      if (__any_sync(0xffffffffu, mine) && (threadIdx.x & 31) == 0) tile.changed = 1;
-      __syncthreads();
-      const int ch = tile.changed;
-      if (ch && threadIdx.x == 0) tile.any_write = 1;
-      __syncthreads();
-      if (!ch) break;
-    }
-    if (tile.any_write) {
-      const size_t base = (size_t)b * OC_B3;
-      for (int v = threadIdx.x; v < OC_B3; v += blockDim.x) a.G[base + v] = tile.G[ot_tidx(v >> 6, (v >> 3) & 7, v & 7)];
-      if (threadIdx.x == 0) {
-        __threadfence();
-        a.epoch[b] = sweep;
-        a.changed[sweep] = 1;
-      }
-    }
-  }
-}
-
-// reachable cells of the submap after the wave -> counts[1]
-__global__ void __launch_bounds__(OT_THREADS) k_octo_travel_count(OcGrid g, OtAux a) {
-  __shared__ int s_n;
-  const int nb = min(*a.nb_seen, g.max_blocks);
-  for (int b = blockIdx.x; b < nb; b += gridDim.x) {
-    if (a.epoch[b] < -1) continue;  // (uniform per CTA)
-    __syncthreads();
-    if (threadIdx.x == 0) s_n = 0;
-    __syncthreads();
-    const size_t base = (size_t)b * OC_B3;
-    int cnt = 0;
-    for (int v = threadIdx.x; v < OC_B3; v += blockDim.x) cnt += isfinite(a.G[base + v]) ? 1 : 0;
-    for (int o = 16; o > 0; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
-    if ((threadIdx.x & 31) == 0 && cnt) atomicAdd(&s_n, cnt);
-    __syncthreads();
-    if (threadIdx.x == 0 && s_n) atomicAdd(&a.counts[1], s_n);
-  }
-}
-
-// (ijk, G) of every reachable cell, in the blocks the update saw
-__global__ void __launch_bounds__(OT_THREADS) k_octo_travel_gather(OcGrid g, OtAux a, int submap, long long cap, int32_t* idx, float* cost,
-                                                                   unsigned long long* counter) {
-  const int nb = min(*a.nb_seen, g.max_blocks);
-  for (int b = blockIdx.x; b < nb; b += gridDim.x) {
-    int s, bx, by, bz;
-    ts_unpack_key(g.block_key[b], s, bx, by, bz);
-    if (s != submap) continue;  // (uniform per CTA)
-    const size_t base = (size_t)b * OC_B3;
-    for (int v = threadIdx.x; v < OC_B3; v += blockDim.x) {
-      const float gv = a.G[base + v];
-      const bool want = isfinite(gv);
-      const unsigned m = __ballot_sync(0xffffffffu, want);
-      if (!m) continue;
-      const int lane = threadIdx.x & 31, leader = __ffs(m) - 1;
-      unsigned long long rb = 0;
-      if (lane == leader) rb = atomicAdd(counter, (unsigned long long)__popc(m));
-      rb = __shfl_sync(0xffffffffu, rb, leader);
-      const long long row = (long long)(rb + __popc(m & ((1u << lane) - 1)));
-      if (want && row < cap) {
-        idx[3 * row] = bx * OC_B + (v >> 6);
-        idx[3 * row + 1] = by * OC_B + ((v >> 3) & 7);
-        idx[3 * row + 2] = bz * OC_B + (v & 7);
-        cost[row] = gv;
-      }
-    }
-  }
-}
-
 // cell rha(p / vs) of a point, and whether it is inside the volume (false for a non-finite coordinate)
 __device__ __forceinline__ bool ot_cell(const OcGrid& g, float vs, const float* p, int c[3]) {
   const float u0 = __fdiv_rn(p[0], vs), u1 = __fdiv_rn(p[1], vs), u2 = __fdiv_rn(p[2], vs);
@@ -287,268 +75,10 @@ __device__ __forceinline__ int ot_block(const OcGrid& g, int submap, int nb_seen
   return (b >= 0 && b < nb_seen) ? b : -1;
 }
 
-// G of the cell of each point; +inf where unreachable, outside the volume, in a newer block or not finite
-__global__ void __launch_bounds__(256) k_octo_travel_query(OcGrid g, OtAux a, int submap, long long n, const float* __restrict__ xyz, float vs,
-                                                           float* __restrict__ cost) {
-  const int nb_seen = *a.nb_seen;
-  for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < n; q += (long long)gridDim.x * blockDim.x) {
-    int c[3];
-    float gv = __int_as_float(0x7f800000);
-    if (ot_cell(g, vs, xyz + 3 * q, c)) {
-      const int b = ot_block(g, submap, nb_seen, c);
-      if (b >= 0) gv = a.G[(size_t)b * OC_B3 + oc_voxel_off(c[0], c[1], c[2])];
-    }
-    cost[q] = gv;
-  }
-}
-
-// Path from the cell of each target to the start: from the current cell v, the predecessor is the reachable
-// 26-neighbour h with an allowed step and G(h) + c == G(v) exactly, smallest G(h), ties to the first in ot_bit order.
-// One hash probe for the target's block; the walk moves through the update's neighbour table.
-__global__ void __launch_bounds__(256) k_octo_travel_path(OcGrid g, OtAux a, int submap, long long n, const float* __restrict__ xyz, float vs,
-                                                          int max_len, int32_t* __restrict__ cells, int32_t* __restrict__ len) {
-  const int nb_seen = *a.nb_seen;
-  const float d1 = vs, d2 = sqrtf(2.0f) * vs, d3 = sqrtf(3.0f) * vs;
-  const float inf = __int_as_float(0x7f800000);
-  for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < n; q += (long long)gridDim.x * blockDim.x) {
-    int c[3];
-    int L = 0;
-    int b = ot_cell(g, vs, xyz + 3 * q, c) ? ot_block(g, submap, nb_seen, c) : -1;
-    float gv = b >= 0 ? a.G[(size_t)b * OC_B3 + oc_voxel_off(c[0], c[1], c[2])] : inf;
-    int32_t* out = cells + 3 * (size_t)q * max_len;
-    while (gv < inf) {
-      if (L < max_len) { out[3 * L] = c[0]; out[3 * L + 1] = c[1]; out[3 * L + 2] = c[2]; }
-      ++L;
-      if (gv == 0.0f) break;  // the start: the only cell at 0
-      const int bx = c[0] >> OC_BSHIFT, by = c[1] >> OC_BSHIFT, bz = c[2] >> OC_BSHIFT;
-      // traversability of the 3^3 neighbourhood as the update left it, then the costs of the allowed steps only
-      unsigned nm = 0u;
-#pragma unroll
-      for (int e = 0; e < 27; e++) {
-        const int i = c[0] + e / 9 - 1, j = c[1] + (e / 3) % 3 - 1, k = c[2] + e % 3 - 1;
-        const int nb_ = a.nbr[b * 27 + ot_bit((i >> OC_BSHIFT) - bx, (j >> OC_BSHIFT) - by, (k >> OC_BSHIFT) - bz)];
-        const int off = oc_voxel_off(i, j, k);
-        if (nb_ >= 0) nm |= ((a.trav[(size_t)nb_ * OT_WORDS + (off >> 5)] >> (off & 31)) & 1u) << e;
-      }
-      const unsigned am = ot_allowed(nm);
-      int best = -1;
-      float bg = inf;
-#pragma unroll
-      for (int e = 0; e < 27; e++) {
-        if (!((am >> e) & 1u)) continue;  // (never the cell itself)
-        const int dx = e / 9 - 1, dy = (e / 3) % 3 - 1, dz = e % 3 - 1;
-        const int i = c[0] + dx, j = c[1] + dy, k = c[2] + dz;
-        const int nb_ = a.nbr[b * 27 + ot_bit((i >> OC_BSHIFT) - bx, (j >> OC_BSHIFT) - by, (k >> OC_BSHIFT) - bz)];
-        const float hg = a.G[(size_t)nb_ * OC_B3 + oc_voxel_off(i, j, k)];  // (an allowed step's cell is traversable: nb_ >= 0)
-        const int nz_ = (dx != 0) + (dy != 0) + (dz != 0);
-        const float dis = nz_ == 1 ? d1 : (nz_ == 2 ? d2 : d3);
-        if (hg < bg && hg + dis == gv) { best = e; bg = hg; }
-      }
-      if (best < 0) {  // cannot happen at the fixed point: reported by the next tslam_octo_sync, never a silent cut
-        atomicOr(g.err, OC_ERR_TRAVEL_PATH);
-        L = 0;
-        break;
-      }
-      const int i = c[0] + best / 9 - 1, j = c[1] + (best / 3) % 3 - 1, k = c[2] + best % 3 - 1;
-      b = a.nbr[b * 27 + ot_bit((i >> OC_BSHIFT) - bx, (j >> OC_BSHIFT) - by, (k >> OC_BSHIFT) - bz)];
-      c[0] = i; c[1] = j; c[2] = k;
-      gv = bg;
-    }
-    len[q] = L;
-  }
-}
-
-// ---- host side -----------------------------------------------------------------------------------------------------
-// bytes per pool block: field 2048 + traversable bits 64 + neighbour table 108 + epoch 4 = 2224
-static size_t ot_bytes(size_t nb) { return nb * (OC_B3 * 4 + OT_WORDS * 4 + 28 * 4) + ((ES_MAX_SWEEPS + 2) + 8) * 4; }
-
-static OtAux ot_aux(tslam_octo* m) {
-  const size_t nb = (size_t)m->g.max_blocks;
-  OtAux a;
-  a.G = (float*)m->tr_mem;
-  a.trav = (uint32_t*)(a.G + nb * OC_B3);
-  a.nbr = (int*)(a.trav + nb * OT_WORDS);
-  a.epoch = a.nbr + nb * 27;
-  a.changed = a.epoch + nb;
-  a.counts = a.changed + (ES_MAX_SWEEPS + 2);
-  a.nb_seen = a.counts + 4;
-  return a;
-}
-
-int oc_travel_free(tslam_octo* m) {
-  if (m->tr_mem) cudaFree(m->tr_mem);
-  m->tr_mem = nullptr;
-  m->tr_ready = 0;
-  if (m->trm_blk) cudaFree(m->trm_blk);
-  if (m->trm_mem) cudaFree(m->trm_mem);
-  m->trm_blk = m->trm_mem = nullptr;
-  m->trm_bytes = 0;
-  m->trm_ready = 0;
-  return TSLAM_OK;
-}
-
-// the checks every travel call makes first
-static int ot_check(tslam_octo* m, int32_t submap, const char* what) {
-  if (!m->logodds) {
-    ts_set_error("%s: the map is a hit counter; a travel-cost field needs a log-odds map (tslam_octo_create_logodds)", what);
-    return TSLAM_E_INVALID;
-  }
-  if (submap < 0 || submap >= m->cfg.max_submaps) { ts_set_error("%s: submap %d out of range", what, submap); return TSLAM_E_INVALID; }
-  return TSLAM_OK;
-}
-
-// the field of `submap` can be read: an update has completed, for that submap, and no reset or fusion came after it
-static int ot_readable(tslam_octo* m, int32_t submap, const char* what) {
-  int rc = ot_check(m, submap, what);
-  if (rc) return rc;
-  if (!m->tr_mem) { ts_set_error("%s: no travel-cost field has been computed (tslam_octo_travel_update has not run)", what); return TSLAM_E_INVALID; }
-  if (!m->tr_ready) {
-    ts_set_error("%s: the map was reset or fused, or the last tslam_octo_travel_update failed, since the last completed update", what);
-    return TSLAM_E_INVALID;
-  }
-  if (m->tr_submap != submap) {
-    ts_set_error("%s: the last tslam_octo_travel_update was for submap %d, not %d", what, m->tr_submap, submap);
-    return TSLAM_E_INVALID;
-  }
-  return TSLAM_OK;
-}
-
-// the clearance and max_cost checks of every travel update, and the occupancy ESDF the clearance test reads
-static int ot_params(tslam_octo* m, int32_t submap, float clearance, float max_cost, const char* what, OcEsdfField* ef) {
-  const float cost_limit = std::ldexp(m->in.vs, 22);  // keeps G + vs > G for every kept value
-  if (!(std::isfinite(clearance) && clearance >= 0.0f)) {
-    ts_set_error("%s: clearance must be finite and >= 0 (got %g)", what, (double)clearance);
-    return TSLAM_E_INVALID;
-  }
-  if (!(std::isfinite(max_cost) && max_cost > 0.0f && max_cost <= cost_limit)) {
-    ts_set_error("%s: max_cost must be finite, > 0 and <= 2^22 * voxel_scale = %g (got %g)", what, (double)cost_limit, (double)max_cost);
-    return TSLAM_E_INVALID;
-  }
-  memset(ef, 0, sizeof(*ef));
-  if (clearance > 0.0f) {
-    const int rc = oc_esdf_field(m, submap, what, ef);
-    if (rc) return rc;
-    if (clearance > ef->D) {
-      ts_set_error("%s: clearance %g exceeds the occupancy ESDF's max_dist %g", what, (double)clearance, (double)ef->D);
-      return TSLAM_E_INVALID;
-    }
-  }
-  return TSLAM_OK;
-}
-
-// start cell c0 = rha(p / vs) of a finite point, f32 division as the kernels do it; false when outside the volume
-static bool ot_start_cell(const tslam_octo* m, const float* p, int c[3]) {
-  for (int q = 0; q < 3; q++) {
-    const float u = p[q] / m->in.vs;
-    if (!(std::fabs(u) < 1e9f)) return false;
-    c[q] = (int)std::round(u);
-  }
-  return c[0] >= -m->g.hN && c[0] < m->g.N - m->g.hN && c[1] >= -m->g.hN && c[1] < m->g.N - m->g.hN && c[2] >= -m->g.hNz &&
-         c[2] < m->g.Nz - m->g.hNz;
-}
-
-extern "C" int tslam_octo_travel_update(tslam_octo_t* m, int32_t submap, const float* start3, float clearance, float max_cost,
-                                        int32_t* stats4, void* stream) {
-  const char* what = "tslam_octo_travel_update";
-  if (!m || !start3) return TSLAM_E_INVALID;
-  int rc = ot_check(m, submap, what);
-  if (rc) return rc;
-  if (!(std::isfinite(start3[0]) && std::isfinite(start3[1]) && std::isfinite(start3[2]))) {
-    ts_set_error("%s: the start must be finite", what);
-    return TSLAM_E_INVALID;
-  }
-  const float vs = m->in.vs;
-  OcEsdfField ef;
-  rc = ot_params(m, submap, clearance, max_cost, what, &ef);
-  if (rc) return rc;
-  if (!m->tr_mem) {
-    const size_t bytes = ot_bytes((size_t)m->g.max_blocks);
-    TS_CUDA(cudaMalloc(&m->tr_mem, bytes));
-    TS_CUDA(cudaMemset(m->tr_mem, 0, bytes));
-  }
-  int c[3] = {0, 0, 0};
-  const bool c_in = ot_start_cell(m, start3, c);
-  cudaStream_t st = (cudaStream_t)stream;
-  OtAux a = ot_aux(m);
-  m->tr_ready = 0;  // until this update has completed
-  TS_CUDA(cudaMemsetAsync(a.changed, 0, ((ES_MAX_SWEEPS + 2) + 4) * 4, st));  // changed, counts
-  const int grid = m->sm_count * 8;
-  k_octo_travel_init<<<grid, OT_THREADS, 0, st>>>(m->g, a, ef, submap, m->lo.l_occ, clearance, c[0], c[1], c[2], c_in ? 1 : 0);
-  TS_LAUNCH_CHECK(m);
-  int sweeps = 0;
-  rc = es_wave(m, st, a.changed, ES_GROUP, [&](int k) { k_octo_travel_sweep<<<grid, OT_THREADS, 0, st>>>(m->g, a, k, vs, max_cost); },
-               &sweeps);
-  if (rc) return rc;
-  if (sweeps > ES_MAX_SWEEPS) {  // the last sweep still changed something: the field is not the fixed point
-    ts_set_error("%s: the wave was still changing after %d sweeps; the field is incomplete and its readers refuse", what, ES_MAX_SWEEPS);
-    return TSLAM_E_INVALID;
-  }
-  k_octo_travel_count<<<grid, OT_THREADS, 0, st>>>(m->g, a);
-  TS_LAUNCH_CHECK(m);
-  int h_counts[4] = {0, 0, 0, 0};
-  TS_CUDA(cudaMemcpyAsync(h_counts, a.counts, 16, cudaMemcpyDeviceToHost, st));
-  TS_CUDA(cudaStreamSynchronize(st));
-  m->tr_ready = 1;
-  m->tr_submap = submap;
-  if (stats4) { stats4[0] = h_counts[1]; stats4[1] = sweeps; stats4[2] = h_counts[0]; stats4[3] = h_counts[2]; }
-  return TSLAM_OK;
-}
-
-extern "C" int tslam_octo_travel_gather(tslam_octo_t* m, int32_t submap, int64_t cap, int32_t* idx, float* cost, int64_t* n_out,
-                                        void* stream) {
-  if (!m || !n_out || cap < 0 || (cap > 0 && (!idx || !cost))) return TSLAM_E_INVALID;
-  int rc = ot_readable(m, submap, "tslam_octo_travel_gather");
-  if (rc) return rc;
-  cudaStream_t st = (cudaStream_t)stream;
-  unsigned long long* ctr = (unsigned long long*)(m->scratch_i + 8);
-  TS_CUDA(cudaMemsetAsync(ctr, 0, 8, st));
-  k_octo_travel_gather<<<m->sm_count * 8, OT_THREADS, 0, st>>>(m->g, ot_aux(m), submap, cap, idx, cost, ctr);
-  TS_LAUNCH_CHECK(m);
-  unsigned long long v = 0;
-  TS_CUDA(cudaMemcpyAsync(&v, ctr, 8, cudaMemcpyDeviceToHost, st));
-  TS_CUDA(cudaStreamSynchronize(st));
-  *n_out = (int64_t)v;
-  if ((int64_t)v > cap) { ts_set_error("octo travel gather: %lld cells > capacity %lld", (long long)v, (long long)cap); return TSLAM_E_CAPACITY; }
-  return TSLAM_OK;
-}
-
-static int ot_grid(tslam_octo* m, long long n) {
-  long long blocks = (n + 255) / 256;
-  if (blocks > (long long)m->sm_count * 16) blocks = (long long)m->sm_count * 16;
-  return (int)blocks;
-}
-
-extern "C" int tslam_octo_travel_query(tslam_octo_t* m, int32_t submap, int64_t n, const float* xyz, float* cost, void* stream) {
-  if (!m || n < 0 || (n && (!xyz || !cost))) return TSLAM_E_INVALID;
-  int rc = ot_readable(m, submap, "tslam_octo_travel_query");
-  if (rc || n == 0) return rc;
-  k_octo_travel_query<<<ot_grid(m, n), 256, 0, (cudaStream_t)stream>>>(m->g, ot_aux(m), submap, n, xyz, m->in.vs, cost);
-  TS_LAUNCH_CHECK(m);
-  return TSLAM_OK;
-}
-
-extern "C" int tslam_octo_travel_path(tslam_octo_t* m, int32_t submap, int64_t n, const float* xyz, int32_t max_len, int32_t* cells,
-                                      int32_t* len, void* stream) {
-  if (!m || n < 0 || (n && (!xyz || !cells || !len))) return TSLAM_E_INVALID;
-  const char* what = "tslam_octo_travel_path";
-  if (max_len < 1) { ts_set_error("%s: max_len must be >= 1 (got %d)", what, max_len); return TSLAM_E_INVALID; }
-  int rc = ot_readable(m, submap, what);
-  if (rc || n == 0) return rc;
-  k_octo_travel_path<<<ot_grid(m, n), 256, 0, (cudaStream_t)stream>>>(m->g, ot_aux(m), submap, n, xyz, m->in.vs, max_len, cells, len);
-  TS_LAUNCH_CHECK(m);
-  return TSLAM_OK;
-}
-
-// ---- many sources (DESIGN.md section 7, "Many-source travel costs") ------------------------------------------------
-// S fields, one per start, computed in the same launches.  Each field is exactly the single-source field from its start:
-// the same traversability, steps, f32 sums and max_cost cut, and a fixed point that does not depend on the schedule.
 // State scales with the B_t submap blocks that hold a traversable cell (compact slots), not with the pool: per pool
 // block only the traversable bits and the slot; per slot the allowed steps of each voxel (fixed during the wave and the
 // same for every source) and the compact neighbour table; per (slot, source) item the field and an epoch.  Items are
-// numbered t * S + s, so consecutive CTAs of a sweep read the same slot's allowed steps.  The parent's single-source
-// kernels keep their own copies of the traversability test and the relaxation loop: calling the helpers below from them
-// changes their SASS (register allocation in k_octo_travel_init, constant order in k_octo_travel_sweep).
-
+// numbered t * S + s, so consecutive CTAs of a sweep read the same slot's allowed steps.
 struct OtmAux {
   uint32_t* trav;  // [max_blocks*16] traversable bits of the update (pool layout)
   int* slot;       // [max_blocks] compact slot of a block of the update with a traversable cell, else -1
@@ -568,7 +98,7 @@ struct OtmAux {
 
 __device__ __forceinline__ float* otm_field(const OtmAux& a, int t, int s) { return a.G + ((size_t)t * a.S + s) * OC_B3; }
 
-// the traversability test of k_octo_travel_init for cell (i, j, k) with map word w at pool offset o = b * 512 + v
+// the traversability test for cell (i, j, k) with map word w at pool offset o = b * 512 + v
 __device__ __forceinline__ bool ot_traversable(const OcGrid& g, const OcEsdfField& ef, int l_occ, float clearance, bool clear, int enb,
                                                int b, size_t o, unsigned int w, int i, int j, int k) {
   bool t = ts_in_bounds(g, i, j, k) && lo_known(w) && lo_val(w) <= l_occ;
@@ -576,10 +106,15 @@ __device__ __forceinline__ bool ot_traversable(const OcGrid& g, const OcEsdfFiel
   return t;
 }
 
-// the relaxation loop of k_octo_travel_sweep: the staged tile in place to local convergence, am[q] the allowed steps into
+struct OtmTile {
+  float G[OT_T3];
+  int nbr[27];  // neighbour items of the same source (-1: none)
+  int active, changed, any_write;
+};
+
+// the relaxation loop of a sweep: the staged tile in place to local convergence, am[q] the allowed steps into
 // voxel threadIdx.x + q * OT_THREADS; tile.any_write is set when a value changed
-template <class Tile>
-__device__ __forceinline__ void ot_relax(Tile& tile, const unsigned (&am)[OC_B3 / OT_THREADS], float d1, float d2, float d3,
+__device__ __forceinline__ void ot_relax(OtmTile& tile, const unsigned (&am)[OC_B3 / OT_THREADS], float d1, float d2, float d3,
                                          float max_cost) {
   for (int iter = 0; iter < 64; ++iter) {
     if (threadIdx.x == 0) tile.changed = 0;
@@ -657,7 +192,7 @@ __global__ void __launch_bounds__(OT_THREADS) k_octo_travel_multi_classify(OcGri
 }
 
 // Per slot: its pool block, the compact neighbour table, and the allowed steps into each voxel from the traversable bits
-// of its 3^3 block neighbourhood (staged as a 10^3 byte tile, as k_octo_travel_sweep stages them)
+// of its 3^3 block neighbourhood (staged as a 10^3 byte tile)
 __global__ void __launch_bounds__(OT_THREADS) k_octo_travel_multi_tables(OcGrid g, OtmAux a) {
   __shared__ unsigned char t_[OT_T3];
   __shared__ int nbr[27];
@@ -728,12 +263,6 @@ __global__ void k_octo_travel_multi_starts(OcGrid g, OtmAux a, int submap) {
   a.sitem[s] = item;
 }
 
-struct OtmTile {
-  float G[OT_T3];
-  int nbr[27];  // neighbour items of the same source (-1: none)
-  int active, changed, any_write;
-};
-
 // One sweep of the S waves: relax the items the wave fronts reach to local convergence.  An item is active when one of
 // its 27 neighbour items of the same source was stamped in the previous sweep or later.
 __global__ void __launch_bounds__(OT_THREADS) k_octo_travel_multi_sweep(OtmAux a, int sweep, float vs, float max_cost) {
@@ -794,6 +323,34 @@ __global__ void __launch_bounds__(OT_THREADS) k_octo_travel_multi_count(OtmAux a
   }
 }
 
+// (ijk, G) of every reachable cell of field s (blocks without a slot hold no traversable cell and list nothing)
+__global__ void __launch_bounds__(OT_THREADS) k_octo_travel_slot_gather(OcGrid g, OtmAux a, int s, long long cap, int32_t* idx, float* cost,
+                                                                        unsigned long long* counter) {
+  for (int t = blockIdx.x; t < a.nt; t += gridDim.x) {
+    if (a.epoch[(size_t)t * a.S + s] < 0) continue;  // never reached: all +inf (uniform per CTA)
+    int sm, bx, by, bz;
+    ts_unpack_key(g.block_key[a.cblk[t]], sm, bx, by, bz);
+    const float* G = otm_field(a, t, s);
+    for (int v = threadIdx.x; v < OC_B3; v += blockDim.x) {
+      const float gv = G[v];
+      const bool want = isfinite(gv);
+      const unsigned m = __ballot_sync(0xffffffffu, want);
+      if (!m) continue;
+      const int lane = threadIdx.x & 31, leader = __ffs(m) - 1;
+      unsigned long long rb = 0;
+      if (lane == leader) rb = atomicAdd(counter, (unsigned long long)__popc(m));
+      rb = __shfl_sync(0xffffffffu, rb, leader);
+      const long long row = (long long)(rb + __popc(m & ((1u << lane) - 1)));
+      if (want && row < cap) {
+        idx[3 * row] = bx * OC_B + (v >> 6);
+        idx[3 * row + 1] = by * OC_B + ((v >> 3) & 7);
+        idx[3 * row + 2] = bz * OC_B + (v & 7);
+        cost[row] = gv;
+      }
+    }
+  }
+}
+
 // slot of the cell of a point in the update's blocks, -1 when outside the volume, not finite, in a newer block or in a
 // block without a traversable cell (whose cells all read +inf)
 __device__ __forceinline__ int otm_slot(const OcGrid& g, const OtmAux& a, int submap, int nb_seen, float vs, const float* p, int c[3]) {
@@ -814,9 +371,10 @@ __global__ void __launch_bounds__(256) k_octo_travel_multi_query(OcGrid g, OtmAu
   }
 }
 
-// Path from the cell of xyz[q] back to the start of field source[q], with the predecessor rule of k_octo_travel_path
-// (exact f32 equality, smallest G(h), ties in ot_bit order) over the compact slots and their allowed steps.  A source
-// outside [0, S) writes len 0 and sets OC_ERR_TRAVEL_SOURCE, reported by the next tslam_octo_sync.
+// Path from the cell of xyz[q] back to the start of field source[q] (field 0 when source is NULL): from the current cell
+// v, the predecessor is the reachable 26-neighbour h with an allowed step and G(h) + c == G(v) exactly, smallest G(h),
+// ties to the first in ot_bit order, walked over the compact slots and their allowed steps.  A source outside [0, S)
+// writes len 0 and sets OC_ERR_TRAVEL_SOURCE, reported by the next tslam_octo_sync.
 __global__ void __launch_bounds__(256) k_octo_travel_multi_path(OcGrid g, OtmAux a, int submap, long long n, const int32_t* __restrict__ source,
                                                                 const float* __restrict__ xyz, float vs, int max_len,
                                                                 int32_t* __restrict__ cells, int32_t* __restrict__ len) {
@@ -824,7 +382,7 @@ __global__ void __launch_bounds__(256) k_octo_travel_multi_path(OcGrid g, OtmAux
   const float d1 = vs, d2 = sqrtf(2.0f) * vs, d3 = sqrtf(3.0f) * vs;
   const float inf = __int_as_float(0x7f800000);
   for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < n; q += (long long)gridDim.x * blockDim.x) {
-    const int s = source[q];
+    const int s = source ? source[q] : 0;
     int L = 0;
     if (s < 0 || s >= a.S) {
       atomicOr(g.err, OC_ERR_TRAVEL_SOURCE);
@@ -845,14 +403,17 @@ __global__ void __launch_bounds__(256) k_octo_travel_multi_path(OcGrid g, OtmAux
       float bg = inf;
 #pragma unroll
       for (int e = 0; e < 27; e++) {
-        if (!((am >> e) & 1u)) continue;  // (never the cell itself)
+        if (e == ot_bit(0, 0, 0)) continue;
         const int dx = e / 9 - 1, dy = (e / 3) % 3 - 1, dz = e % 3 - 1;
         const int i = c[0] + dx, j = c[1] + dy, k = c[2] + dz;
         const int tn = a.cnbr[(size_t)t * 27 + ot_bit((i >> OC_BSHIFT) - bx, (j >> OC_BSHIFT) - by, (k >> OC_BSHIFT) - bz)];
-        const float hg = otm_field(a, tn, s)[oc_voxel_off(i, j, k)];  // (an allowed step's cell is traversable: tn >= 0)
+        // every neighbour is read, a disallowed one from a valid slot, so the loads take no branch and issue together
+        // (an allowed step's cell is traversable: tn >= 0)
+        const bool ok = (am >> e) & 1u;
+        const float hg = otm_field(a, ok ? tn : t, s)[oc_voxel_off(i, j, k)];
         const int nz_ = (dx != 0) + (dy != 0) + (dz != 0);
         const float dis = nz_ == 1 ? d1 : (nz_ == 2 ? d2 : d3);
-        if (hg < bg && hg + dis == gv) { best = e; bg = hg; bt = tn; }
+        if (ok && hg < bg && hg + dis == gv) { best = e; bg = hg; bt = tn; }
       }
       if (best < 0) {  // cannot happen at the fixed point: reported by the next tslam_octo_sync, never a silent cut
         atomicOr(g.err, OC_ERR_TRAVEL_PATH);
@@ -867,6 +428,7 @@ __global__ void __launch_bounds__(256) k_octo_travel_multi_path(OcGrid g, OtmAux
   }
 }
 
+// ---- host side -----------------------------------------------------------------------------------------------------
 // per pool block: traversable bits 64 + slot 4 = 68 B; then change flags, counts and the per-source arrays
 static size_t otm_blk_bytes(size_t nb) {
   return nb * (OT_WORDS * 4 + 4) + ((ES_MAX_SWEEPS + 2) + 8 + TSLAM_OCTO_TRAVEL_MAX_STARTS * 6) * 4;
@@ -874,10 +436,10 @@ static size_t otm_blk_bytes(size_t nb) {
 // per slot: pool block 4 + neighbour table 108 + allowed steps 2048 = 2160 B; per item: field 2048 + epoch 4 = 2052 B
 static size_t otm_bytes(size_t nt, size_t S) { return nt * (4 + 27 * 4 + OC_B3 * 4) + S * nt * (OC_B3 * 4 + 4); }
 
-static OtmAux otm_aux(tslam_octo* m, int S, int nt) {
-  const size_t nb = (size_t)m->g.max_blocks;
+static OtmAux otm_aux(const tslam_octo* m, const OcTravel& f) {
+  const size_t nb = (size_t)m->g.max_blocks, S = f.S, nt = f.nt;
   OtmAux a;
-  a.trav = (uint32_t*)m->trm_blk;
+  a.trav = (uint32_t*)f.blk;
   a.slot = (int*)(a.trav + nb * OT_WORDS);
   a.changed = a.slot + nb;
   a.counts = a.changed + (ES_MAX_SWEEPS + 2);
@@ -885,28 +447,214 @@ static OtmAux otm_aux(tslam_octo* m, int S, int nt) {
   a.start = a.counts + 8;
   a.sitem = a.start + 4 * TSLAM_OCTO_TRAVEL_MAX_STARTS;
   a.reach = a.sitem + TSLAM_OCTO_TRAVEL_MAX_STARTS;
-  a.am = (uint32_t*)m->trm_mem;  // (the two 2 KB-per-row arrays first: 128-byte aligned rows)
-  a.G = (float*)(a.am + (size_t)nt * OC_B3);
-  a.epoch = (int*)(a.G + (size_t)S * nt * OC_B3);
-  a.cblk = a.epoch + (size_t)S * nt;
+  a.am = (uint32_t*)f.mem;  // (the two 2 KB-per-row arrays first: 128-byte aligned rows)
+  a.G = (float*)(a.am + nt * OC_B3);
+  a.epoch = (int*)(a.G + S * nt * OC_B3);
+  a.cblk = a.epoch + S * nt;
   a.cnbr = a.cblk + nt;
-  a.S = S;
-  a.nt = nt;
+  a.S = f.S;
+  a.nt = f.nt;
   return a;
 }
 
-static int otm_readable(tslam_octo* m, int32_t submap, const char* what) {
+int oc_travel_free(tslam_octo* m) {
+  for (OcTravel* f : {&m->tr, &m->trm}) {
+    if (f->blk) cudaFree(f->blk);
+    if (f->mem) cudaFree(f->mem);
+    *f = OcTravel{};
+  }
+  return TSLAM_OK;
+}
+
+// the checks every travel call makes first
+static int ot_check(tslam_octo* m, int32_t submap, const char* what) {
+  if (!m->logodds) {
+    ts_set_error("%s: the map is a hit counter; a travel-cost field needs a log-odds map (tslam_octo_create_logodds)", what);
+    return TSLAM_E_INVALID;
+  }
+  if (submap < 0 || submap >= m->cfg.max_submaps) { ts_set_error("%s: submap %d out of range", what, submap); return TSLAM_E_INVALID; }
+  return TSLAM_OK;
+}
+
+// the fields of f can be read for `submap`: an update has completed, for that submap, and no reset or fusion came after it
+static int ot_readable(tslam_octo* m, const OcTravel& f, int32_t submap, const char* what) {
   int rc = ot_check(m, submap, what);
   if (rc) return rc;
-  if (!m->trm_ready) {
-    ts_set_error("%s: no completed tslam_octo_travel_multi_update since the map was created, reset or fused, or since the last one "
-                 "failed", what);
+  if (!f.ready) {
+    ts_set_error("%s: no completed update of this travel-cost field since the map was created, reset or fused, or since the "
+                 "last update failed", what);
     return TSLAM_E_INVALID;
   }
-  if (m->trm_submap != submap) {
-    ts_set_error("%s: the last tslam_octo_travel_multi_update was for submap %d, not %d", what, m->trm_submap, submap);
+  if (f.submap != submap) {
+    ts_set_error("%s: the last update of this travel-cost field was for submap %d, not %d", what, f.submap, submap);
     return TSLAM_E_INVALID;
   }
+  return TSLAM_OK;
+}
+
+// the clearance and max_cost checks of every travel update, and the occupancy ESDF the clearance test reads
+static int ot_params(tslam_octo* m, int32_t submap, float clearance, float max_cost, const char* what, OcEsdfField* ef) {
+  const float cost_limit = std::ldexp(m->in.vs, 22);  // keeps G + vs > G for every kept value
+  if (!(std::isfinite(clearance) && clearance >= 0.0f)) {
+    ts_set_error("%s: clearance must be finite and >= 0 (got %g)", what, (double)clearance);
+    return TSLAM_E_INVALID;
+  }
+  if (!(std::isfinite(max_cost) && max_cost > 0.0f && max_cost <= cost_limit)) {
+    ts_set_error("%s: max_cost must be finite, > 0 and <= 2^22 * voxel_scale = %g (got %g)", what, (double)cost_limit, (double)max_cost);
+    return TSLAM_E_INVALID;
+  }
+  memset(ef, 0, sizeof(*ef));
+  if (clearance > 0.0f) {
+    const int rc = oc_esdf_field(m, submap, what, ef);
+    if (rc) return rc;
+    if (clearance > ef->D) {
+      ts_set_error("%s: clearance %g exceeds the occupancy ESDF's max_dist %g", what, (double)clearance, (double)ef->D);
+      return TSLAM_E_INVALID;
+    }
+  }
+  return TSLAM_OK;
+}
+
+// start cell c0 = rha(p / vs) of a finite point, f32 division as the kernels do it; false when outside the volume
+static bool ot_start_cell(const tslam_octo* m, const float* p, int c[3]) {
+  for (int q = 0; q < 3; q++) {
+    const float u = p[q] / m->in.vs;
+    if (!(std::fabs(u) < 1e9f)) return false;
+    c[q] = (int)std::round(u);
+  }
+  return c[0] >= -m->g.hN && c[0] < m->g.N - m->g.hN && c[1] >= -m->g.hN && c[1] < m->g.N - m->g.hN && c[2] >= -m->g.hNz &&
+         c[2] < m->g.Nz - m->g.hNz;
+}
+
+static int ot_grid(tslam_octo* m, long long n) {
+  long long blocks = (n + 255) / 256;
+  if (blocks > (long long)m->sm_count * 16) blocks = (long long)m->sm_count * 16;
+  return (int)blocks;
+}
+
+// The fields of `submap` from the S finite starts[S,3] into f, for both update entry points (`what` names the one called
+// in messages).  A refused clearance or max_cost leaves f's last fields readable; from then on f is unreadable until the
+// update completes.  Outputs as tslam_octo_travel_multi_update.
+static int ot_update(tslam_octo* m, OcTravel& f, int32_t submap, int S, const float* starts, float clearance, float max_cost,
+                     const char* what, int32_t* stats2, int32_t* reachable, uint8_t* start_ok, void* stream) {
+  OcEsdfField ef;
+  int rc = ot_params(m, submap, clearance, max_cost, what, &ef);
+  if (rc) return rc;
+  f.ready = 0;  // until this update has completed
+  f.S = S;
+  f.nt = 0;  // (until classify has counted the slots)
+  if (!f.blk) TS_CUDA(cudaMalloc(&f.blk, otm_blk_bytes((size_t)m->g.max_blocks)));
+  std::vector<int> h_start(4 * (size_t)S);
+  for (int s = 0; s < S; s++) h_start[4 * s + 3] = ot_start_cell(m, starts + 3 * s, &h_start[4 * s]) ? 1 : 0;
+  cudaStream_t st = (cudaStream_t)stream;
+  OtmAux a = otm_aux(m, f);
+  TS_CUDA(cudaMemsetAsync(a.changed, 0, ((ES_MAX_SWEEPS + 2) + 4) * 4, st));  // changed, counts
+  TS_CUDA(cudaMemsetAsync(a.reach, 0, (size_t)S * 4, st));
+  TS_CUDA(cudaMemcpyAsync(a.start, h_start.data(), h_start.size() * 4, cudaMemcpyHostToDevice, st));
+  const int grid = m->sm_count * 8;
+  k_octo_travel_multi_classify<<<grid, OT_THREADS, 0, st>>>(m->g, a, ef, submap, m->lo.l_occ, clearance);
+  TS_LAUNCH_CHECK(m);
+  int h_counts[2] = {0, 0};
+  TS_CUDA(cudaMemcpyAsync(h_counts, a.counts, 8, cudaMemcpyDeviceToHost, st));
+  TS_CUDA(cudaStreamSynchronize(st));
+  f.nt = h_counts[1];
+  const size_t need = std::max(otm_bytes((size_t)f.nt, (size_t)S), (size_t)256);
+  if (need > f.bytes) {  // grow geometrically: a map that keeps growing reallocates O(log) times
+    const size_t bytes = std::max(need, std::min(2 * f.bytes, otm_bytes((size_t)m->g.max_blocks, (size_t)S)));
+    if (f.mem) cudaFree(f.mem);
+    f.mem = nullptr;
+    f.bytes = 0;
+    TS_CUDA(cudaMalloc(&f.mem, bytes));
+    f.bytes = bytes;
+  }
+  a = otm_aux(m, f);
+  k_octo_travel_multi_tables<<<grid, OT_THREADS, 0, st>>>(m->g, a);
+  TS_LAUNCH_CHECK(m);
+  k_octo_travel_multi_fill<<<m->sm_count * 16, OT_THREADS, 0, st>>>(a);
+  TS_LAUNCH_CHECK(m);
+  k_octo_travel_multi_starts<<<(S + 127) / 128, 128, 0, st>>>(m->g, a, submap);
+  TS_LAUNCH_CHECK(m);
+  const int sgrid = m->sm_count * 16;
+  int sweeps = 0;
+  rc = es_wave(m, st, a.changed, ES_GROUP,
+               [&](int k) { k_octo_travel_multi_sweep<<<sgrid, OT_THREADS, 0, st>>>(a, k, m->in.vs, max_cost); }, &sweeps);
+  if (rc) return rc;
+  if (sweeps > ES_MAX_SWEEPS) {  // the last sweep still changed something: the fields are not the fixed point
+    ts_set_error("%s: the waves were still changing after %d sweeps; the fields are incomplete and their readers refuse", what, ES_MAX_SWEEPS);
+    return TSLAM_E_INVALID;
+  }
+  k_octo_travel_multi_count<<<sgrid, OT_THREADS, 0, st>>>(a);
+  TS_LAUNCH_CHECK(m);
+  std::vector<int> h_reach(S), h_item(S);
+  TS_CUDA(cudaMemcpyAsync(h_reach.data(), a.reach, (size_t)S * 4, cudaMemcpyDeviceToHost, st));
+  TS_CUDA(cudaMemcpyAsync(h_item.data(), a.sitem, (size_t)S * 4, cudaMemcpyDeviceToHost, st));
+  TS_CUDA(cudaStreamSynchronize(st));
+  f.ready = 1;
+  f.submap = submap;
+  if (stats2) { stats2[0] = sweeps; stats2[1] = h_counts[0]; }
+  for (int s = 0; s < S; s++) {
+    if (reachable) reachable[s] = h_reach[s];
+    if (start_ok) start_ok[s] = h_item[s] >= 0 ? 1 : 0;
+  }
+  return TSLAM_OK;
+}
+
+extern "C" int tslam_octo_travel_update(tslam_octo_t* m, int32_t submap, const float* start3, float clearance, float max_cost,
+                                        int32_t* stats4, void* stream) {
+  const char* what = "tslam_octo_travel_update";
+  if (!m || !start3) return TSLAM_E_INVALID;
+  int rc = ot_check(m, submap, what);
+  if (rc) return rc;
+  if (!(std::isfinite(start3[0]) && std::isfinite(start3[1]) && std::isfinite(start3[2]))) {
+    ts_set_error("%s: the start must be finite", what);
+    return TSLAM_E_INVALID;
+  }
+  int32_t stats2[2], reachable;
+  uint8_t start_ok;
+  rc = ot_update(m, m->tr, submap, 1, start3, clearance, max_cost, what, stats2, &reachable, &start_ok, stream);
+  if (rc) return rc;
+  if (stats4) { stats4[0] = reachable; stats4[1] = stats2[0]; stats4[2] = stats2[1]; stats4[3] = start_ok; }
+  return TSLAM_OK;
+}
+
+extern "C" int tslam_octo_travel_gather(tslam_octo_t* m, int32_t submap, int64_t cap, int32_t* idx, float* cost, int64_t* n_out,
+                                        void* stream) {
+  if (!m || !n_out || cap < 0 || (cap > 0 && (!idx || !cost))) return TSLAM_E_INVALID;
+  int rc = ot_readable(m, m->tr, submap, "tslam_octo_travel_gather");
+  if (rc) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  unsigned long long* ctr = (unsigned long long*)(m->scratch_i + 8);
+  TS_CUDA(cudaMemsetAsync(ctr, 0, 8, st));
+  k_octo_travel_slot_gather<<<m->sm_count * 8, OT_THREADS, 0, st>>>(m->g, otm_aux(m, m->tr), 0, cap, idx, cost, ctr);
+  TS_LAUNCH_CHECK(m);
+  unsigned long long v = 0;
+  TS_CUDA(cudaMemcpyAsync(&v, ctr, 8, cudaMemcpyDeviceToHost, st));
+  TS_CUDA(cudaStreamSynchronize(st));
+  *n_out = (int64_t)v;
+  if ((int64_t)v > cap) { ts_set_error("octo travel gather: %lld cells > capacity %lld", (long long)v, (long long)cap); return TSLAM_E_CAPACITY; }
+  return TSLAM_OK;
+}
+
+extern "C" int tslam_octo_travel_query(tslam_octo_t* m, int32_t submap, int64_t n, const float* xyz, float* cost, void* stream) {
+  if (!m || n < 0 || (n && (!xyz || !cost))) return TSLAM_E_INVALID;
+  int rc = ot_readable(m, m->tr, submap, "tslam_octo_travel_query");
+  if (rc || n == 0) return rc;
+  k_octo_travel_multi_query<<<ot_grid(m, n), 256, 0, (cudaStream_t)stream>>>(m->g, otm_aux(m, m->tr), submap, n, xyz,
+                                                                             m->in.vs, cost);
+  TS_LAUNCH_CHECK(m);
+  return TSLAM_OK;
+}
+
+extern "C" int tslam_octo_travel_path(tslam_octo_t* m, int32_t submap, int64_t n, const float* xyz, int32_t max_len, int32_t* cells,
+                                      int32_t* len, void* stream) {
+  if (!m || n < 0 || (n && (!xyz || !cells || !len))) return TSLAM_E_INVALID;
+  const char* what = "tslam_octo_travel_path";
+  if (max_len < 1) { ts_set_error("%s: max_len must be >= 1 (got %d)", what, max_len); return TSLAM_E_INVALID; }
+  int rc = ot_readable(m, m->tr, submap, what);
+  if (rc || n == 0) return rc;
+  k_octo_travel_multi_path<<<ot_grid(m, n), 256, 0, (cudaStream_t)stream>>>(m->g, otm_aux(m, m->tr), submap, n, nullptr, xyz,
+                                                                            m->in.vs, max_len, cells, len);
+  TS_LAUNCH_CHECK(m);
   return TSLAM_OK;
 }
 
@@ -925,74 +673,15 @@ extern "C" int tslam_octo_travel_multi_update(tslam_octo_t* m, int32_t submap, i
       ts_set_error("%s: start %d is not finite", what, q / 3);
       return TSLAM_E_INVALID;
     }
-  OcEsdfField ef;
-  rc = ot_params(m, submap, clearance, max_cost, what, &ef);
-  if (rc) return rc;
-  const int S = n_starts;
-  m->trm_ready = 0;  // until this update has completed
-  if (!m->trm_blk) TS_CUDA(cudaMalloc(&m->trm_blk, otm_blk_bytes((size_t)m->g.max_blocks)));
-  std::vector<int> h_start(4 * (size_t)S);
-  for (int s = 0; s < S; s++) h_start[4 * s + 3] = ot_start_cell(m, starts + 3 * s, &h_start[4 * s]) ? 1 : 0;
-  cudaStream_t st = (cudaStream_t)stream;
-  OtmAux a = otm_aux(m, S, 0);
-  TS_CUDA(cudaMemsetAsync(a.changed, 0, ((ES_MAX_SWEEPS + 2) + 4) * 4, st));  // changed, counts
-  TS_CUDA(cudaMemsetAsync(a.reach, 0, (size_t)S * 4, st));
-  TS_CUDA(cudaMemcpyAsync(a.start, h_start.data(), h_start.size() * 4, cudaMemcpyHostToDevice, st));
-  const int grid = m->sm_count * 8;
-  k_octo_travel_multi_classify<<<grid, OT_THREADS, 0, st>>>(m->g, a, ef, submap, m->lo.l_occ, clearance);
-  TS_LAUNCH_CHECK(m);
-  int h_counts[2] = {0, 0};
-  TS_CUDA(cudaMemcpyAsync(h_counts, a.counts, 8, cudaMemcpyDeviceToHost, st));
-  TS_CUDA(cudaStreamSynchronize(st));
-  const int nt = h_counts[1];
-  const size_t bytes = std::max(otm_bytes((size_t)nt, (size_t)S), (size_t)256);
-  if (bytes > m->trm_bytes) {  // grow on demand
-    if (m->trm_mem) cudaFree(m->trm_mem);
-    m->trm_mem = nullptr;
-    m->trm_bytes = 0;
-    TS_CUDA(cudaMalloc(&m->trm_mem, bytes));
-    m->trm_bytes = bytes;
-  }
-  a = otm_aux(m, S, nt);
-  k_octo_travel_multi_tables<<<grid, OT_THREADS, 0, st>>>(m->g, a);
-  TS_LAUNCH_CHECK(m);
-  k_octo_travel_multi_fill<<<m->sm_count * 16, OT_THREADS, 0, st>>>(a);
-  TS_LAUNCH_CHECK(m);
-  k_octo_travel_multi_starts<<<(S + 127) / 128, 128, 0, st>>>(m->g, a, submap);
-  TS_LAUNCH_CHECK(m);
-  const int sgrid = m->sm_count * 16;
-  int sweeps = 0;
-  rc = es_wave(m, st, a.changed, ES_GROUP,
-               [&](int k) { k_octo_travel_multi_sweep<<<sgrid, OT_THREADS, 0, st>>>(a, k, m->in.vs, max_cost); }, &sweeps);
-  if (rc) return rc;
-  if (sweeps > ES_MAX_SWEEPS) {
-    ts_set_error("%s: the waves were still changing after %d sweeps; the fields are incomplete and their readers refuse", what, ES_MAX_SWEEPS);
-    return TSLAM_E_INVALID;
-  }
-  k_octo_travel_multi_count<<<sgrid, OT_THREADS, 0, st>>>(a);
-  TS_LAUNCH_CHECK(m);
-  std::vector<int> h_reach(S), h_item(S);
-  TS_CUDA(cudaMemcpyAsync(h_reach.data(), a.reach, (size_t)S * 4, cudaMemcpyDeviceToHost, st));
-  TS_CUDA(cudaMemcpyAsync(h_item.data(), a.sitem, (size_t)S * 4, cudaMemcpyDeviceToHost, st));
-  TS_CUDA(cudaStreamSynchronize(st));
-  m->trm_ready = 1;
-  m->trm_submap = submap;
-  m->trm_S = S;
-  m->trm_nt = nt;
-  if (stats2) { stats2[0] = sweeps; stats2[1] = h_counts[0]; }
-  for (int s = 0; s < S; s++) {
-    if (reachable) reachable[s] = h_reach[s];
-    if (start_ok) start_ok[s] = h_item[s] >= 0 ? 1 : 0;
-  }
-  return TSLAM_OK;
+  return ot_update(m, m->trm, submap, n_starts, starts, clearance, max_cost, what, stats2, reachable, start_ok, stream);
 }
 
 extern "C" int tslam_octo_travel_multi_query(tslam_octo_t* m, int32_t submap, int64_t n, const float* xyz, float* cost, void* stream) {
   if (!m || n < 0 || (n && (!xyz || !cost))) return TSLAM_E_INVALID;
-  int rc = otm_readable(m, submap, "tslam_octo_travel_multi_query");
+  int rc = ot_readable(m, m->trm, submap, "tslam_octo_travel_multi_query");
   if (rc || n == 0) return rc;
-  k_octo_travel_multi_query<<<ot_grid(m, n), 256, 0, (cudaStream_t)stream>>>(m->g, otm_aux(m, m->trm_S, m->trm_nt), submap, n, xyz,
-                                                                             m->in.vs, cost);
+  k_octo_travel_multi_query<<<ot_grid(m, n), 256, 0, (cudaStream_t)stream>>>(m->g, otm_aux(m, m->trm), submap, n,
+                                                                             xyz, m->in.vs, cost);
   TS_LAUNCH_CHECK(m);
   return TSLAM_OK;
 }
@@ -1002,10 +691,10 @@ extern "C" int tslam_octo_travel_multi_path(tslam_octo_t* m, int32_t submap, int
   if (!m || n < 0 || (n && (!source || !xyz || !cells || !len))) return TSLAM_E_INVALID;
   const char* what = "tslam_octo_travel_multi_path";
   if (max_len < 1) { ts_set_error("%s: max_len must be >= 1 (got %d)", what, max_len); return TSLAM_E_INVALID; }
-  int rc = otm_readable(m, submap, what);
+  int rc = ot_readable(m, m->trm, submap, what);
   if (rc || n == 0) return rc;
-  k_octo_travel_multi_path<<<ot_grid(m, n), 256, 0, (cudaStream_t)stream>>>(m->g, otm_aux(m, m->trm_S, m->trm_nt), submap, n, source, xyz,
-                                                                            m->in.vs, max_len, cells, len);
+  k_octo_travel_multi_path<<<ot_grid(m, n), 256, 0, (cudaStream_t)stream>>>(m->g, otm_aux(m, m->trm), submap, n,
+                                                                            source, xyz, m->in.vs, max_len, cells, len);
   TS_LAUNCH_CHECK(m);
   return TSLAM_OK;
 }

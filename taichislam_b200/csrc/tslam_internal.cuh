@@ -195,6 +195,17 @@ __device__ __forceinline__ int warp_append_i32(bool want, int* counter) {
   base = __shfl_sync(0xffffffffu, base, leader);
   return want ? base + __popc(m & ((1u << lane) - 1)) : -1;
 }
+// the same on an unsigned 64-bit counter (the Octomap's count-then-fill gathers)
+__device__ __forceinline__ long long oc_warp_append(bool want, unsigned long long* counter) {
+  const unsigned m = __ballot_sync(0xffffffffu, want);
+  if (!m) return -1;
+  const int lane = threadIdx.x & 31;
+  const int leader = __ffs(m) - 1;
+  unsigned long long base = 0;
+  if (lane == leader) base = atomicAdd(counter, (unsigned long long)__popc(m));
+  base = __shfl_sync(0xffffffffu, base, leader);
+  return want ? (long long)(base + __popc(m & ((1u << lane) - 1))) : -1;
+}
 
 // Low interpolation corner of an ESDF query point (k_esdf_query, k_octo_esdf_query, and k_owner_points which routes the
 // points of a tiled map to the rank that answers them): u = x / vs per axis, correctly rounded, c = floor(u).  False
@@ -484,6 +495,13 @@ __device__ __forceinline__ int oc_voxel_off(int i, int j, int k) {
 __host__ __device__ __forceinline__ bool lo_known(unsigned int w) { return (w & 1u) != 0; }
 __host__ __device__ __forceinline__ int lo_val(unsigned int w) { return (int)w >> 1; }
 __host__ __device__ __forceinline__ unsigned int lo_word(int L) { return ((unsigned int)L << 1) | 1u; }
+// Voxel class of a log-odds word, for every tracker: UNKNOWN = not known, OCC = known and L > l_occ, FREE = known and
+// L <= l_occ.  The values are a data format: the occupancy ESDF stores them in its class bytes, and the travel-cost
+// field reads them back from there (OcEsdfField::free_cls).
+enum { OC_UNK = 0, OC_FREE = 1, OC_OCC = 2 };
+__device__ __forceinline__ unsigned char oc_class(unsigned int w, int l_occ) {
+  return !lo_known(w) ? OC_UNK : (lo_val(w) > l_occ ? OC_OCC : OC_FREE);
+}
 #define OC_MARK_WORDS 32  // mark words per block: 0..15 hit bits, 16..31 miss bits of its 512 voxels (128 B per block)
 struct OcLo {             // per-frame workspace of a log-odds map (allocated in log-odds mode only)
   uint32_t* mark;         // [max_blocks * 32] hit / miss bits of the frame, cleared by k_octo_lo_apply
@@ -495,13 +513,18 @@ struct OcLo {             // per-frame workspace of a log-odds map (allocated in
   float min_ray, max_ray; // f32(min_ray_length), f32(max_ray_length)
   int l_hit, l_miss, l_min, l_max, l_occ;
 };
+// What a tracker of a log-odds map (occupancy ESDF, frontiers, travel-cost fields) kept can be read for `submap` iff an
+// update for that submap has completed and no reset, fusion or failed update came after it (oc_track_readable).
+struct OcTrack {
+  int ready;   // set when an update completes; cleared when one begins, and by reset and fusion (oc_track_invalidate_all)
+  int submap;  // submap of that update
+};
 // S travel-cost fields of one submap as of one update (tslam_octo_travel.cu), allocated by the first update
 struct OcTravel {
   void* blk;      // per pool block: traversable bits, compact slot (68 B); change flags, per-source arrays
   void* mem;      // per compact slot: allowed steps, neighbour table; per (slot, source): field, epoch (grown geometrically)
   size_t bytes;   // bytes of mem
-  int ready;      // the kept fields can be read (an update completed; cleared by reset, fusion, a failed update)
-  int submap;     // submap of the kept fields
+  OcTrack track;  // the kept fields
   int S, nt;      // sources and compact slots of the kept fields
 };
 struct tslam_octo {
@@ -524,14 +547,12 @@ struct tslam_octo {
   // occupancy ESDF of a log-odds map (tslam_octo_esdf_*, tslam_octo_esdf.cu), allocated by the first update
   void* esdf_mem;         // field, class bytes, neighbour table, epochs, change flags
   int* esdf_dirty;        // [max_blocks] block updated by k_octo_lo_apply since the last ESDF update; NULL until then
-  int esdf_full_needed;   // the next update recomputes everything (reset, fusion); readers refuse until it has run
-  int esdf_submap;        // submap of the kept field
+  OcTrack esdf_track;     // the kept field (not ready: the next update recomputes everything)
   float esdf_D;           // truncation distance of the kept field
   // frontier tracker of a log-odds map (tslam_octo_frontier_*, tslam_octo_frontier.cu), allocated by the first update
   void* fr_mem;           // per pool block: frontier mask, dirty and region flags, region list, popcount, offset (84 B)
   int* fr_dirty;          // [max_blocks] block updated by k_octo_lo_apply since the last frontier update; NULL until then
-  int fr_full_needed;     // the next update recomputes everything (reset, fusion); readers refuse until it has run
-  int fr_submap;          // submap of the kept frontier set
+  OcTrack fr_track;       // the kept frontier set (not ready: the next update recomputes everything)
   int fr_nb;              // pool blocks the last update saw
   int fr_n, fr_nc;        // frontier voxels and clusters of the last update
   void* fr_vox;           // per frontier voxel: union-find parent, cluster slot of a root (grown on demand)
@@ -554,7 +575,7 @@ int oc_view_free(tslam_octo* m);      // tslam_octo_view.cu
 int oc_travel_free(tslam_octo* m);    // tslam_octo_travel.cu
 // tslam_octo_esdf.cu: the occupancy ESDF of `submap` as of its last update, for the clearance test of the travel-cost
 // field.  Refused like tslam_octo_esdf_gather (the message naming `what`).  A voxel at pool offset o was FREE at that
-// update, in a block it saw, with field value e[o] iff o / 512 < *nb_seen and (cls[o] & cls_mask) == free_cls.
+// update, in a block it saw, with field value e[o] iff o / 512 < *nb_seen and (cls[o] & cls_mask) == free_cls (OC_FREE).
 struct OcEsdfField {
   const float* e;            // [max_blocks*512] field, in the cnt plane's layout
   const unsigned char* cls;  // [max_blocks*512] class byte of the update
@@ -563,11 +584,11 @@ struct OcEsdfField {
   unsigned char free_cls, cls_mask;
 };
 int oc_esdf_field(tslam_octo* m, int32_t submap, const char* what, OcEsdfField* f);
-// tslam_octo_frontier.cu: the frontier set of `submap` can be read (an update for it has completed and no reset or fusion
-// came since; refused like tslam_octo_frontier_gather, the message naming `what`) ...
-int oc_frontier_readable(tslam_octo* m, int32_t submap, const char* what);
-// ... and its m->fr_n rows (ijk, cluster ordinal) into idx[fr_n * 3], cluster[fr_n] (DEVICE), in compact order, on st
+// tslam_octo_frontier.cu: the m->fr_n rows (ijk, cluster ordinal) of the frontier set into idx[fr_n * 3], cluster[fr_n]
+// (DEVICE), in compact order, on st; the caller has checked m->fr_track
 int oc_frontier_rows(tslam_octo* m, int32_t* idx, int32_t* cluster, cudaStream_t st);
+// tracker bits of g.err next to TS_ERR_POOL_FULL / TS_ERR_TABLE_FULL: the next synchronising call names every bit that is
+// set (oc_deferred, tslam_octo.cu)
 #define OC_ERR_VIEW_WINDOW 16  // g.err: a viewpoint-gain walk left its view's bitmap window (tslam_octo_view.cu)
 #define OC_ERR_TRAVEL_PATH 32  // g.err: a travel path found no predecessor (impossible at the field's fixed point; tslam_octo_travel.cu)
 #define OC_ERR_TRAVEL_SOURCE 64  // g.err: a many-source travel path named a source outside [0, S) (tslam_octo_travel.cu)
@@ -657,3 +678,33 @@ int ts_march_alloc(tslam_tsdf* m);
 void ts_march_free(tslam_tsdf* m);
 int ts_march_setup(tslam_tsdf* m, cudaStream_t st, const TsBatch& batch, uint32_t bucket_shift);  // rays listed since the last call
 int ts_march_launch(tslam_tsdf* m, cudaStream_t st, const TsBatch& batch, uint32_t bucket_shift, cudaEvent_t* sub_ev);
+
+// Octomap host helpers shared by its trackers (tslam_octo.cu)
+// the arguments every tracker call checks first: a log-odds map (`feature` names what needs one), submap in range
+int oc_logodds_submap(tslam_octo* m, int32_t submap, const char* what, const char* feature);
+// the state kept in t can be read for `submap` (see OcTrack); `update` names the entry point that computes it
+int oc_track_readable(tslam_octo* m, const OcTrack& t, int32_t submap, const char* what, const char* update);
+// reset and fusion recycle pool slots: no tracker's kept state describes the map any more
+void oc_track_invalidate_all(tslam_octo* m);
+// *p holds at least `need` bytes: reallocated to exactly `need` when smaller (the contents are not kept)
+int oc_reserve(void** p, size_t* bytes, size_t need);
+// CTAs for `work` items at `per_cta` per CTA: at least 1, at most cap
+static inline int oc_grid(long long work, int per_cta, int cap) {
+  const long long g = (work + per_cta - 1) / per_cta;
+  return (int)(g < 1 ? 1 : (g > cap ? cap : g));
+}
+// Count-then-fill gather: launch(counter) enqueues one kernel on st that appends its rows through oc_warp_append on the
+// zeroed counter and writes those below cap.  Synchronises; *n_out = the rows found, TSLAM_E_CAPACITY when more than cap.
+template <class F>
+int oc_counted_gather(tslam_octo* m, cudaStream_t st, F launch, int64_t cap, int64_t* n_out, const char* what) {
+  unsigned long long* ctr = (unsigned long long*)(m->scratch_i + 8);
+  TS_CUDA(cudaMemsetAsync(ctr, 0, 8, st));
+  launch(ctr);
+  TS_LAUNCH_CHECK(m);
+  unsigned long long v = 0;
+  TS_CUDA(cudaMemcpyAsync(&v, ctr, 8, cudaMemcpyDeviceToHost, st));
+  TS_CUDA(cudaStreamSynchronize(st));
+  *n_out = (int64_t)v;
+  if ((int64_t)v > cap) { ts_set_error("%s: %lld rows > capacity %lld", what, (long long)v, (long long)cap); return TSLAM_E_CAPACITY; }
+  return TSLAM_OK;
+}

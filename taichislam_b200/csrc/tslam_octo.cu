@@ -3,6 +3,7 @@
 // log-odds / ray casting: occupy[ijk] += 1 per point (:116-119) and a threshold
 // test (:86-88); counts are exact integers, compared bit-for-bit with the oracle.
 #include <cstring>
+#include <string>
 #include "tslam_internal.cuh"
 
 __device__ __forceinline__ int oc_iroundf(float x) { return (int)roundf(x); }
@@ -60,17 +61,6 @@ __global__ void __launch_bounds__(256) k_octo_depth(OcGrid g, const uint16_t* __
     cw = oc_color_word(fr.seq, ts_color_pixel(in, i, j, th, tw, ti, tj) ? tex + ((size_t)tj * tw + ti) * 3 : zero3);
   }
   oc_hit(g, fr.submap, oc_iroundf(px / in.vs), oc_iroundf(py / in.vs), oc_iroundf(pz / in.vs), 1u, cw);
-}
-
-__device__ __forceinline__ long long oc_warp_append(bool want, unsigned long long* counter) {
-  const unsigned m = __ballot_sync(0xffffffffu, want);
-  if (!m) return -1;
-  const int lane = threadIdx.x & 31;
-  const int leader = __ffs(m) - 1;
-  unsigned long long base = 0;
-  if (lane == leader) base = atomicAdd(counter, (unsigned long long)__popc(m));
-  base = __shfl_sync(0xffffffffu, base, leader);
-  return want ? (long long)(base + __popc(m & ((1u << lane) - 1))) : -1;
 }
 
 // LO: gather the known voxels of a log-odds map, count[row] = their L (int32 bits)
@@ -574,10 +564,44 @@ extern "C" int tslam_octo_reset(tslam_octo_t* m, void* stream) {
   if (nb) TS_CUDA(cudaMemsetAsync(m->g.cnt, 0, (size_t)nb * OC_B3 * 4, st));
   if (nb && m->g.cw) TS_CUDA(cudaMemsetAsync(m->g.cw, 0, (size_t)nb * OC_B3 * 8, st));
   TS_CUDA(cudaMemsetAsync(m->scratch_i, 0, 4 * 4, st));
-  m->esdf_full_needed = 1;  // pool slots are recycled: the kept ESDF state no longer describes the map
-  m->fr_full_needed = 1;    // ... nor the kept frontier set
-  m->tr.ready = 0;          // ... nor the kept travel-cost fields
-  m->trm.ready = 0;
+  oc_track_invalidate_all(m);
+  return TSLAM_OK;
+}
+
+void oc_track_invalidate_all(tslam_octo* m) {
+  for (OcTrack* t : {&m->esdf_track, &m->fr_track, &m->tr.track, &m->trm.track}) t->ready = 0;
+}
+
+int oc_logodds_submap(tslam_octo* m, int32_t submap, const char* what, const char* feature) {
+  if (!m->logodds) {
+    ts_set_error("%s: the map is a hit counter; %s needs a log-odds map (tslam_octo_create_logodds)", what, feature);
+    return TSLAM_E_INVALID;
+  }
+  if (submap < 0 || submap >= m->cfg.max_submaps) { ts_set_error("%s: submap %d out of range", what, submap); return TSLAM_E_INVALID; }
+  return TSLAM_OK;
+}
+
+int oc_track_readable(tslam_octo* m, const OcTrack& t, int32_t submap, const char* what, const char* update) {
+  int rc = oc_logodds_submap(m, submap, what, update);
+  if (rc) return rc;
+  if (!t.ready) {
+    ts_set_error("%s: no completed %s since the map was created, reset or fused, or since the last one failed", what, update);
+    return TSLAM_E_INVALID;
+  }
+  if (t.submap != submap) {
+    ts_set_error("%s: the last %s was for submap %d, not %d", what, update, t.submap, submap);
+    return TSLAM_E_INVALID;
+  }
+  return TSLAM_OK;
+}
+
+int oc_reserve(void** p, size_t* bytes, size_t need) {
+  if (need <= *bytes) return TSLAM_OK;
+  if (*p) cudaFree(*p);
+  *p = nullptr;
+  *bytes = 0;
+  TS_CUDA(cudaMalloc(p, need));
+  *bytes = need;
   return TSLAM_OK;
 }
 
@@ -628,28 +652,29 @@ static int oc_lo_finish(tslam_octo* m, const TsFrame& fr, int n_max, cudaStream_
   return TSLAM_OK;
 }
 
+// Reads and clears the device error flags.  A pool or table bit means hits were dropped: TSLAM_E_POOL_FULL.  Otherwise
+// one message names every tracker bit that is set: TSLAM_E_INVALID.
 static int oc_deferred(tslam_octo* m) {
   int err = 0;
   TS_CUDA(cudaMemcpy(&err, m->g.err, 4, cudaMemcpyDeviceToHost));
-  if (err) {
-    int zero = 0;
-    cudaMemcpy(m->g.err, &zero, 4, cudaMemcpyHostToDevice);
-    if (err == OC_ERR_VIEW_WINDOW) {
-      ts_set_error("octo view gain: a walk left its view's bitmap window (is every view's R a rotation?): gains are invalid");
-      return TSLAM_E_INVALID;
-    }
-    if (err == OC_ERR_TRAVEL_PATH) {
-      ts_set_error("octo travel path: a cell of the field had no predecessor: paths are invalid");
-      return TSLAM_E_INVALID;
-    }
-    if (err == OC_ERR_TRAVEL_SOURCE) {
-      ts_set_error("octo travel multi path: a source index was outside [0, n_starts): those paths have len 0");
-      return TSLAM_E_INVALID;
-    }
+  if (!err) return TSLAM_OK;
+  int zero = 0;
+  cudaMemcpy(m->g.err, &zero, 4, cudaMemcpyHostToDevice);
+  static const struct { int bit; const char* msg; } flags[] = {
+      {OC_ERR_VIEW_WINDOW, "octo view gain: a walk left its view's bitmap window (is every view's R a rotation?): gains are invalid"},
+      {OC_ERR_TRAVEL_PATH, "octo travel path: a cell of the field had no predecessor: paths are invalid"},
+      {OC_ERR_TRAVEL_SOURCE, "octo travel multi path: a source index was outside [0, n_starts): those paths have len 0"}};
+  int tracker = 0;
+  for (const auto& f : flags) tracker |= f.bit;
+  if (err & ~tracker) {
     ts_set_error("octomap block pool / table exhausted (max_blocks=%d, flags 0x%x): hits were dropped", m->g.max_blocks, err);
     return TSLAM_E_POOL_FULL;
   }
-  return TSLAM_OK;
+  std::string msg;
+  for (const auto& f : flags)
+    if (err & f.bit) msg += (msg.empty() ? "" : "; ") + std::string(f.msg);
+  ts_set_error("%s", msg.c_str());
+  return TSLAM_E_INVALID;
 }
 
 extern "C" int tslam_octo_integrate_points(tslam_octo_t* m, const float* xyz, int mem, int32_t n, const float* R9, const float* T3,
@@ -733,19 +758,12 @@ extern "C" int tslam_octo_integrate_depth_tex(tslam_octo_t* m, const uint16_t* d
 template <bool LO>
 static int oc_gather(tslam_octo* m, int32_t submap, int64_t cap, int32_t* idx, uint32_t* count, float* color, int64_t* n_out,
                      cudaStream_t st) {
-  unsigned long long* ctr = (unsigned long long*)(m->scratch_i + 8);
-  TS_CUDA(cudaMemsetAsync(ctr, 0, 8, st));
-  k_octo_gather<LO><<<m->sm_count * 8, 256, 0, st>>>(m->g, submap, cap, idx, count, color, ctr);
-  m->launches++;
-  TS_CUDA(cudaGetLastError());
-  unsigned long long v = 0;
-  TS_CUDA(cudaMemcpyAsync(&v, ctr, 8, cudaMemcpyDeviceToHost, st));
-  TS_CUDA(cudaStreamSynchronize(st));
-  *n_out = (int64_t)v;
-  int rc = oc_deferred(m);
-  if (rc) return rc;
-  if ((int64_t)v > cap) { ts_set_error("octo gather: %lld voxels > capacity %lld", (long long)v, (long long)cap); return TSLAM_E_CAPACITY; }
-  return TSLAM_OK;
+  const int rc = oc_counted_gather(m, st, [&](unsigned long long* ctr) {
+    k_octo_gather<LO><<<m->sm_count * 8, 256, 0, st>>>(m->g, submap, cap, idx, count, color, ctr);
+  }, cap, n_out, LO ? "tslam_octo_gather_logodds" : "tslam_octo_gather");
+  if (rc && rc != TSLAM_E_CAPACITY) return rc;
+  const int drc = oc_deferred(m);  // dropped hits are reported before a short buffer
+  return drc ? drc : rc;
 }
 
 extern "C" int tslam_octo_gather(tslam_octo_t* m, int32_t submap, int64_t cap, int32_t* idx, uint32_t* count, int64_t* n_out,

@@ -26,8 +26,6 @@
 #define OE_T3 (OE_T * OE_T * OE_T)
 #define OE_THREADS 128
 
-enum { OE_UNK = 0, OE_FREE = 1, OE_OCC = 2 };
-
 struct OeAux {
   float* e;            // [max_blocks*512] the field
   unsigned char* cls;  // [max_blocks*512] class at the last update (+ flags during an update)
@@ -41,10 +39,7 @@ struct OeAux {
   int* nb_prev;        // nb_seen of the update before (incremental update: blocks >= it are new)
 };
 
-__device__ __forceinline__ unsigned char oe_class(unsigned int w, int l_occ) {
-  return !lo_known(w) ? OE_UNK : (lo_val(w) > l_occ ? OE_OCC : OE_FREE);
-}
-__device__ __forceinline__ float oe_seed(unsigned char c, float D) { return c == OE_FREE ? D : (c == OE_OCC ? -D : 0.0f); }
+__device__ __forceinline__ float oe_seed(unsigned char c, float D) { return c == OC_FREE ? D : (c == OC_OCC ? -D : 0.0f); }
 __device__ __forceinline__ int oe_tidx(int lx, int ly, int lz) { return ((lx + 1) * OE_T + (ly + 1)) * OE_T + (lz + 1); }
 
 // full update: every block of the submap seeded, neighbour table built, epoch 0 (a wave source)
@@ -62,7 +57,7 @@ __global__ void __launch_bounds__(OE_THREADS) k_octo_esdf_init(OcGrid g, OeAux a
     }
     const size_t base = (size_t)b * OC_B3;
     for (int v = threadIdx.x; v < OC_B3; v += blockDim.x) {
-      const unsigned char c = oe_class(g.cnt[base + v], l_occ);
+      const unsigned char c = oc_class(g.cnt[base + v], l_occ);
       a.e[base + v] = oe_seed(c, D);
       a.cls[base + v] = c;
     }
@@ -87,7 +82,7 @@ __global__ void __launch_bounds__(256) k_octo_esdf_prepare(OcGrid g, OeAux a, in
     }
     if (b >= nb_prev) {
       const size_t base = (size_t)b * OC_B3;
-      for (int v = lane; v < OC_B3; v += 32) { a.cls[base + v] = OE_UNK; a.e[base + v] = 0.0f; }
+      for (int v = lane; v < OC_B3; v += 32) { a.cls[base + v] = OC_UNK; a.e[base + v] = 0.0f; }
     }
   }
 }
@@ -105,7 +100,7 @@ __global__ void __launch_bounds__(OE_THREADS) k_octo_esdf_detect(OcGrid g, OeAux
     int mine = 0;
     for (int v = threadIdx.x; v < OC_B3; v += blockDim.x) {
       const unsigned char oc = a.cls[base + v] & ES_CLS;
-      if (oe_class(g.cnt[base + v], l_occ) != oc) { a.cls[base + v] = oc | ES_CH; mine++; }
+      if (oc_class(g.cnt[base + v], l_occ) != oc) { a.cls[base + v] = oc | ES_CH; mine++; }
     }
     for (int o = 16; o > 0; o >>= 1) mine += __shfl_xor_sync(0xffffffffu, mine, o);
     if ((threadIdx.x & 31) == 0 && mine) atomicAdd(&s_any, mine);
@@ -130,7 +125,7 @@ __device__ __forceinline__ void oe_stage(const OeAux& a, OeTile& tile) {
     const int lz = c % OE_T - 1, ly = (c / OE_T) % OE_T - 1, lx = c / (OE_T * OE_T) - 1;
     const int nbk = tile.nbr[(((lx + 8) >> 3) * 3 + ((ly + 8) >> 3)) * 3 + ((lz + 8) >> 3)];
     float ev = 0.0f;
-    unsigned char cl = OE_UNK;
+    unsigned char cl = OC_UNK;
     if (nbk >= 0) {
       const size_t off = (size_t)nbk * OC_B3 + oc_voxel_off(lx, ly, lz);
       cl = *(volatile unsigned char*)&a.cls[off];
@@ -168,7 +163,7 @@ __global__ void __launch_bounds__(OE_THREADS) k_octo_esdf_raise(OcGrid g, OeAux 
       for (int v = threadIdx.x; v < OC_B3; v += blockDim.x) {
         const int c0 = oe_tidx(v >> 6, (v >> 3) & 7, v & 7);
         const unsigned char cl = tile.cls[c0];
-        if (cl != OE_FREE && cl != OE_OCC) continue;  // flagged or unknown: nothing to decide
+        if (cl != OC_FREE && cl != OC_OCC) continue;  // flagged or unknown: nothing to decide
         const float cur = tile.e[c0];
         bool hit = false;
 #pragma unroll
@@ -182,10 +177,10 @@ __global__ void __launch_bounds__(OE_THREADS) k_octo_esdf_raise(OcGrid g, OeAux 
               const int cn = c0 + (dx * OE_T + dy) * OE_T + dz;
               const unsigned char hf = tile.cls[cn];
               const unsigned char hc = hf & ES_CLS;  // the neighbour's class at the last update
-              if (!(hf & (ES_CH | ES_SU)) || hc == OE_UNK) continue;
+              if (!(hf & (ES_CH | ES_SU)) || hc == OC_UNK) continue;
               const float dis = nz_ == 1 ? d1 : (nz_ == 2 ? d2 : d3);
               const float he = tile.e[cn];
-              const float cand = (cl == OE_FREE) ? (hc == OE_OCC ? dis : he + dis) : (hc == OE_FREE ? -dis : he - dis);
+              const float cand = (cl == OC_FREE) ? (hc == OC_OCC ? dis : he + dis) : (hc == OC_FREE ? -dis : he - dis);
               hit |= cand == cur;
             }
         if (hit) { tile.cls[c0] = cl | ES_SU; mine = true; }
@@ -226,7 +221,7 @@ __global__ void __launch_bounds__(OE_THREADS) k_octo_esdf_reinit(OcGrid g, OeAux
     for (int v = threadIdx.x; v < OC_B3; v += blockDim.x) {
       const unsigned char c = a.cls[base + v];
       if (!(c & (ES_CH | ES_SU))) continue;
-      const unsigned char nc = oe_class(g.cnt[base + v], l_occ);
+      const unsigned char nc = oc_class(g.cnt[base + v], l_occ);
       a.e[base + v] = oe_seed(nc, D);
       a.cls[base + v] = nc;
       nsu += (c & ES_SU) ? 1 : 0;
@@ -270,7 +265,7 @@ __global__ void __launch_bounds__(OE_THREADS) k_octo_esdf_sweep(OcGrid g, OeAux 
       for (int v = threadIdx.x; v < OC_B3; v += blockDim.x) {
         const int c0 = oe_tidx(v >> 6, (v >> 3) & 7, v & 7);
         const unsigned char cl = tile.cls[c0];
-        if (cl == OE_UNK) continue;
+        if (cl == OC_UNK) continue;
         float best = tile.e[c0];
         const float cur = best;
 #pragma unroll
@@ -283,11 +278,11 @@ __global__ void __launch_bounds__(OE_THREADS) k_octo_esdf_sweep(OcGrid g, OeAux 
               if (nz_ == 0) continue;
               const int cn = c0 + (dx * OE_T + dy) * OE_T + dz;
               const unsigned char hc = tile.cls[cn];
-              if (hc == OE_UNK) continue;
+              if (hc == OC_UNK) continue;
               const float dis = nz_ == 1 ? d1 : (nz_ == 2 ? d2 : d3);
               const float he = tile.e[cn];
-              if (cl == OE_FREE) best = fminf(best, hc == OE_OCC ? dis : he + dis);
-              else best = fmaxf(best, hc == OE_FREE ? -dis : he - dis);
+              if (cl == OC_FREE) best = fminf(best, hc == OC_OCC ? dis : he + dis);
+              else best = fmaxf(best, hc == OC_FREE ? -dis : he - dis);
             }
         if (best != cur) {
           tile.e[c0] = best;
@@ -323,14 +318,8 @@ __global__ void __launch_bounds__(OE_THREADS) k_octo_esdf_gather(OcGrid g, OeAux
     if (s != submap) continue;  // (uniform per CTA)
     const size_t base = (size_t)b * OC_B3;
     for (int v = threadIdx.x; v < OC_B3; v += blockDim.x) {
-      const bool want = (a.cls[base + v] & ES_CLS) != OE_UNK;
-      const unsigned m = __ballot_sync(0xffffffffu, want);
-      if (!m) continue;
-      const int lane = threadIdx.x & 31, leader = __ffs(m) - 1;
-      unsigned long long rb = 0;
-      if (lane == leader) rb = atomicAdd(counter, (unsigned long long)__popc(m));
-      rb = __shfl_sync(0xffffffffu, rb, leader);
-      const long long row = (long long)(rb + __popc(m & ((1u << lane) - 1)));
+      const bool want = (a.cls[base + v] & ES_CLS) != OC_UNK;
+      const long long row = oc_warp_append(want, counter);
       if (want && row < cap) {
         idx[3 * row] = bx * OC_B + (v >> 6);
         idx[3 * row + 1] = by * OC_B + ((v >> 3) & 7);
@@ -384,7 +373,7 @@ __global__ void __launch_bounds__(256) k_octo_esdf_query(OcGrid g, OeAux a, int 
 #pragma unroll
         for (int c = 0; c < 8; c++) {
           const size_t off = (size_t)b[c] * OC_B3 + oc_voxel_off(i0 + (c >> 2), j0 + ((c >> 1) & 1), k0 + (c & 1));
-          ok &= (a.cls[off] & ES_CLS) != OE_UNK;
+          ok &= (a.cls[off] & ES_CLS) != OC_UNK;
           e[c] = a.e[off];
         }
       }
@@ -424,7 +413,6 @@ static int oe_alloc(tslam_octo* m) {
   TS_CUDA(cudaMalloc(&m->esdf_mem, bytes));
   TS_CUDA(cudaMemset(m->esdf_mem, 0, bytes));
   m->esdf_dirty = oe_aux(m).repoch + m->g.max_blocks;
-  m->esdf_full_needed = 1;
   return TSLAM_OK;
 }
 
@@ -435,39 +423,15 @@ int oc_esdf_free(tslam_octo* m) {
   return TSLAM_OK;
 }
 
-static int oe_logodds(tslam_octo* m, const char* what) {
-  if (!m->logodds) {
-    ts_set_error("%s: the map is a hit counter; the occupancy ESDF needs a log-odds map (tslam_octo_create_logodds)", what);
-    return TSLAM_E_INVALID;
-  }
-  return TSLAM_OK;
-}
-
-// the field of `submap` can be read: an update has completed, for that submap, and no reset or fusion came after it
-static int oe_readable(tslam_octo* m, int32_t submap, const char* what) {
-  int rc = oe_logodds(m, what);
-  if (rc) return rc;
-  if (!m->esdf_mem) { ts_set_error("%s: no ESDF has been computed (tslam_octo_esdf_update has not run)", what); return TSLAM_E_INVALID; }
-  if (m->esdf_full_needed) {
-    ts_set_error("%s: the map was reset or fused since the last completed tslam_octo_esdf_update", what);
-    return TSLAM_E_INVALID;
-  }
-  if (m->esdf_submap != submap) {
-    ts_set_error("%s: the last tslam_octo_esdf_update was for submap %d, not %d", what, m->esdf_submap, submap);
-    return TSLAM_E_INVALID;
-  }
-  return TSLAM_OK;
-}
-
 int oc_esdf_field(tslam_octo* m, int32_t submap, const char* what, OcEsdfField* f) {
-  int rc = oe_readable(m, submap, what);
+  int rc = oc_track_readable(m, m->esdf_track, submap, what, "tslam_octo_esdf_update");
   if (rc) return rc;
   const OeAux a = oe_aux(m);
   f->e = a.e;
   f->cls = a.cls;
   f->nb_seen = a.nb_seen;
   f->D = m->esdf_D;
-  f->free_cls = OE_FREE;
+  f->free_cls = OC_FREE;
   f->cls_mask = ES_CLS;
   return TSLAM_OK;
 }
@@ -476,24 +440,23 @@ int oc_esdf_field(tslam_octo* m, int32_t submap, const char* what, OcEsdfField* 
 // 1 = full recompute.  stats4 (HOST, may be NULL): lower sweeps, raise sweeps (-1 = full), changed voxels, suspect voxels.
 extern "C" int tslam_octo_esdf_update(tslam_octo_t* m, int32_t submap, float max_dist, int32_t mode, int32_t* stats4, void* stream) {
   if (!m) return TSLAM_E_INVALID;
-  int rc = oe_logodds(m, "tslam_octo_esdf_update");
+  int rc = oc_logodds_submap(m, submap, "tslam_octo_esdf_update", "the occupancy ESDF");
   if (rc) return rc;
   if (!(std::isfinite(max_dist) && max_dist > 0.0f)) {
     ts_set_error("tslam_octo_esdf_update: max_dist must be finite and > 0 (got %g)", (double)max_dist);
     return TSLAM_E_INVALID;
   }
   if (mode != 0 && mode != 1) { ts_set_error("tslam_octo_esdf_update: mode must be 0 (incremental) or 1 (full)"); return TSLAM_E_INVALID; }
-  if (submap < 0 || submap >= m->cfg.max_submaps) { ts_set_error("tslam_octo_esdf_update: submap %d out of range", submap); return TSLAM_E_INVALID; }
   cudaStream_t st = (cudaStream_t)stream;
   rc = oe_alloc(m);
   if (rc) return rc;
   OeAux a = oe_aux(m);
   const int l_occ = m->lo.l_occ;
   const float vs = m->in.vs;
-  const bool full = mode == 1 || m->esdf_full_needed || m->esdf_submap != submap ||
+  const bool full = mode == 1 || !m->esdf_track.ready || m->esdf_track.submap != submap ||
                     memcmp(&m->esdf_D, &max_dist, sizeof(float)) != 0;
   int h_counts[4] = {0, 0, 0, 0}, n_lower = 0, n_raise = 0;
-  m->esdf_full_needed = 1;  // until this update has completed
+  m->esdf_track.ready = 0;  // until this update has completed
   TS_CUDA(cudaMemsetAsync(a.changed, 0, (2 * (ES_MAX_SWEEPS + 2) + 4) * 4, st));  // changed, rchanged, counts[0..3]
   const int grid = m->sm_count * 8;
   if (full) {
@@ -516,8 +479,7 @@ extern "C" int tslam_octo_esdf_update(tslam_octo_t* m, int32_t submap, float max
     if (rc) return rc;
     TS_CUDA(cudaMemcpy(h_counts, a.counts, 16, cudaMemcpyDeviceToHost));
   }
-  m->esdf_full_needed = 0;
-  m->esdf_submap = submap;
+  m->esdf_track = OcTrack{1, submap};
   m->esdf_D = max_dist;
   if (stats4) { stats4[0] = n_lower; stats4[1] = full ? -1 : n_raise; stats4[2] = h_counts[0]; stats4[3] = h_counts[1]; }
   return TSLAM_OK;
@@ -526,29 +488,22 @@ extern "C" int tslam_octo_esdf_update(tslam_octo_t* m, int32_t submap, float max
 extern "C" int tslam_octo_esdf_gather(tslam_octo_t* m, int32_t submap, int64_t cap, int32_t* idx, float* esdf, int64_t* n_out,
                                       void* stream) {
   if (!m || !n_out || cap < 0 || (cap > 0 && (!idx || !esdf))) return TSLAM_E_INVALID;
-  int rc = oe_readable(m, submap, "tslam_octo_esdf_gather");
+  const char* what = "tslam_octo_esdf_gather";
+  int rc = oc_track_readable(m, m->esdf_track, submap, what, "tslam_octo_esdf_update");
   if (rc) return rc;
   cudaStream_t st = (cudaStream_t)stream;
-  unsigned long long* ctr = (unsigned long long*)(m->scratch_i + 8);
-  TS_CUDA(cudaMemsetAsync(ctr, 0, 8, st));
-  k_octo_esdf_gather<<<m->sm_count * 8, OE_THREADS, 0, st>>>(m->g, oe_aux(m), submap, cap, idx, esdf, ctr);
-  TS_LAUNCH_CHECK(m);
-  unsigned long long v = 0;
-  TS_CUDA(cudaMemcpyAsync(&v, ctr, 8, cudaMemcpyDeviceToHost, st));
-  TS_CUDA(cudaStreamSynchronize(st));
-  *n_out = (int64_t)v;
-  if ((int64_t)v > cap) { ts_set_error("octo esdf gather: %lld voxels > capacity %lld", (long long)v, (long long)cap); return TSLAM_E_CAPACITY; }
-  return TSLAM_OK;
+  return oc_counted_gather(m, st, [&](unsigned long long* ctr) {
+    k_octo_esdf_gather<<<m->sm_count * 8, OE_THREADS, 0, st>>>(m->g, oe_aux(m), submap, cap, idx, esdf, ctr);
+  }, cap, n_out, what);
 }
 
 extern "C" int tslam_octo_esdf_query(tslam_octo_t* m, int32_t submap, int64_t n, const float* xyz, float* dist, float* grad,
                                      uint8_t* valid, void* stream) {
   if (!m || n < 0 || (n && (!xyz || !dist || !grad || !valid))) return TSLAM_E_INVALID;
-  int rc = oe_readable(m, submap, "tslam_octo_esdf_query");
+  int rc = oc_track_readable(m, m->esdf_track, submap, "tslam_octo_esdf_query", "tslam_octo_esdf_update");
   if (rc || n == 0) return rc;
-  long long blocks = (n + 255) / 256;
-  if (blocks > (long long)m->sm_count * 16) blocks = (long long)m->sm_count * 16;
-  k_octo_esdf_query<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(m->g, oe_aux(m), submap, n, xyz, m->in.vs, dist, grad, valid);
+  k_octo_esdf_query<<<oc_grid(n, 256, m->sm_count * 16), 256, 0, (cudaStream_t)stream>>>(m->g, oe_aux(m), submap, n, xyz, m->in.vs, dist,
+                                                                                         grad, valid);
   TS_LAUNCH_CHECK(m);
   return TSLAM_OK;
 }

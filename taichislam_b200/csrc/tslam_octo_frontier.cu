@@ -31,7 +31,7 @@
 #define OF_THREADS 128
 #define OF_REC 16    // int64 fields of a cluster record
 
-enum { OF_UNK = 0, OF_FREE = 1, OF_OCC = 2, OF_OUT = 3 };
+#define OF_OUT 3     // halo class of a cell outside the volume, next to the OC_* classes
 
 struct OfAux {
   uint32_t* mask;  // [max_blocks * 16] frontier bits as of the last update
@@ -54,10 +54,6 @@ struct OfClu {     // per cluster slot
   int* sid_s;                 // slot of the q-th cluster in label order
   int* ord;                   // ordinal of each slot in label order
 };
-
-__device__ __forceinline__ unsigned char of_class(unsigned int w, int l_occ) {
-  return !lo_known(w) ? OF_UNK : (lo_val(w) > l_occ ? OF_OCC : OF_FREE);
-}
 
 // index of the block holding local cell (lx, ly, lz), each in [-1, 8], in a 27-entry neighbour table (13 = the block)
 __device__ __forceinline__ int of_nbr_slot(int lx, int ly, int lz) {
@@ -117,7 +113,7 @@ __global__ void __launch_bounds__(OF_THREADS) k_octo_frontier_classify(OcGrid g,
       const int blk = ox ? fnb[ox > 0] : (oy ? fnb[2 + (oy > 0)] : (oz ? fnb[4 + (oz > 0)] : b));
       const int i = bx * OC_B + lx, j = by * OC_B + ly, k = bz * OC_B + lz;
       unsigned char cl = OF_OUT;  // a cell outside the volume can never be observed: it does not count as UNKNOWN
-      if (ts_in_bounds(g, i, j, k)) cl = blk < 0 ? OF_UNK : of_class(g.cnt[(size_t)blk * OC_B3 + oc_voxel_off(i, j, k)], l_occ);
+      if (ts_in_bounds(g, i, j, k)) cl = blk < 0 ? OC_UNK : oc_class(g.cnt[(size_t)blk * OC_B3 + oc_voxel_off(i, j, k)], l_occ);
       cls[c] = cl;
     }
     __syncthreads();
@@ -125,9 +121,9 @@ __global__ void __launch_bounds__(OF_THREADS) k_octo_frontier_classify(OcGrid g,
     for (int r = 0; r < OC_B3 / OF_THREADS; ++r) {
       const int v = r * OF_THREADS + threadIdx.x;
       const int c0 = ((v >> 6) + 1) * OF_T * OF_T + (((v >> 3) & 7) + 1) * OF_T + ((v & 7) + 1);
-      const bool f = cls[c0] == OF_FREE && (cls[c0 - OF_T * OF_T] == OF_UNK || cls[c0 + OF_T * OF_T] == OF_UNK ||
-                                            cls[c0 - OF_T] == OF_UNK || cls[c0 + OF_T] == OF_UNK || cls[c0 - 1] == OF_UNK ||
-                                            cls[c0 + 1] == OF_UNK);
+      const bool f = cls[c0] == OC_FREE && (cls[c0 - OF_T * OF_T] == OC_UNK || cls[c0 + OF_T * OF_T] == OC_UNK ||
+                                            cls[c0 - OF_T] == OC_UNK || cls[c0 + OF_T] == OC_UNK || cls[c0 - 1] == OC_UNK ||
+                                            cls[c0 + 1] == OC_UNK);
       const unsigned word = __ballot_sync(0xffffffffu, f);
       if ((threadIdx.x & 31) == 0) a.mask[(size_t)b * OF_WORDS + (v >> 5)] = word;
     }
@@ -389,7 +385,6 @@ static int of_alloc(tslam_octo* m) {
   TS_CUDA(cudaMalloc(&m->fr_mem, bytes));
   TS_CUDA(cudaMemset(m->fr_mem, 0, bytes));
   m->fr_dirty = of_aux(m).dirty;
-  m->fr_full_needed = 1;
   return TSLAM_OK;
 }
 
@@ -405,16 +400,6 @@ static int of_grow(void** p, long long* cap, long long need, size_t per) {
   return TSLAM_OK;
 }
 
-static int of_tmp(tslam_octo* m, size_t need) {
-  if (need <= m->fr_tmp_bytes) return TSLAM_OK;
-  if (m->fr_tmp) cudaFree(m->fr_tmp);
-  m->fr_tmp = nullptr;
-  m->fr_tmp_bytes = 0;
-  TS_CUDA(cudaMalloc(&m->fr_tmp, need));
-  m->fr_tmp_bytes = need;
-  return TSLAM_OK;
-}
-
 int oc_frontier_free(tslam_octo* m) {
   if (m->fr_mem) cudaFree(m->fr_mem);
   if (m->fr_vox) cudaFree(m->fr_vox);
@@ -427,66 +412,34 @@ int oc_frontier_free(tslam_octo* m) {
   return TSLAM_OK;
 }
 
-static int of_logodds(tslam_octo* m, const char* what) {
-  if (!m->logodds) {
-    ts_set_error("%s: the map is a hit counter; frontiers need a log-odds map (tslam_octo_create_logodds)", what);
-    return TSLAM_E_INVALID;
-  }
-  return TSLAM_OK;
-}
-
-// the frontier set of `submap` can be read: an update has completed, for that submap, and no reset or fusion came after it
-static int of_readable(tslam_octo* m, int32_t submap, const char* what) {
-  int rc = of_logodds(m, what);
-  if (rc) return rc;
-  if (!m->fr_mem) { ts_set_error("%s: no frontier set has been computed (tslam_octo_frontier_update has not run)", what); return TSLAM_E_INVALID; }
-  if (m->fr_full_needed) {
-    ts_set_error("%s: the map was reset or fused since the last completed tslam_octo_frontier_update", what);
-    return TSLAM_E_INVALID;
-  }
-  if (m->fr_submap != submap) {
-    ts_set_error("%s: the last tslam_octo_frontier_update was for submap %d, not %d", what, m->fr_submap, submap);
-    return TSLAM_E_INVALID;
-  }
-  return TSLAM_OK;
-}
-
-int oc_frontier_readable(tslam_octo* m, int32_t submap, const char* what) { return of_readable(m, submap, what); }
-
-static int of_grid(long long work, int per_cta, int cap) {
-  const long long g = (work + per_cta - 1) / per_cta;
-  return (int)(g < 1 ? 1 : (g > cap ? cap : g));
-}
-
 // mode 0 = incremental when the state allows it (same submap as the last update, no reset / fusion in between), 1 = full.
 // stats4 (HOST, may be NULL): frontier voxels, clusters, blocks re-examined, 1 when the update was full.
 extern "C" int tslam_octo_frontier_update(tslam_octo_t* m, int32_t submap, int32_t mode, int32_t* stats4, void* stream) {
   if (!m) return TSLAM_E_INVALID;
-  int rc = of_logodds(m, "tslam_octo_frontier_update");
+  int rc = oc_logodds_submap(m, submap, "tslam_octo_frontier_update", "a frontier set");
   if (rc) return rc;
   if (mode != 0 && mode != 1) { ts_set_error("tslam_octo_frontier_update: mode must be 0 (incremental) or 1 (full)"); return TSLAM_E_INVALID; }
-  if (submap < 0 || submap >= m->cfg.max_submaps) { ts_set_error("tslam_octo_frontier_update: submap %d out of range", submap); return TSLAM_E_INVALID; }
   cudaStream_t st = (cudaStream_t)stream;
   rc = of_alloc(m);
   if (rc) return rc;
   OfAux a = of_aux(m);
-  const bool full = mode == 1 || m->fr_full_needed || m->fr_submap != submap;
-  m->fr_full_needed = 1;  // until this update has completed
+  const bool full = mode == 1 || !m->fr_track.ready || m->fr_track.submap != submap;
+  m->fr_track.ready = 0;  // until this update has completed
   int nb = 0;
   TS_CUDA(cudaMemcpyAsync(&nb, m->g.n_blocks, 4, cudaMemcpyDeviceToHost, st));
   TS_CUDA(cudaMemsetAsync(a.ctr, 0, 4 * 4, st));
   TS_CUDA(cudaStreamSynchronize(st));
   if (nb > m->g.max_blocks) nb = m->g.max_blocks;
   const int cap_grid = m->sm_count * 16;
-  k_octo_frontier_prepare<<<of_grid(nb, 256, cap_grid), 256, 0, st>>>(m->g, a, submap, nb, full ? 0 : m->fr_nb, full ? 1 : 0);
+  k_octo_frontier_prepare<<<oc_grid(nb, 256, cap_grid), 256, 0, st>>>(m->g, a, submap, nb, full ? 0 : m->fr_nb, full ? 1 : 0);
   TS_LAUNCH_CHECK(m);
   k_octo_frontier_classify<<<m->sm_count * 8, OF_THREADS, 0, st>>>(m->g, a, m->lo.l_occ);
   TS_LAUNCH_CHECK(m);
-  k_octo_frontier_count<<<of_grid((long long)nb + 1, 256, cap_grid), 256, 0, st>>>(m->g, a, submap, nb);
+  k_octo_frontier_count<<<oc_grid((long long)nb + 1, 256, cap_grid), 256, 0, st>>>(m->g, a, submap, nb);
   TS_LAUNCH_CHECK(m);
   size_t tb = 0;
   TS_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tb, a.pc, a.off, nb + 1, st));
-  rc = of_tmp(m, tb);
+  rc = oc_reserve(&m->fr_tmp, &m->fr_tmp_bytes, tb);
   if (rc) return rc;
   TS_CUDA(cub::DeviceScan::ExclusiveSum(m->fr_tmp, tb, a.pc, a.off, nb + 1, st));
   int n = 0, region = 0, nc = 0;
@@ -497,35 +450,34 @@ extern "C" int tslam_octo_frontier_update(tslam_octo_t* m, int32_t submap, int32
     rc = of_grow(&m->fr_vox, &m->fr_vox_cap, n, 2 * sizeof(int));
     if (rc) return rc;
     OfVox x = of_vox(m);
-    k_octo_frontier_iota<<<of_grid(n, 256, cap_grid), 256, 0, st>>>(x.parent, n);
+    k_octo_frontier_iota<<<oc_grid(n, 256, cap_grid), 256, 0, st>>>(x.parent, n);
     TS_LAUNCH_CHECK(m);
-    k_octo_frontier_link<<<of_grid(nb, 8, cap_grid), 256, 0, st>>>(m->g, a, x, nb);
+    k_octo_frontier_link<<<oc_grid(nb, 8, cap_grid), 256, 0, st>>>(m->g, a, x, nb);
     TS_LAUNCH_CHECK(m);
-    k_octo_frontier_compress<<<of_grid(n, 256, cap_grid), 256, 0, st>>>(a, x, n);
+    k_octo_frontier_compress<<<oc_grid(n, 256, cap_grid), 256, 0, st>>>(a, x, n);
     TS_LAUNCH_CHECK(m);
     TS_CUDA(cudaMemcpyAsync(&nc, a.ctr + 1, 4, cudaMemcpyDeviceToHost, st));
     TS_CUDA(cudaStreamSynchronize(st));
     rc = of_grow(&m->fr_clu, &m->fr_clu_cap, nc, OF_REC * 8 + 2 * 8 + 3 * 4);
     if (rc) return rc;
     OfClu c = of_clu(m);
-    k_octo_frontier_rec_init<<<of_grid(nc, 256, cap_grid), 256, 0, st>>>(c, nc);
+    k_octo_frontier_rec_init<<<oc_grid(nc, 256, cap_grid), 256, 0, st>>>(c, nc);
     TS_LAUNCH_CHECK(m);
-    k_octo_frontier_stats<<<of_grid(nb, 8, cap_grid), 256, 0, st>>>(m->g, a, x, c, nb);
+    k_octo_frontier_stats<<<oc_grid(nb, 8, cap_grid), 256, 0, st>>>(m->g, a, x, c, nb);
     TS_LAUNCH_CHECK(m);
     const long long keys = (long long)m->g.N * m->g.N * m->g.Nz;
     int end_bit = 1;
     while (end_bit < 64 && (1ll << end_bit) < keys) end_bit++;
     tb = 0;
     TS_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb, c.key, c.key_s, c.sid, c.sid_s, nc, 0, end_bit, st));
-    rc = of_tmp(m, tb);
+    rc = oc_reserve(&m->fr_tmp, &m->fr_tmp_bytes, tb);
     if (rc) return rc;
     TS_CUDA(cub::DeviceRadixSort::SortPairs(m->fr_tmp, tb, c.key, c.key_s, c.sid, c.sid_s, nc, 0, end_bit, st));
-    k_octo_frontier_order<<<of_grid(nc, 256, cap_grid), 256, 0, st>>>(c, nc);
+    k_octo_frontier_order<<<oc_grid(nc, 256, cap_grid), 256, 0, st>>>(c, nc);
     TS_LAUNCH_CHECK(m);
     TS_CUDA(cudaStreamSynchronize(st));
   }
-  m->fr_full_needed = 0;
-  m->fr_submap = submap;
+  m->fr_track = OcTrack{1, submap};
   m->fr_nb = nb;
   m->fr_n = n;
   m->fr_nc = nc;
@@ -535,7 +487,7 @@ extern "C" int tslam_octo_frontier_update(tslam_octo_t* m, int32_t submap, int32
 
 int oc_frontier_rows(tslam_octo* m, int32_t* idx, int32_t* cluster, cudaStream_t st) {
   if (m->fr_n > 0) {
-    k_octo_frontier_gather<<<of_grid(m->fr_nb, 8, m->sm_count * 16), 256, 0, st>>>(m->g, of_aux(m), of_vox(m), of_clu(m), m->fr_nb,
+    k_octo_frontier_gather<<<oc_grid(m->fr_nb, 8, m->sm_count * 16), 256, 0, st>>>(m->g, of_aux(m), of_vox(m), of_clu(m), m->fr_nb,
                                                                                    m->fr_n, idx, cluster);
     TS_LAUNCH_CHECK(m);
   }
@@ -545,11 +497,11 @@ int oc_frontier_rows(tslam_octo* m, int32_t* idx, int32_t* cluster, cudaStream_t
 extern "C" int tslam_octo_frontier_gather(tslam_octo_t* m, int32_t submap, int64_t cap, int32_t* idx, int32_t* cluster, int64_t* n_out,
                                           void* stream) {
   if (!m || !n_out || cap < 0 || (cap > 0 && (!idx || !cluster))) return TSLAM_E_INVALID;
-  int rc = of_readable(m, submap, "tslam_octo_frontier_gather");
+  int rc = oc_track_readable(m, m->fr_track, submap, "tslam_octo_frontier_gather", "tslam_octo_frontier_update");
   if (rc) return rc;
   *n_out = m->fr_n;
   if (m->fr_n > 0 && cap > 0) {
-    k_octo_frontier_gather<<<of_grid(m->fr_nb, 8, m->sm_count * 16), 256, 0, (cudaStream_t)stream>>>(
+    k_octo_frontier_gather<<<oc_grid(m->fr_nb, 8, m->sm_count * 16), 256, 0, (cudaStream_t)stream>>>(
         m->g, of_aux(m), of_vox(m), of_clu(m), m->fr_nb, cap, idx, cluster);
     TS_LAUNCH_CHECK(m);
   }
@@ -559,12 +511,12 @@ extern "C" int tslam_octo_frontier_gather(tslam_octo_t* m, int32_t submap, int64
 
 extern "C" int tslam_octo_frontier_clusters(tslam_octo_t* m, int32_t submap, int64_t cap, int64_t* rec16, int64_t* n_out, void* stream) {
   if (!m || !n_out || cap < 0 || (cap > 0 && !rec16)) return TSLAM_E_INVALID;
-  int rc = of_readable(m, submap, "tslam_octo_frontier_clusters");
+  int rc = oc_track_readable(m, m->fr_track, submap, "tslam_octo_frontier_clusters", "tslam_octo_frontier_update");
   if (rc) return rc;
   *n_out = m->fr_nc;
   const int n = (int)(m->fr_nc < cap ? m->fr_nc : cap);
   if (n > 0) {
-    k_octo_frontier_records<<<of_grid((long long)n * OF_REC, 256, m->sm_count * 16), 256, 0, (cudaStream_t)stream>>>(of_clu(m), n, rec16);
+    k_octo_frontier_records<<<oc_grid((long long)n * OF_REC, 256, m->sm_count * 16), 256, 0, (cudaStream_t)stream>>>(of_clu(m), n, rec16);
     TS_LAUNCH_CHECK(m);
   }
   if (m->fr_nc > cap) { ts_set_error("octo frontier clusters: %d clusters > capacity %lld", m->fr_nc, (long long)cap); return TSLAM_E_CAPACITY; }

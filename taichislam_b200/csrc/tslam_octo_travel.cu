@@ -334,13 +334,7 @@ __global__ void __launch_bounds__(OT_THREADS) k_octo_travel_slot_gather(OcGrid g
     for (int v = threadIdx.x; v < OC_B3; v += blockDim.x) {
       const float gv = G[v];
       const bool want = isfinite(gv);
-      const unsigned m = __ballot_sync(0xffffffffu, want);
-      if (!m) continue;
-      const int lane = threadIdx.x & 31, leader = __ffs(m) - 1;
-      unsigned long long rb = 0;
-      if (lane == leader) rb = atomicAdd(counter, (unsigned long long)__popc(m));
-      rb = __shfl_sync(0xffffffffu, rb, leader);
-      const long long row = (long long)(rb + __popc(m & ((1u << lane) - 1)));
+      const long long row = oc_warp_append(want, counter);
       if (want && row < cap) {
         idx[3 * row] = bx * OC_B + (v >> 6);
         idx[3 * row + 1] = by * OC_B + ((v >> 3) & 7);
@@ -466,31 +460,9 @@ int oc_travel_free(tslam_octo* m) {
   return TSLAM_OK;
 }
 
-// the checks every travel call makes first
-static int ot_check(tslam_octo* m, int32_t submap, const char* what) {
-  if (!m->logodds) {
-    ts_set_error("%s: the map is a hit counter; a travel-cost field needs a log-odds map (tslam_octo_create_logodds)", what);
-    return TSLAM_E_INVALID;
-  }
-  if (submap < 0 || submap >= m->cfg.max_submaps) { ts_set_error("%s: submap %d out of range", what, submap); return TSLAM_E_INVALID; }
-  return TSLAM_OK;
-}
-
-// the fields of f can be read for `submap`: an update has completed, for that submap, and no reset or fusion came after it
-static int ot_readable(tslam_octo* m, const OcTravel& f, int32_t submap, const char* what) {
-  int rc = ot_check(m, submap, what);
-  if (rc) return rc;
-  if (!f.ready) {
-    ts_set_error("%s: no completed update of this travel-cost field since the map was created, reset or fused, or since the "
-                 "last update failed", what);
-    return TSLAM_E_INVALID;
-  }
-  if (f.submap != submap) {
-    ts_set_error("%s: the last update of this travel-cost field was for submap %d, not %d", what, f.submap, submap);
-    return TSLAM_E_INVALID;
-  }
-  return TSLAM_OK;
-}
+#define OT_UPDATE "tslam_octo_travel_update"
+#define OTM_UPDATE "tslam_octo_travel_multi_update"
+#define OT_FEATURE "a travel-cost field"
 
 // the clearance and max_cost checks of every travel update, and the occupancy ESDF the clearance test reads
 static int ot_params(tslam_octo* m, int32_t submap, float clearance, float max_cost, const char* what, OcEsdfField* ef) {
@@ -526,12 +498,6 @@ static bool ot_start_cell(const tslam_octo* m, const float* p, int c[3]) {
          c[2] < m->g.Nz - m->g.hNz;
 }
 
-static int ot_grid(tslam_octo* m, long long n) {
-  long long blocks = (n + 255) / 256;
-  if (blocks > (long long)m->sm_count * 16) blocks = (long long)m->sm_count * 16;
-  return (int)blocks;
-}
-
 // The fields of `submap` from the S finite starts[S,3] into f, for both update entry points (`what` names the one called
 // in messages).  A refused clearance or max_cost leaves f's last fields readable; from then on f is unreadable until the
 // update completes.  Outputs as tslam_octo_travel_multi_update.
@@ -540,7 +506,7 @@ static int ot_update(tslam_octo* m, OcTravel& f, int32_t submap, int S, const fl
   OcEsdfField ef;
   int rc = ot_params(m, submap, clearance, max_cost, what, &ef);
   if (rc) return rc;
-  f.ready = 0;  // until this update has completed
+  f.track.ready = 0;  // until this update has completed
   f.S = S;
   f.nt = 0;  // (until classify has counted the slots)
   if (!f.blk) TS_CUDA(cudaMalloc(&f.blk, otm_blk_bytes((size_t)m->g.max_blocks)));
@@ -589,8 +555,7 @@ static int ot_update(tslam_octo* m, OcTravel& f, int32_t submap, int S, const fl
   TS_CUDA(cudaMemcpyAsync(h_reach.data(), a.reach, (size_t)S * 4, cudaMemcpyDeviceToHost, st));
   TS_CUDA(cudaMemcpyAsync(h_item.data(), a.sitem, (size_t)S * 4, cudaMemcpyDeviceToHost, st));
   TS_CUDA(cudaStreamSynchronize(st));
-  f.ready = 1;
-  f.submap = submap;
+  f.track = OcTrack{1, submap};
   if (stats2) { stats2[0] = sweeps; stats2[1] = h_counts[0]; }
   for (int s = 0; s < S; s++) {
     if (reachable) reachable[s] = h_reach[s];
@@ -603,7 +568,7 @@ extern "C" int tslam_octo_travel_update(tslam_octo_t* m, int32_t submap, const f
                                         int32_t* stats4, void* stream) {
   const char* what = "tslam_octo_travel_update";
   if (!m || !start3) return TSLAM_E_INVALID;
-  int rc = ot_check(m, submap, what);
+  int rc = oc_logodds_submap(m, submap, what, OT_FEATURE);
   if (rc) return rc;
   if (!(std::isfinite(start3[0]) && std::isfinite(start3[1]) && std::isfinite(start3[2]))) {
     ts_set_error("%s: the start must be finite", what);
@@ -620,27 +585,21 @@ extern "C" int tslam_octo_travel_update(tslam_octo_t* m, int32_t submap, const f
 extern "C" int tslam_octo_travel_gather(tslam_octo_t* m, int32_t submap, int64_t cap, int32_t* idx, float* cost, int64_t* n_out,
                                         void* stream) {
   if (!m || !n_out || cap < 0 || (cap > 0 && (!idx || !cost))) return TSLAM_E_INVALID;
-  int rc = ot_readable(m, m->tr, submap, "tslam_octo_travel_gather");
+  const char* what = "tslam_octo_travel_gather";
+  int rc = oc_track_readable(m, m->tr.track, submap, what, OT_UPDATE);
   if (rc) return rc;
   cudaStream_t st = (cudaStream_t)stream;
-  unsigned long long* ctr = (unsigned long long*)(m->scratch_i + 8);
-  TS_CUDA(cudaMemsetAsync(ctr, 0, 8, st));
-  k_octo_travel_slot_gather<<<m->sm_count * 8, OT_THREADS, 0, st>>>(m->g, otm_aux(m, m->tr), 0, cap, idx, cost, ctr);
-  TS_LAUNCH_CHECK(m);
-  unsigned long long v = 0;
-  TS_CUDA(cudaMemcpyAsync(&v, ctr, 8, cudaMemcpyDeviceToHost, st));
-  TS_CUDA(cudaStreamSynchronize(st));
-  *n_out = (int64_t)v;
-  if ((int64_t)v > cap) { ts_set_error("octo travel gather: %lld cells > capacity %lld", (long long)v, (long long)cap); return TSLAM_E_CAPACITY; }
-  return TSLAM_OK;
+  return oc_counted_gather(m, st, [&](unsigned long long* ctr) {
+    k_octo_travel_slot_gather<<<m->sm_count * 8, OT_THREADS, 0, st>>>(m->g, otm_aux(m, m->tr), 0, cap, idx, cost, ctr);
+  }, cap, n_out, what);
 }
 
 extern "C" int tslam_octo_travel_query(tslam_octo_t* m, int32_t submap, int64_t n, const float* xyz, float* cost, void* stream) {
   if (!m || n < 0 || (n && (!xyz || !cost))) return TSLAM_E_INVALID;
-  int rc = ot_readable(m, m->tr, submap, "tslam_octo_travel_query");
+  int rc = oc_track_readable(m, m->tr.track, submap, "tslam_octo_travel_query", OT_UPDATE);
   if (rc || n == 0) return rc;
-  k_octo_travel_multi_query<<<ot_grid(m, n), 256, 0, (cudaStream_t)stream>>>(m->g, otm_aux(m, m->tr), submap, n, xyz,
-                                                                             m->in.vs, cost);
+  k_octo_travel_multi_query<<<oc_grid(n, 256, m->sm_count * 16), 256, 0, (cudaStream_t)stream>>>(m->g, otm_aux(m, m->tr), submap, n,
+                                                                                                 xyz, m->in.vs, cost);
   TS_LAUNCH_CHECK(m);
   return TSLAM_OK;
 }
@@ -650,10 +609,10 @@ extern "C" int tslam_octo_travel_path(tslam_octo_t* m, int32_t submap, int64_t n
   if (!m || n < 0 || (n && (!xyz || !cells || !len))) return TSLAM_E_INVALID;
   const char* what = "tslam_octo_travel_path";
   if (max_len < 1) { ts_set_error("%s: max_len must be >= 1 (got %d)", what, max_len); return TSLAM_E_INVALID; }
-  int rc = ot_readable(m, m->tr, submap, what);
+  int rc = oc_track_readable(m, m->tr.track, submap, what, OT_UPDATE);
   if (rc || n == 0) return rc;
-  k_octo_travel_multi_path<<<ot_grid(m, n), 256, 0, (cudaStream_t)stream>>>(m->g, otm_aux(m, m->tr), submap, n, nullptr, xyz,
-                                                                            m->in.vs, max_len, cells, len);
+  k_octo_travel_multi_path<<<oc_grid(n, 256, m->sm_count * 16), 256, 0, (cudaStream_t)stream>>>(m->g, otm_aux(m, m->tr), submap, n,
+                                                                                                nullptr, xyz, m->in.vs, max_len, cells, len);
   TS_LAUNCH_CHECK(m);
   return TSLAM_OK;
 }
@@ -662,7 +621,7 @@ extern "C" int tslam_octo_travel_multi_update(tslam_octo_t* m, int32_t submap, i
                                               float max_cost, int32_t* stats2, int32_t* reachable, uint8_t* start_ok, void* stream) {
   const char* what = "tslam_octo_travel_multi_update";
   if (!m || !starts) return TSLAM_E_INVALID;
-  int rc = ot_check(m, submap, what);
+  int rc = oc_logodds_submap(m, submap, what, OT_FEATURE);
   if (rc) return rc;
   if (n_starts < 1 || n_starts > TSLAM_OCTO_TRAVEL_MAX_STARTS) {
     ts_set_error("%s: n_starts must be in [1, %d] (got %d)", what, TSLAM_OCTO_TRAVEL_MAX_STARTS, n_starts);
@@ -678,10 +637,10 @@ extern "C" int tslam_octo_travel_multi_update(tslam_octo_t* m, int32_t submap, i
 
 extern "C" int tslam_octo_travel_multi_query(tslam_octo_t* m, int32_t submap, int64_t n, const float* xyz, float* cost, void* stream) {
   if (!m || n < 0 || (n && (!xyz || !cost))) return TSLAM_E_INVALID;
-  int rc = ot_readable(m, m->trm, submap, "tslam_octo_travel_multi_query");
+  int rc = oc_track_readable(m, m->trm.track, submap, "tslam_octo_travel_multi_query", OTM_UPDATE);
   if (rc || n == 0) return rc;
-  k_octo_travel_multi_query<<<ot_grid(m, n), 256, 0, (cudaStream_t)stream>>>(m->g, otm_aux(m, m->trm), submap, n,
-                                                                             xyz, m->in.vs, cost);
+  k_octo_travel_multi_query<<<oc_grid(n, 256, m->sm_count * 16), 256, 0, (cudaStream_t)stream>>>(m->g, otm_aux(m, m->trm), submap, n,
+                                                                                                 xyz, m->in.vs, cost);
   TS_LAUNCH_CHECK(m);
   return TSLAM_OK;
 }
@@ -691,10 +650,10 @@ extern "C" int tslam_octo_travel_multi_path(tslam_octo_t* m, int32_t submap, int
   if (!m || n < 0 || (n && (!source || !xyz || !cells || !len))) return TSLAM_E_INVALID;
   const char* what = "tslam_octo_travel_multi_path";
   if (max_len < 1) { ts_set_error("%s: max_len must be >= 1 (got %d)", what, max_len); return TSLAM_E_INVALID; }
-  int rc = ot_readable(m, m->trm, submap, what);
+  int rc = oc_track_readable(m, m->trm.track, submap, what, OTM_UPDATE);
   if (rc || n == 0) return rc;
-  k_octo_travel_multi_path<<<ot_grid(m, n), 256, 0, (cudaStream_t)stream>>>(m->g, otm_aux(m, m->trm), submap, n,
-                                                                            source, xyz, m->in.vs, max_len, cells, len);
+  k_octo_travel_multi_path<<<oc_grid(n, 256, m->sm_count * 16), 256, 0, (cudaStream_t)stream>>>(m->g, otm_aux(m, m->trm), submap, n,
+                                                                                                source, xyz, m->in.vs, max_len, cells, len);
   TS_LAUNCH_CHECK(m);
   return TSLAM_OK;
 }

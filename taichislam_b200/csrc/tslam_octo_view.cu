@@ -21,18 +21,19 @@
 #define OV_SCRATCH_BYTES (256ull << 20)  // bitmap budget per chunk of views (TSLAM_VIEW_SCRATCH overrides); >= 1 view
 #define OV_MAX_HALF (1 << 22)            // largest window half-extent in cells: cell indices stay far from int overflow
 
-enum { OV_UNK = 0, OV_FREE = 1, OV_OCC = 2 };
-
 struct OvCam {
   float fx, fy, cx, cy, max_range, wmax, hmax;  // wmax / hmax = f32(width - 1), f32(height - 1)
   int ww, hh, step;                             // rays per row / column, pixel stride
   int half;                                     // window half-extent in cells
 };
 
-__device__ __forceinline__ int ov_class(const OcGrid& g, int blk, int i, int j, int k, int l_occ) {
-  if (blk < 0) return OV_UNK;
+// oc_class of cell (i, j, k) in pool block blk; an absent block (blk < 0) reads UNKNOWN.  The rule is spelled out here
+// because calling oc_class changes the SASS of the three kernels that use it (k_octo_lo_walk keeps its walk for the
+// same reason).
+__device__ __forceinline__ int ov_cell_class(const OcGrid& g, int blk, int i, int j, int k, int l_occ) {
+  if (blk < 0) return OC_UNK;
   const unsigned int w = g.cnt[(size_t)blk * OC_B3 + oc_voxel_off(i, j, k)];
-  return !lo_known(w) ? OV_UNK : (lo_val(w) > l_occ ? OV_OCC : OV_FREE);
+  return !lo_known(w) ? OC_UNK : (lo_val(w) > l_occ ? OC_OCC : OC_FREE);
 }
 
 // valid[v] for every view
@@ -48,7 +49,7 @@ __global__ void __launch_bounds__(256) k_octo_view_valid(OcGrid g, int s, float 
       if (ok) {
         const int i = (int)roundf(u0), j = (int)roundf(u1), k = (int)roundf(u2);
         ok = ts_in_bounds(g, i, j, k) &&
-             ov_class(g, ts_find(g, ts_pack_key(s, i >> OC_BSHIFT, j >> OC_BSHIFT, k >> OC_BSHIFT)), i, j, k, l_occ) == OV_FREE;
+             ov_cell_class(g, ts_find(g, ts_pack_key(s, i >> OC_BSHIFT, j >> OC_BSHIFT, k >> OC_BSHIFT)), i, j, k, l_occ) == OC_FREE;
       }
     }
     valid[v] = ok ? 1 : 0;
@@ -100,9 +101,9 @@ __global__ void __launch_bounds__(256) k_octo_view_unknown(OcGrid g, OvCam cam, 
             ckey = key;
             cblk = ts_find(g, key);
           }
-          const int cl = ov_class(g, cblk, w.cx, w.cy, w.cz, l_occ);
-          if (cl == OV_OCC) break;
-          if (cl == OV_UNK) {
+          const int cl = ov_cell_class(g, cblk, w.cx, w.cy, w.cz, l_occ);
+          if (cl == OC_OCC) break;
+          if (cl == OC_UNK) {
             const int dx = w.cx - lox, dy = w.cy - loy, dz = w.cz - loz;
             if ((unsigned)dx >= (unsigned)nx || (unsigned)dy >= (unsigned)ny || (unsigned)dz >= (unsigned)nz) {
               atomicOr(g.err, OC_ERR_VIEW_WINDOW);  // never dropped silently: the next synchronising call reports it
@@ -174,7 +175,7 @@ __global__ void __launch_bounds__(256) k_octo_view_frontier(OcGrid g, OvCam cam,
                 ckey = key;
                 cblk = ts_find(g, key);
               }
-              if (!ts_in_bounds(g, w.cx, w.cy, w.cz) || ov_class(g, cblk, w.cx, w.cy, w.cz, l_occ) != OV_FREE) {
+              if (!ts_in_bounds(g, w.cx, w.cy, w.cz) || ov_cell_class(g, cblk, w.cx, w.cy, w.cz, l_occ) != OC_FREE) {
                 vis = false;
                 break;
               }
@@ -207,29 +208,13 @@ int oc_view_free(tslam_octo* m) {
   return TSLAM_OK;
 }
 
-static int ov_scratch(tslam_octo* m, size_t need) {
-  if (need <= m->vw_bytes) return TSLAM_OK;
-  oc_view_free(m);
-  TS_CUDA(cudaMalloc(&m->vw_mem, need));
-  m->vw_bytes = need;
-  return TSLAM_OK;
-}
-
-static int ov_grid(long long work, int cap) {
-  const long long g = (work + 255) / 256;
-  return (int)(g < 1 ? 1 : (g > cap ? cap : g));
-}
-
 // The checks both calls share; fills the kernel's camera.  The window half-extent is ceil(r_max / vs) + 2 with r_max the
 // largest |(x, y, dep)| over the image corners at dep = max_range (f64; a rotation keeps the length).
 static int ov_check(tslam_octo* m, int32_t submap, int64_t n, const void* pos, const void* R9, const tslam_view_camera_t* cam,
                     const void* valid, const void* out, const char* what, OvCam& c) {
   if (!m || !cam || n < 0 || (n > 0 && (!pos || !R9 || !valid || !out))) return TSLAM_E_INVALID;
-  if (!m->logodds) {
-    ts_set_error("%s: the map is a hit counter; a viewpoint gain needs a log-odds map (tslam_octo_create_logodds)", what);
-    return TSLAM_E_INVALID;
-  }
-  if (submap < 0 || submap >= m->cfg.max_submaps) { ts_set_error("%s: submap %d out of range", what, submap); return TSLAM_E_INVALID; }
+  const int rc = oc_logodds_submap(m, submap, what, "a viewpoint gain");
+  if (rc) return rc;
   if (!(std::isfinite(cam->fx) && cam->fx > 0.0f && std::isfinite(cam->fy) && cam->fy > 0.0f && std::isfinite(cam->max_range) &&
         cam->max_range > 0.0f && std::isfinite(cam->cx) && std::isfinite(cam->cy))) {
     ts_set_error("%s: the camera needs finite fx, fy, max_range > 0 and finite cx, cy", what);
@@ -279,17 +264,17 @@ extern "C" int tslam_octo_view_gain_unknown(tslam_octo_t* m, int32_t submap, int
   long long chunk = (long long)(budget / ((unsigned long long)words * 4));
   if (chunk < 1) chunk = 1;
   if (chunk > n) chunk = n;
-  rc = ov_scratch(m, (size_t)(chunk * words * 4));
+  rc = oc_reserve(&m->vw_mem, &m->vw_bytes, (size_t)(chunk * words * 4));
   if (rc) return rc;
   uint32_t* bits = (uint32_t*)m->vw_mem;
   TS_CUDA(cudaMemsetAsync(gain, 0, (size_t)n * 8, st));
   const int cap = m->sm_count * 16;
-  k_octo_view_valid<<<ov_grid(n, cap), 256, 0, st>>>(m->g, submap, m->in.vs, m->lo.l_occ, pos, R9, n, valid);
+  k_octo_view_valid<<<oc_grid(n, 256, cap), 256, 0, st>>>(m->g, submap, m->in.vs, m->lo.l_occ, pos, R9, n, valid);
   TS_LAUNCH_CHECK(m);
   for (long long v0 = 0; v0 < n; v0 += chunk) {
     const int nv = (int)(n - v0 < chunk ? n - v0 : chunk);
     TS_CUDA(cudaMemsetAsync(bits, 0, (size_t)nv * words * 4, st));
-    k_octo_view_unknown<<<ov_grid((long long)nv * c.ww * c.hh, m->sm_count * 64), 256, 0, st>>>(
+    k_octo_view_unknown<<<oc_grid((long long)nv * c.ww * c.hh, 256, m->sm_count * 64), 256, 0, st>>>(
         m->g, c, submap, m->in.vs, m->lo.l_occ, pos, R9, valid, v0, nv, words, bits, (unsigned long long*)gain);
     TS_LAUNCH_CHECK(m);
   }
@@ -303,7 +288,7 @@ extern "C" int tslam_octo_view_gain_frontier(tslam_octo_t* m, int32_t submap, in
   OvCam c;
   int rc = ov_check(m, submap, n, pos, R9, cam, valid, total, what, c);
   if (rc) return rc;
-  rc = oc_frontier_readable(m, submap, what);
+  rc = oc_track_readable(m, m->fr_track, submap, what, "tslam_octo_frontier_update");
   if (rc) return rc;
   if (n_clusters != m->fr_nc) {
     ts_set_error("%s: n_clusters = %lld, but the last tslam_octo_frontier_update found %d clusters", what, (long long)n_clusters, m->fr_nc);
@@ -314,17 +299,17 @@ extern "C" int tslam_octo_view_gain_frontier(tslam_octo_t* m, int32_t submap, in
   TS_CUDA(cudaMemsetAsync(total, 0, (size_t)n * 4, st));
   if (per_cluster && n_clusters > 0) TS_CUDA(cudaMemsetAsync(per_cluster, 0, (size_t)n * n_clusters * 4, st));
   const int cap = m->sm_count * 16;
-  k_octo_view_valid<<<ov_grid(n, cap), 256, 0, st>>>(m->g, submap, m->in.vs, m->lo.l_occ, pos, R9, n, valid);
+  k_octo_view_valid<<<oc_grid(n, 256, cap), 256, 0, st>>>(m->g, submap, m->in.vs, m->lo.l_occ, pos, R9, n, valid);
   TS_LAUNCH_CHECK(m);
   const int nf = m->fr_n;
   if (nf == 0) return TSLAM_OK;
-  rc = ov_scratch(m, (size_t)nf * 16);
+  rc = oc_reserve(&m->vw_mem, &m->vw_bytes, (size_t)nf * 16);
   if (rc) return rc;
   int32_t* fidx = (int32_t*)m->vw_mem;
   int32_t* fcl = fidx + 3 * (size_t)nf;
   rc = oc_frontier_rows(m, fidx, fcl, st);
   if (rc) return rc;
-  k_octo_view_frontier<<<ov_grid(n * nf, m->sm_count * 64), 256, 0, st>>>(m->g, c, submap, m->in.vs, m->lo.l_occ, pos, R9, valid, n,
+  k_octo_view_frontier<<<oc_grid(n * nf, 256, m->sm_count * 64), 256, 0, st>>>(m->g, c, submap, m->in.vs, m->lo.l_occ, pos, R9, valid, n,
                                                                           fidx, fcl, nf, (int)n_clusters, total, per_cluster);
   TS_LAUNCH_CHECK(m);
   return TSLAM_OK;

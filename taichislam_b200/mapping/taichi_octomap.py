@@ -162,49 +162,45 @@ class Octomap(BaseMap):
             return np.zeros(len(xyz), bool)
         return self._h.query_near(xyz, int(voxel), submap=self._active())
 
-    # occupancy ESDF (log-odds maps only, DESIGN.md section 7): the interface of DenseTSDF's ESDF
-    def _esdf_map(self):
+    def _logodds_only(self, feature):
         if self.occupancy_model != "logodds":
-            raise ValueError("the occupancy ESDF needs Octomap(..., occupancy_model='logodds'): a hit counter cannot tell "
-                             "free space from unknown space")
+            raise ValueError(f"{feature} needs Octomap(..., occupancy_model='logodds'): a hit counter cannot tell free space "
+                             "from unknown space")
+
+    # occupancy ESDF (log-odds maps only, DESIGN.md section 7): the interface of DenseTSDF's ESDF
 
     def esdf_update(self, max_dist=None):
         """Bring the ESDF of the active submap up to date (incremental when possible), truncated at max_dist (default
         max_ray_length, the TSDF ESDF's far value) -> dict(lower_sweeps, raise_sweeps (-1: full), changed, suspect)."""
-        self._esdf_map()
+        self._logodds_only("the occupancy ESDF")
         self.esdf_max_dist = float(self.max_ray_length if max_dist is None else max_dist)
         return self._h.esdf_update(self._active(), self.esdf_max_dist)
 
     def get_voxels_ESDF(self):
         """(idx int32[n,3], ESDF f32[n]) of the voxels known at the last esdf_update."""
-        self._esdf_map()
+        self._logodds_only("the occupancy ESDF")
         return self._h.esdf_gather(self._active())
 
     def esdf_query(self, xyz, update=True):
         """Interpolated ESDF and its gradient at points [n,3] of the active submap's map frame: (dist, grad, valid), torch
         CUDA tensors for a torch tensor, numpy arrays for a numpy array.  update=True first brings the field up to date
         (with the max_dist of the last esdf_update, else max_ray_length); update=False answers as of the last update."""
-        self._esdf_map()
+        self._logodds_only("the occupancy ESDF")
         if update:
             self.esdf_update(getattr(self, "esdf_max_dist", None))
         return self._h.esdf_query(xyz, submap=self._active())
 
     # exploration frontiers (log-odds maps only, DESIGN.md section 7): FREE voxels next to in-volume UNKNOWN space
-    def _frontier_map(self):
-        if self.occupancy_model != "logodds":
-            raise ValueError("frontiers need Octomap(..., occupancy_model='logodds'): a hit counter cannot tell free space "
-                             "from unknown space")
-
     def frontier_update(self, full=False):
         """Bring the frontier set of the active submap up to date (incremental when possible) -> dict(voxels, clusters,
         blocks (re-examined), full)."""
-        self._frontier_map()
+        self._logodds_only("the frontier tracker")
         return self._h.frontier_update(self._active(), full=full)
 
     def get_frontiers(self):
         """(idx int32[n,3], cluster int32[n]) of the frontier voxels at the last frontier_update; cluster indexes the
         arrays of get_frontier_clusters(min_voxels=1)."""
-        self._frontier_map()
+        self._logodds_only("the frontier tracker")
         return self._h.frontier_gather(self._active())
 
     def get_frontier_clusters(self, min_voxels=1):
@@ -212,7 +208,7 @@ class Octomap(BaseMap):
         arrays: label, size, faces (voxel / UNKNOWN-neighbour pairs), centroid [n,3], bbox_min / bbox_max [n,3] (cell
         centres in metres of the submap frame, f64 of cell index * f32(constructor voxel_scale)) and direction [n,3]
         (the unit mean direction into unknown space, 0 where the offsets cancel)."""
-        self._frontier_map()
+        self._logodds_only("the frontier tracker")
         rec = self._h.frontier_clusters(self._active())
         rec = rec[rec[:, 1] >= int(min_voxels)]
         vs = float(np.float32(self._h.cfg.voxel_scale))
@@ -231,9 +227,7 @@ class Octomap(BaseMap):
         sight, in total and per cluster (frontier=False leaves both None).  The camera is the depth intrinsics with a
         width x height image; step and max_range default to recast_step and max_ray_length.  update=True first runs
         frontier_update(), so frontiers and classes agree.  Torch CUDA tensors in -> torch tensors out; numpy -> numpy."""
-        if self.occupancy_model != "logodds":
-            raise ValueError("a viewpoint gain needs Octomap(..., occupancy_model='logodds'): a hit counter cannot tell free "
-                             "space from unknown space")
+        self._logodds_only("a viewpoint gain")
         if self.K_cam_dep is None:
             raise ValueError("view_gain needs the depth intrinsics: call set_dep_camera_intrinsic first")
         K = self.K_cam_dep
@@ -250,88 +244,74 @@ class Octomap(BaseMap):
         return out
 
     # travel cost through known free space (log-odds maps only, DESIGN.md section 7)
-    def _travel_map(self):
-        if self.occupancy_model != "logodds":
-            raise ValueError("a travel cost needs Octomap(..., occupancy_model='logodds'): a hit counter cannot tell free "
-                             "space from unknown space")
+    def _travel_clearance(self, clearance):
+        """a log-odds map, and with clearance > 0 the occupancy ESDF brought up to date for it"""
+        self._logodds_only("a travel cost")
+        if float(clearance) > 0.0:
+            d = float(getattr(self, "esdf_max_dist", None) or self.max_ray_length)
+            if np.float32(clearance) > np.float32(d):
+                raise ValueError(f"clearance {clearance} exceeds the ESDF's max_dist {d}: call esdf_update(max_dist) with a "
+                                 "larger max_dist first")
+            self.esdf_update(d)
+
+    def _travel_path(self, read, goal, max_len):
+        """the path that read(targets [1,3], max_len) -> (cells, len) returns for `goal`, start to goal in metres, or None"""
+        if isinstance(goal, self._torch.Tensor):
+            goal = goal.detach().cpu().numpy()
+        g = np.asarray(goal, np.float32).reshape(1, 3)
+        cells, n = read(g, max_len)
+        n = int(n[0])
+        if n == 0:
+            return None
+        if n > max_len:   # the buffer was too small: once more with the reported length
+            cells, n2 = read(g, n)
+            assert int(n2[0]) == n
+        vs = float(np.float32(self._h.cfg.voxel_scale))
+        return cells[0, :n][::-1].astype(np.float64) * vs
 
     def travel_update(self, start, clearance=0.0, max_cost=None):
         """Travel-cost field of the active submap from `start` (metres, map frame) through known free space -> dict(
         reachable, sweeps, traversable, start_ok).  clearance > 0 keeps to cells at least that far from occupied space:
         it first runs esdf_update() with the max_dist of the last esdf_update (else max_ray_length) and raises
         ValueError when clearance exceeds it.  max_cost None: no bound below the limit 2^22 * voxel_scale."""
-        self._travel_map()
-        if float(clearance) > 0.0:
-            d = float(getattr(self, "esdf_max_dist", None) or self.max_ray_length)
-            if np.float32(clearance) > np.float32(d):
-                raise ValueError(f"clearance {clearance} exceeds the ESDF's max_dist {d}: call esdf_update(max_dist) with a "
-                                 "larger max_dist first")
-            self.esdf_update(d)
+        self._travel_clearance(clearance)
         return self._h.travel_update(self._active(), start, clearance, max_cost)
 
     def travel_cost(self, xyz):
         """Travel cost of the cells of points [n,3] as of the last travel_update, +inf where unreachable: a torch CUDA
         tensor for a torch tensor, a numpy array for a numpy array."""
-        self._travel_map()
+        self._logodds_only("a travel cost")
         return self._h.travel_query(xyz, submap=self._active())
 
     def travel_path(self, goal, max_len=4096):
         """The path of the last travel_update from its start to the cell of `goal` [3] as cell centres in metres (f64 of
         cell index * f32(constructor voxel_scale)), [n,3] ordered start to goal, or None when the goal is unreachable."""
-        self._travel_map()
-        if isinstance(goal, self._torch.Tensor):
-            goal = goal.detach().cpu().numpy()
-        g = np.asarray(goal, np.float32).reshape(1, 3)
-        cells, n = self._h.travel_path(g, submap=self._active(), max_len=max_len)
-        n = int(n[0])
-        if n == 0:
-            return None
-        if n > max_len:   # the buffer was too small: once more with the reported length
-            cells, n2 = self._h.travel_path(g, submap=self._active(), max_len=n)
-            assert int(n2[0]) == n
-        vs = float(np.float32(self._h.cfg.voxel_scale))
-        return cells[0, :n][::-1].astype(np.float64) * vs
+        self._logodds_only("a travel cost")
+        return self._travel_path(lambda g, m: self._h.travel_path(g, submap=self._active(), max_len=m), goal, max_len)
 
     def travel_update_multi(self, starts, clearance=0.0, max_cost=None):
         """Travel-cost fields of the active submap from each of S starts [S,3] (metres, map frame; 1 <= S <= 1024) in one
         update, row s exactly what travel_update(starts[s]) computes -> dict(sweeps, traversable, reachable int32[S],
         start_ok bool[S]).  clearance and max_cost as for travel_update (which also runs esdf_update() first)."""
-        self._travel_map()
-        if float(clearance) > 0.0:
-            d = float(getattr(self, "esdf_max_dist", None) or self.max_ray_length)
-            if np.float32(clearance) > np.float32(d):
-                raise ValueError(f"clearance {clearance} exceeds the ESDF's max_dist {d}: call esdf_update(max_dist) with a "
-                                 "larger max_dist first")
-            self.esdf_update(d)
+        self._travel_clearance(clearance)
         return self._h.travel_multi_update(self._active(), starts, clearance, max_cost)
 
     def travel_cost_multi(self, xyz):
         """Travel costs [S,n] of the cells of points [n,3] from each start of the last travel_update_multi, +inf where
         unreachable; travel_cost_multi(starts) is the S x S matrix (not symmetrised: entry [s,t] and [t,s] may differ in
         the last bits).  A torch CUDA tensor for a torch tensor, a numpy array for a numpy array."""
-        self._travel_map()
+        self._logodds_only("a travel cost")
         return self._h.travel_multi_query(xyz, submap=self._active())
 
     def travel_path_multi(self, source, goal, max_len=4096):
         """The path from start `source` of the last travel_update_multi to the cell of `goal` [3] as cell centres in
         metres, [n,3] ordered start to goal, or None when the goal is unreachable from that start."""
-        self._travel_map()
-        if isinstance(goal, self._torch.Tensor):
-            goal = goal.detach().cpu().numpy()
-        g = np.asarray(goal, np.float32).reshape(1, 3)
+        self._logodds_only("a travel cost")
         S = getattr(self._h, "_travel_multi_S", 0)
         if not 0 <= int(source) < S:
             raise ValueError(f"source {source} is not a start of the last travel_update_multi ({S} starts)")
         src = np.array([int(source)], np.int32)
-        cells, n = self._h.travel_multi_path(src, g, submap=self._active(), max_len=max_len)
-        n = int(n[0])
-        if n == 0:
-            return None
-        if n > max_len:   # the buffer was too small: once more with the reported length
-            cells, n2 = self._h.travel_multi_path(src, g, submap=self._active(), max_len=n)
-            assert int(n2[0]) == n
-        vs = float(np.float32(self._h.cfg.voxel_scale))
-        return cells[0, :n][::-1].astype(np.float64) * vs
+        return self._travel_path(lambda g, m: self._h.travel_multi_path(src, g, submap=self._active(), max_len=m), goal, max_len)
 
     def saveMap(self, path):  # :201-202 (stub in the reference)
         pass

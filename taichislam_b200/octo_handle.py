@@ -104,39 +104,53 @@ class OctoHandle:
         if mem == capi.MEM_HOST:
             torch.cuda.current_stream().synchronize()
 
-    def gather_device(self, submap=0, cap=None, color=False):
+    def _count_fill(self, call, *alloc, cap=None):
+        """The two-call protocol of a count-then-fill reader.  call(cap, n_ref, *ptrs) makes the C call; a probe with
+        cap 0 and NULL buffers gives the count n (unless cap is given).  Without alloc that count is the result; else
+        each (trailing shape, torch dtype) of alloc becomes a device tensor [max(n, 1), *shape], the second call fills
+        them, and they come back sliced to the rows written."""
         torch = self.torch
-        dev = torch.device("cuda", torch.cuda.current_device())
         n = C.c_int64(0)
         if cap is None:
-            rc = self.L.tslam_octo_gather(self.h, int(submap), 0, None, None, C.byref(n), capi.stream_ptr())
+            rc = call(0, C.byref(n), *(None for _ in alloc))
             if rc not in (capi.TSLAM_OK, capi.E_CAPACITY):
                 capi.check(rc)
             cap = int(n.value)
-        idx = torch.empty((max(cap, 1), 3), dtype=torch.int32, device=dev)
-        cnt = torch.empty(max(cap, 1), dtype=torch.int32, device=dev)
-        col = torch.empty((max(cap, 1), 3), dtype=torch.float32, device=dev) if color else None
-        capi.check(self.L.tslam_octo_gather2(self.h, int(submap), cap, capi.tptr(idx), capi.tptr(cnt),
-                                             capi.tptr(col) if color else None, C.byref(n), capi.stream_ptr()))
+            if not alloc:
+                return cap
+        dev = torch.device("cuda", torch.cuda.current_device())
+        out = [torch.empty((max(cap, 1),) + tuple(shape), dtype=dt, device=dev) for shape, dt in alloc]
+        capi.check(call(cap, C.byref(n), *(capi.tptr(t) for t in out)))
         k = int(n.value)
-        return (idx[:k], cnt[:k], col[:k]) if color else (idx[:k], cnt[:k])
+        return tuple(t[:k] for t in out)
+
+    def _input(self, a, shape, dtype="float32"):
+        """a as a contiguous CUDA tensor of `dtype` and `shape`: a torch tensor is converted on the device (no host
+        synchronisation), anything else through numpy"""
+        torch = self.torch
+        dev = torch.device("cuda", torch.cuda.current_device())
+        if isinstance(a, torch.Tensor):
+            return a.to(device=dev, dtype=getattr(torch, dtype)).reshape(shape).contiguous()
+        return torch.from_numpy(np.ascontiguousarray(np.asarray(a, dtype).reshape(shape))).to(dev)
+
+    @staticmethod
+    def _out(as_torch, *tensors):
+        """torch in -> the CUDA tensors, numpy in -> numpy arrays (one value for one tensor, else a tuple)"""
+        r = tensors if as_torch else tuple(t.cpu().numpy() for t in tensors)
+        return r if len(r) > 1 else r[0]
+
+    def gather_device(self, submap=0, cap=None, color=False):
+        torch = self.torch
+        alloc = [((3,), torch.int32), ((), torch.int32)] + ([((3,), torch.float32)] if color else [])
+        return self._count_fill(lambda cap, n, idx, cnt, col=None: self.L.tslam_octo_gather2(
+            self.h, int(submap), cap, idx, cnt, col, n, capi.stream_ptr()), *alloc, cap=cap)
 
     def gather_logodds_device(self, submap=0, color=False):
         """(idx int32[n,3], L int32[n][, color f32[n,3]]) of the known voxels of a log-odds map, on the device."""
         torch = self.torch
-        dev = torch.device("cuda", torch.cuda.current_device())
-        n = C.c_int64(0)
-        rc = self.L.tslam_octo_gather_logodds(self.h, int(submap), 0, None, None, None, C.byref(n), capi.stream_ptr())
-        if rc not in (capi.TSLAM_OK, capi.E_CAPACITY):
-            capi.check(rc)
-        cap = int(n.value)
-        idx = torch.empty((max(cap, 1), 3), dtype=torch.int32, device=dev)
-        lo = torch.empty(max(cap, 1), dtype=torch.int32, device=dev)
-        col = torch.empty((max(cap, 1), 3), dtype=torch.float32, device=dev) if color else None
-        capi.check(self.L.tslam_octo_gather_logodds(self.h, int(submap), cap, capi.tptr(idx), capi.tptr(lo), capi.tptr(col), C.byref(n),
-                                                    capi.stream_ptr()))
-        k = int(n.value)
-        return (idx[:k], lo[:k], col[:k]) if color else (idx[:k], lo[:k])
+        alloc = [((3,), torch.int32), ((), torch.int32)] + ([((3,), torch.float32)] if color else [])
+        return self._count_fill(lambda cap, n, idx, lo, col=None: self.L.tslam_octo_gather_logodds(
+            self.h, int(submap), cap, idx, lo, col, n, capi.stream_ptr()), *alloc)
 
     def gather(self, submap=0, color=False):
         """Hit counter: (idx, count uint32[, color]).  Log-odds map: (idx, L int32[, color]) of the known voxels."""
@@ -207,42 +221,22 @@ class OctoHandle:
         """(idx int32[n,3], ESDF f32[n]) of the voxels known at the last esdf_update: numpy arrays, or torch CUDA tensors
         with as_torch."""
         torch = self.torch
-        dev = torch.device("cuda", torch.cuda.current_device())
-        n = C.c_int64(0)
-        rc = self.L.tslam_octo_esdf_gather(self.h, int(submap), 0, None, None, C.byref(n), capi.stream_ptr())
-        if rc not in (capi.TSLAM_OK, capi.E_CAPACITY):
-            capi.check(rc)
-        cap = int(n.value)
-        idx = torch.empty((max(cap, 1), 3), dtype=torch.int32, device=dev)
-        e = torch.empty(max(cap, 1), dtype=torch.float32, device=dev)
-        capi.check(self.L.tslam_octo_esdf_gather(self.h, int(submap), cap, capi.tptr(idx), capi.tptr(e), C.byref(n),
-                                                 capi.stream_ptr()))
-        k = int(n.value)
-        if as_torch:
-            return idx[:k], e[:k]
-        return idx[:k].cpu().numpy(), e[:k].cpu().numpy()
+        return self._out(as_torch, *self._count_fill(lambda cap, n, idx, e: self.L.tslam_octo_esdf_gather(
+            self.h, int(submap), cap, idx, e, n, capi.stream_ptr()), ((3,), torch.int32), ((), torch.float32)))
 
     def esdf_query(self, xyz, submap=0):
         """Trilinear ESDF and its exact gradient at points [n,3] of the submap's map frame, as of the last esdf_update:
         (dist f32[n], grad f32[n,3], valid bool[n]); dist and grad are NaN where valid is False.  A torch CUDA tensor in
         -> torch CUDA tensors out, without a host synchronisation; a numpy array in -> numpy arrays out."""
         torch = self.torch
-        as_torch = isinstance(xyz, torch.Tensor)
-        if as_torch:
-            x = xyz.to(device=torch.device("cuda", torch.cuda.current_device()), dtype=torch.float32).contiguous()
-        else:
-            x = torch.from_numpy(np.ascontiguousarray(xyz, dtype=np.float32)).cuda()
-        x = x.reshape(-1, 3)
+        x = self._input(xyz, (-1, 3))
         n = x.shape[0]
         dist = torch.empty(n, dtype=torch.float32, device=x.device)
         grad = torch.empty((n, 3), dtype=torch.float32, device=x.device)
         valid = torch.empty(n, dtype=torch.uint8, device=x.device)
         capi.check(self.L.tslam_octo_esdf_query(self.h, int(submap), n, capi.tptr(x), capi.tptr(dist), capi.tptr(grad),
                                                 capi.tptr(valid), capi.stream_ptr()))
-        valid = valid.view(torch.bool)  # the kernel writes 0 / 1
-        if as_torch:
-            return dist, grad, valid
-        return dist.cpu().numpy(), grad.cpu().numpy(), valid.cpu().numpy()
+        return self._out(isinstance(xyz, torch.Tensor), dist, grad, valid.view(torch.bool))  # the kernel writes 0 / 1
 
     # -- frontiers of a log-odds map (tslam_octo_frontier_*, DESIGN.md section 7) --------------------------------------
     def frontier_update(self, submap=0, full=False):
@@ -256,35 +250,16 @@ class OctoHandle:
         """(idx int32[n,3], cluster int32[n]) of the frontier voxels of the last frontier_update; cluster is the ordinal in
         frontier_clusters.  numpy arrays, or torch CUDA tensors with as_torch."""
         torch = self.torch
-        dev = torch.device("cuda", torch.cuda.current_device())
-        n = C.c_int64(0)
-        rc = self.L.tslam_octo_frontier_gather(self.h, int(submap), 0, None, None, C.byref(n), capi.stream_ptr())
-        if rc not in (capi.TSLAM_OK, capi.E_CAPACITY):
-            capi.check(rc)
-        cap = int(n.value)
-        idx = torch.empty((max(cap, 1), 3), dtype=torch.int32, device=dev)
-        cl = torch.empty(max(cap, 1), dtype=torch.int32, device=dev)
-        capi.check(self.L.tslam_octo_frontier_gather(self.h, int(submap), cap, capi.tptr(idx), capi.tptr(cl), C.byref(n),
-                                                     capi.stream_ptr()))
-        k = int(n.value)
-        if as_torch:
-            return idx[:k], cl[:k]
-        return idx[:k].cpu().numpy(), cl[:k].cpu().numpy()
+        return self._out(as_torch, *self._count_fill(lambda cap, n, idx, cl: self.L.tslam_octo_frontier_gather(
+            self.h, int(submap), cap, idx, cl, n, capi.stream_ptr()), ((3,), torch.int32), ((), torch.int32)))
 
     def frontier_clusters(self, submap=0, as_torch=False):
         """int64[n,16] cluster records of the last frontier_update in label order (label, voxels, sum i / j / k, min i / j
         / k, max i / j / k, faces, sum of the unit offsets towards UNKNOWN x / y / z, 0)."""
-        torch = self.torch
-        dev = torch.device("cuda", torch.cuda.current_device())
-        n = C.c_int64(0)
-        rc = self.L.tslam_octo_frontier_clusters(self.h, int(submap), 0, None, C.byref(n), capi.stream_ptr())
-        if rc not in (capi.TSLAM_OK, capi.E_CAPACITY):
-            capi.check(rc)
-        cap = int(n.value)
-        rec = torch.empty((max(cap, 1), 16), dtype=torch.int64, device=dev)
-        capi.check(self.L.tslam_octo_frontier_clusters(self.h, int(submap), cap, capi.tptr(rec), C.byref(n), capi.stream_ptr()))
-        k = int(n.value)
-        return rec[:k] if as_torch else rec[:k].cpu().numpy()
+        return self._out(as_torch, *self._count_fill(self._clusters_call(submap), ((16,), self.torch.int64)))
+
+    def _clusters_call(self, submap):
+        return lambda cap, n, rec=None: self.L.tslam_octo_frontier_clusters(self.h, int(submap), cap, rec, n, capi.stream_ptr())
 
     # -- viewpoint gain of a log-odds map (tslam_octo_view_gain_*, DESIGN.md section 7) ------------------------------
     @staticmethod
@@ -295,17 +270,9 @@ class OctoHandle:
 
     def _views(self, pos, R):
         """(as_torch, pos f32 [n,3], R f32 [n,9]) as contiguous CUDA tensors"""
-        torch = self.torch
-        as_torch = isinstance(pos, torch.Tensor)
-        dev = torch.device("cuda", torch.cuda.current_device())
-        if as_torch:
-            p = pos.to(device=dev, dtype=torch.float32).reshape(-1, 3).contiguous()
-            r = R.to(device=dev, dtype=torch.float32).reshape(-1, 9).contiguous()
-        else:
-            p = torch.from_numpy(np.ascontiguousarray(np.asarray(pos, np.float32).reshape(-1, 3))).to(dev)
-            r = torch.from_numpy(np.ascontiguousarray(np.asarray(R, np.float32).reshape(-1, 9))).to(dev)
+        p, r = self._input(pos, (-1, 3)), self._input(R, (-1, 9))
         assert p.shape[0] == r.shape[0], "pos [n,3] and R [n,3,3] need the same n"
-        return as_torch, p, r
+        return isinstance(pos, self.torch.Tensor), p, r
 
     def view_gain_unknown(self, pos, R, cam, submap=0):
         """Unknown gain of n views (positions pos [n,3], rotations R [n,3,3], camera `cam` as in view_camera) -> (valid
@@ -320,11 +287,9 @@ class OctoHandle:
         c = self.view_camera(cam)
         capi.check(self.L.tslam_octo_view_gain_unknown(self.h, int(submap), n, capi.tptr(p), capi.tptr(r), C.byref(c), capi.tptr(valid),
                                                        capi.tptr(gain), capi.stream_ptr()))
-        valid = valid.view(torch.bool)
-        if as_torch:
-            return valid, gain
-        self.sync()
-        return valid.cpu().numpy(), gain.cpu().numpy()
+        if not as_torch:
+            self.sync()
+        return self._out(as_torch, valid.view(torch.bool), gain)
 
     def view_gain_frontier(self, pos, R, cam, submap=0):
         """Frontier gain of n views against the frontier set of the last frontier_update -> (valid bool[n], total int32[n],
@@ -333,11 +298,7 @@ class OctoHandle:
         torch = self.torch
         as_torch, p, r = self._views(pos, R)
         n = p.shape[0]
-        nc = C.c_int64(0)
-        rc = self.L.tslam_octo_frontier_clusters(self.h, int(submap), 0, None, C.byref(nc), capi.stream_ptr())
-        if rc not in (capi.TSLAM_OK, capi.E_CAPACITY):
-            capi.check(rc)
-        nc = int(nc.value)
+        nc = self._count_fill(self._clusters_call(submap))
         valid = torch.empty(n, dtype=torch.uint8, device=p.device)
         total = torch.empty(n, dtype=torch.int32, device=p.device)
         per = torch.empty((n, nc), dtype=torch.int32, device=p.device)
@@ -345,10 +306,7 @@ class OctoHandle:
         capi.check(self.L.tslam_octo_view_gain_frontier(self.h, int(submap), n, capi.tptr(p), capi.tptr(r), C.byref(c), nc,
                                                         capi.tptr(valid), capi.tptr(total), capi.tptr(per) if nc else None,
                                                         capi.stream_ptr()))
-        valid = valid.view(torch.bool)
-        if as_torch:
-            return valid, total, per
-        return valid.cpu().numpy(), total.cpu().numpy(), per.cpu().numpy()
+        return self._out(as_torch, valid.view(torch.bool), total, per)
 
     # -- travel cost on a log-odds map (tslam_octo_travel_*, DESIGN.md section 7) --------------------------------------
     def travel_limit(self):
@@ -370,55 +328,33 @@ class OctoHandle:
         """(idx int32[n,3], cost f32[n]) of the cells reachable at the last travel_update: numpy arrays, or torch CUDA
         tensors with as_torch."""
         torch = self.torch
-        dev = torch.device("cuda", torch.cuda.current_device())
-        n = C.c_int64(0)
-        rc = self.L.tslam_octo_travel_gather(self.h, int(submap), 0, None, None, C.byref(n), capi.stream_ptr())
-        if rc not in (capi.TSLAM_OK, capi.E_CAPACITY):
-            capi.check(rc)
-        cap = int(n.value)
-        idx = torch.empty((max(cap, 1), 3), dtype=torch.int32, device=dev)
-        g = torch.empty(max(cap, 1), dtype=torch.float32, device=dev)
-        capi.check(self.L.tslam_octo_travel_gather(self.h, int(submap), cap, capi.tptr(idx), capi.tptr(g), C.byref(n), capi.stream_ptr()))
-        k = int(n.value)
-        if as_torch:
-            return idx[:k], g[:k]
-        return idx[:k].cpu().numpy(), g[:k].cpu().numpy()
-
-    def _points(self, xyz):
-        """(as_torch, contiguous f32 [n,3] CUDA tensor)"""
-        torch = self.torch
-        as_torch = isinstance(xyz, torch.Tensor)
-        if as_torch:
-            x = xyz.to(device=torch.device("cuda", torch.cuda.current_device()), dtype=torch.float32).contiguous()
-        else:
-            x = torch.from_numpy(np.ascontiguousarray(xyz, dtype=np.float32)).cuda()
-        return as_torch, x.reshape(-1, 3)
+        return self._out(as_torch, *self._count_fill(lambda cap, n, idx, g: self.L.tslam_octo_travel_gather(
+            self.h, int(submap), cap, idx, g, n, capi.stream_ptr()), ((3,), torch.int32), ((), torch.float32)))
 
     def travel_query(self, xyz, submap=0):
         """Travel cost f32[n] of the cells of points [n,3] as of the last travel_update (+inf where unreachable).  A torch
         CUDA tensor in -> a torch CUDA tensor out, without a host synchronisation; a numpy array in -> a numpy array out."""
         torch = self.torch
-        as_torch, x = self._points(xyz)
+        x = self._input(xyz, (-1, 3))
         n = x.shape[0]
         cost = torch.empty(n, dtype=torch.float32, device=x.device)
         capi.check(self.L.tslam_octo_travel_query(self.h, int(submap), n, capi.tptr(x), capi.tptr(cost), capi.stream_ptr()))
-        return cost if as_torch else cost.cpu().numpy()
+        return self._out(isinstance(xyz, torch.Tensor), cost)
 
     def travel_path(self, xyz, submap=0, max_len=4096):
         """Paths from the cells of targets [n,3] back to the start of the last travel_update -> (cells int32[n,max_len,3]
         target -> start, len int32[n]: the full cell count, 0 when unreachable; rows beyond min(len, max_len) are
         undefined).  Torch in -> torch out without a host synchronisation; numpy in -> numpy out."""
         torch = self.torch
-        as_torch, x = self._points(xyz)
+        as_torch, x = isinstance(xyz, torch.Tensor), self._input(xyz, (-1, 3))
         n = x.shape[0]
         cells = torch.empty((n, int(max_len), 3), dtype=torch.int32, device=x.device)
         ln = torch.empty(n, dtype=torch.int32, device=x.device)
         capi.check(self.L.tslam_octo_travel_path(self.h, int(submap), n, capi.tptr(x), int(max_len), capi.tptr(cells), capi.tptr(ln),
                                                  capi.stream_ptr()))
-        if as_torch:
-            return cells, ln
-        self.sync()
-        return cells.cpu().numpy(), ln.cpu().numpy()
+        if not as_torch:
+            self.sync()
+        return self._out(as_torch, cells, ln)
 
     def travel_multi_update(self, submap, starts, clearance=0.0, max_cost=None):
         """Travel-cost fields of `submap` from each of S starts [S,3] (metres, submap frame; 1 <= S <= 1024) in one update,
@@ -440,11 +376,11 @@ class OctoHandle:
         unreachable); the starts themselves give the S x S matrix.  Torch in -> torch out without a host
         synchronisation; numpy in -> numpy out."""
         torch = self.torch
-        as_torch, x = self._points(xyz)
+        x = self._input(xyz, (-1, 3))
         n = x.shape[0]
         cost = torch.empty((getattr(self, "_travel_multi_S", 0), n), dtype=torch.float32, device=x.device)
         capi.check(self.L.tslam_octo_travel_multi_query(self.h, int(submap), n, capi.tptr(x), capi.tptr(cost), capi.stream_ptr()))
-        return cost if as_torch else cost.cpu().numpy()
+        return self._out(isinstance(xyz, torch.Tensor), cost)
 
     def travel_multi_path(self, source, xyz, submap=0, max_len=4096):
         """Paths of pairs (source[q], xyz[q]) from the cell of the target back to starts[source[q]] of the last
@@ -452,20 +388,14 @@ class OctoHandle:
         [0, S) gets len 0 and the next sync() raises.  Torch in -> torch out without a host synchronisation; numpy in ->
         numpy out."""
         torch = self.torch
-        as_torch, x = self._points(xyz)
+        x, src = self._input(xyz, (-1, 3)), self._input(source, (-1,), "int32")
         n = x.shape[0]
-        if isinstance(source, torch.Tensor):
-            src = source.to(device=x.device, dtype=torch.int32).reshape(-1).contiguous()
-        else:
-            src = torch.from_numpy(np.ascontiguousarray(np.asarray(source, np.int32).reshape(-1))).to(x.device)
         assert src.shape[0] == n, "source [n] and xyz [n,3] need the same n"
         cells = torch.empty((n, int(max_len), 3), dtype=torch.int32, device=x.device)
         ln = torch.empty(n, dtype=torch.int32, device=x.device)
         capi.check(self.L.tslam_octo_travel_multi_path(self.h, int(submap), n, capi.tptr(src), capi.tptr(x), int(max_len), capi.tptr(cells),
                                                        capi.tptr(ln), capi.stream_ptr()))
-        if as_torch:
-            return cells, ln
-        return cells.cpu().numpy(), ln.cpu().numpy()
+        return self._out(isinstance(xyz, torch.Tensor), cells, ln)
 
     def raycast(self, pos, direction, max_dist, submap=0):
         torch = self.torch

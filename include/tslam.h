@@ -196,6 +196,9 @@ int tslam_tsdf_kernel_ms2(tslam_tsdf_t* m, int32_t n, float* ms7, int32_t* n_out
  * item's block, samples of the generic path, fast-path indices that disagreed with the exact index
  * (TSLAM_MARCH_VERIFY=1 only; must be 0).  Synchronises. */
 int tslam_tsdf_get_march_stats(tslam_tsdf_t* m, int64_t* out6);
+/* The same six, then out7[6] = segments the counting and the scattering walk of the binned march disagreed about:
+ * routed to the generic path by a guard of the scattering walk, or counted but never placed.  Must be 0. */
+int tslam_tsdf_get_march_stats2(tslam_tsdf_t* m, int64_t* out7);
 
 /* ----------------------------------------------------------------------------
  * Map queries for planners - batched forms of the @ti.func helpers of BaseMap (mapping_common.py:165-204) that

@@ -97,6 +97,7 @@ SIGNATURES = {
     "tslam_tsdf_kernel_ms": (C.c_int, [_vp, _i32, _vp, C.POINTER(_i32)]),
     "tslam_tsdf_kernel_ms2": (C.c_int, [_vp, _i32, _vp, C.POINTER(_i32)]),
     "tslam_tsdf_get_march_stats": (C.c_int, [_vp, _vp]),
+    "tslam_tsdf_get_march_stats2": (C.c_int, [_vp, _vp]),
     "tslam_tsdf_query_points": (C.c_int, [_vp, _i32, _i64, _vp, _vp, _vp]),
     "tslam_tsdf_query_near_occupy": (C.c_int, [_vp, _i32, _i64, _vp, _i32, _vp, _vp]),
     "tslam_tsdf_raycast": (C.c_int, [_vp, _i32, _i64, _vp, _vp, _f32, _vp, _vp, _vp, _vp]),

@@ -281,6 +281,26 @@ __device__ __forceinline__ int rm_lookup(const TsGrid& g, unsigned long long* ta
   }
   return blk;
 }
+// read-only form for a kernel that runs after an earlier kernel activated the blocks (the table does not change while
+// it runs): pool index, -1 when the block is not in the grid, -2 when its activation failed (pool exhausted).
+__device__ __forceinline__ int rm_find(const TsGrid& g, unsigned long long* tab, unsigned long long key, int bx, int by, int bz) {
+  const int h = ((bx & 15) << 8) | ((by & 15) << 4) | (bz & 15);
+  const unsigned long long w = tab[h];
+  if ((w >> 24) == key) return (int)(w & TS_IDX_MASK);
+  uint32_t slot = ts_hash(key) & g.table_mask;
+  for (uint32_t probe = 0; probe <= g.table_mask; ++probe) {
+    const unsigned long long cur = g.table[slot];
+    if (cur == TS_EMPTY) return -1;
+    if ((cur >> 24) == key) {
+      const unsigned idx = (unsigned)(cur & TS_IDX_MASK);
+      if (idx >= TS_IDX_OVERFLOW) return -2;
+      tab[h] = cur;
+      return (int)idx;
+    }
+    slot = (slot + 1) & g.table_mask;
+  }
+  return -1;
+}
 
 
 // ---------------------------------------------------------------------------
@@ -326,6 +346,8 @@ struct TsCounters {  // device-side statistics (tslam_tsdf_get_stats)
   unsigned long long n_px, n_valid, n_rays, n_updates, n_oob;
   // block-binned ray march (tslam_march.cu): diagnostics, not part of the parity counters
   unsigned long long n_segs, n_items, n_slow, n_fallback, n_generic, n_verify_bad;
+  // segments the two walks of the binned march disagreed about (k_seg_scatter, k_march_reset): must stay 0
+  unsigned long long n_seg_guard;
 };
 
 // ---------------------------------------------------------------------------
@@ -352,13 +374,12 @@ struct TsMarchCtl {  // device-side control block of one launch (zeroed by k_mar
   int n_full;        // (unused since the items are listed longest first)
   int item_cursor;   // persistent-CTA work cursor of k_march_blocks
   int n_gen;         // generic-list records
-  int overflow;      // work list did not fit: every segment goes through the generic path this launch
+  int overflow;      // segments or work items did not fit: every segment goes through the generic path this launch
   unsigned int total_segs;
   unsigned int fmax_bits;  // float bits of max over rays of max(w, w*|ds|max): sizes the fixed-point scale of the launch
   int scale_k;       // shared-memory sums are kept in units of 2^-scale_k (k_seg_scan: largest k with max * 2^k < 2^30)
   int ticket;
-  unsigned int tmp_cursor;  // next free entry of the segment-list pool
-  int pad0, pad1;
+  int pad0, pad1, pad2;
   int pad[3];
 };
 struct TsMarchWs {
@@ -366,10 +387,9 @@ struct TsMarchWs {
   uint32_t* aux;       // [ray_list_cap]
   TsSeg* seg;          // [seg_cap] segments grouped by block, ordered by length inside a block
   uint32_t seg_cap;
-  TsSeg* tmp_seg;      // [seg_cap] per-CTA segment lists of k_seg_walk (chunks of 4096 entries from one pool)
-  uint32_t* tmp_key;   // [seg_cap] block * 16 + length class of the listed segment
-  int* seg_count;      // [max_blocks * 16] segments per (block, class); then the fill cursor of k_seg_place
-  uint32_t* seg_rel;   // [max_blocks * 16] start of the class inside the block's run
+  int* seg_count;      // [max_blocks * 64] segments per (block, class, replica) (k_seg_count); k_seg_scatter counts
+                       // each back down to 0 as it fills the run
+  uint32_t* seg_rel;   // [max_blocks * 64] end of the (class, replica) range inside the block's run
   uint32_t* seg_off;   // [max_blocks] start of the block's run
   int* touched;        // [max_blocks] blocks with segments
   uint32_t* blk_total; // [max_blocks] segments of touched[i]
@@ -379,9 +399,6 @@ struct TsMarchWs {
   TsSeg* gen;          // [gen_cap] generic-path records (volume boundary, over-long rays, overflow)
   uint32_t gen_cap;
   TsMarchCtl* ctl;
-  int* cta_n;          // [walk CTAs] segments in the CTA's list
-  uint32_t* cta_chunk; // [walk CTAs * 1024] first entry of the CTA's k-th list chunk
-  int walk_x_max;      // walk CTAs of a one-frame launch
   float near_eps;      // |frac - 0.5| below this -> exact index path
 };
 

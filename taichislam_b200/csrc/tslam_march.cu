@@ -4,15 +4,16 @@
 // L2 reduction rate whatever the kernel did) for untextured maps.  process_new_pcl
 // (dense_tsdf.py:236-270) becomes
 //
-//   k_ray_setup    one thread per ray (= bucket, read sequentially from the dense per-ray array): exact bucket mean
-//                  -> unit direction, length, weight, step count n (:240-251), occupy flag (:248), a 32-byte record;
-//   k_seg_walk     one lane per ray: a 3-D DDA cuts the ray into SEGMENTS - runs of consecutive steps that stay in
-//                  one 16^3 voxel block - activates the blocks on the way, appends the segments to per-CTA lists and
-//                  counts them per (block, length class) with warp-aggregated reductions;
+//   k_seg_count    one lane per ray.  Ray set-up (one bucket, read sequentially from the dense per-ray array): exact
+//                  bucket mean -> unit direction, length, weight, step count n (:240-251), occupy flag (:248), a
+//                  32-byte record.  Then a 3-D DDA (seg_generate) cuts the ray into SEGMENTS - runs of consecutive
+//                  steps that stay in one 16^3 voxel block - activates the blocks on the way and counts the segments
+//                  per (block, length class) with warp-aggregated reductions.  It stores no segment;
 //   k_seg_class    per touched block: class counts -> offsets inside the block's run, list of touched blocks;
 //   k_seg_scan     exclusive scan over the touched blocks -> run offsets + work items (<= MR_CHUNK segments of one
 //                  block each, full chunks first);
-//   k_seg_place    moves every listed segment to its place: a block's run is ordered by segment length;
+//   k_seg_scatter  walks every ray again from its stored record (the same seg_generate, so the same segments in the
+//                  same order) and stores each segment at its place: a block's run is ordered by segment length;
 //   k_march_blocks persistent CTAs take work items.  The block's pending sums live in SHARED MEMORY as exact 64-bit
 //                  fixed-point words (no-return ATOMS.ADD: an order of magnitude more lane-atomics/s than
 //                  global reductions, tools/ubench/atoms_bench.cu).  A warp walks 32 segments of equal length
@@ -44,19 +45,20 @@
                                                 // is applied with f32 global reductions instead
 #define MB_SMEM (4 * MB_WORDS * 4)
 #define SEG_CLS 16                               // length classes per block: (count - 1) >> 1
-#define SEG_REP 4                                // counter replicas per (block, class), picked by the walk CTA: the hot
-                                                // blocks' counters would otherwise serialise in one L2 slice
+#define SEG_REP 4                                // counter replicas per (block, class), picked by the ray's group of 256
+                                                // (seg_key): the hot blocks' counters would otherwise serialise in
+                                                // one L2 slice
 #define SEG_KEYS (SEG_CLS * SEG_REP)
 
 // ---------------------------------------------------------------------------
-// K2a: ray set-up (process_new_pcl :240-251), first stage of the walk kernel: one bucket record -> unit direction,
-// length, weight, step count n, occupy flag (:248) and the 32-byte ray record the march kernels read.  The record and
-// its index entry are handed back zeroed (PCLroot.deactivate_all() / new_pcl_count = 0, :163, :270).
+// K2a: ray set-up (process_new_pcl :240-251), first stage of the counting walk: one bucket record -> unit direction,
+// length, weight, step count n, occupy flag (:248) and the 32-byte ray record + aux word the march kernels read,
+// stored at rays[r] / aux[r] and handed back in ra, rb, raux.  The bucket record and its index entry are handed back
+// zeroed (PCLroot.deactivate_all() / new_pcl_count = 0, :163, :270).
 // ---------------------------------------------------------------------------
-struct RaySetup { float ux, uy, uz, tx, ty, tz; int n, s; uint32_t f; bool wide; };
-__device__ __forceinline__ RaySetup ray_setup(const TsBatch& batch, const TsIntrin& in, const TsGrid& g, unsigned long long* btab, TsBucket* buckets,
-                                              unsigned long long* bidx, uint32_t bucket_shift, uint32_t id, uint32_t r, const TsMarchWs& w,
-                                              unsigned int& my_rays, unsigned int& my_fmax) {
+__device__ __forceinline__ void ray_setup(const TsBatch& batch, const TsIntrin& in, const TsGrid& g, unsigned long long* btab, TsBucket* buckets,
+                                          unsigned long long* bidx, uint32_t bucket_shift, uint32_t id, uint32_t r, const TsMarchWs& w,
+                                          unsigned int& my_rays, unsigned int& my_fmax, float4& ra, float4& rb, uint32_t& raux) {
   const float vs = in.vs;
   const uint32_t f = id >> bucket_shift;
   uint4* q = reinterpret_cast<uint4*>(&buckets[id]);  // key sx | sy sz | sd cnt cr | cg cb pad
@@ -71,9 +73,9 @@ __device__ __forceinline__ RaySetup ray_setup(const TsBatch& batch, const TsIntr
   const long long sd = (long long)((unsigned long long)q2.x | ((unsigned long long)q2.y << 32));
   const int cnt = (int)q2.z;
   const TsFrame& fr = batch.f[f];
-  RaySetup o;
+  struct { float ux, uy, uz, tx, ty, tz; int n, s; bool wide; } o;
   o.ux = o.uy = o.uz = o.tx = o.ty = o.tz = 0.0f;
-  o.n = 0; o.s = fr.submap; o.f = f; o.wide = false;
+  o.n = 0; o.s = fr.submap; o.wide = false;
   float L = 0.0f, wgt = 0.0f;
   if (cnt > 0) {  // :240
     my_rays++;
@@ -107,18 +109,21 @@ __device__ __forceinline__ RaySetup ray_setup(const TsBatch& batch, const TsIntr
       L = 0.0f;
     }
   }
+  ra = make_float4(o.ux, o.uy, o.uz, L);
+  rb = make_float4(o.tx, o.ty, o.tz, wgt);
+  raux = ((uint32_t)max(0, min(o.n, 65535)) << 16) | (f << 8) | (o.wide ? TS_AUX_WIDE : 0u);
   float4* dst = reinterpret_cast<float4*>(&w.rays[r]);
-  dst[0] = make_float4(o.ux, o.uy, o.uz, L);
-  dst[1] = make_float4(o.tx, o.ty, o.tz, wgt);
-  o.n = max(0, min(o.n, 65535));
-  w.aux[r] = ((uint32_t)o.n << 16) | (f << 8) | (o.wide ? TS_AUX_WIDE : 0u);
-  return o;
+  dst[0] = ra;
+  dst[1] = rb;
+  w.aux[r] = raux;
 }
 
 // ---------------------------------------------------------------------------
-// K2b: segment walk: 3-D DDA over the 16^3 blocks in voxel-index space, one lane per ray, warp-uniform loop (one
+// K2b: segment walks: 3-D DDA over the 16^3 blocks in voxel-index space, one lane per ray, warp-uniform loop (one
 // block crossing per lane and iteration).  Segments are HINTS - every sample is re-checked exactly by the march
-// kernel - so the crossing parameters may be off by one step.
+// kernel - so the crossing parameters may be off by one step.  The DDA runs twice per launch, in k_seg_count (count
+// the segments per block and length class) and k_seg_scatter (store them in the runs k_seg_scan laid out): recomputing
+// a segment costs a few FMAs per block crossing, storing it in a list and reading it back 24 bytes of traffic.
 // ---------------------------------------------------------------------------
 // 0 = far outside the volume (every sample is out of bounds), 1 = block inside the block range, 2 = outside but
 // adjacent to it (a rounding-boundary sample may still be in bounds: exact path)
@@ -141,116 +146,111 @@ __device__ __forceinline__ void dda_axis(float u, float t, int& b, float& jc, fl
   else { jc = 3.0e38f; dj = 0.0f; sg = 0; }
 }
 
-#define WK_CHUNK 4096   // entries per chunk of the per-CTA segment lists
-#define WK_MAXCH 1024   // chunks per CTA
-struct WalkSmem {
-  unsigned long long btab[RM_TAB];  // block coordinates -> pool index (direct mapped, rm_lookup)
-  uint32_t chunk[WK_MAXCH];         // first entry of the CTA's k-th chunk in tmp_seg / tmp_key
-  int n_chunk, cur, ovf, pad;
-};
+// A ray as both walks see it, decoded from its stored record (rays[r], aux[r]) - never from the set-up's registers -
+// so that the two walks start from the same bits.  An all-zero record is a ray with n = 0.
+struct SegRay { float ux, uy, uz, tx, ty, tz; int n, s; uint32_t f; bool wide; };
+__device__ __forceinline__ SegRay seg_ray(const TsBatch& batch, float4 a, float4 b, uint32_t aux) {
+  SegRay q;
+  q.ux = a.x; q.uy = a.y; q.uz = a.z;
+  q.tx = b.x; q.ty = b.y; q.tz = b.z;
+  q.n = (int)(aux >> 16);
+  q.f = (aux >> 8) & 255u;
+  q.s = batch.f[q.f].submap;
+  q.wide = (aux & TS_AUX_WIDE) != 0u;
+  return q;
+}
 
-__global__ void __launch_bounds__(MS_THREADS, 3) k_seg_walk(const __grid_constant__ TsBatch batch, TsIntrin in, TsGrid g, TsBucket* buckets,
-                                                             unsigned long long* bidx, uint32_t bucket_shift, const uint32_t* __restrict__ ray_list,
-                                                             const int* __restrict__ n_rays_p, uint32_t ray_cap, TsMarchWs w, TsCounters* ctr) {
-  extern __shared__ __align__(16) unsigned char ms_smem[];
-  WalkSmem& S = *reinterpret_cast<WalkSmem*>(ms_smem);
-  for (int e = threadIdx.x; e < RM_TAB; e += MS_THREADS) S.btab[e] = TS_EMPTY;
-  if (threadIdx.x == 0) { S.n_chunk = 0; S.cur = 0; S.ovf = 0; }
+// The segment generator of both walks.  emit(cnt, j, bx, by, bz, cls) runs on EVERY lane of the warp once per
+// iteration (the callers aggregate over the warp); cnt == 0: no segment on this lane this iteration.  A segment is
+// steps j .. j+cnt-1 (cnt <= 32) of the ray in block (bx, by, bz), cls its block_class - 2 (generic path) for every
+// segment of a wide ray.  Returns the first step not walked: <= n only when the iteration bound stopped the walk
+// (non-finite pose).
+template <class Emit>
+__device__ __forceinline__ int seg_generate(const TsGrid& g, const SegRay& q, Emit&& emit) {
+  int bx, by, bz, sx, sy, sz;
+  float jx, jy, jz, dx, dy, dz;
+  dda_axis(q.ux, q.tx, bx, jx, dx, sx);
+  dda_axis(q.uy, q.ty, by, jy, dy, sy);
+  dda_axis(q.uz, q.tz, bz, jz, dz, sz);
+  // whole ray inside the block range (both end points are; the cells in between lie between them)?
+  bool inside = false;
+  if (q.n > 0) {
+    const float nf = (float)q.n;
+    const int ex = __float2int_rn(__fmaf_rn(q.ux, nf, q.tx)) >> TS_BSHIFT, ey = __float2int_rn(__fmaf_rn(q.uy, nf, q.ty)) >> TS_BSHIFT,
+              ez = __float2int_rn(__fmaf_rn(q.uz, nf, q.tz)) >> TS_BSHIFT;
+    inside = block_class(g, bx, by, bz) == 1 && block_class(g, ex, ey, ez) == 1;
+  }
+  int j = 1;
+  const int max_iter = 3 * (q.n / 16 + 4);
+  for (int it = 0;; ++it) {
+    const bool act = j <= q.n && it < max_iter;
+    if (!__any_sync(FULL, act)) break;
+    int cnt = 0, jl = 0;
+    if (act) {
+      const float je = fminf(fminf(jx, jy), jz);
+      jl = min((int)ceilf(je) - 1, q.n);  // last step strictly before the crossing
+      if (jl >= j) cnt = min(jl - j + 1, 32);
+    }
+    const int cls = cnt == 0 ? 0 : q.wide ? 2 : inside ? 1 : block_class(g, bx, by, bz);
+    emit(cnt, j, bx, by, bz, cls);
+    j += cnt;
+    if (act && j > jl) {  // the run up to the crossing is out: step into the next block
+      if (jx <= jy && jx <= jz) { bx += sx; jx += dx; }
+      else if (jy <= jz) { by += sy; jy += dy; }
+      else { bz += sz; jz += dz; }
+    }
+  }
+  return j;
+}
+
+// counter of a segment: (block, length class, replica).  The replica depends on the ray index alone (its group of 256
+// rays), so both walks pick the same one, and groups walked at the same time spread a hot block over SEG_REP counters.
+__device__ __forceinline__ int seg_key(int blk, int cnt, uint32_t r) {
+  return (blk * SEG_CLS + ((cnt - 1) >> 1)) * SEG_REP + (int)((r >> 8) & (SEG_REP - 1));
+}
+
+// CTAs per SM of the two walks (tools/bench_march.py on an H100 SXM at 400 W: the counting walk 5-12 % faster with 3 than
+// with 4 on S1-S4; the scattering walk with 6 as fast as with 4 on S1-S3 and 13 % faster on S4)
+#define WC_MINB 3
+#define WS_MINB 6
+
+// K2b-1: counting walk.  Ray set-up, then the segments: activates their blocks (rm_lookup) and counts them per (block,
+// class, replica).  Segments for the generic path (wide rays, blocks next to the volume, non-finite poses) are appended
+// to `gen` here and only here; segments in blocks far outside the volume are counted out of bounds.
+__global__ void __launch_bounds__(MS_THREADS, WC_MINB) k_seg_count(const __grid_constant__ TsBatch batch, TsIntrin in, TsGrid g, TsBucket* buckets,
+                                                                   unsigned long long* bidx, uint32_t bucket_shift, const uint32_t* __restrict__ ray_list,
+                                                                   const int* __restrict__ n_rays_p, uint32_t ray_cap, TsMarchWs w, TsCounters* ctr) {
+  __shared__ unsigned long long s_btab[RM_TAB];  // block coordinates -> pool index (direct mapped, rm_lookup)
+  for (int e = threadIdx.x; e < RM_TAB; e += MS_THREADS) s_btab[e] = TS_EMPTY;
   __syncthreads();
   const uint32_t nme = min((uint32_t)*n_rays_p, ray_cap);
   const uint32_t lane = threadIdx.x & 31u;
-  const int max_seg_ray = (int)(in.max_steps * 0.125f) + 8;  // block crossings of the longest ray (+ slack)
   unsigned int my_oob = 0, my_rays = 0, my_fmax = 0;
   for (uint32_t base = blockIdx.x * MS_THREADS; base < nme; base += gridDim.x * MS_THREADS) {
-    // room for this round's segments in the CTA's list
-    if (threadIdx.x == 0 && !S.ovf) {
-      const long long need = (long long)S.cur + (long long)MS_THREADS * max_seg_ray;
-      while ((long long)S.n_chunk * WK_CHUNK < need) {
-        uint32_t c0 = 0;
-        bool okc = S.n_chunk < WK_MAXCH;
-        if (okc) { c0 = atomicAdd(&w.ctl->tmp_cursor, (unsigned)WK_CHUNK); okc = c0 + WK_CHUNK <= w.seg_cap; }
-        if (!okc) { S.ovf = 1; break; }  // workspace exhausted: the rest of this CTA's rays take the generic path
-        S.chunk[S.n_chunk++] = c0;
-      }
-    }
-    __syncthreads();
-    const bool ovf = S.ovf != 0;
     const uint32_t r = base + threadIdx.x;
-    float ux = 0.f, uy = 0.f, uz = 0.f, tx = 0.f, ty = 0.f, tz = 0.f;
-    int n = 0, s = 0;
-    uint32_t f = 0;
-    bool wide = false;
-    if (r < nme) {
-      const RaySetup rs = ray_setup(batch, in, g, S.btab, buckets, bidx, bucket_shift, ray_list[r], r, w, my_rays, my_fmax);
-      ux = rs.ux; uy = rs.uy; uz = rs.uz; tx = rs.tx; ty = rs.ty; tz = rs.tz;
-      n = rs.n; f = rs.f; s = rs.s; wide = rs.wide;
-    }
-    int bx, by, bz, sx, sy, sz;
-    float jx, jy, jz, dx, dy, dz;
-    dda_axis(ux, tx, bx, jx, dx, sx);
-    dda_axis(uy, ty, by, jy, dy, sy);
-    dda_axis(uz, tz, bz, jz, dz, sz);
-    // whole ray inside the block range (both end points are; the cells in between lie between them)?
-    bool inside = false;
-    if (n > 0) {
-      const float nf = (float)n;
-      const int ex = __float2int_rn(__fmaf_rn(ux, nf, tx)) >> TS_BSHIFT, ey = __float2int_rn(__fmaf_rn(uy, nf, ty)) >> TS_BSHIFT,
-                ez = __float2int_rn(__fmaf_rn(uz, nf, tz)) >> TS_BSHIFT;
-      inside = block_class(g, bx, by, bz) == 1 && block_class(g, ex, ey, ez) == 1;
-    }
-    const uint32_t rj = (f << 24);  // frame of the ray rides in the top byte of the segment word
-    int j = 1;
-    const int max_iter = 3 * (n / 16 + 4);
-    for (int it = 0;; ++it) {
-      const bool act = j <= n && it < max_iter;
-      if (!__any_sync(FULL, act)) break;
-      int cnt = 0, jl = 0;
-      if (act) {
-        const float je = fminf(fminf(jx, jy), jz);
-        jl = min((int)ceilf(je) - 1, n);  // last step strictly before the crossing
-        if (jl >= j) cnt = min(jl - j + 1, 32);
-      }
-      int key = -1;  // block * SEG_CLS + length class
+    float4 ra = make_float4(0.f, 0.f, 0.f, 0.f), rb = ra;
+    uint32_t raux = 0u;
+    if (r < nme) ray_setup(batch, in, g, s_btab, buckets, bidx, bucket_shift, ray_list[r], r, w, my_rays, my_fmax, ra, rb, raux);
+    const SegRay q = seg_ray(batch, ra, rb, raux);
+    int j = seg_generate(g, q, [&](int cnt, int j0, int bx, int by, int bz, int cls) {
+      int key = -1;
       if (cnt > 0) {
-        const int cls = inside ? 1 : block_class(g, bx, by, bz);
-        if (wide || cls == 2 || ovf) gen_append(w, g.err, r, j, cnt);
+        if (cls == 2) gen_append(w, g.err, r, j0, cnt);
         else if (cls == 0) my_oob += (unsigned)cnt;
         else {
-          const int blk = rm_lookup(g, S.btab, ts_pack_key(s, bx, by, bz), bx, by, bz);  // activates + marks the block dirty
-          if (blk >= 0) key = (blk * SEG_CLS + ((cnt - 1) >> 1)) * SEG_REP + (int)(blockIdx.x & (SEG_REP - 1));  // (< 0: pool exhausted)
+          const int blk = rm_lookup(g, s_btab, ts_pack_key(q.s, bx, by, bz), bx, by, bz);  // activates + marks the block dirty
+          if (blk >= 0) key = seg_key(blk, cnt, r);  // (< 0: pool exhausted, the segment is dropped)
         }
       }
-      const bool rec = key >= 0;
-      const unsigned mrec = __ballot_sync(FULL, rec);
-      if (mrec) {
-        const int leader = __ffs(mrec) - 1;
-        int p0 = 0;
-        if ((int)lane == leader) p0 = atomicAdd(&S.cur, __popc(mrec));
-        p0 = __shfl_sync(FULL, p0, leader);
-        if (rec) {
-          const int p = p0 + __popc(mrec & ((1u << lane) - 1u));
-          const uint32_t gp = S.chunk[p >> 12] + (uint32_t)(p & (WK_CHUNK - 1));
-          w.tmp_seg[gp] = TsSeg{r, rj | ((uint32_t)j << 8) | (uint32_t)cnt};
-          w.tmp_key[gp] = (uint32_t)key;
-          const unsigned grp = __match_any_sync(mrec, key);
-          if ((int)lane == __ffs(grp) - 1) red_add_u32((unsigned int*)&w.seg_count[key], (unsigned)__popc(grp));
-        }
+      const unsigned mrec = __ballot_sync(FULL, key >= 0);
+      if (key >= 0) {
+        const unsigned grp = __match_any_sync(mrec, key);
+        if ((int)lane == __ffs(grp) - 1) red_add_u32((unsigned int*)&w.seg_count[key], (unsigned)__popc(grp));
       }
-      j += cnt;
-      if (act && j > jl) {  // the run up to the crossing is out: step into the next block
-        if (jx <= jy && jx <= jz) { bx += sx; jx += dx; }
-        else if (jy <= jz) { by += sy; jy += dy; }
-        else { bz += sz; jz += dz; }
-      }
-    }
+    });
     // non-finite pose: hand the rest to the exact path in bounded pieces
-    while (j <= n) { const int c = min(n - j + 1, 4095); gen_append(w, g.err, r, j, c); j += c; }
+    while (j <= q.n) { const int c = min(q.n - j + 1, 4095); gen_append(w, g.err, r, j, c); j += c; }
   }
-  __syncthreads();
-  const uint32_t cta = blockIdx.x;
-  uint32_t* cch = w.cta_chunk + (size_t)cta * WK_MAXCH;
-  for (int k = threadIdx.x; k < S.n_chunk; k += MS_THREADS) cch[k] = S.chunk[k];
-  if (threadIdx.x == 0) w.cta_n[cta] = S.cur;
   for (int o = 16; o > 0; o >>= 1) {
     my_oob += __shfl_xor_sync(FULL, my_oob, o);
     my_rays += __shfl_xor_sync(FULL, my_rays, o);
@@ -263,9 +263,67 @@ __global__ void __launch_bounds__(MS_THREADS, 3) k_seg_walk(const __grid_constan
   }
 }
 
+// K2b-2: scattering walk.  The same generator over the same stored records, so the same binned segments in the same
+// order per ray.  Each takes a slot of its range with a warp-aggregated returning atomic that counts seg_count[key] down
+// from the count of the counting walk (k_seg_class left it there): a group of n finding `left` slots still free takes
+// the n slots from end - left on, in lane order, so a range fills from its start in the order the groups arrive.  Guards that
+// never fire while the two walks agree route a segment to the generic path instead of writing outside its run, and are
+// counted in n_seg_guard: a block that is not in the grid, a run that is already full.  A block whose activation failed
+// (pool exhausted) was dropped by the counting walk: its segments are dropped here too.  When the launch overflowed
+// (k_seg_scan), every binned segment takes the generic path.
+__global__ void __launch_bounds__(MS_THREADS, WS_MINB) k_seg_scatter(const __grid_constant__ TsBatch batch, TsGrid g, const int* __restrict__ n_rays_p,
+                                                                     uint32_t ray_cap, TsMarchWs w, TsCounters* ctr) {
+  __shared__ unsigned long long s_btab[RM_TAB];  // block coordinates -> pool index (direct mapped, rm_find)
+  for (int e = threadIdx.x; e < RM_TAB; e += MS_THREADS) s_btab[e] = TS_EMPTY;
+  __syncthreads();
+  const uint32_t nme = min((uint32_t)*n_rays_p, ray_cap);
+  const uint32_t lane = threadIdx.x & 31u;
+  const bool overflow = w.ctl->overflow != 0;
+  unsigned int my_guard = 0;
+  for (uint32_t base = blockIdx.x * MS_THREADS; base < nme; base += gridDim.x * MS_THREADS) {
+    const uint32_t r = base + threadIdx.x;
+    float4 ra = make_float4(0.f, 0.f, 0.f, 0.f), rb = ra;
+    uint32_t raux = 0u;
+    if (r < nme) {
+      const float4* src = reinterpret_cast<const float4*>(&w.rays[r]);
+      ra = src[0]; rb = src[1];
+      raux = w.aux[r];
+    }
+    const SegRay q = seg_ray(batch, ra, rb, raux);
+    const uint32_t rj = q.f << 24;  // frame of the ray rides in the top byte of the segment word
+    seg_generate(g, q, [&](int cnt, int j0, int bx, int by, int bz, int cls) {
+      int key = -1, blk = -1;
+      bool to_gen = false;
+      if (cnt > 0 && cls == 1) {
+        if (overflow) to_gen = true;
+        else {
+          blk = rm_find(g, s_btab, ts_pack_key(q.s, bx, by, bz), bx, by, bz);
+          if (blk >= 0) key = seg_key(blk, cnt, r);
+          else if (blk == -1) { to_gen = true; my_guard++; }  // guard: the counting walk activated every binned block
+        }
+      }
+      const unsigned mrec = __ballot_sync(FULL, key >= 0);
+      if (key >= 0) {
+        const unsigned grp = __match_any_sync(mrec, key);
+        const int leader = __ffs(grp) - 1;
+        int left = 0;
+        if ((int)lane == leader) left = atomicSub(&w.seg_count[key], __popc(grp));
+        left = __shfl_sync(grp, left, leader);
+        const int k = __popc(grp & ((1u << lane) - 1u));
+        if (k < left) w.seg[w.seg_off[blk] + w.seg_rel[key] - (uint32_t)(left - k)] = TsSeg{r, rj | ((uint32_t)j0 << 8) | (uint32_t)cnt};
+        else { to_gen = true; my_guard++; }  // guard: more segments than the counting walk counted
+      }
+      if (to_gen) gen_append(w, g.err, r, j0, cnt);
+    });
+  }
+  for (int o = 16; o > 0; o >>= 1) my_guard += __shfl_xor_sync(FULL, my_guard, o);
+  if (lane == 0 && my_guard) atomicAdd(&ctr->n_seg_guard, (unsigned long long)my_guard);
+}
+
 // ---------------------------------------------------------------------------
-// K2c: per block with segments: class counts -> offsets inside the block's run (seg_rel), list of touched blocks.
-// seg_count is handed on zeroed: k_seg_place uses it as the fill cursor.
+// K2c: per block with segments: class counts -> end of each (class, replica) range inside the block's run (seg_rel),
+// list of touched blocks.  seg_count keeps the counts: k_seg_scatter counts each back down to 0 as it fills the range
+// from its start (end - count).
 // ---------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) k_seg_class(TsGrid g, TsMarchWs w) {
   const int nb = min(*g.n_blocks, g.max_blocks);
@@ -281,10 +339,9 @@ __global__ void __launch_bounds__(256) k_seg_class(TsGrid g, TsMarchWs w) {
       for (int q = 0; q < SEG_KEYS / 4; q++) {
         const uint4 c = c4[q];
         if ((c.x | c.y | c.z | c.w) == 0u) { continue; }
-        r4[q] = make_uint4(tot, tot + c.x, tot + c.x + c.y, tot + c.x + c.y + c.z);
         tot += c.x + c.y + c.z + c.w;
+        r4[q] = make_uint4(tot - c.y - c.z - c.w, tot - c.z - c.w, tot - c.w, tot);  // ends of the ranges
         cost += (c.x + c.y + c.z + c.w) * (unsigned)(2 * (q / (SEG_REP / 4)) + 2);
-        c4[q] = make_uint4(0u, 0u, 0u, 0u);
       }
     }
     const unsigned mt = __ballot_sync(FULL, tot > 0u);
@@ -362,7 +419,7 @@ __global__ void __launch_bounds__(1024) k_seg_scan(TsMarchWs w, TsCounters* ctr)
     unsigned int tot_items = 0;
     for (int b = SC_BINS - 1; b >= 0; b--) { s_base[b] = tot_items; tot_items += s_hist[b]; s_hist[b] = 0u; }  // s_hist becomes the fill cursor
     const uint32_t tot = s_run;
-    const bool ovf = tot_items > w.item_cap;  // (segments cannot exceed seg_cap: they come out of the same pool)
+    const bool ovf = tot > w.seg_cap || tot_items > w.item_cap;  // (tot <= seg_cap bounds the items below item_cap)
     s_ovf = ovf ? 1 : 0;
     w.ctl->total_segs = tot;
     w.ctl->overflow = ovf ? 1 : 0;
@@ -396,56 +453,6 @@ __global__ void __launch_bounds__(1024) k_seg_scan(TsMarchWs w, TsCounters* ctr)
 }
 
 // ---------------------------------------------------------------------------
-// K2e: placement.  Same grid as k_seg_walk: CTA i moves the segments of its list into the blocks' runs:
-// seg_off[block] + seg_rel[block, class] + cursor (warp-aggregated global atomic on seg_count, zero on entry).
-// ---------------------------------------------------------------------------
-#define PL_SPLIT 2
-#define PL_THREADS 1024  // the kernel waits on one returning atomic per (warp, key): more warps per list hide it
-__global__ void __launch_bounds__(PL_THREADS) k_seg_place(TsMarchWs w) {
-  __shared__ uint32_t s_chunk[WK_MAXCH];
-  const uint32_t cta = blockIdx.x / PL_SPLIT, part = blockIdx.x % PL_SPLIT;  // PL_SPLIT CTAs share one walk list
-  const int total = w.cta_n[cta];
-  if (total == 0) return;
-  const uint32_t lane = threadIdx.x & 31u;
-  const uint32_t* cch = w.cta_chunk + (size_t)cta * WK_MAXCH;
-  const int nch = (total + WK_CHUNK - 1) / WK_CHUNK;
-  for (int k = threadIdx.x; k < nch; k += PL_THREADS) s_chunk[k] = cch[k];
-  __syncthreads();
-  const bool overflow = w.ctl->overflow != 0;  // work list did not fit: every segment goes to the generic path
-  for (int p0 = (int)(part * PL_THREADS + (threadIdx.x & ~31)); p0 < total; p0 += PL_SPLIT * PL_THREADS) {
-    const int p = p0 + (int)lane;
-    const bool have = p < total;
-    TsSeg sg = TsSeg{0u, 0u};
-    int key = -1;
-    if (have) {
-      const uint32_t gp = s_chunk[p >> 12] + (uint32_t)(p & (WK_CHUNK - 1));
-      sg = w.tmp_seg[gp];
-      key = (int)w.tmp_key[gp];
-    }
-    // Unreachable: a block with c segments makes ceil(c / MR_CHUNK) <= c / MR_CHUNK + 1 items, the segments of a
-    // launch come out of the seg_cap pool and at most max_blocks blocks are touched, so the item count never exceeds
-    // seg_cap / MR_CHUNK + max_blocks < item_cap (ts_march_alloc) and k_seg_scan never sets `overflow`.  That is also
-    // why a segment past gen_cap here is not reported.
-    if (overflow) {
-      if (have) {
-        const int pg = atomicAdd(&w.ctl->n_gen, 1);
-        if ((uint32_t)pg < w.gen_cap) w.gen[pg] = TsSeg{sg.ray, (((sg.jc >> 8) & 0xFFFFu) << 12) | (sg.jc & 255u)};
-      }
-      continue;
-    }
-    const unsigned mh = __ballot_sync(FULL, have);
-    if (have) {
-      const unsigned grp = __match_any_sync(mh, key);
-      const int leader = __ffs(grp) - 1;
-      int c0 = 0;
-      if ((int)lane == leader) c0 = atomicAdd(&w.seg_count[key], __popc(grp));
-      c0 = __shfl_sync(grp, c0, leader) + __popc(grp & ((1u << lane) - 1u));
-      w.seg[w.seg_off[key / SEG_KEYS] + w.seg_rel[key] + (uint32_t)c0] = sg;
-    }
-  }
-}
-
-// ---------------------------------------------------------------------------
 // exact sample index, as the reference states it (:253-254)
 // ---------------------------------------------------------------------------
 __device__ __forceinline__ void exact_index(float ux, float uy, float uz, const float* T, int j, float vs, float rvs, int& xi, int& yi, int& zi) {
@@ -474,7 +481,7 @@ __device__ __forceinline__ void global_sample(const TsGrid& g, int s, int xi, in
 // ---------------------------------------------------------------------------
 // K2f: the march proper.  Persistent CTAs, one work item (block, <= MR_CHUNK segments) at a time.
 //
-// A block's run is ordered by segment length (k_seg_place), so the 32 segments a warp takes - ONE PER LANE, ray
+// A block's run is ordered by segment length (k_seg_scatter), so the 32 segments a warp takes - ONE PER LANE, ray
 // parameters in registers - have (nearly) equal length and are walked in lock step.  Lane l starts at step
 // (7*l mod cnt) of its segment and wraps around: neighbouring rays are nearly parallel, so with every lane at a
 // different depth the 32 shared-memory atomics of a step hit 32 different voxels (same-step marching puts 4-16 rays
@@ -715,11 +722,22 @@ __global__ void __launch_bounds__(256) k_march_generic(const __grid_constant__ T
   }
 }
 
-// end of a launch: fill cursors back to zero, control block cleared
-__global__ void __launch_bounds__(256) k_march_reset(TsMarchWs w) {
+// end of a launch: fill cursors back to zero, control block cleared.  k_seg_scatter counted every run down to 0 unless
+// the launch overflowed; a count left above 0 is a slot of a run that no segment filled (n_seg_guard, must stay 0).
+__global__ void __launch_bounds__(256) k_march_reset(TsMarchWs w, TsCounters* ctr) {
   const int nt = w.ctl->n_touched;
-  for (int q = blockIdx.x * 256 + threadIdx.x; q < nt * (SEG_KEYS / 4); q += gridDim.x * 256)
-    reinterpret_cast<uint4*>(w.seg_count + (size_t)w.touched[q / (SEG_KEYS / 4)] * SEG_KEYS)[q % (SEG_KEYS / 4)] = make_uint4(0u, 0u, 0u, 0u);
+  const bool check = w.ctl->overflow == 0;
+  unsigned int left = 0;
+  for (int q = blockIdx.x * 256 + threadIdx.x; q < nt * (SEG_KEYS / 4); q += gridDim.x * 256) {
+    int4* c4 = reinterpret_cast<int4*>(w.seg_count + (size_t)w.touched[q / (SEG_KEYS / 4)] * SEG_KEYS) + q % (SEG_KEYS / 4);
+    if (check) {
+      const int4 c = *c4;
+      left += (unsigned)(max(c.x, 0) + max(c.y, 0) + max(c.z, 0) + max(c.w, 0));
+    }
+    *c4 = make_int4(0, 0, 0, 0);
+  }
+  for (int o = 16; o > 0; o >>= 1) left += __shfl_xor_sync(FULL, left, o);
+  if ((threadIdx.x & 31) == 0 && left) atomicAdd(&ctr->n_seg_guard, (unsigned long long)left);
   // the last CTA to finish clears the control block
   __shared__ int s_last;
   __syncthreads();
@@ -747,8 +765,6 @@ int ts_march_alloc(tslam_tsdf* m) {
   if (e && atoll(e) > 0) sc = (size_t)atoll(e);
   w.seg_cap = (uint32_t)sc;
   TS_CUDA(cudaMalloc(&w.seg, sc * sizeof(TsSeg)));
-  TS_CUDA(cudaMalloc(&w.tmp_seg, sc * sizeof(TsSeg)));
-  TS_CUDA(cudaMalloc(&w.tmp_key, sc * 4));
   TS_CUDA(cudaMalloc(&w.seg_count, nb * SEG_KEYS * 4));
   TS_CUDA(cudaMemset(w.seg_count, 0, nb * SEG_KEYS * 4));
   TS_CUDA(cudaMalloc(&w.seg_rel, nb * SEG_KEYS * 4));
@@ -760,13 +776,6 @@ int ts_march_alloc(tslam_tsdf* m) {
   TS_CUDA(cudaMalloc(&w.items, (size_t)w.item_cap * sizeof(TsItem)));
   w.gen_cap = (uint32_t)(nr > (1u << 20) ? nr : (1u << 20));
   TS_CUDA(cudaMalloc(&w.gen, (size_t)w.gen_cap * sizeof(TsSeg)));
-  w.walk_x_max = m->sm_count * 3;  // one segment list per CTA (4 and 5 CTAs per SM were slower on an earlier GPU, not re-measured on
-                                   // H100: the per-(block, class) counters are the limit)
-  const size_t ncta = (size_t)w.walk_x_max + TSLAM_MAX_BATCH + 8;
-  TS_CUDA(cudaMalloc(&w.cta_n, ncta * 4));
-  TS_CUDA(cudaMemset(w.cta_n, 0, ncta * 4));
-  TS_CUDA(cudaMalloc(&w.cta_chunk, ncta * WK_MAXCH * 4));
-  TS_CUDA(cudaFuncSetAttribute(k_seg_walk, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(WalkSmem)));
   TS_CUDA(cudaMalloc(&w.ctl, sizeof(TsMarchCtl)));
   TS_CUDA(cudaMemset(w.ctl, 0, sizeof(TsMarchCtl)));
   // |fast index - exact index| bound in voxel units (DESIGN.md "exact indices from a one-FMA fast path"):
@@ -787,9 +796,8 @@ int ts_march_alloc(tslam_tsdf* m) {
 
 void ts_march_free(tslam_tsdf* m) {
   TsMarchWs& w = m->mw;
-  cudaFree(w.rays); cudaFree(w.aux); cudaFree(w.seg); cudaFree(w.tmp_seg); cudaFree(w.tmp_key); cudaFree(w.seg_count); cudaFree(w.seg_rel);
-  cudaFree(w.seg_off); cudaFree(w.touched); cudaFree(w.blk_total); cudaFree(w.blk_cost); cudaFree(w.items); cudaFree(w.gen); cudaFree(w.ctl); cudaFree(w.cta_n);
-  cudaFree(w.cta_chunk);
+  cudaFree(w.rays); cudaFree(w.aux); cudaFree(w.seg); cudaFree(w.seg_count); cudaFree(w.seg_rel); cudaFree(w.seg_off); cudaFree(w.touched);
+  cudaFree(w.blk_total); cudaFree(w.blk_cost); cudaFree(w.items); cudaFree(w.gen); cudaFree(w.ctl);
 }
 
 // workspace of the binned march (allocated at the first launch that needs it)
@@ -799,20 +807,20 @@ int ts_march_setup(tslam_tsdf* m, cudaStream_t st, const TsBatch& batch, uint32_
   return TSLAM_OK;
 }
 
-// sub_ev (profiling, may be null): 4 events recorded at the start, after walk + class + scan, placement and the march kernels
+// sub_ev (profiling, may be null): 4 events recorded at the start, after counting walk + class + scan, the scattering
+// walk and the march kernels
 int ts_march_launch(tslam_tsdf* m, cudaStream_t st, const TsBatch& batch, uint32_t bucket_shift, cudaEvent_t* sub_ev) {
   const int sms = m->sm_count;
-  const int gx = m->mw.walk_x_max;
   if (sub_ev) TS_CUDA(cudaEventRecord(sub_ev[0], st));
-  k_seg_walk<<<gx, MS_THREADS, (int)sizeof(WalkSmem), st>>>(batch, m->in, m->g, m->buckets, m->bidx, bucket_shift, m->ray_list, m->n_rays, m->ray_list_cap,
-                                                            m->mw, m->counters);
+  k_seg_count<<<sms * WC_MINB, MS_THREADS, 0, st>>>(batch, m->in, m->g, m->buckets, m->bidx, bucket_shift, m->ray_list, m->n_rays, m->ray_list_cap,
+                                                    m->mw, m->counters);
   TS_LAUNCH_CHECK(m);
   k_seg_class<<<sms * 2, 256, 0, st>>>(m->g, m->mw);
   TS_LAUNCH_CHECK(m);
   k_seg_scan<<<1, 1024, 0, st>>>(m->mw, m->counters);
   TS_LAUNCH_CHECK(m);
   if (sub_ev) TS_CUDA(cudaEventRecord(sub_ev[1], st));
-  k_seg_place<<<gx * PL_SPLIT, PL_THREADS, 0, st>>>(m->mw);
+  k_seg_scatter<<<sms * WS_MINB, MS_THREADS, 0, st>>>(batch, m->g, m->n_rays, m->ray_list_cap, m->mw, m->counters);
   TS_LAUNCH_CHECK(m);
   if (sub_ev) TS_CUDA(cudaEventRecord(sub_ev[2], st));
   const int grid = (sms - m->rm_reserve) * 3;
@@ -821,7 +829,7 @@ int ts_march_launch(tslam_tsdf* m, cudaStream_t st, const TsBatch& batch, uint32
   TS_LAUNCH_CHECK(m);
   k_march_generic<<<sms * 2, 256, 0, st>>>(batch, m->in, m->g, m->mw, m->counters);
   TS_LAUNCH_CHECK(m);
-  k_march_reset<<<32, 256, 0, st>>>(m->mw);
+  k_march_reset<<<32, 256, 0, st>>>(m->mw, m->counters);
   TS_LAUNCH_CHECK(m);
   if (sub_ev) TS_CUDA(cudaEventRecord(sub_ev[3], st));
   return TSLAM_OK;

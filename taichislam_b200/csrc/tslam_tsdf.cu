@@ -1834,6 +1834,16 @@ extern "C" int tslam_tsdf_get_march_stats(tslam_tsdf_t* m, int64_t* out6) {
   return TSLAM_OK;
 }
 
+extern "C" int tslam_tsdf_get_march_stats2(tslam_tsdf_t* m, int64_t* out7) {
+  if (!m || !out7) return TSLAM_E_INVALID;
+  int rc = tslam_tsdf_get_march_stats(m, out7);
+  if (rc) return rc;
+  TsCounters c;
+  TS_CUDA(cudaMemcpy(&c, m->counters, sizeof(c), cudaMemcpyDeviceToHost));
+  out7[6] = (int64_t)c.n_seg_guard;
+  return TSLAM_OK;
+}
+
 extern "C" int tslam_tsdf_sync(tslam_tsdf_t* m, void* stream) {
   if (!m) return TSLAM_E_INVALID;
   TS_CUDA(cudaStreamSynchronize((cudaStream_t)stream));

@@ -377,8 +377,9 @@ class TsdfHandle:
         return o[:k.value]
 
     def march_stats(self):
-        """Diagnostics of the block-binned ray march since the last stats(clear=True)."""
-        o = np.zeros(6, np.int64)
-        capi.check(self.L.tslam_tsdf_get_march_stats(self.h, capi.np_ptr(o)))
+        """Diagnostics of the block-binned ray march since the last stats(clear=True).  n_seg_guard counts segments the
+        counting and the scattering walk disagreed about; it must stay 0."""
+        o = np.zeros(7, np.int64)
+        capi.check(self.L.tslam_tsdf_get_march_stats2(self.h, capi.np_ptr(o)))
         return dict(n_segs=int(o[0]), n_items=int(o[1]), n_slow=int(o[2]), n_fallback=int(o[3]), n_generic=int(o[4]),
-                    n_verify_bad=int(o[5]))
+                    n_verify_bad=int(o[5]), n_seg_guard=int(o[6]))

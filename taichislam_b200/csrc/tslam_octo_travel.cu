@@ -14,7 +14,7 @@
 // One update computes S such fields, one per start, in the same launches.  The single-source API
 // (tslam_octo_travel_update and its readers) is the S = 1 case, kept in a state of its own so that it and the
 // many-source fields never change each other's answers.  The scheme is the occupancy ESDF's lower wave
-// (k_octo_esdf_sweep): a CTA stages one (block, source) item plus a one-voxel halo of G in shared memory and relaxes it
+// (es_k_wave): a CTA stages one (block, source) item plus a one-voxel halo of G in shared memory and relaxes it
 // in place to local convergence (values only decrease); sweep k runs the items with a neighbour item of the same source
 // stamped >= k-1, starting from the starts' items, and es_wave drives the sweeps.  A step's box lies inside the 3^3
 // neighbourhood of its target cell, so the step rule never leaves the staged tile.
@@ -269,7 +269,7 @@ __global__ void __launch_bounds__(OT_THREADS) k_octo_travel_multi_sweep(OtmAux a
   __shared__ OtmTile tile;
   if (sweep > 1 && a.changed[sweep - 1] == 0) return;  // already converged: nothing to do
   const long long items = (long long)a.S * a.nt;
-  const float d1 = vs, d2 = sqrtf(2.0f) * vs, d3 = sqrtf(3.0f) * vs;  // the edge costs of k_octo_esdf_sweep
+  const float d1 = vs, d2 = sqrtf(2.0f) * vs, d3 = sqrtf(3.0f) * vs;  // the edge costs of es_k_wave
   for (long long it = blockIdx.x; it < items; it += gridDim.x) {
     const int t = (int)(it / a.S), s = (int)(it % a.S);
     __syncthreads();

@@ -600,6 +600,31 @@ int tslam_octo_travel_multi_query(tslam_octo_t* m, int32_t submap, int64_t n, co
 int tslam_octo_travel_multi_path(tslam_octo_t* m, int32_t submap, int64_t n, const int32_t* source, const float* xyz,
                                  int32_t max_len, int32_t* cells, int32_t* len, void* stream);
 
+/* ----------------------------------------------------------------------------
+ * Exploration tours (DESIGN.md section 7): the order in which to visit goals, from a cost matrix such as the S x S
+ * matrix of tslam_octo_travel_multi_query.  Stateless.  cost f32[n,n] (DEVICE), 1 <= n <= TSLAM_OCTO_TRAVEL_MAX_STARTS:
+ * node 0 is the start, nodes 1..n-1 the goals, the diagonal is ignored and every other entry is +inf, zero or a
+ * positive normal f32 (a NaN, a negative value or a subnormal is refused).  Costs are exact: with e_lo / e_hi the least /
+ * greatest floor(log2 x) over the positive finite off-diagonal entries (0 / 0 when there are none), e_hi - e_lo <= 28 is
+ * required, every finite entry is the integer q(x) = x / U units of U = 2^(e_lo - 23), and a leg weighs (inf, q) =
+ * (1, 0) for +inf, (0, q(x)) otherwise.  A tour's cost is the sum of its legs, compared lexicographically (fewer
+ * infinite legs first).  The kept goals K are the g >= 1 with cost[0][g] finite, m = |K|; the others are unreachable.
+ * A tour is open: t[0] = 0, t[1..m] a permutation of K, cost sum_{p<m} w(t[p], t[p+1]).
+ * Restart 0 starts from the nearest-neighbour tour (least w, ties to the smaller node); restart r >= 1 from a
+ * Fisher-Yates shuffle of K ascending: for i = m-1 down to 1, j = mix64(seed ^ (r << 32) ^ i) % (i + 1) in uint64, swap
+ * a[i], a[j] (mix64: the SplitMix64 finaliser).  Each step applies the move giving the cheapest tour if it is strictly
+ * cheaper, ties to the first in the order 2-opt (reverse t[i..j], 1 <= i < j <= m, reversed legs charged in their new
+ * direction) by (i, j), then Or-opt (move t[i..i+L-1], L in {1,2,3}, orientation kept, to follow t[p], p in [0, m] minus
+ * [i-1, i+L-1]) by (L, i, p).  A restart ends when no move improves (converged 1) or when a further move would exceed
+ * max_passes applied moves (converged 0).
+ * --------------------------------------------------------------------------*/
+/* restarts in [1, 4096], max_passes >= 0.  Outputs (DEVICE): tours int32[R,n] (row r: t[0..m], then -1), cost2
+ * int64[R,2] (infinite legs, q), passes int32[R] (moves applied), converged uint8[R], best int32[1] (the least cost,
+ * ties to the smallest r); info2 (HOST): m, e_lo - 23 (U = 2^info2[1]).  Reads the matrix's scan once (synchronises),
+ * then runs asynchronously on `stream`. */
+int tslam_tour_open(int32_t n, const float* cost, int32_t restarts, uint64_t seed, int32_t max_passes, int32_t* tours,
+                    int64_t* cost2, int32_t* passes, uint8_t* converged, int32_t* best, int32_t* info2, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

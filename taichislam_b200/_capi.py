@@ -174,6 +174,7 @@ SIGNATURES = {
     "tslam_octo_travel_multi_update": (C.c_int, [_vp, _i32, _i32, _vp, _f32, _f32, _vp, _vp, _vp, _vp]),
     "tslam_octo_travel_multi_query": (C.c_int, [_vp, _i32, _i64, _vp, _vp, _vp]),
     "tslam_octo_travel_multi_path": (C.c_int, [_vp, _i32, _i64, _vp, _vp, _i32, _vp, _vp, _vp]),
+    "tslam_tour_open": (C.c_int, [_i32, _vp, _i32, C.c_uint64, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
 }
 
 _lib = None

@@ -313,6 +313,34 @@ class Octomap(BaseMap):
         src = np.array([int(source)], np.int32)
         return self._travel_path(lambda g, m: self._h.travel_multi_path(src, g, submap=self._active(), max_len=m), goal, max_len)
 
+    def exploration_tour(self, position, goals, clearance=0.0, max_cost=None, restarts=64, seed=0):
+        """The order in which to visit goals [k,3] (metres, map frame; k <= 1023) from `position` through known free
+        space: travel_update_multi([position] + goals) with the clearance and max_cost of travel_update, the cost matrix
+        travel_cost_multi of the same points (kept on the device), then solve_open_tour on it -> dict(
+          order int64[m]: indices into goals in visiting order (the goals reachable from position);
+          unreachable int64: the other goals' indices;  cost: the tour's travel cost in metres (the exact sum of its
+          matrix entries, as f64);  leg_costs f32[m]: those entries;  inf_legs: legs between goals with no free path;
+          converged: whether the best restart ended in a local optimum;
+          path: travel_path_multi(0, goals[order[0]]), or None when no goal is reachable).
+        The multi fields stay readable: travel_path_multi(s, ...) gives the path of any later leg (start s = goal s-1)."""
+        self._logodds_only("an exploration tour")
+        from ..tour import solve_open_tour
+        torch = self._torch
+        as_np = lambda a: a.detach().cpu().numpy() if isinstance(a, torch.Tensor) else a
+        g = np.asarray(as_np(goals), np.float32).reshape(-1, 3)
+        if g.shape[0] > 1023:
+            raise ValueError(f"exploration_tour takes at most 1023 goals (the start is the 1024th point), not {g.shape[0]}")
+        pts = np.ascontiguousarray(np.concatenate([np.asarray(as_np(position), np.float32).reshape(1, 3), g]))
+        self.travel_update_multi(pts, clearance, max_cost)
+        C = self.travel_cost_multi(torch.from_numpy(pts).to(torch.device("cuda", torch.cuda.current_device())))
+        r = solve_open_tour(C, restarts=restarts, seed=seed)
+        tour = torch.from_numpy(np.concatenate([[0], r["order"]])).to(C.device)
+        leg = C[tour[:-1], tour[1:]].cpu().numpy()
+        order = r["order"] - 1
+        path = self.travel_path_multi(0, g[order[0]]) if order.size else None
+        return dict(order=order, unreachable=r["unreachable"] - 1, cost=r["cost"], leg_costs=leg, inf_legs=r["inf_legs"],
+                    converged=bool(r["converged"][r["best"]]), path=path)
+
     def saveMap(self, path):  # :201-202 (stub in the reference)
         pass
 

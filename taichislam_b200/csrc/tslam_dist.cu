@@ -311,7 +311,7 @@ __global__ void __launch_bounds__(256) k_owner_points(TsGrid g, TsTiling t, floa
 }
 
 // ---- planner queries of a tiled map (tslam_query.cu) ---------------------------------------------------------------
-// owner rank of the block holding each point's cell round(x / vs) - the cell tsdf_probe reads, by the same helper -
+// owner rank of the block holding each point's cell round(x / vs) - the cell TsdfProbe reads, by the same helper -
 // or -1 for a cell outside the volume (it reads occupied and unobserved on any rank)
 __global__ void __launch_bounds__(256) k_owner_cells(TsGrid g, TsTiling t, float vs, long long n, const float* __restrict__ xyz,
                                                       int* __restrict__ owner) {
@@ -323,25 +323,23 @@ __global__ void __launch_bounds__(256) k_owner_cells(TsGrid g, TsTiling t, float
 }
 
 // One round of BaseMap.raycast (mapping_common.py:165-178) on a tiled map, one lane per ray row f32[8] = pos, dir,
-// max_dist, next sample j (int32 bits).  Sample j is a function of (pos, dir, j) alone, computed by the expressions of
-// k_tsdf_raycast, so a ray that stops at sample j here and continues at j on another rank visits the same cells with
-// the same bits as one uninterrupted march.  The march runs while the sample's cell lies in a block this rank owns;
+// max_dist, next sample j (int32 bits).  The samples and their count come from raycast_steps / raycast_sample, as in
+// k_raycast, so a ray that stops at sample j here and continues at j on another rank visits the same cells with the
+// same bits as one uninterrupted march.  The march runs while the sample's cell lies in a block this rank owns;
 // ghosts are not read.  A sample in a foreign block hands the ray over: dest = its owner, j written back.  A hit, a
 // sample outside the volume (occupied on any rank) or the last step ends the ray here: dest = -1 and the answer of
-// k_tsdf_raycast in row i of hit / xyz_out / len_out (for a miss: the last sample's position and length).
+// the TSDF's k_raycast in row i of hit / xyz_out / len_out (for a miss: the last sample's position and length).
 __global__ void __launch_bounds__(256) k_tsdf_raycast_tiled(TsGrid g, TsTiling t, int s, long long n, float* __restrict__ ray, float vs,
                                                              float thres, int* __restrict__ dest, uint8_t* hit, float* xyz_out, float* len_out) {
   for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < n; q += (long long)gridDim.x * blockDim.x) {
     float* r = ray + 8 * q;
-    const float px = r[0], py = r[1], pz = r[2];
-    const float dx = r[3], dy = r[4], dz = r[5];
-    const int steps = (int)(r[6] / vs);  // as k_tsdf_raycast
+    const float3 org = make_float3(r[0], r[1], r[2]), dr = make_float3(r[3], r[4], r[5]);
+    const int steps = raycast_steps(r[6], vs);
     int j = __float_as_int(r[7]), to = -1;
     float x = 0.f, y = 0.f, z = 0.f, len = 0.f;
     bool succ = false;
     for (; j < steps; j++) {
-      len = (float)j * vs;
-      x = dx * len + px; y = dy * len + py; z = dz * len + pz;
+      raycast_sample(org, dr, j, vs, x, y, z, len);
       int c[3];
       if (!ts_query_cell(g, x, y, z, vs, c)) { succ = true; break; }  // outside the volume: TSDF 0 on every rank
       const int o = tile_owner(t, c[0] >> TS_BSHIFT, c[1] >> TS_BSHIFT, c[2] >> TS_BSHIFT);

@@ -142,13 +142,7 @@ __global__ void __launch_bounds__(256) k_esdf_gather(TsGrid g, int submap, long 
     const size_t base = (size_t)b * TS_B3;
     for (int v = threadIdx.x; v < TS_B3; v += blockDim.x) {
       const bool want = g.obs[base + v] > 0;
-      const unsigned m = __ballot_sync(0xffffffffu, want);
-      if (!m) continue;
-      const int lane = threadIdx.x & 31, leader = __ffs(m) - 1;
-      unsigned long long rb = 0;
-      if (lane == leader) rb = atomicAdd(counter, (unsigned long long)__popc(m));
-      rb = __shfl_sync(0xffffffffu, rb, leader);
-      const long long row = (long long)(rb + __popc(m & ((1u << lane) - 1)));
+      const long long row = warp_append_u64(want, counter);
       if (want && row < cap) {
         idx[3 * row] = bx * TS_B + (v >> 8);
         idx[3 * row + 1] = by * TS_B + ((v >> 4) & 15);

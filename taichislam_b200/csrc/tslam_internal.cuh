@@ -195,8 +195,8 @@ __device__ __forceinline__ int warp_append_i32(bool want, int* counter) {
   base = __shfl_sync(0xffffffffu, base, leader);
   return want ? base + __popc(m & ((1u << lane) - 1)) : -1;
 }
-// the same on an unsigned 64-bit counter (the Octomap's count-then-fill gathers)
-__device__ __forceinline__ long long oc_warp_append(bool want, unsigned long long* counter) {
+// the same on an unsigned 64-bit counter (the count-then-fill gathers)
+__device__ __forceinline__ long long warp_append_u64(bool want, unsigned long long* counter) {
   const unsigned m = __ballot_sync(0xffffffffu, want);
   if (!m) return -1;
   const int lane = threadIdx.x & 31;
@@ -230,6 +230,15 @@ __device__ __forceinline__ bool ts_query_cell(const TsGrid& g, float x, float y,
   return ts_in_bounds(g, c[0], c[1], c[2]);
 }
 
+// BaseMap.raycast (mapping_common.py:165-178) marches sample j = 0 .. raycast_steps - 1 of a ray; sample j depends on
+// (pos, dir, j) alone.  k_raycast and k_tsdf_raycast_tiled both take their samples from here, so a tiled ray that
+// continues at sample j on another rank visits the same points, bit for bit, as one uninterrupted march.
+__device__ __forceinline__ int raycast_steps(float max_dist, float vs) { return (int)(max_dist / vs); }  // :167, range(float) truncates
+__device__ __forceinline__ void raycast_sample(float3 pos, float3 dir, int j, float vs, float& x, float& y, float& z, float& len) {
+  len = (float)j * vs;                                                             // :173
+  x = dir.x * len + pos.x; y = dir.y * len + pos.y; z = dir.z * len + pos.z;     // :174
+}
+
 // TSDF and observed byte of in-volume cell c of submap s as the planner queries read them: a block that is absent reads
 // (0, 0), i.e. occupied and unobserved, and so does a ghost block unless Ghosts.
 template <bool Ghosts>
@@ -242,16 +251,20 @@ __device__ __forceinline__ void ts_query_read(const TsGrid& g, int s, const int 
   }
 }
 
+// (x, y, z) = R l + T of a submap pose (row-major R), summed as ((R0 lx + R1 ly) + R2 lz) + T0: the build has
+// -fmad=false, so these are the bits of the reference's f32 expression (submap_i_j_k_to_xyz, mapping_common.py:229-232)
+__device__ __forceinline__ void pose_apply(const float* R, const float* T, float lx, float ly, float lz, float& x, float& y, float& z) {
+  x = ((R[0] * lx + R[1] * ly) + R[2] * lz) + T[0];
+  y = ((R[3] * lx + R[4] * ly) + R[5] * lz) + T[1];
+  z = ((R[6] * lx + R[7] * ly) + R[8] * lz) + T[2];
+}
+
 // position of voxel (i, j, k) of submap s as the exporters write it (tslam_tsdf.cu, tslam_esdf.cu)
 __device__ __forceinline__ void voxel_xyz(const TsGrid& g, bool global_map, const float* pR, const float* pT, int s, int i, int j,
                                           int k, float vs, float& x, float& y, float& z) {
   const float lx = (float)i * vs, ly = (float)j * vs, lz = (float)k * vs;  // ijk_to_xyz mapping_common.py:221-223
   if (global_map) { x = lx; y = ly; z = lz; return; }                      // i_j_k_to_xyz
-  const float* R = pR + 9 * s;                                             // submap_i_j_k_to_xyz :229-232
-  const float* T = pT + 3 * s;
-  x = ((R[0] * lx + R[1] * ly) + R[2] * lz) + T[0];
-  y = ((R[3] * lx + R[4] * ly) + R[5] * lz) + T[1];
-  z = ((R[6] * lx + R[7] * ly) + R[8] * lz) + T[2];
+  pose_apply(pR + 9 * s, pT + 3 * s, lx, ly, lz, x, y, z);                 // submap_i_j_k_to_xyz :229-232
 }
 
 __device__ __forceinline__ void red_add_f32x2(float2* addr, float a, float b) {
@@ -519,6 +532,38 @@ enum { OC_UNK = 0, OC_FREE = 1, OC_OCC = 2 };
 __device__ __forceinline__ unsigned char oc_class(unsigned int w, int l_occ) {
   return !lo_known(w) ? OC_UNK : (lo_val(w) > l_occ ? OC_OCC : OC_FREE);
 }
+// Occupancy rule of the Octomap readers (planner queries, LoD export, fusion, gather) for a cnt word c: OcHits for a hit
+// counter, OcLogodds for a log-odds map.  The readers are written once over the rule (tslam_query.cu, tslam_octo.cu).
+struct OcHits {
+  float thres;  // (float)min_occupy_thres
+  // is_occupy (taichi_octomap.py:86-88); an absent cell reads 0, so there is no c > 0 test
+  __device__ __forceinline__ bool occ(unsigned int c) const { return (float)c > thres; }
+  __device__ __forceinline__ bool unknown(unsigned int) const { return false; }
+  // LoD export: the group's corner voxel exists (c > 0) and is occupied (:90-114)
+  __device__ __forceinline__ bool export_occ(unsigned int c) const { return c > 0 && (float)c > thres; }
+  // fusion: which source voxels are carried over (:181), and how one adds to its target voxel (occupy[ijk_] += c, :183-186)
+  __device__ __forceinline__ bool fuse_src(unsigned int c) const { return (float)c > thres; }
+  __device__ __forceinline__ void fuse_add(unsigned int* p, unsigned int c) const { atomicAdd(p, c); }
+  // gather: the voxels with a hit, and their count
+  static __device__ __forceinline__ bool gather_keep(unsigned int c) { return c > 0; }
+  static __device__ __forceinline__ unsigned int gather_val(unsigned int c) { return c; }
+};
+struct OcLogodds {
+  int l_occ;
+  __device__ __forceinline__ bool occ(unsigned int c) const { return lo_known(c) && lo_val(c) > l_occ; }
+  __device__ __forceinline__ bool unknown(unsigned int c) const { return !lo_known(c); }
+  __device__ __forceinline__ bool export_occ(unsigned int c) const { return lo_known(c) && lo_val(c) > l_occ; }
+  // every known voxel is carried over; the target collects (sum L) << 1 by additions of L << 1 and its known bit by an
+  // OR, so the result does not depend on the order (k_octo_lo_clamp clamps it once all sums are in)
+  __device__ __forceinline__ bool fuse_src(unsigned int c) const { return lo_known(c); }
+  __device__ __forceinline__ void fuse_add(unsigned int* p, unsigned int c) const {
+    red_add_u32(p, (unsigned int)lo_val(c) << 1);
+    atomicOr(p, 1u);
+  }
+  // gather: the known voxels, and their L (int32 bits)
+  static __device__ __forceinline__ bool gather_keep(unsigned int c) { return lo_known(c); }
+  static __device__ __forceinline__ unsigned int gather_val(unsigned int c) { return (unsigned int)lo_val(c); }
+};
 #define OC_MARK_WORDS 32  // mark words per block: 0..15 hit bits, 16..31 miss bits of its 512 voxels (128 B per block)
 struct OcLo {             // per-frame workspace of a log-odds map (allocated in log-odds mode only)
   uint32_t* mark;         // [max_blocks * 32] hit / miss bits of the frame, cleared by k_octo_lo_apply
@@ -710,7 +755,13 @@ static inline int oc_grid(long long work, int per_cta, int cap) {
   const long long g = (work + per_cta - 1) / per_cta;
   return (int)(g < 1 ? 1 : (g > cap ? cap : g));
 }
-// Count-then-fill gather: launch(counter) enqueues one kernel on st that appends its rows through oc_warp_append on the
+// f(rule) with the occupancy rule of the map's mode (OcHits / OcLogodds): one launch site for both readers' instantiations
+template <class F>
+static void oc_with_rule(const tslam_octo* m, F f) {
+  if (m->logodds) f(OcLogodds{m->lo.l_occ});
+  else f(OcHits{(float)m->cfg.min_occupy_thres});
+}
+// Count-then-fill gather: launch(counter) enqueues one kernel on st that appends its rows through warp_append_u64 on the
 // zeroed counter and writes those below cap.  Synchronises; *n_out = the rows found, TSLAM_E_CAPACITY when more than cap.
 template <class F>
 int oc_counted_gather(tslam_octo* m, cudaStream_t st, F launch, int64_t cap, int64_t* n_out, const char* what) {

@@ -63,8 +63,8 @@ __global__ void __launch_bounds__(256) k_octo_depth(OcGrid g, const uint16_t* __
   oc_hit(g, fr.submap, oc_iroundf(px / in.vs), oc_iroundf(py / in.vs), oc_iroundf(pz / in.vs), 1u, cw);
 }
 
-// LO: gather the known voxels of a log-odds map, count[row] = their L (int32 bits)
-template <bool LO>
+// the voxels of submap `submap` the rule keeps (OcHits: a hit, OcLogodds: known), with their count (OcLogodds: L)
+template <class Rule>
 __global__ void __launch_bounds__(256) k_octo_gather(OcGrid g, int submap, long long cap, int32_t* idx, unsigned int* count,
                                                       float* color, unsigned long long* counter) {
   const int nb = min(*g.n_blocks, g.max_blocks);
@@ -81,14 +81,14 @@ __global__ void __launch_bounds__(256) k_octo_gather(OcGrid g, int submap, long 
       v = (int)(e & 511);
       ts_unpack_key(g.block_key[b], s, bx, by, bz);
       c = g.cnt[e];
-      want = (s == submap) && (LO ? lo_known(c) : c > 0);
+      want = (s == submap) && Rule::gather_keep(c);
     }
-    const long long row = oc_warp_append(want, counter);
+    const long long row = warp_append_u64(want, counter);
     if (want && row < cap) {
       idx[3 * row] = bx * OC_B + (v >> 6);
       idx[3 * row + 1] = by * OC_B + ((v >> 3) & 7);
       idx[3 * row + 2] = bz * OC_B + (v & 7);
-      count[row] = LO ? (unsigned int)lo_val(c) : c;
+      count[row] = Rule::gather_val(c);
       if (color) {
         if (g.cw) oc_word_to_rgb(g.cw[e], color + 3 * row);
         else color[3 * row] = color[3 * row + 1] = color[3 * row + 2] = 0.0f;
@@ -100,14 +100,16 @@ __global__ void __launch_bounds__(256) k_octo_gather(OcGrid g, int submap, long 
 // cvt_occupy_to_voxels(level) / cvt_occupy_voxels_to (taichi_octomap.py:90-114).
 // occupy.parent(level) visits the active ancestor cells, reported at the group's base
 // coordinate, and is_occupy (:86-88) is evaluated AT that coordinate: a group is
-// exported iff its corner voxel exists and has count > min_occupy_thres.
-__global__ void __launch_bounds__(256) k_octo_extract(OcGrid g, int submap, int group, float thres, const float* pR, const float* pT,
+// exported iff its corner voxel passes rule.export_occ (hits: exists and has count > min_occupy_thres; log-odds: known
+// and L > l_occ).
+template <class Rule>
+__global__ void __launch_bounds__(256) k_octo_extract(OcGrid g, int submap, int group, Rule rule, const float* pR, const float* pT,
                                                        float vs, long long cap, float* xyz, float* rgb, int* counter) {
   const int nb = min(*g.n_blocks, g.max_blocks);
   const long long total = (long long)nb * OC_B3;
   const long long stride = (long long)gridDim.x * blockDim.x;
   const long long iters = (total + stride - 1) / stride;
-  for (long long it = 0; it < iters; ++it) {
+  for (long long it = 0; it < iters; ++it) {  // uniform trip count: the warp ballot below needs all lanes
     const long long e = it * stride + (long long)blockIdx.x * blockDim.x + threadIdx.x;
     bool want = false;
     int i = 0, j = 0, k = 0, s = 0;
@@ -117,93 +119,43 @@ __global__ void __launch_bounds__(256) k_octo_extract(OcGrid g, int submap, int 
       int bx, by, bz;
       ts_unpack_key(g.block_key[b], s, bx, by, bz);
       i = bx * OC_B + (v >> 6); j = by * OC_B + ((v >> 3) & 7); k = bz * OC_B + (v & 7);
-      const unsigned int c = g.cnt[e];
       // tree offset is -N/2 (taichi_octomap.py:72): groups are aligned in offset coordinates
       const bool aligned = ((i + g.hN) % group == 0) && ((j + g.hN) % group == 0) && ((k + g.hNz) % group == 0);
-      want = (s == submap) && c > 0 && aligned && ((float)c > thres);
+      want = (s == submap) && aligned && rule.export_occ(g.cnt[e]);
     }
-    const unsigned m = __ballot_sync(0xffffffffu, want);
-    int row = -1;
-    if (m) {
-      const int lane = threadIdx.x & 31, leader = __ffs(m) - 1;
-      int base = 0;
-      if (lane == leader) base = atomicAdd(counter, __popc(m));
-      base = __shfl_sync(0xffffffffu, base, leader);
-      row = base + __popc(m & ((1u << lane) - 1));
-    }
+    const int row = warp_append_i32(want, counter);
     if (want && row < cap) {
-      const float lx = (float)i * vs, ly = (float)j * vs, lz = (float)k * vs;  // sijk_to_xyz mapping_common.py:234-238
-      const float* R = pR + 9 * s;
-      const float* T = pT + 3 * s;
-      xyz[3 * (size_t)row] = ((R[0] * lx + R[1] * ly) + R[2] * lz) + T[0];
-      xyz[3 * (size_t)row + 1] = ((R[3] * lx + R[4] * ly) + R[5] * lz) + T[1];
-      xyz[3 * (size_t)row + 2] = ((R[6] * lx + R[7] * ly) + R[8] * lz) + T[2];
+      // sijk_to_xyz mapping_common.py:234-238
+      pose_apply(pR + 9 * s, pT + 3 * s, (float)i * vs, (float)j * vs, (float)k * vs, xyz[3 * (size_t)row], xyz[3 * (size_t)row + 1],
+                 xyz[3 * (size_t)row + 2]);
       if (rgb && g.cw) oc_word_to_rgb(g.cw[e], rgb + 3 * (size_t)row);  // export_color[index] = color[sijk] (:101-102)
     }
   }
 }
 
-// the same LoD export on a log-odds map: the group's corner voxel is known and L > l_occ
-__global__ void __launch_bounds__(256) k_octo_lo_extract(OcGrid g, int submap, int group, int l_occ, const float* pR, const float* pT,
-                                                       float vs, long long cap, float* xyz, float* rgb, int* counter) {
-  const int nb = min(*g.n_blocks, g.max_blocks);
-  const long long total = (long long)nb * OC_B3;
-  const long long stride = (long long)gridDim.x * blockDim.x;
-  const long long iters = (total + stride - 1) / stride;
-  for (long long it = 0; it < iters; ++it) {
-    const long long e = it * stride + (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    bool want = false;
-    int i = 0, j = 0, k = 0, s = 0;
-    if (e < total) {
-      const int b = (int)(e >> 9);
-      const int v = (int)(e & 511);
-      int bx, by, bz;
-      ts_unpack_key(g.block_key[b], s, bx, by, bz);
-      i = bx * OC_B + (v >> 6); j = by * OC_B + ((v >> 3) & 7); k = bz * OC_B + (v & 7);
-      const unsigned int c = g.cnt[e];
-      const bool aligned = ((i + g.hN) % group == 0) && ((j + g.hN) % group == 0) && ((k + g.hNz) % group == 0);
-      want = (s == submap) && lo_known(c) && aligned && lo_val(c) > l_occ;
-    }
-    const unsigned m = __ballot_sync(0xffffffffu, want);
-    int row = -1;
-    if (m) {
-      const int lane = threadIdx.x & 31, leader = __ffs(m) - 1;
-      int base = 0;
-      if (lane == leader) base = atomicAdd(counter, __popc(m));
-      base = __shfl_sync(0xffffffffu, base, leader);
-      row = base + __popc(m & ((1u << lane) - 1));
-    }
-    if (want && row < cap) {
-      const float lx = (float)i * vs, ly = (float)j * vs, lz = (float)k * vs;  // sijk_to_xyz mapping_common.py:234-238
-      const float* R = pR + 9 * s;
-      const float* T = pT + 3 * s;
-      xyz[3 * (size_t)row] = ((R[0] * lx + R[1] * ly) + R[2] * lz) + T[0];
-      xyz[3 * (size_t)row + 1] = ((R[3] * lx + R[4] * ly) + R[5] * lz) + T[1];
-      xyz[3 * (size_t)row + 2] = ((R[6] * lx + R[7] * ly) + R[8] * lz) + T[2];
-      if (rgb && g.cw) oc_word_to_rgb(g.cw[e], rgb + 3 * (size_t)row);  // export_color[index] = color[sijk] (:101-102)
-    }
-  }
-}
-
-// fuse_submaps_kernel (taichi_octomap.py:171-189)
-__global__ void __launch_bounds__(256) k_octo_fuse(OcGrid dst, OcGrid src, float thres, const float* pR, const float* pT, float vs) {
+// fuse_submaps_kernel (taichi_octomap.py:171-189): every source voxel the rule carries over (rule.fuse_src) is placed at
+// the nearest target voxel of its submap's pose and added there (rule.fuse_add); the largest colour word wins.
+template <class Rule>
+__global__ void __launch_bounds__(256) k_octo_fuse(OcGrid dst, OcGrid src, Rule rule, const float* pR, const float* pT, float vs) {
   const int nb = min(*src.n_blocks, src.max_blocks);
   const long long total = (long long)nb * OC_B3;
   for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
     const unsigned int c = src.cnt[e];
-    if (!((float)c > thres)) continue;  // :181
+    if (!rule.fuse_src(c)) continue;  // :181
     const int b = (int)(e >> 9), v = (int)(e & 511);
     int s, bx, by, bz;
     ts_unpack_key(src.block_key[b], s, bx, by, bz);
-    const float lx = (float)(bx * OC_B + (v >> 6)) * vs, ly = (float)(by * OC_B + ((v >> 3) & 7)) * vs,
-                lz = (float)(bz * OC_B + (v & 7)) * vs;
-    const float* R = pR + 9 * s;
-    const float* T = pT + 3 * s;
-    const float x = ((R[0] * lx + R[1] * ly) + R[2] * lz) + T[0];  // :182
-    const float y = ((R[3] * lx + R[4] * ly) + R[5] * lz) + T[1];
-    const float z = ((R[6] * lx + R[7] * ly) + R[8] * lz) + T[2];
+    float x, y, z;
+    pose_apply(pR + 9 * s, pT + 3 * s, (float)(bx * OC_B + (v >> 6)) * vs, (float)(by * OC_B + ((v >> 3) & 7)) * vs,
+               (float)(bz * OC_B + (v & 7)) * vs, x, y, z);  // :182
+    const int i = oc_iroundf(x / vs), j = oc_iroundf(y / vs), k = oc_iroundf(z / vs);  // :183-186
+    if (!ts_in_bounds(dst, i, j, k)) continue;
+    const int blk = ts_get_or_alloc(dst, ts_pack_key(0, i >> OC_BSHIFT, j >> OC_BSHIFT, k >> OC_BSHIFT));
+    if (blk < 0) continue;
+    const size_t o = (size_t)blk * OC_B3 + oc_voxel_off(i, j, k);
+    rule.fuse_add(&dst.cnt[o], c);
     const unsigned long long cw = (dst.cw && src.cw) ? src.cw[e] : 0ull;  // color[ijk_] = submap_color[s,i,j,k] (:189)
-    oc_hit(dst, 0, oc_iroundf(x / vs), oc_iroundf(y / vs), oc_iroundf(z / vs), c, cw);  // :183-186
+    if (cw) ts_red_max_u64(&dst.cw[o], cw);
   }
 }
 
@@ -395,36 +347,7 @@ __global__ void __launch_bounds__(128) k_octo_lo_apply(OcGrid g, OcLo lo, int* e
   }
 }
 
-// Fusion of log-odds maps: every known source voxel adds its L to the nearest target voxel (placement as k_octo_fuse).
-// The target word collects (sum L) << 1 by additions of L << 1 and gets its known bit by an OR, so the result does not
-// depend on the order; k_octo_lo_clamp clamps every target voxel once when all sums are in.
-__global__ void __launch_bounds__(256) k_octo_lo_fuse(OcGrid dst, OcGrid src, const float* pR, const float* pT, float vs) {
-  const int nb = min(*src.n_blocks, src.max_blocks);
-  const long long total = (long long)nb * OC_B3;
-  for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
-    const unsigned int c = src.cnt[e];
-    if (!lo_known(c)) continue;
-    const int b = (int)(e >> 9), v = (int)(e & 511);
-    int s, bx, by, bz;
-    ts_unpack_key(src.block_key[b], s, bx, by, bz);
-    const float lx = (float)(bx * OC_B + (v >> 6)) * vs, ly = (float)(by * OC_B + ((v >> 3) & 7)) * vs,
-                lz = (float)(bz * OC_B + (v & 7)) * vs;
-    const float* R = pR + 9 * s;
-    const float* T = pT + 3 * s;
-    const float x = ((R[0] * lx + R[1] * ly) + R[2] * lz) + T[0];
-    const float y = ((R[3] * lx + R[4] * ly) + R[5] * lz) + T[1];
-    const float z = ((R[6] * lx + R[7] * ly) + R[8] * lz) + T[2];
-    const int i = oc_iroundf(x / vs), j = oc_iroundf(y / vs), k = oc_iroundf(z / vs);
-    if (!ts_in_bounds(dst, i, j, k)) continue;
-    const int blk = ts_get_or_alloc(dst, ts_pack_key(0, i >> OC_BSHIFT, j >> OC_BSHIFT, k >> OC_BSHIFT));
-    if (blk < 0) continue;
-    const size_t o = (size_t)blk * OC_B3 + oc_voxel_off(i, j, k);
-    red_add_u32(&dst.cnt[o], (unsigned int)lo_val(c) << 1);
-    atomicOr(&dst.cnt[o], 1u);
-    const unsigned long long cw = (dst.cw && src.cw) ? src.cw[e] : 0ull;
-    if (cw) ts_red_max_u64(&dst.cw[o], cw);
-  }
-}
+// after k_octo_fuse<OcLogodds>: clamps every known target voxel once, when all sums are in
 __global__ void __launch_bounds__(256) k_octo_lo_clamp(OcGrid g, int l_min, int l_max) {
   const int nb = min(*g.n_blocks, g.max_blocks);
   const long long total = (long long)nb * OC_B3;
@@ -635,8 +558,7 @@ static void oc_fill_frame(tslam_octo* m, TsFrame& fr, const float* R9, const flo
 // steps 2 and 3 of a log-odds frame; n_max bounds the ray records the endpoint kernel wrote
 static int oc_lo_finish(tslam_octo* m, const TsFrame& fr, int n_max, cudaStream_t st) {
   k_octo_lo_walk<<<(n_max + 255) / 256, 256, 0, st>>>(m->g, m->lo, fr.submap, m->in.vs, fr.T[0], fr.T[1], fr.T[2]);
-  m->launches++;
-  TS_CUDA(cudaGetLastError());
+  TS_LAUNCH_CHECK(m);
   const unsigned track = (m->esdf_dirty ? OC_TRACK_ESDF : 0u) | (m->fr_dirty ? OC_TRACK_FRONTIER : 0u);
   const int grid = m->sm_count * 16;
   if (track == 0u)
@@ -647,8 +569,7 @@ static int oc_lo_finish(tslam_octo* m, const TsFrame& fr, int n_max, cudaStream_
     k_octo_lo_apply<OC_TRACK_FRONTIER><<<grid, 128, 0, st>>>(m->g, m->lo, nullptr, m->fr_dirty);
   else
     k_octo_lo_apply<OC_TRACK_ESDF | OC_TRACK_FRONTIER><<<grid, 128, 0, st>>>(m->g, m->lo, m->esdf_dirty, m->fr_dirty);
-  m->launches++;
-  TS_CUDA(cudaGetLastError());
+  TS_LAUNCH_CHECK(m);
   return TSLAM_OK;
 }
 
@@ -704,13 +625,11 @@ extern "C" int tslam_octo_integrate_points_rgb(tslam_octo_t* m, const float* xyz
     if (n > m->ray_cap) { ts_set_error("n=%d exceeds the ray records of a log-odds map (%d)", n, m->ray_cap); return TSLAM_E_INVALID; }
     TS_CUDA(cudaMemsetAsync(m->lo.ctr, 0, 8, st));
     k_octo_lo_points<<<(n + 255) / 256, 256, 0, st>>>(m->g, m->lo, src, n, fr, m->in.vs, csrc);
-    m->launches++;
-    TS_CUDA(cudaGetLastError());
+    TS_LAUNCH_CHECK(m);
     return oc_lo_finish(m, fr, n, st);
   }
   k_octo_points<<<(n + 255) / 256, 256, 0, st>>>(m->g, src, n, fr, m->in.vs, csrc);
-  m->launches++;
-  TS_CUDA(cudaGetLastError());
+  TS_LAUNCH_CHECK(m);
   return TSLAM_OK;
 }
 
@@ -745,22 +664,21 @@ extern "C" int tslam_octo_integrate_depth_tex(tslam_octo_t* m, const uint16_t* d
   if (m->logodds) {
     TS_CUDA(cudaMemsetAsync(m->lo.ctr, 0, 8, st));
     k_octo_lo_depth<<<(hh * ww + 255) / 256, 256, 0, st>>>(m->g, m->lo, src, h, w, hh, ww, fr, m->in, tsrc, th, tw);
-    m->launches++;
-    TS_CUDA(cudaGetLastError());
+    TS_LAUNCH_CHECK(m);
     return oc_lo_finish(m, fr, hh * ww, st);
   }
   k_octo_depth<<<(hh * ww + 255) / 256, 256, 0, st>>>(m->g, src, h, w, hh, ww, fr, m->in, tsrc, th, tw);
-  m->launches++;
-  TS_CUDA(cudaGetLastError());
+  TS_LAUNCH_CHECK(m);
   return TSLAM_OK;
 }
 
-template <bool LO>
 static int oc_gather(tslam_octo* m, int32_t submap, int64_t cap, int32_t* idx, uint32_t* count, float* color, int64_t* n_out,
                      cudaStream_t st) {
   const int rc = oc_counted_gather(m, st, [&](unsigned long long* ctr) {
-    k_octo_gather<LO><<<m->sm_count * 8, 256, 0, st>>>(m->g, submap, cap, idx, count, color, ctr);
-  }, cap, n_out, LO ? "tslam_octo_gather_logodds" : "tslam_octo_gather");
+    oc_with_rule(m, [&](auto rule) {
+      k_octo_gather<decltype(rule)><<<m->sm_count * 8, 256, 0, st>>>(m->g, submap, cap, idx, count, color, ctr);
+    });
+  }, cap, n_out, m->logodds ? "tslam_octo_gather_logodds" : "tslam_octo_gather");
   if (rc && rc != TSLAM_E_CAPACITY) return rc;
   const int drc = oc_deferred(m);  // dropped hits are reported before a short buffer
   return drc ? drc : rc;
@@ -774,13 +692,13 @@ extern "C" int tslam_octo_gather2(tslam_octo_t* m, int32_t submap, int64_t cap, 
                                   int64_t* n_out, void* stream) {
   if (!m || !n_out) return TSLAM_E_INVALID;
   if (m->logodds) { ts_set_error("tslam_octo_gather*: the map holds log-odds, read it with tslam_octo_gather_logodds"); return TSLAM_E_INVALID; }
-  return oc_gather<false>(m, submap, cap, idx, count, color, n_out, (cudaStream_t)stream);
+  return oc_gather(m, submap, cap, idx, count, color, n_out, (cudaStream_t)stream);
 }
 extern "C" int tslam_octo_gather_logodds(tslam_octo_t* m, int32_t submap, int64_t cap, int32_t* idx, int32_t* L, float* color,
                                          int64_t* n_out, void* stream) {
   if (!m || !n_out) return TSLAM_E_INVALID;
   if (!m->logodds) { ts_set_error("tslam_octo_gather_logodds: the map is a hit counter"); return TSLAM_E_INVALID; }
-  return oc_gather<true>(m, submap, cap, idx, (uint32_t*)L, color, n_out, (cudaStream_t)stream);
+  return oc_gather(m, submap, cap, idx, (uint32_t*)L, color, n_out, (cudaStream_t)stream);
 }
 
 extern "C" int tslam_octo_extract(tslam_octo_t* m, int32_t submap, int32_t level, int64_t cap, float* xyz, int32_t* count_dev,
@@ -794,14 +712,10 @@ extern "C" int tslam_octo_extract2(tslam_octo_t* m, int32_t submap, int32_t leve
   long long group = 1;
   for (int l = 1; l < level; l++) group *= m->cfg.K;
   if (group > (1 << 20)) group = 1 << 20;
-  if (m->logodds)
-    k_octo_lo_extract<<<m->sm_count * 8, 256, 0, st>>>(m->g, submap, (int)group, m->lo.l_occ, m->pose_R, m->pose_T, m->in.vs, cap, xyz,
-                                                       rgb, count_dev);
-  else
-    k_octo_extract<<<m->sm_count * 8, 256, 0, st>>>(m->g, submap, (int)group, (float)m->cfg.min_occupy_thres, m->pose_R, m->pose_T,
-                                                    m->in.vs, cap, xyz, rgb, count_dev);
-  m->launches++;
-  TS_CUDA(cudaGetLastError());
+  oc_with_rule(m, [&](auto rule) {
+    k_octo_extract<<<m->sm_count * 8, 256, 0, st>>>(m->g, submap, (int)group, rule, m->pose_R, m->pose_T, m->in.vs, cap, xyz, rgb, count_dev);
+  });
+  TS_LAUNCH_CHECK(m);
   return TSLAM_OK;
 }
 
@@ -811,19 +725,14 @@ extern "C" int tslam_octo_fuse(tslam_octo_t* dst, tslam_octo_t* src, void* strea
   int rc = tslam_octo_reset(dst, stream);  // taichi_octomap.py:195-196
   if (rc) return rc;
   cudaStream_t st = (cudaStream_t)stream;
+  oc_with_rule(dst, [&](auto rule) {
+    k_octo_fuse<<<dst->sm_count * 8, 256, 0, st>>>(dst->g, src->g, rule, dst->pose_R, dst->pose_T, dst->in.vs);
+  });
+  TS_LAUNCH_CHECK(dst);
   if (dst->logodds) {
-    k_octo_lo_fuse<<<dst->sm_count * 8, 256, 0, st>>>(dst->g, src->g, dst->pose_R, dst->pose_T, dst->in.vs);
-    dst->launches++;
-    TS_CUDA(cudaGetLastError());
     k_octo_lo_clamp<<<dst->sm_count * 8, 256, 0, st>>>(dst->g, dst->lo.l_min, dst->lo.l_max);
-    dst->launches++;
-    TS_CUDA(cudaGetLastError());
-    return TSLAM_OK;
+    TS_LAUNCH_CHECK(dst);
   }
-  k_octo_fuse<<<dst->sm_count * 8, 256, 0, st>>>(dst->g, src->g, (float)dst->cfg.min_occupy_thres, dst->pose_R, dst->pose_T,
-                                                 dst->in.vs);
-  dst->launches++;
-  TS_CUDA(cudaGetLastError());
   return TSLAM_OK;
 }
 

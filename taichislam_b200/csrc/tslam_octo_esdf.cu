@@ -88,7 +88,7 @@ __global__ void __launch_bounds__(EsOcto::THREADS) k_octo_esdf_gather(OcGrid g, 
     const size_t base = (size_t)b * OC_B3;
     for (int v = threadIdx.x; v < OC_B3; v += blockDim.x) {
       const bool want = (a.cls[base + v] & ES_CLS) != OC_UNK;
-      const long long row = oc_warp_append(want, counter);
+      const long long row = warp_append_u64(want, counter);
       if (want && row < cap) {
         idx[3 * row] = bx * OC_B + (v >> 6);
         idx[3 * row + 1] = by * OC_B + ((v >> 3) & 7);

@@ -334,7 +334,7 @@ __global__ void __launch_bounds__(OT_THREADS) k_octo_travel_slot_gather(OcGrid g
     for (int v = threadIdx.x; v < OC_B3; v += blockDim.x) {
       const float gv = G[v];
       const bool want = isfinite(gv);
-      const long long row = oc_warp_append(want, counter);
+      const long long row = warp_append_u64(want, counter);
       if (want && row < cap) {
         idx[3 * row] = bx * OC_B + (v >> 6);
         idx[3 * row + 1] = by * OC_B + ((v >> 3) & 7);

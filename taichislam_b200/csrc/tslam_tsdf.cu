@@ -638,13 +638,8 @@ __global__ void __launch_bounds__(256) k_collect_dirty(TsGrid g) {
   for (int it = 0; it < iters; ++it) {
     const int b = it * stride + blockIdx.x * blockDim.x + threadIdx.x;
     const bool want = b < nb && g.dirty_flag[b] != 0;
-    const unsigned m = __ballot_sync(0xffffffffu, want);
-    if (!m) continue;
-    const int lane = threadIdx.x & 31, leader = __ffs(m) - 1;
-    int base = 0;
-    if (lane == leader) base = atomicAdd(g.n_dirty, __popc(m));
-    base = __shfl_sync(0xffffffffu, base, leader);
-    if (want) g.dirty_list[base + __popc(m & ((1u << lane) - 1))] = b;
+    const int row = warp_append_i32(want, g.n_dirty);
+    if (want) g.dirty_list[row] = b;
   }
 }
 __global__ void k_reset_counters(int* a, int* b) {
@@ -1496,17 +1491,6 @@ __global__ void __launch_bounds__(256) k_count_active(TsGrid g, int submap, unsi
   if ((threadIdx.x & 31) == 0 && c) atomicAdd(out, (unsigned long long)c);
 }
 
-// warp-aggregated append: returns the output row of this lane (or -1)
-__device__ __forceinline__ long long warp_append(bool want, unsigned long long* counter) {
-  const unsigned m = __ballot_sync(0xffffffffu, want);
-  if (!m) return -1;
-  const int lane = threadIdx.x & 31;
-  const int leader = __ffs(m) - 1;
-  unsigned long long base = 0;
-  if (lane == leader) base = atomicAdd(counter, (unsigned long long)__popc(m));
-  base = __shfl_sync(0xffffffffu, base, leader);
-  return want ? (long long)(base + __popc(m & ((1u << lane) - 1))) : -1;
-}
 __global__ void __launch_bounds__(256) k_gather(TsGrid g, int submap, long long cap, int32_t* idx, float* tsdf, float* wts,
                                                  int8_t* occ, float* color, unsigned long long* counter) {
   const int nb = min(*g.n_blocks, g.max_blocks);
@@ -1517,7 +1501,7 @@ __global__ void __launch_bounds__(256) k_gather(TsGrid g, int submap, long long 
     const size_t base = (size_t)b * TS_B3;
     for (int v = threadIdx.x; v < TS_B3; v += blockDim.x) {
       const bool want = g.obs[base + v] > 0;
-      const long long row = warp_append(want, counter);
+      const long long row = warp_append_u64(want, counter);
       if (want && row < cap) {
         idx[3 * row] = bx * TS_B + (v >> 8);
         idx[3 * row + 1] = by * TS_B + ((v >> 4) & 15);
@@ -1733,8 +1717,6 @@ __global__ void __launch_bounds__(256) k_fuse(TsGrid dst, TsGrid src, const floa
     int s, bx, by, bz;
     ts_unpack_key(src.block_key[b], s, bx, by, bz);
     if (src.ghost[b]) continue;
-    const float* R = pR + 9 * s;
-    const float* T = pT + 3 * s;
     const size_t base = (size_t)b * TS_B3;
     unsigned long long cur_key = TS_EMPTY;
     int cur_blk = -1;
@@ -1745,11 +1727,10 @@ __global__ void __launch_bounds__(256) k_fuse(TsGrid dst, TsGrid src, const floa
       const bool tex = dst.col != nullptr && src.col != nullptr;
       float4 sc = make_float4(0.f, 0.f, 0.f, 0.f);
       if (tex) sc = src.col[base + v];
-      const float lx = (float)(bx * TS_B + (v >> 8)) * vs, ly = (float)(by * TS_B + ((v >> 4) & 15)) * vs,
-                  lz = (float)(bz * TS_B + (v & 15)) * vs;
-      const float gx = (((R[0] * lx + R[1] * ly) + R[2] * lz) + T[0]) / vs;  // :293-294
-      const float gy = (((R[3] * lx + R[4] * ly) + R[5] * lz) + T[1]) / vs;
-      const float gz = (((R[6] * lx + R[7] * ly) + R[8] * lz) + T[2]) / vs;
+      float x, y, z;
+      pose_apply(pR + 9 * s, pT + 3 * s, (float)(bx * TS_B + (v >> 8)) * vs, (float)(by * TS_B + ((v >> 4) & 15)) * vs,
+                 (float)(bz * TS_B + (v & 15)) * vs, x, y, z);  // :293-294
+      const float gx = x / vs, gy = y / vs, gz = z / vs;
       const int lo0 = (int)floorf(gx), lo1 = (int)floorf(gy), lo2 = (int)floorf(gz);  // :296
 #pragma unroll
       for (int c = 1; c < 8; c++) {  // c=0 (di=dj=dk=0) skipped: reference quirk :300

@@ -198,7 +198,7 @@ class LogoddsMap:
         return known & (val > self.p["l_occ"]), known
 
     def query_points(self, xyz, submap=0):
-        """(occupied, unknown) of the points' cells (k_octo_lo_query_points)."""
+        """(occupied, unknown) of the points' cells (k_query_points<OcProbe<OcLogodds>>)."""
         occ, known = self.occupied_cells(cells(xyz, self.vs), submap)
         return occ, ~known
 

@@ -1,8 +1,9 @@
-"""numpy f32 statement of the planner raycast's samples and of the tiling (k_tsdf_raycast / k_tsdf_raycast_tiled,
-ts_query_cell, tile_coord / tile_owner of csrc/tslam_dist.cu): sample j of a ray is len = f32(j) * vs, x = dir * len +
-pos (two roundings: the library builds with -fmad=false), cell = (int)roundf(x / vs) with roundf half away from zero
-and the float -> int conversion of the GPU (NaN -> 0, saturating).  Used for the round bound of the hand-over
-(test_tiled_raycast_cpu.py) and as a stand-in march for the host round loop under gloo."""
+"""numpy f32 statement of the planner raycast's samples and of the tiling (raycast_sample / raycast_steps, which
+k_raycast and k_tsdf_raycast_tiled share, ts_query_cell, tile_coord / tile_owner of csrc/tslam_dist.cu): sample j of
+a ray is len = f32(j) * vs, x = dir * len + pos (two roundings: the library builds with -fmad=false), cell =
+(int)roundf(x / vs) with roundf half away from zero and the float -> int conversion of the GPU (NaN -> 0,
+saturating).  Used for the round bound of the hand-over (test_tiled_raycast_cpu.py) and as a stand-in march for the
+host round loop under gloo."""
 import numpy as np
 
 F = np.float32

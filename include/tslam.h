@@ -543,6 +543,28 @@ int tslam_octo_view_gain_frontier(tslam_octo_t* m, int32_t submap, int64_t n, co
                                   const tslam_view_camera_t* cam, int64_t n_clusters, uint8_t* valid, int32_t* total,
                                   int32_t* per_cluster, void* stream);
 
+/* Frontier viewpoints: candidate sensor poses around each frontier cluster of the last tslam_octo_frontier_update, the
+ * best top_k per cluster (DESIGN.md section 7).  Classes as of the call.  Candidate (c, s) for cluster ordinal c and
+ * sample s < n_samples: m = (float)((double)sum / (double)voxels * (double)vs) per axis from c's record, p = m +
+ * offsets[s] (f32), and the level camera facing m: (dx, dy) = (m - p)_xy, h = sqrtf(dx*dx + dy*dy), (ux, uy) =
+ * (dx, dy) / h, R = [[uy, 0, ux], [-ux, 0, uy], [0, -1, 0]] row-major (the view-gain convention).  A candidate is valid
+ * iff p is finite, h > 0 and its cell round_half_away(p / vs) is traversable under the travel-cost rule with `clearance`;
+ * an invalid candidate is not an error.  Its score is the number of cluster c's frontier voxels the frontier gain would
+ * count for (p, R) with `cam`.  Kept: valid and score >= min_visible, ordered by score descending, then s ascending.
+ * Outputs (DEVICE): count int32[nc] = min(top_k, kept); per slot j < top_k of cluster c (index c * top_k + j): sample
+ * int32, visible int32, pos f32[3], R9 f32[9]; slots at and beyond count hold sample -1, visible 0 and a zero pose.
+ * offsets f32[n_samples,3] (DEVICE), 1 <= n_samples, top_k <= TSLAM_OCTO_VIEWPOINT_MAX_SAMPLES, min_visible >= 1.
+ * Refused (TSLAM_E_INVALID): a NULL handle, camera or offsets, NULL outputs when n_clusters > 0, n_samples or top_k out
+ * of range, min_visible < 1, the camera checks of the view-gain calls, clearance as tslam_octo_travel_update refuses it,
+ * where tslam_octo_frontier_gather is refused, n_clusters different from the last update's cluster count, and more than
+ * 2^31 - 1 scoring items.  n_clusters == 0 is a no-op.  Asynchronous; changes neither the map nor any tracker state.
+ * Scratch (in the handle, grown on demand, freed by tslam_octo_destroy): 152 B per cluster, 28 B per frontier voxel, 4 B per candidate
+ * and 8 B per scoring item (n_samples * (ceil(frontier voxels / 64) + n_clusters) of them). */
+#define TSLAM_OCTO_VIEWPOINT_MAX_SAMPLES 1024
+int tslam_octo_frontier_viewpoints(tslam_octo_t* m, int32_t submap, const tslam_view_camera_t* cam, int32_t n_samples,
+                                   const float* offsets, float clearance, int32_t min_visible, int32_t top_k, int64_t n_clusters,
+                                   int32_t* count, int32_t* sample, int32_t* visible, float* pos, float* R9, void* stream);
+
 /* ----------------------------------------------------------------------------
  * Travel cost on a log-odds map (DESIGN.md section 7): per submap, as of one update, the geodesic cost G from a start
  * cell through known free space.  A cell is traversable iff it is inside the volume and FREE (known, L <= l_occ), and,

@@ -167,6 +167,8 @@ SIGNATURES = {
     "tslam_octo_frontier_clusters": (C.c_int, [_vp, _i32, _i64, _vp, C.POINTER(_i64), _vp]),
     "tslam_octo_view_gain_unknown": (C.c_int, [_vp, _i32, _i64, _vp, _vp, C.POINTER(ViewCamera), _vp, _vp, _vp]),
     "tslam_octo_view_gain_frontier": (C.c_int, [_vp, _i32, _i64, _vp, _vp, C.POINTER(ViewCamera), _i64, _vp, _vp, _vp, _vp]),
+    "tslam_octo_frontier_viewpoints": (C.c_int, [_vp, _i32, C.POINTER(ViewCamera), _i32, _vp, _f32, _i32, _i32, _i64, _vp, _vp, _vp,
+                                                 _vp, _vp, _vp]),
     "tslam_octo_travel_update": (C.c_int, [_vp, _i32, _vp, _f32, _f32, _vp, _vp]),
     "tslam_octo_travel_gather": (C.c_int, [_vp, _i32, _i64, _vp, _vp, C.POINTER(_i64), _vp]),
     "tslam_octo_travel_query": (C.c_int, [_vp, _i32, _i64, _vp, _vp, _vp]),

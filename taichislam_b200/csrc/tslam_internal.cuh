@@ -646,9 +646,24 @@ struct OcEsdfField {
   unsigned char free_cls, cls_mask;
 };
 int oc_esdf_field(tslam_octo* m, int32_t submap, const char* what, OcEsdfField* f);
+// The traversability rule of the travel-cost fields, for cell (i, j, k) with map word w at pool offset o = b * 512 + v:
+// inside the volume and FREE, and with clear (clearance > 0) also FREE at the last ESDF update, in a block it saw
+// (b < enb = *ef.nb_seen), with ESDF value >= clearance.  The travel classify and the viewpoint candidates test it.
+__device__ __forceinline__ bool oc_traversable(const OcGrid& g, const OcEsdfField& ef, int l_occ, float clearance, bool clear, int enb,
+                                               int b, size_t o, unsigned int w, int i, int j, int k) {
+  bool t = ts_in_bounds(g, i, j, k) && lo_known(w) && lo_val(w) <= l_occ;
+  if (t && clear) t = b < enb && (ef.cls[o] & ef.cls_mask) == ef.free_cls && ef.e[o] >= clearance;
+  return t;
+}
+// tslam_octo_travel.cu: the clearance check of every call that tests oc_traversable - finite and >= 0, and when > 0 a
+// readable occupancy ESDF of `submap` (into *ef) whose max_dist is >= clearance; *ef is zeroed when clearance == 0
+int oc_clearance_field(tslam_octo* m, int32_t submap, float clearance, const char* what, OcEsdfField* ef);
 // tslam_octo_frontier.cu: the m->fr_n rows (ijk, cluster ordinal) of the frontier set into idx[fr_n * 3], cluster[fr_n]
 // (DEVICE), in compact order, on st; the caller has checked m->fr_track
 int oc_frontier_rows(tslam_octo* m, int32_t* idx, int32_t* cluster, cudaStream_t st);
+// tslam_octo_frontier.cu: the m->fr_nc cluster records in label (ordinal) order into rec16[fr_nc * 16] (DEVICE), as
+// tslam_octo_frontier_clusters writes them, on st; the caller has checked m->fr_track
+int oc_frontier_records(tslam_octo* m, int64_t* rec16, cudaStream_t st);
 // tracker bits of g.err next to TS_ERR_POOL_FULL / TS_ERR_TABLE_FULL: the next synchronising call names every bit that is
 // set (oc_deferred, tslam_octo.cu)
 #define OC_ERR_VIEW_WINDOW 16  // g.err: a viewpoint-gain walk left its view's bitmap window (tslam_octo_view.cu)

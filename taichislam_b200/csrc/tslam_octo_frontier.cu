@@ -494,6 +494,14 @@ int oc_frontier_rows(tslam_octo* m, int32_t* idx, int32_t* cluster, cudaStream_t
   return TSLAM_OK;
 }
 
+int oc_frontier_records(tslam_octo* m, int64_t* rec16, cudaStream_t st) {
+  if (m->fr_nc > 0) {
+    k_octo_frontier_records<<<oc_grid((long long)m->fr_nc * OF_REC, 256, m->sm_count * 16), 256, 0, st>>>(of_clu(m), m->fr_nc, rec16);
+    TS_LAUNCH_CHECK(m);
+  }
+  return TSLAM_OK;
+}
+
 extern "C" int tslam_octo_frontier_gather(tslam_octo_t* m, int32_t submap, int64_t cap, int32_t* idx, int32_t* cluster, int64_t* n_out,
                                           void* stream) {
   if (!m || !n_out || cap < 0 || (cap > 0 && (!idx || !cluster))) return TSLAM_E_INVALID;

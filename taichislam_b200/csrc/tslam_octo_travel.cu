@@ -98,14 +98,6 @@ struct OtmAux {
 
 __device__ __forceinline__ float* otm_field(const OtmAux& a, int t, int s) { return a.G + ((size_t)t * a.S + s) * OC_B3; }
 
-// the traversability test for cell (i, j, k) with map word w at pool offset o = b * 512 + v
-__device__ __forceinline__ bool ot_traversable(const OcGrid& g, const OcEsdfField& ef, int l_occ, float clearance, bool clear, int enb,
-                                               int b, size_t o, unsigned int w, int i, int j, int k) {
-  bool t = ts_in_bounds(g, i, j, k) && lo_known(w) && lo_val(w) <= l_occ;
-  if (t && clear) t = b < enb && (ef.cls[o] & ef.cls_mask) == ef.free_cls && ef.e[o] >= clearance;
-  return t;
-}
-
 struct OtmTile {
   float G[OT_T3];
   int nbr[27];  // neighbour items of the same source (-1: none)
@@ -176,7 +168,7 @@ __global__ void __launch_bounds__(OT_THREADS) k_octo_travel_multi_classify(OcGri
     int cnt = 0;
     for (int v = threadIdx.x; v < OC_B3; v += blockDim.x) {
       const int i = bx * OC_B + (v >> 6), j = by * OC_B + ((v >> 3) & 7), k = bz * OC_B + (v & 7);
-      const bool t = ot_traversable(g, ef, l_occ, clearance, clear, enb, b, base + v, g.cnt[base + v], i, j, k);
+      const bool t = oc_traversable(g, ef, l_occ, clearance, clear, enb, b, base + v, g.cnt[base + v], i, j, k);
       const unsigned m = __ballot_sync(0xffffffffu, t);
       if ((threadIdx.x & 31) == 0) a.trav[(size_t)b * OT_WORDS + (v >> 5)] = m;
       cnt += t ? 1 : 0;
@@ -464,17 +456,27 @@ int oc_travel_free(tslam_octo* m) {
 #define OTM_UPDATE "tslam_octo_travel_multi_update"
 #define OT_FEATURE "a travel-cost field"
 
+static int ot_clearance_finite(float clearance, const char* what) {
+  if (std::isfinite(clearance) && clearance >= 0.0f) return TSLAM_OK;
+  ts_set_error("%s: clearance must be finite and >= 0 (got %g)", what, (double)clearance);
+  return TSLAM_E_INVALID;
+}
+
 // the clearance and max_cost checks of every travel update, and the occupancy ESDF the clearance test reads
 static int ot_params(tslam_octo* m, int32_t submap, float clearance, float max_cost, const char* what, OcEsdfField* ef) {
   const float cost_limit = std::ldexp(m->in.vs, 22);  // keeps G + vs > G for every kept value
-  if (!(std::isfinite(clearance) && clearance >= 0.0f)) {
-    ts_set_error("%s: clearance must be finite and >= 0 (got %g)", what, (double)clearance);
-    return TSLAM_E_INVALID;
-  }
+  int rc = ot_clearance_finite(clearance, what);
+  if (rc) return rc;
   if (!(std::isfinite(max_cost) && max_cost > 0.0f && max_cost <= cost_limit)) {
     ts_set_error("%s: max_cost must be finite, > 0 and <= 2^22 * voxel_scale = %g (got %g)", what, (double)cost_limit, (double)max_cost);
     return TSLAM_E_INVALID;
   }
+  return oc_clearance_field(m, submap, clearance, what, ef);
+}
+
+int oc_clearance_field(tslam_octo* m, int32_t submap, float clearance, const char* what, OcEsdfField* ef) {
+  int rc = ot_clearance_finite(clearance, what);
+  if (rc) return rc;
   memset(ef, 0, sizeof(*ef));
   if (clearance > 0.0f) {
     const int rc = oc_esdf_field(m, submap, what, ef);

@@ -220,6 +220,16 @@ class Octomap(BaseMap):
                     bbox_min=rec[:, 5:8].astype(np.float64) * vs, bbox_max=rec[:, 8:11].astype(np.float64) * vs,
                     direction=np.divide(d, norm, out=np.zeros_like(d), where=norm > 0))
 
+    def _camera(self, width, height, step, max_range):
+        """the simulated depth camera of the view calls: the depth intrinsics with a width x height image; step and
+        max_range default to recast_step and max_ray_length"""
+        if self.K_cam_dep is None:
+            raise ValueError("the view calls need the depth intrinsics: call set_dep_camera_intrinsic first")
+        K = self.K_cam_dep
+        return dict(fx=K[0], fy=K[4], cx=K[2], cy=K[5], width=int(width), height=int(height),
+                    step=int(self.recast_step if step is None else step),
+                    max_range=float(self.max_ray_length if max_range is None else max_range))
+
     def view_gain(self, pos, R, width, height, step=None, max_range=None, frontier=True, update=True):
         """What a depth camera would see from n candidate views of the active submap (positions pos [n,3], rotations R
         [n,3,3] in its map frame, integrate_depth's convention) -> dict(valid, unknown, frontier, frontier_per_cluster):
@@ -228,12 +238,7 @@ class Octomap(BaseMap):
         width x height image; step and max_range default to recast_step and max_ray_length.  update=True first runs
         frontier_update(), so frontiers and classes agree.  Torch CUDA tensors in -> torch tensors out; numpy -> numpy."""
         self._logodds_only("a viewpoint gain")
-        if self.K_cam_dep is None:
-            raise ValueError("view_gain needs the depth intrinsics: call set_dep_camera_intrinsic first")
-        K = self.K_cam_dep
-        cam = dict(fx=K[0], fy=K[4], cx=K[2], cy=K[5], width=int(width), height=int(height),
-                   step=int(self.recast_step if step is None else step),
-                   max_range=float(self.max_ray_length if max_range is None else max_range))
+        cam = self._camera(width, height, step, max_range)
         s = self._active()
         out = dict(frontier=None, frontier_per_cluster=None)
         if frontier and update:
@@ -340,6 +345,70 @@ class Octomap(BaseMap):
         path = self.travel_path_multi(0, g[order[0]]) if order.size else None
         return dict(order=order, unreachable=r["unreachable"] - 1, cost=r["cost"], leg_costs=leg, inf_legs=r["inf_legs"],
                     converged=bool(r["converged"][r["best"]]), path=path)
+
+    @staticmethod
+    def viewpoint_offsets(radii=(1.0, 1.5, 2.0), angles=16, heights=(0.0,)):
+        """The cylinder of candidate offsets [S,3] f32 around a cluster centroid: heights outermost, then radii, then
+        angles phi_j = 2 pi j / angles; each (r cos phi, r sin phi, h) computed in f64 and rounded to f32."""
+        phi = 2.0 * np.pi * np.arange(int(angles), dtype=np.float64) / float(int(angles))
+        rows = [(float(r) * np.cos(phi), float(r) * np.sin(phi), np.full(phi.shape, float(h))) for h in heights for r in radii]
+        if not rows:
+            return np.zeros((0, 3), np.float32)
+        return np.concatenate([np.stack(t, 1) for t in rows]).astype(np.float32)
+
+    def frontier_viewpoints(self, width, height, radii=(1.0, 1.5, 2.0), angles=16, heights=(0.0,), clearance=0.0, min_visible=1,
+                            top_k=1, max_range=None, step=None, update=True):
+        """Candidate sensor poses for every frontier cluster of the active submap (DESIGN.md section 7, "Frontier
+        viewpoints"): around each cluster's centroid the offsets of viewpoint_offsets(radii, angles, heights), each a
+        level camera facing the centroid, kept when its cell is traversable under travel_update's rule with `clearance`
+        and it sees at least min_visible of the cluster's frontier voxels (view_gain's test, camera as there), the best
+        top_k per cluster by that count (ties to the earlier sample).  update=True first runs frontier_update().  -> dict
+        of numpy arrays, rows in the order of get_frontier_clusters(min_voxels=1): count int32[nc] (slots used), pos
+        f32[nc,top_k,3], R f32[nc,top_k,3,3], yaw f64[nc,top_k] (atan2 of the viewing direction's y, x), visible
+        int32[nc,top_k], sample int32[nc,top_k] (row of the offsets; -1 in unused slots, whose pose is zero)."""
+        self._logodds_only("frontier viewpoints")
+        cam = self._camera(width, height, step, max_range)
+        self._travel_clearance(clearance)
+        if update:
+            self.frontier_update()
+        off = self.viewpoint_offsets(radii, angles, heights)
+        count, sample, visible, pos, R = self._h.frontier_viewpoints(off, cam, clearance, min_visible, top_k, submap=self._active())
+        yaw = np.arctan2(R[..., 0, 0].astype(np.float64), R[..., 0, 2].astype(np.float64))
+        return dict(count=count, pos=pos, R=R, yaw=yaw, visible=visible, sample=sample)
+
+    def plan_exploration(self, position, width, height, radii=(1.0, 1.5, 2.0), angles=16, heights=(0.0,), clearance=0.0,
+                         min_visible=1, top_k=1, max_range=None, step=None, max_cost=None, min_voxels=1, restarts=64, seed=0):
+        """One exploration planning step of the active submap from `position` (metres, map frame), composed of public
+        calls: frontier_viewpoints(...) (which runs frontier_update()), travel_update(position, clearance, max_cost) and
+        travel_cost of every kept viewpoint; per cluster with at least min_voxels voxels, its best-ranked viewpoint with a
+        finite travel cost; then exploration_tour(position, those viewpoints) -> dict(
+          clusters int64[m]: cluster ordinals (rows of get_frontier_clusters(min_voxels=1)) in visiting order;
+          pos f32[m,3], R f32[m,3,3], yaw f64[m], visible int32[m], sample int32[m]: their chosen viewpoints;
+          unreachable int64: the qualifying clusters with no reachable kept viewpoint, ascending;
+          cost, leg_costs, inf_legs, converged, path: as exploration_tour returns them).
+        Raises ValueError when more than 1023 clusters have a reachable viewpoint."""
+        self._logodds_only("an exploration plan")
+        fv = self.frontier_viewpoints(width, height, radii, angles, heights, clearance, min_visible, top_k, max_range, step)
+        size = self.get_frontier_clusters(min_voxels=1)["size"]
+        self.travel_update(position, clearance, max_cost)
+        nc, k = fv["sample"].shape
+        kept = np.arange(k)[None, :] < fv["count"][:, None]
+        cost = np.full((nc, k), np.inf, np.float32)
+        if kept.any():
+            cost[kept] = self.travel_cost(fv["pos"][kept])
+        ok = kept & np.isfinite(cost)
+        qual = size >= int(min_voxels)
+        goals = np.nonzero(qual & ok.any(1))[0]
+        if goals.size > 1023:
+            raise ValueError(f"plan_exploration tours at most 1023 clusters, but {goals.size} have a reachable viewpoint: raise "
+                             "min_voxels")
+        j = np.argmax(ok, axis=1)[goals]
+        tour = self.exploration_tour(position, fv["pos"][goals, j], clearance, max_cost, restarts, seed)
+        c, jo = goals[tour["order"]], j[tour["order"]]
+        unreachable = np.sort(np.concatenate([np.nonzero(qual & ~ok.any(1))[0], goals[tour["unreachable"]]])).astype(np.int64)
+        return dict(clusters=c.astype(np.int64), pos=fv["pos"][c, jo], R=fv["R"][c, jo], yaw=fv["yaw"][c, jo],
+                    visible=fv["visible"][c, jo], sample=fv["sample"][c, jo], unreachable=unreachable, cost=tour["cost"],
+                    leg_costs=tour["leg_costs"], inf_legs=tour["inf_legs"], converged=tour["converged"], path=tour["path"])
 
     def saveMap(self, path):  # :201-202 (stub in the reference)
         pass

@@ -308,6 +308,31 @@ class OctoHandle:
                                                         capi.stream_ptr()))
         return self._out(as_torch, valid.view(torch.bool), total, per)
 
+    def frontier_viewpoints(self, offsets, cam, clearance=0.0, min_visible=1, top_k=1, submap=0):
+        """The best top_k candidate views per frontier cluster of the last frontier_update (DESIGN.md section 7, "Frontier
+        viewpoints"): candidate s of cluster c sits at the cluster's f32 centroid plus offsets[s] (metres, [S,3],
+        1 <= S <= 1024), level and facing the centroid; it is kept when its cell is traversable under travel_update's
+        rule with `clearance` (> 0 reads the last esdf_update) and it sees at least min_visible of the cluster's frontier
+        voxels -> (count int32[nc], sample int32[nc,top_k], visible int32[nc,top_k], pos f32[nc,top_k,3],
+        R f32[nc,top_k,3,3]), rows in cluster ordinal order, slots at and beyond count[c] hold sample -1 and zeros.
+        Torch in -> torch out without a host synchronisation; numpy in -> numpy out."""
+        torch = self.torch
+        off = self._input(offsets, (-1, 3))
+        S, k = off.shape[0], int(top_k)
+        nc = self._count_fill(self._clusters_call(submap))
+        dev = off.device
+        count = torch.empty(nc, dtype=torch.int32, device=dev)
+        sample = torch.empty((nc, max(k, 0)), dtype=torch.int32, device=dev)
+        visible = torch.empty((nc, max(k, 0)), dtype=torch.int32, device=dev)
+        pos = torch.empty((nc, max(k, 0), 3), dtype=torch.float32, device=dev)
+        R = torch.empty((nc, max(k, 0), 3, 3), dtype=torch.float32, device=dev)
+        c = self.view_camera(cam)
+        ptr = (lambda t: capi.tptr(t) if nc else None)
+        capi.check(self.L.tslam_octo_frontier_viewpoints(self.h, int(submap), C.byref(c), S, capi.tptr(off), float(clearance),
+                                                         int(min_visible), k, nc, ptr(count), ptr(sample), ptr(visible), ptr(pos),
+                                                         ptr(R), capi.stream_ptr()))
+        return self._out(isinstance(offsets, torch.Tensor), count, sample, visible, pos, R)
+
     # -- travel cost on a log-odds map (tslam_octo_travel_*, DESIGN.md section 7) --------------------------------------
     def travel_limit(self):
         """The largest max_cost a travel update accepts: 2^22 * f32(voxel_scale)."""

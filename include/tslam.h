@@ -647,6 +647,39 @@ int tslam_octo_travel_multi_path(tslam_octo_t* m, int32_t submap, int64_t n, con
 int tslam_tour_open(int32_t n, const float* cost, int32_t restarts, uint64_t seed, int32_t max_passes, int32_t* tours,
                     int64_t* cost2, int32_t* passes, uint8_t* converged, int32_t* best, int32_t* info2, void* stream);
 
+/* ----------------------------------------------------------------------------
+ * SDF-to-SDF registration of TSDF submap pairs (DESIGN.md section 7, "Submap registration").  Pair p registers reference
+ * submap ref_submaps[p] of map A against reading submap read_submaps[p] of map B (A == B allowed; the voxel scales must
+ * be the same f32 bits).  T_p = (R, t) maps points of the reference submap's local frame into the reading submap's local
+ * frame (a global map's local frame is the world frame).
+ *   points     the voxels v of the reference submap in non-ghost blocks of A with obs = 1, W > 0, W >= min_weight and
+ *              |TSDF| <= band; p_v = (f32(i) vs, f32(j) vs, f32(k) vs), d_v = TSDF(v)
+ *   residual   x = R p_v + t in f32 (R, t rounded to f32 once per evaluation; pose_apply's operation order); D_B(x) the
+ *              trilinear interpolant of B's committed TSDF of the reading submap with the ESDF queries' low-corner and
+ *              interpolation rules, g its exact gradient; valid iff all 8 corners lie in the volume, in present
+ *              non-ghost blocks, with obs = 1 and W > 0; r = D_B(x) - d_v (f32); J = [g, x cross g] (f64, left
+ *              perturbation T <- exp(xi) T, xi = (rho, phi)); Huber weight w = 1 if |r| <= huber else huber / |r|
+ *   sums       H = sum w J J^T, b = sum w J r, cost = sum rho_huber(r), n_valid (f64, fixed order per pair)
+ *   solver     Levenberg-Marquardt (f64, host): (H + lam diag(max(H_ii, 1e-9 max_j H_jj))) xi = -b by Cholesky, lam
+ *              from 1e-4; a step is accepted when n_valid >= min_points and cost / n_valid decreases (lam / 10), else
+ *              rejected (lam * 10, pose kept).  Stops when |rho| < 1e-4 vs and |phi| < 1e-6 (converged), after
+ *              max_iters evaluations, or when the damped matrix is not positive definite.  max_iters = 0 returns the
+ *              normal equations at T0.
+ * Inputs (HOST): R0 f64[P,9] row-major, T0 f64[P,3], finite.  1 <= P <= TSLAM_REG_MAX_PAIRS; submaps in range; band and
+ * huber finite and > 0; min_weight finite; max_iters, min_points >= 0.  Outputs (HOST): R_out f64[P,9], T_out f64[P,3]
+ * (final pose), H_out f64[P,36], b_out f64[P,6] (at the final pose), cost2 f64[P,2] (initial, final cost), info5
+ * int64[P,5] (n_points, n_valid at the final pose, evaluations after the first, converged, status: 0 ok, 1 fewer than
+ * min_points valid points at T0 - not a call error).  A pair's result does not depend on the other pairs of the call.
+ * Flushes both maps, synchronises once per iteration, and writes no map word, flag, ESDF, mesh state or statistic other
+ * than A's kernel-launch counter (tslam_tsdf_launch_count), which counts the call's launches as it does every call's.
+ * Scratch in A's handle, grown geometrically, freed by tslam_tsdf_destroy: 28 B per pool block of A, 16 B per selected
+ * point, 232 B per 1024-point chunk of every pair, ~300 B per pair. */
+#define TSLAM_REG_MAX_PAIRS 1024
+int tslam_tsdf_register(tslam_tsdf_t* A, tslam_tsdf_t* B, int32_t n_pairs, const int32_t* ref_submaps, const int32_t* read_submaps,
+                        const double* R0, const double* T0, float band, float min_weight, float huber, int32_t max_iters,
+                        int32_t min_points, double* R_out, double* T_out, double* H_out, double* b_out, double* cost2,
+                        int64_t* info5, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -16,6 +16,7 @@ E_INVALID, E_CUDA, E_POOL_FULL, E_CAPACITY, E_NOGPU = -1, -2, -3, -4, -5
 MEM_DEVICE, MEM_HOST = 0, 1
 F_COMMIT = 1
 MAX_BATCH = 64
+REG_MAX_PAIRS = 1024
 ABI_VERSION = 6
 
 
@@ -177,6 +178,8 @@ SIGNATURES = {
     "tslam_octo_travel_multi_query": (C.c_int, [_vp, _i32, _i64, _vp, _vp, _vp]),
     "tslam_octo_travel_multi_path": (C.c_int, [_vp, _i32, _i64, _vp, _vp, _i32, _vp, _vp, _vp]),
     "tslam_tour_open": (C.c_int, [_i32, _vp, _i32, C.c_uint64, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "tslam_tsdf_register": (C.c_int, [_vp, _vp, _i32, _vp, _vp, _vp, _vp, _f32, _f32, _f32, _i32, _i32, _vp, _vp, _vp, _vp, _vp,
+                                      _vp, _vp]),
 }
 
 _lib = None

@@ -341,17 +341,53 @@ __device__ __forceinline__ int es_qblock(const P& p, int nb_seen, int bx, int by
   if constexpr (P::GHOSTS) return (b >= 0 && b < nb_seen && (p.ghosts || !p.g.ghost[b])) ? b : -1;
   else return (b >= 0 && b < nb_seen) ? b : -1;
 }
+// The 8 interpolation corners of the cell with low corner (i0, j0, k0) on blocks of edge 1 << S: e[dx*4 + dy*2 + dz] is
+// the value of corner (i0+dx, j0+dy, k0+dz).  find(bx, by, bz) -> pool index of a block, or -1 when it does not count;
+// each distinct corner block is looked up once (the corner cube spans 2, 4 or 8 blocks only where i0 is the last voxel
+// of its block on some axis).  read(off, e) -> whether the corner at pool offset off has a value, stored in e.  False
+// (e unspecified) when a block is refused or a corner has no value.  The ESDF queries and the SDF-to-SDF registration
+// (tslam_register.cu) read their corners through this one function.
+template <int S, class Find, class Read>
+__device__ __forceinline__ bool es_corners(int i0, int j0, int k0, Find find, Read read, float e[8]) {
+  constexpr int M = (1 << S) - 1, B3 = 1 << 3 * S;
+  const bool sx = (i0 & M) == M, sy = (j0 & M) == M, sz = (k0 & M) == M;
+  const int x0 = i0 >> S, y0 = j0 >> S, z0 = k0 >> S;
+  // b[dx*4 + dy*2 + dz]: block of corner (i0+dx, j0+dy, k0+dz); a corner that shares its block with a lower one reuses it
+  int b[8];
+  b[0] = find(x0, y0, z0);
+  b[1] = sz ? find(x0, y0, z0 + 1) : b[0];
+  b[2] = sy ? find(x0, y0 + 1, z0) : b[0];
+  b[3] = sy ? (sz ? find(x0, y0 + 1, z0 + 1) : b[2]) : b[1];
+  b[4] = sx ? find(x0 + 1, y0, z0) : b[0];
+  b[5] = sx ? (sz ? find(x0 + 1, y0, z0 + 1) : b[4]) : b[1];
+  b[6] = sx ? (sy ? find(x0 + 1, y0 + 1, z0) : b[4]) : b[2];
+  b[7] = sx ? (sy ? (sz ? find(x0 + 1, y0 + 1, z0 + 1) : b[6]) : b[5]) : b[3];
+  bool ok = true;
+#pragma unroll
+  for (int c = 0; c < 8; c++) {
+    ok &= b[c] >= 0;
+    e[c] = 0.0f;
+  }
+  if (ok) {
+#pragma unroll
+    for (int c = 0; c < 8; c++) {
+      const size_t off = (size_t)b[c] * B3 + es_voff<S>(i0 + (c >> 2), j0 + ((c >> 1) & 1), k0 + (c & 1));
+      ok &= read(off, e[c]);
+    }
+  }
+  return ok;
+}
+
 // Trilinear interpolation of the field over the 8 voxels around each point (voxel i centred at i*vs, submap-local frame)
-// and the exact partial derivatives of that interpolant, as of the last update.  One thread per point; each distinct
-// corner block is looked up once (the corner cube spans 2, 4 or 8 blocks only where i0 is the last voxel of its block
-// on some axis).  Invalid (NaN, valid = 0): a non-finite coordinate, a corner outside the volume, a corner in a block
+// and the exact partial derivatives of that interpolant, as of the last update.  One thread per point, corners from
+// es_corners.  Invalid (NaN, valid = 0): a non-finite coordinate, a corner outside the volume, a corner in a block
 // es_qblock refuses, a corner whose class at the last update has no value.  The body of each ESDF's query kernel, which
 // keeps the grid and the state as separate parameters: built around one rule parameter, the occupancy ESDF's query
 // compiles to 40 registers instead of 32 (6 instead of 8 CTAs per SM).
 template <class P>
 __device__ __forceinline__ void es_query(const P& p, long long n, const float* __restrict__ xyz, float* __restrict__ dist,
                                                   float* __restrict__ grad, uint8_t* __restrict__ valid) {
-  constexpr int S = P::SHIFT, M = (1 << S) - 1, B3 = 1 << 3 * S;
+  constexpr int S = P::SHIFT;
   const int nb_seen = *p.a.nb_seen;
   const float vs = p.vs, qnan = __int_as_float(0x7fc00000);
   for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < n; q += (long long)gridDim.x * blockDim.x) {
@@ -364,32 +400,15 @@ __device__ __forceinline__ void es_query(const P& p, long long n, const float* _
     if (ok) {
       const int i0 = c0[0], j0 = c0[1], k0 = c0[2];
       const float fx = __fsub_rn(u[0], (float)i0), fy = __fsub_rn(u[1], (float)j0), fz = __fsub_rn(u[2], (float)k0);
-      const bool sx = (i0 & M) == M, sy = (j0 & M) == M, sz = (k0 & M) == M;
-      const int x0 = i0 >> S, y0 = j0 >> S, z0 = k0 >> S;
-      // b[dx*4 + dy*2 + dz]: block of corner (i0+dx, j0+dy, k0+dz); a corner that shares its block with a lower one reuses it
-      int b[8];
-      b[0] = es_qblock(p, nb_seen, x0, y0, z0);
-      b[1] = sz ? es_qblock(p, nb_seen, x0, y0, z0 + 1) : b[0];
-      b[2] = sy ? es_qblock(p, nb_seen, x0, y0 + 1, z0) : b[0];
-      b[3] = sy ? (sz ? es_qblock(p, nb_seen, x0, y0 + 1, z0 + 1) : b[2]) : b[1];
-      b[4] = sx ? es_qblock(p, nb_seen, x0 + 1, y0, z0) : b[0];
-      b[5] = sx ? (sz ? es_qblock(p, nb_seen, x0 + 1, y0, z0 + 1) : b[4]) : b[1];
-      b[6] = sx ? (sy ? es_qblock(p, nb_seen, x0 + 1, y0 + 1, z0) : b[4]) : b[2];
-      b[7] = sx ? (sy ? (sz ? es_qblock(p, nb_seen, x0 + 1, y0 + 1, z0 + 1) : b[6]) : b[5]) : b[3];
       float e[8];
-#pragma unroll
-      for (int c = 0; c < 8; c++) {
-        ok &= b[c] >= 0;
-        e[c] = 0.0f;
-      }
-      if (ok) {
-#pragma unroll
-        for (int c = 0; c < 8; c++) {
-          const size_t off = (size_t)b[c] * B3 + es_voff<S>(i0 + (c >> 2), j0 + ((c >> 1) & 1), k0 + (c & 1));
-          ok &= P::valid(p.a.cls[off] & ES_CLS);
-          e[c] = p.field()[off];
-        }
-      }
+      ok = es_corners<S>(
+          i0, j0, k0, [&](int bx, int by, int bz) { return es_qblock(p, nb_seen, bx, by, bz); },
+          [&](size_t off, float& ev) {
+            const bool has = P::valid(p.a.cls[off] & ES_CLS);
+            ev = p.field()[off];
+            return has;
+          },
+          e);
       if (ok) esq_interp(e, fx, fy, fz, vs, d, gx, gy, gz);
       else d = gx = gy = gz = qnan;
     }

@@ -484,6 +484,12 @@ struct tslam_tsdf {
   int tile_cuts_set, tile_cuts_tiles[3], tile_cuts[3][17];  // data-driven tile boundaries of a tiled global map (tslam_dist.cu)
   int* tile_hist;      // device scratch of tslam_tsdf_dirty_hist (allocated on first use)
   TsMarchWs mw;        // block-binned ray march workspace (tslam_march.cu)
+  // SDF-to-SDF registration (tslam_tsdf_register, tslam_register.cu) with this map as the reference map: per pool block
+  // scratch of the point selection, and the point records and per-iteration sums (each grown geometrically)
+  void* reg_blk;
+  size_t reg_blk_bytes;
+  void* reg_pts;
+  size_t reg_pts_bytes;
   int march_mode;      // 0 = legacy k_raymarch, 1 = block-binned (default for untextured maps), env TSLAM_MARCH
   int march_verify;    // TSLAM_MARCH_VERIFY=1: every fast-path index is re-computed exactly, mismatches counted
   bool clamp_on_commit;

@@ -367,3 +367,38 @@ class DenseTSDF(BaseMap):
         """dense_esdf.py:569-571."""
         self.cvt_ESDF_to_voxels_slice(z)
         return self.export_ESDF_xyz.to_numpy(), self.export_ESDF.to_numpy()
+
+    def base_pose(self, submap_id):
+        """f64 (R, T) of a submap's local frame in the world frame: the stored base pose, the identity for a global map."""
+        if self.is_global_map:
+            return np.eye(3), np.zeros(3)
+        return np.array(self.submaps_base_R_np[submap_id], dtype=np.float64), np.array(self.submaps_base_T_np[submap_id], dtype=np.float64)
+
+    def register_submaps(self, ref_submaps, reading_submaps, reading=None, poses=None, band=None, min_weight=0.0, huber=None,
+                         max_iters=20, min_points=100):
+        """SDF-to-SDF registration of submap pairs on the GPU (tslam_tsdf_register, DESIGN.md section 7): pair p aligns
+        the near-surface voxels (|TSDF| <= band, W >= min_weight) of submap ref_submaps[p] of this map with the TSDF of
+        submap reading_submaps[p] of `reading` (default: this map) and returns the pose T_p = (R, T) that maps points of
+        the reference submap's local frame into the reading submap's local frame.  poses: initial (R [P,3,3], T [P,3]);
+        default base_b^-1 * base_a from the stored base poses in f64.  band defaults to 4 voxels (the weight ramp
+        theta, :219), huber to one voxel.  Flushes both maps.  -> one dict per pair: R, T, H (6x6 information at the
+        final pose, xi = (rho, phi) of the left perturbation), b, cost_init, cost, n_points, n_valid, iterations,
+        converged, status (1: fewer than min_points valid points at the initial pose)."""
+        reading = self if reading is None else reading
+        a = [int(s) for s in np.asarray(ref_submaps).reshape(-1)]
+        r = [int(s) for s in np.asarray(reading_submaps).reshape(-1)]
+        assert len(a) == len(r), "one reading submap per reference submap"
+        if poses is None:
+            R0, T0 = np.zeros((len(a), 3, 3)), np.zeros((len(a), 3))
+            for p, (sa, sb) in enumerate(zip(a, r)):
+                Ra, Ta = self.base_pose(sa)
+                Rb, Tb = reading.base_pose(sb)
+                R0[p], T0[p] = Rb.T @ Ra, Rb.T @ (Ta - Tb)
+        else:
+            R0, T0 = poses
+        self._flush()
+        reading._flush()
+        band = 4.0 * self.voxel_scale if band is None else band
+        out = self._h.register(reading._h, a, r, R0, T0, band, min_weight, huber, max_iters, min_points)
+        keys = ("R", "T", "H", "b", "cost_init", "cost", "n_points", "n_valid", "iterations", "converged", "status")
+        return [{k: (out[k][p].copy() if out[k].ndim > 1 else out[k][p].item()) for k in keys} for p in range(len(a))]

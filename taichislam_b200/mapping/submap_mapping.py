@@ -96,6 +96,30 @@ class SubmapMapping:
         if not from_remote:
             self.send_traj(used)
 
+    def align_submap(self, frame_id, reference_frame_id=None, apply=False, **opts):
+        """Register the submap created on `frame_id` against the submap of `reference_frame_id` (default: the submap
+        created just before it) with DenseTSDF.register_submaps, starting from their current world poses (the global
+        map's base poses).  Returns the registration result plus "world_R" / "world_T": the corrected world pose
+        base_ref * T of the frame's submap.  apply=True hands that pose to set_frame_poses, which moves the submap in
+        the global map.  opts: band, min_weight, huber, max_iters, min_points."""
+        assert self.submap_type is DenseTSDF, "submap registration needs TSDF submaps"
+        if reference_frame_id is None:
+            older = [f for f in self.submaps if self.submaps[f] < self.submaps[frame_id]]
+            if not older:
+                raise ValueError(f"frame {frame_id} has no earlier submap to align against")
+            reference_frame_id = max(older, key=lambda f: self.submaps[f])
+        sa, sb = self.submaps[frame_id], self.submaps[reference_frame_id]
+        g = self.global_map
+        Ra, Ta = g.submaps_base_R_np[sa], g.submaps_base_T_np[sa]
+        Rb, Tb = g.submaps_base_R_np[sb], g.submaps_base_T_np[sb]
+        pose0 = ((Rb.T @ Ra)[None], (Rb.T @ (Ta - Tb))[None])
+        res = self.submap_collection.register_submaps([sa], [sb], poses=pose0, **opts)[0]
+        res["world_R"] = Rb @ res["R"]
+        res["world_T"] = Rb @ res["T"] + Tb
+        if apply and res["status"] == 0:
+            self.set_frame_poses({frame_id: (res["world_R"], res["world_T"])})
+        return res
+
     def convert_by_pgo(self, frame_id, R, T):  # :162-169
         self.ego_motion_poses[frame_id] = (R, T)
         if self.last_frame_id is None:

@@ -349,6 +349,29 @@ class TsdfHandle:
         k = min(n, cap)
         return n, xyz[:k].cpu().numpy(), val[:k].cpu().numpy()
 
+    # -- SDF-to-SDF registration of submap pairs (tslam_tsdf_register) -------------------------------------
+    def register(self, reading, ref_submaps, read_submaps, R0, T0, band, min_weight=0.0, huber=None, max_iters=20,
+                 min_points=100):
+        """Register reference submaps of this map against reading submaps of `reading` (a TsdfHandle, may be self).
+        R0 [P,3,3], T0 [P,3]: initial poses (reference local frame -> reading local frame), f64.  huber defaults to the
+        voxel scale.  -> dict of numpy arrays: R [P,3,3], T [P,3], H [P,6,6], b [P,6], cost_init, cost [P], n_points,
+        n_valid, iterations [P] int64, converged, status [P] int64 (1: fewer than min_points valid points at R0, T0)."""
+        a = np.ascontiguousarray(np.asarray(ref_submaps, dtype=np.int32).reshape(-1))
+        r = np.ascontiguousarray(np.asarray(read_submaps, dtype=np.int32).reshape(-1))
+        P = a.shape[0]
+        R0 = np.ascontiguousarray(np.asarray(R0, dtype=np.float64).reshape(P, 9))
+        T0 = np.ascontiguousarray(np.asarray(T0, dtype=np.float64).reshape(P, 3))
+        huber = float(self.cfg.voxel_scale) if huber is None else float(huber)
+        R, T = np.zeros((P, 9)), np.zeros((P, 3))
+        H, b, cost2 = np.zeros((P, 36)), np.zeros((P, 6)), np.zeros((P, 2))
+        info = np.zeros((P, 5), np.int64)
+        capi.check(self.L.tslam_tsdf_register(self.h, reading.h, P, capi.np_ptr(a), capi.np_ptr(r), capi.np_ptr(R0), capi.np_ptr(T0),
+                                              float(band), float(min_weight), huber, int(max_iters), int(min_points), capi.np_ptr(R),
+                                              capi.np_ptr(T), capi.np_ptr(H), capi.np_ptr(b), capi.np_ptr(cost2), capi.np_ptr(info),
+                                              capi.stream_ptr()))
+        return dict(R=R.reshape(P, 3, 3), T=T, H=H.reshape(P, 6, 6), b=b, cost_init=cost2[:, 0], cost=cost2[:, 1],
+                    n_points=info[:, 0], n_valid=info[:, 1], iterations=info[:, 2], converged=info[:, 3], status=info[:, 4])
+
     # -- introspection --------------------------------------------------------------------
     def stats(self, clear=False):
         o = np.zeros(8, np.int64)

@@ -345,14 +345,24 @@ struct TsIntrin {
   int same_proj;   // color_same_proj
 };
 
-// per-frame bucket entry (dense_tsdf.py:64-70 new_pcl_count / new_pcl_sum_pos / new_pcl_z),
-// exact fixed-point sums (2^-20 m).  64-byte stride = two 32-byte sectors.
-struct __align__(64) TsBucket {
-  unsigned long long key;  // packed (bx,by,bz)+1, 0 = empty
-  long long sx, sy, sz, sd;
-  int cnt;
-  unsigned int cr, cg, cb;  // new_pcl_sum_color: exact integer channel sums
-  int pad[2];
+// per-frame bucket record (dense_tsdf.py:64-70 new_pcl_count / new_pcl_sum_pos / new_pcl_z), exact fixed-point sums
+// (2^-20 m) in one 32-byte sector.  cd = cnt << cnt_shift | sum(d): the depth sum is non-negative, and the launch picks
+// cnt_shift so that neither field can overflow into the other (ts_bucket_launch); a launch in which no shift can do that
+// keeps the counts in a plane of their own instead (TsBucketLaunch::cnt).  The opener of a bucket stores the
+// whole record; nobody clears it.  Textured maps keep the colour sums (new_pcl_sum_color, exact integer channel sums)
+// in a second plane of uint4 {r, g, b, 0} at the same slot.
+struct __align__(32) TsBucket {
+  long long sx, sy, sz;
+  unsigned long long cd;
+};
+// per-launch parameters of the bucket index (tslam_tsdf.cu, ts_bucket_launch)
+struct TsBucketLaunch {
+  unsigned long long etag;  // launch epoch in the entry's epoch field; 0 in clearing mode
+  int slot_bits;            // width of the slot + 1 field; 25 in clearing mode (no epoch field)
+  int cnt_shift;            // cd = cnt << cnt_shift | sum(d)
+  uint32_t* cnt;            // counts of the records when one bucket can collect more points than the word has room for
+                            // (cd = sum(d) alone); else null
+  uint32_t* bpos;           // clearing mode only: index entry of every opened record, zeroed by the consumer; else null
 };
 
 struct TsCounters {  // device-side statistics (tslam_tsdf_get_stats)
@@ -423,12 +433,18 @@ struct tslam_tsdf {
   TsIntrin in;
   size_t table_cap;
   // integrate workspace
-  // per-frame bucket grid, split in two: a small open-addressing INDEX (8 B per entry: record slot + 39-bit key) that
-  // the bucket kernel probes, and the 64-byte RECORDS with the exact sums (every warp of the bucket kernel owns 32 of them), filled in the order the buckets
-  // are opened - so the ray set-up reads and zeroes them in short runs instead of 64 random bytes per ray
+  // per-frame bucket grid, split in two: a small open-addressing INDEX (8 B per entry: launch epoch + record slot +
+  // 39-bit key) that the bucket kernel probes, and the 32-byte RECORDS with the exact sums (every warp of the bucket
+  // kernel owns 32 of them), filled in the order the buckets are opened - so the ray set-up reads them in short runs
   TsBucket* buckets;   // records [TSLAM_MAX_BATCH * bucket_cap]; frame f owns [f * bucket_cap, (f + 1) * bucket_cap)
+  uint4* bcol;         // colour sums of the records (texture_enabled only)
   unsigned long long* bidx;  // index [TSLAM_MAX_BATCH * bucket_cap]
   uint32_t bucket_cap; // power of two
+  int bk_slot_bits;    // width of the index entry's slot + 1 field (25: clearing mode, no epoch field)
+  unsigned int bk_epoch, bk_epoch_max;  // epoch of the last launch, 1 .. 2^(25 - bk_slot_bits) - 1
+  uint32_t* bpos;      // clearing mode only: [TSLAM_MAX_BATCH * bucket_cap] index entry of every opened record
+  uint32_t* bcnt;      // [TSLAM_MAX_BATCH * bucket_cap] record counts, for launches whose counts do not fit the packed
+                       // word; allocated only when the handle accepts such launches
   uint32_t* ray_list;  // [TSLAM_MAX_BATCH * max_rays_per_frame]
   uint32_t ray_list_cap;
   int* n_rays;         // device counter
@@ -760,7 +776,7 @@ int* ts_esdf_xmark(tslam_tsdf* m);
 int ts_march_alloc(tslam_tsdf* m);
 void ts_march_free(tslam_tsdf* m);
 int ts_march_setup(tslam_tsdf* m, cudaStream_t st, const TsBatch& batch, uint32_t bucket_shift);  // rays listed since the last call
-int ts_march_launch(tslam_tsdf* m, cudaStream_t st, const TsBatch& batch, uint32_t bucket_shift, cudaEvent_t* sub_ev);
+int ts_march_launch(tslam_tsdf* m, cudaStream_t st, const TsBatch& batch, uint32_t bucket_shift, const TsBucketLaunch& bl, cudaEvent_t* sub_ev);
 
 // Octomap host helpers shared by its trackers (tslam_octo.cu)
 // the arguments every tracker call checks first: a log-odds map (`feature` names what needs one), submap in range

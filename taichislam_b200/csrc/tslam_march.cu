@@ -53,25 +53,23 @@
 // ---------------------------------------------------------------------------
 // K2a: ray set-up (process_new_pcl :240-251), first stage of the counting walk: one bucket record -> unit direction,
 // length, weight, step count n, occupy flag (:248) and the 32-byte ray record + aux word the march kernels read,
-// stored at rays[r] / aux[r] and handed back in ra, rb, raux.  The bucket record and its index entry are handed back
-// zeroed (PCLroot.deactivate_all() / new_pcl_count = 0, :163, :270).
+// stored at rays[r] / aux[r] and handed back in ra, rb, raux.  The bucket record needs no clearing (its next opener
+// stores it whole); in clearing mode its index entry is handed back zeroed (PCLroot.deactivate_all(), :163).
 // ---------------------------------------------------------------------------
-__device__ __forceinline__ void ray_setup(const TsBatch& batch, const TsIntrin& in, const TsGrid& g, unsigned long long* btab, TsBucket* buckets,
-                                          unsigned long long* bidx, uint32_t bucket_shift, uint32_t id, uint32_t r, const TsMarchWs& w,
-                                          unsigned int& my_rays, unsigned int& my_fmax, float4& ra, float4& rb, uint32_t& raux) {
+__device__ __forceinline__ void ray_setup(const TsBatch& batch, const TsIntrin& in, const TsGrid& g, unsigned long long* btab, const TsBucket* buckets,
+                                          unsigned long long* bidx, uint32_t bucket_shift, const TsBucketLaunch& bl, uint32_t id, uint32_t r,
+                                          const TsMarchWs& w, unsigned int& my_rays, unsigned int& my_fmax, float4& ra, float4& rb, uint32_t& raux) {
   const float vs = in.vs;
   const uint32_t f = id >> bucket_shift;
-  uint4* q = reinterpret_cast<uint4*>(&buckets[id]);  // key sx | sy sz | sd cnt cr | cg cb pad
-  const uint4 q0 = q[0], q1 = q[1], q2 = q[2];
-  const unsigned long long ie = (unsigned long long)q0.x | ((unsigned long long)q0.y << 32);
-  if (ie) bidx[ie - 1ull] = 0ull;
-  const uint4 z4 = make_uint4(0, 0, 0, 0);
-  q[0] = z4; q[1] = z4; q[2] = z4; q[3] = z4;
-  const long long sx = (long long)((unsigned long long)q0.z | ((unsigned long long)q0.w << 32));
-  const long long sy = (long long)((unsigned long long)q1.x | ((unsigned long long)q1.y << 32));
-  const long long sz = (long long)((unsigned long long)q1.z | ((unsigned long long)q1.w << 32));
-  const long long sd = (long long)((unsigned long long)q2.x | ((unsigned long long)q2.y << 32));
-  const int cnt = (int)q2.z;
+  const uint4* q = reinterpret_cast<const uint4*>(&buckets[id]);  // sx sy | sz cd
+  const uint4 q0 = q[0], q1 = q[1];
+  if (bl.bpos) bidx[bl.bpos[id]] = 0ull;
+  const long long sx = (long long)((unsigned long long)q0.x | ((unsigned long long)q0.y << 32));
+  const long long sy = (long long)((unsigned long long)q0.z | ((unsigned long long)q0.w << 32));
+  const long long sz = (long long)((unsigned long long)q1.x | ((unsigned long long)q1.y << 32));
+  const unsigned long long cd = (unsigned long long)q1.z | ((unsigned long long)q1.w << 32);
+  const long long sd = bl.cnt ? (long long)cd : (long long)(cd & ((1ull << bl.cnt_shift) - 1ull));
+  const int cnt = bl.cnt ? (int)bl.cnt[id] : (int)(cd >> bl.cnt_shift);
   const TsFrame& fr = batch.f[f];
   struct { float ux, uy, uz, tx, ty, tz; int n, s; bool wide; } o;
   o.ux = o.uy = o.uz = o.tx = o.ty = o.tz = 0.0f;
@@ -217,8 +215,9 @@ __device__ __forceinline__ int seg_key(int blk, int cnt, uint32_t r) {
 // K2b-1: counting walk.  Ray set-up, then the segments: activates their blocks (rm_lookup) and counts them per (block,
 // class, replica).  Segments for the generic path (wide rays, blocks next to the volume, non-finite poses) are appended
 // to `gen` here and only here; segments in blocks far outside the volume are counted out of bounds.
-__global__ void __launch_bounds__(MS_THREADS, WC_MINB) k_seg_count(const __grid_constant__ TsBatch batch, TsIntrin in, TsGrid g, TsBucket* buckets,
-                                                                   unsigned long long* bidx, uint32_t bucket_shift, const uint32_t* __restrict__ ray_list,
+__global__ void __launch_bounds__(MS_THREADS, WC_MINB) k_seg_count(const __grid_constant__ TsBatch batch, TsIntrin in, TsGrid g, const TsBucket* buckets,
+                                                                   unsigned long long* bidx, uint32_t bucket_shift, TsBucketLaunch bl,
+                                                                   const uint32_t* __restrict__ ray_list,
                                                                    const int* __restrict__ n_rays_p, uint32_t ray_cap, TsMarchWs w, TsCounters* ctr) {
   __shared__ unsigned long long s_btab[RM_TAB];  // block coordinates -> pool index (direct mapped, rm_lookup)
   for (int e = threadIdx.x; e < RM_TAB; e += MS_THREADS) s_btab[e] = TS_EMPTY;
@@ -230,7 +229,7 @@ __global__ void __launch_bounds__(MS_THREADS, WC_MINB) k_seg_count(const __grid_
     const uint32_t r = base + threadIdx.x;
     float4 ra = make_float4(0.f, 0.f, 0.f, 0.f), rb = ra;
     uint32_t raux = 0u;
-    if (r < nme) ray_setup(batch, in, g, s_btab, buckets, bidx, bucket_shift, ray_list[r], r, w, my_rays, my_fmax, ra, rb, raux);
+    if (r < nme) ray_setup(batch, in, g, s_btab, buckets, bidx, bucket_shift, bl, ray_list[r], r, w, my_rays, my_fmax, ra, rb, raux);
     const SegRay q = seg_ray(batch, ra, rb, raux);
     int j = seg_generate(g, q, [&](int cnt, int j0, int bx, int by, int bz, int cls) {
       int key = -1;
@@ -809,11 +808,11 @@ int ts_march_setup(tslam_tsdf* m, cudaStream_t st, const TsBatch& batch, uint32_
 
 // sub_ev (profiling, may be null): 4 events recorded at the start, after counting walk + class + scan, the scattering
 // walk and the march kernels
-int ts_march_launch(tslam_tsdf* m, cudaStream_t st, const TsBatch& batch, uint32_t bucket_shift, cudaEvent_t* sub_ev) {
+int ts_march_launch(tslam_tsdf* m, cudaStream_t st, const TsBatch& batch, uint32_t bucket_shift, const TsBucketLaunch& bl, cudaEvent_t* sub_ev) {
   const int sms = m->sm_count;
   if (sub_ev) TS_CUDA(cudaEventRecord(sub_ev[0], st));
-  k_seg_count<<<sms * WC_MINB, MS_THREADS, 0, st>>>(batch, m->in, m->g, m->buckets, m->bidx, bucket_shift, m->ray_list, m->n_rays, m->ray_list_cap,
-                                                    m->mw, m->counters);
+  k_seg_count<<<sms * WC_MINB, MS_THREADS, 0, st>>>(batch, m->in, m->g, m->buckets, m->bidx, bucket_shift, bl, m->ray_list, m->n_rays,
+                                                    m->ray_list_cap, m->mw, m->counters);
   TS_LAUNCH_CHECK(m);
   k_seg_class<<<sms * 2, 256, 0, st>>>(m->g, m->mw);
   TS_LAUNCH_CHECK(m);

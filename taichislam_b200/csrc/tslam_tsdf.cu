@@ -5,6 +5,7 @@
 // Compiled with -fmad=false: the index-forming arithmetic must round exactly like
 // the strict-IEEE statement of the reference source (voxel indices are compared
 // bit-for-bit by the parity tests).
+#include <algorithm>
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
@@ -13,6 +14,7 @@
 #include <vector>
 #include <cuda_fp16.h>
 #include "tslam_internal.cuh"
+#include "tslam_bucket.cuh"
 
 // ---------------------------------------------------------------------------
 // error plumbing
@@ -39,13 +41,29 @@ extern "C" int tslam_device_count(void) {
   return n;
 }
 
-// bucket index entry: [record slot + 1 : 25][bx + 4096 : 13][by + 4096 : 13][bz + 4096 : 13]; 0 = empty
+// bucket index entry: [launch epoch : 25 - S][record slot + 1 : S][bx + 4096 : 13][by + 4096 : 13][bz + 4096 : 13],
+// S = TsBucketLaunch::slot_bits.  An entry whose epoch is not the launch's counts as empty, so nobody clears the index
+// between launches: the host clears it once when the epoch wraps (ts_bucket_launch).  A handle whose record slots
+// leave fewer than TS_BK_MIN_EPOCH_BITS for the epoch runs in clearing mode instead: S = 25, no epoch, and the ray
+// set-up zeroes the entry of every record it reads (TsBucketLaunch::bpos).
 #define BK_OFF 4096
 #define BK_KEY_BITS 39
 #define BK_KEY_MASK ((1ull << BK_KEY_BITS) - 1ull)
 #define BK_MAX_SLOTS ((1u << 25) - 2u)
 __device__ __forceinline__ unsigned long long bucket_key(int bx, int by, int bz) {
   return ((unsigned long long)(bx + BK_OFF) << 26) | ((unsigned long long)(by + BK_OFF) << 13) | (unsigned long long)(bz + BK_OFF);
+}
+__device__ __forceinline__ unsigned long long ld_acquire_u64(const unsigned long long* p) {
+  unsigned long long v;
+  asm volatile("ld.acquire.gpu.global.b64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
+  return v;
+}
+// release: the opener's record stores are visible to whoever reads the entry; acquire: a lane that loses the race
+// reads the winner's entry and then adds into the winner's record
+__device__ __forceinline__ unsigned long long cas_acq_rel_u64(unsigned long long* p, unsigned long long cmp, unsigned long long val) {
+  unsigned long long old;
+  asm volatile("atom.acq_rel.gpu.global.cas.b64 %0, [%1], %2, %3;" : "=l"(old) : "l"(p), "l"(cmp), "l"(val) : "memory");
+  return old;
 }
 
 // accumulate one unprojected point per lane into the frame's bucket grid.
@@ -54,13 +72,15 @@ __device__ __forceinline__ unsigned long long bucket_key(int bx, int by, int bz)
 // one set of reductions per distinct bucket per warp instead of per pixel.  The index maps the bucket's
 // voxel to a RECORD slot.  Slots need no allocator: every warp owns the 32 records [slot_base, slot_base + 32)
 // (it holds at most 32 distinct buckets), a probing lane brings the slot of its rank along and publishes it
-// with the key in ONE 64-bit CAS, so nobody ever waits for a slot; the slot of a lane that finds its bucket
-// already open stays unused (zero record).
+// with the key in ONE 64-bit CAS, so nobody ever waits for a slot.  The slot is private until that CAS publishes it,
+// so the lane STORES its warp's sums there first (the record needs no zeroing); lanes that find the bucket open add
+// into its record.  A lane that loses the race leaves its slot written but unnamed: nobody reads it.
 // Must be called by all 32 lanes; `valid` masks lanes without a point.  Returns the record slot when this
 // lane OPENED a bucket (the bucket becomes one ray; the caller appends it to the ray list), else -1.
 __device__ __forceinline__ int bucket_accumulate(bool valid, unsigned long long* idx, uint32_t cap_mask, uint32_t idx_base, TsBucket* recs,
-                                                 uint32_t rec_cap, uint32_t slot_base, float px, float py, float pz, float dep,
-                                                 float vs, bool agg_ok, int* err, bool tex = false, int cr = 0, int cg = 0, int cb = 0) {
+                                                 uint4* cols, uint32_t* cnts, uint32_t rec_cap, uint32_t slot_base, const TsBucketLaunch& bl, float px,
+                                                 float py, float pz, float dep, float vs, bool agg_ok, int* err, bool tex = false, int cr = 0,
+                                                 int cg = 0, int cb = 0) {
   const int bx = iroundf(px / vs), by = iroundf(py / vs), bz = iroundf(pz / vs);  // xyz_to_ijk mapping_common.py:240-243
   if (valid && ((unsigned)(bx + (BK_OFF - 1)) > 2u * (BK_OFF - 1) || (unsigned)(by + (BK_OFF - 1)) > 2u * (BK_OFF - 1) ||
                 (unsigned)(bz + (BK_OFF - 1)) > 2u * (BK_OFF - 1))) {
@@ -104,33 +124,47 @@ __device__ __forceinline__ int bucket_accumulate(bool valid, unsigned long long*
   if (!act) return -1;
   const uint32_t my_slot = slot_base + (uint32_t)__popc(amask & ((1u << (threadIdx.x & 31)) - 1u));
   if (my_slot >= rec_cap) { atomicOr(err, TS_ERR_RAYLIST_FULL); return -1; }
-  unsigned long long cur = ts_ld_volatile(&idx[h]);
+  // qd >= 0; with a count plane the word holds the depth sum alone
+  const unsigned long long cd = (cnts ? 0ull : (unsigned long long)cnt << bl.cnt_shift) + (unsigned long long)qd;
+  const unsigned long long emask = bl.slot_bits >= TS_BK_SLOT_FIELD ? 0ull : ~0ull << (BK_KEY_BITS + bl.slot_bits);
+  const unsigned long long smask = (1ull << bl.slot_bits) - 1ull;
+  const unsigned long long mine = bl.etag | ((unsigned long long)(my_slot + 1) << BK_KEY_BITS) | key;
+  unsigned long long cur = ld_acquire_u64(&idx[h]);
+  bool stored = false;
   int slot = -1, fresh = -1;
   for (uint32_t probe = 0; probe <= cap_mask; ++probe) {
-    if (cur == 0ull) {
-      const unsigned long long prev = atomicCAS(&idx[h], 0ull, ((unsigned long long)(my_slot + 1) << BK_KEY_BITS) | key);
-      if (prev == 0ull) {  // this point opened the bucket: it becomes one ray
-        slot = fresh = (int)my_slot;
-        recs[slot].key = (unsigned long long)(idx_base + h) + 1ull;  // where the consumer clears the index
-        break;
+    if (cur == 0ull || (cur & emask) != bl.etag) {  // empty, or left by an earlier launch
+      if (!stored) {
+        uint4* q = reinterpret_cast<uint4*>(&recs[my_slot]);
+        q[0] = make_uint4((unsigned)qx, (unsigned)((unsigned long long)qx >> 32), (unsigned)qy, (unsigned)((unsigned long long)qy >> 32));
+        q[1] = make_uint4((unsigned)qz, (unsigned)((unsigned long long)qz >> 32), (unsigned)cd, (unsigned)(cd >> 32));
+        if (cols) cols[my_slot] = make_uint4((unsigned)cr, (unsigned)cg, (unsigned)cb, 0u);  // textured map: zero without colours
+        if (cnts) cnts[my_slot] = (unsigned)cnt;
+        stored = true;
       }
-      cur = prev;
+      const unsigned long long prev = cas_acq_rel_u64(&idx[h], cur, mine);
+      if (prev == cur) {  // this point opened the bucket: it becomes one ray
+        fresh = (int)my_slot;
+        if (bl.bpos) bl.bpos[idx_base + my_slot] = idx_base + h;  // where the consumer clears the index
+        return fresh;
+      }
+      cur = prev;  // the winner's entry, of this launch
     }
-    if ((cur & BK_KEY_MASK) == key) { slot = (int)(cur >> BK_KEY_BITS) - 1; break; }
+    if ((cur & BK_KEY_MASK) == key) { slot = (int)((cur >> BK_KEY_BITS) & smask) - 1; break; }
     h = (h + 1) & cap_mask;
-    cur = ts_ld_volatile(&idx[h]);
+    cur = ld_acquire_u64(&idx[h]);
   }
   if (slot < 0) { atomicOr(err, TS_ERR_TABLE_FULL); return -1; }
   TsBucket* b = &recs[slot];
-  red_add_u32((unsigned int*)&b->cnt, (unsigned int)cnt);
   red_add_u64((unsigned long long*)&b->sx, (unsigned long long)qx);
   red_add_u64((unsigned long long*)&b->sy, (unsigned long long)qy);
   red_add_u64((unsigned long long*)&b->sz, (unsigned long long)qz);
-  red_add_u64((unsigned long long*)&b->sd, (unsigned long long)qd);
+  red_add_u64(&b->cd, cd);
+  if (cnts) red_add_u32(&cnts[slot], (unsigned int)cnt);
   if (tex) {  // new_pcl_sum_color += rgb (dense_tsdf.py:233-234), exact integer sums
-    red_add_u32(&b->cr, (unsigned int)cr);
-    red_add_u32(&b->cg, (unsigned int)cg);
-    red_add_u32(&b->cb, (unsigned int)cb);
+    red_add_u32(&cols[slot].x, (unsigned int)cr);
+    red_add_u32(&cols[slot].y, (unsigned int)cg);
+    red_add_u32(&cols[slot].z, (unsigned int)cb);
   }
   return fresh;
 }
@@ -167,8 +201,8 @@ __device__ __forceinline__ void append_rays_cta(int fresh_slot, uint32_t tab_bas
 // ---------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) k_bucket_depth(const uint16_t* __restrict__ depth, int frame_stride, int row_mul, int w, int hh, int ww,
                                                        const __grid_constant__ TsBatch batch, TsIntrin in, int agg_ok,
-                                                       TsBucket* buckets, unsigned long long* bidx, uint32_t bucket_cap,
-                                                       uint32_t* ray_list, int* n_rays, uint32_t ray_cap, TsCounters* ctr, int* err,
+                                                       TsBucket* buckets, uint4* bcol, unsigned long long* bidx, uint32_t bucket_cap,
+                                                       TsBucketLaunch bl, uint32_t* ray_list, int* n_rays, uint32_t ray_cap, TsCounters* ctr, int* err,
                                                        const uint8_t* __restrict__ tex, int th, int tw) {
   const int tz = blockIdx.z;    // frame of the batch = its bucket grid
   const int f = tz;
@@ -203,15 +237,17 @@ __global__ void __launch_bounds__(256) k_bucket_depth(const uint16_t* __restrict
   }
   const unsigned nv = __popc(__ballot_sync(0xffffffffu, valid));
   const int fresh = bucket_accumulate(valid, bidx + (size_t)tz * bucket_cap, bucket_cap - 1, (uint32_t)tz * bucket_cap, buckets + (size_t)tz * bucket_cap,
-                                      bucket_cap, ((blockIdx.y * gridDim.x + blockIdx.x) * 8u + (uint32_t)wid) * 32u, px, py, pz, dep, in.vs, agg_ok != 0, err, tex != nullptr, cr, cg, cb);
+                                      bcol ? bcol + (size_t)tz * bucket_cap : nullptr, bl.cnt ? bl.cnt + (size_t)tz * bucket_cap : nullptr, bucket_cap,
+                                      ((blockIdx.y * gridDim.x + blockIdx.x) * 8u + (uint32_t)wid) * 32u, bl, px, py, pz, dep, in.vs, agg_ok != 0,
+                                      err, tex != nullptr, cr, cg, cb);
   append_rays_cta(fresh, (uint32_t)tz * bucket_cap, nv, ray_list, n_rays, ray_cap, ctr, err);
   if (blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) atomicAdd(&ctr->n_px, (unsigned long long)(hh * ww));
 }
 
 // K1b: point cloud -> buckets.  recast_pcl_to_map_kernel (dense_tsdf.py:167-185).
 __global__ void __launch_bounds__(256) k_bucket_points(const float* __restrict__ xyz, int n, const __grid_constant__ TsBatch batch,
-                                                        TsIntrin in, int agg_ok, TsBucket* buckets, unsigned long long* bidx,
-                                                        uint32_t bucket_cap, uint32_t rec_cap, uint32_t* ray_list, int* n_rays, uint32_t ray_cap, TsCounters* ctr,
+                                                        TsIntrin in, int agg_ok, TsBucket* buckets, uint4* bcol, unsigned long long* bidx,
+                                                        uint32_t bucket_cap, uint32_t rec_cap, TsBucketLaunch bl, uint32_t* ray_list, int* n_rays, uint32_t ray_cap, TsCounters* ctr,
                                                         int* err, const uint8_t* __restrict__ rgb) {
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
   int cr = 0, cg = 0, cb = 0;
@@ -228,8 +264,8 @@ __global__ void __launch_bounds__(256) k_bucket_points(const float* __restrict__
     if (rgb) { cr = rgb[3 * (size_t)t]; cg = rgb[3 * (size_t)t + 1]; cb = rgb[3 * (size_t)t + 2]; }  // :179-182
   }
   const unsigned nv = __popc(__ballot_sync(0xffffffffu, valid));
-  const int fresh = bucket_accumulate(valid, bidx, bucket_cap - 1, 0u, buckets, rec_cap, (uint32_t)(t & ~31), px, py, pz, len, in.vs, agg_ok != 0, err,
-                                      rgb != nullptr, cr, cg, cb);  // :183/:185
+  const int fresh = bucket_accumulate(valid, bidx, bucket_cap - 1, 0u, buckets, bcol, bl.cnt, rec_cap, (uint32_t)(t & ~31), bl, px, py, pz, len, in.vs,
+                                      agg_ok != 0, err, rgb != nullptr, cr, cg, cb);  // :183/:185
   append_rays_cta(fresh, 0u, nv, ray_list, n_rays, ray_cap, ctr, err);
   if (t == 0) atomicAdd(&ctr->n_px, (unsigned long long)n);
 }
@@ -268,8 +304,8 @@ __device__ __forceinline__ void win_add(unsigned int* lo, int* hi, int x) {
 
 template <bool TEX>
 __global__ void __launch_bounds__(RM_THREADS, 2) k_raymarch(const __grid_constant__ TsBatch batch, TsIntrin in, TsGrid g,
-                                                              TsBucket* buckets, unsigned long long* bidx, uint32_t bucket_shift,
-                                                              const uint32_t* __restrict__ ray_list, const int* __restrict__ n_rays_p, uint32_t ray_cap,
+                                                              const TsBucket* buckets, const uint4* bcol, unsigned long long* bidx,
+                                                              uint32_t bucket_shift, TsBucketLaunch bl, const uint32_t* __restrict__ ray_list, const int* __restrict__ n_rays_p, uint32_t ray_cap,
                                                               TsCounters* ctr) {
   extern __shared__ __align__(16) unsigned int win[];  // [4][4096]: A.lo, A.hi, B.lo, B.hi
   unsigned int* const w_alo = win;
@@ -311,16 +347,14 @@ __global__ void __launch_bounds__(RM_THREADS, 2) k_raymarch(const __grid_constan
     if (live) {
       const uint32_t id = ray_list[r];
       f = id >> bucket_shift;
-      TsBucket* bk = &buckets[id];
-      cnt = bk->cnt;
-      sx = bk->sx; sy = bk->sy; sz = bk->sz; sd = bk->sd;
-      if (TEX) { ccr = bk->cr; ccg = bk->cg; ccb = bk->cb; }
-      // PCLroot.deactivate_all() / new_pcl_count = 0 (:163, :270): hand the record and its index entry back zeroed
-      const unsigned long long ie = bk->key;
-      if (ie) bidx[ie - 1ull] = 0ull;
-      const uint4 z4 = make_uint4(0, 0, 0, 0);
-      uint4* q = reinterpret_cast<uint4*>(bk);
-      q[0] = z4; q[1] = z4; q[2] = z4; q[3] = z4;
+      const TsBucket* bk = &buckets[id];
+      sx = bk->sx; sy = bk->sy; sz = bk->sz;
+      const unsigned long long cd = bk->cd;
+      cnt = bl.cnt ? (int)bl.cnt[id] : (int)(cd >> bl.cnt_shift);
+      sd = bl.cnt ? (long long)cd : (long long)(cd & ((1ull << bl.cnt_shift) - 1ull));
+      if (TEX) { const uint4 c = bcol[id]; ccr = c.x; ccg = c.y; ccb = c.z; }
+      // PCLroot.deactivate_all() (:163): clearing mode hands the index entry back zeroed
+      if (bl.bpos) bidx[bl.bpos[id]] = 0ull;
       live = cnt > 0;  // :240
     }
     float mx = 0.f, my = 0.f, mz = 0.f, ux = 0.f, uy = 0.f, uz = 0.f, Tx = 0.f, Ty = 0.f, Tz = 0.f, Px = 0.f, Py = 0.f, Pz = 0.f,
@@ -692,6 +726,11 @@ static void ts_fill_intrin(tslam_tsdf* m) {
   m->in.tex = c.texture_enabled;
 }
 
+// largest depth (or point-cloud ray length) a bucket sum can add, in metres
+static double ts_bucket_dmax(const tslam_tsdf* m) {
+  return std::max((double)m->in.dmax_mm / 1000.0, (double)m->in.max_ray) * (1.0 + 1e-6);
+}
+
 extern "C" int tslam_tsdf_create(const tslam_tsdf_config_t* cfg, tslam_tsdf_t** out) {
   if (!cfg || !out) { ts_set_error("null argument"); return TSLAM_E_INVALID; }
   *out = nullptr;
@@ -782,9 +821,17 @@ extern "C" int tslam_tsdf_create(const tslam_tsdf_config_t* cfg, tslam_tsdf_t** 
     return TSLAM_E_INVALID;
   }
   TS_CUDA(cudaMalloc(&m->buckets, (size_t)TSLAM_MAX_BATCH * m->bucket_cap * sizeof(TsBucket)));
-  TS_CUDA(cudaMemset(m->buckets, 0, (size_t)TSLAM_MAX_BATCH * m->bucket_cap * sizeof(TsBucket)));
+  if (m->cfg.texture_enabled) TS_CUDA(cudaMalloc(&m->bcol, (size_t)TSLAM_MAX_BATCH * m->bucket_cap * sizeof(uint4)));
   TS_CUDA(cudaMalloc(&m->bidx, (size_t)TSLAM_MAX_BATCH * m->bucket_cap * 8));
   TS_CUDA(cudaMemset(m->bidx, 0, (size_t)TSLAM_MAX_BATCH * m->bucket_cap * 8));
+  m->bk_slot_bits = ts_bucket_slot_bits(m->bucket_cap, (uint32_t)m->cfg.max_points);
+  if (m->bk_slot_bits >= TS_BK_SLOT_FIELD) TS_CUDA(cudaMalloc(&m->bpos, (size_t)TSLAM_MAX_BATCH * m->bucket_cap * 4));
+  m->bk_epoch_max = m->bk_slot_bits >= TS_BK_SLOT_FIELD ? 0u : (1u << (TS_BK_SLOT_FIELD - m->bk_slot_bits)) - 1u;
+  m->bk_epoch = 0;
+  {  // a launch in which one bucket can collect more points than the packed count word holds keeps its counts in a plane
+    const uint64_t n_max = std::max((uint64_t)m->cfg.max_image_pixels / ((uint64_t)step * step), (uint64_t)m->cfg.max_points);
+    if (ts_bucket_cnt_shift(n_max, ts_bucket_dmax(m)) < 0) TS_CUDA(cudaMalloc(&m->bcnt, (size_t)TSLAM_MAX_BATCH * m->bucket_cap * 4));
+  }
   m->ray_list_cap = (uint32_t)((size_t)TSLAM_MAX_BATCH * sampled);
   if (m->ray_list_cap < (uint32_t)m->cfg.max_points) m->ray_list_cap = (uint32_t)m->cfg.max_points;
   TS_CUDA(cudaMalloc(&m->ray_list, (size_t)m->ray_list_cap * 4));
@@ -880,7 +927,11 @@ extern "C" int tslam_tsdf_destroy(tslam_tsdf_t* m) {
   if (m->tex_stage) cudaFree(m->tex_stage);
   if (m->rgb_stage) cudaFree(m->rgb_stage);
   cudaFree(g.ghost); cudaFree(g.dirty_flag); cudaFree(g.esdf_dirty); cudaFree(m->blk_stamp); cudaFree(g.dirty_list); cudaFree(m->scratch_i);
-  cudaFree(m->buckets); cudaFree(m->bidx); cudaFree(m->ray_list); cudaFree(m->depth_stage); cudaFree(m->points_stage);
+  cudaFree(m->buckets); cudaFree(m->bidx); cudaFree(m->ray_list);
+  if (m->bcol) cudaFree(m->bcol);
+  if (m->bpos) cudaFree(m->bpos);
+  if (m->bcnt) cudaFree(m->bcnt);
+  cudaFree(m->depth_stage); cudaFree(m->points_stage);
   cudaStreamDestroy(m->copy_stream);
   if (m->h_ring) cudaFreeHost(m->h_ring);
   for (int i = 0; i < 2; i++) { cudaEventDestroy(m->ev_copied[i]); cudaEventDestroy(m->ev_free[i]); }
@@ -1054,6 +1105,34 @@ static int ts_seq_renorm(tslam_tsdf* m, cudaStream_t st, int n_new) {
   return TSLAM_OK;
 }
 
+// Bucket index and record parameters of the next launch, in which one bucket can collect at most n points.  Advances
+// the launch epoch, and clears the index when it wraps.
+static int ts_bucket_launch(tslam_tsdf* m, cudaStream_t st, uint64_t n, TsBucketLaunch& bl) {
+  const int shift = ts_bucket_cnt_shift(n, ts_bucket_dmax(m));
+  bl.cnt_shift = shift < 0 ? 0 : shift;
+  bl.cnt = shift < 0 ? m->bcnt : nullptr;
+  if (shift < 0 && !m->bcnt) {  // the plane is sized at create time for the largest launch the handle accepts
+    ts_set_error("bucket count plane missing for a launch of %llu points", (unsigned long long)n);
+    return TSLAM_E_INVALID;
+  }
+  bl.slot_bits = m->bk_slot_bits;
+  bl.bpos = m->bpos;
+  bl.etag = 0ull;
+  if (m->bpos) return TSLAM_OK;
+  if (++m->bk_epoch > m->bk_epoch_max) {
+    TS_CUDA(cudaMemsetAsync(m->bidx, 0, (size_t)TSLAM_MAX_BATCH * m->bucket_cap * 8, st));
+    m->bk_epoch = 1;
+  }
+  bl.etag = (unsigned long long)m->bk_epoch << (BK_KEY_BITS + m->bk_slot_bits);
+  return TSLAM_OK;
+}
+// A launch that stops between the bucket kernel and the ray set-up leaves index entries behind: harmless with epochs
+// (the next launch has a new one), cleared here in clearing mode.
+static int ts_bucket_abandon(tslam_tsdf* m, cudaStream_t st, int rc) {
+  if (m->bpos) TS_CUDA(cudaMemsetAsync(m->bidx, 0, (size_t)TSLAM_MAX_BATCH * m->bucket_cap * 8, st));
+  return rc;
+}
+
 static int ts_integrate_depth_impl(tslam_tsdf_t* m, const uint16_t* depth, int mem, int32_t n_frames, int32_t h, int32_t w,
                                    const float* R9s, const float* T3s, const int32_t* submap_ids, int flags, void* stream, int rows_compacted,
                                    const uint8_t* tex, int th, int tw) {
@@ -1095,21 +1174,23 @@ static int ts_integrate_depth_impl(tslam_tsdf_t* m, const uint16_t* depth, int m
       ts_set_error("frame %dx%d (sampled %dx%d) has too many partial pixel tiles for max_image_pixels=%d", h, w, hh, ww, m->cfg.max_image_pixels);
       return TSLAM_E_INVALID;
     }
-    k_bucket_depth<<<grid1, 256, 0, st>>>(src, rows_stored * w, rows_compacted ? 1 : step, w, hh, ww, batch, m->in, agg_ok, m->buckets, m->bidx,
-                                          m->bucket_cap, m->ray_list, m->n_rays, m->ray_list_cap, m->counters, m->g.err, tsrc, th, tw);
+    TsBucketLaunch bl;
+    { int rcb = ts_bucket_launch(m, st, (uint64_t)hh * ww, bl); if (rcb) return rcb; }
+    k_bucket_depth<<<grid1, 256, 0, st>>>(src, rows_stored * w, rows_compacted ? 1 : step, w, hh, ww, batch, m->in, agg_ok, m->buckets, m->bcol,
+                                          m->bidx, m->bucket_cap, bl, m->ray_list, m->n_rays, m->ray_list_cap, m->counters, m->g.err, tsrc, th, tw);
     TS_LAUNCH_CHECK(m);
     if (pe) TS_CUDA(cudaEventRecord(pe[1], st));
     if (!m->g.cword && m->march_mode) {
       int rcs = ts_march_setup(m, st, batch, bshift);
-      if (rcs) return rcs;
-      int rcm = ts_march_launch(m, st, batch, bshift, pe ? pe + 4 : nullptr);
-      if (rcm) return rcm;
+      if (rcs) return ts_bucket_abandon(m, st, rcs);
+      int rcm = ts_march_launch(m, st, batch, bshift, bl, pe ? pe + 4 : nullptr);
+      if (rcm) return ts_bucket_abandon(m, st, rcm);
     } else if (m->g.cword) {
-      k_raymarch<true><<<m->sm_count, RM_THREADS, RM_SMEM_TEX, st>>>(batch, m->in, m->g, m->buckets, m->bidx, bshift, m->ray_list, m->n_rays,
-                                                                     m->ray_list_cap, m->counters);
+      k_raymarch<true><<<m->sm_count, RM_THREADS, RM_SMEM_TEX, st>>>(batch, m->in, m->g, m->buckets, m->bcol, m->bidx, bshift, bl, m->ray_list,
+                                                                     m->n_rays, m->ray_list_cap, m->counters);
     } else {
-      k_raymarch<false><<<(m->sm_count - m->rm_reserve) * 2, RM_THREADS, RM_SMEM, st>>>(batch, m->in, m->g, m->buckets, m->bidx, bshift, m->ray_list, m->n_rays,
-                                                                                     m->ray_list_cap, m->counters);
+      k_raymarch<false><<<(m->sm_count - m->rm_reserve) * 2, RM_THREADS, RM_SMEM, st>>>(batch, m->in, m->g, m->buckets, m->bcol, m->bidx, bshift, bl,
+                                                                                     m->ray_list, m->n_rays, m->ray_list_cap, m->counters);
     }
     TS_LAUNCH_CHECK(m);
     if (pe) TS_CUDA(cudaEventRecord(pe[2], st));
@@ -1156,25 +1237,27 @@ extern "C" int tslam_tsdf_integrate_points_rgb(tslam_tsdf_t* m, const float* xyz
   }
   const uint32_t bshift = 31;  // every ray belongs to batch.f[0]
   const uint32_t cap_total = (uint32_t)TSLAM_MAX_BATCH * m->bucket_cap;  // power of two
-  const uint32_t rec_cap = cap_total < BK_MAX_SLOTS ? cap_total : BK_MAX_SLOTS;
+  const uint32_t rec_cap = ((uint32_t)n + 31u) & ~31u;  // a warp's slots start at its first point
   cudaEvent_t* pe = m->profiling ? m->ev + TS_PROF_EV * (m->prof_launches % TS_PROF_RING) : nullptr;
     if (pe) TS_CUDA(cudaEventRecord(pe[0], st));
   const int agg_ok = m->cfg.max_ray_length < 30.0 ? 1 : 0;  // 32-lane int32 sums: |p| <= max_ray * sqrt(1 + tan^2) < 64 m even at 60 deg half-FOV
-  k_bucket_points<<<(n + 255) / 256, 256, 0, st>>>(src, n, batch, m->in, agg_ok, m->buckets, m->bidx, cap_total, rec_cap, m->ray_list, m->n_rays,
-                                                    m->ray_list_cap, m->counters, m->g.err, csrc);
+  TsBucketLaunch bl;
+  { int rcb = ts_bucket_launch(m, st, (uint64_t)n, bl); if (rcb) return rcb; }
+  k_bucket_points<<<(n + 255) / 256, 256, 0, st>>>(src, n, batch, m->in, agg_ok, m->buckets, m->bcol, m->bidx, cap_total, rec_cap, bl, m->ray_list,
+                                                    m->n_rays, m->ray_list_cap, m->counters, m->g.err, csrc);
   TS_LAUNCH_CHECK(m);
   if (pe) TS_CUDA(cudaEventRecord(pe[1], st));
   if (m->g.cword)
-    k_raymarch<true><<<m->sm_count, RM_THREADS, RM_SMEM_TEX, st>>>(batch, m->in, m->g, m->buckets, m->bidx, bshift, m->ray_list, m->n_rays,
-                                                                   m->ray_list_cap, m->counters);
+    k_raymarch<true><<<m->sm_count, RM_THREADS, RM_SMEM_TEX, st>>>(batch, m->in, m->g, m->buckets, m->bcol, m->bidx, bshift, bl, m->ray_list,
+                                                                   m->n_rays, m->ray_list_cap, m->counters);
   else if (m->march_mode) {
     int rcm = ts_march_setup(m, st, batch, bshift);
-    if (rcm) return rcm;
-    rcm = ts_march_launch(m, st, batch, bshift, pe ? pe + 4 : nullptr);
-    if (rcm) return rcm;
+    if (rcm) return ts_bucket_abandon(m, st, rcm);
+    rcm = ts_march_launch(m, st, batch, bshift, bl, pe ? pe + 4 : nullptr);
+    if (rcm) return ts_bucket_abandon(m, st, rcm);
   } else
-    k_raymarch<false><<<m->sm_count * 2, RM_THREADS, RM_SMEM, st>>>(batch, m->in, m->g, m->buckets, m->bidx, bshift, m->ray_list, m->n_rays,
-                                                                    m->ray_list_cap, m->counters);
+    k_raymarch<false><<<m->sm_count * 2, RM_THREADS, RM_SMEM, st>>>(batch, m->in, m->g, m->buckets, m->bcol, m->bidx, bshift, bl, m->ray_list,
+                                                                    m->n_rays, m->ray_list_cap, m->counters);
   TS_LAUNCH_CHECK(m);
   if (pe) TS_CUDA(cudaEventRecord(pe[2], st));
   k_reset_counters<<<1, 1, 0, st>>>(m->n_rays, nullptr);

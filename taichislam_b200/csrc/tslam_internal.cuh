@@ -15,6 +15,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <utility>
 #include "../../include/tslam.h"
 
 #define TS_B 16
@@ -369,7 +370,7 @@ struct TsCounters {  // device-side statistics (tslam_tsdf_get_stats)
   unsigned long long n_px, n_valid, n_rays, n_updates, n_oob;
   // block-binned ray march (tslam_march.cu): diagnostics, not part of the parity counters
   unsigned long long n_segs, n_items, n_slow, n_fallback, n_generic, n_verify_bad;
-  // segments the two walks of the binned march disagreed about (k_seg_scatter, k_march_reset): must stay 0
+  // segments the two walks of the binned march disagreed about (k_seg_scatter, k_march_blocks): must stay 0
   unsigned long long n_seg_guard;
 };
 
@@ -391,18 +392,20 @@ struct TsSeg { uint32_t ray, jc; };
 // generic-list records use jc = j0 << 12 | count (count <= 4095)
 struct TsItem { int blk; uint32_t seg0, nseg, pad; };  // work item of k_march_blocks: <= MR_CHUNK segments of one block
 #define MR_CHUNK 4096
-struct TsMarchCtl {  // device-side control block of one launch (zeroed by k_march_reset at its end)
+struct TsMarchCtl {  // device-side control block of one launch (zeroed by the last CTA of k_march_blocks)
   int n_touched;     // blocks that received at least one segment
-  int n_items;       // work items built by k_seg_scan
+  int n_items;       // work items built by k_seg_class_scan
   int n_full;        // (unused since the items are listed longest first)
   int item_cursor;   // persistent-CTA work cursor of k_march_blocks
   int n_gen;         // generic-list records
   int overflow;      // segments or work items did not fit: every segment goes through the generic path this launch
   unsigned int total_segs;
   unsigned int fmax_bits;  // float bits of max over rays of max(w, w*|ds|max): sizes the fixed-point scale of the launch
-  int scale_k;       // shared-memory sums are kept in units of 2^-scale_k (k_seg_scan: largest k with max * 2^k < 2^30)
-  int ticket;
-  int pad0, pad1, pad2;
+  int scale_k;       // shared-memory sums are kept in units of 2^-scale_k (k_seg_class_scan: largest k with max * 2^k < 2^30)
+  int ticket;        // CTAs of k_march_blocks done: the last one clears this block
+  int ticket_scan;   // CTAs of k_seg_class_scan done: the last one runs the scan
+  int gen_cursor;    // generic-list cursor of k_march_blocks
+  int pad2;
   int pad[3];
 };
 struct TsMarchWs {
@@ -764,6 +767,24 @@ int ts_cuda_fail(cudaError_t e, const char* what);
     cudaError_t _e = cudaGetLastError();                                \
     if (_e != cudaSuccess) return ts_cuda_fail(_e, "kernel launch");    \
   } while (0)
+
+// Launch with programmatic dependent launch (Hopper): the kernel may start while its predecessor on `st` is still
+// running, and must call cudaGridDependencySynchronize() before it reads anything the predecessor writes - on every
+// path, so that it never completes before the predecessor.  After an event record or a memset it is an ordinary launch.
+template <class... KArgs, class... Args>
+static cudaError_t ts_launch_pdl(void (*k)(KArgs...), int grid, int block, size_t smem, cudaStream_t st, Args&&... args) {
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3((unsigned)grid);
+  cfg.blockDim = dim3((unsigned)block);
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = st;
+  cudaLaunchAttribute at[1];
+  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  at[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = at;
+  cfg.numAttrs = 1;
+  return cudaLaunchKernelEx(&cfg, k, std::forward<Args>(args)...);
+}
 
 // shared across translation units
 int ts_flush_pending(tslam_tsdf* m, cudaStream_t st);   // commit if anything is pending

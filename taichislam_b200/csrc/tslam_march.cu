@@ -9,9 +9,9 @@
 //                  32-byte record.  Then a 3-D DDA (seg_generate) cuts the ray into SEGMENTS - runs of consecutive
 //                  steps that stay in one 16^3 voxel block - activates the blocks on the way and counts the segments
 //                  per (block, length class) with warp-aggregated reductions.  It stores no segment;
-//   k_seg_class    per touched block: class counts -> offsets inside the block's run, list of touched blocks;
-//   k_seg_scan     exclusive scan over the touched blocks -> run offsets + work items (<= MR_CHUNK segments of one
-//                  block each, full chunks first);
+//   k_seg_class_scan  per touched block: class counts -> offsets inside the block's run, list of touched blocks;
+//                  then its last CTA: exclusive scan over the touched blocks -> run offsets + work items
+//                  (<= MR_CHUNK segments of one block each, longest first);
 //   k_seg_scatter  walks every ray again from its stored record (the same seg_generate, so the same segments in the
 //                  same order) and stores each segment at its place: a block's run is ordered by segment length;
 //   k_march_blocks persistent CTAs take work items.  The block's pending sums live in SHARED MEMORY as exact 64-bit
@@ -23,9 +23,13 @@
 //                  recomputes round((u*j*vs + T)/vs) exactly as the reference states it (:253-254), so voxel
 //                  indices stay bit-exact; a sample whose exact voxel is not in the item's block takes a global
 //                  reduction.  At the end of the item every touched voxel is flushed with ONE coalesced
-//                  REDG.ADD.F32x2 into the block's `acc` plane (what k_commit folds into TSDF/W, :264-267);
-//   k_march_generic  the exact one-reduction-per-sample march for what the binned path does not take: segments
-//                  next to the volume boundary, rays with more than 65535 steps, workspace overflow.
+//                  REDG.ADD.F32x2 into the block's `acc` plane (what k_commit folds into TSDF/W, :264-267).
+//                  Once the items run out, its CTAs take the generic path - the exact one-reduction-per-sample march
+//                  for what the binned path does not take: segments next to the volume boundary, rays with more than
+//                  65535 steps, workspace overflow - zero the fill counters, and the last CTA clears the control block.
+//
+// Every kernel here is launched with programmatic dependent launch (ts_launch_pdl): its launch and prologue overlap its
+// predecessor's tail, and it waits (cudaGridDependencySynchronize) where it first reads the predecessor's output.
 //
 // Sample value: ds = L - j*vs (the reference forms |P - x| * sign((P - x).m), :258-260, which equals it up to the
 // f32 rounding of x: <= 3e-6 m on a 25 m map, tolerance 1e-4).
@@ -120,7 +124,7 @@ __device__ __forceinline__ void ray_setup(const TsBatch& batch, const TsIntrin& 
 // K2b: segment walks: 3-D DDA over the 16^3 blocks in voxel-index space, one lane per ray, warp-uniform loop (one
 // block crossing per lane and iteration).  Segments are HINTS - every sample is re-checked exactly by the march
 // kernel - so the crossing parameters may be off by one step.  The DDA runs twice per launch, in k_seg_count (count
-// the segments per block and length class) and k_seg_scatter (store them in the runs k_seg_scan laid out): recomputing
+// the segments per block and length class) and k_seg_scatter (store them in the runs k_seg_class_scan laid out): recomputing
 // a segment costs a few FMAs per block crossing, storing it in a list and reading it back 24 bytes of traffic.
 // ---------------------------------------------------------------------------
 // 0 = far outside the volume (every sample is out of bounds), 1 = block inside the block range, 2 = outside but
@@ -222,6 +226,7 @@ __global__ void __launch_bounds__(MS_THREADS, WC_MINB) k_seg_count(const __grid_
   __shared__ unsigned long long s_btab[RM_TAB];  // block coordinates -> pool index (direct mapped, rm_lookup)
   for (int e = threadIdx.x; e < RM_TAB; e += MS_THREADS) s_btab[e] = TS_EMPTY;
   __syncthreads();
+  cudaGridDependencySynchronize();  // the ray list and its buckets come from the bucket kernel
   const uint32_t nme = min((uint32_t)*n_rays_p, ray_cap);
   const uint32_t lane = threadIdx.x & 31u;
   unsigned int my_oob = 0, my_rays = 0, my_fmax = 0;
@@ -250,6 +255,7 @@ __global__ void __launch_bounds__(MS_THREADS, WC_MINB) k_seg_count(const __grid_
     // non-finite pose: hand the rest to the exact path in bounded pieces
     while (j <= q.n) { const int c = min(q.n - j + 1, 4095); gen_append(w, g.err, r, j, c); j += c; }
   }
+  cudaTriggerProgrammaticLaunchCompletion();
   for (int o = 16; o > 0; o >>= 1) {
     my_oob += __shfl_xor_sync(FULL, my_oob, o);
     my_rays += __shfl_xor_sync(FULL, my_rays, o);
@@ -264,17 +270,18 @@ __global__ void __launch_bounds__(MS_THREADS, WC_MINB) k_seg_count(const __grid_
 
 // K2b-2: scattering walk.  The same generator over the same stored records, so the same binned segments in the same
 // order per ray.  Each takes a slot of its range with a warp-aggregated returning atomic that counts seg_count[key] down
-// from the count of the counting walk (k_seg_class left it there): a group of n finding `left` slots still free takes
+// from the count of the counting walk (k_seg_class_scan left it there): a group of n finding `left` slots still free takes
 // the n slots from end - left on, in lane order, so a range fills from its start in the order the groups arrive.  Guards that
 // never fire while the two walks agree route a segment to the generic path instead of writing outside its run, and are
 // counted in n_seg_guard: a block that is not in the grid, a run that is already full.  A block whose activation failed
 // (pool exhausted) was dropped by the counting walk: its segments are dropped here too.  When the launch overflowed
-// (k_seg_scan), every binned segment takes the generic path.
+// (k_seg_class_scan), every binned segment takes the generic path.
 __global__ void __launch_bounds__(MS_THREADS, WS_MINB) k_seg_scatter(const __grid_constant__ TsBatch batch, TsGrid g, const int* __restrict__ n_rays_p,
                                                                      uint32_t ray_cap, TsMarchWs w, TsCounters* ctr) {
   __shared__ unsigned long long s_btab[RM_TAB];  // block coordinates -> pool index (direct mapped, rm_find)
   for (int e = threadIdx.x; e < RM_TAB; e += MS_THREADS) s_btab[e] = TS_EMPTY;
   __syncthreads();
+  cudaGridDependencySynchronize();  // the runs and the overflow flag come from k_seg_class_scan
   const uint32_t nme = min((uint32_t)*n_rays_p, ray_cap);
   const uint32_t lane = threadIdx.x & 31u;
   const bool overflow = w.ctl->overflow != 0;
@@ -315,55 +322,23 @@ __global__ void __launch_bounds__(MS_THREADS, WS_MINB) k_seg_scatter(const __gri
       if (to_gen) gen_append(w, g.err, r, j0, cnt);
     });
   }
+  cudaTriggerProgrammaticLaunchCompletion();
   for (int o = 16; o > 0; o >>= 1) my_guard += __shfl_xor_sync(FULL, my_guard, o);
   if (lane == 0 && my_guard) atomicAdd(&ctr->n_seg_guard, (unsigned long long)my_guard);
 }
 
 // ---------------------------------------------------------------------------
-// K2c: per block with segments: class counts -> end of each (class, replica) range inside the block's run (seg_rel),
-// list of touched blocks.  seg_count keeps the counts: k_seg_scatter counts each back down to 0 as it fills the range
-// from its start (end - count).
+// K2c: one kernel, two stages.  Grid-wide: per block with segments, class counts -> end of each (class, replica) range
+// inside the block's run (seg_rel), list of touched blocks.  seg_count keeps the counts: k_seg_scatter counts each back
+// down to 0 as it fills the range from its start (end - count).  Then the CTA that finishes last runs the scan over the
+// touched blocks -> run offsets + work items (seg_scan): the scan needs every CTA's list entries, and a kernel boundary
+// costs more than the few hundred blocks the class stage handles.
+//
+// The items are listed LONGEST FIRST (estimated samples, 32 bins): the persistent march kernel takes them in list order,
+// so its tail is made of the cheapest items (with the items in block order, SMs idled through a long tail of the
+// kernel's time).
 // ---------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) k_seg_class(TsGrid g, TsMarchWs w) {
-  const int nb = min(*g.n_blocks, g.max_blocks);
-  const uint32_t lane = threadIdx.x & 31u;
-  const int stride = gridDim.x * 256;
-  for (int b0 = blockIdx.x * 256; b0 < nb; b0 += stride) {
-    const int b = b0 + (int)threadIdx.x;
-    unsigned tot = 0, cost = 0;  // segments / samples (upper estimate: class q holds segments of 2q+1 or 2q+2 steps)
-    if (b < nb && g.dirty_flag[b]) {
-      uint4* c4 = reinterpret_cast<uint4*>(&w.seg_count[(size_t)b * SEG_KEYS]);
-      uint4* r4 = reinterpret_cast<uint4*>(&w.seg_rel[(size_t)b * SEG_KEYS]);
-#pragma unroll 4
-      for (int q = 0; q < SEG_KEYS / 4; q++) {
-        const uint4 c = c4[q];
-        if ((c.x | c.y | c.z | c.w) == 0u) { continue; }
-        tot += c.x + c.y + c.z + c.w;
-        r4[q] = make_uint4(tot - c.y - c.z - c.w, tot - c.z - c.w, tot - c.w, tot);  // ends of the ranges
-        cost += (c.x + c.y + c.z + c.w) * (unsigned)(2 * (q / (SEG_REP / 4)) + 2);
-      }
-    }
-    const unsigned mt = __ballot_sync(FULL, tot > 0u);
-    if (mt) {
-      const int leader = __ffs(mt) - 1;
-      int p0 = 0;
-      if ((int)lane == leader) p0 = atomicAdd(&w.ctl->n_touched, __popc(mt));
-      p0 = __shfl_sync(FULL, p0, leader);
-      if (tot > 0u) {
-        const int p = p0 + __popc(mt & ((1u << lane) - 1u));
-        w.touched[p] = b;
-        w.blk_total[p] = tot;
-        w.blk_cost[p] = cost;
-      }
-    }
-  }
-}
-
-// ---------------------------------------------------------------------------
-// K2d: scan over the touched blocks -> run offsets + work items (one CTA).  The items are listed LONGEST FIRST
-// (estimated samples, 32 bins): the persistent march kernel takes them in list order, so its tail is made of the
-// cheapest items (with the items in block order, SMs idled through a long tail of the kernel's time).
-// ---------------------------------------------------------------------------
+#define SC_THREADS 1024
 #define SC_BINS 32
 __device__ __forceinline__ int item_bin(uint32_t cnt, uint32_t cost, uint32_t q, uint32_t nq) {
   // a block's run is ordered by segment length: chunk q of nq holds longer segments than chunk q-1 (ramp .5 .. 1.5)
@@ -371,22 +346,24 @@ __device__ __forceinline__ int item_bin(uint32_t cnt, uint32_t cost, uint32_t q,
   const float est = (float)nseg * ((float)cost / (float)cnt) * (0.5f + ((float)q + 0.5f) / (float)nq);
   return min(SC_BINS - 1, (int)(est * (1.0f / 4096.0f)));
 }
-__global__ void __launch_bounds__(1024) k_seg_scan(TsMarchWs w, TsCounters* ctr) {
+// run by the last CTA alone; the class stage's list (touched, blk_total, blk_cost, n_touched) was written by other CTAs,
+// so it is read through L2 (__ldcg)
+__device__ __forceinline__ void seg_scan(const TsMarchWs& w, TsCounters* ctr) {
   __shared__ uint32_t s_a[32];
   __shared__ uint32_t s_run;
   __shared__ unsigned int s_hist[SC_BINS], s_base[SC_BINS];
   __shared__ int s_ovf;
-  const int nt = w.ctl->n_touched;
+  const int nt = __ldcg(&w.ctl->n_touched);
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   if (threadIdx.x == 0) s_run = 0;
   if (threadIdx.x < SC_BINS) s_hist[threadIdx.x] = 0u;
   __syncthreads();
   // pass A: run offsets (exclusive scan of the blocks' segment counts), then the histogram of the items' estimated cost
-  for (int base = 0; base < nt; base += 1024) {
+  for (int base = 0; base < nt; base += SC_THREADS) {
     const int i = base + threadIdx.x;
     int blk = -1;
     uint32_t cnt = 0;
-    if (i < nt) { blk = w.touched[i]; cnt = w.blk_total[i]; }
+    if (i < nt) { blk = __ldcg(&w.touched[i]); cnt = __ldcg(&w.blk_total[i]); }
     uint32_t a = cnt;  // inclusive warp scan
     for (int o = 1; o < 32; o <<= 1) {
       const uint32_t ta = __shfl_up_sync(FULL, a, o);
@@ -409,7 +386,7 @@ __global__ void __launch_bounds__(1024) k_seg_scan(TsMarchWs w, TsCounters* ctr)
     __syncthreads();
   }
   for (int i = wid; i < nt; i += 32) {  // one warp per block, one lane per chunk: the busiest blocks have dozens of chunks
-    const uint32_t cnt = w.blk_total[i], cost = w.blk_cost[i];
+    const uint32_t cnt = __ldcg(&w.blk_total[i]), cost = __ldcg(&w.blk_cost[i]);
     const uint32_t nq = (cnt + MR_CHUNK - 1) / MR_CHUNK;
     for (uint32_t q = lane; q < nq; q += 32) atomicAdd(&s_hist[item_bin(cnt, cost, q, nq)], 1u);
   }
@@ -440,8 +417,8 @@ __global__ void __launch_bounds__(1024) k_seg_scan(TsMarchWs w, TsCounters* ctr)
   if (s_ovf) return;
   // pass B: the items, longest bin first
   for (int i = wid; i < nt; i += 32) {
-    const int blk = w.touched[i];
-    const uint32_t cnt = w.blk_total[i], cost = w.blk_cost[i], ex_seg = w.seg_off[blk];
+    const int blk = __ldcg(&w.touched[i]);
+    const uint32_t cnt = __ldcg(&w.blk_total[i]), cost = __ldcg(&w.blk_cost[i]), ex_seg = w.seg_off[blk];
     const uint32_t nq = (cnt + MR_CHUNK - 1) / MR_CHUNK;
     for (uint32_t q = lane; q < nq; q += 32) {
       const int b = item_bin(cnt, cost, q, nq);
@@ -449,6 +426,51 @@ __global__ void __launch_bounds__(1024) k_seg_scan(TsMarchWs w, TsCounters* ctr)
       w.items[pos] = TsItem{blk, ex_seg + q * MR_CHUNK, min((uint32_t)MR_CHUNK, cnt - q * MR_CHUNK), 0u};
     }
   }
+}
+__global__ void __launch_bounds__(SC_THREADS, 1) k_seg_class_scan(TsGrid g, TsMarchWs w, TsCounters* ctr) {
+  cudaGridDependencySynchronize();  // seg_count and the dirty flags come from k_seg_count
+  const int nb = min(*g.n_blocks, g.max_blocks);
+  const uint32_t lane = threadIdx.x & 31u;
+  const int stride = gridDim.x * SC_THREADS;
+  for (int b0 = blockIdx.x * SC_THREADS; b0 < nb; b0 += stride) {
+    const int b = b0 + (int)threadIdx.x;
+    unsigned tot = 0, cost = 0;  // segments / samples (upper estimate: class q holds segments of 2q+1 or 2q+2 steps)
+    if (b < nb && g.dirty_flag[b]) {
+      uint4* c4 = reinterpret_cast<uint4*>(&w.seg_count[(size_t)b * SEG_KEYS]);
+      uint4* r4 = reinterpret_cast<uint4*>(&w.seg_rel[(size_t)b * SEG_KEYS]);
+#pragma unroll 4
+      for (int q = 0; q < SEG_KEYS / 4; q++) {
+        const uint4 c = c4[q];
+        if ((c.x | c.y | c.z | c.w) == 0u) { continue; }
+        tot += c.x + c.y + c.z + c.w;
+        r4[q] = make_uint4(tot - c.y - c.z - c.w, tot - c.z - c.w, tot - c.w, tot);  // ends of the ranges
+        cost += (c.x + c.y + c.z + c.w) * (unsigned)(2 * (q / (SEG_REP / 4)) + 2);
+      }
+    }
+    const unsigned mt = __ballot_sync(FULL, tot > 0u);
+    if (mt) {
+      const int leader = __ffs(mt) - 1;
+      int p0 = 0;
+      if ((int)lane == leader) p0 = atomicAdd(&w.ctl->n_touched, __popc(mt));
+      p0 = __shfl_sync(FULL, p0, leader);
+      if (tot > 0u) {
+        const int p = p0 + __popc(mt & ((1u << lane) - 1u));
+        w.touched[p] = b;
+        w.blk_total[p] = tot;
+        w.blk_cost[p] = cost;
+      }
+    }
+  }
+  __shared__ int s_last;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    __threadfence();
+    s_last = atomicAdd(&w.ctl->ticket_scan, 1) == (int)gridDim.x - 1;
+  }
+  __syncthreads();
+  if (!s_last) return;
+  __threadfence();
+  seg_scan(w, ctr);
 }
 
 // ---------------------------------------------------------------------------
@@ -499,7 +521,7 @@ __device__ __forceinline__ double mb_sum(unsigned int lo, int hi) {
 
 template <bool VERIFY, int MB_THREADS, int MB_MINB>
 __global__ void __launch_bounds__(MB_THREADS, MB_MINB) k_march_blocks(const __grid_constant__ TsBatch batch, TsIntrin in, TsGrid g, TsMarchWs w,
-                                                                 TsCounters* ctr) {
+                                                                 TsCounters* ctr, int* n_rays) {
   extern __shared__ __align__(16) unsigned int mb_smem[];
   unsigned int* const a_lo = mb_smem;
   int* const a_hi = (int*)(mb_smem + MB_WORDS);
@@ -508,11 +530,12 @@ __global__ void __launch_bounds__(MB_THREADS, MB_MINB) k_march_blocks(const __gr
   __shared__ int s_item;
   const uint32_t lane = threadIdx.x & 31u, wid = threadIdx.x >> 5;
   const float vs = in.vs, rvs = in.rvs, eps_hi = 0.5f - w.near_eps;
+  for (int e = threadIdx.x; e < 4 * MB_WORDS; e += MB_THREADS) mb_smem[e] = 0u;
+  cudaGridDependencySynchronize();  // the items, segments and control block come from k_seg_scatter and before
   const int scale_k = w.ctl->scale_k;
   const float fix = __uint_as_float((unsigned)(127 + scale_k) << 23);   // 2^k
   const double unfix = 1.0 / (double)fix;
   unsigned int my_upd = 0, my_oob = 0, my_slow = 0, my_fb = 0, my_bad = 0;
-  for (int e = threadIdx.x; e < 4 * MB_WORDS; e += MB_THREADS) mb_smem[e] = 0u;
   const int n_items = w.ctl->n_items;
   while (true) {
     __syncthreads();
@@ -520,7 +543,7 @@ __global__ void __launch_bounds__(MB_THREADS, MB_MINB) k_march_blocks(const __gr
     __syncthreads();
     const int it = s_item;
     if (it >= n_items) break;
-    const TsItem item = w.items[it];  // longest first (k_seg_scan)
+    const TsItem item = w.items[it];  // longest first (k_seg_class_scan)
     int sm, kx, ky, kz;
     ts_unpack_key(g.block_key[item.blk], sm, kx, ky, kz);
     const int ox = kx << TS_BSHIFT, oy = ky << TS_BSHIFT, oz = kz << TS_BSHIFT;
@@ -660,16 +683,62 @@ __global__ void __launch_bounds__(MB_THREADS, MB_MINB) k_march_blocks(const __gr
       red_add_f32x2(&acc[v], (float)(mb_sum(alo, ahi) * unfix), (float)(mb_sum(blo, bhi) * unfix));
     }
   }
+  // ---- tail of the launch, once the item cursor has run out: the generic path, the fill counters, the control block ----
+  // generic path: exact index and one global reduction per sample, for the segments k_seg_count and k_seg_scatter listed
+  // (next to the volume boundary, over-long rays, overflow), MB_THREADS records per claim
+  const int n_gen = min(w.ctl->n_gen, (int)w.gen_cap);
+  unsigned int my_gen = 0;
+  while (true) {
+    __syncthreads();
+    if (threadIdx.x == 0) s_item = atomicAdd(&w.ctl->gen_cursor, MB_THREADS);
+    __syncthreads();
+    const int i = s_item + (int)threadIdx.x;
+    if (s_item >= n_gen) break;
+    if (i < n_gen) {
+      const TsSeg sg = w.gen[i];
+      const float4* src = reinterpret_cast<const float4*>(&w.rays[sg.ray]);
+      const float4 a = src[0], b = src[1];
+      const TsFrame& fr = batch.f[(w.aux[sg.ray] >> 8) & 255u];
+      const int j0 = (int)(sg.jc >> 12), cnt = (int)(sg.jc & 4095u);
+      for (int q = 0; q < cnt; q++) {
+        const int j = j0 + q;
+        int xi, yi, zi;
+        exact_index(a.x, a.y, a.z, fr.T, j, vs, rvs, xi, yi, zi);
+        const float ds = __fmaf_rn(-(float)j, vs, a.w);
+        global_sample(g, fr.submap, xi, yi, zi, b.w * ds, b.w, my_upd, my_oob);
+        my_gen++;
+      }
+    }
+  }
+  cudaTriggerProgrammaticLaunchCompletion();
+  // fill counters back to zero.  k_seg_scatter counted every run down to 0 unless the launch overflowed; a count left
+  // above 0 is a slot of a run that no segment filled (n_seg_guard, must stay 0)
+  unsigned int my_left = 0;
+  {
+    const int nt = w.ctl->n_touched;
+    const bool check = w.ctl->overflow == 0;
+    for (int q = blockIdx.x * MB_THREADS + threadIdx.x; q < nt * (SEG_KEYS / 4); q += gridDim.x * MB_THREADS) {
+      int4* c4 = reinterpret_cast<int4*>(w.seg_count + (size_t)w.touched[q / (SEG_KEYS / 4)] * SEG_KEYS) + q % (SEG_KEYS / 4);
+      if (check) {
+        const int4 c = *c4;
+        my_left += (unsigned)(max(c.x, 0) + max(c.y, 0) + max(c.z, 0) + max(c.w, 0));
+      }
+      *c4 = make_int4(0, 0, 0, 0);
+    }
+  }
   for (int o = 16; o > 0; o >>= 1) {
     my_upd += __shfl_xor_sync(FULL, my_upd, o);
     my_oob += __shfl_xor_sync(FULL, my_oob, o);
     my_slow += __shfl_xor_sync(FULL, my_slow, o);
     my_fb += __shfl_xor_sync(FULL, my_fb, o);
     my_bad += __shfl_xor_sync(FULL, my_bad, o);
+    my_gen += __shfl_xor_sync(FULL, my_gen, o);
+    my_left += __shfl_xor_sync(FULL, my_left, o);
   }
   // one global reduction per CTA and counter (same-address atomics serialise in L2)
-  __shared__ unsigned int s_stat[5];
-  if (threadIdx.x < 5) s_stat[threadIdx.x] = 0u;
+  __shared__ unsigned int s_stat[7];
+  __shared__ int s_last;
+  if (threadIdx.x < 7) s_stat[threadIdx.x] = 0u;
   __syncthreads();
   if (lane == 0) {
     if (my_upd) atomicAdd(&s_stat[0], my_upd);
@@ -677,6 +746,8 @@ __global__ void __launch_bounds__(MB_THREADS, MB_MINB) k_march_blocks(const __gr
     if (my_slow) atomicAdd(&s_stat[2], my_slow);
     if (my_fb) atomicAdd(&s_stat[3], my_fb);
     if (my_bad) atomicAdd(&s_stat[4], my_bad);
+    if (my_gen) atomicAdd(&s_stat[5], my_gen);
+    if (my_left) atomicAdd(&s_stat[6], my_left);
   }
   __syncthreads();
   if (threadIdx.x == 0) {
@@ -685,67 +756,18 @@ __global__ void __launch_bounds__(MB_THREADS, MB_MINB) k_march_blocks(const __gr
     if (s_stat[2]) atomicAdd(&ctr->n_slow, (unsigned long long)s_stat[2]);
     if (s_stat[3]) atomicAdd(&ctr->n_fallback, (unsigned long long)s_stat[3]);
     if (s_stat[4]) atomicAdd(&ctr->n_verify_bad, (unsigned long long)s_stat[4]);
-  }
-}
-
-// ---------------------------------------------------------------------------
-// K2g: generic path - exact index and one global reduction per sample
-// ---------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) k_march_generic(const __grid_constant__ TsBatch batch, TsIntrin in, TsGrid g, TsMarchWs w, TsCounters* ctr) {
-  const int n_gen = min(w.ctl->n_gen, (int)w.gen_cap);
-  unsigned int my_upd = 0, my_oob = 0, my_gen = 0;
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n_gen; i += gridDim.x * blockDim.x) {
-    const TsSeg sg = w.gen[i];
-    const float4* src = reinterpret_cast<const float4*>(&w.rays[sg.ray]);
-    const float4 a = src[0], b = src[1];
-    const TsFrame& fr = batch.f[(w.aux[sg.ray] >> 8) & 255u];
-    const int j0 = (int)(sg.jc >> 12), cnt = (int)(sg.jc & 4095u);
-    for (int q = 0; q < cnt; q++) {
-      const int j = j0 + q;
-      int xi, yi, zi;
-      exact_index(a.x, a.y, a.z, fr.T, j, in.vs, in.rvs, xi, yi, zi);
-      const float ds = __fmaf_rn(-(float)j, in.vs, a.w);
-      global_sample(g, fr.submap, xi, yi, zi, b.w * ds, b.w, my_upd, my_oob);
-      my_gen++;
-    }
-  }
-  for (int o = 16; o > 0; o >>= 1) {
-    my_upd += __shfl_xor_sync(FULL, my_upd, o);
-    my_oob += __shfl_xor_sync(FULL, my_oob, o);
-    my_gen += __shfl_xor_sync(FULL, my_gen, o);
-  }
-  if ((threadIdx.x & 31) == 0) {
-    if (my_upd) atomicAdd(&ctr->n_updates, (unsigned long long)my_upd);
-    if (my_oob) atomicAdd(&ctr->n_oob, (unsigned long long)my_oob);
-    if (my_gen) atomicAdd(&ctr->n_generic, (unsigned long long)my_gen);
-  }
-}
-
-// end of a launch: fill cursors back to zero, control block cleared.  k_seg_scatter counted every run down to 0 unless
-// the launch overflowed; a count left above 0 is a slot of a run that no segment filled (n_seg_guard, must stay 0).
-__global__ void __launch_bounds__(256) k_march_reset(TsMarchWs w, TsCounters* ctr) {
-  const int nt = w.ctl->n_touched;
-  const bool check = w.ctl->overflow == 0;
-  unsigned int left = 0;
-  for (int q = blockIdx.x * 256 + threadIdx.x; q < nt * (SEG_KEYS / 4); q += gridDim.x * 256) {
-    int4* c4 = reinterpret_cast<int4*>(w.seg_count + (size_t)w.touched[q / (SEG_KEYS / 4)] * SEG_KEYS) + q % (SEG_KEYS / 4);
-    if (check) {
-      const int4 c = *c4;
-      left += (unsigned)(max(c.x, 0) + max(c.y, 0) + max(c.z, 0) + max(c.w, 0));
-    }
-    *c4 = make_int4(0, 0, 0, 0);
-  }
-  for (int o = 16; o > 0; o >>= 1) left += __shfl_xor_sync(FULL, left, o);
-  if ((threadIdx.x & 31) == 0 && left) atomicAdd(&ctr->n_seg_guard, (unsigned long long)left);
-  // the last CTA to finish clears the control block
-  __shared__ int s_last;
-  __syncthreads();
-  if (threadIdx.x == 0) {
+    if (s_stat[5]) atomicAdd(&ctr->n_generic, (unsigned long long)s_stat[5]);
+    if (s_stat[6]) atomicAdd(&ctr->n_seg_guard, (unsigned long long)s_stat[6]);
     __threadfence();
     s_last = atomicAdd(&w.ctl->ticket, 1) == (int)gridDim.x - 1;
   }
   __syncthreads();
-  if (s_last && threadIdx.x < sizeof(TsMarchCtl) / 4) reinterpret_cast<int*>(w.ctl)[threadIdx.x] = 0;
+  // the last CTA to finish (every other one is past its last read of the control block) clears it and the ray count
+  // of the launch
+  if (s_last) {
+    if (threadIdx.x < sizeof(TsMarchCtl) / 4) reinterpret_cast<int*>(w.ctl)[threadIdx.x] = 0;
+    if (threadIdx.x == 0) *n_rays = 0;
+  }
 }
 
 // ---------------------------------------------------------------------------
@@ -806,30 +828,26 @@ int ts_march_setup(tslam_tsdf* m, cudaStream_t st, const TsBatch& batch, uint32_
   return TSLAM_OK;
 }
 
-// sub_ev (profiling, may be null): 4 events recorded at the start, after counting walk + class + scan, the scattering
-// walk and the march kernels
+// sub_ev (profiling, may be null): 2 events recorded after counting walk + class + scan and after the scattering walk;
+// the caller's events before and after this call close the first and the last part.  The kernels after the first are
+// launched with programmatic dependent launch: each waits (cudaGridDependencySynchronize) only where it first reads its
+// predecessor's output, so its launch and prologue overlap the predecessor's tail.
 int ts_march_launch(tslam_tsdf* m, cudaStream_t st, const TsBatch& batch, uint32_t bucket_shift, const TsBucketLaunch& bl, cudaEvent_t* sub_ev) {
   const int sms = m->sm_count;
+  TS_CUDA(ts_launch_pdl(k_seg_count, sms * WC_MINB, MS_THREADS, 0, st, batch, m->in, m->g, (const TsBucket*)m->buckets, m->bidx, bucket_shift, bl,
+                        (const uint32_t*)m->ray_list, (const int*)m->n_rays, (uint32_t)m->ray_list_cap, m->mw, m->counters));
+  TS_LAUNCH_CHECK(m);
+  const int nsc = (m->g.max_blocks + SC_THREADS - 1) / SC_THREADS;
+  TS_CUDA(ts_launch_pdl(k_seg_class_scan, nsc < sms ? nsc : sms, SC_THREADS, 0, st, m->g, m->mw, m->counters));
+  TS_LAUNCH_CHECK(m);
   if (sub_ev) TS_CUDA(cudaEventRecord(sub_ev[0], st));
-  k_seg_count<<<sms * WC_MINB, MS_THREADS, 0, st>>>(batch, m->in, m->g, m->buckets, m->bidx, bucket_shift, bl, m->ray_list, m->n_rays,
-                                                    m->ray_list_cap, m->mw, m->counters);
-  TS_LAUNCH_CHECK(m);
-  k_seg_class<<<sms * 2, 256, 0, st>>>(m->g, m->mw);
-  TS_LAUNCH_CHECK(m);
-  k_seg_scan<<<1, 1024, 0, st>>>(m->mw, m->counters);
+  TS_CUDA(ts_launch_pdl(k_seg_scatter, sms * WS_MINB, MS_THREADS, 0, st, batch, m->g, (const int*)m->n_rays, (uint32_t)m->ray_list_cap, m->mw,
+                        m->counters));
   TS_LAUNCH_CHECK(m);
   if (sub_ev) TS_CUDA(cudaEventRecord(sub_ev[1], st));
-  k_seg_scatter<<<sms * WS_MINB, MS_THREADS, 0, st>>>(batch, m->g, m->n_rays, m->ray_list_cap, m->mw, m->counters);
-  TS_LAUNCH_CHECK(m);
-  if (sub_ev) TS_CUDA(cudaEventRecord(sub_ev[2], st));
   const int grid = (sms - m->rm_reserve) * 3;
-  if (m->march_verify) k_march_blocks<true, 320, 3><<<grid, 320, MB_SMEM, st>>>(batch, m->in, m->g, m->mw, m->counters);
-  else k_march_blocks<false, 320, 3><<<grid, 320, MB_SMEM, st>>>(batch, m->in, m->g, m->mw, m->counters);
+  if (m->march_verify) TS_CUDA(ts_launch_pdl(k_march_blocks<true, 320, 3>, grid, 320, MB_SMEM, st, batch, m->in, m->g, m->mw, m->counters, m->n_rays));
+  else TS_CUDA(ts_launch_pdl(k_march_blocks<false, 320, 3>, grid, 320, MB_SMEM, st, batch, m->in, m->g, m->mw, m->counters, m->n_rays));
   TS_LAUNCH_CHECK(m);
-  k_march_generic<<<sms * 2, 256, 0, st>>>(batch, m->in, m->g, m->mw, m->counters);
-  TS_LAUNCH_CHECK(m);
-  k_march_reset<<<32, 256, 0, st>>>(m->mw, m->counters);
-  TS_LAUNCH_CHECK(m);
-  if (sub_ev) TS_CUDA(cudaEventRecord(sub_ev[3], st));
   return TSLAM_OK;
 }

@@ -535,7 +535,19 @@ __global__ void __launch_bounds__(RM_THREADS, 2) k_raymarch(const __grid_constan
 // (dense_tsdf.py:264-267 applied once per voxel per batch).  One CTA per block,
 // fully coalesced float2 streams.  clamp=0 is the fusion variant (:274-278).
 // ---------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) k_commit(TsGrid g, int clamp, int fused_obs, unsigned long long* stamp, unsigned long long seq) {
+// The last CTA to finish (every CTA read n_dirty at its start) sets the dirty-list count and `ticket` back to zero.
+__device__ __forceinline__ void commit_done(const TsGrid& g, int* ticket) {
+  __shared__ int s_last;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    __threadfence();
+    s_last = atomicAdd(ticket, 1) == (int)gridDim.x - 1;
+  }
+  __syncthreads();
+  if (s_last && threadIdx.x == 0) { *g.n_dirty = 0; *ticket = 0; }
+}
+__global__ void __launch_bounds__(256) k_commit(TsGrid g, int clamp, int fused_obs, unsigned long long* stamp, unsigned long long seq, int* ticket) {
+  cudaGridDependencySynchronize();  // the dirty list comes from k_collect_dirty
   const int nd = *g.n_dirty;
   for (int q = blockIdx.x; q < nd; q += gridDim.x) {
     const int blk = g.dirty_list[q];
@@ -571,6 +583,7 @@ __global__ void __launch_bounds__(256) k_commit(TsGrid g, int clamp, int fused_o
     }
     if (threadIdx.x == 0) { g.dirty_flag[blk] = 0; g.esdf_dirty[blk] = 1; stamp[blk] = seq; }
   }
+  commit_done(g, ticket);
 }
 // ---------------------------------------------------------------------------
 // K3 (TMA variant): the same commit, with each dirty block's two 32 KB planes moved by the bulk-copy engine
@@ -610,17 +623,18 @@ __device__ __forceinline__ void bulk_s2g(void* dst_gmem, const void* src_smem, u
   asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(dst_gmem), "r"(smem_u32(src_smem)), "r"(bytes) : "memory");
 }
 
-__global__ void __launch_bounds__(256) k_commit_tma(TsGrid g, int clamp, int fused_obs, unsigned long long* stamp, unsigned long long seq) {
+__global__ void __launch_bounds__(256) k_commit_tma(TsGrid g, int clamp, int fused_obs, unsigned long long* stamp, unsigned long long seq, int* ticket) {
   extern __shared__ __align__(128) unsigned char cm_smem[];
   float2* s_acc = reinterpret_cast<float2*>(cm_smem);
   float2* s_tw = reinterpret_cast<float2*>(cm_smem + CM_PLANE_BYTES);
   unsigned long long* bar = reinterpret_cast<unsigned long long*>(cm_smem + 2 * CM_PLANE_BYTES);
-  const int nd = *g.n_dirty;
   if (threadIdx.x == 0) {
     mbar_init(bar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
+  cudaGridDependencySynchronize();  // the dirty list comes from k_collect_dirty
+  const int nd = *g.n_dirty;
   unsigned phase = 0;
   for (int q = blockIdx.x; q < nd; q += gridDim.x) {
     const int blk = g.dirty_list[q];
@@ -662,10 +676,12 @@ __global__ void __launch_bounds__(256) k_commit_tma(TsGrid g, int clamp, int fus
     __syncthreads();
   }
   if (threadIdx.x == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
+  commit_done(g, ticket);
 }
 
 // compact the per-block dirty flags into dirty_list (warp-aggregated append)
 __global__ void __launch_bounds__(256) k_collect_dirty(TsGrid g) {
+  cudaGridDependencySynchronize();  // the flags are set by the kernels before it
   const int nb = min(*g.n_blocks, g.max_blocks);
   const int stride = gridDim.x * blockDim.x;
   const int iters = (nb + stride - 1) / stride;
@@ -996,17 +1012,19 @@ extern "C" int tslam_tsdf_set_submap_pose(tslam_tsdf_t* m, int32_t s, const floa
 // ---------------------------------------------------------------------------
 // host: integrate
 // ---------------------------------------------------------------------------
+// k_collect_dirty, then the commit, whose last CTA sets the dirty-list count back to zero (ticket: scratch_i[4]).  Both
+// are launched with programmatic dependent launch (ts_launch_pdl).
 static int ts_launch_commit(tslam_tsdf* m, cudaStream_t st, int clamp, int fused) {
   int grid = m->sm_count * 8;
-  k_collect_dirty<<<(m->g.max_blocks + 255) / 256 < m->sm_count * 4 ? (m->g.max_blocks + 255) / 256 : m->sm_count * 4, 256, 0, st>>>(m->g);
+  const int gc = (m->g.max_blocks + 255) / 256 < m->sm_count * 4 ? (m->g.max_blocks + 255) / 256 : m->sm_count * 4;
+  TS_CUDA(ts_launch_pdl(k_collect_dirty, gc, 256, 0, st, m->g));
   TS_LAUNCH_CHECK(m);
   static const bool plain_env = getenv("TSLAM_COMMIT_PLAIN") != nullptr;  // A/B switch for the non-TMA variant
   const bool plain = plain_env || m->g.col != nullptr;  // textured maps: the per-thread variant also folds the colours
   const unsigned long long seq = ++m->commit_seq;        // stamp of every block this commit writes (incremental mesh)
-  if (plain) k_commit<<<grid, 256, 0, st>>>(m->g, clamp, fused, m->blk_stamp, seq);
-  else k_commit_tma<<<m->sm_count * 3, 256, CM_SMEM, st>>>(m->g, clamp, fused, m->blk_stamp, seq);
-  TS_LAUNCH_CHECK(m);
-  k_reset_counters<<<1, 1, 0, st>>>(m->g.n_dirty, nullptr);
+  int* ticket = m->scratch_i + 4;
+  if (plain) TS_CUDA(ts_launch_pdl(k_commit, grid, 256, 0, st, m->g, clamp, fused, m->blk_stamp, seq, ticket));
+  else TS_CUDA(ts_launch_pdl(k_commit_tma, m->sm_count * 3, 256, CM_SMEM, st, m->g, clamp, fused, m->blk_stamp, seq, ticket));
   TS_LAUNCH_CHECK(m);
   return TSLAM_OK;
 }
@@ -1183,19 +1201,22 @@ static int ts_integrate_depth_impl(tslam_tsdf_t* m, const uint16_t* depth, int m
     if (!m->g.cword && m->march_mode) {
       int rcs = ts_march_setup(m, st, batch, bshift);
       if (rcs) return ts_bucket_abandon(m, st, rcs);
-      int rcm = ts_march_launch(m, st, batch, bshift, bl, pe ? pe + 4 : nullptr);
+      int rcm = ts_march_launch(m, st, batch, bshift, bl, pe ? pe + 4 : nullptr);  // clears n_rays itself
       if (rcm) return ts_bucket_abandon(m, st, rcm);
-    } else if (m->g.cword) {
-      k_raymarch<true><<<m->sm_count, RM_THREADS, RM_SMEM_TEX, st>>>(batch, m->in, m->g, m->buckets, m->bcol, m->bidx, bshift, bl, m->ray_list,
-                                                                     m->n_rays, m->ray_list_cap, m->counters);
+      if (pe) TS_CUDA(cudaEventRecord(pe[2], st));
     } else {
-      k_raymarch<false><<<(m->sm_count - m->rm_reserve) * 2, RM_THREADS, RM_SMEM, st>>>(batch, m->in, m->g, m->buckets, m->bcol, m->bidx, bshift, bl,
-                                                                                     m->ray_list, m->n_rays, m->ray_list_cap, m->counters);
+      if (m->g.cword) {
+        k_raymarch<true><<<m->sm_count, RM_THREADS, RM_SMEM_TEX, st>>>(batch, m->in, m->g, m->buckets, m->bcol, m->bidx, bshift, bl, m->ray_list,
+                                                                       m->n_rays, m->ray_list_cap, m->counters);
+      } else {
+        k_raymarch<false><<<(m->sm_count - m->rm_reserve) * 2, RM_THREADS, RM_SMEM, st>>>(batch, m->in, m->g, m->buckets, m->bcol, m->bidx, bshift,
+                                                                                       bl, m->ray_list, m->n_rays, m->ray_list_cap, m->counters);
+      }
+      TS_LAUNCH_CHECK(m);
+      if (pe) TS_CUDA(cudaEventRecord(pe[2], st));
+      k_reset_counters<<<1, 1, 0, st>>>(m->n_rays, nullptr);
+      TS_LAUNCH_CHECK(m);
     }
-    TS_LAUNCH_CHECK(m);
-    if (pe) TS_CUDA(cudaEventRecord(pe[2], st));
-    k_reset_counters<<<1, 1, 0, st>>>(m->n_rays, nullptr);
-    TS_LAUNCH_CHECK(m);
     m->n_integrate_calls++;
     if (flags & TSLAM_F_COMMIT) {
       int rc = ts_flush_pending(m, st);
@@ -1247,21 +1268,24 @@ extern "C" int tslam_tsdf_integrate_points_rgb(tslam_tsdf_t* m, const float* xyz
                                                     m->n_rays, m->ray_list_cap, m->counters, m->g.err, csrc);
   TS_LAUNCH_CHECK(m);
   if (pe) TS_CUDA(cudaEventRecord(pe[1], st));
-  if (m->g.cword)
-    k_raymarch<true><<<m->sm_count, RM_THREADS, RM_SMEM_TEX, st>>>(batch, m->in, m->g, m->buckets, m->bcol, m->bidx, bshift, bl, m->ray_list,
-                                                                   m->n_rays, m->ray_list_cap, m->counters);
-  else if (m->march_mode) {
+  if (!m->g.cword && m->march_mode) {
     int rcm = ts_march_setup(m, st, batch, bshift);
     if (rcm) return ts_bucket_abandon(m, st, rcm);
-    rcm = ts_march_launch(m, st, batch, bshift, bl, pe ? pe + 4 : nullptr);
+    rcm = ts_march_launch(m, st, batch, bshift, bl, pe ? pe + 4 : nullptr);  // clears n_rays itself
     if (rcm) return ts_bucket_abandon(m, st, rcm);
-  } else
-    k_raymarch<false><<<m->sm_count * 2, RM_THREADS, RM_SMEM, st>>>(batch, m->in, m->g, m->buckets, m->bcol, m->bidx, bshift, bl, m->ray_list,
-                                                                    m->n_rays, m->ray_list_cap, m->counters);
-  TS_LAUNCH_CHECK(m);
-  if (pe) TS_CUDA(cudaEventRecord(pe[2], st));
-  k_reset_counters<<<1, 1, 0, st>>>(m->n_rays, nullptr);
-  TS_LAUNCH_CHECK(m);
+    if (pe) TS_CUDA(cudaEventRecord(pe[2], st));
+  } else {
+    if (m->g.cword)
+      k_raymarch<true><<<m->sm_count, RM_THREADS, RM_SMEM_TEX, st>>>(batch, m->in, m->g, m->buckets, m->bcol, m->bidx, bshift, bl, m->ray_list,
+                                                                     m->n_rays, m->ray_list_cap, m->counters);
+    else
+      k_raymarch<false><<<m->sm_count * 2, RM_THREADS, RM_SMEM, st>>>(batch, m->in, m->g, m->buckets, m->bcol, m->bidx, bshift, bl, m->ray_list,
+                                                                      m->n_rays, m->ray_list_cap, m->counters);
+    TS_LAUNCH_CHECK(m);
+    if (pe) TS_CUDA(cudaEventRecord(pe[2], st));
+    k_reset_counters<<<1, 1, 0, st>>>(m->n_rays, nullptr);
+    TS_LAUNCH_CHECK(m);
+  }
   m->n_integrate_calls++;
   if (flags & TSLAM_F_COMMIT) {
     int rc = ts_flush_pending(m, st);
@@ -1930,8 +1954,9 @@ extern "C" int tslam_tsdf_set_profiling(tslam_tsdf_t* m, int on) {
 }
 // ms3[3*i + {0,1,2}] = bucket / ray-march / commit(+reset) kernel time of the i-th most recent
 // recorded integrate launch, i < n (n <= TS_PROF_RING).  Returns the number of rows written in *n_out.
-// ms7[7*i + ...] = bucket, ray march (all of its kernels), commit, then the parts of the ray march: set-up + segment
-// count, scan, segment fill, march (+ generic + reset).  The last four are 0 for launches of the legacy kernel.
+// ms7[7*i + ...] = bucket, ray march (all of its kernels), commit, then the parts of the ray march: the interval between
+// the bucket kernel and the first march kernel (0: nothing runs there), set-up + segment count + class + scan, segment
+// fill, march (with the generic path and the resets).  The last four are 0 for launches of the legacy kernel.
 extern "C" int tslam_tsdf_kernel_ms2(tslam_tsdf_t* m, int32_t n, float* ms7, int32_t* n_out) {
   if (!m || !ms7 || !n_out || !m->ev) return TSLAM_E_INVALID;
   TS_CUDA(cudaDeviceSynchronize());
@@ -1941,9 +1966,10 @@ extern "C" int tslam_tsdf_kernel_ms2(tslam_tsdf_t* m, int32_t n, float* ms7, int
     cudaEvent_t* pe = m->ev + TS_PROF_EV * ((m->prof_launches - 1 - i) % TS_PROF_RING);
     for (int q = 0; q < 3; q++) TS_CUDA(cudaEventElapsedTime(&ms7[7 * i + q], pe[q], pe[q + 1]));
     for (int q = 0; q < 4; q++) ms7[7 * i + 3 + q] = 0.0f;
-    if (m->march_mode && !m->g.cword) {
-      TS_CUDA(cudaEventElapsedTime(&ms7[7 * i + 3], pe[1], pe[4]));
-      for (int q = 0; q < 3; q++) TS_CUDA(cudaEventElapsedTime(&ms7[7 * i + 4 + q], pe[4 + q], pe[5 + q]));
+    if (m->march_mode && !m->g.cword) {  // pe[4], pe[5]: after the scan and after the scattering walk (ts_march_launch)
+      TS_CUDA(cudaEventElapsedTime(&ms7[7 * i + 4], pe[1], pe[4]));
+      TS_CUDA(cudaEventElapsedTime(&ms7[7 * i + 5], pe[4], pe[5]));
+      TS_CUDA(cudaEventElapsedTime(&ms7[7 * i + 6], pe[5], pe[2]));
     }
   }
   *n_out = n;

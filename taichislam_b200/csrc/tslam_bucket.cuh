@@ -1,4 +1,4 @@
-// Sizing of the packed fields of the per-frame bucket grid (tslam_tsdf.cu).  Host-only C++ without CUDA, so that the
+// Sizing of the packed fields of the per-frame bucket grid (tslam_integrate.cu).  Host-only C++ without CUDA, so that the
 // bounds can be unit-tested without a GPU.
 #pragma once
 #include <cmath>
@@ -6,6 +6,7 @@
 
 #define TS_BK_SLOT_FIELD 25      // bits of an index entry left beside the 39-bit key: slot + 1 and the launch epoch
 #define TS_BK_MIN_EPOCH_BITS 4   // fewer epoch bits than this: clearing mode (no epoch, the consumer zeroes every entry)
+#define BK_MAX_SLOTS ((1u << 25) - 2u)  // record slots the slot + 1 field can name when it takes all TS_BK_SLOT_FIELD bits
 
 static inline int ts_bit_length(uint64_t x) {
   int b = 0;

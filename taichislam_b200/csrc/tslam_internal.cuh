@@ -164,7 +164,7 @@ __device__ __forceinline__ int ts_get_or_alloc_cached(const G& g, unsigned long 
 }
 
 // ---------------------------------------------------------------------------
-// arithmetic helpers shared by the integrate kernels (tslam_tsdf.cu, tslam_march.cu)
+// arithmetic helpers shared by the integrate kernels (tslam_integrate.cu, tslam_march.cu)
 // ---------------------------------------------------------------------------
 #define WMAX 1000.0f          // dense_tsdf.py:8
 #define FIXQ 1048576.0f       // 2^20: fixed-point quantum of the per-frame bucket sums
@@ -356,7 +356,7 @@ struct __align__(32) TsBucket {
   long long sx, sy, sz;
   unsigned long long cd;
 };
-// per-launch parameters of the bucket index (tslam_tsdf.cu, ts_bucket_launch)
+// per-launch parameters of the bucket index (tslam_integrate.cu, ts_bucket_launch)
 struct TsBucketLaunch {
   unsigned long long etag;  // launch epoch in the entry's epoch field; 0 in clearing mode
   int slot_bits;            // width of the slot + 1 field; 25 in clearing mode (no epoch field)
@@ -395,7 +395,7 @@ struct TsItem { int blk; uint32_t seg0, nseg, pad; };  // work item of k_march_b
 struct TsMarchCtl {  // device-side control block of one launch (zeroed by the last CTA of k_march_blocks)
   int n_touched;     // blocks that received at least one segment
   int n_items;       // work items built by k_seg_class_scan
-  int n_full;        // (unused since the items are listed longest first)
+  int n_full;        // always 0 (k_seg_class_scan writes it, nobody reads it: the items are listed longest first)
   int item_cursor;   // persistent-CTA work cursor of k_march_blocks
   int n_gen;         // generic-list records
   int overflow;      // segments or work items did not fit: every segment goes through the generic path this launch
@@ -497,7 +497,7 @@ struct tslam_tsdf {
   long long launches;
   int n_integrate_calls;
   int profiling;
-  cudaEvent_t* ev;          // profiling ring: TS_PROF_RING launches x 4 events (created lazily)
+  cudaEvent_t* ev;          // profiling ring: TS_PROF_RING launches x TS_PROF_EV events (created lazily)
   long long prof_launches;  // integrate launches recorded since profiling was switched on
   int sm_count;
   int tile_cuts_set, tile_cuts_tiles[3], tile_cuts[3][17];  // data-driven tile boundaries of a tiled global map (tslam_dist.cu)
@@ -787,16 +787,29 @@ static cudaError_t ts_launch_pdl(void (*k)(KArgs...), int grid, int block, size_
 }
 
 // shared across translation units
+// tslam_integrate.cu
+int ts_integrate_init();                                 // once per process, before the first integrate launch
 int ts_flush_pending(tslam_tsdf* m, cudaStream_t st);   // commit if anything is pending
+int ts_launch_commit(tslam_tsdf* m, cudaStream_t st, int clamp, int fused);  // k_collect_dirty + commit of the dirty blocks
 int ts_check_deferred(tslam_tsdf* m);                    // read + translate device error flags (synchronises)
 int ts_check_deferred_async(tslam_tsdf* m, cudaStream_t st);  // same, after the work queued on st
+double ts_bucket_dmax(const tslam_tsdf* m);
+int ts_check_tex(tslam_tsdf* m, const uint8_t* tex, int th, int tw);  // a colour image the map can take, or none
+int ts_integrate_depth_impl(tslam_tsdf_t* m, const uint16_t* depth, int mem, int32_t n_frames, int32_t h, int32_t w, const float* R9s,
+                            const float* T3s, const int32_t* submap_ids, int flags, void* stream, const uint8_t* tex = nullptr, int th = 0,
+                            int tw = 0);
+// the integrate launch marches with tslam_march.cu (else k_raymarch): its dispatch, and how its profiling row reads
+static inline bool ts_uses_binned_march(const tslam_tsdf* m) { return m->march_mode && !m->g.cword; }
+// tslam_queue.cu: the per-frame queue's switches, copy stream and events of a new handle / their release
+int ts_queue_init(tslam_tsdf* m);
+void ts_queue_free(tslam_tsdf* m);
+int ts_launch_queue(tslam_tsdf* m, cudaStream_t st);     // integrate the queued frames, if any
 // tslam_esdf.cu: per-block exchange mark of the tiled ESDF ([max_blocks]; owned block: ESDF changed since it was last
 // packed, ghost block: ESDF unpacked since the last relax), or NULL before the first ESDF update
 int* ts_esdf_xmark(tslam_tsdf* m);
 // tslam_march.cu: block-binned ray march of the rays listed in m->ray_list (replaces k_raymarch<false>)
 int ts_march_alloc(tslam_tsdf* m);
 void ts_march_free(tslam_tsdf* m);
-int ts_march_setup(tslam_tsdf* m, cudaStream_t st, const TsBatch& batch, uint32_t bucket_shift);  // rays listed since the last call
 int ts_march_launch(tslam_tsdf* m, cudaStream_t st, const TsBatch& batch, uint32_t bucket_shift, const TsBucketLaunch& bl, cudaEvent_t* sub_ev);
 
 // Octomap host helpers shared by its trackers (tslam_octo.cu)

@@ -821,18 +821,12 @@ void ts_march_free(tslam_tsdf* m) {
   cudaFree(w.blk_total); cudaFree(w.blk_cost); cudaFree(w.items); cudaFree(w.gen); cudaFree(w.ctl);
 }
 
-// workspace of the binned march (allocated at the first launch that needs it)
-int ts_march_setup(tslam_tsdf* m, cudaStream_t st, const TsBatch& batch, uint32_t bucket_shift) {
-  (void)st; (void)batch; (void)bucket_shift;
-  if (!m->mw.rays) { int rca = ts_march_alloc(m); if (rca) return rca; }
-  return TSLAM_OK;
-}
-
 // sub_ev (profiling, may be null): 2 events recorded after counting walk + class + scan and after the scattering walk;
 // the caller's events before and after this call close the first and the last part.  The kernels after the first are
 // launched with programmatic dependent launch: each waits (cudaGridDependencySynchronize) only where it first reads its
 // predecessor's output, so its launch and prologue overlap the predecessor's tail.
 int ts_march_launch(tslam_tsdf* m, cudaStream_t st, const TsBatch& batch, uint32_t bucket_shift, const TsBucketLaunch& bl, cudaEvent_t* sub_ev) {
+  if (!m->mw.rays) { int rca = ts_march_alloc(m); if (rca) return rca; }  // the workspace, at the first launch that needs it
   const int sms = m->sm_count;
   TS_CUDA(ts_launch_pdl(k_seg_count, sms * WC_MINB, MS_THREADS, 0, st, batch, m->in, m->g, (const TsBucket*)m->buckets, m->bidx, bucket_shift, bl,
                         (const uint32_t*)m->ray_list, (const int*)m->n_rays, (uint32_t)m->ray_list_cap, m->mw, m->counters));

@@ -37,22 +37,32 @@ __device__ __forceinline__ unsigned long long cas_acq_rel_u64(unsigned long long
   return old;
 }
 
-// accumulate one unprojected point per lane into the frame's bucket grid.
-// process_point (dense_tsdf.py:227-234) with exact fixed-point sums.  Lanes of a warp that fall into
-// the same bucket (neighbouring pixels usually do) are merged first (match.any + redux): one probe and
-// one set of reductions per distinct bucket per warp instead of per pixel.  The index maps the bucket's
-// voxel to a RECORD slot.  Slots need no allocator: every warp owns the 32 records [slot_base, slot_base + 32)
-// (it holds at most 32 distinct buckets), a probing lane brings the slot of its rank along and publishes it
-// with the key in ONE 64-bit CAS, so nobody ever waits for a slot.  The slot is private until that CAS publishes it,
-// so the lane STORES its warp's sums there first (the record needs no zeroing); lanes that find the bucket open add
-// into its record.  A lane that loses the race leaves its slot written but unnamed: nobody reads it.
-// Must be called by all 32 lanes; `valid` masks lanes without a point.  Returns the record slot when this
-// lane OPENED a bucket (the bucket becomes one ray; the caller appends it to the ray list), else -1.
+#define BK_CTA_TAB 512  // CTA bucket table: open addressing, twice the 256 keys a CTA can bring
+#define BK_ROW 13       // words of a CTA bucket's sums: lo x, y, z, d; hi x, y, z, d; count; r, g, b (13: odd row stride)
+
+// S from lo = S mod 2^32 and hi = sum(x >> 16) over fewer than 2^16 int32 addends x (as mb_sum, tslam_march.cu)
+__device__ __forceinline__ long long bk_row_sum(unsigned int lo, unsigned int hi) {
+  return (long long)(int)hi * 65536ll + (long long)(unsigned int)(lo - (hi << 16));
+}
+
+// accumulate one unprojected point per thread into the frame's bucket grid.
+// process_point (dense_tsdf.py:227-234) with exact fixed-point sums.  Points that fall into the same bucket
+// (neighbouring pixels usually do) are merged on chip in two stages before anyone touches the index: lanes of a warp
+// (match.any, per-warp slots), then the warps of the CTA (a shared-memory table keyed by the bucket, exact two-word
+// sums).  One probe and one set of reductions per distinct bucket per CTA instead of per pixel.  The index maps the
+// bucket's voxel to a RECORD slot.  Slots need no allocator: every CTA owns the 256 records [slot_base, slot_base + 256)
+// (it holds at most 256 distinct buckets), the thread that owns a bucket's CTA sums brings the slot of its thread index
+// along and publishes it with the key in ONE 64-bit CAS, so nobody ever waits for a slot.  The slot is private until
+// that CAS publishes it, so the thread STORES its CTA's sums there first (the record needs no zeroing); threads that
+// find the bucket open add into its record.  A thread that loses the race leaves its slot written but unnamed.
+// Must be called by all 256 threads of the CTA; `valid` masks threads without a point.  Returns the record slot when
+// this thread OPENED a bucket (the bucket becomes one ray; the caller appends it to the ray list), else -1.
 __device__ __forceinline__ int bucket_accumulate(bool valid, unsigned long long* idx, uint32_t cap_mask, uint32_t idx_base, TsBucket* recs,
                                                  uint4* cols, uint32_t* cnts, uint32_t rec_cap, uint32_t slot_base, const TsBucketLaunch& bl, float px,
-                                                 float py, float pz, float dep, float vs, bool agg_ok, int* err, bool tex = false, int cr = 0,
-                                                 int cg = 0, int cb = 0) {
-  const int bx = iroundf(px / vs), by = iroundf(py / vs), bz = iroundf(pz / vs);  // xyz_to_ijk mapping_common.py:240-243
+                                                 float py, float pz, float dep, float vs, float rvs, bool agg_ok, int* err, bool tex = false,
+                                                 int cr = 0, int cg = 0, int cb = 0) {
+  // xyz_to_ijk mapping_common.py:240-243; div_vs is the correctly rounded px / vs
+  const int bx = iroundf(div_vs(px, vs, rvs)), by = iroundf(div_vs(py, vs, rvs)), bz = iroundf(div_vs(pz, vs, rvs));
   if (valid && ((unsigned)(bx + (BK_OFF - 1)) > 2u * (BK_OFF - 1) || (unsigned)(by + (BK_OFF - 1)) > 2u * (BK_OFF - 1) ||
                 (unsigned)(bz + (BK_OFF - 1)) > 2u * (BK_OFF - 1))) {
     atomicOr(err, TS_ERR_BUCKET_RANGE);
@@ -61,22 +71,34 @@ __device__ __forceinline__ int bucket_accumulate(bool valid, unsigned long long*
   const unsigned long long key = bucket_key(bx, by, bz);
   long long qx = __float2ll_rn(px * FIXQ), qy = __float2ll_rn(py * FIXQ), qz = __float2ll_rn(pz * FIXQ), qd = __float2ll_rn(dep * FIXQ);
   int cnt = 1;
-  bool act = valid;  // this lane probes and adds
+  bool act = valid;  // this thread probes and adds
   const unsigned vmask = __ballot_sync(0xffffffffu, valid);
+  const uint32_t hk = ts_hash(key);
   if (agg_ok) {  // |q| < 2^26 (max_ray < 64 m): a 32-lane sum fits int32
     // every lane adds its point to the shared-memory slot of its group's first lane (native 32-bit ATOMS; slots of
     // different groups sit in different banks: stride 9 words), the leaders read the totals back.  (The
     // redux-per-group loop this replaces was 17 % of the kernel's instructions.)
     __shared__ int s_agg[8][32][9];
+    // CTA stage: the table maps a key to the thread that owns the bucket's row, entry = key << 8 | owner (~0: empty)
+    __shared__ unsigned long long s_tab[BK_CTA_TAB];
+    __shared__ unsigned int s_row[256][BK_ROW];
     const int lane = threadIdx.x & 31, wid = (threadIdx.x >> 5) & 7;
     int* mine = s_agg[wid][lane];
     mine[0] = 0; mine[1] = 0; mine[2] = 0; mine[3] = 0; mine[4] = 0;
     if (tex) { mine[5] = 0; mine[6] = 0; mine[7] = 0; }
+    unsigned int* row = s_row[threadIdx.x];
+    for (int e = 0; e < 9; e++) row[e] = 0u;
+    if (tex) { row[9] = 0u; row[10] = 0u; row[11] = 0u; }
+    s_tab[threadIdx.x] = ~0ull;
+    s_tab[threadIdx.x + 256] = ~0ull;
     __syncwarp();
     if (valid) {
       const unsigned grp = __match_any_sync(vmask, key);
       const int lead = __ffs(grp) - 1;
       act = lane == lead;
+      // the index entry this bucket will probe: an index line is rarely in L2 (64 frames x 1 MB), so its DRAM fetch
+      // starts here and overlaps the merge and its two barriers instead of following them
+      if (act) asm volatile("prefetch.global.L2 [%0];" ::"l"(idx + (hk & cap_mask)));
       cnt = __popc(grp);
       int* slot = s_agg[wid][lead];
       if (grp & (grp - 1u)) {  // more than one lane in the bucket
@@ -89,11 +111,36 @@ __device__ __forceinline__ int bucket_accumulate(bool valid, unsigned long long*
       qx = (long long)mine[0]; qy = (long long)mine[1]; qz = (long long)mine[2]; qd = (long long)mine[3];
       if (tex) { cr = mine[5]; cg = mine[6]; cb = mine[7]; }
     }
+    __syncthreads();  // the CTA table and rows are cleared
+    if (valid && act) {  // warp leaders: at most one per warp and bucket, so a row sums at most 8 addends
+      const unsigned long long want = (key << 8) | (unsigned long long)threadIdx.x;
+      uint32_t hs = hk & (BK_CTA_TAB - 1);
+      int own;
+      for (;;) {  // 256 keys at most in 512 entries: an empty entry is always found
+        const unsigned long long prev = atomicCAS(&s_tab[hs], ~0ull, want);
+        if (prev == ~0ull) { own = (int)threadIdx.x; break; }
+        if ((prev >> 8) == key) { own = (int)(prev & 255ull); break; }
+        hs = (hs + 1) & (BK_CTA_TAB - 1);
+      }
+      unsigned int* o = s_row[own];
+      const int wx = (int)qx, wy = (int)qy, wz = (int)qz, wd = (int)qd;
+      atomicAdd(&o[0], (unsigned)wx); atomicAdd(&o[1], (unsigned)wy); atomicAdd(&o[2], (unsigned)wz); atomicAdd(&o[3], (unsigned)wd);
+      atomicAdd(&o[4], (unsigned)(wx >> 16)); atomicAdd(&o[5], (unsigned)(wy >> 16)); atomicAdd(&o[6], (unsigned)(wz >> 16));
+      atomicAdd(&o[7], (unsigned)(wd >> 16));
+      atomicAdd(&o[8], (unsigned)cnt);
+      if (tex) { atomicAdd(&o[9], (unsigned)cr); atomicAdd(&o[10], (unsigned)cg); atomicAdd(&o[11], (unsigned)cb); }
+      act = own == (int)threadIdx.x;
+    }
+    __syncthreads();  // the CTA's sums are complete
+    if (act) {
+      qx = bk_row_sum(row[0], row[4]); qy = bk_row_sum(row[1], row[5]); qz = bk_row_sum(row[2], row[6]); qd = bk_row_sum(row[3], row[7]);
+      cnt = (int)row[8];
+      if (tex) { cr = (int)row[9]; cg = (int)row[10]; cb = (int)row[11]; }
+    }
   }
-  uint32_t h = ts_hash(key) & cap_mask;
-  const unsigned amask = __ballot_sync(0xffffffffu, act);
+  uint32_t h = hk & cap_mask;
   if (!act) return -1;
-  const uint32_t my_slot = slot_base + (uint32_t)__popc(amask & ((1u << (threadIdx.x & 31)) - 1u));
+  const uint32_t my_slot = slot_base + threadIdx.x;
   if (my_slot >= rec_cap) { atomicOr(err, TS_ERR_RAYLIST_FULL); return -1; }
   // qd >= 0; with a count plane the word holds the depth sum alone
   const unsigned long long cd = (cnts ? 0ull : (unsigned long long)cnt << bl.cnt_shift) + (unsigned long long)qd;
@@ -168,9 +215,10 @@ __device__ __forceinline__ void append_rays_cta(int fresh_slot, uint32_t tab_bas
 // recast_depth_to_map_kernel phase 1 (dense_tsdf.py:188-213) + unproject_point_dep
 // (mapping_common.py:31-41).  One thread per SAMPLED pixel (the reference walks a
 // row per thread, :192-194); a warp covers an 8x4 tile of sampled pixels, a CTA 32x8;
-// blockIdx.z = frame of the batch.
+// blockIdx.z = frame of the batch.  Six CTAs per SM (40 registers): each CTA is one chain of dependent round trips
+// (depth load, index probe, CAS, ray append), so resident CTAs, not bandwidth, set the kernel's rate.
 // ---------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) k_bucket_depth(const uint16_t* __restrict__ depth, int frame_stride, int row_mul, int w, int hh, int ww,
+__global__ void __launch_bounds__(256, 6) k_bucket_depth(const uint16_t* __restrict__ depth, int frame_stride, int row_mul, int w, int hh, int ww,
                                                        const __grid_constant__ TsBatch batch, TsIntrin in, int agg_ok,
                                                        TsBucket* buckets, uint4* bcol, unsigned long long* bidx, uint32_t bucket_cap,
                                                        TsBucketLaunch bl, uint32_t* ray_list, int* n_rays, uint32_t ray_cap, TsCounters* ctr, int* err,
@@ -190,9 +238,12 @@ __global__ void __launch_bounds__(256) k_bucket_depth(const uint16_t* __restrict
     const float df = (float)d;
     if (d != 0 && !(df > in.dmax_mm || df < in.dmin_mm)) {  // :196-199
       valid = true;
-      dep = df / 1000.0f;                                    // :201
-      const float x = ((float)i - in.cx) * dep / in.fx;     // mapping_common.py:37-40
-      const float y = ((float)j - in.cy) * dep / in.fy;
+      // the quotients of the reference, correctly rounded without IEEE division: df / 1000 for every uint16 df
+      // (tests/test_gpu_bucket_merge.py checks all of them), t / fx and t / fy where ts_fill_intrin proved the form
+      dep = div_vs(df, 1000.0f, 1.0f / 1000.0f);             // :201
+      const float tx = ((float)i - in.cx) * dep, ty = ((float)j - in.cy) * dep;  // mapping_common.py:37-40
+      const float x = in.fdiv ? div_vs(tx, in.fx, in.rfx) : tx / in.fx;
+      const float y = in.fdiv ? div_vs(ty, in.fy, in.rfy) : ty / in.fy;
       const TsFrame& fr = batch.f[f];
       px = (fr.R[0] * x + fr.R[1] * y) + fr.R[2] * dep;     // :203 input_R @ pt (rotation only)
       py = (fr.R[3] * x + fr.R[4] * y) + fr.R[5] * dep;
@@ -209,14 +260,14 @@ __global__ void __launch_bounds__(256) k_bucket_depth(const uint16_t* __restrict
   const unsigned nv = __popc(__ballot_sync(0xffffffffu, valid));
   const int fresh = bucket_accumulate(valid, bidx + (size_t)tz * bucket_cap, bucket_cap - 1, (uint32_t)tz * bucket_cap, buckets + (size_t)tz * bucket_cap,
                                       bcol ? bcol + (size_t)tz * bucket_cap : nullptr, bl.cnt ? bl.cnt + (size_t)tz * bucket_cap : nullptr, bucket_cap,
-                                      ((blockIdx.y * gridDim.x + blockIdx.x) * 8u + (uint32_t)wid) * 32u, bl, px, py, pz, dep, in.vs, agg_ok != 0,
-                                      err, tex != nullptr, cr, cg, cb);
+                                      (blockIdx.y * gridDim.x + blockIdx.x) * 256u, bl, px, py, pz, dep, in.vs, in.rvs, agg_ok != 0, err,
+                                      tex != nullptr, cr, cg, cb);
   append_rays_cta(fresh, (uint32_t)tz * bucket_cap, nv, ray_list, n_rays, ray_cap, ctr, err);
   if (blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) atomicAdd(&ctr->n_px, (unsigned long long)(hh * ww));
 }
 
 // K1b: point cloud -> buckets.  recast_pcl_to_map_kernel (dense_tsdf.py:167-185).
-__global__ void __launch_bounds__(256) k_bucket_points(const float* __restrict__ xyz, int n, const __grid_constant__ TsBatch batch,
+__global__ void __launch_bounds__(256, 6) k_bucket_points(const float* __restrict__ xyz, int n, const __grid_constant__ TsBatch batch,
                                                         TsIntrin in, int agg_ok, TsBucket* buckets, uint4* bcol, unsigned long long* bidx,
                                                         uint32_t bucket_cap, uint32_t rec_cap, TsBucketLaunch bl, uint32_t* ray_list, int* n_rays, uint32_t ray_cap, TsCounters* ctr,
                                                         int* err, const uint8_t* __restrict__ rgb) {
@@ -235,8 +286,8 @@ __global__ void __launch_bounds__(256) k_bucket_points(const float* __restrict__
     if (rgb) { cr = rgb[3 * (size_t)t]; cg = rgb[3 * (size_t)t + 1]; cb = rgb[3 * (size_t)t + 2]; }  // :179-182
   }
   const unsigned nv = __popc(__ballot_sync(0xffffffffu, valid));
-  const int fresh = bucket_accumulate(valid, bidx, bucket_cap - 1, 0u, buckets, bcol, bl.cnt, rec_cap, (uint32_t)(t & ~31), bl, px, py, pz, len, in.vs,
-                                      agg_ok != 0, err, rgb != nullptr, cr, cg, cb);  // :183/:185
+  const int fresh = bucket_accumulate(valid, bidx, bucket_cap - 1, 0u, buckets, bcol, bl.cnt, rec_cap, blockIdx.x * 256u, bl, px, py, pz, len, in.vs,
+                                      in.rvs, agg_ok != 0, err, rgb != nullptr, cr, cg, cb);  // :183/:185
   append_rays_cta(fresh, 0u, nv, ray_list, n_rays, ray_cap, ctr, err);
   if (t == 0) atomicAdd(&ctr->n_px, (unsigned long long)n);
 }
@@ -892,7 +943,7 @@ int ts_integrate_depth_impl(tslam_tsdf_t* m, const uint16_t* depth, int mem, int
       tsrc = m->tex_stage;
     }
     dim3 grid1((ww + 31) / 32, (hh + 7) / 8, nf);
-    if ((size_t)grid1.x * grid1.y * 256 > m->bucket_cap) {  // every 8x4-pixel warp tile owns 32 bucket records of its frame
+    if ((size_t)grid1.x * grid1.y * 256 > m->bucket_cap) {  // every 32x8-pixel CTA tile owns 256 bucket records of its frame
       ts_set_error("frame %dx%d (sampled %dx%d) has too many partial pixel tiles for max_image_pixels=%d", h, w, hh, ww, m->cfg.max_image_pixels);
       return TSLAM_E_INVALID;
     }
@@ -936,7 +987,7 @@ extern "C" int tslam_tsdf_integrate_points_rgb(tslam_tsdf_t* m, const float* xyz
   }
   const uint32_t bshift = 31;  // every ray belongs to batch.f[0]
   const uint32_t cap_total = (uint32_t)TSLAM_MAX_BATCH * m->bucket_cap;  // power of two
-  const uint32_t rec_cap = ((uint32_t)n + 31u) & ~31u;  // a warp's slots start at its first point
+  const uint32_t rec_cap = (uint32_t)n;  // a bucket's record slot is the index of the point whose thread owns its CTA sums
   return ts_integrate_launch(m, st, batch, bshift, (uint64_t)n, flags, [&](const TsBucketLaunch& bl, int agg_ok) {
     k_bucket_points<<<(n + 255) / 256, 256, 0, st>>>(src, n, batch, m->in, agg_ok, m->buckets, m->bcol, m->bidx, cap_total, rec_cap, bl, m->ray_list,
                                                       m->n_rays, m->ray_list_cap, m->counters, m->g.err, csrc);

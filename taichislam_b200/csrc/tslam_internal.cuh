@@ -336,6 +336,8 @@ struct TsIntrin {
   float dmin_mm, dmax_mm;  // f32(min_ray*1000), f32(max_ray*1000)
   float vs;
   float rvs;               // RN(1/vs), for the exact FMA division in the march loop
+  float rfx, rfy;          // RN(1/fx), RN(1/fy): div_vs(t, fx, rfx) unprojects a pixel when fdiv is set
+  int fdiv;                // div_vs is correctly rounded for every dividend with divisor fx and with fy (ts_fill_intrin)
   float max_steps;         // f32(max_ray_length / voxel_scale)
   float max_ray;           // f32(max_ray_length)
   int internal_voxels;

@@ -11,6 +11,8 @@
 #include <cstring>
 #include <cstdlib>
 #include <cmath>
+#include <mutex>
+#include <unordered_map>
 #include <vector>
 #include <cuda_fp16.h>
 #include "tslam_internal.cuh"
@@ -72,9 +74,38 @@ static void fill_jet_host(float* cm) {
   }
 }
 
+// Whether div_vs(a, b, RN(1/b)) equals the IEEE quotient a / b for every f32 a whose quotient and residual stay normal
+// (|a| within about 2^+-100 of b).  Scaling a by a power of two scales q0, the residual and the result alike, so the
+// 2^23 significands of [1, 2) decide it.  About 70 ms per divisor; the answers are kept, since handles are created
+// and re-calibrated with a handful of focal lengths.
+static bool ts_fdiv_exact(float b) {
+  static std::mutex mu;
+  static std::unordered_map<uint32_t, bool> known;
+  uint32_t bb;
+  std::memcpy(&bb, &b, 4);
+  std::lock_guard<std::mutex> lock(mu);
+  const auto it = known.find(bb);
+  if (it != known.end()) return it->second;
+  bool ok = std::isnormal(b) && std::isnormal(1.0f / b);
+  const volatile float vb = b;  // a / vb: the IEEE division, not a multiplication by a folded reciprocal
+  const float r = 1.0f / b;
+  for (uint32_t s = 0; ok && s < (1u << 23); ++s) {
+    const uint32_t ab = 0x3f800000u | s;
+    float a;
+    std::memcpy(&a, &ab, 4);
+    const float q0 = a * r;
+    const float q1 = std::fmaf(std::fmaf(-q0, b, a), r, q0);
+    ok = q1 == a / vb;
+  }
+  known.emplace(bb, ok);
+  return ok;
+}
+
 static void ts_fill_intrin(tslam_tsdf* m) {
   const tslam_tsdf_config_t& c = m->cfg;
   m->in.fx = (float)c.fx; m->in.fy = (float)c.fy; m->in.cx = (float)c.cx; m->in.cy = (float)c.cy;
+  m->in.rfx = 1.0f / m->in.fx; m->in.rfy = 1.0f / m->in.fy;
+  m->in.fdiv = ts_fdiv_exact(m->in.fx) && ts_fdiv_exact(m->in.fy);
   m->in.dmin_mm = (float)(c.min_ray_length * 1000.0);
   m->in.dmax_mm = (float)(c.max_ray_length * 1000.0);
   m->in.vs = (float)c.voxel_scale;

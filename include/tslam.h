@@ -188,7 +188,8 @@ int64_t tslam_tsdf_launch_count(tslam_tsdf_t* m);
 int tslam_tsdf_set_profiling(tslam_tsdf_t* m, int on);
 int tslam_tsdf_kernel_ms(tslam_tsdf_t* m, int32_t n, float* ms3, int32_t* n_out);
 /* Same ring, 7 columns per launch: bucket, ray march (all its kernels), commit, then the ray march split into
- * ray set-up + segment count / scan / segment fill / block march (tslam_march.cu; zeros for the legacy kernel). */
+ * ray set-up + segment count / scan / segment fill / block march (tslam_march.cu; zeros for textured maps, which
+ * march with one thread per ray). */
 int tslam_tsdf_kernel_ms2(tslam_tsdf_t* m, int32_t n, float* ms7, int32_t* n_out);
 /* Diagnostics of the block-binned ray march (process_new_pcl, dense_tsdf.py:236-270) since the last clear of
  * tslam_tsdf_get_stats: out6 = segments, work items, samples that took the exact-index path (fraction within

@@ -293,10 +293,11 @@ __global__ void __launch_bounds__(256, 6) k_bucket_points(const float* __restric
 }
 
 // ---------------------------------------------------------------------------
-// K2: ray march.  process_new_pcl (dense_tsdf.py:236-270).  One thread per live
-// bucket (= ray) of any frame of the batch; every step adds (w*d, w) to the voxel's
-// pending sums - the reference's racy RMW (:264-267) becomes an order-independent
-// sum that k_commit folds into (TSDF, W).
+// K2: ray march of textured maps.  process_new_pcl (dense_tsdf.py:236-270) incl. the colour
+// (:268-269).  One thread per live bucket (= ray) of any frame of the batch; every step adds
+// (w*d, w) to the voxel's pending sums - the reference's racy RMW (:264-267) becomes an
+// order-independent sum that k_commit_tma folds into (TSDF, W) - and raises the voxel's colour
+// word.  Untextured maps march with tslam_march.cu.
 //
 // Two accumulation paths:
 //  * far field: one 8-byte vector reduction REDG.E.ADD.F32x2 per step into the block's
@@ -314,8 +315,7 @@ __global__ void __launch_bounds__(256, 6) k_bucket_points(const float* __restric
 #define RM_WIN3 4096
 #define RM_FIX 16777216.0f   // 2^24
 #define RM_WIN_STEPS 18      // a sample >= 18 voxels from the sensor origin lies outside the +-8 voxel window on some axis
-#define RM_SMEM (RM_WIN3 * 16 + RM_TAB * 8)
-#define RM_SMEM_TEX (RM_SMEM + RM_WIN3 * 8)  // textured maps: + one 64-bit colour word per window voxel
+#define RM_SMEM (RM_WIN3 * 24 + RM_TAB * 8)  // A, B (lo/hi words) and the 64-bit colour word per window voxel, block table
 
 __device__ __forceinline__ void win_add(unsigned int* lo, int* hi, int x) {
   const unsigned int ux = (unsigned int)x;
@@ -324,7 +324,6 @@ __device__ __forceinline__ void win_add(unsigned int* lo, int* hi, int x) {
   if (c) atomicAdd(hi, c);
 }
 
-template <bool TEX>
 __global__ void __launch_bounds__(RM_THREADS, 2) k_raymarch(const __grid_constant__ TsBatch batch, TsIntrin in, TsGrid g,
                                                               const TsBucket* buckets, const uint4* bcol, unsigned long long* bidx,
                                                               uint32_t bucket_shift, TsBucketLaunch bl, const uint32_t* __restrict__ ray_list, const int* __restrict__ n_rays_p, uint32_t ray_cap,
@@ -335,7 +334,7 @@ __global__ void __launch_bounds__(RM_THREADS, 2) k_raymarch(const __grid_constan
   unsigned int* const w_blo = win + 2 * RM_WIN3;
   int* const w_bhi = (int*)(win + 3 * RM_WIN3);
   unsigned long long* const btab = (unsigned long long*)(win + 4 * RM_WIN3);
-  unsigned long long* const w_cw = btab + RM_TAB;  // TEX only: colour word of every window voxel
+  unsigned long long* const w_cw = btab + RM_TAB;  // colour word of every window voxel
   __shared__ int s_org[4];   // window origin (voxels) and submap
   __shared__ int s_blk[8];   // the <= 8 blocks the window overlaps
 
@@ -346,8 +345,7 @@ __global__ void __launch_bounds__(RM_THREADS, 2) k_raymarch(const __grid_constan
   const float rvs = in.rvs;
   for (int e = threadIdx.x; e < 4 * RM_WIN3; e += RM_THREADS) win[e] = 0u;
   for (int e = threadIdx.x; e < RM_TAB; e += RM_THREADS) btab[e] = TS_EMPTY;
-  if (TEX)
-    for (int e = threadIdx.x; e < RM_WIN3; e += RM_THREADS) w_cw[e] = 0ull;
+  for (int e = threadIdx.x; e < RM_WIN3; e += RM_THREADS) w_cw[e] = 0ull;
 
   // control flow is kept WARP-UNIFORM (32 consecutive rays per warp, march to the longest ray, predicated lanes)
   for (uint32_t base = blockIdx.x * RM_THREADS; base < n_rays; base += gridDim.x * RM_THREADS) {
@@ -363,20 +361,16 @@ __global__ void __launch_bounds__(RM_THREADS, 2) k_raymarch(const __grid_constan
     const uint32_t r = base + threadIdx.x;
     bool live = r < n_rays;
     int cnt = 0, s = 0, n = 0;
-    long long sx = 0, sy = 0, sz = 0, sd = 0;
     unsigned int ccr = 0, ccg = 0, ccb = 0;
     uint32_t f = 0;
+    TsBucketSums b = {};
     if (live) {
       const uint32_t id = ray_list[r];
       f = id >> bucket_shift;
-      const TsBucket* bk = &buckets[id];
-      sx = bk->sx; sy = bk->sy; sz = bk->sz;
-      const unsigned long long cd = bk->cd;
-      cnt = bl.cnt ? (int)bl.cnt[id] : (int)(cd >> bl.cnt_shift);
-      sd = bl.cnt ? (long long)cd : (long long)(cd & ((1ull << bl.cnt_shift) - 1ull));
-      if (TEX) { const uint4 c = bcol[id]; ccr = c.x; ccg = c.y; ccb = c.z; }
-      // PCLroot.deactivate_all() (:163): clearing mode hands the index entry back zeroed
-      if (bl.bpos) bidx[bl.bpos[id]] = 0ull;
+      b = ts_read_bucket(buckets, bidx, bl, id);
+      cnt = b.cnt;
+      const uint4 c = bcol[id];
+      ccr = c.x; ccg = c.y; ccb = c.z;
       live = cnt > 0;  // :240
     }
     float mx = 0.f, my = 0.f, mz = 0.f, ux = 0.f, uy = 0.f, uz = 0.f, Tx = 0.f, Ty = 0.f, Tz = 0.f, Px = 0.f, Py = 0.f, Pz = 0.f,
@@ -387,35 +381,29 @@ __global__ void __launch_bounds__(RM_THREADS, 2) k_raymarch(const __grid_constan
       my_rays++;
       const TsFrame& fr = batch.f[f];
       s = fr.submap;
-      const double den = (double)cnt * FIXQ_D;
-      mx = (float)((double)sx / den);  // pos_s2p = sum/c (:243), exact mean
-      my = (float)((double)sy / den);
-      mz = (float)((double)sz / den);
-      const float zc = (float)((double)sd / den);  // z = new_pcl_z/c (:247)
-      const float L = sqrtf((mx * mx + my * my) + mz * mz);  // :244
-      if (L > 0.0f) {
-        ux = mx / L; uy = my / L; uz = mz / L;  // :245
+      TsRayGeom rg;
+      if (ts_ray_geom(b, fr.T, in, rg)) {
+        mx = rg.mx; my = rg.my; mz = rg.mz;
+        ux = rg.ux; uy = rg.uy; uz = rg.uz;
         Tx = fr.T[0]; Ty = fr.T[1]; Tz = fr.T[2];
-        Px = mx + Tx; Py = my + Ty; Pz = mz + Tz;  // :246
-        // occupy[sxyz_to_ijk(pos_p)] = 1 (:248)
-        const int oi = iroundf(Px / vs), oj = iroundf(Py / vs), ok = iroundf(Pz / vs);
-        if (ts_in_bounds(g, oi, oj, ok)) {
-          cur_key = ts_pack_key(s, oi >> TS_BSHIFT, oj >> TS_BSHIFT, ok >> TS_BSHIFT);
+        Px = rg.Px; Py = rg.Py; Pz = rg.Pz;
+        if (ts_in_bounds(g, rg.oi, rg.oj, rg.ok)) {  // occupy[sxyz_to_ijk(pos_p)] = 1 (:248)
+          cur_key = ts_pack_key(s, rg.oi >> TS_BSHIFT, rg.oj >> TS_BSHIFT, rg.ok >> TS_BSHIFT);
           cur_blk = ts_get_or_alloc_cached(g, cur_key);
           if (cur_blk >= 0) {
-            g.occ[(size_t)cur_blk * TS_B3 + ts_voxel_off(oi, oj, ok)] = 1;
+            g.occ[(size_t)cur_blk * TS_B3 + ts_voxel_off(rg.oi, rg.oj, rg.ok)] = 1;
             ts_mark_dirty(g, cur_blk);  // touched blocks are listed even when only `occupy` changed
           }
         }
-        n = (int)fminf(L / vs + (float)in.internal_voxels, in.max_steps);  // :249-251
-        wgt = 1.0f / (zc * zc);  // w_x_p(d>=0, z) (:216-225, :262)
+        n = rg.n;
+        wgt = rg.w;
       }
     }
     const bool win_ok = (s == ws) && wgt < 120.0f;  // fixed-point range of the window words
-    // textured maps: every sample also raises the voxel's colour word [frame seq : 22][closeness : 12][rgb : 30]
-    // (atomicMax; decoded by k_commit) - in the window's shared-memory copy for near-field samples
+    // every sample also raises the voxel's colour word [frame seq : 22][closeness : 12][rgb : 30] (atomicMax; decoded
+    // by the commit) - in the window's shared-memory copy for near-field samples
     unsigned long long cw_hi = 0ull;
-    if (TEX && live && cnt > 0) {
+    if (live) {
       const float c = (float)cnt;
       const int qr = min(1023, (int)((((float)ccr / c) / 255.0f) * 1023.0f + 0.5f));  // sum_color/c/255 (:269), 10 bits
       const int qg = min(1023, (int)((((float)ccg / c) / 255.0f) * 1023.0f + 0.5f));
@@ -457,10 +445,8 @@ __global__ void __launch_bounds__(RM_THREADS, 2) k_raymarch(const __grid_constan
           const int e = (int)((dx << 8) | (dy << 4) | dz);
           win_add(&w_alo[e], &w_ahi[e], __float2int_rn(a * RM_FIX));
           win_add(&w_blo[e], &w_bhi[e], wq);
-          if (TEX) {
-            const int cl = min(4095, (int)(fabsf(ds) / vs * 16.0f));
-            atomicMax(&w_cw[e], cw_hi | ((unsigned long long)(4095 - cl) << 30));
-          }
+          const int cl = min(4095, (int)(fabsf(ds) / vs * 16.0f));
+          atomicMax(&w_cw[e], cw_hi | ((unsigned long long)(4095 - cl) << 30));
           my_updates++;
         }
         far = inb && !in_win;
@@ -474,10 +460,9 @@ __global__ void __launch_bounds__(RM_THREADS, 2) k_raymarch(const __grid_constan
       if (far && cur_blk >= 0) {  // cur_blk < 0: pool exhausted (error flag raised)
         const size_t vo = (size_t)cur_blk * TS_B3 + ts_voxel_off(xi, yi, zi);
         red_add_f32x2(&g.acc[vo], a, wgt);  // :264,:267
-        if (TEX) {  // color[xi] = ray colour (:268-269): latest frame, then the sample closest to its surface point
-          const int cl = min(4095, (int)(fabsf(ds) / vs * 16.0f));
-          ts_red_max_u64(&g.cword[vo], cw_hi | ((unsigned long long)(4095 - cl) << 30));
-        }
+        // color[xi] = ray colour (:268-269): latest frame, then the sample closest to its surface point
+        const int cl = min(4095, (int)(fabsf(ds) / vs * 16.0f));
+        ts_red_max_u64(&g.cword[vo], cw_hi | ((unsigned long long)(4095 - cl) << 30));
         my_updates++;
       }
     };
@@ -531,10 +516,8 @@ __global__ void __launch_bounds__(RM_THREADS, 2) k_raymarch(const __grid_constan
       const float A = (float)(((double)ahi * 4294967296.0 + (double)alo) * (1.0 / 16777216.0));
       const float B = (float)(((double)bhi * 4294967296.0 + (double)blo) * (1.0 / 16777216.0));
       red_add_f32x2(&g.acc[(size_t)blk * TS_B3 + ts_voxel_off(xi, yi, zi)], A, B);
-      if (TEX) {
-        ts_red_max_u64(&g.cword[(size_t)blk * TS_B3 + ts_voxel_off(xi, yi, zi)], w_cw[e]);
-        w_cw[e] = 0ull;
-      }
+      ts_red_max_u64(&g.cword[(size_t)blk * TS_B3 + ts_voxel_off(xi, yi, zi)], w_cw[e]);
+      w_cw[e] = 0ull;
     }
     __syncthreads();
   }
@@ -554,8 +537,12 @@ __global__ void __launch_bounds__(RM_THREADS, 2) k_raymarch(const __grid_constan
 // ---------------------------------------------------------------------------
 // K3: commit.  Folds the pending (sum w*d, sum w) of every dirty block into
 // (TSDF, W_TSDF):  T' = (T*W + A)/(W + B), W' = min(W + B, Wmax), observed = 1
-// (dense_tsdf.py:264-267 applied once per voxel per batch).  One CTA per block,
-// fully coalesced float2 streams.  clamp=0 is the fusion variant (:274-278).
+// (dense_tsdf.py:264-267 applied once per voxel per batch).  clamp=0 is the fusion variant (:274-278).
+// Each dirty block's two 32 KB planes are moved by the bulk-copy engine (cp.async.bulk: SASS UBLKCP) instead of
+// per-thread loads/stores: one elected thread arms an mbarrier with the expected byte count and issues two
+// global->shared bulk copies; the CTA waits on the barrier, folds the sums in shared memory, and the elected thread
+// streams the updated (TSDF, W) plane and a zeroed accumulator plane back with shared->global bulk stores.  Textured
+// maps also set the colour of every touched voxel, per thread in global memory (the colour planes are not copied).
 // ---------------------------------------------------------------------------
 // The last CTA to finish (every CTA read n_dirty at its start) sets the dirty-list count and `ticket` back to zero.
 __device__ __forceinline__ void commit_done(const TsGrid& g, int* ticket) {
@@ -568,52 +555,6 @@ __device__ __forceinline__ void commit_done(const TsGrid& g, int* ticket) {
   __syncthreads();
   if (s_last && threadIdx.x == 0) { *g.n_dirty = 0; *ticket = 0; }
 }
-__global__ void __launch_bounds__(256) k_commit(TsGrid g, int clamp, int fused_obs, unsigned long long* stamp, unsigned long long seq, int* ticket) {
-  cudaGridDependencySynchronize();  // the dirty list comes from k_collect_dirty
-  const int nd = *g.n_dirty;
-  for (int q = blockIdx.x; q < nd; q += gridDim.x) {
-    const int blk = g.dirty_list[q];
-    float2* acc = g.acc + (size_t)blk * TS_B3;
-    float2* tw = g.tw + (size_t)blk * TS_B3;
-    uint8_t* obs = g.obs + (size_t)blk * TS_B3;
-    for (int v = threadIdx.x; v < TS_B3; v += blockDim.x) {
-      const float2 a = acc[v];
-      // integrate: a voxel is touched iff sum w > 0.  fusion: also voxels whose observed
-      // flag was raised by a zero-weight corner (0/0 = NaN is reference behaviour).
-      const bool touched = fused_obs ? (a.y != 0.0f || a.x != 0.0f || obs[v] == 2) : (a.y > 0.0f);
-      if (touched) {
-        const float2 o = tw[v];
-        const float wn = o.y + a.y;
-        float2 r;
-        r.x = (o.x * o.y + a.x) / wn;
-        r.y = clamp ? fminf(wn, WMAX) : wn;
-        tw[v] = r;
-        obs[v] = 1;
-        acc[v] = make_float2(0.0f, 0.0f);
-        if (g.col) {
-          float4* col = g.col + (size_t)blk * TS_B3;
-          if (fused_obs) {  // fusion: col holds sum(w*c) (:277) -> weighted mean
-            float4 c = col[v];
-            c.x = c.x / wn; c.y = c.y / wn; c.z = c.z / wn;
-            col[v] = c;
-          } else {
-            const unsigned long long cw = g.cword[(size_t)blk * TS_B3 + v];
-            if (cw) col[v] = make_float4((float)((cw >> 20) & 1023) / 1023.0f, (float)((cw >> 10) & 1023) / 1023.0f, (float)(cw & 1023) / 1023.0f, 0.0f);
-          }
-        }
-      }
-    }
-    if (threadIdx.x == 0) { g.dirty_flag[blk] = 0; g.esdf_dirty[blk] = 1; stamp[blk] = seq; }
-  }
-  commit_done(g, ticket);
-}
-// ---------------------------------------------------------------------------
-// K3 (TMA variant): the same commit, with each dirty block's two 32 KB planes moved by the bulk-copy engine
-// (cp.async.bulk: SASS UBLKCP) instead of per-thread loads/stores: one elected thread arms an mbarrier with the
-// expected byte count and issues two global->shared bulk copies; the CTA waits on the barrier, folds the sums in
-// shared memory, and the elected thread streams the updated (TSDF, W) plane and a zeroed accumulator plane back
-// with shared->global bulk stores.
-// ---------------------------------------------------------------------------
 #define CM_PLANE_BYTES (TS_B3 * 8)
 #define CM_SMEM (2 * CM_PLANE_BYTES + 16)
 
@@ -672,6 +613,8 @@ __global__ void __launch_bounds__(256) k_commit_tma(TsGrid g, int clamp, int fus
     phase ^= 1;
     for (int v = threadIdx.x; v < TS_B3; v += blockDim.x) {
       const float2 a = s_acc[v];
+      // integrate: a voxel is touched iff sum w > 0.  fusion: also voxels whose observed
+      // flag was raised by a zero-weight corner (0/0 = NaN is reference behaviour).
       const bool touched = fused_obs ? (a.y != 0.0f || a.x != 0.0f || obs[v] == 2) : (a.y > 0.0f);
       if (touched) {
         const float2 o = s_tw[v];
@@ -682,6 +625,17 @@ __global__ void __launch_bounds__(256) k_commit_tma(TsGrid g, int clamp, int fus
         s_tw[v] = r;
         obs[v] = 1;
         s_acc[v] = make_float2(0.0f, 0.0f);
+        if (g.col) {
+          float4* col = g.col + (size_t)blk * TS_B3;
+          if (fused_obs) {  // fusion: col holds sum(w*c) (:277) -> weighted mean
+            float4 c = col[v];
+            c.x = c.x / wn; c.y = c.y / wn; c.z = c.z / wn;
+            col[v] = c;
+          } else {
+            const unsigned long long cw = g.cword[(size_t)blk * TS_B3 + v];
+            if (cw) col[v] = make_float4((float)((cw >> 20) & 1023) / 1023.0f, (float)((cw >> 10) & 1023) / 1023.0f, (float)(cw & 1023) / 1023.0f, 0.0f);
+          }
+        }
       }
     }
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy smem writes -> visible to the bulk engine
@@ -718,8 +672,7 @@ __global__ void k_reset_counters(int* n_rays) { *n_rays = 0; }
 
 // the kernels of this file that need more dynamic shared memory than the default limit
 int ts_integrate_init() {
-  TS_CUDA(cudaFuncSetAttribute(k_raymarch<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, RM_SMEM));
-  TS_CUDA(cudaFuncSetAttribute(k_raymarch<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, RM_SMEM_TEX));
+  TS_CUDA(cudaFuncSetAttribute(k_raymarch, cudaFuncAttributeMaxDynamicSharedMemorySize, RM_SMEM));
   TS_CUDA(cudaFuncSetAttribute(k_commit_tma, cudaFuncAttributeMaxDynamicSharedMemorySize, CM_SMEM));
   return TSLAM_OK;
 }
@@ -730,16 +683,11 @@ int ts_integrate_init() {
 // k_collect_dirty, then the commit, whose last CTA sets the dirty-list count back to zero (ticket: scratch_i[4]).  Both
 // are launched with programmatic dependent launch (ts_launch_pdl).
 int ts_launch_commit(tslam_tsdf* m, cudaStream_t st, int clamp, int fused) {
-  int grid = m->sm_count * 8;
   const int gc = (m->g.max_blocks + 255) / 256 < m->sm_count * 4 ? (m->g.max_blocks + 255) / 256 : m->sm_count * 4;
   TS_CUDA(ts_launch_pdl(k_collect_dirty, gc, 256, 0, st, m->g));
   TS_LAUNCH_CHECK(m);
-  static const bool plain_env = getenv("TSLAM_COMMIT_PLAIN") != nullptr;  // A/B switch for the non-TMA variant
-  const bool plain = plain_env || m->g.col != nullptr;  // textured maps: the per-thread variant also folds the colours
-  const unsigned long long seq = ++m->commit_seq;        // stamp of every block this commit writes (incremental mesh)
-  int* ticket = m->scratch_i + 4;
-  if (plain) TS_CUDA(ts_launch_pdl(k_commit, grid, 256, 0, st, m->g, clamp, fused, m->blk_stamp, seq, ticket));
-  else TS_CUDA(ts_launch_pdl(k_commit_tma, m->sm_count * 3, 256, CM_SMEM, st, m->g, clamp, fused, m->blk_stamp, seq, ticket));
+  const unsigned long long seq = ++m->commit_seq;  // stamp of every block this commit writes (incremental mesh)
+  TS_CUDA(ts_launch_pdl(k_commit_tma, m->sm_count * 3, 256, CM_SMEM, st, m->g, clamp, fused, m->blk_stamp, seq, m->scratch_i + 4));
   TS_LAUNCH_CHECK(m);
   return TSLAM_OK;
 }
@@ -885,18 +833,13 @@ static int ts_integrate_launch(tslam_tsdf* m, cudaStream_t st, const TsBatch& ba
   launch_bucket(bl, agg_ok);
   TS_LAUNCH_CHECK(m);
   if (pe) TS_CUDA(cudaEventRecord(pe[1], st));
-  if (ts_uses_binned_march(m)) {
+  if (!m->g.cword) {  // untextured maps: the block-binned march (tslam_march.cu)
     int rcm = ts_march_launch(m, st, batch, bshift, bl, pe ? pe + 4 : nullptr);  // clears n_rays itself
     if (rcm) return ts_bucket_abandon(m, st, rcm);
     if (pe) TS_CUDA(cudaEventRecord(pe[2], st));
   } else {
-    if (m->g.cword) {
-      k_raymarch<true><<<m->sm_count, RM_THREADS, RM_SMEM_TEX, st>>>(batch, m->in, m->g, m->buckets, m->bcol, m->bidx, bshift, bl, m->ray_list,
-                                                                     m->n_rays, m->ray_list_cap, m->counters);
-    } else {
-      k_raymarch<false><<<(m->sm_count - m->rm_reserve) * 2, RM_THREADS, RM_SMEM, st>>>(batch, m->in, m->g, m->buckets, m->bcol, m->bidx, bshift,
-                                                                                     bl, m->ray_list, m->n_rays, m->ray_list_cap, m->counters);
-    }
+    k_raymarch <<<m->sm_count, RM_THREADS, RM_SMEM, st>>>(batch, m->in, m->g, m->buckets, m->bcol, m->bidx, bshift, bl, m->ray_list, m->n_rays,
+                                                         m->ray_list_cap, m->counters);
     TS_LAUNCH_CHECK(m);
     if (pe) TS_CUDA(cudaEventRecord(pe[2], st));
     k_reset_counters<<<1, 1, 0, st>>>(m->n_rays);

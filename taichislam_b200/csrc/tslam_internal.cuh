@@ -368,6 +368,56 @@ struct TsBucketLaunch {
   uint32_t* bpos;           // clearing mode only: index entry of every opened record, zeroed by the consumer; else null
 };
 
+// The two ray set-ups (ray_setup, tslam_march.cu; k_raymarch, tslam_integrate.cu) read a bucket and form its ray
+// through these two functions, so that both know the record format once and round alike (the parity tests compare
+// their voxel indices bit for bit).
+struct TsBucketSums {
+  long long sx, sy, sz, sd;  // exact fixed-point sums of the points and of their depths
+  int cnt;                   // points in the bucket
+};
+// record `id`, read with two 16-byte loads.  The record needs no clearing (its next opener stores it whole); in clearing
+// mode its index entry is handed back zeroed (PCLroot.deactivate_all(), dense_tsdf.py:163).
+__device__ __forceinline__ TsBucketSums ts_read_bucket(const TsBucket* buckets, unsigned long long* bidx, const TsBucketLaunch& bl, uint32_t id) {
+  const uint4* q = reinterpret_cast<const uint4*>(&buckets[id]);  // sx sy | sz cd
+  const uint4 q0 = q[0], q1 = q[1];
+  if (bl.bpos) bidx[bl.bpos[id]] = 0ull;
+  TsBucketSums b;
+  b.sx = (long long)((unsigned long long)q0.x | ((unsigned long long)q0.y << 32));
+  b.sy = (long long)((unsigned long long)q0.z | ((unsigned long long)q0.w << 32));
+  b.sz = (long long)((unsigned long long)q1.x | ((unsigned long long)q1.y << 32));
+  const unsigned long long cd = (unsigned long long)q1.z | ((unsigned long long)q1.w << 32);
+  b.sd = bl.cnt ? (long long)cd : (long long)(cd & ((1ull << bl.cnt_shift) - 1ull));
+  b.cnt = bl.cnt ? (int)bl.cnt[id] : (int)(cd >> bl.cnt_shift);
+  return b;
+}
+// The ray of a bucket with cnt > 0 (process_new_pcl, dense_tsdf.py:240-251), seen from sensor origin T.  Returns false
+// when the mean has no positive length (the ray marches no step); the other fields are then unset.
+struct TsRayGeom {
+  float mx, my, mz;  // pos_s2p: the exact mean (:243)
+  float L;           // its length (:244)
+  float ux, uy, uz;  // unit direction (:245)
+  float Px, Py, Pz;  // pos_p = mean + T (:246)
+  int oi, oj, ok;    // occupy voxel sxyz_to_ijk(pos_p) (:248)
+  int n;             // march steps (:249-251)
+  float w;           // sample weight w_x_p(d >= 0, z) = 1/z^2 with z = new_pcl_z/c (:216-225, :247, :262)
+};
+__device__ __forceinline__ bool ts_ray_geom(const TsBucketSums& b, const float* T, const TsIntrin& in, TsRayGeom& r) {
+  const float vs = in.vs;
+  const double den = (double)b.cnt * FIXQ_D;
+  r.mx = (float)((double)b.sx / den);
+  r.my = (float)((double)b.sy / den);
+  r.mz = (float)((double)b.sz / den);
+  const float zc = (float)((double)b.sd / den);
+  r.L = sqrtf((r.mx * r.mx + r.my * r.my) + r.mz * r.mz);
+  if (!(r.L > 0.0f)) return false;
+  r.ux = r.mx / r.L; r.uy = r.my / r.L; r.uz = r.mz / r.L;
+  r.Px = r.mx + T[0]; r.Py = r.my + T[1]; r.Pz = r.mz + T[2];
+  r.oi = iroundf(r.Px / vs); r.oj = iroundf(r.Py / vs); r.ok = iroundf(r.Pz / vs);
+  r.n = (int)fminf(r.L / vs + (float)in.internal_voxels, in.max_steps);
+  r.w = 1.0f / (zc * zc);
+  return true;
+}
+
 struct TsCounters {  // device-side statistics (tslam_tsdf_get_stats)
   unsigned long long n_px, n_valid, n_rays, n_updates, n_oob;
   // block-binned ray march (tslam_march.cu): diagnostics, not part of the parity counters
@@ -489,7 +539,7 @@ struct tslam_tsdf {
   int esdf_full_needed, esdf_submap;  // the next update recomputes everything (first use, reset, bulk load) / submap of the kept state
   int esdf_tiled;      // tiled ESDF (tslam_esdf_tiled_*): 0 = none (plain update), 1 = begun, exchange in progress, 2 = ended
   void* mc_scratch;    // marching cubes: per-block triangle counts / offsets (allocated on first use)
-  // Change tracking for the incremental mesh (tslam_mesh_*, tslam_mc.cu).  Every commit (k_commit / k_commit_tma) and
+  // Change tracking for the incremental mesh (tslam_mesh_*, tslam_mc.cu).  Every commit (k_commit_tma) and
   // every ghost import (k_ghost_unpack) takes the next commit_seq and stores it in blk_stamp[] of each block it writes;
   // every other writer of the tw / obs / col planes, and whatever recycles pool slots, bumps mesh_epoch instead
   // (DESIGN.md section 4 lists them).
@@ -511,7 +561,6 @@ struct tslam_tsdf {
   size_t reg_blk_bytes;
   void* reg_pts;
   size_t reg_pts_bytes;
-  int march_mode;      // 0 = legacy k_raymarch, 1 = block-binned (default for untextured maps), env TSLAM_MARCH
   int march_verify;    // TSLAM_MARCH_VERIFY=1: every fast-path index is re-computed exactly, mismatches counted
   bool clamp_on_commit;
   // frame queue of the per-frame API (tslam_tsdf_queue_depth): double-buffered device staging fed by a copy stream
@@ -800,8 +849,6 @@ int ts_check_tex(tslam_tsdf* m, const uint8_t* tex, int th, int tw);  // a colou
 int ts_integrate_depth_impl(tslam_tsdf_t* m, const uint16_t* depth, int mem, int32_t n_frames, int32_t h, int32_t w, const float* R9s,
                             const float* T3s, const int32_t* submap_ids, int flags, void* stream, const uint8_t* tex = nullptr, int th = 0,
                             int tw = 0);
-// the integrate launch marches with tslam_march.cu (else k_raymarch): its dispatch, and how its profiling row reads
-static inline bool ts_uses_binned_march(const tslam_tsdf* m) { return m->march_mode && !m->g.cword; }
 // tslam_queue.cu: the per-frame queue's switches, copy stream and events of a new handle / their release
 int ts_queue_init(tslam_tsdf* m);
 void ts_queue_free(tslam_tsdf* m);
@@ -809,7 +856,7 @@ int ts_launch_queue(tslam_tsdf* m, cudaStream_t st);     // integrate the queued
 // tslam_esdf.cu: per-block exchange mark of the tiled ESDF ([max_blocks]; owned block: ESDF changed since it was last
 // packed, ghost block: ESDF unpacked since the last relax), or NULL before the first ESDF update
 int* ts_esdf_xmark(tslam_tsdf* m);
-// tslam_march.cu: block-binned ray march of the rays listed in m->ray_list (replaces k_raymarch<false>)
+// tslam_march.cu: block-binned ray march of the rays listed in m->ray_list (untextured maps)
 int ts_march_alloc(tslam_tsdf* m);
 void ts_march_free(tslam_tsdf* m);
 int ts_march_launch(tslam_tsdf* m, cudaStream_t st, const TsBatch& batch, uint32_t bucket_shift, const TsBucketLaunch& bl, cudaEvent_t* sub_ev);

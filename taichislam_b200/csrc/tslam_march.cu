@@ -23,7 +23,7 @@
 //                  recomputes round((u*j*vs + T)/vs) exactly as the reference states it (:253-254), so voxel
 //                  indices stay bit-exact; a sample whose exact voxel is not in the item's block takes a global
 //                  reduction.  At the end of the item every touched voxel is flushed with ONE coalesced
-//                  REDG.ADD.F32x2 into the block's `acc` plane (what k_commit folds into TSDF/W, :264-267).
+//                  REDG.ADD.F32x2 into the block's `acc` plane (what k_commit_tma folds into TSDF/W, :264-267).
 //                  Once the items run out, its CTAs take the generic path - the exact one-reduction-per-sample march
 //                  for what the binned path does not take: segments next to the volume boundary, rays with more than
 //                  65535 steps, workspace overflow - zero the fill counters, and the last CTA clears the control block.
@@ -57,48 +57,32 @@
 // ---------------------------------------------------------------------------
 // K2a: ray set-up (process_new_pcl :240-251), first stage of the counting walk: one bucket record -> unit direction,
 // length, weight, step count n, occupy flag (:248) and the 32-byte ray record + aux word the march kernels read,
-// stored at rays[r] / aux[r] and handed back in ra, rb, raux.  The bucket record needs no clearing (its next opener
-// stores it whole); in clearing mode its index entry is handed back zeroed (PCLroot.deactivate_all(), :163).
+// stored at rays[r] / aux[r] and handed back in ra, rb, raux.
 // ---------------------------------------------------------------------------
 __device__ __forceinline__ void ray_setup(const TsBatch& batch, const TsIntrin& in, const TsGrid& g, unsigned long long* btab, const TsBucket* buckets,
                                           unsigned long long* bidx, uint32_t bucket_shift, const TsBucketLaunch& bl, uint32_t id, uint32_t r,
                                           const TsMarchWs& w, unsigned int& my_rays, unsigned int& my_fmax, float4& ra, float4& rb, uint32_t& raux) {
   const float vs = in.vs;
   const uint32_t f = id >> bucket_shift;
-  const uint4* q = reinterpret_cast<const uint4*>(&buckets[id]);  // sx sy | sz cd
-  const uint4 q0 = q[0], q1 = q[1];
-  if (bl.bpos) bidx[bl.bpos[id]] = 0ull;
-  const long long sx = (long long)((unsigned long long)q0.x | ((unsigned long long)q0.y << 32));
-  const long long sy = (long long)((unsigned long long)q0.z | ((unsigned long long)q0.w << 32));
-  const long long sz = (long long)((unsigned long long)q1.x | ((unsigned long long)q1.y << 32));
-  const unsigned long long cd = (unsigned long long)q1.z | ((unsigned long long)q1.w << 32);
-  const long long sd = bl.cnt ? (long long)cd : (long long)(cd & ((1ull << bl.cnt_shift) - 1ull));
-  const int cnt = bl.cnt ? (int)bl.cnt[id] : (int)(cd >> bl.cnt_shift);
+  const TsBucketSums b = ts_read_bucket(buckets, bidx, bl, id);
   const TsFrame& fr = batch.f[f];
   struct { float ux, uy, uz, tx, ty, tz; int n, s; bool wide; } o;
   o.ux = o.uy = o.uz = o.tx = o.ty = o.tz = 0.0f;
   o.n = 0; o.s = fr.submap; o.wide = false;
   float L = 0.0f, wgt = 0.0f;
-  if (cnt > 0) {  // :240
+  if (b.cnt > 0) {  // :240
     my_rays++;
-    const double den = (double)cnt * FIXQ_D;
-    const float mx = (float)((double)sx / den);  // pos_s2p = sum/c (:243), exact mean
-    const float my = (float)((double)sy / den);
-    const float mz = (float)((double)sz / den);
-    const float zc = (float)((double)sd / den);  // z = new_pcl_z/c (:247)
-    L = sqrtf((mx * mx + my * my) + mz * mz);  // :244
-    if (L > 0.0f) {
-      o.ux = mx / L; o.uy = my / L; o.uz = mz / L;  // :245
-      const float Px = mx + fr.T[0], Py = my + fr.T[1], Pz = mz + fr.T[2];  // :246
-      // occupy[sxyz_to_ijk(pos_p)] = 1 (:248)
-      const int oi = iroundf(Px / vs), oj = iroundf(Py / vs), ok = iroundf(Pz / vs);
-      if (ts_in_bounds(g, oi, oj, ok)) {
-        const int bx = oi >> TS_BSHIFT, by = oj >> TS_BSHIFT, bz = ok >> TS_BSHIFT;
+    TsRayGeom rg;
+    if (ts_ray_geom(b, fr.T, in, rg)) {
+      L = rg.L;
+      o.ux = rg.ux; o.uy = rg.uy; o.uz = rg.uz;
+      if (ts_in_bounds(g, rg.oi, rg.oj, rg.ok)) {  // occupy[sxyz_to_ijk(pos_p)] = 1 (:248)
+        const int bx = rg.oi >> TS_BSHIFT, by = rg.oj >> TS_BSHIFT, bz = rg.ok >> TS_BSHIFT;
         const int blk = rm_lookup(g, btab, ts_pack_key(o.s, bx, by, bz), bx, by, bz);  // touched blocks are listed even when only `occupy` changed
-        if (blk >= 0) g.occ[(size_t)blk * TS_B3 + ts_voxel_off(oi, oj, ok)] = 1;
+        if (blk >= 0) g.occ[(size_t)blk * TS_B3 + ts_voxel_off(rg.oi, rg.oj, rg.ok)] = 1;
       }
-      o.n = (int)fminf(L / vs + (float)in.internal_voxels, in.max_steps);  // :249-251
-      wgt = 1.0f / (zc * zc);  // w_x_p(d>=0, z) (:216-225, :262)
+      o.n = rg.n;
+      wgt = rg.w;
       o.tx = (float)((double)fr.T[0] / (double)vs);
       o.ty = (float)((double)fr.T[1] / (double)vs);
       o.tz = (float)((double)fr.T[2] / (double)vs);
@@ -107,8 +91,6 @@ __device__ __forceinline__ void ray_setup(const TsBatch& batch, const TsIntrin& 
       const unsigned fb = __float_as_uint(fminf(fmaxf(wgt, wgt * dmax), 3.0e38f));  // non-negative floats order like their bits
       if (fb > my_fmax) my_fmax = fb;
       o.wide = o.n > 65535;
-    } else {
-      L = 0.0f;
     }
   }
   ra = make_float4(o.ux, o.uy, o.uz, L);

@@ -239,15 +239,9 @@ extern "C" int tslam_tsdf_create(const tslam_tsdf_config_t* cfg, tslam_tsdf_t** 
   fill_jet_host(cm.data());
   TS_CUDA(cudaMalloc(&m->colormap, cm.size() * 4));
   TS_CUDA(cudaMemcpy(m->colormap, cm.data(), cm.size() * 4, cudaMemcpyHostToDevice));
-  {
-    // ray march: block-binned shared-memory accumulation (tslam_march.cu) for untextured maps; TSLAM_MARCH=legacy
-    // keeps the round-1 kernel (one global reduction per sample) for A/B runs.  Textured maps use k_raymarch<true>.
-    const char* mm = getenv("TSLAM_MARCH");
-    m->march_mode = (m->cfg.texture_enabled || (mm && mm[0] == 'l') || m->cfg.max_ray_length / m->cfg.voxel_scale > 60000.0) ? 0 : 1;
-    m->march_verify = getenv("TSLAM_MARCH_VERIFY") != nullptr;
-    // (the march workspace - ~2 GB for 640x480 frames - is allocated by the first integrate launch: global maps that are
-    // only ever fused into never pay for it)
-  }
+  m->march_verify = getenv("TSLAM_MARCH_VERIFY") != nullptr;
+  // (the workspace of the block-binned march - ~2 GB for 640x480 frames - is allocated by the first integrate launch:
+  // global maps that are only ever fused into never pay for it)
   { int rci = ts_integrate_init(); if (rci) return rci; }
   TS_CUDA(cudaDeviceSynchronize());
   *out = m;
@@ -689,7 +683,7 @@ extern "C" int tslam_tsdf_set_profiling(tslam_tsdf_t* m, int on) {
 // recorded integrate launch, i < n (n <= TS_PROF_RING).  Returns the number of rows written in *n_out.
 // ms7[7*i + ...] = bucket, ray march (all of its kernels), commit, then the parts of the ray march: the interval between
 // the bucket kernel and the first march kernel (0: nothing runs there), set-up + segment count + class + scan, segment
-// fill, march (with the generic path and the resets).  The last four are 0 for launches of the legacy kernel.
+// fill, march (with the generic path and the resets).  The last four are 0 for textured maps (k_raymarch).
 // Both write `cols` columns per row (3 or 7), walking the profiling ring backwards from the last recorded launch.
 static int ts_kernel_ms(tslam_tsdf* m, int32_t n, int cols, float* ms, int32_t* n_out) {
   if (!m || !ms || !n_out || !m->ev) return TSLAM_E_INVALID;
@@ -701,7 +695,7 @@ static int ts_kernel_ms(tslam_tsdf* m, int32_t n, int cols, float* ms, int32_t* 
     float* row = ms + cols * i;
     for (int q = 0; q < 3; q++) TS_CUDA(cudaEventElapsedTime(&row[q], pe[q], pe[q + 1]));
     for (int q = 3; q < cols; q++) row[q] = 0.0f;
-    if (cols == 7 && ts_uses_binned_march(m)) {  // pe[4], pe[5]: after the scan and after the scattering walk (ts_march_launch)
+    if (cols == 7 && !m->g.cword) {  // pe[4], pe[5]: after the scan and after the scattering walk (ts_march_launch)
       TS_CUDA(cudaEventElapsedTime(&row[4], pe[1], pe[4]));
       TS_CUDA(cudaEventElapsedTime(&row[5], pe[4], pe[5]));
       TS_CUDA(cudaEventElapsedTime(&row[6], pe[5], pe[2]));

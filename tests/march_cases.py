@@ -102,8 +102,17 @@ def tiny_weights(rng):
     return dict(pts=p, T=np.float32([0.37, -0.11, 0.05]), vs=vs, N=640, Nz=640, max_ray_length=64.0)
 
 
+def fine_long(rng):
+    """vs = 0.2 mm with a 12.5 m range (max_ray_length / vs = 62500 steps) in a 5 cm volume: points up to 0.75 m away
+    (3750 voxels: the bucket key reaches 4095), so that most samples of a ray fall outside the volume."""
+    vs = 0.0002
+    d = rng.normal(size=(2000, 3))
+    p = one_per_bucket(snap(d / np.linalg.norm(d, axis=1, keepdims=True) * rng.uniform(0.3, 0.75, (2000, 1))), vs)
+    return dict(pts=p, T=np.float32([0.0013, -0.0021, 0.0004]), vs=vs, N=256, Nz=256, max_ray_length=12.5)
+
+
 CASES = {"hot_bundle": hot_bundle, "ties_and_axes": ties_and_axes, "short_rays": short_rays, "anisotropic": anisotropic,
-         "tiny_weights": tiny_weights}
+         "tiny_weights": tiny_weights, "fine_long": fine_long}
 
 
 def make_case(name, seed=0):

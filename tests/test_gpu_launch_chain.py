@@ -44,9 +44,10 @@ def test_generic_path_in_the_march_tail(seg_cap, monkeypatch):
     compare_voxels(g.gather(), o.gather(), 2e-3 if seg_cap else TOL)
 
 
-def test_march_stats_match_a_reference_run(monkeypatch):
+def test_march_stats_match_a_reference_run():
     """n_seg_guard stays 0 and n_generic / n_updates are the same on every run of the same launches; n_updates is the
-    one-thread-per-ray march's."""
+    canonical oracle's."""
+    from oracle.oracle import OracleTSDF
     from taichislam_b200.tsdf_handle import TsdfHandle
     d = syn.scene_room()  # N = 200: rays reach the volume boundary, the generic path has work
     Rs = np.stack([rot_xyz(0.1, -0.15 + 0.05 * q, 0.3) for q in range(4)])
@@ -57,10 +58,11 @@ def test_march_stats_match_a_reference_run(monkeypatch):
         g.integrate_depth(np.stack([d] * 4), Rs, Ts)
         g.sync()
         runs.append((g.stats(), g.march_stats()))
-    monkeypatch.setenv("TSLAM_MARCH", "legacy")
-    ref = TsdfHandle(200, 200, K=syn.K_DEPTH, is_global_map=True)
-    ref.integrate_depth(np.stack([d] * 4), Rs, Ts)
-    ref.sync()
+    # num_voxel_per_blk_axis = 1 and a map scale half a voxel short of 200 voxels: N = Nz = 200 exactly
+    ref = OracleTSDF(map_scale=[199.5 * 0.05, 199.5 * 0.05], num_voxel_per_blk_axis=1, K=syn.K_DEPTH, is_global_map=True)
+    assert (ref.N, ref.Nz) == (200, 200)
+    for q in range(4):
+        ref.integrate_depth(Rs[q], Ts[q], d, commit=(q == 3))
     (s0, m0), (s1, m1) = runs
     assert m0["n_seg_guard"] == 0 and m1["n_seg_guard"] == 0
     assert m0["n_generic"] > 0
@@ -95,7 +97,7 @@ def test_back_to_back_launches_equal_one_at_a_time():
 
 
 def test_point_cloud_and_textured_launches():
-    """Point clouds take the same chain (one frame); textured maps the per-thread commit.  Both against the oracle, twice in
+    """Point clouds take the same chain (one frame); textured maps k_raymarch and the colour commit.  Both against the oracle, twice in
     a row (the second launch starts from what the first one's tail cleared)."""
     rng = np.random.default_rng(11)
     u = rng.normal(size=(20000, 3))

@@ -21,7 +21,7 @@ def gpu_map(case, **kw):
                       internal_voxels=case["internal_voxels"], is_global_map=True, **kw)
 
 
-@pytest.mark.parametrize("name", ["hot_bundle", "ties_and_axes", "short_rays", "anisotropic", "tiny_weights"])
+@pytest.mark.parametrize("name", ["hot_bundle", "ties_and_axes", "short_rays", "anisotropic", "tiny_weights", "fine_long"])
 def test_binned_march_matches_reference(name):
     c = make_case(name)
     ref = reference_of(c)
@@ -37,6 +37,8 @@ def test_binned_march_matches_reference(name):
         assert ms["n_items"] >= 5 and ref["count"].max() >= 20000
     if name == "tiny_weights":
         assert ms["n_fallback"] >= ref["n_tiny"] > 0, "the tiny-weight rays did not take the f32 global path"
+    if name == "fine_long":
+        assert ms["n_items"] > 0
 
 
 def test_submap_1023_next_to_submap_0():
@@ -107,7 +109,7 @@ def _queue(g, d, Rs, Ts):
     capi.check(g.L.tslam_tsdf_flush(g.h, capi.stream_ptr()))
 
 
-PATHS = {"default": {}, "legacy": {"TSLAM_MARCH": "legacy"}, "generic": {"TSLAM_SEG_CAP": "3000"},
+PATHS = {"default": {}, "generic": {"TSLAM_SEG_CAP": "3000"},
          "verify": {"TSLAM_MARCH_VERIFY": "1"}, "textured": {}, "queue": {}}
 
 
@@ -138,7 +140,7 @@ def test_sample_conservation(path, planes, monkeypatch):
         assert ms["n_generic"] > 0
     if path == "verify":
         assert ms["n_verify_bad"] == 0
-    if path in ("legacy", "textured"):
+    if path == "textured":
         assert ms["n_segs"] == 0
     assert_conserved(g, o, per, wf)
 

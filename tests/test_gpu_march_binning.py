@@ -9,6 +9,7 @@ from taichislam_b200 import synthetic as syn
 from util import as_dict_rows, compare_voxels, rot_xyz
 
 pytestmark = pytest.mark.gpu
+TOL = 1e-4
 
 SCENES = {"S1": lambda: syn.scene_plane(3.0), "S2": lambda: syn.scene_sphere(4.0), "S3": lambda: syn.scene_sphere(8.0),
           "S4": lambda: syn.scene_noise()}
@@ -21,22 +22,25 @@ def _stream(g, d, n, start=3):
 
 
 @pytest.mark.parametrize("scene", sorted(SCENES))
-def test_walks_agree_on_bench_scenes(scene, monkeypatch):
-    """64 frames of the bench stream into a 512^3 map; the map must equal the one of the one-thread-per-ray march."""
+def test_walks_agree_on_bench_scenes(scene):
+    """64 frames of the bench stream into a 512^3 map, in one launch; the map must equal the canonical oracle's."""
+    from oracle.oracle import OracleTSDF
     from taichislam_b200.tsdf_handle import TsdfHandle
     d = SCENES[scene]()
-    g = TsdfHandle(512, 512, K=syn.K_DEPTH, is_global_map=True)
+    o = OracleTSDF(map_scale=[25.6, 25.6], K=syn.K_DEPTH, is_global_map=True)
+    g = TsdfHandle(o.N, o.Nz, K=syn.K_DEPTH, is_global_map=True)
     _stream(g, d, 64)
     st, ms = g.stats(), g.march_stats()
     assert st["err_flags"] == 0
     assert ms["n_segs"] > 0 and ms["n_items"] > 0
     assert ms["n_seg_guard"] == 0
-    monkeypatch.setenv("TSLAM_MARCH", "legacy")
-    g1 = TsdfHandle(512, 512, K=syn.K_DEPTH, is_global_map=True)
-    _stream(g1, d, 64)
-    st1 = g1.stats()
-    assert (st["n_rays"], st["n_updates"], st["n_oob"]) == (st1["n_rays"], st1["n_updates"], st1["n_oob"])
-    _same_map(g, g1)
+    Rs, Ts = syn.stream_poses(64, start=3)
+    for q in range(64):  # the launch commits once, after its last frame
+        o.integrate_depth(Rs[q], Ts[q], d, commit=(q == 63))
+    so = o.stats()
+    for k in ("n_rays", "n_updates", "n_oob"):
+        assert st[k] == so[k], k
+    compare_voxels(g.gather(), o.gather(), TOL)
 
 
 def _same_map(g, g_f32):
@@ -64,7 +68,7 @@ def test_walks_agree_under_generic_poses(scene):
         assert st[k] == so[k], k
     assert st["err_flags"] == 0
     assert ms["n_segs"] > 0 and ms["n_seg_guard"] == 0
-    compare_voxels(g.gather(), o.gather(), 1e-4)
+    compare_voxels(g.gather(), o.gather(), TOL)
 
 
 def test_walks_agree_on_long_range_and_cut_blocks():

@@ -64,3 +64,8 @@ def test_cases_reach_their_edges():
     ref = reference_of(c)
     r = ray_setup(c["pts"], c["vs"], c["internal_voxels"], c["max_ray_length"])
     assert 0 < r["tiny"].sum() < r["tiny"].shape[0] and ref["n_tiny"] > 0
+    c = make_case("fine_long")
+    assert c["max_ray_length"] / c["vs"] > 60000
+    assert np.all(np.abs(np.round(c["pts"] / np.float32(c["vs"]))) <= 4095)  # inside the bucket key range
+    ref = reference_of(c)
+    assert ref["n_updates"] > 0 and ref["n_oob"] > ref["n_updates"]

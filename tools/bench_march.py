@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
-"""Ray-march A/B on one GPU: per-kernel CUDA-event times of the integrate launch for the four scenes, with the
-block-binned march (default) or the round-1 kernel (TSLAM_MARCH=legacy).  Prints one JSON line per scene.
+"""Per-kernel CUDA-event times of the integrate launch (block-binned march) for the four scenes on one GPU.  Prints one
+JSON line per scene.
 Usage: python tools/bench_march.py [reps]"""
 import json, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -10,7 +10,6 @@ from taichislam_b200.tsdf_handle import TsdfHandle
 
 PEAK = 6564.2
 reps = int(sys.argv[1]) if len(sys.argv) > 1 else 20
-mode = os.environ.get("TSLAM_MARCH", "binned")
 for name, d in (("S2 sphere 4 m", syn.scene_sphere(4.0)), ("S1 plane 3 m", syn.scene_plane(3.0)), ("S3 sphere 8 m", syn.scene_sphere(8.0)),
                 ("S4 noise 1.5-4.5 m", syn.scene_noise())):
     g = TsdfHandle(512, 512, K=syn.K_DEPTH, is_global_map=True)
@@ -33,7 +32,7 @@ for name, d in (("S2 sphere 4 m", syn.scene_sphere(4.0)), ("S1 plane 3 m", syn.s
     k = g.kernel_ms2(reps).mean(axis=0)
     rays, upd = st["n_rays"] / reps, st["n_updates"] / reps
     alg = 17.0 * rays + 9.0 * upd
-    out = {"scene": name, "march": mode, "frames_per_s": 64e3 / ms, "ms_per_64": ms, "rays": rays, "updates": upd,
+    out = {"scene": name, "frames_per_s": 64e3 / ms, "ms_per_64": ms, "rays": rays, "updates": upd,
            "kernel_ms": {"bucket": float(k[0]), "raymarch_total": float(k[1]), "commit": float(k[2]), "setup": float(k[3]),
                          "scan": float(k[4]), "fill": float(k[5]), "march": float(k[6])},
            "raymarch_alg_GBs": float(alg / (k[1] * 1e-3) / 1e9), "raymarch_frac": float(alg / (k[1] * 1e-3) / 1e9 / PEAK),

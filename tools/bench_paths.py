@@ -114,7 +114,7 @@ ms = timed(lambda: glo.fuse_from(sub), reps=3, warm=1)
 rows.append(("D1 submap -> global fusion (8 submaps)", f"{nsrc / ms * 1e3 / 1e6:,.0f} M source voxels/s", f"{ms:.2f} ms",
              f"{nsrc:,} observed source voxels x 7 corners; 90 B/voxel algorithmic -> {90.0 * nsrc / ms / 1e6:,.0f} GB/s"))
 
-# --- texture: coloured integrate (k_raymarch<true>: colour-word atomicMax next to every reduction) + coloured MC ---
+# --- texture: coloured integrate (k_raymarch: colour-word atomicMax next to every reduction) + coloured MC ---
 gt = TsdfHandle(512, 512, K=syn.K_DEPTH, is_global_map=True, texture_enabled=True)
 gt.set_color_intrinsics([1, 0, 0, 0, 1, 0, 0, 0, 1], True)
 d = syn.scene_sphere(4.0)

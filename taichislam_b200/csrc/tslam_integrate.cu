@@ -307,13 +307,15 @@ __global__ void __launch_bounds__(256, 6) k_bucket_points(const float* __restric
 //    serialise in L2 (a ray-like pattern reaches a fraction of the scattered update rate,
 //    tools/ubench/red_bench.cu).  Each CTA therefore keeps a 16^3-voxel WINDOW around
 //    the sensor origin in shared memory, accumulates samples that fall inside it with
-//    native 32-bit integer shared atomics (exact 2^-24 fixed point, lo/hi words), and
+//    native 32-bit integer shared atomics (exact fixed point, lo/hi words), and
 //    flushes one reduction per touched window voxel per round.
+// The fixed-point scale 2^k is chosen per round from the round's rays, as k_seg_scan chooses it per launch: the largest
+// k with max(w, w*dmax) * 2^k < 2^30 (one sample's integer fits 31 bits), so that long rays with small weights keep their
+// precision.  A ray with w * 2^k < MB_MIN_WQ (fewer than 14 significant bits) marches on the far path instead.
 // ---------------------------------------------------------------------------
 #define RM_THREADS 512
 #define RM_WIN 16
 #define RM_WIN3 4096
-#define RM_FIX 16777216.0f   // 2^24
 #define RM_WIN_STEPS 18      // a sample >= 18 voxels from the sensor origin lies outside the +-8 voxel window on some axis
 #define RM_SMEM (RM_WIN3 * 24 + RM_TAB * 8)  // A, B (lo/hi words) and the 64-bit colour word per window voxel, block table
 
@@ -336,6 +338,7 @@ __global__ void __launch_bounds__(RM_THREADS, 2) k_raymarch(const __grid_constan
   unsigned long long* const btab = (unsigned long long*)(win + 4 * RM_WIN3);
   unsigned long long* const w_cw = btab + RM_TAB;  // colour word of every window voxel
   __shared__ int s_org[4];   // window origin (voxels) and submap
+  __shared__ unsigned s_fmax;  // round's largest max(w, w*dmax), as bits (non-negative floats order like their bits)
   __shared__ int s_blk[8];   // the <= 8 blocks the window overlaps
 
   const uint32_t n_rays = min((uint32_t)*n_rays_p, ray_cap);
@@ -355,6 +358,7 @@ __global__ void __launch_bounds__(RM_THREADS, 2) k_raymarch(const __grid_constan
       s_org[1] = iroundf(f0.T[1] / vs) - RM_WIN / 2;
       s_org[2] = iroundf(f0.T[2] / vs) - RM_WIN / 2;
       s_org[3] = f0.submap;
+      s_fmax = 0u;
     }
     __syncthreads();
     const int wx = s_org[0], wy = s_org[1], wz = s_org[2], ws = s_org[3];
@@ -374,7 +378,7 @@ __global__ void __launch_bounds__(RM_THREADS, 2) k_raymarch(const __grid_constan
       live = cnt > 0;  // :240
     }
     float mx = 0.f, my = 0.f, mz = 0.f, ux = 0.f, uy = 0.f, uz = 0.f, Tx = 0.f, Ty = 0.f, Tz = 0.f, Px = 0.f, Py = 0.f, Pz = 0.f,
-          wgt = 0.f;
+          wgt = 0.f, Lr = 0.f;
     unsigned long long cur_key = TS_EMPTY;
     int cur_blk = -1;
     if (live) {
@@ -397,9 +401,26 @@ __global__ void __launch_bounds__(RM_THREADS, 2) k_raymarch(const __grid_constan
         }
         n = rg.n;
         wgt = rg.w;
+        Lr = rg.L;
       }
     }
-    const bool win_ok = (s == ws) && wgt < 120.0f;  // fixed-point range of the window words
+    {  // the round's fixed-point scale (tslam_march.cu ray_setup and k_seg_scan form the same bound per launch)
+      const float dmax = fmaxf(Lr, (float)n * vs - Lr) + vs;
+      unsigned fb = __float_as_uint(fminf(fmaxf(wgt, wgt * dmax), 3.0e38f));
+      fb = __reduce_max_sync(0xffffffffu, fb);
+      if (lane == 0 && fb) atomicMax(&s_fmax, fb);
+    }
+    __syncthreads();
+    int sk = 30;
+    if (s_fmax) {
+      int ex;
+      frexpf(__uint_as_float(s_fmax), &ex);  // fmax < 2^ex
+      sk = 30 - ex;
+    }
+    sk = max(0, min(48, sk));
+    const float fix = __uint_as_float((unsigned)(127 + sk) << 23);  // 2^k
+    const int wq = __float2int_rn(wgt * fix);
+    const bool win_ok = (s == ws) && wq >= MB_MIN_WQ;
     // every sample also raises the voxel's colour word [frame seq : 22][closeness : 12][rgb : 30] (atomicMax; decoded
     // by the commit) - in the window's shared-memory copy for near-field samples
     unsigned long long cw_hi = 0ull;
@@ -410,7 +431,6 @@ __global__ void __launch_bounds__(RM_THREADS, 2) k_raymarch(const __grid_constan
       const int qb = min(1023, (int)((((float)ccb / c) / 255.0f) * 1023.0f + 0.5f));
       cw_hi = ((unsigned long long)batch.f[f].seq << 42) | ((unsigned long long)qr << 20) | ((unsigned long long)qg << 10) | (unsigned long long)qb;
     }
-    const int wq = __float2int_rn(wgt * RM_FIX);
     const int nmax = __reduce_max_sync(0xffffffffu, n);
     // voxel of the previous far-field sample: a new block is looked up only when a coordinate leaves its 16-cell
     // (bits >= 4 differ).  Starts at the occupy voxel's block (cur_blk), or at a value no in-bounds voxel shares.
@@ -440,10 +460,10 @@ __global__ void __launch_bounds__(RM_THREADS, 2) k_raymarch(const __grid_constan
       bool far = inb;
       if (WIN) {
         const unsigned dx = (unsigned)(xi - wx), dy = (unsigned)(yi - wy), dz = (unsigned)(zi - wz);
-        const bool in_win = inb && win_ok && dx < RM_WIN && dy < RM_WIN && dz < RM_WIN && fabsf(a) < 120.0f;
+        const bool in_win = inb && win_ok && dx < RM_WIN && dy < RM_WIN && dz < RM_WIN;
         if (in_win) {  // near field: exact fixed-point sums in shared memory
           const int e = (int)((dx << 8) | (dy << 4) | dz);
-          win_add(&w_alo[e], &w_ahi[e], __float2int_rn(a * RM_FIX));
+          win_add(&w_alo[e], &w_ahi[e], __float2int_rn(a * fix));
           win_add(&w_blo[e], &w_bhi[e], wq);
           const int cl = min(4095, (int)(fabsf(ds) / vs * 16.0f));
           atomicMax(&w_cw[e], cw_hi | ((unsigned long long)(4095 - cl) << 30));
@@ -513,8 +533,9 @@ __global__ void __launch_bounds__(RM_THREADS, 2) k_raymarch(const __grid_constan
                        ((zi >> TS_BSHIFT) - (wz >> TS_BSHIFT));
       const int blk = s_blk[bsel];
       if (blk < 0) continue;  // pool exhausted (error flag raised)
-      const float A = (float)(((double)ahi * 4294967296.0 + (double)alo) * (1.0 / 16777216.0));
-      const float B = (float)(((double)bhi * 4294967296.0 + (double)blo) * (1.0 / 16777216.0));
+      const double rfix = __hiloint2double((1023 - sk) << 20, 0);  // 2^-k
+      const float A = (float)(((double)ahi * 4294967296.0 + (double)alo) * rfix);
+      const float B = (float)(((double)bhi * 4294967296.0 + (double)blo) * rfix);
       red_add_f32x2(&g.acc[(size_t)blk * TS_B3 + ts_voxel_off(xi, yi, zi)], A, B);
       ts_red_max_u64(&g.cword[(size_t)blk * TS_B3 + ts_voxel_off(xi, yi, zi)], w_cw[e]);
       w_cw[e] = 0ull;

@@ -281,6 +281,8 @@ __device__ __forceinline__ void red_add_u32(unsigned int* addr, unsigned int v) 
   asm volatile("red.relaxed.gpu.global.add.u32 [%0], %1;" ::"l"(addr), "r"(v) : "memory");
 }
 
+// both marches: a ray whose weight is < 2^14 fixed-point units (relative rounding error > 3e-5) takes f32 reductions
+#define MB_MIN_WQ 16384
 #define RM_TAB 4096          // shared block-lookup table: 16^3 entries indexed by the low 4 bits of the block coords
 // block lookup for the march loop: shared-memory table first (global loads queue behind the reduction traffic in
 // the in-order L1TEX pipe: measured as the top stall), hash grid on a miss.

@@ -45,7 +45,6 @@
 #define MB_SX 277
 #define MB_SY 17
 #define MB_WORDS (15 * MB_SX + 15 * MB_SY + 16)  // 4426
-#define MB_MIN_WQ 16384                          // a ray whose weight is < 2^14 fixed-point units (relative rounding error > 3e-5)
                                                 // is applied with f32 global reductions instead
 #define MB_SMEM (4 * MB_WORDS * 4)
 #define SEG_CLS 16                               // length classes per block: (count - 1) >> 1

@@ -240,6 +240,8 @@ extern "C" int tslam_tsdf_create(const tslam_tsdf_config_t* cfg, tslam_tsdf_t** 
   TS_CUDA(cudaMalloc(&m->colormap, cm.size() * 4));
   TS_CUDA(cudaMemcpy(m->colormap, cm.data(), cm.size() * 4, cudaMemcpyHostToDevice));
   m->march_verify = getenv("TSLAM_MARCH_VERIFY") != nullptr;
+  // tests: start the frame counter close to the 22-bit limit of the colour word, to run its renormalisation (ts_seq_renorm)
+  if (const char* fs = getenv("TSLAM_FRAME_SEQ0")) m->frame_seq = (unsigned)std::min(strtoul(fs, nullptr, 10), (1ul << 22) - 2ul);
   // (the workspace of the block-binned march - ~2 GB for 640x480 frames - is allocated by the first integrate launch:
   // global maps that are only ever fused into never pay for it)
   { int rci = ts_integrate_init(); if (rci) return rci; }

@@ -1,6 +1,7 @@
 """Seeded edge-case point clouds for the ray-march audit (tests/test_march_reference_cpu.py, tests/test_gpu_march_audit.py).
 
-Every cloud meets the input contract of march_reference: points on the 2^-20 m grid, one point per bucket, R = I."""
+Every cloud meets the input contract of march_reference: points on the 2^-20 m grid, one point per bucket, R = I.  Each
+point also has a colour (a seeded draw from a small palette of distinct colours), for the textured march."""
 import numpy as np
 
 from march_reference import round_half_away
@@ -111,17 +112,39 @@ def fine_long(rng):
     return dict(pts=p, T=np.float32([0.0013, -0.0021, 0.0004]), vs=vs, N=256, Nz=256, max_ray_length=12.5)
 
 
+def long_range(rng):
+    """20 000 rays in all directions at 55-60 m (vs 0.2, max_ray_length 64): w = 1/z^2 ~ 3e-4 for every ray, so the
+    window next to the sensor holds thousands of tiny weights, where a fixed point too coarse for them shows.  The sensor
+sits inside a block, away from its faces."""
+    vs = 0.2
+    d = rng.normal(size=(24000, 3))
+    p = one_per_bucket(snap(d / np.linalg.norm(d, axis=1, keepdims=True) * rng.uniform(55.0, 60.0, (d.shape[0], 1))), vs)
+    return dict(pts=p[:20000], T=np.float32([7.3, 7.6, 8.2]) * np.float32(vs), vs=vs, N=640, Nz=640, max_ray_length=64.0)
+
+
+def near_sensor(rng):
+    """Points 0.05-0.12 m from the sensor with internal_voxels 40 (vs 0.02): weights 70-400 (some rays w >= 120) and
+    rays 0.8 m past their point, so that some samples have |w*ds| >= 120."""
+    vs = 0.02
+    d = rng.normal(size=(4000, 3))
+    p = one_per_bucket(snap(d / np.linalg.norm(d, axis=1, keepdims=True) * rng.uniform(0.05, 0.12, (4000, 1))), vs)
+    return dict(pts=p, T=np.float32([0.0031, -0.0047, 0.0013]), vs=vs, N=256, Nz=256, internal_voxels=40)
+
+
 CASES = {"hot_bundle": hot_bundle, "ties_and_axes": ties_and_axes, "short_rays": short_rays, "anisotropic": anisotropic,
-         "tiny_weights": tiny_weights, "fine_long": fine_long}
+         "tiny_weights": tiny_weights, "fine_long": fine_long, "long_range": long_range, "near_sensor": near_sensor}
+PALETTE = np.array([[230, 25, 75], [60, 180, 75], [255, 225, 25], [0, 130, 200], [245, 130, 48], [145, 30, 180],
+                    [70, 240, 240], [240, 50, 230], [1, 1, 1], [255, 255, 255]], np.uint8)
 
 
 def make_case(name, seed=0):
     c = dict(internal_voxels=10, max_ray_length=10.0, pow2=False)
     c.update(CASES[name](np.random.default_rng(seed)))
+    c["rgb"] = PALETTE[np.random.default_rng([seed, 1]).integers(0, PALETTE.shape[0], c["pts"].shape[0])]
     return c
 
 
-def reference_of(case):
+def reference_of(case, path="binned", seq=1):
     from march_reference import reference_march
     return reference_march(case["pts"], case["T"], case["vs"], case["N"], case["Nz"], case["internal_voxels"],
-                           case["max_ray_length"])
+                           case["max_ray_length"], path=path, rgb=case["rgb"], seq=seq)

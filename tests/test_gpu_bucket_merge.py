@@ -70,10 +70,11 @@ def test_depth_division_all_uint16():
     assert_exact(np.arange(1 << 16, dtype=np.float32), 1000.0)
 
 
-@pytest.mark.parametrize("b", [syn.FX, K_OTHER[0], K_OTHER[4], 0.05])
+@pytest.mark.parametrize("b", [syn.FX, K_OTHER[0], K_OTHER[4], 0.05, 0.2, 0.02, 0.0002])
 def test_division_every_significand(b):
-    """The focal lengths of both test cameras and the 0.05 m voxel of the bucket key: every f32 significand, which by
-    scaling covers every dividend whose quotient stays normal (the check ts_fill_intrin makes when a handle is set up)."""
+    """The focal lengths of both test cameras, the 0.05 m voxel of the bucket key and the other voxel sizes of the
+    march audit (tests/march_cases.py; 1/16 is a power of two): every f32 significand, which by scaling covers every
+    dividend whose quotient stays normal (the check ts_fill_intrin makes when a handle is set up)."""
     for a in all_significands():
         assert_exact(a, np.float32(b))
         assert_exact(-a, np.float32(b))

@@ -21,7 +21,8 @@ def gpu_map(case, **kw):
                       internal_voxels=case["internal_voxels"], is_global_map=True, **kw)
 
 
-@pytest.mark.parametrize("name", ["hot_bundle", "ties_and_axes", "short_rays", "anisotropic", "tiny_weights", "fine_long"])
+@pytest.mark.parametrize("name", ["hot_bundle", "ties_and_axes", "short_rays", "anisotropic", "tiny_weights", "fine_long", "long_range",
+                                  "near_sensor"])
 def test_binned_march_matches_reference(name):
     c = make_case(name)
     ref = reference_of(c)

@@ -1,6 +1,7 @@
 """The f64 march reference (tests/march_reference.py) pinned to the CPU oracle on every edge-case cloud of the audit,
 before any GPU run trusts it: same voxel set, same per-voxel sample counts (recovered from W where every weight is a
-power of two), same in-bounds and out-of-bounds sample totals, TSDF and W within the bounds of util.march_bounds."""
+power of two), same in-bounds and out-of-bounds sample totals, TSDF and W within the bounds of util.march_bounds.  The
+textured path of the reference is pinned the same way, and its colour words to the oracle's colours exactly."""
 import numpy as np
 import pytest
 
@@ -23,6 +24,15 @@ def case_ref(request):
     return c, reference_of(c)
 
 
+def assert_pow2_counts(c, ref, oi, ot, ow):
+    w = np.unique(ref["w32"])
+    assert w.shape == (1,) and np.log2(w[0]) == np.round(np.log2(w[0]))
+    _, _, ws = as_dict_rows(oi, ot, ow)
+    free = ref["sw"] < 999.0
+    assert free.mean() > 0.99
+    assert np.array_equal(ws[free] / w[0], ref["count"][free]), "per-voxel sample counts differ"
+
+
 @pytest.mark.parametrize("mode", ["canonical", "f32_literal"])
 def test_reference_matches_oracle(case_ref, mode):
     from oracle.oracle import MODE_CANONICAL, MODE_F32_LITERAL
@@ -37,13 +47,32 @@ def test_reference_matches_oracle(case_ref, mode):
     oi, ot, ow, _ = o.gather()
     compare_to_reference((oi, ot, ow), ref, sequential=(mode == "f32_literal"), sharp=(mode == "canonical"))
     if c["pow2"]:
-        w = np.unique(ref["w32"])
-        assert w.shape == (1,) and np.log2(w[0]) == np.round(np.log2(w[0]))
-        _, _, ws = as_dict_rows(oi, ot, ow)
-        free = ref["sw"] < 999.0
-        assert free.mean() > 0.99
-        assert np.array_equal(ws[free] / w[0], ref["count"][free]), "per-voxel sample counts differ"
+        assert_pow2_counts(c, ref, oi, ot, ow)
 
+
+@pytest.mark.parametrize("name", sorted(CASES))
+def test_textured_reference_matches_oracle(name):
+    """The textured path of the reference against the canonical oracle with colours: same sample totals and voxel set,
+    values within the textured bounds (sharp at the hottest voxel), colours equal wherever the reference's f32 and
+    exact closeness bins agree on the winner - and they must agree almost everywhere."""
+    from oracle.oracle import MODE_CANONICAL
+    c = make_case(name)
+    ref = reference_of(c, "textured")
+    o = oracle_map(c, MODE_CANONICAL)
+    o.set_color(True, True)
+    o.integrate_points_rgb(np.eye(3), c["T"], c["pts"], c["rgb"])
+    o.commit()
+    st = o.stats()
+    assert st["n_rays"] == ref["n_rays"] and st["n_updates"] == ref["n_updates"] and st["n_oob"] == ref["n_oob"]
+    oi, ot, ow, _ = o.gather()
+    compare_to_reference((oi, ot, ow), ref, sharp=name != "hot_bundle")
+    if c["pow2"]:
+        assert_pow2_counts(c, ref, oi, ot, ow)
+    _, oc = as_dict_rows(oi, o.gather_color())
+    bad = (oc != ref["color"]).any(1)
+    assert not (bad & ~ref["color_amb"]).any(), f"{int(bad.sum())} colours differ from the reference's words"
+    assert ref["color_amb"].mean() < (0.5 if c["pow2"] else 0.01)  # pow2: |ds| sits on the bin edges by construction
+    assert len(np.unique(ref["color"], axis=0)) >= 5  # several colours compete: a wrong winner shows
 
 def test_cases_reach_their_edges():
     """Each cloud exercises what it is there for (numbers from the reference alone)."""
@@ -69,3 +98,14 @@ def test_cases_reach_their_edges():
     assert np.all(np.abs(np.round(c["pts"] / np.float32(c["vs"]))) <= 4095)  # inside the bucket key range
     ref = reference_of(c)
     assert ref["n_updates"] > 0 and ref["n_oob"] > ref["n_updates"]
+    c = make_case("long_range")
+    r = ray_setup(c["pts"], c["vs"], c["internal_voxels"], c["max_ray_length"])
+    assert c["pts"].shape[0] == 20000 and np.all((r["L"] >= 55.0) & (r["L"] <= 60.0)) and c["max_ray_length"] == 64.0
+    ref = reference_of(c, "textured")
+    assert ref["nwin"].max() >= 1000 and r["w32"].max() < 4e-4  # thousands of tiny weights in one window voxel
+    c = make_case("near_sensor")
+    r = ray_setup(c["pts"], c["vs"], c["internal_voxels"], c["max_ray_length"])
+    assert c["internal_voxels"] == 40 and np.all((r["L"] >= 0.05) & (r["L"] <= 0.12))
+    assert 0 < (r["w32"] >= 120.0).sum() < r["w32"].shape[0]
+    ref = reference_of(c, "textured")
+    assert np.any(r["w32"][:, None] * (r["L"][:, None] - np.arange(1, 19) * c["vs"]) <= -120.0)  # samples with |w*ds| >= 120

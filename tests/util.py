@@ -45,17 +45,24 @@ ref_wmax = 1000.0   # Wmax (dense_tsdf.py:8)
 def march_bounds(ref, sequential=False):
     """Per-voxel bounds (bW, bT) on |W - W_ref| and |TSDF - TSDF_ref| for one launch, ref = march_reference output.
 
-    S = sum w, A = sum w*ds, T = A/S, c = samples of the voxel; u = 2^-24.  The binned march adds, per sample, an
-    integer x = rint(v * 2^k) for v = w and v = w*ds (k: the launch's fixed-point scale, DESIGN §4 "Fixed point per
-    launch"); rays with w * 2^k < MB_MIN_WQ go through f32 reductions unquantised instead.  Error sources of W:
-      * fixed point: <= 2^-(k+1) per quantised sample                                   -> qcount * 2^-(k+1)
+    S = sum w, A = sum w*ds, T = A/S, c = samples of the voxel; u = 2^-24.  A march adds some samples as integers
+    x = rint(v * 2^k) for v = w and v = w*ds and the others through f32 reductions unquantised (DESIGN §4 "Fixed point
+    per launch"):
+      * binned march (tslam_march.cu): every sample is quantised at the launch's scale k, except rays with
+        w * 2^k < MB_MIN_WQ and samples on block faces, which may take the global f32 path;
+      * textured march (k_raymarch): samples in the 16^3 window around the sensor origin are quantised at the scale of
+        their round of 512 rays (>= the launch's k, and w * 2^k_r >= MB_MIN_WQ); all others are f32 reductions.
+    The reference reports per voxel the sum of the fixed-point bounds (q), the reductions that may reach it (n_red) and
+    the rounding of the kernels' sample values (eval).  Error sources of W:
+      * fixed point: <= 2^-(k_r+1) per quantised sample                                 -> q
       * the kernels' weight 1/(z*z) in f32 of the 2^-20-quantised z, not 1/|p|^2        -> sum |w32 - w|   (measured)
       * f32 rounding of each reduction that reaches the voxel (item flushes, global-path samples) and of the
         commit, each of a partial sum <= S                                              -> (n_red + 1) * u * S
     Error sources of A, besides the same fixed-point term:
-      * the sample value L - j*vs instead of the exact |P - x_| * sign                  -> sum w*|(L - j*vs) - ds| (measured)
-      * f32 rounding of the chain fma(-j0, vs, L), fma(-k, vs, L0), times w, and the global path's conversion:
-        four roundings of values <= L + j*vs (times w)                                   -> 4u * sum w*(L + j*vs)
+      * the sample value (binned: L - j*vs; textured: |P - x_| * sign in f32) instead of the exact |P - x_| * sign
+                                                                                        -> sum w*|ds_kernel - ds| (measured)
+      * f32 rounding in forming each summand (binned: fma(-j0, vs, L), fma(-k, vs, L0), times w, and the global path's
+        conversion, four roundings of values <= L + j*vs; textured: w * ds)            -> eval
       * w32 instead of w                                                                 -> sum |w32 - w| * |ds|
       * f32 reductions of partial sums <= sum w*|ds|                                     -> (n_red + 1) * u * sum w*|ds|
     TSDF = A'/S' with |A' - A| <= bA, |S' - S| <= bW: |T' - T| <= (bA + |T| bW) / S to first order, plus the commit
@@ -66,12 +73,12 @@ def march_bounds(ref, sequential=False):
     """
     c = ref["count"].astype(np.float64)
     n_red = c if sequential else ref["n_red"]
-    q = ref["qcount"] * 2.0 ** -(ref["k"] + 1)
+    q = ref["q"]
     S, T = ref["sw"], np.abs(ref["tsdf"])
     # (sequential: the weight is 1/(z*z) of the unquantised f32 z, within 3u of w)
     ew = (n_red + 1.0 + (3.0 if sequential else 0.0)) * F32_U
     bW = q + ref["dw"] + ew * S
-    bA = q + ref["dds"] + 4.0 * F32_U * ref["span"] + ref["dwd"] + ew * ref["swabsd"]
+    bA = q + ref["dds"] + ref["eval"] + ref["dwd"] + ew * ref["swabsd"]
     bT = (bA + T * bW) / S + 3.0 * F32_U * T
     if sequential:  # once the clamp binds mid-frame the running average is no longer the weighted mean: unbounded
         bT = np.where(S < ref_wmax, bT + c * 4.0 * F32_U * ref["max_absd"], np.inf)
@@ -105,7 +112,8 @@ def compare_to_reference(got, ref, sequential=False, sharp=True):
         assert bW[h] < 0.1 * eW[h], f"W bound {bW[h]:.3g} not well below one sample ({eW[h]:.3g}) at the hottest voxel"
         # (eT = 0: every sample of the voxel carries the same ds, and no sample count changes its TSDF)
         assert eT[h] == 0.0 or bT[h] < 0.5 * eT[h], f"TSDF bound {bT[h]:.3g} not well below one sample ({eT[h]:.3g}) at the hottest voxel"
-    return float(np.max(dW / bW)), float(np.max(dT / bT))
+    with np.errstate(invalid="ignore", divide="ignore"):  # (bound 0 where the sums are exact, and so is the result)
+        return float(np.max(np.where(bW > 0, dW / bW, 0.0))), float(np.max(np.where(bT > 0, dT / bT, 0.0)))
 
 
 def tri_multiset(verts, decimals=5):

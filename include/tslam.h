@@ -681,6 +681,49 @@ int tslam_tsdf_register(tslam_tsdf_t* A, tslam_tsdf_t* B, int32_t n_pairs, const
                         int32_t min_points, double* R_out, double* T_out, double* H_out, double* b_out, double* cost2,
                         int64_t* info5, void* stream);
 
+/* ----------------------------------------------------------------------------
+ * Frame tracking against the TSDF (DESIGN.md section 7, "Frame tracking"): the pose at which a depth frame's or a point
+ * cloud's points lie on the zero level of the map's committed TSDF, found before the frame is integrated (point-to-SDF
+ * alignment, Bylow et al. 2013).
+ *   pose       T_f = (R, t), f64 in and out, is the pose of frame f in the local frame of submap submaps[f] (a global map's
+ *              local frame is the world frame): the (R, T) tslam_tsdf_integrate_depth takes for that frame, so integrating
+ *              at the returned pose integrates at the tracked pose.
+ *   depth      n frames uint16 [n, height, width] mm in `mem`.  Frame f's candidates are the sampled pixels (i, j) =
+ *              (step ii, step jj), ii < width / step, jj < height / step (integer quotients: the pixels integrate samples
+ *              at recast_step = step).  A pixel of d mm is kept when d != 0 && !(f32(d) > dmax_mm || f32(d) < dmin_mm)
+ *              (dmin_mm, dmax_mm = f32(min_ray_length 1000), f32(max_ray_length 1000)); its point is (x, y, dep) with
+ *              the bucket kernel's f32 operations: dep = f32(d) / 1000, x = ((f32(i) - cx) dep) / fx, y = ((f32(j) - cy)
+ *              dep) / fy, each correctly rounded.  submaps: HOST int32 [n], or NULL for all zero.
+ *   points     one cloud f32 [n_points, 3] in the sensor frame, in `mem`, tracked against `submap`.  A point is kept when
+ *              x, y, z are finite and min_ray_length <= r < max_ray_length (f32 bounds) with r = sqrtf((x x + y y) + z z)
+ *              in f32: integrate's upper bound, applied before the rotation (the unknown), and a lower bound that drops
+ *              the (0, 0, 0) a LiDAR driver reports for a missing return.
+ *   records    (x, y, z, 0): a frame's records are contiguous, in row-major sampled-pixel order (depth) or input order
+ *              (points), whatever else the call holds.
+ *   residual, sums, solver   those of tslam_tsdf_register with d_v = 0 and the reading submap submaps[f] of this map: the
+ *              same corner validity, Huber weight, f64 sums, LM schedule, stopping rules and max_iters = 0 semantics.  H
+ *              and b are for the left perturbation T <- exp(xi) T in the submap's local frame.
+ * Inputs (HOST): R0 f64[n,9] row-major, T0 f64[n,3], finite.  Outputs (HOST), per frame, as tslam_tsdf_register's per
+ * pair: R_out f64[n,9], T_out f64[n,3], H_out f64[n,36], b_out f64[n,6], cost2 f64[n,2] (initial, final cost), info5
+ * int64[n,5] (points selected, valid at the final pose, evaluations after the first, converged, status: 0 ok, 1 fewer
+ * than min_points valid points at T0 - not a call error, the normal answer for the first frame of an empty submap).
+ * A frame's result does not depend on the other frames of the call; two identical calls give the same bits, and host and
+ * device input give the same bits.
+ * Refused (TSLAM_E_INVALID) before the handle is looked at: n outside [1, TSLAM_REG_MAX_PAIRS] (n_points < 0), step < 1,
+ * height or width not positive, huber not finite or not > 0, max_iters < 0 or min_points < 0, mem not a TSLAM_MEM_*;
+ * then a NULL handle or array, a submap out of range, a non-finite initial pose.
+ * Flushes the queued frames and pending commits first, synchronises once per iteration, and writes no map word, flag,
+ * ESDF, mesh state or statistic other than the kernel-launch counter.  Scratch in the handle (shared with
+ * tslam_tsdf_register, grown geometrically, freed by tslam_tsdf_destroy): 16 B per candidate chunk of 1024, the input
+ * when it is in host memory, 16 B per kept point, 232 B per 1024-point chunk of every frame, ~300 B per frame. */
+int tslam_tsdf_track_depth(tslam_tsdf_t* m, const uint16_t* depth, int mem, int32_t n, int32_t height, int32_t width,
+                           const int32_t* submaps, const double* R0, const double* T0, int32_t step, float huber, int32_t max_iters,
+                           int32_t min_points, double* R_out, double* T_out, double* H_out, double* b_out, double* cost2, int64_t* info5,
+                           void* stream);
+int tslam_tsdf_track_points(tslam_tsdf_t* m, const float* xyz, int mem, int32_t n_points, int32_t submap, const double* R0,
+                            const double* T0, float huber, int32_t max_iters, int32_t min_points, double* R_out, double* T_out,
+                            double* H_out, double* b_out, double* cost2, int64_t* info5, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -180,6 +180,10 @@ SIGNATURES = {
     "tslam_tour_open": (C.c_int, [_i32, _vp, _i32, C.c_uint64, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "tslam_tsdf_register": (C.c_int, [_vp, _vp, _i32, _vp, _vp, _vp, _vp, _f32, _f32, _f32, _i32, _i32, _vp, _vp, _vp, _vp, _vp,
                                       _vp, _vp]),
+    "tslam_tsdf_track_depth": (C.c_int, [_vp, _vp, C.c_int, _i32, _i32, _i32, _vp, _vp, _vp, _i32, _f32, _i32, _i32, _vp, _vp, _vp, _vp,
+                                         _vp, _vp, _vp]),
+    "tslam_tsdf_track_points": (C.c_int, [_vp, _vp, C.c_int, _i32, _i32, _vp, _vp, _f32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp,
+                                          _vp]),
 }
 
 _lib = None

@@ -235,15 +235,11 @@ __global__ void __launch_bounds__(256, 6) k_bucket_depth(const uint16_t* __restr
     const int j = jj * in.step, i = ii * in.step;
     // row_mul = recast_step for full frames, 1 when the staging copy already dropped the unsampled rows
     const uint16_t d = depth[(size_t)f * frame_stride + (size_t)(jj * row_mul) * w + i];
-    const float df = (float)d;
-    if (d != 0 && !(df > in.dmax_mm || df < in.dmin_mm)) {  // :196-199
+    if (ts_depth_kept(in, d)) {  // :196-199
       valid = true;
-      // the quotients of the reference, correctly rounded without IEEE division: df / 1000 for every uint16 df
-      // (tests/test_gpu_bucket_merge.py checks all of them), t / fx and t / fy where ts_fill_intrin proved the form
-      dep = div_vs(df, 1000.0f, 1.0f / 1000.0f);             // :201
-      const float tx = ((float)i - in.cx) * dep, ty = ((float)j - in.cy) * dep;  // mapping_common.py:37-40
-      const float x = in.fdiv ? div_vs(tx, in.fx, in.rfx) : tx / in.fx;
-      const float y = in.fdiv ? div_vs(ty, in.fy, in.rfy) : ty / in.fy;
+      const float3 c = ts_unproject(in, i, j, d);            // :201, mapping_common.py:37-40
+      const float x = c.x, y = c.y;
+      dep = c.z;
       const TsFrame& fr = batch.f[f];
       px = (fr.R[0] * x + fr.R[1] * y) + fr.R[2] * dep;     // :203 input_R @ pt (rotation only)
       py = (fr.R[3] * x + fr.R[4] * y) + fr.R[5] * dep;

@@ -350,6 +350,22 @@ struct TsIntrin {
   int same_proj;   // color_same_proj
 };
 
+// The depth rule of every reader of depth frames (k_bucket_depth, tslam_tsdf_track_depth): a pixel of d mm is kept when
+// d != 0 and min_ray <= d <= max_ray (dense_tsdf.py:196-199), and its camera-frame point (x, y, dep) is
+// unproject_point_dep (mapping_common.py:31-41, dense_tsdf.py:201): dep = df / 1000, x = ((i - cx) dep) / fx,
+// y = ((j - cy) dep) / fy, each quotient correctly rounded without IEEE division: div_vs gives df / 1000 for every
+// uint16 df (tests/test_gpu_bucket_merge.py checks all of them), and t / fx and t / fy where ts_fill_intrin proved the
+// form.
+__device__ __forceinline__ bool ts_depth_kept(const TsIntrin& in, uint16_t d) {
+  const float df = (float)d;
+  return d != 0 && !(df > in.dmax_mm || df < in.dmin_mm);
+}
+__device__ __forceinline__ float3 ts_unproject(const TsIntrin& in, int i, int j, uint16_t d) {
+  const float dep = div_vs((float)d, 1000.0f, 1.0f / 1000.0f);
+  const float tx = ((float)i - in.cx) * dep, ty = ((float)j - in.cy) * dep;
+  return make_float3(in.fdiv ? div_vs(tx, in.fx, in.rfx) : tx / in.fx, in.fdiv ? div_vs(ty, in.fy, in.rfy) : ty / in.fy, dep);
+}
+
 // per-frame bucket record (dense_tsdf.py:64-70 new_pcl_count / new_pcl_sum_pos / new_pcl_z), exact fixed-point sums
 // (2^-20 m) in one 32-byte sector.  cd = cnt << cnt_shift | sum(d): the depth sum is non-negative, and the launch picks
 // cnt_shift so that neither field can overflow into the other (ts_bucket_launch); a launch in which no shift can do that

@@ -14,6 +14,9 @@
 //               doubles, the iteration's one synchronisation.  Every sum is over a fixed order that depends on the pair
 //               alone, so a pair's result is the same bits alone or in a batch, and two identical calls agree bit for bit.
 // The call reads the committed tw / obs planes and writes nothing to either map.
+// Frame tracking (tslam_tsdf_track_depth / _points, DESIGN.md section 7, "Frame tracking") is the same solver (rg_lm)
+// over other records: the kept points of depth frames or a point cloud in the sensor frame, with d = 0, selected by
+// k_tr_select (count, scan, fill).
 #include <cub/cub.cuh>
 #include <cmath>
 #include <cstring>
@@ -279,6 +282,127 @@ static bool rg_solve(const double* S, double lam, double xi[6]) {
 
 static double rg_mean_cost(const double* S) { return S[28] > 0.0 ? S[27] / S[28] : INFINITY; }
 
+// Chunks (CTAs of one evaluation) of P problems of n[p] points
+static long long rg_lm_ctas(int P, const int* n) {
+  long long c = 0;
+  for (int p = 0; p < P; p++) c += (n[p] + RG_CHUNK - 1) / RG_CHUNK;
+  return c;
+}
+// Device scratch of rg_lm: chunk partials, jobs, sums
+static size_t rg_lm_bytes(int P, long long ctas) {
+  return rg_align((size_t)(ctas + 1) * RG_NS * 8) + rg_align((size_t)P * sizeof(RgJob)) + rg_align((size_t)P * RG_NS * 8);
+}
+
+// Levenberg-Marquardt of P problems, all active problems evaluated by one launch per iteration: problem p solves for the
+// pose of the records pts[p0[p] .. p0[p] + n[p]) against submap sub[p] of the grid g, from (R0, T0) row p.  The launches
+// count on A.  scratch: rg_lm_bytes(P, rg_lm_ctas(P, n)) bytes of device memory.  Writes the outputs of
+// tslam_tsdf_register (include/tslam.h), info5[5p] = n[p].
+static int rg_lm(tslam_tsdf_t* A, const TsGrid& g, const float4* pts, void* scratch, int P, const long long* p0, const int* n,
+                 const int* sub, const double* R0, const double* T0, float vs, float huber, int max_iters, int min_points,
+                 double* R_out, double* T_out, double* H_out, double* b_out, double* cost2, int64_t* info5, cudaStream_t st) {
+  char* w = (char*)scratch;
+  double* part = (double*)w; w += rg_align((size_t)(rg_lm_ctas(P, n) + 1) * RG_NS * 8);
+  RgJob* d_jobs = (RgJob*)w; w += rg_align((size_t)P * sizeof(RgJob));
+  double* d_sums = (double*)w;
+  std::vector<RgPose> T(P), trial(P);
+  std::vector<double> S((size_t)P * RG_NS), Sn((size_t)P * RG_NS), lam(P, 1e-4);
+  std::vector<int> iters(P, 0), conv(P, 0), status(P, 0);
+  std::vector<char> active(P, 0);
+  std::vector<RgJob> jobs;
+  jobs.reserve(P);
+  const double delta = (double)huber;
+  // evaluate the poses Q[p] of the listed problems into out
+  auto evaluate = [&](const std::vector<int>& list, const std::vector<RgPose>& Q, std::vector<double>& out) -> int {
+    jobs.clear();
+    int ctas = 0;
+    for (int p : list) {
+      RgJob j;
+      for (int i = 0; i < 9; i++) j.R[i] = (float)Q[p].R[i];
+      for (int i = 0; i < 3; i++) j.t[i] = (float)Q[p].t[i];
+      j.p0 = p0[p];
+      j.n = n[p];
+      j.submap = sub[p];
+      j.pair = p;
+      j.cta0 = ctas;
+      ctas += (j.n + RG_CHUNK - 1) / RG_CHUNK;
+      jobs.push_back(j);
+    }
+    TS_CUDA(cudaMemsetAsync(d_sums, 0, (size_t)P * RG_NS * 8, st));
+    TS_CUDA(cudaMemcpyAsync(d_jobs, jobs.data(), jobs.size() * sizeof(RgJob), cudaMemcpyHostToDevice, st));
+    if (ctas > 0) {
+      k_rg_eval<<<ctas, RG_THREADS, 0, st>>>(g, pts, d_jobs, (int)jobs.size(), vs, delta, part);
+      TS_LAUNCH_CHECK(A);
+      k_rg_final<<<((int)jobs.size() * 32 + 255) / 256, 256, 0, st>>>(d_jobs, (int)jobs.size(), ctas, part, d_sums);
+      TS_LAUNCH_CHECK(A);
+    }
+    TS_CUDA(cudaMemcpyAsync(out.data(), d_sums, (size_t)P * RG_NS * 8, cudaMemcpyDeviceToHost, st));
+    TS_CUDA(cudaStreamSynchronize(st));
+    return TSLAM_OK;
+  };
+  std::vector<int> list;
+  for (int p = 0; p < P; p++) {
+    for (int i = 0; i < 9; i++) T[p].R[i] = R0[9 * p + i];
+    for (int i = 0; i < 3; i++) T[p].t[i] = T0[3 * p + i];
+    list.push_back(p);
+  }
+  int rc = evaluate(list, T, S);
+  if (rc) return rc;
+  std::vector<double> cost0(P);
+  for (int p = 0; p < P; p++) {
+    const double* s = &S[(size_t)p * RG_NS];
+    cost0[p] = s[27];
+    if (s[28] < (double)min_points) status[p] = 1;
+    active[p] = status[p] == 0 && max_iters > 0;
+  }
+  const double rho_tol = 1e-4 * (double)vs, phi_tol = 1e-6;
+  for (;;) {
+    list.clear();
+    for (int p = 0; p < P; p++) {
+      if (!active[p]) continue;
+      double xi[6];
+      if (!rg_solve(&S[(size_t)p * RG_NS], lam[p], xi)) { active[p] = 0; continue; }  // H + lam D singular: stop here
+      const double nr = std::sqrt(xi[0] * xi[0] + xi[1] * xi[1] + xi[2] * xi[2]);
+      const double nf = std::sqrt(xi[3] * xi[3] + xi[4] * xi[4] + xi[5] * xi[5]);
+      if (nr < rho_tol && nf < phi_tol) { conv[p] = 1; active[p] = 0; continue; }
+      trial[p] = rg_update(T[p], xi);
+      list.push_back(p);
+    }
+    if (list.empty()) break;
+    rc = evaluate(list, trial, Sn);
+    if (rc) return rc;
+    for (int p : list) {
+      const double* sn = &Sn[(size_t)p * RG_NS];
+      double* s = &S[(size_t)p * RG_NS];
+      iters[p]++;
+      if (sn[28] >= (double)min_points && rg_mean_cost(sn) < rg_mean_cost(s)) {
+        T[p] = trial[p];
+        std::memcpy(s, sn, RG_NS * 8);
+        lam[p] /= 10.0;
+      } else {
+        lam[p] *= 10.0;
+      }
+      if (iters[p] >= max_iters) active[p] = 0;
+    }
+  }
+  for (int p = 0; p < P; p++) {
+    const double* s = &S[(size_t)p * RG_NS];
+    std::memcpy(R_out + 9 * p, T[p].R, 9 * 8);
+    std::memcpy(T_out + 3 * p, T[p].t, 3 * 8);
+    int q = 0;
+    for (int i = 0; i < 6; i++)
+      for (int j = i; j < 6; j++) H_out[36 * p + 6 * i + j] = H_out[36 * p + 6 * j + i] = s[q++];
+    for (int i = 0; i < 6; i++) b_out[6 * p + i] = s[21 + i];
+    cost2[2 * p] = cost0[p];
+    cost2[2 * p + 1] = s[27];
+    info5[5 * p] = n[p];
+    info5[5 * p + 1] = (int64_t)s[28];
+    info5[5 * p + 2] = iters[p];
+    info5[5 * p + 3] = conv[p];
+    info5[5 * p + 4] = status[p];
+  }
+  return TSLAM_OK;
+}
+
 extern "C" int tslam_tsdf_register(tslam_tsdf_t* A, tslam_tsdf_t* B, int32_t n_pairs, const int32_t* ref_submaps,
                                    const int32_t* read_submaps, const double* R0, const double* T0, float band, float min_weight,
                                    float huber, int32_t max_iters, int32_t min_points, double* R_out, double* T_out, double* H_out,
@@ -370,119 +494,213 @@ extern "C" int tslam_tsdf_register(tslam_tsdf_t* A, tslam_tsdf_t* B, int32_t n_p
   std::vector<long long> slot_p0(U + 1, 0);
   for (int u = 0; u < U; u++) slot_p0[u + 1] = slot_p0[u] + slot_cnt[u];
   const long long n_pts = slot_p0[U];
-  long long max_ctas = 0;  // a launch covers at most every pair
-  for (int p = 0; p < n_pairs; p++) max_ctas += (slot_cnt[pair_slot[p]] + RG_CHUNK - 1) / RG_CHUNK;
+  std::vector<long long> p0(n_pairs);
+  std::vector<int> np(n_pairs);
+  for (int p = 0; p < n_pairs; p++) { p0[p] = slot_p0[pair_slot[p]]; np[p] = slot_cnt[pair_slot[p]]; }
+  const long long max_ctas = rg_lm_ctas(n_pairs, np.data());  // a launch covers at most every pair
   if (max_ctas > INT32_MAX / 2) { ts_set_error("tslam_tsdf_register: too many points (%lld)", n_pts); return TSLAM_E_CAPACITY; }
-  const size_t pts_b = rg_align((size_t)n_pts * 16), part_b = rg_align((size_t)(max_ctas + 1) * RG_NS * 8);
-  const size_t job_b = rg_align((size_t)n_pairs * sizeof(RgJob)), sum_b = rg_align((size_t)n_pairs * RG_NS * 8);
-  rc = rg_reserve(&A->reg_pts, &A->reg_pts_bytes, pts_b + part_b + job_b + sum_b);
+  const size_t pts_b = rg_align((size_t)n_pts * 16);
+  rc = rg_reserve(&A->reg_pts, &A->reg_pts_bytes, pts_b + rg_lm_bytes(n_pairs, max_ctas));
   if (rc) return rc;
-  w = (char*)A->reg_pts;
-  float4* pts = (float4*)w; w += pts_b;
-  double* part = (double*)w; w += part_b;
-  RgJob* d_jobs = (RgJob*)w; w += job_b;
-  double* d_sums = (double*)w;
+  float4* pts = (float4*)A->reg_pts;
   if (n_pts > 0) {
     k_rg_fill<<<A->sm_count * 4, 256, 0, st>>>(A->g, nb, val_s, cs, off, band, min_weight, vs, pts);
     TS_LAUNCH_CHECK(A);
   }
+  return rg_lm(A, B->g, pts, (char*)A->reg_pts + pts_b, n_pairs, p0.data(), np.data(), read_submaps, R0, T0, vs, huber, max_iters,
+               min_points, R_out, T_out, H_out, b_out, cost2, info5, st);
+}
 
-  // ---- Levenberg-Marquardt, all active pairs evaluated by one launch per iteration
-  std::vector<RgPose> T(n_pairs), trial(n_pairs);
-  std::vector<double> S((size_t)n_pairs * RG_NS), Sn((size_t)n_pairs * RG_NS), lam(n_pairs, 1e-4);
-  std::vector<int> iters(n_pairs, 0), conv(n_pairs, 0), status(n_pairs, 0);
-  std::vector<char> active(n_pairs, 0);
-  std::vector<RgJob> jobs;
-  jobs.reserve(n_pairs);
-  const double delta = (double)huber;
-  // evaluate the poses P[p] of the listed pairs into out
-  auto evaluate = [&](const std::vector<int>& list, const std::vector<RgPose>& P, std::vector<double>& out) -> int {
-    jobs.clear();
-    int ctas = 0;
-    for (int p : list) {
-      RgJob j;
-      for (int i = 0; i < 9; i++) j.R[i] = (float)P[p].R[i];
-      for (int i = 0; i < 3; i++) j.t[i] = (float)P[p].t[i];
-      j.p0 = slot_p0[pair_slot[p]];
-      j.n = slot_cnt[pair_slot[p]];
-      j.submap = read_submaps[p];
-      j.pair = p;
-      j.cta0 = ctas;
-      ctas += (j.n + RG_CHUNK - 1) / RG_CHUNK;
-      jobs.push_back(j);
-    }
-    TS_CUDA(cudaMemsetAsync(d_sums, 0, (size_t)n_pairs * RG_NS * 8, st));
-    TS_CUDA(cudaMemcpyAsync(d_jobs, jobs.data(), jobs.size() * sizeof(RgJob), cudaMemcpyHostToDevice, st));
-    if (ctas > 0) {
-      k_rg_eval<<<ctas, RG_THREADS, 0, st>>>(B->g, pts, d_jobs, (int)jobs.size(), vs, delta, part);
-      TS_LAUNCH_CHECK(A);
-      k_rg_final<<<((int)jobs.size() * 32 + 255) / 256, 256, 0, st>>>(d_jobs, (int)jobs.size(), ctas, part, d_sums);
-      TS_LAUNCH_CHECK(A);
-    }
-    TS_CUDA(cudaMemcpyAsync(out.data(), d_sums, (size_t)n_pairs * RG_NS * 8, cudaMemcpyDeviceToHost, st));
-    TS_CUDA(cudaStreamSynchronize(st));
-    return TSLAM_OK;
-  };
-  std::vector<int> list;
-  for (int p = 0; p < n_pairs; p++) {
-    for (int i = 0; i < 9; i++) T[p].R[i] = R0[9 * p + i];
-    for (int i = 0; i < 3; i++) T[p].t[i] = T0[3 * p + i];
-    list.push_back(p);
+// ---- frame tracking (tslam_tsdf_track_depth / tslam_tsdf_track_points, DESIGN.md section 7, "Frame tracking") --------
+// The records of a frame are its kept points (x, y, z, 0) in the sensor frame, aligned with rg_lm against d = 0: the
+// pose that puts them on the zero level of the map's TSDF.  Selection is a count, a scan and a fill over chunks of
+// TR_CHUNK consecutive candidates of one frame (CTA (chunk, frame)), so that a frame's records are contiguous and in
+// candidate order whatever else the call holds.
+#define TR_PPT 4                           // candidates per thread and chunk
+#define TR_CHUNK (256 * TR_PPT)            // candidates per CTA
+
+// candidates of a depth call: the sampled pixels (step ii, step jj), ii < ww, jj < hh, of n frames of h x w, row-major
+struct TrDepth {
+  const uint16_t* data;
+  int w, step, ww;
+  long long frame_px, n;  // h w, hh ww
+  TsIntrin in;
+  __device__ __forceinline__ bool point(int f, long long q, float4& r) const {
+    const int qi = (int)q, jj = qi / ww, ii = qi - jj * ww, i = ii * step, j = jj * step;  // q < INT32_MAX
+    const uint16_t d = data[(size_t)f * frame_px + (size_t)j * w + i];
+    if (!ts_depth_kept(in, d)) return false;
+    const float3 c = ts_unproject(in, i, j, d);
+    r = make_float4(c.x, c.y, c.z, 0.0f);
+    return true;
   }
-  rc = evaluate(list, T, S);
+};
+// candidates of a point-cloud call: the n points of one cloud f32[n, 3]
+struct TrCloud {
+  const float* data;
+  float rmin, rmax;       // f32(min_ray_length), f32(max_ray_length)
+  long long n;
+  __device__ __forceinline__ bool point(int, long long q, float4& r) const {
+    const float x = data[3 * q], y = data[3 * q + 1], z = data[3 * q + 2];
+    if (!(isfinite(x) && isfinite(y) && isfinite(z))) return false;
+    const float len = sqrtf((x * x + y * y) + z * z);
+    if (!(len >= rmin && len < rmax)) return false;
+    r = make_float4(x, y, z, 0.0f);
+    return true;
+  }
+};
+
+// CTA (c, f): candidates c TR_CHUNK .. of frame f, TR_PPT consecutive ones per thread.  COUNT: cnt[f C + c] = kept;
+// else the kept records go to pts[off[f C + c] ..] in candidate order (a block scan places each thread's run).
+template <class Src, bool COUNT>
+__global__ void __launch_bounds__(256) k_tr_select(Src src, int C, long long* __restrict__ cnt, const long long* __restrict__ off,
+                                                   float4* __restrict__ pts) {
+  typedef cub::BlockScan<int, 256> Scan;
+  __shared__ typename Scan::TempStorage tmp;
+  const int f = blockIdx.y;
+  const long long q0 = (long long)blockIdx.x * TR_CHUNK + threadIdx.x * TR_PPT;
+  float4 r[TR_PPT];
+  unsigned keep = 0;
+#pragma unroll
+  for (int k = 0; k < TR_PPT; k++) keep |= (q0 + k < src.n && src.point(f, q0 + k, r[k])) ? 1u << k : 0u;
+  int pos, total;
+  Scan(tmp).ExclusiveSum(__popc(keep), pos, total);
+  const size_t chunk = (size_t)f * C + blockIdx.x;
+  if (COUNT) {
+    if (threadIdx.x == 0) cnt[chunk] = total;
+    return;
+  }
+  long long row = off[chunk] + pos;
+#pragma unroll
+  for (int k = 0; k < TR_PPT; k++)
+    if (keep >> k & 1u) pts[row++] = r[k];
+}
+
+// Tracking of n frames against submaps sub of m: selection of src (whose data is `input`, in `mem`, in_bytes long), then
+// rg_lm.  The arguments have been checked.
+template <class Src>
+static int tr_track(tslam_tsdf_t* m, Src src, const void* input, int mem, size_t in_bytes, int n, const int* sub, const double* R0,
+                    const double* T0, float huber, int max_iters, int min_points, double* R_out, double* T_out, double* H_out,
+                    double* b_out, double* cost2, int64_t* info5, cudaStream_t st) {
+  int rc = ts_flush_pending(m, st);
+  if (!rc) rc = ts_check_deferred_async(m, st);
   if (rc) return rc;
-  std::vector<double> cost0(n_pairs);
-  for (int p = 0; p < n_pairs; p++) {
-    const double* s = &S[(size_t)p * RG_NS];
-    cost0[p] = s[27];
-    if (s[28] < (double)min_points) status[p] = 1;
-    active[p] = status[p] == 0 && max_iters > 0;
+  const long long C = src.n > 0 ? (src.n + TR_CHUNK - 1) / TR_CHUNK : 1;  // chunks per frame
+  const long long nc = (long long)n * C;
+  if (C > INT32_MAX) { ts_set_error("tslam_tsdf_track: %lld candidates per frame", src.n); return TSLAM_E_INVALID; }
+  size_t scan_tmp = 0;
+  TS_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, scan_tmp, (long long*)nullptr, (long long*)nullptr, nc + 1, st));
+  const size_t cb = rg_align((size_t)(nc + 1) * 8), stage_b = mem == TSLAM_MEM_HOST ? rg_align(in_bytes) : 0;
+  rc = rg_reserve(&m->reg_blk, &m->reg_blk_bytes, 2 * cb + rg_align(scan_tmp) + stage_b);
+  if (rc) return rc;
+  char* w = (char*)m->reg_blk;
+  long long* cnt = (long long*)w; w += cb;
+  long long* off = (long long*)w; w += cb;
+  void* tmp = w; w += rg_align(scan_tmp);
+  src.data = (decltype(src.data))input;
+  if (mem == TSLAM_MEM_HOST) {
+    TS_CUDA(cudaMemcpyAsync(w, input, in_bytes, cudaMemcpyHostToDevice, st));
+    src.data = (decltype(src.data))w;
   }
-  const double rho_tol = 1e-4 * (double)vs, phi_tol = 1e-6;
-  for (;;) {
-    list.clear();
-    for (int p = 0; p < n_pairs; p++) {
-      if (!active[p]) continue;
-      double xi[6];
-      if (!rg_solve(&S[(size_t)p * RG_NS], lam[p], xi)) { active[p] = 0; continue; }  // H + lam D singular: stop here
-      const double nr = std::sqrt(xi[0] * xi[0] + xi[1] * xi[1] + xi[2] * xi[2]);
-      const double nf = std::sqrt(xi[3] * xi[3] + xi[4] * xi[4] + xi[5] * xi[5]);
-      if (nr < rho_tol && nf < phi_tol) { conv[p] = 1; active[p] = 0; continue; }
-      trial[p] = rg_update(T[p], xi);
-      list.push_back(p);
+  const dim3 grid((unsigned)C, (unsigned)n);
+  TS_CUDA(cudaMemsetAsync(cnt + nc, 0, 8, st));
+  k_tr_select<Src, true><<<grid, 256, 0, st>>>(src, (int)C, cnt, nullptr, nullptr);
+  TS_LAUNCH_CHECK(m);
+  TS_CUDA(cub::DeviceScan::ExclusiveSum(tmp, scan_tmp, cnt, off, nc + 1, st));
+  std::vector<long long> p0(n + 1);  // off[f C]: the first record of frame f, p0[n] = every record
+  TS_CUDA(cudaMemcpy2DAsync(p0.data(), 8, off, (size_t)C * 8, 8, (size_t)n + 1, cudaMemcpyDeviceToHost, st));
+  TS_CUDA(cudaStreamSynchronize(st));
+  std::vector<int> np(n);
+  for (int f = 0; f < n; f++) np[f] = (int)(p0[f + 1] - p0[f]);  // at most src.n <= INT32_MAX
+  const long long ctas = rg_lm_ctas(n, np.data());
+  if (ctas > INT32_MAX / 2) { ts_set_error("tslam_tsdf_track: too many points (%lld)", p0[n]); return TSLAM_E_CAPACITY; }
+  const size_t pts_b = rg_align((size_t)p0[n] * 16);
+  rc = rg_reserve(&m->reg_pts, &m->reg_pts_bytes, pts_b + rg_lm_bytes(n, ctas));
+  if (rc) return rc;
+  float4* pts = (float4*)m->reg_pts;
+  if (p0[n] > 0) {
+    k_tr_select<Src, false><<<grid, 256, 0, st>>>(src, (int)C, nullptr, off, pts);
+    TS_LAUNCH_CHECK(m);
+  }
+  return rg_lm(m, m->g, pts, (char*)m->reg_pts + pts_b, n, p0.data(), np.data(), sub, R0, T0, m->in.vs, huber, max_iters, min_points,
+               R_out, T_out, H_out, b_out, cost2, info5, st);
+}
+
+// Argument checks shared by both entries: the submaps and the initial poses of n frames
+static int tr_check_frames(const tslam_tsdf_t* m, const char* fn, int n, const int32_t* submaps, const double* R0, const double* T0) {
+  for (int f = 0; f < n; f++) {
+    const int s = submaps ? submaps[f] : 0;
+    if (s < 0 || s >= m->cfg.max_submaps) {
+      ts_set_error("%s: frame %d: submap %d out of range", fn, f, s);
+      return TSLAM_E_INVALID;
     }
-    if (list.empty()) break;
-    rc = evaluate(list, trial, Sn);
-    if (rc) return rc;
-    for (int p : list) {
-      const double* sn = &Sn[(size_t)p * RG_NS];
-      double* s = &S[(size_t)p * RG_NS];
-      iters[p]++;
-      if (sn[28] >= (double)min_points && rg_mean_cost(sn) < rg_mean_cost(s)) {
-        T[p] = trial[p];
-        std::memcpy(s, sn, RG_NS * 8);
-        lam[p] /= 10.0;
-      } else {
-        lam[p] *= 10.0;
+    for (int i = 0; i < 12; i++) {
+      if (!std::isfinite(i < 9 ? R0[9 * f + i] : T0[3 * f + i - 9])) {
+        ts_set_error("%s: frame %d: initial pose not finite", fn, f);
+        return TSLAM_E_INVALID;
       }
-      if (iters[p] >= max_iters) active[p] = 0;
     }
-  }
-  for (int p = 0; p < n_pairs; p++) {
-    const double* s = &S[(size_t)p * RG_NS];
-    std::memcpy(R_out + 9 * p, T[p].R, 9 * 8);
-    std::memcpy(T_out + 3 * p, T[p].t, 3 * 8);
-    int q = 0;
-    for (int i = 0; i < 6; i++)
-      for (int j = i; j < 6; j++) H_out[36 * p + 6 * i + j] = H_out[36 * p + 6 * j + i] = s[q++];
-    for (int i = 0; i < 6; i++) b_out[6 * p + i] = s[21 + i];
-    cost2[2 * p] = cost0[p];
-    cost2[2 * p + 1] = s[27];
-    info5[5 * p] = slot_cnt[pair_slot[p]];
-    info5[5 * p + 1] = (int64_t)s[28];
-    info5[5 * p + 2] = iters[p];
-    info5[5 * p + 3] = conv[p];
-    info5[5 * p + 4] = status[p];
   }
   return TSLAM_OK;
+}
+
+static bool tr_bad_params(float huber, int32_t max_iters, int32_t min_points) {
+  return !std::isfinite(huber) || !(huber > 0.0f) || max_iters < 0 || min_points < 0;
+}
+
+extern "C" int tslam_tsdf_track_depth(tslam_tsdf_t* m, const uint16_t* depth, int mem, int32_t n, int32_t height, int32_t width,
+                                      const int32_t* submaps, const double* R0, const double* T0, int32_t step, float huber,
+                                      int32_t max_iters, int32_t min_points, double* R_out, double* T_out, double* H_out, double* b_out,
+                                      double* cost2, int64_t* info5, void* stream) {
+  static const char* fn = "tslam_tsdf_track_depth";
+  if (n < 1 || n > TSLAM_REG_MAX_PAIRS) {
+    ts_set_error("%s: n %d outside [1, %d]", fn, n, TSLAM_REG_MAX_PAIRS);
+    return TSLAM_E_INVALID;
+  }
+  if (step < 1 || height <= 0 || width <= 0 || tr_bad_params(huber, max_iters, min_points) ||
+      (mem != TSLAM_MEM_DEVICE && mem != TSLAM_MEM_HOST)) {
+    ts_set_error("%s: step >= 1, height and width > 0, huber finite and > 0, max_iters and min_points >= 0, mem a TSLAM_MEM_*", fn);
+    return TSLAM_E_INVALID;
+  }
+  if (!m || !depth || !R0 || !T0 || !R_out || !T_out || !H_out || !b_out || !cost2 || !info5) {
+    ts_set_error("%s: NULL handle or array", fn);
+    return TSLAM_E_INVALID;
+  }
+  int rc = tr_check_frames(m, fn, n, submaps, R0, T0);
+  if (rc) return rc;
+  TrDepth src;
+  src.data = nullptr;
+  src.w = width;
+  src.step = step;
+  src.ww = width / step;
+  src.frame_px = (long long)height * width;
+  src.n = (long long)(height / step) * src.ww;  // range(0, h / step) x range(0, w / step), as integrate samples
+  src.in = m->in;
+  if (src.n > INT32_MAX) { ts_set_error("%s: %lld sampled pixels per frame", fn, src.n); return TSLAM_E_INVALID; }
+  std::vector<int> sub(n);
+  for (int f = 0; f < n; f++) sub[f] = submaps ? submaps[f] : 0;
+  return tr_track(m, src, depth, mem, (size_t)n * src.frame_px * 2, n, sub.data(), R0, T0, huber, max_iters, min_points, R_out, T_out,
+                  H_out, b_out, cost2, info5, (cudaStream_t)stream);
+}
+
+extern "C" int tslam_tsdf_track_points(tslam_tsdf_t* m, const float* xyz, int mem, int32_t n_points, int32_t submap, const double* R0,
+                                       const double* T0, float huber, int32_t max_iters, int32_t min_points, double* R_out, double* T_out,
+                                       double* H_out, double* b_out, double* cost2, int64_t* info5, void* stream) {
+  static const char* fn = "tslam_tsdf_track_points";
+  if (n_points < 0 || tr_bad_params(huber, max_iters, min_points) || (mem != TSLAM_MEM_DEVICE && mem != TSLAM_MEM_HOST)) {
+    ts_set_error("%s: n_points >= 0, huber finite and > 0, max_iters and min_points >= 0, mem a TSLAM_MEM_*", fn);
+    return TSLAM_E_INVALID;
+  }
+  if (!m || (!xyz && n_points > 0) || !R0 || !T0 || !R_out || !T_out || !H_out || !b_out || !cost2 || !info5) {
+    ts_set_error("%s: NULL handle or array", fn);
+    return TSLAM_E_INVALID;
+  }
+  int rc = tr_check_frames(m, fn, 1, &submap, R0, T0);
+  if (rc) return rc;
+  TrCloud src;
+  src.data = nullptr;
+  src.rmin = (float)m->cfg.min_ray_length;
+  src.rmax = m->in.max_ray;
+  src.n = n_points;
+  return tr_track(m, src, xyz, mem, (size_t)n_points * 12, 1, &submap, R0, T0, huber, max_iters, min_points, R_out, T_out, H_out, b_out,
+                  cost2, info5, (cudaStream_t)stream);
 }

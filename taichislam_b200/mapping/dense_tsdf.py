@@ -402,3 +402,43 @@ class DenseTSDF(BaseMap):
         out = self._h.register(reading._h, a, r, R0, T0, band, min_weight, huber, max_iters, min_points)
         keys = ("R", "T", "H", "b", "cost_init", "cost", "n_points", "n_valid", "iterations", "converged", "status")
         return [{k: (out[k][p].copy() if out[k].ndim > 1 else out[k][p].item()) for k in keys} for p in range(len(a))]
+
+    def track_depth(self, R, T, depthmap, step=None, huber=None, max_iters=20, min_points=100):
+        """Track one depth frame (uint16 mm [h,w]) against the TSDF of the active submap (submap 0 of a global map) on the
+        GPU (tslam_tsdf_track_depth, DESIGN.md section 7, "Frame tracking"), before it is integrated: the pose at which
+        the frame's points lie on the map's zero level.  R, T: the initial pose in the frame recast_depth_to_map takes.
+        step defaults to recast_step, huber to one voxel.  Flushes the queued frames first.  -> dict: R, T (the tracked
+        pose in the caller's frame, to hand to recast_depth_to_map; the input R, T unchanged, bit for bit, when status
+        is 1 or no step was accepted), R_local, T_local (in the submap's local frame), H, b (information at the tracked
+        pose, xi = (rho, phi) of the left perturbation in the local frame), cost_init, cost, n_points, n_valid,
+        iterations, converged, status (1: fewer than min_points valid points at the initial pose)."""
+        if self.K_cam_dep is None:
+            raise RuntimeError("set_dep_camera_intrinsic() must be called before track_depth")
+        depth = np.ascontiguousarray(depthmap, dtype=np.uint16)
+        return self._track(R, T, lambda R0, T0, s: self._h.track_depth(depth, R0[None], T0[None], submaps=[s], step=step, huber=huber,
+                                                                      max_iters=max_iters, min_points=min_points))
+
+    def track_pcl(self, R, T, xyz_array, huber=None, max_iters=20, min_points=100):
+        """track_depth for a point cloud xyz_array [n,3] in the sensor frame (recast_pcl_to_map's input): points that are
+        not finite or whose range lies outside [min_ray_length, max_ray_length) are dropped.  -> the same dict."""
+        xyz = np.ascontiguousarray(np.asarray(xyz_array, dtype=np.float32).reshape(-1, 3))
+        return self._track(R, T, lambda R0, T0, s: self._h.track_points(xyz, R0, T0, submap=s, huber=huber, max_iters=max_iters,
+                                                                       min_points=min_points))
+
+    def _track(self, R, T, call):
+        R_in, T_in = np.array(R, dtype=np.float64), np.array(T, dtype=np.float64).reshape(3)
+        R0, T0 = self.convert_by_base(R_in, T_in)
+        if self.submap_enabled:  # the base pose convert_by_base used
+            b = self.active_submap_id[None]
+            Rb, Tb = self.submaps_base_R_np[b], self.submaps_base_T_np[b]
+        else:
+            Rb, Tb = self.base_R_np, self.base_T_np
+        out = call(R0, T0, self._active())
+        res = {k: (v[0].copy() if v.ndim > 1 else v[0].item()) for k, v in out.items()}
+        res["R_local"], res["T_local"] = res.pop("R"), res.pop("T")
+        moved = not (np.array_equal(res["R_local"], R0) and np.array_equal(res["T_local"], T0))
+        if res["status"] == 0 and moved:
+            res["R"], res["T"] = Rb @ res["R_local"], Rb @ res["T_local"] + Tb
+        else:
+            res["R"], res["T"] = R_in, T_in
+        return res

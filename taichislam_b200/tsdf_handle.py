@@ -369,8 +369,59 @@ class TsdfHandle:
                                               float(band), float(min_weight), huber, int(max_iters), int(min_points), capi.np_ptr(R),
                                               capi.np_ptr(T), capi.np_ptr(H), capi.np_ptr(b), capi.np_ptr(cost2), capi.np_ptr(info),
                                               capi.stream_ptr()))
+        return self._solver_out(P, R, T, H, b, cost2, info)
+
+    @staticmethod
+    def _solver_out(P, R, T, H, b, cost2, info):
         return dict(R=R.reshape(P, 3, 3), T=T, H=H.reshape(P, 6, 6), b=b, cost_init=cost2[:, 0], cost=cost2[:, 1],
                     n_points=info[:, 0], n_valid=info[:, 1], iterations=info[:, 2], converged=info[:, 3], status=info[:, 4])
+
+    # -- frame tracking against the TSDF (tslam_tsdf_track_depth / _points) ----------------------------------------
+    def _track(self, name, n, args, R0, T0, huber, max_iters, min_points):
+        R0 = np.ascontiguousarray(np.asarray(R0, dtype=np.float64).reshape(n, 9))
+        T0 = np.ascontiguousarray(np.asarray(T0, dtype=np.float64).reshape(n, 3))
+        huber = float(self.cfg.voxel_scale) if huber is None else float(huber)
+        R, T = np.zeros((n, 9)), np.zeros((n, 3))
+        H, b, cost2 = np.zeros((n, 36)), np.zeros((n, 6)), np.zeros((n, 2))
+        info = np.zeros((n, 5), np.int64)
+        head, tail = args
+        capi.check(getattr(self.L, name)(self.h, *head, capi.np_ptr(R0), capi.np_ptr(T0), *tail, huber, int(max_iters), int(min_points),
+                                         capi.np_ptr(R), capi.np_ptr(T), capi.np_ptr(H), capi.np_ptr(b), capi.np_ptr(cost2),
+                                         capi.np_ptr(info), capi.stream_ptr()))
+        return self._solver_out(n, R, T, H, b, cost2, info)
+
+    def track_depth(self, depth, Rs, Ts, submaps=None, step=None, huber=None, max_iters=20, min_points=100):
+        """Track depth frames against the map's TSDF: the pose of each frame in its submap's local frame at which the
+        frame's points lie on the zero level.  depth: uint16 [n,h,w] (or [h,w]) numpy (host) or torch CUDA tensor; Rs
+        [n,3,3], Ts [n,3]: initial poses (f64, the frame of integrate_depth's Rs, Ts); submaps: per frame (default 0);
+        step defaults to recast_step, huber to the voxel scale.  -> dict of numpy arrays keyed like register()."""
+        torch = self.torch
+        if isinstance(depth, torch.Tensor):
+            assert depth.is_cuda and depth.dtype in (torch.uint16, torch.int16) and depth.is_contiguous()
+            mem, ptr, shape = capi.MEM_DEVICE, capi.tptr(depth), tuple(depth.shape)
+        else:
+            depth = np.ascontiguousarray(depth, dtype=np.uint16)
+            mem, ptr, shape = capi.MEM_HOST, capi.np_ptr(depth), depth.shape
+        if len(shape) == 2:
+            shape = (1,) + tuple(shape)
+        n, h, w = shape
+        sm = np.ascontiguousarray(np.broadcast_to(np.asarray(0 if submaps is None else submaps, dtype=np.int32), (n,)))
+        step = int(self.cfg.recast_step) if step is None else int(step)
+        return self._track("tslam_tsdf_track_depth", n, ((ptr, mem, n, h, w, capi.np_ptr(sm)), (step,)), Rs, Ts, huber, max_iters,
+                           min_points)
+
+    def track_points(self, xyz, R, T, submap=0, huber=None, max_iters=20, min_points=100):
+        """Track one point cloud xyz [n,3] (sensor frame; numpy or torch CUDA f32) against submap `submap`: points that are
+        not finite or whose range lies outside [min_ray_length, max_ray_length) are dropped.  R [3,3], T [3]: initial pose
+        (f64).  -> dict of numpy arrays keyed like register(), one row."""
+        torch = self.torch
+        if isinstance(xyz, torch.Tensor):
+            assert xyz.is_cuda and xyz.dtype == torch.float32 and xyz.is_contiguous()
+            mem, ptr, n = capi.MEM_DEVICE, capi.tptr(xyz), xyz.shape[0]
+        else:
+            xyz = np.ascontiguousarray(np.asarray(xyz, dtype=np.float32).reshape(-1, 3))
+            mem, ptr, n = capi.MEM_HOST, capi.np_ptr(xyz), xyz.shape[0]
+        return self._track("tslam_tsdf_track_points", 1, ((ptr, mem, n, int(submap)), ()), R, T, huber, max_iters, min_points)
 
     # -- introspection --------------------------------------------------------------------
     def stats(self, clear=False):

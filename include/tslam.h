@@ -724,6 +724,48 @@ int tslam_tsdf_track_points(tslam_tsdf_t* m, const float* xyz, int mem, int32_t 
                             const double* T0, float huber, int32_t max_iters, int32_t min_points, double* R_out, double* T_out,
                             double* H_out, double* b_out, double* cost2, int64_t* info5, void* stream);
 
+/* ----------------------------------------------------------------------------
+ * Rendering of the TSDF's zero level (DESIGN.md section 7, "Rendering"): depth, normal and colour images of n pinhole
+ * cameras, ray-cast to the surface that registration and frame tracking align to (KinectFusion's model image).
+ *   cameras    1 <= n <= TSLAM_RENDER_MAX_CAMERAS, one pinhole K4 = (fx, fy, cx, cy) (HOST f64, rounded to f32 once) and
+ *              one image size height x width for all.  Camera c has pose (R_c, T_c) (HOST f64 [n,9] row-major and [n,3],
+ *              rounded to f32 once), which maps camera points into the local frame of submap submaps[c] (HOST int32 [n],
+ *              or NULL for all zero): the (R, T) tslam_tsdf_integrate_depth and tslam_tsdf_track_depth take.
+ *   ray        pixel (i, j) (column i, row j, no half-pixel offset): camera-frame direction r = ((f32(i) - cx) / fx,
+ *              (f32(j) - cy) / fy, 1), each operation correctly rounded, turned into the local frame in pose_apply's
+ *              order ((R0 rx + R1 ry) + R2 1) + 0 per row, giving dir.  The ray parameter is the camera-frame depth z.
+ *   samples    K = floor((z_max - z_min) / step) + 1 (host, f64 of the f32 parameters); for k = 0 .. K-1:
+ *              z_k = z_min + f32(k) step, x_k = T + z_k dir per axis, each operation one correctly rounded f32 operation.
+ *   value      D_k = the trilinear interpolant of the committed TSDF of the camera's submap at x_k (u = x / vs,
+ *              c0 = floor(u), fractions u - c0, lerp along x, then y, then z: the ESDF query's arithmetic).  Valid iff all
+ *              8 corners lie in the volume, in present non-ghost blocks, and each has obs != 0 and W > 0: the corner rule
+ *              of tslam_tsdf_register, with no other threshold.
+ *   hit        the first k with samples k and k+1 both valid, D_k > 0 and D_{k+1} <= 0 (free space into the surface;
+ *              back faces and crossings across an invalid sample are not hits).  a = D_k - D_{k+1}, f = D_k / a,
+ *              z* = z_k + step f, x* = T + z* dir, each f32 in that order.
+ * Outputs (DEVICE, row-major):
+ *   depth      f32 [n,h,w]: z*, or 0 where there is no hit (the depth-image convention, which integrate drops).
+ *   status     u8 [n,h,w]: 0 no hit; 1 hit with normal (and colour); 2 hit, but a corner of x*'s cell is not valid or
+ *              |g| = 0.
+ *   normal     f32 [n,h,w,3] (may be NULL): g / |g| in the submap's local frame, g the interpolant's gradient at x*
+ *              (the ESDF query's), |g| = sqrtf((gx gx + gy gy) + gz gz).  NaN unless status is 1.
+ *   color      f32 [n,h,w,3] (may be NULL; textured maps only): each channel of the committed colour interpolated at x*
+ *              over the same 8 corners in the same lerp order.  NaN unless status is 1.
+ * Every pixel is independent: batches, repeated calls and single-camera calls give the same bits.
+ * Refused (TSLAM_E_INVALID) before the handle is looked at: n outside [1, TSLAM_RENDER_MAX_CAMERAS]; height or width < 1
+ * or n h w >= 2^31; f32(fx), f32(fy) not finite or not > 0, f32(cx), f32(cy) not finite; z_min not finite or not > 0;
+ * z_max not finite or not > z_min; step not finite or not > 0; K > TSLAM_RENDER_MAX_SAMPLES; K4, depth or status NULL.
+ * Then: a NULL handle or pose array, a submap out of range, a pose not finite (in f64 or after rounding to f32), color
+ * requested on a map without texture.
+ * Flushes the queued frames and pending commits first; writes no map word, flag, ESDF, mesh state or statistic other
+ * than the kernel-launch counter.  Asynchronous on `stream` apart from the upload of the per-camera jobs (52 B per
+ * camera, in a scratch buffer of the handle grown geometrically and freed by tslam_tsdf_destroy). */
+#define TSLAM_RENDER_MAX_CAMERAS 1024
+#define TSLAM_RENDER_MAX_SAMPLES 65536
+int tslam_tsdf_render(tslam_tsdf_t* m, int32_t n, int32_t height, int32_t width, const double* K4, const int32_t* submaps,
+                      const double* R, const double* T, float z_min, float z_max, float step, float* depth, float* normal,
+                      float* color, uint8_t* status, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

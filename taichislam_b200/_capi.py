@@ -17,6 +17,8 @@ MEM_DEVICE, MEM_HOST = 0, 1
 F_COMMIT = 1
 MAX_BATCH = 64
 REG_MAX_PAIRS = 1024
+RENDER_MAX_CAMERAS = 1024
+RENDER_MAX_SAMPLES = 65536
 ABI_VERSION = 6
 
 
@@ -184,6 +186,7 @@ SIGNATURES = {
                                          _vp, _vp, _vp]),
     "tslam_tsdf_track_points": (C.c_int, [_vp, _vp, C.c_int, _i32, _i32, _vp, _vp, _f32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp,
                                           _vp]),
+    "tslam_tsdf_render": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _f32, _f32, _f32, _vp, _vp, _vp, _vp, _vp]),
 }
 
 _lib = None

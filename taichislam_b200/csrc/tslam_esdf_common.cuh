@@ -62,14 +62,19 @@ static int es_wave(M* m, cudaStream_t st, int* flags, int group, Launch launch, 
 // lerp(a, b, t) = a + t*(b - a), rounded step by step (never contracted to an FMA): tests/esdf_query_reference.py
 __device__ __forceinline__ float esq_lerp(float a, float b, float t) { return __fadd_rn(a, __fmul_rn(t, __fsub_rn(b, a))); }
 
-// Trilinear interpolant of the 8 corner values e[dx*4 + dy*2 + dz] at fractions (fx, fy, fz) of the cell, and its
-// exact partial derivatives (tests/esdf_query_reference.py states the same arithmetic operation by operation).
-__device__ __forceinline__ void esq_interp(const float e[8], float fx, float fy, float fz, float vs, float& d, float& gx, float& gy,
-                                           float& gz) {
-  // dist: along x, then y, then z
+// Trilinear interpolant of the 8 corner values e[dx*4 + dy*2 + dz] at fractions (fx, fy, fz) of the cell: along x, then
+// y, then z
+__device__ __forceinline__ float esq_value(const float e[8], float fx, float fy, float fz) {
   const float c00 = esq_lerp(e[0], e[4], fx), c01 = esq_lerp(e[1], e[5], fx);
   const float c10 = esq_lerp(e[2], e[6], fx), c11 = esq_lerp(e[3], e[7], fx);
-  d = esq_lerp(esq_lerp(c00, c10, fy), esq_lerp(c01, c11, fy), fz);
+  return esq_lerp(esq_lerp(c00, c10, fy), esq_lerp(c01, c11, fy), fz);
+}
+
+// esq_value and the interpolant's exact partial derivatives (tests/esdf_query_reference.py states the same arithmetic
+// operation by operation).
+__device__ __forceinline__ void esq_interp(const float e[8], float fx, float fy, float fz, float vs, float& d, float& gx, float& gy,
+                                           float& gz) {
+  d = esq_value(e, fx, fy, fz);
   // d/dx: the four x-differences along y, then z
   const float ax00 = __fsub_rn(e[4], e[0]), ax01 = __fsub_rn(e[5], e[1]), ax10 = __fsub_rn(e[6], e[2]), ax11 = __fsub_rn(e[7], e[3]);
   gx = __fdiv_rn(esq_lerp(esq_lerp(ax00, ax10, fy), esq_lerp(ax01, ax11, fy), fz), vs);
@@ -346,7 +351,7 @@ __device__ __forceinline__ int es_qblock(const P& p, int nb_seen, int bx, int by
 // each distinct corner block is looked up once (the corner cube spans 2, 4 or 8 blocks only where i0 is the last voxel
 // of its block on some axis).  read(off, e) -> whether the corner at pool offset off has a value, stored in e.  False
 // (e unspecified) when a block is refused or a corner has no value.  The ESDF queries and the SDF-to-SDF registration
-// (tslam_register.cu) read their corners through this one function.
+// (tslam_register.cu) and rendering (tslam_render.cu) read their corners through this one function.
 template <int S, class Find, class Read>
 __device__ __forceinline__ bool es_corners(int i0, int j0, int k0, Find find, Read read, float e[8]) {
   constexpr int M = (1 << S) - 1, B3 = 1 << 3 * S;
@@ -376,6 +381,32 @@ __device__ __forceinline__ bool es_corners(int i0, int j0, int k0, Find find, Re
     }
   }
   return ok;
+}
+
+// The zero level that registration, frame tracking and rendering share: the committed TSDF of one submap, interpolated
+// over the 8 corners of a cell.  A block counts when it is present and not a ghost (ts_sdf_block); a corner has a value
+// when it is observed and its weight is > 0 (ts_sdf_corners); no other threshold.
+__device__ __forceinline__ int ts_sdf_block(const TsGrid& g, int sb, int bx, int by, int bz) {
+  const int b = ts_find(g, ts_pack_key(sb, bx, by, bz));
+  return (b >= 0 && !g.ghost[b]) ? b : -1;
+}
+// find(bx, by, bz) -> ts_sdf_block's answer (a caller may memoise it); seen(c, off) gets the pool offset of corner c
+// (e[c]) for each corner read (all 8 whenever every corner block counts)
+template <class Find, class Seen>
+__device__ __forceinline__ bool ts_sdf_corners(const TsGrid& g, const int c0[3], Find find, float e[8], Seen seen) {
+  return es_corners<TS_BSHIFT>(
+      c0[0], c0[1], c0[2], find,
+      [&](size_t off, float& ev) {
+        const float2 tw = g.tw[off];
+        ev = tw.x;
+        seen((int)(&ev - e), off);
+        return g.obs[off] != 0 && tw.y > 0.0f;
+      },
+      e);
+}
+template <class Find>
+__device__ __forceinline__ bool ts_sdf_corners(const TsGrid& g, const int c0[3], Find find, float e[8]) {
+  return ts_sdf_corners(g, c0, find, e, [](int, size_t) {});
 }
 
 // Trilinear interpolation of the field over the 8 voxels around each point (voxel i centred at i*vs, submap-local frame)

@@ -579,6 +579,8 @@ struct tslam_tsdf {
   size_t reg_blk_bytes;
   void* reg_pts;
   size_t reg_pts_bytes;
+  void* render_jobs;   // per-camera jobs of tslam_tsdf_render (tslam_render.cu), grown geometrically
+  size_t render_jobs_bytes;
   int march_verify;    // TSLAM_MARCH_VERIFY=1: every fast-path index is re-computed exactly, mismatches counted
   bool clamp_on_commit;
   // frame queue of the per-frame API (tslam_tsdf_queue_depth): double-buffered device staging fed by a copy stream
@@ -867,6 +869,8 @@ int ts_check_tex(tslam_tsdf* m, const uint8_t* tex, int th, int tw);  // a colou
 int ts_integrate_depth_impl(tslam_tsdf_t* m, const uint16_t* depth, int mem, int32_t n_frames, int32_t h, int32_t w, const float* R9s,
                             const float* T3s, const int32_t* submap_ids, int flags, void* stream, const uint8_t* tex = nullptr, int th = 0,
                             int tw = 0);
+// tslam_register.cu: *p holds at least `need` bytes: reallocated (contents dropped) to max(need, 2 x the old size) when smaller
+int rg_reserve(void** p, size_t* bytes, size_t need);
 // tslam_queue.cu: the per-frame queue's switches, copy stream and events of a new handle / their release
 int ts_queue_init(tslam_tsdf* m);
 void ts_queue_free(tslam_tsdf* m);

@@ -114,19 +114,7 @@ __device__ __forceinline__ void rg_term(const TsGrid& g, int sb, float4 p, const
   int c0[3];
   if (!(esq_low_corner(g, vs, x, u, c0) && c0[0] < g.N - g.hN - 1 && c0[1] < g.N - g.hN - 1 && c0[2] < g.Nz - g.hNz - 1)) return;
   float e[8];
-  const bool ok = es_corners<TS_BSHIFT>(
-      c0[0], c0[1], c0[2],
-      [&](int bx, int by, int bz) {
-        const int b = ts_find(g, ts_pack_key(sb, bx, by, bz));
-        return (b >= 0 && !g.ghost[b]) ? b : -1;
-      },
-      [&](size_t off, float& ev) {
-        const float2 tw = g.tw[off];
-        ev = tw.x;
-        return g.obs[off] != 0 && tw.y > 0.0f;
-      },
-      e);
-  if (!ok) return;
+  if (!ts_sdf_corners(g, c0, [&](int bx, int by, int bz) { return ts_sdf_block(g, sb, bx, by, bz); }, e)) return;
   const float fx = __fsub_rn(u[0], (float)c0[0]), fy = __fsub_rn(u[1], (float)c0[1]), fz = __fsub_rn(u[2], (float)c0[2]);
   float d, gx, gy, gz;
   esq_interp(e, fx, fy, fz, vs, d, gx, gy, gz);
@@ -203,7 +191,7 @@ __global__ void __launch_bounds__(256) k_rg_final(const RgJob* __restrict__ jobs
 
 // ---- host --------------------------------------------------------------------------------------------------------
 // *p holds at least `need` bytes: reallocated (contents dropped) to max(need, 2 x the old size) when smaller
-static int rg_reserve(void** p, size_t* bytes, size_t need) {
+int rg_reserve(void** p, size_t* bytes, size_t need) {
   if (need <= *bytes) return TSLAM_OK;
   const size_t nb = need > 2 * *bytes ? need : 2 * *bytes;
   if (*p) cudaFree(*p);

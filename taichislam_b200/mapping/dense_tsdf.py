@@ -442,3 +442,29 @@ class DenseTSDF(BaseMap):
         else:
             res["R"], res["T"] = R_in, T_in
         return res
+
+    def render(self, R, T, height, width, K=None, submap=None, z_min=None, z_max=None, step=None, color=False):
+        """Depth, normal (and colour) images of the TSDF's zero level seen from a pinhole camera at pose R, T, in the frame
+        recast_depth_to_map takes (tslam_tsdf_render, DESIGN.md section 7, "Rendering").  The pose is carried into the
+        local frame of `submap` (default: the active submap, submap 0 of a global map) through that submap's base pose
+        in f64.  K defaults to the depth intrinsics; z_min, z_max, step to min_ray_length, max_ray_length and the voxel
+        scale.  Flushes the queued frames first.  -> dict of numpy arrays: depth f32 [h,w] (0: no hit), status u8 [h,w]
+        (0 no hit, 1 hit, 2 hit without normal), normal f32 [h,w,3] in the caller's frame (NaN unless status is 1), and
+        color f32 [h,w,3] when asked (textured maps)."""
+        K = self.K_cam_dep if K is None else [float(k) for k in np.asarray(K).reshape(-1)]
+        if K is None:
+            raise RuntimeError("set_dep_camera_intrinsic() must be called before render, or K given")
+        s = self._active() if submap is None else int(submap)
+        if self.submap_enabled:
+            Rb, Tb = self.submaps_base_R_np[s], self.submaps_base_T_np[s]
+        else:
+            Rb, Tb = self.base_R_np, self.base_T_np
+        R, T = np.asarray(R, dtype=np.float64), np.asarray(T, dtype=np.float64).reshape(3)
+        Rl, Tl = Rb.T @ R, Rb.T @ (T - Tb)  # convert_by_base, for submap s
+        depth, status, nrm, col = self._h.render(Rl[None], Tl[None], height, width, K, submaps=[s], z_min=z_min, z_max=z_max,
+                                                 step=step, color=color)
+        out = dict(depth=depth[0].cpu().numpy(), status=status[0].cpu().numpy())
+        out["normal"] = (nrm[0].cpu().numpy().astype(np.float64) @ np.asarray(Rb, np.float64).T).astype(np.float32)
+        if color:
+            out["color"] = col[0].cpu().numpy()
+        return out

@@ -423,6 +423,33 @@ class TsdfHandle:
             mem, ptr, n = capi.MEM_HOST, capi.np_ptr(xyz), xyz.shape[0]
         return self._track("tslam_tsdf_track_points", 1, ((ptr, mem, n, int(submap)), ()), R, T, huber, max_iters, min_points)
 
+    # -- rendering (tslam_tsdf_render) -----------------------------------------------------
+    def render(self, Rs, Ts, height, width, K9, submaps=None, z_min=None, z_max=None, step=None, normals=True, color=False):
+        """Ray-cast n cameras to the zero level of the committed TSDF: Rs [n,3,3], Ts [n,3] (f64) map camera points into
+        the local frame of each camera's submap (the frame of integrate_depth's Rs, Ts); K9 the pinhole (fx, fy, cx, cy
+        at 0, 4, 2, 5); submaps per camera (default 0); z_min, z_max, step default to min_ray_length, max_ray_length
+        and the voxel scale.  -> torch CUDA tensors (depth f32 [n,h,w] (0: no hit), status u8 [n,h,w] (0 no hit, 1 hit,
+        2 hit without normal), normal f32 [n,h,w,3] or None, colour f32 [n,h,w,3] or None), NaN where status is not 1."""
+        torch = self.torch
+        R = np.ascontiguousarray(np.asarray(Rs, dtype=np.float64).reshape(-1, 9))
+        n = R.shape[0]
+        T = np.ascontiguousarray(np.asarray(Ts, dtype=np.float64).reshape(n, 3))
+        K4 = np.ascontiguousarray([K9[0], K9[4], K9[2], K9[5]], dtype=np.float64)
+        sm = np.ascontiguousarray(np.broadcast_to(np.asarray(0 if submaps is None else submaps, dtype=np.int32), (n,)))
+        z_min = float(self.cfg.min_ray_length) if z_min is None else float(z_min)
+        z_max = float(self.cfg.max_ray_length) if z_max is None else float(z_max)
+        step = float(self.cfg.voxel_scale) if step is None else float(step)
+        dev = torch.device("cuda", torch.cuda.current_device())
+        h, w = int(height), int(width)
+        depth = torch.empty((n, h, w), dtype=torch.float32, device=dev)
+        status = torch.empty((n, h, w), dtype=torch.uint8, device=dev)
+        nrm = torch.empty((n, h, w, 3), dtype=torch.float32, device=dev) if normals else None
+        col = torch.empty((n, h, w, 3), dtype=torch.float32, device=dev) if color else None
+        capi.check(self.L.tslam_tsdf_render(self.h, n, h, w, capi.np_ptr(K4), capi.np_ptr(sm), capi.np_ptr(R), capi.np_ptr(T), z_min,
+                                            z_max, step, capi.tptr(depth), capi.tptr(nrm) if normals else None,
+                                            capi.tptr(col) if color else None, capi.tptr(status), capi.stream_ptr()))
+        return depth, status, nrm, col
+
     # -- introspection --------------------------------------------------------------------
     def stats(self, clear=False):
         o = np.zeros(8, np.int64)

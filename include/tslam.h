@@ -163,6 +163,27 @@ int tslam_tsdf_scatter(tslam_tsdf_t* m, int32_t submap, int64_t n, const int32_t
  * trilinear splat (7 corners, :300) of every observed voxel of every submap of `src`
  * into submap 0 of `dst`, using dst's pose table.  No Wmax clamp (:274-278). */
 int tslam_tsdf_fuse(tslam_tsdf_t* dst, tslam_tsdf_t* src, void* stream);
+/* Incremental fusion of the submaps of `src` into the global map `dst` (DESIGN.md section 7, "Incremental global
+ * fusion"): an opt-in alternative to tslam_tsdf_fuse that keeps exact int64 sums (24 B per voxel, 48 B textured, grown
+ * with the pool blocks in use) of the terms k_fuse splats, each quantised to llrint(f * 2^24), and re-reads only the
+ * blocks a call changed.  After the call dst equals the fusion of every submap s with include[s] != 0 (include: host,
+ * max_submaps bytes; NULL = all) at its fused pose: dst's base pose of s, unless s was fused before with the same
+ * content and |T - T0| + angle(R0^T R) * r_s <= tolerance (r_s: farthest allocated block corner of s from its origin;
+ * tolerance 0: iff the pose bits are unchanged).  The result does not depend on the history of calls.  A full update
+ * (reset, then add every included submap) runs on the first call, when full != 0, for another src, after any other
+ * write of dst, when a fused submap's content changed, and when subtracting and re-adding would splat more source
+ * blocks than a rebuild; both paths give the same bits.  Differences from tslam_tsdf_fuse: the quantisation, occ
+ * saturates once on the total, and blocks left empty by removals stay allocated (a full update compacts them).
+ * stats8 (may be NULL): full-update reason (0 incremental, 1 first call, 2 full requested, 3 other src, 4 dst written,
+ * 5 content changed, 6 cheaper than subtract and re-add), submaps added, moved, removed, left within tolerance, source
+ * voxels splatted (adds + subtracts), source voxels skipped (a term not finite or >= 2^23), blocks committed.
+ * Refused (TSLAM_E_INVALID, nothing written), before the handles are looked at: tolerance not finite or < 0, a NULL
+ * handle, dst == src; then a dst that is not a global map, different max_submaps, voxel size or texture setting,
+ * and a tiled dst (tile cuts set or ghost blocks).  TSLAM_E_CUDA (byte count in tslam_last_error) when the sum planes
+ * cannot grow; TSLAM_E_POOL_FULL when dst's pool runs out (nothing added; the next call is a full update).
+ * Synchronises with `stream`. */
+int tslam_tsdf_fuse_update(tslam_tsdf_t* dst, tslam_tsdf_t* src, const uint8_t* include, float tolerance, int32_t full,
+                           int64_t* stats8, void* stream);
 /* cvt_TSDF_surface_to_voxels_kernel (dense_tsdf.py:339-365): append |TSDF|<1.8*vs
  * voxels of `submap` to xyz/rgb f32[cap,3] (DEVICE) starting at *count_dev (DEVICE
  * int32 counter, incremented; entries beyond cap are counted but not written). */

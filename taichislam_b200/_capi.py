@@ -20,6 +20,8 @@ REG_MAX_PAIRS = 1024
 RENDER_MAX_CAMERAS = 1024
 RENDER_MAX_SAMPLES = 65536
 ABI_VERSION = 6
+FUSE_REASONS = ("incremental", "first call", "full requested", "other source", "destination written", "content changed",
+                "cheaper than subtract and re-add")
 
 
 class TslamError(RuntimeError):
@@ -186,6 +188,7 @@ SIGNATURES = {
                                          _vp, _vp, _vp]),
     "tslam_tsdf_track_points": (C.c_int, [_vp, _vp, C.c_int, _i32, _i32, _vp, _vp, _f32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp,
                                           _vp]),
+    "tslam_tsdf_fuse_update": (C.c_int, [_vp, _vp, _vp, _f32, _i32, _vp, _vp]),
     "tslam_tsdf_render": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _f32, _f32, _f32, _vp, _vp, _vp, _vp, _vp]),
 }
 

@@ -699,10 +699,14 @@ int ts_integrate_init() {
 // ---------------------------------------------------------------------------
 // k_collect_dirty, then the commit, whose last CTA sets the dirty-list count back to zero (ticket: scratch_i[4]).  Both
 // are launched with programmatic dependent launch (ts_launch_pdl).
-int ts_launch_commit(tslam_tsdf* m, cudaStream_t st, int clamp, int fused) {
+int ts_collect_dirty(tslam_tsdf* m, cudaStream_t st) {
   const int gc = (m->g.max_blocks + 255) / 256 < m->sm_count * 4 ? (m->g.max_blocks + 255) / 256 : m->sm_count * 4;
   TS_CUDA(ts_launch_pdl(k_collect_dirty, gc, 256, 0, st, m->g));
   TS_LAUNCH_CHECK(m);
+  return TSLAM_OK;
+}
+int ts_launch_commit(tslam_tsdf* m, cudaStream_t st, int clamp, int fused) {
+  { int rc = ts_collect_dirty(m, st); if (rc) return rc; }
   const unsigned long long seq = ++m->commit_seq;  // stamp of every block this commit writes (incremental mesh)
   TS_CUDA(ts_launch_pdl(k_commit_tma, m->sm_count * 3, 256, CM_SMEM, st, m->g, clamp, fused, m->blk_stamp, seq, m->scratch_i + 4));
   TS_LAUNCH_CHECK(m);
@@ -760,6 +764,7 @@ static void ts_fill_frame(tslam_tsdf* m, TsFrame& fr, const float* R9, const flo
   memcpy(fr.R, R9, 36);
   memcpy(fr.T, T3, 12);
   fr.submap = submap;
+  ts_map_written(m, submap);
   m->frame_seq++;  // 1, 2, ... (texture: later frames win); < 2^22 - TSLAM_MAX_BATCH (ts_seq_renorm runs before that)
   fr.seq = m->frame_seq;
 }

@@ -268,6 +268,30 @@ __device__ __forceinline__ void voxel_xyz(const TsGrid& g, bool global_map, cons
   pose_apply(pR + 9 * s, pT + 3 * s, lx, ly, lz, x, y, z);                 // submap_i_j_k_to_xyz :229-232
 }
 
+// Placement of one observed source voxel by the submap -> global fusions (k_fuse, k_fz_splat; dense_tsdf.py:293-303):
+// (i, j, k) of submap pose (R, T) lands at g = pose_apply(i vs, j vs, k vs) / vs in the global grid, and splats into the
+// 7 upper trilinear corners lo + (c >> 2 & 1, c >> 1 & 1, c & 1), c = 1 .. 7, of lo = floor(g) (c = 0 is skipped: the
+// reference quirk :300) with weight wt.  Both fusions call these two, so they place every term alike.
+struct TsSplatPos {
+  float gx, gy, gz;
+  int lo0, lo1, lo2;
+};
+// (lx, ly, lz) = (float)i * vs, ... are formed by the caller (the expression order of k_fuse's arguments is kept)
+__device__ __forceinline__ TsSplatPos ts_splat_pos(const float* R, const float* T, float lx, float ly, float lz, float vs) {
+  float x, y, z;
+  pose_apply(R, T, lx, ly, lz, x, y, z);  // :293-294
+  TsSplatPos p;
+  p.gx = x / vs; p.gy = y / vs; p.gz = z / vs;
+  p.lo0 = (int)floorf(p.gx); p.lo1 = (int)floorf(p.gy); p.lo2 = (int)floorf(p.gz);  // :296
+  return p;
+}
+// corner c of p: its cell (ci, cj, ck), weight wt (:303), and whether it lies in the volume of `dst`
+__device__ __forceinline__ bool ts_splat_corner(const TsGrid& dst, const TsSplatPos& p, int c, int& ci, int& cj, int& ck, float& wt) {
+  ci = p.lo0 + ((c >> 2) & 1); cj = p.lo1 + ((c >> 1) & 1); ck = p.lo2 + (c & 1);
+  wt = (1.0f - fabsf((float)ci - p.gx)) * (1.0f - fabsf((float)cj - p.gy)) * (1.0f - fabsf((float)ck - p.gz));
+  return ts_in_bounds(dst, ci, cj, ck);
+}
+
 __device__ __forceinline__ void red_add_f32x2(float2* addr, float a, float b) {
   // one 8-byte vector reduction without return value: REDG.E.ADD.F32x2 (sm_90+).  Spelled in PTX because
   // atomicAdd(float2*) was lowered to ATOMG (response sector per update) inside the divergent march loop.
@@ -581,6 +605,13 @@ struct tslam_tsdf {
   size_t reg_pts_bytes;
   void* render_jobs;   // per-camera jobs of tslam_tsdf_render (tslam_render.cu), grown geometrically
   size_t render_jobs_bytes;
+  // Change tracking of the incremental global fusion (tslam_tsdf_fuse_update, tslam_fuse.cu).  Every entry that writes a
+  // submap's planes calls ts_map_written, which bumps that submap's content version and the map's write generation;
+  // the update compares both against what it recorded when it last ran.
+  unsigned long long serial;        // process-unique number of the handle (an address can be reused by a new handle)
+  unsigned long long write_gen;     // writes of the planes by any entry other than tslam_tsdf_fuse_update
+  unsigned long long* content_ver;  // [max_submaps] host: writes of each submap's planes
+  struct TsFuse* fz;                // state of this map as the destination of tslam_tsdf_fuse_update (first call allocates)
   int march_verify;    // TSLAM_MARCH_VERIFY=1: every fast-path index is re-computed exactly, mismatches counted
   bool clamp_on_commit;
   // frame queue of the per-frame API (tslam_tsdf_queue_depth): double-buffered device staging fed by a copy stream
@@ -869,6 +900,12 @@ int ts_check_tex(tslam_tsdf* m, const uint8_t* tex, int th, int tw);  // a colou
 int ts_integrate_depth_impl(tslam_tsdf_t* m, const uint16_t* depth, int mem, int32_t n_frames, int32_t h, int32_t w, const float* R9s,
                             const float* T3s, const int32_t* submap_ids, int flags, void* stream, const uint8_t* tex = nullptr, int th = 0,
                             int tw = 0);
+// tslam_fuse.cu: change tracking of the incremental global fusion (tslam_tsdf::serial, write_gen, content_ver)
+int ts_fuse_init(tslam_tsdf* m);                         // at create: serial and content versions
+void ts_fuse_free(tslam_tsdf* m);                        // at destroy
+void ts_map_written(tslam_tsdf* m, int submap);          // submap's planes were written (submap < 0: every submap)
+// tslam_integrate.cu: k_collect_dirty on st (dirty_flag -> dirty_list, n_dirty)
+int ts_collect_dirty(tslam_tsdf* m, cudaStream_t st);
 // tslam_register.cu: *p holds at least `need` bytes: reallocated (contents dropped) to max(need, 2 x the old size) when smaller
 int rg_reserve(void** p, size_t* bytes, size_t need);
 // tslam_queue.cu: the per-frame queue's switches, copy stream and events of a new handle / their release

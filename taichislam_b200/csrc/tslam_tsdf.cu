@@ -245,6 +245,7 @@ extern "C" int tslam_tsdf_create(const tslam_tsdf_config_t* cfg, tslam_tsdf_t** 
   // (the workspace of the block-binned march - ~2 GB for 640x480 frames - is allocated by the first integrate launch:
   // global maps that are only ever fused into never pay for it)
   { int rci = ts_integrate_init(); if (rci) return rci; }
+  { int rcf = ts_fuse_init(m); if (rcf) return rcf; }
   TS_CUDA(cudaDeviceSynchronize());
   *out = m;
   return TSLAM_OK;
@@ -273,6 +274,7 @@ extern "C" int tslam_tsdf_destroy(tslam_tsdf_t* m) {
   if (m->bcnt) cudaFree(m->bcnt);
   cudaFree(m->depth_stage); cudaFree(m->points_stage);
   ts_queue_free(m);
+  ts_fuse_free(m);
   if (m->mw.rays) ts_march_free(m);
   cudaFree(m->counters); cudaFree(m->pose_R); cudaFree(m->pose_T); cudaFree(m->colormap);
   if (m->ev) { for (int i = 0; i < TS_PROF_EV * TS_PROF_RING; i++) cudaEventDestroy(m->ev[i]); delete[] m->ev; }
@@ -290,6 +292,7 @@ extern "C" int tslam_tsdf_reset(tslam_tsdf_t* m, void* stream) {
   m->mesh_epoch++;           // ... and the incremental mesh (planes cleared and pool slots recycled without stamps)
   m->q_n = 0;                // ... and so are queued frames
   m->q_gathered = 0;
+  ts_map_written(m, -1);     // ... and every submap's content
   TS_CUDA(cudaMemcpyAsync(&nb, g.n_blocks, 4, cudaMemcpyDeviceToHost, st));
   TS_CUDA(cudaStreamSynchronize(st));
   if (nb > g.max_blocks) nb = g.max_blocks;
@@ -445,6 +448,7 @@ extern "C" int tslam_tsdf_scatter2(tslam_tsdf_t* m, int32_t submap, int64_t n, c
   if (grid > m->sm_count * 32) grid = m->sm_count * 32;
   m->esdf_full_needed = 1;  // bulk load: values change without a commit
   m->mesh_epoch++;          // (same for the incremental mesh)
+  ts_map_written(m, submap);
   k_scatter<<<grid, 256, 0, st>>>(m->g, submap, n, idx, tsdf, w, occ, color);
   TS_LAUNCH_CHECK(m);
   return TSLAM_OK;
@@ -584,16 +588,13 @@ __global__ void __launch_bounds__(256) k_fuse(TsGrid dst, TsGrid src, const floa
       const bool tex = dst.col != nullptr && src.col != nullptr;
       float4 sc = make_float4(0.f, 0.f, 0.f, 0.f);
       if (tex) sc = src.col[base + v];
-      float x, y, z;
-      pose_apply(pR + 9 * s, pT + 3 * s, (float)(bx * TS_B + (v >> 8)) * vs, (float)(by * TS_B + ((v >> 4) & 15)) * vs,
-                 (float)(bz * TS_B + (v & 15)) * vs, x, y, z);  // :293-294
-      const float gx = x / vs, gy = y / vs, gz = z / vs;
-      const int lo0 = (int)floorf(gx), lo1 = (int)floorf(gy), lo2 = (int)floorf(gz);  // :296
+      const TsSplatPos p = ts_splat_pos(pR + 9 * s, pT + 3 * s, (float)(bx * TS_B + (v >> 8)) * vs, (float)(by * TS_B + ((v >> 4) & 15)) * vs,
+                                        (float)(bz * TS_B + (v & 15)) * vs, vs);
 #pragma unroll
       for (int c = 1; c < 8; c++) {  // c=0 (di=dj=dk=0) skipped: reference quirk :300
-        const int ci = lo0 + ((c >> 2) & 1), cj = lo1 + ((c >> 1) & 1), ck = lo2 + (c & 1);
-        const float wt = (1.0f - fabsf((float)ci - gx)) * (1.0f - fabsf((float)cj - gy)) * (1.0f - fabsf((float)ck - gz));  // :303
-        if (!ts_in_bounds(dst, ci, cj, ck)) continue;
+        int ci, cj, ck;
+        float wt;
+        if (!ts_splat_corner(dst, p, c, ci, cj, ck, wt)) continue;
         const unsigned long long key = ts_pack_key(0, ci >> TS_BSHIFT, cj >> TS_BSHIFT, ck >> TS_BSHIFT);
         if (key != cur_key) {
           cur_key = key;

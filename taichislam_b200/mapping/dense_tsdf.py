@@ -187,6 +187,13 @@ class DenseTSDF(BaseMap):
         print(f"[DenseTSDF] Fuse submaps {(time.time() - t) * 1000:.1f}ms, active local: {submaps.active_submap_id[None]} "
               f"remote: {submaps.remote_submap_num[None]}")
 
+    def update_fused_submaps(self, submaps, include=None, tolerance=0.0, full=False):
+        """Keep this global map equal to the fusion of `submaps` (a DenseTSDF collection) with exact integer sums,
+        re-splatting only the submaps that were added, moved or removed since the last call (TsdfHandle.fuse_update).
+        Queued frames of `submaps` are integrated first.  -> dict of the call's statistics."""
+        submaps._flush()
+        return self._h.fuse_update(submaps._h, include=include, tolerance=tolerance, full=full)
+
     # ------------------------------------------------------------------ exporters (:320-389)
     def _active(self):
         return 0 if self.is_global_map else self.active_submap_id[None]

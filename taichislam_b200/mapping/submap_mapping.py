@@ -7,6 +7,13 @@ scripts/taichislam_node.py can drive it unchanged.  Differences, all fixes of re
 (SURVEY.md Appendix B): no hard-coded save path (submap_mapping.py:144-145 writes to /home/xuhao/...),
 `recast_depth_to_map(R, T, ...)` works (the reference calls need_create_new_submap with the wrong arity,
 :195-196), send handles are optional.
+
+global_fusion="incremental" (TSDF submaps only) keeps the global map with DenseTSDF.update_fused_submaps instead of
+rebuilding it at every submap switch: only submaps that were added, moved or removed are re-splatted, so
+set_frame_poses and input_remote_submap refresh the global map (its mesh and the callback) at once.  The active
+submap is left out of the global map in that mode: the reference fuses at the switch, when the active submap is
+empty, and its global-mode exporters add the active submap separately.  One deviation: when a remote submap arrives
+in the middle of a submap, the reference's rebuild also fuses the local active submap; the incremental mode does not.
 """
 import io
 import time
@@ -29,7 +36,15 @@ _COMMON = dict(voxel_scale=0.05, texture_enabled=False, min_ray_length=0.3, max_
 
 
 class SubmapMapping:
-    def __init__(self, submap_type=DenseTSDF, keyframe_step=20, sub_opts={}, global_opts={}, autosave_path=None):
+    def __init__(self, submap_type=DenseTSDF, keyframe_step=20, sub_opts={}, global_opts={}, autosave_path=None,
+                 global_fusion="rebuild", fusion_tolerance=0.0):
+        if global_fusion not in ("rebuild", "incremental"):
+            raise ValueError(f"global_fusion must be 'rebuild' or 'incremental', not {global_fusion!r}")
+        if global_fusion == "incremental" and submap_type is not DenseTSDF:
+            raise ValueError("global_fusion='incremental' needs TSDF submaps")
+        self.global_fusion = global_fusion
+        self.fusion_tolerance = float(fusion_tolerance)
+        self.last_fusion_stats = None  # statistics of the last incremental update
         self.submap_type = submap_type
         self.keyframe_step = keyframe_step
         self.autosave_path = autosave_path
@@ -55,6 +70,8 @@ class SubmapMapping:
     def create_globalmap(self, global_opts={}):  # submap_mapping.py:58-84
         kind = dict(num_voxel_per_blk_axis=10, max_submap_num=1024) if self.submap_type is DenseTSDF else dict(K=2, max_submap_num=1000)
         opts = _merged(_merged(_COMMON, dict(map_scale=[100, 100], is_global_map=True, **kind)), global_opts)
+        if getattr(self, "global_fusion", "rebuild") == "incremental" and "max_submap_num" not in (global_opts or {}):
+            opts["max_submap_num"] = self.sub_opts["max_submap_num"]  # the incremental fusion pairs submap tables of one size
         return self.submap_type(**opts)
 
     # -- intrinsics ----------------------------------------------------------------------------
@@ -93,6 +110,8 @@ class SubmapMapping:
             if fid in self.submaps:
                 self.global_map.set_base_pose_submap(self.submaps[fid], R, T)
                 used[fid] = (R, T)
+        if used and self.global_fusion == "incremental":
+            self.local_to_global()  # the correction reaches the global map now, not at the next submap switch
         if not from_remote:
             self.send_traj(used)
 
@@ -156,7 +175,13 @@ class SubmapMapping:
         return self.submap_collection
 
     def local_to_global(self):
-        self.global_map.fuse_submaps(self.submap_collection)
+        if self.global_fusion == "incremental":
+            sc = self.submap_collection
+            include = np.ones(sc.max_submap_num, bool)
+            include[sc.get_active_submap_id()] = False  # the growing submap is exported separately (see above)
+            self.last_fusion_stats = self.global_map.update_fused_submaps(sc, include=include, tolerance=self.fusion_tolerance)
+        else:
+            self.global_map.fuse_submaps(self.submap_collection)
         if self.post_local_to_global_callback is not None:
             self.post_local_to_global_callback(self.global_map)
 

@@ -183,6 +183,25 @@ class TsdfHandle:
     def fuse_from(self, src):
         capi.check(self.L.tslam_tsdf_fuse(self.h, src.h, capi.stream_ptr()))
 
+    def fuse_update(self, src, include=None, tolerance=0.0, full=False):
+        """Incremental fusion of the submaps of `src` (a TsdfHandle) into this global map (tslam_tsdf_fuse_update):
+        afterwards this map is the exact-sum fusion of the included submaps at their fused poses.  include: None (all) or
+        bools / 0-1 per submap (up to max_submaps); tolerance: how far (metres, translation + angle x radius) a fused
+        submap may move before it is re-splatted; full=True forces a rebuild.  -> dict of the call's statistics."""
+        inc = None
+        if include is not None:
+            n = int(self.cfg.max_submaps)
+            a = np.asarray(include).reshape(-1).astype(bool)
+            assert a.shape[0] <= n, "include has more entries than max_submaps"
+            inc = np.zeros(n, np.uint8)
+            inc[:a.shape[0]] = a
+        st = np.zeros(8, np.int64)
+        capi.check(self.L.tslam_tsdf_fuse_update(self.h, src.h, capi.np_ptr(inc) if inc is not None else None, float(tolerance),
+                                                 int(bool(full)), capi.np_ptr(st), capi.stream_ptr()))
+        return dict(full=bool(st[0] != 0), reason=capi.FUSE_REASONS[int(st[0])], added=int(st[1]), moved=int(st[2]),
+                    removed=int(st[3]), within_tolerance=int(st[4]), voxels_splatted=int(st[5]), voxels_skipped=int(st[6]),
+                    blocks_committed=int(st[7]))
+
     def extract_surface(self, submap, xyz, rgb, count):
         """Append to torch CUDA buffers xyz/rgb f32[cap,3]; count: int32[1] device counter."""
         capi.check(self.L.tslam_tsdf_extract_surface(self.h, int(submap), xyz.shape[0], capi.tptr(xyz), capi.tptr(rgb),

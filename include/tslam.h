@@ -787,6 +787,61 @@ int tslam_tsdf_render(tslam_tsdf_t* m, int32_t n, int32_t height, int32_t width,
                       const double* R, const double* T, float z_min, float z_max, float step, float* depth, float* normal,
                       float* color, uint8_t* status, void* stream);
 
+/* ----------------------------------------------------------------------------
+ * Trajectories against an ESDF (DESIGN.md section 7, "Trajectories"; tslam_traj.cuh states every operation)
+ *
+ * T uniform cubic B-splines, trajectory t with N_t = n_ctrl[t] control points Q_0 .. Q_{N-1} (f64, the submap-local map
+ * frame tslam_esdf_query takes) and knot span dt, optimised against the ESDF of `submap` as of its last update.  The
+ * first three and the last three control points are fixed (start and end position, velocity and acceleration); the
+ * free variables are Q_3 .. Q_{N-4}.  Span j = 0 .. N-4 uses Q_j .. Q_{j+3}; collision samples sit at u = k/K,
+ * k = 0 .. K-1, on every span plus u = 1 on the last ((N-3) K + 1 samples); a sample's position is
+ * ((b0 Q_j + b1 Q_{j+1}) + b2 Q_{j+2}) + b3 Q_{j+3} in f64, rounded to f32 once, and its distance d and gradient g are
+ * exactly what the ESDF query returns at that f32 point, with its validity rule.  Cost, f64:
+ *   J_s = sum |Q_{i+3} - 3 Q_{i+2} + 3 Q_{i+1} - Q_i|^2                        (smoothness)
+ *   J_c = sum over valid samples with d < c of (c - d)^2                        (collision, c = clearance)
+ *   J_u = number of invalid samples, no gradient                                (unknown or absent space)
+ *   J_f = sum max(0, |V_i|^2 - v^2)^2 + sum max(0, |A_i|^2 - a^2)^2,  V_i = (Q_{i+1} - Q_i)/dt,
+ *         A_i = (Q_{i+2} - 2 Q_{i+1} + Q_i)/dt^2                                (feasibility)
+ *   J   = w_s J_s + w_c J_c + w_f J_f + w_u J_u
+ * Solver: L-BFGS on the device in f64, memory M; the first direction is -g scaled to one voxel in its largest
+ * component, and a direction that does not descend resets the history; Armijo backtracking from alpha = 1 (c1 = 1e-4,
+ * halving, at most 30 trials); a pair is kept when s'y > 1e-10 y'y.  Status: 1 |g|inf <= g_tol, 2 line search
+ * exhausted, 0 max_iters steps taken, 3 N < 7 (nothing to optimise: evaluated only).  max_iters = 0 evaluates the input
+ * (a batched safety check of committed trajectories).  Then a dense check of the result at C samples per span, placed
+ * the same way.  Every sum runs in a fixed order (tslam_traj.cuh), so one trajectory's result depends on nothing else
+ * in the call, and repeated calls give the same bits.
+ *
+ * Arrays (HOST): n_ctrl i32[T]; ctrl_in, ctrl_out f64[sum N, 3] (trajectories back to back); cost f64[T, 6]: J_s, J_c,
+ * J_f, J_u at the result, J at the input, the least d over the valid check samples (+inf when none); info i32[T, 7]:
+ * iterations, evaluations, status, invalid check samples, valid check samples with d < c, and the span and k of the
+ * least d (lowest (span, k) on ties; -1 when no sample is valid).
+ * Refused (TSLAM_E_INVALID) before the handle is looked at: a NULL array or params; T outside [1, 1024]; an N outside
+ * [4, 1024]; sum N > 2^20; samples (K) outside [1, 16], check_samples (C) outside [1, 64], memory (M) outside [1, 16];
+ * dt, v_max, a_max not finite and > 0; a weight, the clearance or g_tol not finite and >= 0; max_iters < 0; a
+ * non-finite control point.  Then: a NULL handle; the field not readable (tslam_esdf_query's rules for the TSDF;
+ * tslam_octo_esdf_query's for the Octomap, which refuse a hit-count map); a clearance above the field's far value (the
+ * TSDF's max_ray_length; the max_dist of the Octomap's last ESDF update).
+ * Writes no map word, ESDF, frontier, travel or mesh state and no statistic other than the kernel-launch counter.  One
+ * launch; synchronises on `stream`.  Device scratch of (18 + 6 M) 8 sum N bytes plus the inputs and outputs, grown
+ * geometrically and freed by destroy; an allocation failure is TSLAM_E_CUDA with the byte count in tslam_last_error. */
+typedef struct tslam_traj_params {
+  double dt;                  /* knot span (s) */
+  double v_max, a_max;        /* velocity and acceleration limits */
+  double w_smooth, w_collision, w_feasibility, w_unknown;
+  double clearance;           /* c (m) */
+  double g_tol;               /* stop when |g|inf <= g_tol */
+  int32_t max_iters;          /* L-BFGS steps at most (0: evaluate and check only) */
+  int32_t memory;             /* M, L-BFGS pairs kept */
+  int32_t samples;            /* K, collision samples per span */
+  int32_t check_samples;      /* C, check samples per span */
+} tslam_traj_params_t;
+#define TSLAM_TRAJ_MAX 1024
+#define TSLAM_TRAJ_MAX_CTRL 1024
+int tslam_esdf_trajectory(tslam_tsdf_t* m, int32_t submap, int32_t T, const int32_t* n_ctrl, const double* ctrl_in,
+                          const tslam_traj_params_t* params, double* ctrl_out, double* cost, int32_t* info, void* stream);
+int tslam_octo_esdf_trajectory(tslam_octo_t* m, int32_t submap, int32_t T, const int32_t* n_ctrl, const double* ctrl_in,
+                               const tslam_traj_params_t* params, double* ctrl_out, double* cost, int32_t* info, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

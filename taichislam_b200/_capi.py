@@ -30,6 +30,14 @@ class TslamError(RuntimeError):
         self.code = code
 
 
+class TrajParams(C.Structure):
+    """tslam_traj_params_t"""
+    _fields_ = [("dt", C.c_double), ("v_max", C.c_double), ("a_max", C.c_double), ("w_smooth", C.c_double),
+                ("w_collision", C.c_double), ("w_feasibility", C.c_double), ("w_unknown", C.c_double),
+                ("clearance", C.c_double), ("g_tol", C.c_double), ("max_iters", C.c_int32), ("memory", C.c_int32),
+                ("samples", C.c_int32), ("check_samples", C.c_int32)]
+
+
 class TsdfConfig(C.Structure):
     _fields_ = [("voxel_scale", C.c_double), ("N", C.c_int32), ("Nz", C.c_int32),
                 ("max_ray_length", C.c_double), ("min_ray_length", C.c_double),
@@ -190,6 +198,8 @@ SIGNATURES = {
                                           _vp]),
     "tslam_tsdf_fuse_update": (C.c_int, [_vp, _vp, _vp, _f32, _i32, _vp, _vp]),
     "tslam_tsdf_render": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _f32, _f32, _f32, _vp, _vp, _vp, _vp, _vp]),
+    "tslam_esdf_trajectory": (C.c_int, [_vp, _i32, _i32, _vp, _vp, C.POINTER(TrajParams), _vp, _vp, _vp, _vp]),
+    "tslam_octo_esdf_trajectory": (C.c_int, [_vp, _i32, _i32, _vp, _vp, C.POINTER(TrajParams), _vp, _vp, _vp, _vp]),
 }
 
 _lib = None

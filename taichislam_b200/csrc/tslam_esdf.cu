@@ -30,6 +30,7 @@
 // from the voxels the frame just touched (dense_esdf.py:309-330) and has a raise and a lower queue (:260-299).
 #include <cstring>
 #include "tslam_esdf_common.cuh"
+#include "tslam_traj.cuh"
 
 enum { ES_UNOBS = 0, ES_FIXED = 1, ES_POS = 2, ES_NEG = 3, ES_INERT = 4 };  // INERT: observed, TSDF is NaN
 
@@ -383,4 +384,23 @@ extern "C" int tslam_esdf_extract_slice(tslam_tsdf_t* m, int32_t submap, float z
                                                                           val, count_dev);
   TS_LAUNCH_CHECK(m);
   return TSLAM_OK;
+}
+
+// Trajectories against this ESDF (tslam_traj.cuh), read as tslam_esdf_query reads it
+extern "C" int tslam_esdf_trajectory(tslam_tsdf_t* m, int32_t submap, int32_t T, const int32_t* n_ctrl, const double* ctrl_in,
+                                     const tslam_traj_params_t* params, double* ctrl_out, double* cost, int32_t* info, void* stream) {
+  const char* what = "tslam_esdf_trajectory";
+  long long sum_n = 0;
+  int rc = tj_check_args(what, T, n_ctrl, ctrl_in, params, ctrl_out, cost, info, &sum_n);
+  if (rc) return rc;
+  if (!m) { ts_set_error("%s: NULL handle", what); return TSLAM_E_INVALID; }
+  rc = es_readable(m, submap, what);
+  if (rc) return rc;
+  if (params->clearance > m->cfg.max_ray_length) {
+    ts_set_error("%s: clearance %g above the ESDF's far value max_ray_length %g", what, params->clearance, m->cfg.max_ray_length);
+    return TSLAM_E_INVALID;
+  }
+  const EsTsdf p{m->g, es_aux(m), submap, 0.0f, 0.0f, m->in.vs, m->esdf_tiled == 2};
+  return tj_run(m, p, m->in.vs, what, &m->traj_mem, &m->traj_mem_bytes, T, n_ctrl, sum_n, ctrl_in, params, ctrl_out, cost, info,
+                (cudaStream_t)stream);
 }

@@ -415,34 +415,43 @@ __device__ __forceinline__ bool ts_sdf_corners(const TsGrid& g, const int c0[3],
 // es_qblock refuses, a corner whose class at the last update has no value.  The body of each ESDF's query kernel, which
 // keeps the grid and the state as separate parameters: built around one rule parameter, the occupancy ESDF's query
 // compiles to 40 registers instead of 32 (6 instead of 8 CTAs per SM).
+//
+// es_point is the answer at one point x (nb_seen = *p.a.nb_seen): whether it is valid, and d, gx, gy, gz (NaN when
+// not).  The query kernels and the trajectory solver (tslam_traj.cuh) both read the field through it.
+template <class P>
+__device__ __forceinline__ bool es_point(const P& p, int nb_seen, const float* x, float& d, float& gx, float& gy, float& gz) {
+  constexpr int S = P::SHIFT;
+  const float vs = p.vs, qnan = __int_as_float(0x7fc00000);
+  // both corners i0, i0 + 1 inside the volume: the low corner and i0 < N - hN - 1 per axis
+  float u[3];
+  int c0[3];
+  bool ok = esq_low_corner(p.g, vs, x, u, c0) && c0[0] < p.g.N - p.g.hN - 1 && c0[1] < p.g.N - p.g.hN - 1 &&
+            c0[2] < p.g.Nz - p.g.hNz - 1;
+  d = qnan; gx = qnan; gy = qnan; gz = qnan;
+  if (ok) {
+    const int i0 = c0[0], j0 = c0[1], k0 = c0[2];
+    const float fx = __fsub_rn(u[0], (float)i0), fy = __fsub_rn(u[1], (float)j0), fz = __fsub_rn(u[2], (float)k0);
+    float e[8];
+    ok = es_corners<S>(
+        i0, j0, k0, [&](int bx, int by, int bz) { return es_qblock(p, nb_seen, bx, by, bz); },
+        [&](size_t off, float& ev) {
+          const bool has = P::valid(p.a.cls[off] & ES_CLS);
+          ev = p.field()[off];
+          return has;
+        },
+        e);
+    if (ok) esq_interp(e, fx, fy, fz, vs, d, gx, gy, gz);
+    else d = gx = gy = gz = qnan;
+  }
+  return ok;
+}
 template <class P>
 __device__ __forceinline__ void es_query(const P& p, long long n, const float* __restrict__ xyz, float* __restrict__ dist,
                                                   float* __restrict__ grad, uint8_t* __restrict__ valid) {
-  constexpr int S = P::SHIFT;
   const int nb_seen = *p.a.nb_seen;
-  const float vs = p.vs, qnan = __int_as_float(0x7fc00000);
   for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < n; q += (long long)gridDim.x * blockDim.x) {
-    // both corners i0, i0 + 1 inside the volume: the low corner and i0 < N - hN - 1 per axis
-    float u[3];
-    int c0[3];
-    bool ok = esq_low_corner(p.g, vs, xyz + 3 * q, u, c0) && c0[0] < p.g.N - p.g.hN - 1 && c0[1] < p.g.N - p.g.hN - 1 &&
-              c0[2] < p.g.Nz - p.g.hNz - 1;
-    float d = qnan, gx = qnan, gy = qnan, gz = qnan;
-    if (ok) {
-      const int i0 = c0[0], j0 = c0[1], k0 = c0[2];
-      const float fx = __fsub_rn(u[0], (float)i0), fy = __fsub_rn(u[1], (float)j0), fz = __fsub_rn(u[2], (float)k0);
-      float e[8];
-      ok = es_corners<S>(
-          i0, j0, k0, [&](int bx, int by, int bz) { return es_qblock(p, nb_seen, bx, by, bz); },
-          [&](size_t off, float& ev) {
-            const bool has = P::valid(p.a.cls[off] & ES_CLS);
-            ev = p.field()[off];
-            return has;
-          },
-          e);
-      if (ok) esq_interp(e, fx, fy, fz, vs, d, gx, gy, gz);
-      else d = gx = gy = gz = qnan;
-    }
+    float d, gx, gy, gz;
+    const bool ok = es_point(p, nb_seen, xyz + 3 * q, d, gx, gy, gz);
     dist[q] = d;
     grad[3 * q] = gx; grad[3 * q + 1] = gy; grad[3 * q + 2] = gz;
     valid[q] = ok ? 1 : 0;

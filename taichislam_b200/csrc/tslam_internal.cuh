@@ -605,6 +605,8 @@ struct tslam_tsdf {
   size_t reg_pts_bytes;
   void* render_jobs;   // per-camera jobs of tslam_tsdf_render (tslam_render.cu), grown geometrically
   size_t render_jobs_bytes;
+  void* traj_mem;      // inputs, outputs and solver work of tslam_esdf_trajectory (tslam_traj.cuh), grown geometrically
+  size_t traj_mem_bytes;
   // Change tracking of the incremental global fusion (tslam_tsdf_fuse_update, tslam_fuse.cu).  Every entry that writes a
   // submap's planes calls ts_map_written, which bumps that submap's content version and the map's write generation;
   // the update compares both against what it recorded when it last ran.
@@ -757,6 +759,9 @@ struct tslam_octo {
   // travel-cost fields of a log-odds map (tslam_octo_travel_*, tslam_octo_travel.cu): the single-source field
   // (tslam_octo_travel_update, S = 1) and the many-source fields (tslam_octo_travel_multi_update), kept apart
   OcTravel tr, trm;
+  // inputs, outputs and solver work of tslam_octo_esdf_trajectory (tslam_traj.cuh), grown geometrically
+  void* traj_mem;
+  size_t traj_mem_bytes;
 };
 int oc_esdf_free(tslam_octo* m);      // tslam_octo_esdf.cu
 int oc_frontier_free(tslam_octo* m);  // tslam_octo_frontier.cu

@@ -472,6 +472,7 @@ extern "C" int tslam_octo_destroy(tslam_octo_t* m) {
   oc_frontier_free(m);
   oc_view_free(m);
   oc_travel_free(m);
+  if (m->traj_mem) cudaFree(m->traj_mem);
   delete m;
   return TSLAM_OK;
 }

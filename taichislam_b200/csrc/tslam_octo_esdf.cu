@@ -20,6 +20,7 @@
 #include <cmath>
 #include <cstring>
 #include "tslam_esdf_common.cuh"
+#include "tslam_traj.cuh"
 
 struct OeAux {
   float* e;            // [max_blocks*512] the field
@@ -206,4 +207,24 @@ extern "C" int tslam_octo_esdf_query(tslam_octo_t* m, int32_t submap, int64_t n,
                                                                                          grad, valid);
   TS_LAUNCH_CHECK(m);
   return TSLAM_OK;
+}
+
+// Trajectories against the occupancy ESDF (tslam_traj.cuh), read as tslam_octo_esdf_query reads it
+extern "C" int tslam_octo_esdf_trajectory(tslam_octo_t* m, int32_t submap, int32_t T, const int32_t* n_ctrl, const double* ctrl_in,
+                                          const tslam_traj_params_t* params, double* ctrl_out, double* cost, int32_t* info,
+                                          void* stream) {
+  const char* what = "tslam_octo_esdf_trajectory";
+  long long sum_n = 0;
+  int rc = tj_check_args(what, T, n_ctrl, ctrl_in, params, ctrl_out, cost, info, &sum_n);
+  if (rc) return rc;
+  if (!m) { ts_set_error("%s: NULL handle", what); return TSLAM_E_INVALID; }
+  rc = oc_track_readable(m, m->esdf_track, submap, what, "tslam_octo_esdf_update");
+  if (rc) return rc;
+  if (params->clearance > (double)m->esdf_D) {
+    ts_set_error("%s: clearance %g above the max_dist %g of the last ESDF update", what, params->clearance, (double)m->esdf_D);
+    return TSLAM_E_INVALID;
+  }
+  const EsOcto p{m->g, oe_aux(m), submap, 0, 0.0f, m->in.vs, nullptr};
+  return tj_run(m, p, m->in.vs, what, &m->traj_mem, &m->traj_mem_bytes, T, n_ctrl, sum_n, ctrl_in, params, ctrl_out, cost, info,
+                (cudaStream_t)stream);
 }

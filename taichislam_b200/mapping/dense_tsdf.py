@@ -360,6 +360,23 @@ class DenseTSDF(BaseMap):
             self._h.esdf_update(self._active())
         return self._h.esdf_query(xyz, submap=self._active())
 
+    def optimize_trajectories(self, paths_or_ctrl, clearance, spacing=None, ctrl=False, update=True, **settings):
+        """Smooth collision-free trajectories along paths or control points of the active submap's map frame: each
+        entry of paths_or_ctrl is a path f[n,3] (e.g. plan_exploration()["path"] or a travel_path result), made into
+        control points by trajectory.control_points(path, spacing) (spacing defaults to two voxels), or, with
+        ctrl=True, control points themselves.  The free control points are optimised on the GPU against the ESDF
+        (L-BFGS, include/tslam.h tslam_esdf_trajectory) and the result checked densely.  update=True first brings the
+        field up to date, as esdf_query(update=True) does.  -> a list of dicts, one per trajectory: ctrl f64[N,3], the
+        cost terms, iterations, evaluations, status and the check (min_dist, min_at, invalid, close, ok).  settings:
+        trajectory.DEFAULTS (dt, v_max, a_max, weights, g_tol, max_iters, memory, samples, check_samples)."""
+        from ..trajectory import control_points
+        self._flush()
+        if update:
+            self._h.esdf_update(self._active())
+        sp = 2.0 * self.voxel_scale if spacing is None else float(spacing)
+        qs = [np.asarray(q, np.float64) if ctrl else control_points(q, sp) for q in paths_or_ctrl]
+        return self._h.trajectory(qs, clearance, submap=self._active(), **settings)
+
     def cvt_ESDF_to_voxels_slice(self, z):
         """dense_esdf.py:498-509, after bringing the field up to date: the ESDF voxels of the slice at height z into
         export_ESDF / export_ESDF_xyz, their number into num_export_ESDF_particles.  Only voxels observed at the update

@@ -190,6 +190,23 @@ class Octomap(BaseMap):
             self.esdf_update(getattr(self, "esdf_max_dist", None))
         return self._h.esdf_query(xyz, submap=self._active())
 
+    def optimize_trajectories(self, paths_or_ctrl, clearance, spacing=None, ctrl=False, update=True, **settings):
+        """Smooth collision-free trajectories along paths or control points of the active submap's map frame: each
+        entry of paths_or_ctrl is a path f[n,3] (e.g. plan_exploration()["path"] or a travel_path result), made into
+        control points by trajectory.control_points(path, spacing) (spacing defaults to two voxels), or, with
+        ctrl=True, control points themselves.  The free control points are optimised on the GPU against the ESDF
+        (L-BFGS, include/tslam.h tslam_octo_esdf_trajectory) and the result checked densely.  update=True first brings the
+        field up to date, as esdf_query(update=True) does.  -> a list of dicts, one per trajectory: ctrl f64[N,3], the
+        cost terms, iterations, evaluations, status and the check (min_dist, min_at, invalid, close, ok).  settings:
+        trajectory.DEFAULTS (dt, v_max, a_max, weights, g_tol, max_iters, memory, samples, check_samples)."""
+        self._logodds_only("trajectory optimisation")
+        from ..trajectory import control_points
+        if update:
+            self.esdf_update(getattr(self, "esdf_max_dist", None))
+        sp = 2.0 * self.voxel_scale if spacing is None else float(spacing)
+        qs = [np.asarray(q, np.float64) if ctrl else control_points(q, sp) for q in paths_or_ctrl]
+        return self._h.esdf_trajectory(qs, clearance, submap=self._active(), **settings)
+
     # exploration frontiers (log-odds maps only, DESIGN.md section 7): FREE voxels next to in-volume UNKNOWN space
     def frontier_update(self, full=False):
         """Bring the frontier set of the active submap up to date (incremental when possible) -> dict(voxels, clusters,

@@ -238,6 +238,13 @@ class OctoHandle:
                                                 capi.tptr(valid), capi.stream_ptr()))
         return self._out(isinstance(xyz, torch.Tensor), dist, grad, valid.view(torch.bool))  # the kernel writes 0 / 1
 
+    def esdf_trajectory(self, ctrls, clearance, submap=0, **settings):
+        """Optimise uniform cubic B-splines (control points f[N,3] each, the submap's map frame) against the occupancy
+        ESDF of `submap` as of its last esdf_update (tslam_octo_esdf_trajectory) -> a list of dicts (trajectory.solve).
+        settings: trajectory.DEFAULTS."""
+        from . import trajectory
+        return trajectory.solve(self.L.tslam_octo_esdf_trajectory, self.h, submap, ctrls, clearance, **settings)
+
     # -- frontiers of a log-odds map (tslam_octo_frontier_*, DESIGN.md section 7) --------------------------------------
     def frontier_update(self, submap=0, full=False):
         """Bring the frontier set of `submap` up to date (incremental unless full, the last update was for another submap,

@@ -351,6 +351,13 @@ class TsdfHandle:
             return dist, grad, valid
         return dist.cpu().numpy(), grad.cpu().numpy(), valid.cpu().numpy()
 
+    def trajectory(self, ctrls, clearance, submap=0, **settings):
+        """Optimise uniform cubic B-splines (control points f[N,3] each, the submap's map frame) against the ESDF of
+        `submap` as of its last esdf_update (tslam_esdf_trajectory) -> a list of dicts (trajectory.solve).  settings:
+        trajectory.DEFAULTS."""
+        from . import trajectory
+        return trajectory.solve(self.L.tslam_esdf_trajectory, self.h, submap, ctrls, clearance, **settings)
+
     def esdf_extract_slice(self, submap, z, xyz, val, count):
         """Append the ESDF slice at height z to torch CUDA buffers xyz f32[cap,3] / val f32[cap]; count: int32[1] device counter."""
         capi.check(self.L.tslam_esdf_extract_slice(self.h, int(submap), float(z), xyz.shape[0], capi.tptr(xyz), capi.tptr(val),

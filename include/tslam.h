@@ -202,15 +202,17 @@ int tslam_tsdf_get_stats(tslam_tsdf_t* m, int64_t* out8, int clear);
 int tslam_tsdf_sync(tslam_tsdf_t* m, void* stream);
 /* Kernels launched by this handle since creation (bench.py `gpu_launches`). */
 int64_t tslam_tsdf_launch_count(tslam_tsdf_t* m);
-/* CUDA-event timing of the integrate kernels, recorded on the launching stream when
- * profiling is on (ring of the last 512 integrate launches).  tslam_tsdf_kernel_ms writes
- * ms3[3*i+{0,1,2}] = bucket / ray-march / commit kernel time of the i-th most recent launch,
- * i < min(n, recorded); *n_out = rows written.  Synchronises. */
+/* Timing of the integrate kernels when profiling is on (ring of the last 512 integrate launches): each kernel
+ * stamps the GPU's global timer at the entry of its first CTA and the exit of its last one; nothing is recorded on
+ * the stream.  A stage is charged from the later of its first kernel's start and the end of the stage before it,
+ * to its last kernel's end, so the columns of a launch never sum to more than its span.  tslam_tsdf_kernel_ms writes
+ * ms3[3*i+{0,1,2}] = bucket / ray-march / commit time of the i-th most recent launch (commit 0 for a launch
+ * without one), i < min(n, recorded); *n_out = rows written.  Synchronises. */
 int tslam_tsdf_set_profiling(tslam_tsdf_t* m, int on);
 int tslam_tsdf_kernel_ms(tslam_tsdf_t* m, int32_t n, float* ms3, int32_t* n_out);
-/* Same ring, 7 columns per launch: bucket, ray march (all its kernels), commit, then the ray march split into
- * ray set-up + segment count / scan / segment fill / block march (tslam_march.cu; zeros for textured maps, which
- * march with one thread per ray). */
+/* Same ring, 7 columns per launch: bucket, ray march (all its kernels), commit, 0, then the ray march split into
+ * ray set-up + counting walk + class + scan / scattering walk / block march (tslam_march.cu; zeros for textured
+ * maps, which march with one thread per ray). */
 int tslam_tsdf_kernel_ms2(tslam_tsdf_t* m, int32_t n, float* ms7, int32_t* n_out);
 /* Diagnostics of the block-binned ray march (process_new_pcl, dense_tsdf.py:236-270) since the last clear of
  * tslam_tsdf_get_stats: out6 = segments, work items, samples that took the exact-index path (fraction within

@@ -217,12 +217,28 @@ __device__ __forceinline__ void append_rays_cta(int fresh_slot, uint32_t tab_bas
 // row per thread, :192-194); a warp covers an 8x4 tile of sampled pixels, a CTA 32x8;
 // blockIdx.z = frame of the batch.  Six CTAs per SM (40 registers): each CTA is one chain of dependent round trips
 // (depth load, index probe, CAS, ray append), so resident CTAs, not bandwidth, set the kernel's rate.
+//
+// Both bucket kernels are launched with programmatic dependent launch (ts_launch_pdl) after the previous launch's
+// commit (or march), so their grid is dispatched while that kernel finishes.  They wait for it at entry, before the
+// first load.  What the kernel reads or writes that an earlier kernel on the stream may still own:
+//   * the frames / points: the caller's device memory may come from the caller's own kernel right before this launch
+//     (PDL relaxes exactly that dependency), so even the depth load waits.  Host batches and queued frames are copied
+//     into the staging buffers by a copy the stream waits for in full (memcpy, event wait: an ordinary launch);
+//   * n_rays: set back to 0 by the previous launch's march tail (k_march_blocks, last CTA) or by k_reset_counters.
+//     k_march_blocks triggers no early launch, so every wait of the chain after it covers its whole grid;
+//   * the bucket index: cleared by a memset when the epoch wraps (every 15 launches; an ordinary launch again) and
+//     probed / written by the previous launch's bucket kernel and set-up, two kernels back;
+//   * staging buffer 0 (host batches) and ev_free[0]: the host waits on ev_free before it refills a buffer, and
+//     k_gather_rows runs on the copy stream behind ev_copied: neither is a kernel this one follows;
+//   * rm_reserve only sizes the march grid on the host.
 // ---------------------------------------------------------------------------
 __global__ void __launch_bounds__(256, 6) k_bucket_depth(const uint16_t* __restrict__ depth, int frame_stride, int row_mul, int w, int hh, int ww,
                                                        const __grid_constant__ TsBatch batch, TsIntrin in, int agg_ok,
                                                        TsBucket* buckets, uint4* bcol, unsigned long long* bidx, uint32_t bucket_cap,
                                                        TsBucketLaunch bl, uint32_t* ray_list, int* n_rays, uint32_t ray_cap, TsCounters* ctr, int* err,
-                                                       const uint8_t* __restrict__ tex, int th, int tw) {
+                                                       const uint8_t* __restrict__ tex, int th, int tw, unsigned long long* prof) {
+  ts_stamp_begin(prof, TS_K_BUCKET);
+  cudaGridDependencySynchronize();
   const int tz = blockIdx.z;    // frame of the batch = its bucket grid
   const int f = tz;
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
@@ -260,13 +276,16 @@ __global__ void __launch_bounds__(256, 6) k_bucket_depth(const uint16_t* __restr
                                       tex != nullptr, cr, cg, cb);
   append_rays_cta(fresh, (uint32_t)tz * bucket_cap, nv, ray_list, n_rays, ray_cap, ctr, err);
   if (blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) atomicAdd(&ctr->n_px, (unsigned long long)(hh * ww));
+  ts_stamp_end(prof, TS_K_BUCKET);
 }
 
 // K1b: point cloud -> buckets.  recast_pcl_to_map_kernel (dense_tsdf.py:167-185).
 __global__ void __launch_bounds__(256, 6) k_bucket_points(const float* __restrict__ xyz, int n, const __grid_constant__ TsBatch batch,
                                                         TsIntrin in, int agg_ok, TsBucket* buckets, uint4* bcol, unsigned long long* bidx,
                                                         uint32_t bucket_cap, uint32_t rec_cap, TsBucketLaunch bl, uint32_t* ray_list, int* n_rays, uint32_t ray_cap, TsCounters* ctr,
-                                                        int* err, const uint8_t* __restrict__ rgb) {
+                                                        int* err, const uint8_t* __restrict__ rgb, unsigned long long* prof) {
+  ts_stamp_begin(prof, TS_K_BUCKET);
+  cudaGridDependencySynchronize();  // as k_bucket_depth
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
   int cr = 0, cg = 0, cb = 0;
   bool valid = false;
@@ -286,6 +305,7 @@ __global__ void __launch_bounds__(256, 6) k_bucket_points(const float* __restric
                                       in.rvs, agg_ok != 0, err, rgb != nullptr, cr, cg, cb);  // :183/:185
   append_rays_cta(fresh, 0u, nv, ray_list, n_rays, ray_cap, ctr, err);
   if (t == 0) atomicAdd(&ctr->n_px, (unsigned long long)n);
+  ts_stamp_end(prof, TS_K_BUCKET);
 }
 
 // ---------------------------------------------------------------------------
@@ -325,7 +345,8 @@ __device__ __forceinline__ void win_add(unsigned int* lo, int* hi, int x) {
 __global__ void __launch_bounds__(RM_THREADS, 2) k_raymarch(const __grid_constant__ TsBatch batch, TsIntrin in, TsGrid g,
                                                               const TsBucket* buckets, const uint4* bcol, unsigned long long* bidx,
                                                               uint32_t bucket_shift, TsBucketLaunch bl, const uint32_t* __restrict__ ray_list, const int* __restrict__ n_rays_p, uint32_t ray_cap,
-                                                              TsCounters* ctr) {
+                                                              TsCounters* ctr, unsigned long long* prof) {
+  ts_stamp_begin(prof, TS_K_MARCH);
   extern __shared__ __align__(16) unsigned int win[];  // [4][4096]: A.lo, A.hi, B.lo, B.hi
   unsigned int* const w_alo = win;
   int* const w_ahi = (int*)(win + RM_WIN3);
@@ -549,6 +570,7 @@ __global__ void __launch_bounds__(RM_THREADS, 2) k_raymarch(const __grid_constan
     if (my_oob) atomicAdd(&ctr->n_oob, (unsigned long long)my_oob);
     if (my_rays) atomicAdd(&ctr->n_rays, (unsigned long long)my_rays);
   }
+  ts_stamp_end(prof, TS_K_MARCH);
 }
 
 // ---------------------------------------------------------------------------
@@ -562,7 +584,8 @@ __global__ void __launch_bounds__(RM_THREADS, 2) k_raymarch(const __grid_constan
 // maps also set the colour of every touched voxel, per thread in global memory (the colour planes are not copied).
 // ---------------------------------------------------------------------------
 // The last CTA to finish (every CTA read n_dirty at its start) sets the dirty-list count and `ticket` back to zero.
-__device__ __forceinline__ void commit_done(const TsGrid& g, int* ticket) {
+// It also stamps the end of the commit (prof).
+__device__ __forceinline__ void commit_done(const TsGrid& g, int* ticket, unsigned long long* prof) {
   __shared__ int s_last;
   __syncthreads();
   if (threadIdx.x == 0) {
@@ -570,7 +593,11 @@ __device__ __forceinline__ void commit_done(const TsGrid& g, int* ticket) {
     s_last = atomicAdd(ticket, 1) == (int)gridDim.x - 1;
   }
   __syncthreads();
-  if (s_last && threadIdx.x == 0) { *g.n_dirty = 0; *ticket = 0; }
+  if (s_last && threadIdx.x == 0) {
+    *g.n_dirty = 0;
+    *ticket = 0;
+    ts_stamp_end_thread(prof, TS_K_COMMIT);
+  }
 }
 #define CM_PLANE_BYTES (TS_B3 * 8)
 #define CM_SMEM (2 * CM_PLANE_BYTES + 16)
@@ -603,8 +630,10 @@ __device__ __forceinline__ void bulk_s2g(void* dst_gmem, const void* src_smem, u
   asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(dst_gmem), "r"(smem_u32(src_smem)), "r"(bytes) : "memory");
 }
 
-__global__ void __launch_bounds__(256) k_commit_tma(TsGrid g, int clamp, int fused_obs, unsigned long long* stamp, unsigned long long seq, int* ticket) {
+__global__ void __launch_bounds__(256) k_commit_tma(TsGrid g, int clamp, int fused_obs, unsigned long long* stamp, unsigned long long seq, int* ticket,
+                                                    unsigned long long* prof) {
   extern __shared__ __align__(128) unsigned char cm_smem[];
+  ts_stamp_begin(prof, TS_K_COMMIT);
   float2* s_acc = reinterpret_cast<float2*>(cm_smem);
   float2* s_tw = reinterpret_cast<float2*>(cm_smem + CM_PLANE_BYTES);
   unsigned long long* bar = reinterpret_cast<unsigned long long*>(cm_smem + 2 * CM_PLANE_BYTES);
@@ -669,11 +698,12 @@ __global__ void __launch_bounds__(256) k_commit_tma(TsGrid g, int clamp, int fus
     __syncthreads();
   }
   if (threadIdx.x == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-  commit_done(g, ticket);
+  commit_done(g, ticket, prof);
 }
 
 // compact the per-block dirty flags into dirty_list (warp-aggregated append)
-__global__ void __launch_bounds__(256) k_collect_dirty(TsGrid g) {
+__global__ void __launch_bounds__(256) k_collect_dirty(TsGrid g, unsigned long long* prof) {
+  ts_stamp_begin(prof, TS_K_COLLECT);
   cudaGridDependencySynchronize();  // the flags are set by the kernels before it
   const int nb = min(*g.n_blocks, g.max_blocks);
   const int stride = gridDim.x * blockDim.x;
@@ -684,6 +714,7 @@ __global__ void __launch_bounds__(256) k_collect_dirty(TsGrid g) {
     const int row = warp_append_i32(want, g.n_dirty);
     if (want) g.dirty_list[row] = b;
   }
+  ts_stamp_end(prof, TS_K_COLLECT);
 }
 __global__ void k_reset_counters(int* n_rays) { *n_rays = 0; }
 
@@ -699,27 +730,27 @@ int ts_integrate_init() {
 // ---------------------------------------------------------------------------
 // k_collect_dirty, then the commit, whose last CTA sets the dirty-list count back to zero (ticket: scratch_i[4]).  Both
 // are launched with programmatic dependent launch (ts_launch_pdl).
-int ts_collect_dirty(tslam_tsdf* m, cudaStream_t st) {
+int ts_collect_dirty(tslam_tsdf* m, cudaStream_t st, unsigned long long* prof) {
   const int gc = (m->g.max_blocks + 255) / 256 < m->sm_count * 4 ? (m->g.max_blocks + 255) / 256 : m->sm_count * 4;
-  TS_CUDA(ts_launch_pdl(k_collect_dirty, gc, 256, 0, st, m->g));
+  TS_CUDA(ts_launch_pdl(k_collect_dirty, gc, 256, 0, st, m->g, prof));
   TS_LAUNCH_CHECK(m);
   return TSLAM_OK;
 }
-int ts_launch_commit(tslam_tsdf* m, cudaStream_t st, int clamp, int fused) {
-  { int rc = ts_collect_dirty(m, st); if (rc) return rc; }
+int ts_launch_commit(tslam_tsdf* m, cudaStream_t st, int clamp, int fused, unsigned long long* prof) {
+  { int rc = ts_collect_dirty(m, st, prof); if (rc) return rc; }
   const unsigned long long seq = ++m->commit_seq;  // stamp of every block this commit writes (incremental mesh)
-  TS_CUDA(ts_launch_pdl(k_commit_tma, m->sm_count * 3, 256, CM_SMEM, st, m->g, clamp, fused, m->blk_stamp, seq, m->scratch_i + 4));
+  TS_CUDA(ts_launch_pdl(k_commit_tma, m->sm_count * 3, 256, CM_SMEM, st, m->g, clamp, fused, m->blk_stamp, seq, m->scratch_i + 4, prof));
   TS_LAUNCH_CHECK(m);
   return TSLAM_OK;
 }
 
-int ts_flush_pending(tslam_tsdf* m, cudaStream_t st) {
+int ts_flush_pending(tslam_tsdf* m, cudaStream_t st, unsigned long long* prof) {
   if (m->q_n > 0) {  // frames queued by the per-frame API
     int rc = ts_launch_queue(m, st);
     if (rc) return rc;
   }
   if (m->n_integrate_calls > 0) {  // something may be pending
-    int rc = ts_launch_commit(m, st, m->clamp_on_commit ? 1 : 0, 0);
+    int rc = ts_launch_commit(m, st, m->clamp_on_commit ? 1 : 0, 0, prof);
     if (rc) return rc;
     m->n_integrate_calls = 0;
   }
@@ -842,37 +873,41 @@ static int ts_bucket_abandon(tslam_tsdf* m, cudaStream_t st, int rc) {
 }
 
 // One integrate launch on st: the bucket kernel, the ray march of the buckets it opened, and the commit when flags
-// holds TSLAM_F_COMMIT.  launch_bucket(bl, agg_ok) enqueues k_bucket_depth or k_bucket_points, the only step that
+// holds TSLAM_F_COMMIT.  launch_bucket(bl, agg_ok, prof) enqueues k_bucket_depth or k_bucket_points, the only step that
 // differs between depth frames and point clouds; n_bucket_points is the most points one bucket can collect.
+// Nothing but kernels goes on the stream between the bucket kernel and the commit, so every boundary of the untextured
+// chain is a programmatic dependent launch.  With profiling on, the kernels stamp the launch's row of the profiling
+// ring themselves (TS_PROF_WORDS): no event record breaks the chain.
 template <class F>
 static int ts_integrate_launch(tslam_tsdf* m, cudaStream_t st, const TsBatch& batch, uint32_t bshift, uint64_t n_bucket_points, int flags,
                                F launch_bucket) {
-  cudaEvent_t* pe = m->profiling ? m->ev + TS_PROF_EV * (m->prof_launches % TS_PROF_RING) : nullptr;
-  if (pe) TS_CUDA(cudaEventRecord(pe[0], st));
+  const long long prow = m->prof_launches % TS_PROF_RING;
+  unsigned long long* prof = m->profiling ? m->prof + TS_PROF_WORDS * prow : nullptr;
   const int agg_ok = m->cfg.max_ray_length < 30.0 ? 1 : 0;  // 32-lane int32 sums: |p| <= max_ray * sqrt(1 + tan^2) < 64 m even at 60 deg half-FOV
   TsBucketLaunch bl;
   { int rcb = ts_bucket_launch(m, st, n_bucket_points, bl); if (rcb) return rcb; }
-  launch_bucket(bl, agg_ok);
+  TS_CUDA(launch_bucket(bl, agg_ok, prof));
   TS_LAUNCH_CHECK(m);
-  if (pe) TS_CUDA(cudaEventRecord(pe[1], st));
+  unsigned ran = 1u << TS_K_BUCKET;
   if (!m->g.cword) {  // untextured maps: the block-binned march (tslam_march.cu)
-    int rcm = ts_march_launch(m, st, batch, bshift, bl, pe ? pe + 4 : nullptr);  // clears n_rays itself
+    int rcm = ts_march_launch(m, st, batch, bshift, bl, prof);  // clears n_rays itself
     if (rcm) return ts_bucket_abandon(m, st, rcm);
-    if (pe) TS_CUDA(cudaEventRecord(pe[2], st));
+    ran |= (1u << TS_K_COUNT) | (1u << TS_K_CLASS_SCAN) | (1u << TS_K_SCATTER) | (1u << TS_K_MARCH);
   } else {
     k_raymarch <<<m->sm_count, RM_THREADS, RM_SMEM, st>>>(batch, m->in, m->g, m->buckets, m->bcol, m->bidx, bshift, bl, m->ray_list, m->n_rays,
-                                                         m->ray_list_cap, m->counters);
+                                                         m->ray_list_cap, m->counters, prof);
     TS_LAUNCH_CHECK(m);
-    if (pe) TS_CUDA(cudaEventRecord(pe[2], st));
     k_reset_counters<<<1, 1, 0, st>>>(m->n_rays);
     TS_LAUNCH_CHECK(m);
+    ran |= 1u << TS_K_MARCH;
   }
   m->n_integrate_calls++;
-  if (flags & TSLAM_F_COMMIT) {
-    int rc = ts_flush_pending(m, st);
+  if (flags & TSLAM_F_COMMIT) {  // commits this launch (it is pending): k_collect_dirty + k_commit_tma
+    int rc = ts_flush_pending(m, st, prof);
     if (rc) return rc;
+    ran |= (1u << TS_K_COLLECT) | (1u << TS_K_COMMIT);
   }
-  if (pe) { TS_CUDA(cudaEventRecord(pe[3], st)); m->prof_launches++; }
+  if (prof) { m->prof_ran[prow] = (unsigned char)ran; m->prof_launches++; }
   return TSLAM_OK;
 }
 
@@ -912,9 +947,9 @@ int ts_integrate_depth_impl(tslam_tsdf_t* m, const uint16_t* depth, int mem, int
       ts_set_error("frame %dx%d (sampled %dx%d) has too many partial pixel tiles for max_image_pixels=%d", h, w, hh, ww, m->cfg.max_image_pixels);
       return TSLAM_E_INVALID;
     }
-    int rc = ts_integrate_launch(m, st, batch, bshift, (uint64_t)hh * ww, flags, [&](const TsBucketLaunch& bl, int agg_ok) {
-      k_bucket_depth<<<grid1, 256, 0, st>>>(src, h * w, step, w, hh, ww, batch, m->in, agg_ok, m->buckets, m->bcol, m->bidx, m->bucket_cap, bl,
-                                            m->ray_list, m->n_rays, m->ray_list_cap, m->counters, m->g.err, tsrc, th, tw);
+    int rc = ts_integrate_launch(m, st, batch, bshift, (uint64_t)hh * ww, flags, [&](const TsBucketLaunch& bl, int agg_ok, unsigned long long* prof) {
+      return ts_launch_pdl(k_bucket_depth, grid1, 256, 0, st, (const uint16_t*)src, h * w, step, w, hh, ww, batch, m->in, agg_ok, m->buckets, m->bcol,
+                           m->bidx, m->bucket_cap, bl, m->ray_list, m->n_rays, m->ray_list_cap, m->counters, m->g.err, tsrc, th, tw, prof);
     });
     if (rc) return rc;
     if (stage0) {  // the queue must not refill buffer 0 before these kernels have read it
@@ -953,8 +988,8 @@ extern "C" int tslam_tsdf_integrate_points_rgb(tslam_tsdf_t* m, const float* xyz
   const uint32_t bshift = 31;  // every ray belongs to batch.f[0]
   const uint32_t cap_total = (uint32_t)TSLAM_MAX_BATCH * m->bucket_cap;  // power of two
   const uint32_t rec_cap = (uint32_t)n;  // a bucket's record slot is the index of the point whose thread owns its CTA sums
-  return ts_integrate_launch(m, st, batch, bshift, (uint64_t)n, flags, [&](const TsBucketLaunch& bl, int agg_ok) {
-    k_bucket_points<<<(n + 255) / 256, 256, 0, st>>>(src, n, batch, m->in, agg_ok, m->buckets, m->bcol, m->bidx, cap_total, rec_cap, bl, m->ray_list,
-                                                      m->n_rays, m->ray_list_cap, m->counters, m->g.err, csrc);
+  return ts_integrate_launch(m, st, batch, bshift, (uint64_t)n, flags, [&](const TsBucketLaunch& bl, int agg_ok, unsigned long long* prof) {
+    return ts_launch_pdl(k_bucket_points, (n + 255) / 256, 256, 0, st, src, n, batch, m->in, agg_ok, m->buckets, m->bcol, m->bidx, cap_total, rec_cap, bl,
+                         m->ray_list, m->n_rays, m->ray_list_cap, m->counters, m->g.err, csrc, prof);
   });
 }

@@ -35,7 +35,31 @@
 #define TS_ERR_RAYLIST_FULL 4
 #define TS_ERR_BUCKET_RANGE 8   // a point further than 4095 voxels from the sensor origin: beyond the bucket index's key range
 #define TS_PROF_RING 512
-#define TS_PROF_EV 8   // events per profiled integrate launch
+// Kernel stamps of a profiled integrate launch (tslam_tsdf_kernel_ms2): one row of TS_PROF_WORDS %globaltimer words per
+// launch, [2k] = entry of CTA 0 of kernel k, [2k + 1] = exit of its last CTA (atomicMax: the timer only grows, so a
+// row reused from 512 launches earlier needs no clearing).  The row travels to the kernels by value; with profiling
+// off they get a null pointer and stamp nothing.
+#define TS_PROF_WORDS 16
+enum { TS_K_BUCKET = 0, TS_K_COUNT, TS_K_CLASS_SCAN, TS_K_SCATTER, TS_K_MARCH, TS_K_COLLECT, TS_K_COMMIT, TS_K_N };
+__device__ __forceinline__ unsigned long long ts_globaltimer() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
+// at kernel entry, by every thread: CTA 0 (dispatched first) stores the start
+__device__ __forceinline__ void ts_stamp_begin(unsigned long long* prof, int k) {
+  if (prof && (blockIdx.x | blockIdx.y | blockIdx.z | threadIdx.x) == 0) prof[2 * k] = ts_globaltimer();
+}
+// by one thread of a CTA once the CTA's work is done: raises the kernel's end
+__device__ __forceinline__ void ts_stamp_end_thread(unsigned long long* prof, int k) {
+  if (prof) asm volatile("red.relaxed.gpu.global.max.u64 [%0], %1;" ::"l"(prof + 2 * k + 1), "l"(ts_globaltimer()) : "memory");
+}
+// at kernel exit, by every thread of the CTA (a barrier when profiling: the CTA's last thread is done)
+__device__ __forceinline__ void ts_stamp_end(unsigned long long* prof, int k) {
+  if (!prof) return;
+  __syncthreads();
+  if (threadIdx.x == 0) ts_stamp_end_thread(prof, k);
+}
 
 struct TsGrid {
   unsigned long long* table;  // hash words
@@ -591,8 +615,9 @@ struct tslam_tsdf {
   long long launches;
   int n_integrate_calls;
   int profiling;
-  cudaEvent_t* ev;          // profiling ring: TS_PROF_RING launches x TS_PROF_EV events (created lazily)
-  long long prof_launches;  // integrate launches recorded since profiling was switched on
+  unsigned long long* prof;  // device profiling ring: TS_PROF_RING launches x TS_PROF_WORDS kernel stamps (allocated lazily)
+  unsigned char prof_ran[TS_PROF_RING];  // per ring row: bit k = kernel k (TS_K_*) stamped that row
+  long long prof_launches;   // integrate launches recorded since profiling was switched on
   int sm_count;
   int tile_cuts_set, tile_cuts_tiles[3], tile_cuts[3][17];  // data-driven tile boundaries of a tiled global map (tslam_dist.cu)
   int* tile_hist;      // device scratch of tslam_tsdf_dirty_hist (allocated on first use)
@@ -879,9 +904,9 @@ int ts_cuda_fail(cudaError_t e, const char* what);
 // running, and must call cudaGridDependencySynchronize() before it reads anything the predecessor writes - on every
 // path, so that it never completes before the predecessor.  After an event record or a memset it is an ordinary launch.
 template <class... KArgs, class... Args>
-static cudaError_t ts_launch_pdl(void (*k)(KArgs...), int grid, int block, size_t smem, cudaStream_t st, Args&&... args) {
+static cudaError_t ts_launch_pdl(void (*k)(KArgs...), dim3 grid, int block, size_t smem, cudaStream_t st, Args&&... args) {
   cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)grid);
+  cfg.gridDim = grid;
   cfg.blockDim = dim3((unsigned)block);
   cfg.dynamicSmemBytes = smem;
   cfg.stream = st;
@@ -896,8 +921,10 @@ static cudaError_t ts_launch_pdl(void (*k)(KArgs...), int grid, int block, size_
 // shared across translation units
 // tslam_integrate.cu
 int ts_integrate_init();                                 // once per process, before the first integrate launch
-int ts_flush_pending(tslam_tsdf* m, cudaStream_t st);   // commit if anything is pending
-int ts_launch_commit(tslam_tsdf* m, cudaStream_t st, int clamp, int fused);  // k_collect_dirty + commit of the dirty blocks
+// commit if anything is pending; prof: the stamp row of the profiled integrate launch it belongs to, or null
+int ts_flush_pending(tslam_tsdf* m, cudaStream_t st, unsigned long long* prof = nullptr);
+// k_collect_dirty + commit of the dirty blocks
+int ts_launch_commit(tslam_tsdf* m, cudaStream_t st, int clamp, int fused, unsigned long long* prof = nullptr);
 int ts_check_deferred(tslam_tsdf* m);                    // read + translate device error flags (synchronises)
 int ts_check_deferred_async(tslam_tsdf* m, cudaStream_t st);  // same, after the work queued on st
 double ts_bucket_dmax(const tslam_tsdf* m);
@@ -910,7 +937,7 @@ int ts_fuse_init(tslam_tsdf* m);                         // at create: serial an
 void ts_fuse_free(tslam_tsdf* m);                        // at destroy
 void ts_map_written(tslam_tsdf* m, int submap);          // submap's planes were written (submap < 0: every submap)
 // tslam_integrate.cu: k_collect_dirty on st (dirty_flag -> dirty_list, n_dirty)
-int ts_collect_dirty(tslam_tsdf* m, cudaStream_t st);
+int ts_collect_dirty(tslam_tsdf* m, cudaStream_t st, unsigned long long* prof = nullptr);
 // tslam_register.cu: *p holds at least `need` bytes: reallocated (contents dropped) to max(need, 2 x the old size) when smaller
 int rg_reserve(void** p, size_t* bytes, size_t need);
 // tslam_queue.cu: the per-frame queue's switches, copy stream and events of a new handle / their release
@@ -923,7 +950,7 @@ int* ts_esdf_xmark(tslam_tsdf* m);
 // tslam_march.cu: block-binned ray march of the rays listed in m->ray_list (untextured maps)
 int ts_march_alloc(tslam_tsdf* m);
 void ts_march_free(tslam_tsdf* m);
-int ts_march_launch(tslam_tsdf* m, cudaStream_t st, const TsBatch& batch, uint32_t bucket_shift, const TsBucketLaunch& bl, cudaEvent_t* sub_ev);
+int ts_march_launch(tslam_tsdf* m, cudaStream_t st, const TsBatch& batch, uint32_t bucket_shift, const TsBucketLaunch& bl, unsigned long long* prof);
 
 // Octomap host helpers shared by its trackers (tslam_octo.cu)
 // the arguments every tracker call checks first: a log-odds map (`feature` names what needs one), submap in range

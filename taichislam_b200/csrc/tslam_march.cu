@@ -203,8 +203,10 @@ __device__ __forceinline__ int seg_key(int blk, int cnt, uint32_t r) {
 __global__ void __launch_bounds__(MS_THREADS, WC_MINB) k_seg_count(const __grid_constant__ TsBatch batch, TsIntrin in, TsGrid g, const TsBucket* buckets,
                                                                    unsigned long long* bidx, uint32_t bucket_shift, TsBucketLaunch bl,
                                                                    const uint32_t* __restrict__ ray_list,
-                                                                   const int* __restrict__ n_rays_p, uint32_t ray_cap, TsMarchWs w, TsCounters* ctr) {
+                                                                   const int* __restrict__ n_rays_p, uint32_t ray_cap, TsMarchWs w, TsCounters* ctr,
+                                                                   unsigned long long* prof) {
   __shared__ unsigned long long s_btab[RM_TAB];  // block coordinates -> pool index (direct mapped, rm_lookup)
+  ts_stamp_begin(prof, TS_K_COUNT);
   for (int e = threadIdx.x; e < RM_TAB; e += MS_THREADS) s_btab[e] = TS_EMPTY;
   __syncthreads();
   cudaGridDependencySynchronize();  // the ray list and its buckets come from the bucket kernel
@@ -236,7 +238,6 @@ __global__ void __launch_bounds__(MS_THREADS, WC_MINB) k_seg_count(const __grid_
     // non-finite pose: hand the rest to the exact path in bounded pieces
     while (j <= q.n) { const int c = min(q.n - j + 1, 4095); gen_append(w, g.err, r, j, c); j += c; }
   }
-  cudaTriggerProgrammaticLaunchCompletion();
   for (int o = 16; o > 0; o >>= 1) {
     my_oob += __shfl_xor_sync(FULL, my_oob, o);
     my_rays += __shfl_xor_sync(FULL, my_rays, o);
@@ -247,6 +248,10 @@ __global__ void __launch_bounds__(MS_THREADS, WC_MINB) k_seg_count(const __grid_
     if (my_rays) atomicAdd(&ctr->n_rays, (unsigned long long)my_rays);
     if (my_fmax) atomicMax(&w.ctl->fmax_bits, my_fmax);
   }
+  // after the fmax reduction: k_seg_class_scan's scan reads fmax_bits, and what a kernel writes after its trigger is
+  // not ordered before its dependent's cudaGridDependencySynchronize
+  cudaTriggerProgrammaticLaunchCompletion();
+  ts_stamp_end(prof, TS_K_COUNT);
 }
 
 // K2b-2: scattering walk.  The same generator over the same stored records, so the same binned segments in the same
@@ -258,8 +263,9 @@ __global__ void __launch_bounds__(MS_THREADS, WC_MINB) k_seg_count(const __grid_
 // (pool exhausted) was dropped by the counting walk: its segments are dropped here too.  When the launch overflowed
 // (k_seg_class_scan), every binned segment takes the generic path.
 __global__ void __launch_bounds__(MS_THREADS, WS_MINB) k_seg_scatter(const __grid_constant__ TsBatch batch, TsGrid g, const int* __restrict__ n_rays_p,
-                                                                     uint32_t ray_cap, TsMarchWs w, TsCounters* ctr) {
+                                                                     uint32_t ray_cap, TsMarchWs w, TsCounters* ctr, unsigned long long* prof) {
   __shared__ unsigned long long s_btab[RM_TAB];  // block coordinates -> pool index (direct mapped, rm_find)
+  ts_stamp_begin(prof, TS_K_SCATTER);
   for (int e = threadIdx.x; e < RM_TAB; e += MS_THREADS) s_btab[e] = TS_EMPTY;
   __syncthreads();
   cudaGridDependencySynchronize();  // the runs and the overflow flag come from k_seg_class_scan
@@ -306,6 +312,7 @@ __global__ void __launch_bounds__(MS_THREADS, WS_MINB) k_seg_scatter(const __gri
   cudaTriggerProgrammaticLaunchCompletion();
   for (int o = 16; o > 0; o >>= 1) my_guard += __shfl_xor_sync(FULL, my_guard, o);
   if (lane == 0 && my_guard) atomicAdd(&ctr->n_seg_guard, (unsigned long long)my_guard);
+  ts_stamp_end(prof, TS_K_SCATTER);
 }
 
 // ---------------------------------------------------------------------------
@@ -328,14 +335,23 @@ __device__ __forceinline__ int item_bin(uint32_t cnt, uint32_t cost, uint32_t q,
   return min(SC_BINS - 1, (int)(est * (1.0f / 4096.0f)));
 }
 // run by the last CTA alone; the class stage's list (touched, blk_total, blk_cost, n_touched) was written by other CTAs,
-// so it is read through L2 (__ldcg)
+// so it is read through L2 (__ldcg), once: pass A keeps the first SC_THREADS entries (a few hundred on the bench's map)
+// and their run offsets in shared memory, where the histogram and pass B find them without a dependent L2 round trip
+// per 32 entries.
 __device__ __forceinline__ void seg_scan(const TsMarchWs& w, TsCounters* ctr) {
   __shared__ uint32_t s_a[32];
   __shared__ uint32_t s_run;
   __shared__ unsigned int s_hist[SC_BINS], s_base[SC_BINS];
   __shared__ int s_ovf;
+  __shared__ int s_tblk[SC_THREADS];
+  __shared__ uint32_t s_tcnt[SC_THREADS], s_tcost[SC_THREADS], s_toff[SC_THREADS];
   const int nt = __ldcg(&w.ctl->n_touched);
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  // entry i of the touched list: block, segments, cost, run offset
+  auto entry = [&](int i, int& blk, uint32_t& cnt, uint32_t& cost, uint32_t& off) {
+    if (i < SC_THREADS) { blk = s_tblk[i]; cnt = s_tcnt[i]; cost = s_tcost[i]; off = s_toff[i]; }
+    else { blk = __ldcg(&w.touched[i]); cnt = __ldcg(&w.blk_total[i]); cost = __ldcg(&w.blk_cost[i]); off = __ldcg(&w.seg_off[blk]); }
+  };
   if (threadIdx.x == 0) s_run = 0;
   if (threadIdx.x < SC_BINS) s_hist[threadIdx.x] = 0u;
   __syncthreads();
@@ -343,8 +359,8 @@ __device__ __forceinline__ void seg_scan(const TsMarchWs& w, TsCounters* ctr) {
   for (int base = 0; base < nt; base += SC_THREADS) {
     const int i = base + threadIdx.x;
     int blk = -1;
-    uint32_t cnt = 0;
-    if (i < nt) { blk = __ldcg(&w.touched[i]); cnt = __ldcg(&w.blk_total[i]); }
+    uint32_t cnt = 0, cost = 0;
+    if (i < nt) { blk = __ldcg(&w.touched[i]); cnt = __ldcg(&w.blk_total[i]); cost = __ldcg(&w.blk_cost[i]); }
     uint32_t a = cnt;  // inclusive warp scan
     for (int o = 1; o < 32; o <<= 1) {
       const uint32_t ta = __shfl_up_sync(FULL, a, o);
@@ -361,13 +377,19 @@ __device__ __forceinline__ void seg_scan(const TsMarchWs& w, TsCounters* ctr) {
       s_a[lane] = ta;  // inclusive over warps
     }
     __syncthreads();
-    if (i < nt) w.seg_off[blk] = s_run + (wid ? s_a[wid - 1] : 0u) + a - cnt;
+    if (i < nt) {
+      const uint32_t off = s_run + (wid ? s_a[wid - 1] : 0u) + a - cnt;
+      w.seg_off[blk] = off;
+      if (i < SC_THREADS) { s_tblk[i] = blk; s_tcnt[i] = cnt; s_tcost[i] = cost; s_toff[i] = off; }
+    }
     __syncthreads();
     if (threadIdx.x == 0) s_run += s_a[31];
     __syncthreads();
   }
   for (int i = wid; i < nt; i += 32) {  // one warp per block, one lane per chunk: the busiest blocks have dozens of chunks
-    const uint32_t cnt = __ldcg(&w.blk_total[i]), cost = __ldcg(&w.blk_cost[i]);
+    int blk;
+    uint32_t cnt, cost, off;
+    entry(i, blk, cnt, cost, off);
     const uint32_t nq = (cnt + MR_CHUNK - 1) / MR_CHUNK;
     for (uint32_t q = lane; q < nq; q += 32) atomicAdd(&s_hist[item_bin(cnt, cost, q, nq)], 1u);
   }
@@ -398,8 +420,9 @@ __device__ __forceinline__ void seg_scan(const TsMarchWs& w, TsCounters* ctr) {
   if (s_ovf) return;
   // pass B: the items, longest bin first
   for (int i = wid; i < nt; i += 32) {
-    const int blk = __ldcg(&w.touched[i]);
-    const uint32_t cnt = __ldcg(&w.blk_total[i]), cost = __ldcg(&w.blk_cost[i]), ex_seg = w.seg_off[blk];
+    int blk;
+    uint32_t cnt, cost, ex_seg;
+    entry(i, blk, cnt, cost, ex_seg);
     const uint32_t nq = (cnt + MR_CHUNK - 1) / MR_CHUNK;
     for (uint32_t q = lane; q < nq; q += 32) {
       const int b = item_bin(cnt, cost, q, nq);
@@ -408,7 +431,8 @@ __device__ __forceinline__ void seg_scan(const TsMarchWs& w, TsCounters* ctr) {
     }
   }
 }
-__global__ void __launch_bounds__(SC_THREADS, 1) k_seg_class_scan(TsGrid g, TsMarchWs w, TsCounters* ctr) {
+__global__ void __launch_bounds__(SC_THREADS, 1) k_seg_class_scan(TsGrid g, TsMarchWs w, TsCounters* ctr, unsigned long long* prof) {
+  ts_stamp_begin(prof, TS_K_CLASS_SCAN);
   cudaGridDependencySynchronize();  // seg_count and the dirty flags come from k_seg_count
   const int nb = min(*g.n_blocks, g.max_blocks);
   const uint32_t lane = threadIdx.x & 31u;
@@ -452,6 +476,7 @@ __global__ void __launch_bounds__(SC_THREADS, 1) k_seg_class_scan(TsGrid g, TsMa
   if (!s_last) return;
   __threadfence();
   seg_scan(w, ctr);
+  ts_stamp_end(prof, TS_K_CLASS_SCAN);  // the last CTA ends the kernel
 }
 
 // ---------------------------------------------------------------------------
@@ -502,7 +527,8 @@ __device__ __forceinline__ double mb_sum(unsigned int lo, int hi) {
 
 template <bool VERIFY, int MB_THREADS, int MB_MINB>
 __global__ void __launch_bounds__(MB_THREADS, MB_MINB) k_march_blocks(const __grid_constant__ TsBatch batch, TsIntrin in, TsGrid g, TsMarchWs w,
-                                                                 TsCounters* ctr, int* n_rays) {
+                                                                 TsCounters* ctr, int* n_rays, unsigned long long* prof) {
+  ts_stamp_begin(prof, TS_K_MARCH);
   extern __shared__ __align__(16) unsigned int mb_smem[];
   unsigned int* const a_lo = mb_smem;
   int* const a_hi = (int*)(mb_smem + MB_WORDS);
@@ -691,7 +717,10 @@ __global__ void __launch_bounds__(MB_THREADS, MB_MINB) k_march_blocks(const __gr
       }
     }
   }
-  cudaTriggerProgrammaticLaunchCompletion();
+  // No early trigger (cudaTriggerProgrammaticLaunchCompletion) in this kernel: what its tail writes - seg_count back to
+  // zero, the cleared control block and ray count - is read by the next launch's bucket kernel and counting walk, which
+  // reach this grid through a chain of programmatic launches (k_collect_dirty, k_commit_tma, k_bucket_depth), and a
+  // write after a trigger is not ordered before the dependent's cudaGridDependencySynchronize.
   // fill counters back to zero.  k_seg_scatter counted every run down to 0 unless the launch overflowed; a count left
   // above 0 is a slot of a run that no segment filled (n_seg_guard, must stay 0)
   unsigned int my_left = 0;
@@ -747,7 +776,10 @@ __global__ void __launch_bounds__(MB_THREADS, MB_MINB) k_march_blocks(const __gr
   // of the launch
   if (s_last) {
     if (threadIdx.x < sizeof(TsMarchCtl) / 4) reinterpret_cast<int*>(w.ctl)[threadIdx.x] = 0;
-    if (threadIdx.x == 0) *n_rays = 0;
+    if (threadIdx.x == 0) {
+      *n_rays = 0;
+      ts_stamp_end_thread(prof, TS_K_MARCH);
+    }
   }
 }
 
@@ -802,27 +834,24 @@ void ts_march_free(tslam_tsdf* m) {
   cudaFree(w.blk_total); cudaFree(w.blk_cost); cudaFree(w.items); cudaFree(w.gen); cudaFree(w.ctl);
 }
 
-// sub_ev (profiling, may be null): 2 events recorded after counting walk + class + scan and after the scattering walk;
-// the caller's events before and after this call close the first and the last part.  The kernels after the first are
-// launched with programmatic dependent launch: each waits (cudaGridDependencySynchronize) only where it first reads its
-// predecessor's output, so its launch and prologue overlap the predecessor's tail.
-int ts_march_launch(tslam_tsdf* m, cudaStream_t st, const TsBatch& batch, uint32_t bucket_shift, const TsBucketLaunch& bl, cudaEvent_t* sub_ev) {
+// prof (profiling, may be null): the launch's row of kernel stamps.  Every kernel is launched with programmatic dependent
+// launch: each waits (cudaGridDependencySynchronize) only where it first reads its predecessor's output, so its launch
+// and prologue overlap the predecessor's tail.
+int ts_march_launch(tslam_tsdf* m, cudaStream_t st, const TsBatch& batch, uint32_t bucket_shift, const TsBucketLaunch& bl, unsigned long long* prof) {
   if (!m->mw.rays) { int rca = ts_march_alloc(m); if (rca) return rca; }  // the workspace, at the first launch that needs it
   const int sms = m->sm_count;
   TS_CUDA(ts_launch_pdl(k_seg_count, sms * WC_MINB, MS_THREADS, 0, st, batch, m->in, m->g, (const TsBucket*)m->buckets, m->bidx, bucket_shift, bl,
-                        (const uint32_t*)m->ray_list, (const int*)m->n_rays, (uint32_t)m->ray_list_cap, m->mw, m->counters));
+                        (const uint32_t*)m->ray_list, (const int*)m->n_rays, (uint32_t)m->ray_list_cap, m->mw, m->counters, prof));
   TS_LAUNCH_CHECK(m);
   const int nsc = (m->g.max_blocks + SC_THREADS - 1) / SC_THREADS;
-  TS_CUDA(ts_launch_pdl(k_seg_class_scan, nsc < sms ? nsc : sms, SC_THREADS, 0, st, m->g, m->mw, m->counters));
+  TS_CUDA(ts_launch_pdl(k_seg_class_scan, nsc < sms ? nsc : sms, SC_THREADS, 0, st, m->g, m->mw, m->counters, prof));
   TS_LAUNCH_CHECK(m);
-  if (sub_ev) TS_CUDA(cudaEventRecord(sub_ev[0], st));
   TS_CUDA(ts_launch_pdl(k_seg_scatter, sms * WS_MINB, MS_THREADS, 0, st, batch, m->g, (const int*)m->n_rays, (uint32_t)m->ray_list_cap, m->mw,
-                        m->counters));
+                        m->counters, prof));
   TS_LAUNCH_CHECK(m);
-  if (sub_ev) TS_CUDA(cudaEventRecord(sub_ev[1], st));
   const int grid = (sms - m->rm_reserve) * 3;
-  if (m->march_verify) TS_CUDA(ts_launch_pdl(k_march_blocks<true, 320, 3>, grid, 320, MB_SMEM, st, batch, m->in, m->g, m->mw, m->counters, m->n_rays));
-  else TS_CUDA(ts_launch_pdl(k_march_blocks<false, 320, 3>, grid, 320, MB_SMEM, st, batch, m->in, m->g, m->mw, m->counters, m->n_rays));
+  if (m->march_verify) TS_CUDA(ts_launch_pdl(k_march_blocks<true, 320, 3>, grid, 320, MB_SMEM, st, batch, m->in, m->g, m->mw, m->counters, m->n_rays, prof));
+  else TS_CUDA(ts_launch_pdl(k_march_blocks<false, 320, 3>, grid, 320, MB_SMEM, st, batch, m->in, m->g, m->mw, m->counters, m->n_rays, prof));
   TS_LAUNCH_CHECK(m);
   return TSLAM_OK;
 }

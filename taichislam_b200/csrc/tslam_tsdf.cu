@@ -278,7 +278,7 @@ extern "C" int tslam_tsdf_destroy(tslam_tsdf_t* m) {
   ts_fuse_free(m);
   if (m->mw.rays) ts_march_free(m);
   cudaFree(m->counters); cudaFree(m->pose_R); cudaFree(m->pose_T); cudaFree(m->colormap);
-  if (m->ev) { for (int i = 0; i < TS_PROF_EV * TS_PROF_RING; i++) cudaEventDestroy(m->ev[i]); delete[] m->ev; }
+  if (m->prof) cudaFree(m->prof);
   delete m;
   return TSLAM_OK;
 }
@@ -676,36 +676,59 @@ extern "C" int64_t tslam_tsdf_launch_count(tslam_tsdf_t* m) { return m ? m->laun
 
 extern "C" int tslam_tsdf_set_profiling(tslam_tsdf_t* m, int on) {
   if (!m) return TSLAM_E_INVALID;
-  if (on && !m->ev) {
-    m->ev = new cudaEvent_t[TS_PROF_EV * TS_PROF_RING];
-    for (int i = 0; i < TS_PROF_EV * TS_PROF_RING; i++) TS_CUDA(cudaEventCreate(&m->ev[i]));
+  if (on && !m->prof) {
+    TS_CUDA(cudaMalloc(&m->prof, (size_t)TS_PROF_RING * TS_PROF_WORDS * 8));
+    TS_CUDA(cudaMemset(m->prof, 0, (size_t)TS_PROF_RING * TS_PROF_WORDS * 8));
   }
   m->profiling = on;
   m->prof_launches = 0;
   return TSLAM_OK;
 }
-// ms3[3*i + {0,1,2}] = bucket / ray-march / commit(+reset) kernel time of the i-th most recent
-// recorded integrate launch, i < n (n <= TS_PROF_RING).  Returns the number of rows written in *n_out.
-// ms7[7*i + ...] = bucket, ray march (all of its kernels), commit, then the parts of the ray march: the interval between
-// the bucket kernel and the first march kernel (0: nothing runs there), set-up + segment count + class + scan, segment
-// fill, march (with the generic path and the resets).  The last four are 0 for textured maps (k_raymarch).
+// ms3[3*i + {0,1,2}] = bucket / ray-march / commit kernel time of the i-th most recent recorded integrate launch,
+// i < n (n <= TS_PROF_RING).  Returns the number of rows written in *n_out.
+// ms7[7*i + ...] = bucket, ray march (all of its kernels), commit (k_collect_dirty + k_commit_tma; 0 without one), then
+// the parts of the ray march: 0 (kept for the ABI: nothing is charged between the bucket kernel and the march),
+// set-up + segment count + class + scan, scattering walk, march (with the generic path and the resets).  The last
+// three are 0 for textured maps (k_raymarch).
+// Times come from the kernels' %globaltimer stamps (TS_PROF_WORDS).  Under programmatic dependent launch a kernel can
+// start before its predecessor ends, so one rule charges every column: a stage runs from the LATER of its first kernel's
+// start and the end of the stage before it, to its last kernel's end.  The stages of a launch are disjoint intervals:
+// the columns never sum to more than the launch's span, and the gaps between stages are charged to none.
 // Both write `cols` columns per row (3 or 7), walking the profiling ring backwards from the last recorded launch.
 static int ts_kernel_ms(tslam_tsdf* m, int32_t n, int cols, float* ms, int32_t* n_out) {
-  if (!m || !ms || !n_out || !m->ev) return TSLAM_E_INVALID;
+  if (!m || !ms || !n_out || !m->prof) return TSLAM_E_INVALID;
   TS_CUDA(cudaDeviceSynchronize());
+  static_assert(2 * TS_K_N <= TS_PROF_WORDS, "stamp row");
+  unsigned long long* ring = new unsigned long long[(size_t)TS_PROF_RING * TS_PROF_WORDS];
+  const cudaError_t e = cudaMemcpy(ring, m->prof, (size_t)TS_PROF_RING * TS_PROF_WORDS * 8, cudaMemcpyDeviceToHost);
+  if (e != cudaSuccess) { delete[] ring; return ts_cuda_fail(e, "cudaMemcpy(profiling ring)"); }
   long long have = m->prof_launches < TS_PROF_RING ? m->prof_launches : TS_PROF_RING;
   if (n > have) n = (int32_t)have;
   for (int i = 0; i < n; i++) {
-    cudaEvent_t* pe = m->ev + TS_PROF_EV * ((m->prof_launches - 1 - i) % TS_PROF_RING);
-    float* row = ms + cols * i;
-    for (int q = 0; q < 3; q++) TS_CUDA(cudaEventElapsedTime(&row[q], pe[q], pe[q + 1]));
-    for (int q = 3; q < cols; q++) row[q] = 0.0f;
-    if (cols == 7 && !m->g.cword) {  // pe[4], pe[5]: after the scan and after the scattering walk (ts_march_launch)
-      TS_CUDA(cudaEventElapsedTime(&row[4], pe[1], pe[4]));
-      TS_CUDA(cudaEventElapsedTime(&row[5], pe[4], pe[5]));
-      TS_CUDA(cudaEventElapsedTime(&row[6], pe[5], pe[2]));
+    const long long r = (m->prof_launches - 1 - i) % TS_PROF_RING;
+    const unsigned long long* s = ring + TS_PROF_WORDS * r;
+    const unsigned ran = m->prof_ran[r];
+    // stage [first, last] kernel, charged after `prev_end`; returns the stage's end (prev_end when it did not run)
+    auto stage = [&](int first, int last, unsigned long long prev_end, float& out) {
+      out = 0.0f;
+      if (!(ran & (1u << last))) return prev_end;
+      const unsigned long long b = std::max(s[2 * first], prev_end), en = s[2 * last + 1];
+      out = en > b ? (float)((double)(en - b) * 1e-6) : 0.0f;
+      return en;
+    };
+    float c[7] = {0, 0, 0, 0, 0, 0, 0};
+    const unsigned long long e0 = stage(TS_K_BUCKET, TS_K_BUCKET, 0ull, c[0]);
+    const bool binned = (ran & (1u << TS_K_COUNT)) != 0;
+    const unsigned long long e1 = stage(binned ? TS_K_COUNT : TS_K_MARCH, TS_K_MARCH, e0, c[1]);
+    stage(TS_K_COLLECT, TS_K_COMMIT, e1, c[2]);
+    if (binned) {
+      const unsigned long long e2 = stage(TS_K_COUNT, TS_K_CLASS_SCAN, e0, c[4]);
+      const unsigned long long e3 = stage(TS_K_SCATTER, TS_K_SCATTER, e2, c[5]);
+      stage(TS_K_MARCH, TS_K_MARCH, e3, c[6]);
     }
+    for (int q = 0; q < cols; q++) ms[cols * i + q] = c[q];
   }
+  delete[] ring;
   *n_out = n;
   return TSLAM_OK;
 }

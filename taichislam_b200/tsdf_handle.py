@@ -497,7 +497,9 @@ class TsdfHandle:
         return o[:k.value]
 
     def kernel_ms2(self, n=512):
-        """[rows,7] ms: bucket, ray march (total), commit, then ray set-up+segment count, scan, segment fill, block march."""
+        """[rows,7] ms: bucket, ray march (total), commit, 0, then ray set-up + counting walk + class + scan, scattering
+        walk, block march - from the kernels' own timer stamps, each stage charged from the end of the one before it
+        (DESIGN.md section 5)."""
         o = np.zeros((n, 7), np.float32)
         k = C.c_int32(0)
         capi.check(self.L.tslam_tsdf_kernel_ms2(self.h, n, capi.np_ptr(o), C.byref(k)))

@@ -2,16 +2,19 @@
 """Kernel chain of one integrate launch, from torch.profiler (CUPTI): where the launch's time goes between kernels.
 
 Runs the device-resident arm of bench.py - a 512^3 map, the S2 stream, 64-frame depth launches with commit, the same
-three warm-up steps of 16 launches and the same per-launch profiling events (kernel_ms2) - then traces a few launches
+three warm-up steps of 16 launches and profiling on as bench.py sets it (kernel_ms2) - then traces a few launches
 in a run of their own.  Writes OUT/trace.json (Chrome trace) and OUT/summary.json, and prints the summary:
 
   kernels          per kernel name: launches, mean and total duration (us)
   gaps             idle time between consecutive kernels of a launch (k_bucket_depth opens a launch), per kernel pair
+                   (mean, median, min, max; negative where a programmatic dependent launch starts before its predecessor ends)
   bookkeeping      kernels that do no voxel work (class/scan, generic march, resets, dirty-list compaction)
   share            (bookkeeping kernel time + all gaps inside the launches) / launch span, and each part alone
 
 The card's name and power limit are read in the same run.
-Usage: python tools/trace_integrate.py [--out DIR] [--launches K] [--no-events]"""
+The first --skip traced launches (default 1) are left out of the statistics: the first launch after the synchronise
+waits on the host, which enqueues it under the profiler for the first time.
+Usage: python tools/trace_integrate.py [--out DIR] [--launches K] [--skip S] [--no-events]"""
 import argparse
 import json
 import os
@@ -41,8 +44,9 @@ def main():
     ap.add_argument("--out", default=os.path.join(tempfile.gettempdir(), "trace_integrate"),
                     help="output directory (default: trace_integrate under the system temporary directory)")
     ap.add_argument("--launches", type=int, default=8)
+    ap.add_argument("--skip", type=int, default=1, help="traced launches left out of the statistics at the start")
     ap.add_argument("--warmup", type=int, default=3, help="warm-up steps of 16 launches (bench.py's default)")
-    ap.add_argument("--no-events", action="store_true", help="trace without the per-launch profiling events bench.py records")
+    ap.add_argument("--no-events", action="store_true", help="trace with profiling off (bench.py times its launches with it on)")
     args = ap.parse_args()
 
     import torch
@@ -57,7 +61,7 @@ def main():
     for b in range(POOL_BATCHES):
         d, _, _ = bench.make_inputs(BATCH, b * BATCH)
         pool.append(torch.from_numpy(np.ascontiguousarray(d).view(np.int16)).cuda())
-    n_launches = args.warmup * LAUNCHES_PER_STEP + args.launches
+    n_launches = args.warmup * LAUNCHES_PER_STEP + args.skip + args.launches
     Rs, Ts = syn.stream_poses(n_launches * BATCH, start=0)
     Rs = np.ascontiguousarray(Rs.astype(np.float32).reshape(n_launches, BATCH, 9))
     Ts = np.ascontiguousarray(Ts.astype(np.float32).reshape(n_launches, BATCH, 3))
@@ -73,11 +77,11 @@ def main():
     l0 = g.launch_count()
     torch.cuda.synchronize()
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        for _ in range(args.launches):
+        for _ in range(args.skip + args.launches):
             launch(k)
             k += 1
         torch.cuda.synchronize()
-    kernels_per_launch = (g.launch_count() - l0) / args.launches
+    kernels_per_launch = (g.launch_count() - l0) / (args.skip + args.launches)
     os.makedirs(args.out, exist_ok=True)
     trace_path = os.path.join(args.out, "trace.json")
     prof.export_chrome_trace(trace_path)
@@ -96,6 +100,7 @@ def main():
             launches.append(cur)
         if cur is not None:
             cur.append(s)
+    launches = launches[args.skip:]
     per_kernel, gaps = {}, {}
     spans, book_us, gap_us, between = [], [], [], []
     for i, L in enumerate(launches):
@@ -121,7 +126,8 @@ def main():
         "kernels_per_launch": kernels_per_launch,
         "launch_chain": [s[0] for s in launches[0]] if launches else [],
         "kernels_us": {k_: {"n": len(v), "mean": float(np.mean(v)), "total": float(np.sum(v))} for k_, v in per_kernel.items()},
-        "gaps_us": {k_: {"mean": float(np.mean(v)), "min": float(np.min(v)), "max": float(np.max(v))} for k_, v in gaps.items()},
+        "gaps_us": {k_: {"mean": float(np.mean(v)), "median": float(np.median(v)), "min": float(np.min(v)), "max": float(np.max(v))}
+                    for k_, v in gaps.items()},
         "launch_span_us": span,
         "bookkeeping_kernels_us": float(np.mean(book_us)) if book_us else None,
         "gaps_inside_launch_us": float(np.mean(gap_us)) if gap_us else None,

@@ -748,6 +748,63 @@ int tslam_tsdf_track_points(tslam_tsdf_t* m, const float* xyz, int mem, int32_t 
                             double* H_out, double* b_out, double* cost2, int64_t* info5, void* stream);
 
 /* ----------------------------------------------------------------------------
+ * Place recognition between TSDF submaps (DESIGN.md section 7, "Loop detection"): a descriptor per submap that ignores
+ * yaw, and a batched search that shortlists, per query, database entries with a coarse 4-DoF pose (Scan Context, Kim &
+ * Kim 2018, adapted to TSDF submaps).  The caller verifies a candidate with tslam_tsdf_register started from that pose.
+ *   frames     M9 (HOST f32 [n,9] row-major, finite) is the levelled rotation M_s = L R_s of entry s, rounded to f32 once
+ *              by the caller: R_s the submap's f64 base rotation (identity for a global map), L the minimal f64 rotation
+ *              taking the world unit vector `up` to +z.  A point is x = M_s p_v in f32, pose_apply's operation order with
+ *              a zero translation (((M0 px + M1 py) + M2 pz) + 0 per row); horizontal (x0, x1), height x2.
+ *   points     the registration points of tslam_tsdf_register: voxels of non-ghost blocks with obs = 1, W > 0,
+ *              W >= min_weight, |TSDF| <= band; p_v = (f32(i) vs, f32(j) vs, f32(k) vs).
+ *   rings      rho2 = x0 x0 + x1 x1 (f32); ring = the first i with rho2 < B_i, B_i = f32((f64(r_max) (i + 1) / 20)^2);
+ *              points with rho2 >= B_19 are left out of the polar grid.
+ *   sectors    f_k = c_k x1 - s_k x0 (f32, in that order), (c_k, s_k) = f32(cos, sin(2 pi k / 60)), k mod 60; the
+ *              sector is the first k in [0, 60) with f_k >= 0 and f_{k+1} < 0, or 0 when there is none (rho2 = 0).
+ *   sc         f32 [n, 20 x 60] (DEVICE), row = ring: zmax - zmin (f32) of the bin's heights, 0 for an empty bin.
+ *   ring       f32 [n, 20] (DEVICE): f32(non-empty bins of ring i) / 60.
+ *   bev        u32 [n, 512] (DEVICE): the 128 x 128 bird's-eye bitmap, cell size c = f32(r_max) / 64, u = floor(x0 / c) +
+ *              64, v = floor(x1 / c) + 64 (f32 division; points outside [0, 128) left out); bit v % 32 of word 4 u + v / 32
+ *              is set iff the cell's zmax - zmin >= h_min (vertical structure, not floor).
+ *   n_points   int64 [n] (HOST): the entry's registration points.
+ * Every output is an exact function of the points (min and max commute): the same bits whatever the atomics' order.
+ * Refused (TSLAM_E_INVALID, nothing written) before the handle is looked at: n outside [1, 1024], a NULL array or
+ * params, r_max, h_min or band not finite or not > 0, min_weight not finite, a non-finite M9; then a NULL handle or a
+ * submap out of range.  A submap may appear twice.  Flushes the queued frames first, synchronises once, and writes no map
+ * word, flag, ESDF, mesh state or statistic other than the kernel-launch counter.  Scratch: tslam_tsdf_register's. */
+typedef struct {
+  float r_max;       /* radius of the polar grid, half the bitmap's side (m) */
+  float h_min;       /* least height span of a set bitmap cell (m) */
+  float band;        /* registration points: |TSDF| <= band */
+  float min_weight;  /* registration points: W >= min_weight */
+} tslam_place_params_t;
+int tslam_tsdf_place_describe(tslam_tsdf_t* m, int32_t n, const int32_t* submaps, const float* M9, const tslam_place_params_t* params,
+                              float* sc, float* ring, uint32_t* bev, int64_t* n_points, void* stream);
+
+/* Matching of queries against a database of n_db descriptors (DEVICE sc, ring, bev as above; n_points, ids int64 [n_db]
+ * DEVICE).  No handle: descriptors can be kept across calls.  queries (HOST int32 [n_q]) are database indices.
+ *   eligible   d != q, |ids[q] - ids[d]| >= min_gap, n_points of both >= min_points.
+ *   shortlist  ring distance sum_i (k_qi - k_di)^2 in f32, i ascending; the top_k eligible entries by (distance, index).
+ *   yaw        for m in [0, 60): columns j where |sc_q[:, j]| and |sc_d[:, (j + m) % 60]| are both non-zero (norm sqrtf of
+ *              the f32 sum of squares in ring order); cos_j = dot / (|a| |b|) (dot in ring order); D(m) = 1 - (sum_j
+ *              cos_j, j ascending) / f32(n_j), 1 when n_j = 0; m* = argmin, ties to the smaller m.  x_d ~ Rz(6 m* deg) x_q.
+ *   offset     yaws psi_y = (2 m* + y - 1) x 3 deg, y = 0, 1, 2 (f32 cos, sin of 2 pi h / 120).  q's bitmap is rotated by
+ *              inverse mapping: cell (u, v) takes (a, b) = (f32(u - 64) + 0.5, f32(v - 64) + 0.5), (a', b') = (c a + s b,
+ *              c b - s a) in f32, source cell (floor(a') + 64, floor(b') + 64), 0 outside.  score(dx, dy) = popc of rot
+ *              q shifted by (dx, dy) cells AND d, dx, dy in [-32, 32].  Best: the largest score, ties to the smaller |dx| +
+ *              |dy|, then the smaller y, then dy, then dx.  overlap = f32(score) / f32(min(popc(rot q), popc(d))), 0 when
+ *              that is 0.  Then x_d ~ Rz(psi) x_q + (dx c, dy c).
+ * Outputs (DEVICE), row qi top_k + slot: info6 int32 [.,6] (match index or -1 past the eligible entries, m*, y, dx, dy,
+ * score), dist3 f32 [.,3] (ring distance, D(m*), overlap); an unmatched row is (-1, 0, 0, 0, 0, 0), (0, 1, 0).  A query's
+ * rows do not depend on the other queries.  Refused (TSLAM_E_INVALID, nothing written): n_db or n_q outside [1, 1024],
+ * top_k outside [1, TSLAM_PLACE_MAX_TOP_K], min_gap < 0, a NULL array, a query outside [0, n_db).  Runs asynchronously on
+ * `stream` (stream-ordered scratch of about 40 B per row). */
+#define TSLAM_PLACE_MAX_TOP_K 32
+int tslam_place_match(int32_t n_db, const float* sc, const float* ring, const uint32_t* bev, const int64_t* n_points, const int64_t* ids,
+                      int32_t n_q, const int32_t* queries, int32_t top_k, int64_t min_gap, int64_t min_points, int32_t* info6,
+                      float* dist3, void* stream);
+
+/* ----------------------------------------------------------------------------
  * Rendering of the TSDF's zero level (DESIGN.md section 7, "Rendering"): depth, normal and colour images of n pinhole
  * cameras, ray-cast to the surface that registration and frame tracking align to (KinectFusion's model image).
  *   cameras    1 <= n <= TSLAM_RENDER_MAX_CAMERAS, one pinhole K4 = (fx, fy, cx, cy) (HOST f64, rounded to f32 once) and

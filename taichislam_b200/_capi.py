@@ -196,11 +196,18 @@ SIGNATURES = {
                                          _vp, _vp, _vp]),
     "tslam_tsdf_track_points": (C.c_int, [_vp, _vp, C.c_int, _i32, _i32, _vp, _vp, _f32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp,
                                           _vp]),
+    "tslam_tsdf_place_describe": (C.c_int, [_vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "tslam_place_match": (C.c_int, [_i32, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _i32, _i64, _i64, _vp, _vp, _vp]),
     "tslam_tsdf_fuse_update": (C.c_int, [_vp, _vp, _vp, _f32, _i32, _vp, _vp]),
     "tslam_tsdf_render": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _f32, _f32, _f32, _vp, _vp, _vp, _vp, _vp]),
     "tslam_esdf_trajectory": (C.c_int, [_vp, _i32, _i32, _vp, _vp, C.POINTER(TrajParams), _vp, _vp, _vp, _vp]),
     "tslam_octo_esdf_trajectory": (C.c_int, [_vp, _i32, _i32, _vp, _vp, C.POINTER(TrajParams), _vp, _vp, _vp, _vp]),
 }
+
+class PlaceParams(C.Structure):
+    """tslam_place_params_t"""
+    _fields_ = [("r_max", _f32), ("h_min", _f32), ("band", _f32), ("min_weight", _f32)]
+
 
 _lib = None
 

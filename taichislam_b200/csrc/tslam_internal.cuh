@@ -16,6 +16,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <utility>
+#include <vector>
 #include "../../include/tslam.h"
 
 #define TS_B 16
@@ -940,6 +941,15 @@ void ts_map_written(tslam_tsdf* m, int submap);          // submap's planes were
 int ts_collect_dirty(tslam_tsdf* m, cudaStream_t st, unsigned long long* prof = nullptr);
 // tslam_register.cu: *p holds at least `need` bytes: reallocated (contents dropped) to max(need, 2 x the old size) when smaller
 int rg_reserve(void** p, size_t* bytes, size_t need);
+// tslam_register.cu: the registration point selection (k_rg_count, sort, k_rg_permute, scan, then k_rg_fill) that
+// tslam_tsdf_register and tslam_tsdf_place_describe share; the block arrays it leaves in A->reg_blk
+struct RgSel {
+  int nb;                                 // pool blocks scanned
+  const int* order; const int* cs; const int* off;  // blocks sorted by slot, their counts and exclusive scan
+};
+int rg_select_count(tslam_tsdf* A, const std::vector<int>& slot_of, int U, float band, float min_weight, RgSel& sel,
+                    std::vector<int>& slot_cnt, cudaStream_t st);
+int rg_select_fill(tslam_tsdf* A, const RgSel& sel, float band, float min_weight, float4* pts, cudaStream_t st);
 // tslam_queue.cu: the per-frame queue's switches, copy stream and events of a new handle / their release
 int ts_queue_init(tslam_tsdf* m);
 void ts_queue_free(tslam_tsdf* m);

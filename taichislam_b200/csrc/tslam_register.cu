@@ -391,6 +391,65 @@ static int rg_lm(tslam_tsdf_t* A, const TsGrid& g, const float4* pts, void* scra
   return TSLAM_OK;
 }
 
+// Point selection (shared by tslam_tsdf_register and tslam_tsdf_place_describe): the registration points of the submaps
+// s with slot_of[s] >= 0 (slots 0 .. U-1), in slot order, then pool order, then voxel order.  rg_select_count counts them
+// per block and per slot (k_rg_count), sorts the blocks by slot and scans their counts, and returns the per-slot counts
+// (synchronises); the block arrays live in A->reg_blk.  rg_select_fill writes the records (k_rg_fill) to pts, which
+// holds at least the total.
+int rg_select_count(tslam_tsdf_t* A, const std::vector<int>& slot_of, int U, float band, float min_weight, RgSel& sel,
+                    std::vector<int>& slot_cnt, cudaStream_t st) {
+  const int ms = (int)slot_of.size();
+  int nb = 0;
+  TS_CUDA(cudaMemcpyAsync(&nb, A->g.n_blocks, 4, cudaMemcpyDeviceToHost, st));
+  TS_CUDA(cudaStreamSynchronize(st));
+  if (nb > A->g.max_blocks) nb = A->g.max_blocks;
+  int end_bit = 1;
+  while ((1 << end_bit) <= U) end_bit++;
+  size_t sort_tmp = 0, scan_tmp = 0;
+  TS_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, sort_tmp, (int*)nullptr, (int*)nullptr, (int*)nullptr, (int*)nullptr, nb, 0, end_bit, st));
+  TS_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, scan_tmp, (int*)nullptr, (int*)nullptr, nb + 1, st));
+  const size_t nbs = rg_align((size_t)(nb + 1) * 4), mss = rg_align((size_t)ms * 4);
+  const size_t tmp_bytes = rg_align(sort_tmp > scan_tmp ? sort_tmp : scan_tmp);
+  int rc = rg_reserve(&A->reg_blk, &A->reg_blk_bytes, 7 * nbs + 2 * mss + tmp_bytes);
+  if (rc) return rc;
+  char* w = (char*)A->reg_blk;
+  int* cnt = (int*)w; w += nbs;
+  int* key = (int*)w; w += nbs;
+  int* val = (int*)w; w += nbs;
+  int* key_s = (int*)w; w += nbs;
+  int* val_s = (int*)w; w += nbs;
+  int* cs = (int*)w; w += nbs;
+  int* off = (int*)w; w += nbs;
+  int* d_slot_of = (int*)w; w += mss;
+  int* d_slot_cnt = (int*)w; w += mss;
+  void* tmp = w;
+  TS_CUDA(cudaMemcpyAsync(d_slot_of, slot_of.data(), (size_t)ms * 4, cudaMemcpyHostToDevice, st));
+  TS_CUDA(cudaMemsetAsync(d_slot_cnt, 0, (size_t)U * 4, st));
+  slot_cnt.assign(U, 0);
+  if (nb > 0) {
+    const float bw = band, mw = min_weight;
+    k_rg_count<<<A->sm_count * 4, 256, 0, st>>>(A->g, nb, d_slot_of, U, bw, mw, cnt, key, val, d_slot_cnt);
+    TS_LAUNCH_CHECK(A);
+    TS_CUDA(cub::DeviceRadixSort::SortPairs(tmp, sort_tmp, key, key_s, val, val_s, nb, 0, end_bit, st));
+    k_rg_permute<<<oc_grid(nb + 1, 256, A->sm_count * 8), 256, 0, st>>>(nb, cnt, val_s, cs);
+    TS_LAUNCH_CHECK(A);
+    TS_CUDA(cub::DeviceScan::ExclusiveSum(tmp, scan_tmp, cs, off, nb + 1, st));
+    TS_CUDA(cudaMemcpyAsync(slot_cnt.data(), d_slot_cnt, (size_t)U * 4, cudaMemcpyDeviceToHost, st));
+    TS_CUDA(cudaStreamSynchronize(st));
+  }
+  sel.nb = nb;
+  sel.order = val_s;
+  sel.cs = cs;
+  sel.off = off;
+  return TSLAM_OK;
+}
+
+int rg_select_fill(tslam_tsdf_t* A, const RgSel& sel, float band, float min_weight, float4* pts, cudaStream_t st) {
+  k_rg_fill<<<A->sm_count * 4, 256, 0, st>>>(A->g, sel.nb, sel.order, sel.cs, sel.off, band, min_weight, A->in.vs, pts);
+  TS_LAUNCH_CHECK(A);
+  return TSLAM_OK;
+}
+
 extern "C" int tslam_tsdf_register(tslam_tsdf_t* A, tslam_tsdf_t* B, int32_t n_pairs, const int32_t* ref_submaps,
                                    const int32_t* read_submaps, const double* R0, const double* T0, float band, float min_weight,
                                    float huber, int32_t max_iters, int32_t min_points, double* R_out, double* T_out, double* H_out,
@@ -441,44 +500,10 @@ extern "C" int tslam_tsdf_register(tslam_tsdf_t* A, tslam_tsdf_t* B, int32_t n_p
     pair_slot[p] = sl;
   }
   const int U = (int)slot_sub.size();
-  int nb = 0;
-  TS_CUDA(cudaMemcpyAsync(&nb, A->g.n_blocks, 4, cudaMemcpyDeviceToHost, st));
-  TS_CUDA(cudaStreamSynchronize(st));
-  if (nb > A->g.max_blocks) nb = A->g.max_blocks;
-  int end_bit = 1;
-  while ((1 << end_bit) <= U) end_bit++;
-  size_t sort_tmp = 0, scan_tmp = 0;
-  TS_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, sort_tmp, (int*)nullptr, (int*)nullptr, (int*)nullptr, (int*)nullptr, nb, 0, end_bit, st));
-  TS_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, scan_tmp, (int*)nullptr, (int*)nullptr, nb + 1, st));
-  const size_t nbs = rg_align((size_t)(nb + 1) * 4), mss = rg_align((size_t)ms * 4);
-  const size_t tmp_bytes = rg_align(sort_tmp > scan_tmp ? sort_tmp : scan_tmp);
-  rc = rg_reserve(&A->reg_blk, &A->reg_blk_bytes, 7 * nbs + 2 * mss + tmp_bytes);
+  RgSel sel;
+  std::vector<int> slot_cnt;
+  rc = rg_select_count(A, slot_of, U, band, min_weight, sel, slot_cnt, st);
   if (rc) return rc;
-  char* w = (char*)A->reg_blk;
-  int* cnt = (int*)w; w += nbs;
-  int* key = (int*)w; w += nbs;
-  int* val = (int*)w; w += nbs;
-  int* key_s = (int*)w; w += nbs;
-  int* val_s = (int*)w; w += nbs;
-  int* cs = (int*)w; w += nbs;
-  int* off = (int*)w; w += nbs;
-  int* d_slot_of = (int*)w; w += mss;
-  int* d_slot_cnt = (int*)w; w += mss;
-  void* tmp = w;
-  TS_CUDA(cudaMemcpyAsync(d_slot_of, slot_of.data(), (size_t)ms * 4, cudaMemcpyHostToDevice, st));
-  TS_CUDA(cudaMemsetAsync(d_slot_cnt, 0, (size_t)U * 4, st));
-  std::vector<int> slot_cnt(U, 0);
-  if (nb > 0) {
-    const float bw = band, mw = min_weight;
-    k_rg_count<<<A->sm_count * 4, 256, 0, st>>>(A->g, nb, d_slot_of, U, bw, mw, cnt, key, val, d_slot_cnt);
-    TS_LAUNCH_CHECK(A);
-    TS_CUDA(cub::DeviceRadixSort::SortPairs(tmp, sort_tmp, key, key_s, val, val_s, nb, 0, end_bit, st));
-    k_rg_permute<<<oc_grid(nb + 1, 256, A->sm_count * 8), 256, 0, st>>>(nb, cnt, val_s, cs);
-    TS_LAUNCH_CHECK(A);
-    TS_CUDA(cub::DeviceScan::ExclusiveSum(tmp, scan_tmp, cs, off, nb + 1, st));
-    TS_CUDA(cudaMemcpyAsync(slot_cnt.data(), d_slot_cnt, (size_t)U * 4, cudaMemcpyDeviceToHost, st));
-    TS_CUDA(cudaStreamSynchronize(st));
-  }
   std::vector<long long> slot_p0(U + 1, 0);
   for (int u = 0; u < U; u++) slot_p0[u + 1] = slot_p0[u] + slot_cnt[u];
   const long long n_pts = slot_p0[U];
@@ -492,8 +517,8 @@ extern "C" int tslam_tsdf_register(tslam_tsdf_t* A, tslam_tsdf_t* B, int32_t n_p
   if (rc) return rc;
   float4* pts = (float4*)A->reg_pts;
   if (n_pts > 0) {
-    k_rg_fill<<<A->sm_count * 4, 256, 0, st>>>(A->g, nb, val_s, cs, off, band, min_weight, vs, pts);
-    TS_LAUNCH_CHECK(A);
+    rc = rg_select_fill(A, sel, band, min_weight, pts, st);
+    if (rc) return rc;
   }
   return rg_lm(A, B->g, pts, (char*)A->reg_pts + pts_b, n_pairs, p0.data(), np.data(), read_submaps, R0, T0, vs, huber, max_iters,
                min_points, R_out, T_out, H_out, b_out, cost2, info5, st);

@@ -427,6 +427,87 @@ class DenseTSDF(BaseMap):
         keys = ("R", "T", "H", "b", "cost_init", "cost", "n_points", "n_valid", "iterations", "converged", "status")
         return [{k: (out[k][p].copy() if out[k].ndim > 1 else out[k][p].item()) for k in keys} for p in range(len(a))]
 
+    # ------------------------------------------------------------------ loop detection (DESIGN.md section 7)
+    LOOP_DEFAULTS = dict(r_max=8.0, h_min=0.3, band=None, min_weight=0.0, top_k=8, min_gap=1, min_points=200, max_sc_dist=0.35,
+                         min_overlap=0.3, min_inlier_ratio=0.5, max_cost=None, huber=None, max_iters=100)
+
+    def describe_places(self, submaps, up=None, r_max=8.0, h_min=0.3, band=None, min_weight=0.0, base_poses=None):
+        """Place descriptors of `submaps` on the GPU (tslam_tsdf_place_describe): each submap's registration points,
+        levelled by M_s = L R_s (L takes `up`, default +z, to +z; R_s the f64 base rotation), binned into a 20 x 60
+        polar grid of height spans, a ring key and a 128 x 128 bird's-eye bitmap of cells whose span is >= h_min.
+        band defaults to 4 voxels.  base_poses: submap -> world (R, T) to use instead of the stored base poses (a
+        collection whose poses are kept elsewhere).  Flushes the queued frames.  -> dict: sc, ring, bev (torch CUDA
+        tensors), n_points (numpy), M (f64 [n,3,3], the levelled rotations)."""
+        from .. import place
+        sm = [int(s) for s in np.asarray(submaps).reshape(-1)]
+        L = place.level((0.0, 0.0, 1.0) if up is None else up)
+        pose = self.base_pose if base_poses is None else (lambda s: base_poses[s])
+        M = np.stack([L @ np.asarray(pose(s)[0], np.float64) for s in sm]) if sm else np.zeros((0, 3, 3))
+        self._flush()
+        band = 4.0 * self.voxel_scale if band is None else band
+        out = self._h.place_describe(sm, M, r_max, h_min, band, min_weight)
+        out["M"] = M
+        return out
+
+    def detect_loops(self, query_submaps, database_submaps=None, up=None, base_poses=None, **opts):
+        """Find loop closures between the query submaps and the database on the GPU: describe every submap
+        (describe_places), shortlist and coarsely align each query against the database (place.match: ring keys, the
+        best yaw of the polar descriptor, the bird's-eye offset), then verify each candidate with D <= max_sc_dist and
+        overlap >= min_overlap by registering it from the coarse pose (register_submaps, query = reference).  The
+        database defaults to every submap up to the active one, queries included (a query never matches itself;
+        entries need min_points points and submap ids at least min_gap apart).  opts: LOOP_DEFAULTS; max_cost defaults
+        to (0.5 voxel)^2 / 2, the mean Huber cost of a half-voxel residual, huber and band to register_submaps'.
+        base_poses: as describe_places.
+        Returns one dict per verified candidate: query, match (submap ids), R, T (query local -> match local), H, b,
+        sc_distance, yaw_deg, dx, dy, overlap, n_points, n_valid, cost (final, summed), converged, accepted (status 0,
+        converged, n_valid >= min_points, n_valid / n_points >= min_inlier_ratio, cost / n_valid <= max_cost).  Moves
+        nothing: the constraints are for the caller's pose graph."""
+        from .. import place
+        o = dict(self.LOOP_DEFAULTS)
+        unknown = set(opts) - set(o)
+        if unknown:
+            raise TypeError(f"detect_loops: unknown options {sorted(unknown)}")
+        o.update(opts)
+        vs = self.voxel_scale
+        max_cost = 0.5 * (0.5 * vs) ** 2 if o["max_cost"] is None else o["max_cost"]
+        queries = [int(s) for s in np.asarray(query_submaps).reshape(-1)]
+        if database_submaps is None:
+            last = 0 if self.is_global_map else int(self.active_submap_id[None])
+            database_submaps = range(0, max([last] + queries) + 1)
+        entries = sorted(set(int(s) for s in database_submaps) | set(queries))
+        at = {s: i for i, s in enumerate(entries)}
+        desc = self.describe_places(entries, up=up, r_max=o["r_max"], h_min=o["h_min"], band=o["band"], min_weight=o["min_weight"],
+                                    base_poses=base_poses)
+        mt = place.match(desc["sc"], desc["ring"], desc["bev"], desc["n_points"], np.array(entries, np.int64), [at[q] for q in queries],
+                         top_k=o["top_k"], min_gap=o["min_gap"], min_points=o["min_points"])
+        cand = []
+        for qi, q in enumerate(queries):
+            if desc["n_points"][at[q]] < o["min_points"]:
+                continue
+            for k in range(o["top_k"]):
+                d = int(mt["match"][qi, k])
+                if d < 0 or not (mt["sc_dist"][qi, k] <= o["max_sc_dist"] and mt["overlap"][qi, k] >= o["min_overlap"]):
+                    continue
+                R0, T0 = place.coarse_pose(desc["M"][at[q]], desc["M"][d], mt["yaw_deg"][qi, k], mt["dx"][qi, k], mt["dy"][qi, k],
+                                           o["r_max"])
+                cand.append((q, entries[d], qi, k, R0, T0))
+        out = []
+        for c0 in range(0, len(cand), 1024):
+            batch = cand[c0:c0 + 1024]
+            res = self.register_submaps([c[0] for c in batch], [c[1] for c in batch],
+                                        poses=(np.stack([c[4] for c in batch]), np.stack([c[5] for c in batch])), band=o["band"],
+                                        min_weight=o["min_weight"], huber=o["huber"], max_iters=o["max_iters"],
+                                        min_points=o["min_points"])
+            for (q, d, qi, k, _, _), r in zip(batch, res):
+                nv, npt = int(r["n_valid"]), int(r["n_points"])
+                ok = (r["status"] == 0 and bool(r["converged"]) and nv >= o["min_points"] and npt > 0 and nv / npt >= o["min_inlier_ratio"]
+                      and r["cost"] / max(nv, 1) <= max_cost)
+                out.append(dict(query=q, match=d, R=r["R"], T=r["T"], H=r["H"], b=r["b"], sc_distance=float(mt["sc_dist"][qi, k]),
+                                yaw_deg=float(mt["yaw_deg"][qi, k]), dx=int(mt["dx"][qi, k]), dy=int(mt["dy"][qi, k]),
+                                overlap=float(mt["overlap"][qi, k]), n_points=npt, n_valid=nv, cost=float(r["cost"]),
+                                converged=bool(r["converged"]), accepted=bool(ok)))
+        return out
+
     def track_depth(self, R, T, depthmap, step=None, huber=None, max_iters=20, min_points=100):
         """Track one depth frame (uint16 mm [h,w]) against the TSDF of the active submap (submap 0 of a global map) on the
         GPU (tslam_tsdf_track_depth, DESIGN.md section 7, "Frame tracking"), before it is integrated: the pose at which

@@ -139,6 +139,31 @@ class SubmapMapping:
             self.set_frame_poses({frame_id: (res["world_R"], res["world_T"])})
         return res
 
+    def detect_loops(self, frame_id=None, **opts):
+        """Find loop closures for the submap created on `frame_id` (default: the newest submap) among the other submaps
+        with DenseTSDF.detect_loops, describing every submap at its current world pose (the global map's base poses).
+        Applies nothing: the caller's pose graph decides.  Returns the accepted constraints keyed by (frame_id,
+        matched frame_id): the detect_loops dict (R, T: query-local -> match-local, H, b, ...) plus "world_R" /
+        "world_T", the query submap's world pose that the constraint implies (base_match * T).  opts: up and
+        DenseTSDF.LOOP_DEFAULTS."""
+        assert self.submap_type is DenseTSDF, "loop detection needs TSDF submaps"
+        if not self.submaps:
+            return {}
+        frame_of = {s: f for f, s in self.submaps.items()}
+        if frame_id is None:
+            frame_id = frame_of[max(frame_of)]
+        g = self.global_map
+        poses = {s: (g.submaps_base_R_np[s], g.submaps_base_T_np[s]) for s in frame_of}
+        found = self.submap_collection.detect_loops([self.submaps[frame_id]], sorted(frame_of), base_poses=poses, **opts)
+        out = {}
+        for c in found:
+            if not c["accepted"]:
+                continue
+            Rb, Tb = (np.asarray(a, np.float64) for a in poses[c["match"]])
+            c["world_R"], c["world_T"] = Rb @ c["R"], Rb @ c["T"] + Tb
+            out[(frame_id, frame_of[c["match"]])] = c
+        return out
+
     def convert_by_pgo(self, frame_id, R, T):  # :162-169
         self.ego_motion_poses[frame_id] = (R, T)
         if self.last_frame_id is None:

@@ -397,6 +397,26 @@ class TsdfHandle:
                                               capi.stream_ptr()))
         return self._solver_out(P, R, T, H, b, cost2, info)
 
+    # -- place descriptors for loop detection (tslam_tsdf_place_describe) --------------------------------------------
+    def place_describe(self, submaps, M, r_max, h_min, band, min_weight=0.0):
+        """Place descriptors of `submaps` (DESIGN.md section 7, "Loop detection"): M [n,3,3] the levelled rotations (f64,
+        rounded to f32 here).  -> dict: sc f32 [n,20,60], ring f32 [n,20], bev int32 [n,512] (the uint32 words' bits)
+        as torch CUDA tensors, n_points int64 [n] numpy."""
+        torch = self.torch
+        sm = np.ascontiguousarray(np.asarray(submaps, dtype=np.int32).reshape(-1))
+        n = sm.shape[0]
+        M9 = np.ascontiguousarray(np.asarray(M, dtype=np.float64).reshape(n, 9).astype(np.float32))
+        params = capi.PlaceParams(float(r_max), float(h_min), float(band), float(min_weight))
+        dev = torch.device("cuda", torch.cuda.current_device())
+        rows = max(n, 1)
+        sc = torch.empty((rows, 20, 60), dtype=torch.float32, device=dev)
+        ring = torch.empty((rows, 20), dtype=torch.float32, device=dev)
+        bev = torch.empty((rows, 512), dtype=torch.int32, device=dev)
+        npts = np.zeros(rows, np.int64)
+        capi.check(self.L.tslam_tsdf_place_describe(self.h, n, capi.np_ptr(sm), capi.np_ptr(M9), C.byref(params), capi.tptr(sc),
+                                                    capi.tptr(ring), capi.tptr(bev), capi.np_ptr(npts), capi.stream_ptr()))
+        return dict(sc=sc[:n], ring=ring[:n], bev=bev[:n], n_points=npts[:n])
+
     @staticmethod
     def _solver_out(P, R, T, H, b, cost2, info):
         return dict(R=R.reshape(P, 3, 3), T=T, H=H.reshape(P, 6, 6), b=b, cost_init=cost2[:, 0], cost=cost2[:, 1],

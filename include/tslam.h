@@ -334,6 +334,46 @@ int tslam_esdf_halo_pack(tslam_tsdf_t* m, const int32_t* tiles3, int32_t rank, i
 int tslam_esdf_ghost_unpack(tslam_tsdf_t* m, int64_t n, const int64_t* keys, const float* esdf, void* stream);
 int tslam_esdf_tiled_relax(tslam_tsdf_t* m, int32_t* n_sweeps_out, void* stream);
 int tslam_esdf_tiled_end(tslam_tsdf_t* m);
+/* Incremental fusion of a tiled global map (DESIGN.md section 6, "Incremental tiled fusion"): tslam_tsdf_fuse_update
+ * over the ranks.  Rank r's `src` holds the submaps r contributes; every rank's dst has the pose table of all of them.
+ * Terms, quantisation, skip rule, int64 sums and readout are tslam_tsdf_fuse_update's.  The sums of a dst block live
+ * on its owner only (tile_owner with the current cuts); the other ranks send the integer deltas of the blocks their
+ * added, moved or removed submaps touch.  Integer sums commute, so after an update the union of the ranks' owned
+ * blocks is bit for bit tslam_tsdf_fuse_update of all ranks' submaps into one map, for any world size, cuts and
+ * history.  The host layer (TiledGlobalMap.update_fused_submaps) calls, on every rank:
+ *   _plan     the single-map plan of this rank's submaps.  plan3 (HOST int64[3]) = local full-update reason (as
+ *             tslam_tsdf_fuse_update's stats8[0], without 6; plus 7 = tile cuts changed since the last update, 8 = the
+ *             sums are not valid, e.g. after a failed update), cost and cost_full (source blocks an incremental and a
+ *             full update would splat); present (HOST u8[max_submaps]) = src holds blocks of the submap.  Synchronises.
+ *   merge     over the ranks: a submap present on two ranks is refused; include must be the same everywhere; the
+ *             update is full when any rank's reason is, or when the summed cost exceeds the summed cost_full (6); the
+ *             reason is the smallest non-zero one.
+ *   _splat    with the merged reason: a full update resets dst, zeroes the sums and adds every included submap; an
+ *             incremental one subtracts and adds as planned, removals also activating their FOREIGN dst blocks (a
+ *             removal that misses an owned block raises TSLAM_E_CUDA at the commit).  Synchronises.
+ *   (full update with balanced cuts: tslam_tsdf_dirty_hist of the activated blocks, summed, new cuts installed)
+ *   tslam_tsdf_foreign_count, then _pack: the sum rows of the foreign dirty blocks into rows int64[cap, 1 + planes *
+ *             4096] (DEVICE; key, then planes S_wT, S_w, count * 2^32 + S_occ and, textured, S_c[3]) grouped by owner;
+ *             they are zeroed here.  An incremental update refuses cuts that changed since _plan.  Synchronises.
+ *   exchange (all-to-all of the rows), then
+ *   _unpack   n received rows: activate their blocks (TSLAM_E_POOL_FULL when the pool runs out), add them into the
+ *             sums with wrapping int64 adds, read the touched owned blocks out of the sums (stamped for
+ *             tslam_mesh_update, ESDF-dirty).  A voxel whose count decodes as negative: TSLAM_E_CUDA.  Synchronises.
+ *   _finish   ok != 0 on every rank when every rank's phases succeeded: record the submaps' new state; stats8 as
+ *             tslam_tsdf_fuse_update's (this rank's part).  ok = 0: nothing recorded, and when the update got past its
+ *             plan the sums are invalid (the next update is full on every rank).
+ * A halo exchange and a tiled ESDF between two updates do not force a full update; any other write of dst does.  A
+ * removal or move makes the next ESDF update full.  Refused (TSLAM_E_INVALID) before the handles are looked at: tolerance
+ * not finite or < 0, a NULL handle or plan buffer, dst == src, tiles3 NULL or not a factorisation of world (1..24, at
+ * most 16 per axis), rank outside [0, world); then what tslam_tsdf_fuse_update refuses except a tiled dst, and a phase
+ * called out of order or with another src than the plan. */
+int tslam_tsdf_fuse_update_tiled_plan(tslam_tsdf_t* dst, tslam_tsdf_t* src, const int32_t* tiles3, int32_t rank, int32_t world,
+                                      const uint8_t* include, float tolerance, int32_t full, int64_t* plan3, uint8_t* present, void* stream);
+int tslam_tsdf_fuse_update_tiled_splat(tslam_tsdf_t* dst, tslam_tsdf_t* src, int32_t reason, void* stream);
+int tslam_tsdf_fuse_update_tiled_pack(tslam_tsdf_t* dst, const int32_t* tiles3, int32_t rank, int32_t world, const int32_t* counts,
+                                      int64_t cap, int64_t* rows, void* stream);
+int tslam_tsdf_fuse_update_tiled_unpack(tslam_tsdf_t* dst, int64_t n, const int64_t* rows, void* stream);
+int tslam_tsdf_fuse_update_tiled_finish(tslam_tsdf_t* dst, tslam_tsdf_t* src, int32_t ok, int64_t* stats8, void* stream);
 
 /* ----------------------------------------------------------------------------
  * Marching cubes  (MarchingCubeMesher, marching_cube_mesher.py)

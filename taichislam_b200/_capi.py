@@ -22,6 +22,7 @@ RENDER_MAX_SAMPLES = 65536
 ABI_VERSION = 6
 FUSE_REASONS = ("incremental", "first call", "full requested", "other source", "destination written", "content changed",
                 "cheaper than subtract and re-add")
+TILED_FUSE_REASONS = FUSE_REASONS + ("tile cuts changed", "sums not valid")  # tslam_tsdf_fuse_update_tiled_*
 
 
 class TslamError(RuntimeError):
@@ -199,6 +200,11 @@ SIGNATURES = {
     "tslam_tsdf_place_describe": (C.c_int, [_vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "tslam_place_match": (C.c_int, [_i32, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _i32, _i64, _i64, _vp, _vp, _vp]),
     "tslam_tsdf_fuse_update": (C.c_int, [_vp, _vp, _vp, _f32, _i32, _vp, _vp]),
+    "tslam_tsdf_fuse_update_tiled_plan": (C.c_int, [_vp, _vp, _vp, _i32, _i32, _vp, _f32, _i32, _vp, _vp, _vp]),
+    "tslam_tsdf_fuse_update_tiled_splat": (C.c_int, [_vp, _vp, _i32, _vp]),
+    "tslam_tsdf_fuse_update_tiled_pack": (C.c_int, [_vp, _vp, _i32, _i32, _vp, _i64, _vp, _vp]),
+    "tslam_tsdf_fuse_update_tiled_unpack": (C.c_int, [_vp, _i64, _vp, _vp]),
+    "tslam_tsdf_fuse_update_tiled_finish": (C.c_int, [_vp, _vp, _i32, _vp, _vp]),
     "tslam_tsdf_render": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _f32, _f32, _f32, _vp, _vp, _vp, _vp, _vp]),
     "tslam_esdf_trajectory": (C.c_int, [_vp, _i32, _i32, _vp, _vp, C.POINTER(TrajParams), _vp, _vp, _vp, _vp]),
     "tslam_octo_esdf_trajectory": (C.c_int, [_vp, _i32, _i32, _vp, _vp, C.POINTER(TrajParams), _vp, _vp, _vp, _vp]),

@@ -12,26 +12,10 @@
 #include <cstring>
 #include "tslam_internal.cuh"
 
-#define TS_MAX_TILES_AXIS 16
-struct TsTiling {
-  int tiles[3];
-  int rank, world;
-  int cuts[3][TS_MAX_TILES_AXIS + 1];  // tile k of axis a owns block coordinates [cuts[a][k], cuts[a][k+1])
-};
-
-__host__ __device__ __forceinline__ int tile_coord(const TsTiling& t, int axis, int b) {
-  int c = 0;
-  while (c + 1 < t.tiles[axis] && b >= t.cuts[axis][c + 1]) ++c;  // (blocks outside the cut range belong to the end tiles)
-  return c;
-}
-__host__ __device__ __forceinline__ int tile_owner(const TsTiling& t, int bx, int by, int bz) {
-  return (tile_coord(t, 0, bx) * t.tiles[1] + tile_coord(t, 1, by)) * t.tiles[2] + tile_coord(t, 2, bz);
-}
-
-// Tile boundaries: the cuts set by tslam_tiling_set_cuts when they match `tiles3` (data-driven: the host layer puts
-// them at the quantiles of the occupied blocks' marginal histograms, so a flat flight volume does not leave half the
-// ranks empty), else equal slices of the volume.
-static int fill_tiling(tslam_tsdf* m, const int32_t* tiles3, int rank, int world, TsTiling* t) {
+// Tile boundaries (TsTiling, tile_owner: tslam_internal.cuh): the cuts set by tslam_tiling_set_cuts when they match
+// `tiles3` (data-driven: the host layer puts them at the quantiles of the occupied blocks' marginal histograms, so a
+// flat flight volume does not leave half the ranks empty), else equal slices of the volume.
+int fill_tiling(tslam_tsdf* m, const int32_t* tiles3, int rank, int world, TsTiling* t) {
   if (!tiles3 || tiles3[0] < 1 || tiles3[1] < 1 || tiles3[2] < 1 || tiles3[0] * tiles3[1] * tiles3[2] != world || rank < 0 || rank >= world ||
       tiles3[0] > TS_MAX_TILES_AXIS || tiles3[1] > TS_MAX_TILES_AXIS || tiles3[2] > TS_MAX_TILES_AXIS) {
     ts_set_error("bad tiling: %d x %d x %d tiles for world size %d", tiles3 ? tiles3[0] : -1, tiles3 ? tiles3[1] : -1, tiles3 ? tiles3[2] : -1, world);
@@ -568,6 +552,7 @@ extern "C" int tslam_tsdf_ghost_unpack2(tslam_tsdf_t* m, int64_t n, const int64_
   if (n == 0) return TSLAM_OK;
   cudaStream_t st = (cudaStream_t)stream;
   ts_map_written(m, -1);
+  m->ghost_gen++;
   m->esdf_full_needed = 1;
   const unsigned long long seq = ++m->commit_seq;  // the imported ghosts are stamped like committed blocks (incremental mesh)
   k_ghost_unpack<<<(int)(n < m->sm_count * 4 ? n : m->sm_count * 4), 256, 0, st>>>(m->g, n, (const long long*)keys, (const float2*)tw, obs, (const float4*)col,

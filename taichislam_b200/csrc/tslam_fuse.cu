@@ -24,6 +24,11 @@
 // submaps with work (k_fz_list), activates the dst blocks the additions need (k_fz_splat<0>), grows the sum planes
 // to the pool blocks in use, splats (k_fz_splat<1>: removals at the old pose, additions at the new one) and reads the
 // touched blocks out of the sums (k_fz_commit), stamping them for the incremental mesh and the ESDF.
+//
+// Tiled global maps (tslam_tsdf_fuse_update_tiled_*, DESIGN.md section 6) run the same plan, splat and commit per rank:
+// the sums of a block live on its owner, the other ranks pack the sum rows of their foreign blocks (k_fz_pack) and the
+// owner adds them (k_fz_unpack_add).  The terms are the same multiset per voxel, so the bounds above carry over and the
+// union of the tiles is bit for bit the single map's.
 #include <cmath>
 #include <cstring>
 #include <vector>
@@ -34,7 +39,10 @@
 #define TS_ERR_FUSE_MISSING 16      // g.err: a removal found no dst block (the sums and the pool disagree)
 
 // full-update reasons (stats8[0]; 0 = incremental)
-enum { FZ_INCR = 0, FZ_FIRST = 1, FZ_ASKED = 2, FZ_OTHER_SRC = 3, FZ_DST_WRITTEN = 4, FZ_CONTENT = 5, FZ_COST = 6 };
+// 7, 8: tiled updates only (tslam_tsdf_fuse_update_tiled_*)
+enum { FZ_INCR = 0, FZ_FIRST = 1, FZ_ASKED = 2, FZ_OTHER_SRC = 3, FZ_DST_WRITTEN = 4, FZ_CONTENT = 5, FZ_COST = 6, FZ_CUTS = 7,
+       FZ_INVALID = 8 };
+enum { FZ_NONE = 0, FZ_ADD, FZ_REMOVE, FZ_MOVE, FZ_KEEP };  // what an update does with a submap
 
 struct FzJob {        // one placement of one submap: sign +1 adds, -1 removes
   float R[9], T[3];
@@ -53,7 +61,8 @@ struct FzDev {        // device scratch of one update (TsFuse::dev)
   int2* job_of;       // [max_submaps] (removal job, addition job), -1 none
   FzJob* jobs;        // [2 * max_submaps]
   int* list;          // [src max_blocks] source blocks with work
-  unsigned long long* ctr;  // [0] list length, [1] voxels splatted, [2] voxels skipped, [3] dst ghost blocks, [4] dirty blocks
+  unsigned long long* ctr;  // [0] list length, [1] voxels splatted, [2] voxels skipped, [3] dst ghost blocks, [4] dirty blocks,
+                            // [5] voxels whose count decodes as negative (tiled updates)
 };
 
 struct FzSub {        // what a submap contributes to dst (TsFuse::sub)
@@ -62,15 +71,32 @@ struct FzSub {        // what a submap contributes to dst (TsFuse::sub)
   unsigned long long ver;  // src content version at that time
   int nblk;           // its non-ghost source blocks then
 };
+struct FzPlan {        // one update, from its plan to its record
+  int reason;         // FZ_*
+  bool full;
+  std::vector<unsigned char> want, act;  // per submap: included with source blocks; FZ_NONE .. FZ_KEEP
+  std::vector<int> nblk;
+  std::vector<float> rad, pR, pT;        // radius, dst pose table
+  long long n_add, n_move, n_remove, n_tol, cost, cost_full;  // cost: source blocks an incremental update splats
+  unsigned long long ghosts;             // dst ghost blocks
+};
 struct TsFuse {
   int valid;          // the sums describe dst (cleared by a failed update)
-  unsigned long long src_serial, gen;  // src handle and dst write generation of the last update
+  unsigned long long src_serial, gen;  // src handle and dst write generation of the last update (tiled: write_gen - ghost_gen)
   std::vector<FzSub> sub;
   void* sums;         // sum planes (grown geometrically, never shrunk)
   size_t cap_blocks;
   void* dev;          // FzDev arrays
   size_t dev_bytes;
   int dev_submaps, dev_blocks;
+  // tiled updates (tslam_tsdf_fuse_update_tiled_*)
+  int ever_valid;     // the sums were valid once: invalid sums read "sums not valid", not "first call"
+  int tiled;          // the last update was tiled, with this tiling (world 0 for a single-map update)
+  TsTiling tiling;
+  int phase;          // of the update in progress: 0 none, 1 planned, 2 splatted, 3 packed, 4 unpacked
+  FzPlan plan;        // its plan (phase >= 1), source handle and the tiling it packs with
+  unsigned long long plan_src;
+  TsTiling plan_tiling;
 };
 
 static unsigned long long g_serial = 0;  // handle numbers (create is not called concurrently with itself here)
@@ -78,6 +104,7 @@ static unsigned long long g_serial = 0;  // handle numbers (create is not called
 int ts_fuse_init(tslam_tsdf* m) {
   m->serial = __atomic_add_fetch(&g_serial, 1ull, __ATOMIC_RELAXED);
   m->write_gen = 0;
+  m->ghost_gen = 0;
   m->content_ver = new unsigned long long[m->cfg.max_submaps]();
   m->fz = nullptr;
   return TSLAM_OK;
@@ -150,8 +177,14 @@ __device__ __forceinline__ long long fz_q(float x) { return __double2ll_rn((doub
 
 // One CTA per listed source block.  PASS 0 activates the dst blocks of the additions; PASS 1 adds each job's signed
 // terms into the sum planes (removals find their blocks, or raise TS_ERR_FUSE_MISSING) and flags the blocks it touched.
+// the block of cell (ci, cj, ck) lies in a foreign tile (not inlined: inlined, the cut search costs k_fz_splat<0> spills)
+__device__ __noinline__ bool fz_foreign(const TsTiling* tl, int ci, int cj, int ck) {
+  return tile_owner(*tl, ci >> TS_BSHIFT, cj >> TS_BSHIFT, ck >> TS_BSHIFT) != tl->rank;
+}
+// On a tiled map (tl: its tiling, in device memory; null otherwise) PASS 0 also activates the foreign blocks of removals: their negative terms travel to the
+// owner as deltas.  A removal never activates a block of this rank's own tile, which must already hold it.
 template <int PASS>
-__global__ void __launch_bounds__(256) k_fz_splat(TsGrid dst, TsGrid src, FzDev f, FzSums S, float vs) {
+__global__ void __launch_bounds__(256) k_fz_splat(TsGrid dst, TsGrid src, FzDev f, FzSums S, float vs, const TsTiling* tl) {
   const int nl = (int)f.ctr[0];
   const bool tex = dst.col != nullptr && src.col != nullptr;  // (the host refuses maps that differ in it)
   unsigned long long n_splat = 0, n_skip = 0;
@@ -165,7 +198,7 @@ __global__ void __launch_bounds__(256) k_fz_splat(TsGrid dst, TsGrid src, FzDev 
       if (job < 0) continue;
       const FzJob& J = f.jobs[job];
       const int sign = J.sign;
-      if (PASS == 0 && sign < 0) continue;
+      if (PASS == 0 && sign < 0 && !tl) continue;
       const size_t base = (size_t)b * TS_B3;
       unsigned long long cur_key = TS_EMPTY;
       int cur_blk = -1;
@@ -198,7 +231,7 @@ __global__ void __launch_bounds__(256) k_fz_splat(TsGrid dst, TsGrid src, FzDev 
           if (key != cur_key) {
             cur_key = key;
             if (PASS == 0) {
-              cur_blk = ts_get_or_alloc_cached(dst, key);
+              if (sign > 0 || fz_foreign(tl, ci, cj, ck)) cur_blk = ts_get_or_alloc_cached(dst, key);
             } else {
               cur_blk = ts_find(dst, key);
               if (cur_blk >= 0) ts_mark_dirty(dst, cur_blk);
@@ -267,6 +300,74 @@ __global__ void __launch_bounds__(256) k_fz_commit(TsGrid g, FzSums S, unsigned 
   }
 }
 
+// ---- tiled updates: the sums of foreign blocks travel to their owner as deltas --------------------------------------
+// One CTA per pool block: a dirty block of a foreign tile (ghost or not) copies its sum rows into the slot group of its
+// owner (row = key, then planes x 4096 int64 in plane order S_wT, S_w, co, S_c[3]), zeroes them and drops its flag.
+__global__ void __launch_bounds__(256) k_fz_pack(TsGrid g, TsTiling t, FzSums S, int planes, const int* offsets, int* cursor, long long cap,
+                                                  long long* rows) {
+  __shared__ long long s_slot;
+  const int nb = min(*g.n_blocks, g.max_blocks);
+  const long long rl = 1 + (long long)planes * TS_B3;
+  for (int b = blockIdx.x; b < nb; b += gridDim.x) {
+    if (!g.dirty_flag[b]) continue;  // uniform per CTA
+    int s, bx, by, bz;
+    ts_unpack_key(g.block_key[b], s, bx, by, bz);
+    const int o = tile_owner(t, bx, by, bz);
+    if (o == t.rank) continue;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      s_slot = (long long)offsets[o] + atomicAdd(&cursor[o], 1);
+      if (s_slot < cap) rows[s_slot * rl] = (long long)g.block_key[b];
+      g.dirty_flag[b] = 0;  // not ours: never committed here
+    }
+    __syncthreads();
+    const long long slot = s_slot;
+    for (int p = 0; p < planes; p++) {
+      long long* sp = S.wt + (size_t)p * S.stride + (size_t)b * TS_B3;
+      for (int v = threadIdx.x; v < TS_B3; v += blockDim.x) {
+        if (slot < cap) rows[slot * rl + 1 + (long long)p * TS_B3 + v] = sp[v];
+        sp[v] = 0;
+      }
+    }
+  }
+}
+
+// the owner activates the received blocks (one thread per row) ...
+__global__ void __launch_bounds__(256) k_fz_unpack_alloc(TsGrid g, long long n, long long rl, const long long* rows) {
+  for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < n; q += (long long)gridDim.x * blockDim.x)
+    ts_get_or_alloc(g, (unsigned long long)rows[q * rl]);
+}
+
+// ... and, once its sum planes cover them, adds the rows with wrapping int64 adds (several ranks may send the same block)
+// and flags the blocks for the commit.  One CTA per row.
+__global__ void __launch_bounds__(256) k_fz_unpack_add(TsGrid g, FzSums S, int planes, long long n, const long long* rows) {
+  const long long rl = 1 + (long long)planes * TS_B3;
+  for (long long q = blockIdx.x; q < n; q += gridDim.x) {
+    const long long* row = rows + q * rl;
+    const int blk = ts_find(g, (unsigned long long)row[0]);
+    if (blk < 0) continue;  // (not activated: the pool ran out, which the allocation pass reported)
+    if (threadIdx.x == 0) ts_mark_dirty(g, blk);
+    for (int p = 0; p < planes; p++) {
+      unsigned long long* sp = (unsigned long long*)(S.wt + (size_t)p * S.stride + (size_t)blk * TS_B3);
+      for (int v = threadIdx.x; v < TS_B3; v += blockDim.x) {
+        const long long x = row[1 + (long long)p * TS_B3 + v];
+        if (x) red_add_u64(sp + v, (unsigned long long)x);
+      }
+    }
+  }
+}
+
+// voxels of the dirty blocks whose contribution count decodes as negative: the sums of the ranks disagree
+__global__ void __launch_bounds__(256) k_fz_negative(TsGrid g, FzSums S, unsigned long long* bad) {
+  const int nd = *g.n_dirty;
+  unsigned long long n = 0;
+  for (int q = blockIdx.x; q < nd; q += gridDim.x) {
+    const long long* co = S.co + (size_t)g.dirty_list[q] * TS_B3;
+    for (int v = threadIdx.x; v < TS_B3; v += blockDim.x) n += ((co[v] + (1ll << 31)) >> 32) < 0;
+  }
+  if (n) atomicAdd(bad, n);
+}
+
 // ---------------------------------------------------------------------------
 // host
 // ---------------------------------------------------------------------------
@@ -315,18 +416,26 @@ static int fz_reserve_sums(tslam_tsdf* m, size_t need, cudaStream_t st) {
   return TSLAM_OK;
 }
 
+static void fz_dev(TsFuse* z, FzDev& f);
 static int fz_reserve_dev(tslam_tsdf* dst, tslam_tsdf* src, FzDev& f) {
   TsFuse* z = dst->fz;
   const int S = dst->cfg.max_submaps, B = src->g.max_blocks;
   if (!z->dev || z->dev_submaps != S || z->dev_blocks < B) {
     if (z->dev) TS_CUDA(cudaFree(z->dev));
     z->dev = nullptr;
-    const size_t bytes = (size_t)S * (4 + 4 + 8) + (size_t)2 * S * sizeof(FzJob) + (size_t)B * 4 + 8 * 8 + 256;
+    const size_t bytes = (size_t)S * (4 + 4 + 8) + (size_t)2 * S * sizeof(FzJob) + (size_t)B * 4 + 8 * 8 + sizeof(TsTiling) + 256;
     TS_CUDA(cudaMalloc(&z->dev, bytes));
     z->dev_bytes = bytes;
     z->dev_submaps = S;
     z->dev_blocks = B;
   }
+  fz_dev(z, f);
+  return TSLAM_OK;
+}
+
+// the FzDev arrays in z->dev (as the last fz_reserve_dev sized them)
+static void fz_dev(TsFuse* z, FzDev& f) {
+  const int S = z->dev_submaps;
   char* p = (char*)z->dev;
   f.ctr = (unsigned long long*)p; p += 8 * 8;
   f.jobs = (FzJob*)p; p += (size_t)2 * S * sizeof(FzJob);
@@ -334,7 +443,13 @@ static int fz_reserve_dev(tslam_tsdf* dst, tslam_tsdf* src, FzDev& f) {
   f.nblk = (int*)p; p += (size_t)S * 4;
   f.rbits = (unsigned*)p; p += (size_t)S * 4;
   f.list = (int*)p;
-  return TSLAM_OK;
+}
+
+// device copy of a tiled update's tiling, after the FzDev arrays (k_fz_splat indexes its cuts: as a kernel parameter
+// they would be copied to the stack)
+static TsTiling* fz_dev_tiling(TsFuse* z) {
+  const size_t S = (size_t)z->dev_submaps;
+  return (TsTiling*)((char*)z->dev + 8 * 8 + 2 * S * sizeof(FzJob) + S * (8 + 4 + 4) + (size_t)z->dev_blocks * 4);
 }
 
 // rotation angle of R0^T R (row-major 3x3), in double
@@ -347,20 +462,26 @@ static double fz_angle(const float* R0, const float* R) {
   return std::acos(c);
 }
 
-extern "C" int tslam_tsdf_fuse_update(tslam_tsdf_t* dst, tslam_tsdf_t* src, const uint8_t* include, float tolerance, int32_t full,
-                                      int64_t* stats8, void* stream) {
+// Refusals that need no handle contents (TSLAM_E_INVALID, nothing written)
+static int fz_check_args(tslam_tsdf* dst, tslam_tsdf* src, float tolerance) {
   if (!std::isfinite(tolerance) || tolerance < 0.0f) { ts_set_error("fuse_update: tolerance %g must be finite and >= 0", (double)tolerance); return TSLAM_E_INVALID; }
   if (!dst || !src) { ts_set_error("fuse_update: NULL handle"); return TSLAM_E_INVALID; }
   if (dst == src) { ts_set_error("fuse_update: dst == src (a map cannot be fused into itself)"); return TSLAM_E_INVALID; }
+  return TSLAM_OK;
+}
+
+static int fz_check_maps(tslam_tsdf* dst, tslam_tsdf* src) {
   if (!dst->cfg.is_global_map) { ts_set_error("fuse_update: dst is not a global map (is_global_map = 0)"); return TSLAM_E_INVALID; }
   if (dst->cfg.max_submaps != src->cfg.max_submaps || dst->in.vs != src->in.vs || (dst->g.col != nullptr) != (src->g.col != nullptr)) {
     ts_set_error("fuse_update: dst and src differ in max_submaps (%d, %d), voxel size (%g, %g) or texture setting (%d, %d)", dst->cfg.max_submaps,
                  src->cfg.max_submaps, (double)dst->in.vs, (double)src->in.vs, dst->g.col != nullptr, src->g.col != nullptr);
     return TSLAM_E_INVALID;
   }
-  if (dst->tile_cuts_set) { ts_set_error("fuse_update: dst is a tiled map (tile cuts set): not supported"); return TSLAM_E_INVALID; }
-  cudaStream_t st = (cudaStream_t)stream;
-  const int S = dst->cfg.max_submaps;
+  return TSLAM_OK;
+}
+
+// flush both maps' pending work, create dst's fusion state, reserve its device scratch
+static int fz_open(tslam_tsdf* dst, tslam_tsdf* src, cudaStream_t st, FzDev& f) {
   int rc = ts_flush_pending(src, st);
   if (rc) return rc;
   rc = ts_flush_pending(dst, st);
@@ -371,86 +492,102 @@ extern "C" int tslam_tsdf_fuse_update(tslam_tsdf_t* dst, tslam_tsdf_t* src, cons
     dst->fz->sums = nullptr;
     dst->fz->cap_blocks = 0;
     dst->fz->dev = nullptr;
-    dst->fz->sub.assign(S, FzSub());
+    dst->fz->sub.assign(dst->cfg.max_submaps, FzSub());
   }
-  TsFuse* z = dst->fz;
-  FzDev f;
-  rc = fz_reserve_dev(dst, src, f);
-  if (rc) return rc;
+  return fz_reserve_dev(dst, src, f);
+}
 
-  // plan: source blocks and radius per submap, dst ghosts, dst poses
+// The plan of an update (k_fz_plan: source blocks and radius per submap, dst ghosts; dst's pose table).  `reason` is the
+// full-update reason found from the host state; when it is FZ_INCR the per-submap actions of an incremental update are
+// planned, which may still find a fused submap whose content changed (FZ_CONTENT).  The cost rule and the switch to
+// a full update's actions are the caller's (fz_settle), as a tiled update decides them over all ranks.
+static int fz_plan(tslam_tsdf* dst, tslam_tsdf* src, const uint8_t* include, float tolerance, int reason, cudaStream_t st, const FzDev& f,
+                   FzPlan& P) {
+  TsFuse* z = dst->fz;
+  const int S = dst->cfg.max_submaps;
   TS_CUDA(cudaMemsetAsync(f.ctr, 0, 8 * 8, st));
   TS_CUDA(cudaMemsetAsync(f.nblk, 0, (size_t)S * 8, st));  // nblk and rbits
   const int gp = src->sm_count * 4;
   k_fz_plan<<<gp, 256, 0, st>>>(src->g, dst->g, src->in.vs, f);
   TS_LAUNCH_CHECK(dst);
-  std::vector<int> nblk(S);
-  std::vector<float> rad(S), pR((size_t)S * 9), pT((size_t)S * 3);
+  P.nblk.assign(S, 0);
+  P.rad.assign(S, 0.0f);
+  P.pR.assign((size_t)S * 9, 0.0f);
+  P.pT.assign((size_t)S * 3, 0.0f);
   unsigned long long ctr0[8];
-  TS_CUDA(cudaMemcpyAsync(nblk.data(), f.nblk, (size_t)S * 4, cudaMemcpyDeviceToHost, st));
-  TS_CUDA(cudaMemcpyAsync(rad.data(), f.rbits, (size_t)S * 4, cudaMemcpyDeviceToHost, st));
+  TS_CUDA(cudaMemcpyAsync(P.nblk.data(), f.nblk, (size_t)S * 4, cudaMemcpyDeviceToHost, st));
+  TS_CUDA(cudaMemcpyAsync(P.rad.data(), f.rbits, (size_t)S * 4, cudaMemcpyDeviceToHost, st));
   TS_CUDA(cudaMemcpyAsync(ctr0, f.ctr, sizeof(ctr0), cudaMemcpyDeviceToHost, st));
-  TS_CUDA(cudaMemcpyAsync(pR.data(), dst->pose_R, (size_t)S * 36, cudaMemcpyDeviceToHost, st));
-  TS_CUDA(cudaMemcpyAsync(pT.data(), dst->pose_T, (size_t)S * 12, cudaMemcpyDeviceToHost, st));
+  TS_CUDA(cudaMemcpyAsync(P.pR.data(), dst->pose_R, (size_t)S * 36, cudaMemcpyDeviceToHost, st));
+  TS_CUDA(cudaMemcpyAsync(P.pT.data(), dst->pose_T, (size_t)S * 12, cudaMemcpyDeviceToHost, st));
   TS_CUDA(cudaStreamSynchronize(st));
-  if (ctr0[3] > 0) { ts_set_error("fuse_update: dst holds %llu ghost blocks (a tiled map): not supported", ctr0[3]); return TSLAM_E_INVALID; }
+  P.ghosts = ctr0[3];
 
-  int reason = FZ_INCR;
-  if (full) reason = FZ_ASKED;
-  else if (!z->valid) reason = FZ_FIRST;
-  else if (z->src_serial != src->serial) reason = FZ_OTHER_SRC;
-  else if (z->gen != dst->write_gen) reason = FZ_DST_WRITTEN;
-  enum { NONE = 0, ADD, REMOVE, MOVE, KEEP };
-  std::vector<unsigned char> act(S, NONE);
-  long long n_add = 0, n_move = 0, n_remove = 0, n_tol = 0, cost = 0, cost_full = 0;
+  P.want.assign(S, 0);
+  P.act.assign(S, FZ_NONE);
+  P.n_add = P.n_move = P.n_remove = P.n_tol = P.cost = P.cost_full = 0;
+  const std::vector<int>& nblk = P.nblk;
   for (int s = 0; s < S; s++) {
     const bool want = (!include || include[s]) && nblk[s] > 0;
-    if (want) cost_full += nblk[s];
+    P.want[s] = want;
+    if (want) P.cost_full += nblk[s];
     if (reason != FZ_INCR) continue;
     const FzSub& r = z->sub[s];
     if (!r.fused) {
-      if (want) { act[s] = ADD; cost += nblk[s]; }
+      if (want) { P.act[s] = FZ_ADD; P.cost += nblk[s]; }
       continue;
     }
     if (r.ver != src->content_ver[s]) { reason = FZ_CONTENT; continue; }  // its old content is gone: cannot be subtracted
-    if (!want) { act[s] = REMOVE; cost += r.nblk; continue; }
-    const float* R = &pR[(size_t)9 * s];
-    const float* T = &pT[(size_t)3 * s];
-    if (!memcmp(R, r.R, 36) && !memcmp(T, r.T, 12)) { act[s] = KEEP; continue; }
+    if (!want) { P.act[s] = FZ_REMOVE; P.cost += r.nblk; continue; }
+    const float* R = &P.pR[(size_t)9 * s];
+    const float* T = &P.pT[(size_t)3 * s];
+    if (!memcmp(R, r.R, 36) && !memcmp(T, r.T, 12)) { P.act[s] = FZ_KEEP; continue; }
     if (tolerance > 0.0f) {
       const double dx = (double)T[0] - r.T[0], dy = (double)T[1] - r.T[1], dz = (double)T[2] - r.T[2];
-      const double move = std::sqrt(dx * dx + dy * dy + dz * dz) + fz_angle(r.R, R) * (double)rad[s];
-      if (move <= (double)tolerance) { act[s] = KEEP; n_tol++; continue; }
+      const double move = std::sqrt(dx * dx + dy * dy + dz * dz) + fz_angle(r.R, R) * (double)P.rad[s];
+      if (move <= (double)tolerance) { P.act[s] = FZ_KEEP; P.n_tol++; continue; }
     }
-    act[s] = MOVE;
-    cost += r.nblk + nblk[s];
+    P.act[s] = FZ_MOVE;
+    P.cost += r.nblk + nblk[s];
   }
-  if (reason == FZ_INCR && cost > cost_full) reason = FZ_COST;
-  const bool is_full = reason != FZ_INCR;
-  if (is_full) {
-    n_add = n_move = n_remove = n_tol = 0;
-    for (int s = 0; s < S; s++) act[s] = ((!include || include[s]) && nblk[s] > 0) ? ADD : NONE;
-  }
-  for (int s = 0; s < S; s++) {
-    n_add += act[s] == ADD;
-    n_move += act[s] == MOVE;
-    n_remove += act[s] == REMOVE;
-  }
+  P.reason = reason;
+  return TSLAM_OK;
+}
 
-  // jobs
+// the update's final reason: a full update adds every included submap
+static void fz_settle(FzPlan& P, int reason) {
+  P.reason = reason;
+  P.full = reason != FZ_INCR;
+  if (P.full) {
+    P.n_tol = 0;
+    for (size_t s = 0; s < P.act.size(); s++) P.act[s] = P.want[s] ? FZ_ADD : FZ_NONE;
+  }
+  P.n_add = P.n_move = P.n_remove = 0;
+  for (size_t s = 0; s < P.act.size(); s++) {
+    P.n_add += P.act[s] == FZ_ADD;
+    P.n_move += P.act[s] == FZ_MOVE;
+    P.n_remove += P.act[s] == FZ_REMOVE;
+  }
+}
+
+// Splat the plan into the sums: a full update resets dst and zeroes the sums first.  Tiled (t: the tiling, else null):
+// removals also activate their foreign blocks.  Invalidates the sums until the update is recorded.
+static int fz_execute(tslam_tsdf* dst, tslam_tsdf* src, const FzDev& f, const FzPlan& P, const TsTiling* t, cudaStream_t st) {
+  TsFuse* z = dst->fz;
+  const int S = dst->cfg.max_submaps;
   std::vector<FzJob> jobs;
   std::vector<int2> job_of(S, make_int2(-1, -1));
   for (int s = 0; s < S; s++) {
-    if (act[s] == REMOVE || act[s] == MOVE) {
+    if (P.act[s] == FZ_REMOVE || P.act[s] == FZ_MOVE) {
       FzJob j;
       memcpy(j.R, z->sub[s].R, 36); memcpy(j.T, z->sub[s].T, 12);
       j.sign = -1; j.pad = 0;
       job_of[s].x = (int)jobs.size();
       jobs.push_back(j);
     }
-    if (act[s] == ADD || act[s] == MOVE) {
+    if (P.act[s] == FZ_ADD || P.act[s] == FZ_MOVE) {
       FzJob j;
-      memcpy(j.R, &pR[(size_t)9 * s], 36); memcpy(j.T, &pT[(size_t)3 * s], 12);
+      memcpy(j.R, &P.pR[(size_t)9 * s], 36); memcpy(j.T, &P.pT[(size_t)3 * s], 12);
       j.sign = 1; j.pad = 0;
       job_of[s].y = (int)jobs.size();
       jobs.push_back(j);
@@ -459,9 +596,9 @@ extern "C" int tslam_tsdf_fuse_update(tslam_tsdf_t* dst, tslam_tsdf_t* src, cons
 
   const int planes = fz_planes(dst);
   z->valid = 0;  // until this update completes
-  if (is_full) {
+  if (P.full) {
     const unsigned long long gen = dst->write_gen;
-    rc = tslam_tsdf_reset(dst, stream);  // also compacts the pool: blocks left empty by removals are dropped
+    int rc = tslam_tsdf_reset(dst, (void*)st);  // also compacts the pool: blocks left empty by removals are dropped
     if (rc) return rc;
     dst->write_gen = gen;
     // every plane in full: a reset of dst since the last update left the pool empty but not the sums (at most 2x the
@@ -475,8 +612,13 @@ extern "C" int tslam_tsdf_fuse_update(tslam_tsdf_t* dst, tslam_tsdf_t* src, cons
     k_fz_list<<<gl, 256, 0, st>>>(src->g, f);
     TS_LAUNCH_CHECK(dst);
     const int gs = dst->sm_count * 8;
-    if (n_add + n_move > 0) {
-      k_fz_splat<0><<<gs, 256, 0, st>>>(dst->g, src->g, f, FzSums{}, dst->in.vs);
+    if (P.n_add + P.n_move > 0 || (t && P.n_remove > 0)) {
+      TsTiling* td = nullptr;
+      if (t) {
+        td = fz_dev_tiling(z);
+        TS_CUDA(cudaMemcpyAsync(td, t, sizeof(TsTiling), cudaMemcpyHostToDevice, st));
+      }
+      k_fz_splat<0><<<gs, 256, 0, st>>>(dst->g, src->g, f, FzSums{}, dst->in.vs, td);
       TS_LAUNCH_CHECK(dst);
     }
     int nb = 0, err = 0;
@@ -484,24 +626,34 @@ extern "C" int tslam_tsdf_fuse_update(tslam_tsdf_t* dst, tslam_tsdf_t* src, cons
     TS_CUDA(cudaMemcpyAsync(&err, dst->g.err, 4, cudaMemcpyDeviceToHost, st));
     TS_CUDA(cudaStreamSynchronize(st));
     if (err) return ts_check_deferred(dst);  // pool exhausted: nothing was added; the next update is a full one
-    rc = fz_reserve_sums(dst, (size_t)std::min(nb, dst->g.max_blocks), st);
+    int rc = fz_reserve_sums(dst, (size_t)std::min(nb, dst->g.max_blocks), st);
     if (rc) return rc;
-    k_fz_splat<1><<<gs, 256, 0, st>>>(dst->g, src->g, f, fz_sums(z, planes), dst->in.vs);
+    k_fz_splat<1><<<gs, 256, 0, st>>>(dst->g, src->g, f, fz_sums(z, planes), dst->in.vs, nullptr);
     TS_LAUNCH_CHECK(dst);
   }
-  // commit the touched blocks
-  rc = ts_collect_dirty(dst, st);
+  return TSLAM_OK;
+}
+
+// Read the dirty blocks out of the sums (ctr[4] = their number); tiled updates first count the voxels whose count
+// decodes as negative (ctr[5]).  Then the error words: a removal that found no block, inconsistent sums, device flags.
+static int fz_commit(tslam_tsdf* dst, const FzDev& f, bool check_negative, cudaStream_t st, unsigned long long* ctr) {
+  TsFuse* z = dst->fz;
+  const int planes = fz_planes(dst);
+  int rc = ts_collect_dirty(dst, st);
   if (rc) return rc;
   TS_CUDA(cudaMemcpyAsync(&f.ctr[4], dst->g.n_dirty, 4, cudaMemcpyDeviceToDevice, st));
   if (z->sums) {
+    if (check_negative) {
+      k_fz_negative<<<dst->sm_count * 4, 256, 0, st>>>(dst->g, fz_sums(z, planes), &f.ctr[5]);
+      TS_LAUNCH_CHECK(dst);
+    }
     const unsigned long long seq = ++dst->commit_seq;  // stamp of every block this update writes (incremental mesh)
     k_fz_commit<<<dst->sm_count * 4, 256, 0, st>>>(dst->g, fz_sums(z, planes), dst->blk_stamp, seq);
     TS_LAUNCH_CHECK(dst);
   }
   TS_CUDA(cudaMemsetAsync(dst->g.n_dirty, 0, 4, st));
-  unsigned long long ctr[8];
   int err = 0;
-  TS_CUDA(cudaMemcpyAsync(ctr, f.ctr, sizeof(ctr), cudaMemcpyDeviceToHost, st));
+  TS_CUDA(cudaMemcpyAsync(ctr, f.ctr, 8 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
   TS_CUDA(cudaMemcpyAsync(&err, dst->g.err, 4, cudaMemcpyDeviceToHost, st));
   TS_CUDA(cudaStreamSynchronize(st));
   if (err & TS_ERR_FUSE_MISSING) {
@@ -510,35 +662,260 @@ extern "C" int tslam_tsdf_fuse_update(tslam_tsdf_t* dst, tslam_tsdf_t* src, cons
     ts_set_error("fuse_update: a removal found no block of dst (its sums and pool disagree); the next update is a full one");
     return TSLAM_E_CUDA;
   }
-  rc = ts_check_deferred(dst);
-  if (rc) return rc;
-  // voxels that lose their last contribution become unobserved, which the incremental ESDF does not undo
-  if (n_remove + n_move > 0) dst->esdf_full_needed = 1;
+  if (ctr[5]) {
+    ts_set_error("fuse_update: %llu voxels of dst decode a negative contribution count (the ranks' sums disagree); the next update is a full "
+                 "one", ctr[5]);
+    return TSLAM_E_CUDA;
+  }
+  return ts_check_deferred(dst);
+}
 
-  for (int s = 0; s < S; s++) {
+// the submaps' new state after a successful update
+static void fz_record(tslam_tsdf* dst, tslam_tsdf* src, const FzPlan& P) {
+  TsFuse* z = dst->fz;
+  for (int s = 0; s < dst->cfg.max_submaps; s++) {
     FzSub& r = z->sub[s];
-    if (is_full) r.fused = 0;
-    if (act[s] == REMOVE) r.fused = 0;
-    if (act[s] == ADD || act[s] == MOVE) {
+    if (P.full) r.fused = 0;
+    if (P.act[s] == FZ_REMOVE) r.fused = 0;
+    if (P.act[s] == FZ_ADD || P.act[s] == FZ_MOVE) {
       r.fused = 1;
-      memcpy(r.R, &pR[(size_t)9 * s], 36);
-      memcpy(r.T, &pT[(size_t)3 * s], 12);
+      memcpy(r.R, &P.pR[(size_t)9 * s], 36);
+      memcpy(r.T, &P.pT[(size_t)3 * s], 12);
       r.ver = src->content_ver[s];
-      r.nblk = nblk[s];
+      r.nblk = P.nblk[s];
     }
   }
+  // voxels that lose their last contribution become unobserved, which the incremental ESDF does not undo
+  if (P.n_remove + P.n_move > 0) dst->esdf_full_needed = 1;
   z->valid = 1;
+  z->ever_valid = 1;
   z->src_serial = src->serial;
+}
+
+static void fz_stats(const FzPlan& P, const unsigned long long* ctr, int64_t* stats8) {
+  if (!stats8) return;
+  stats8[0] = P.reason;
+  stats8[1] = P.n_add;
+  stats8[2] = P.n_move;
+  stats8[3] = P.n_remove;
+  stats8[4] = P.n_tol;
+  stats8[5] = (int64_t)ctr[1];
+  stats8[6] = (int64_t)ctr[2];
+  stats8[7] = (int64_t)(unsigned)ctr[4];
+}
+
+extern "C" int tslam_tsdf_fuse_update(tslam_tsdf_t* dst, tslam_tsdf_t* src, const uint8_t* include, float tolerance, int32_t full,
+                                      int64_t* stats8, void* stream) {
+  int rc = fz_check_args(dst, src, tolerance);
+  if (rc) return rc;
+  rc = fz_check_maps(dst, src);
+  if (rc) return rc;
+  if (dst->tile_cuts_set) { ts_set_error("fuse_update: dst is a tiled map (tile cuts set): not supported"); return TSLAM_E_INVALID; }
+  cudaStream_t st = (cudaStream_t)stream;
+  FzDev f;
+  rc = fz_open(dst, src, st, f);
+  if (rc) return rc;
+  TsFuse* z = dst->fz;
+  int reason = FZ_INCR;
+  if (full) reason = FZ_ASKED;
+  else if (!z->valid) reason = FZ_FIRST;
+  else if (z->src_serial != src->serial) reason = FZ_OTHER_SRC;
+  else if (z->gen != dst->write_gen || z->tiled) reason = FZ_DST_WRITTEN;  // (sums of a tiled update hold one tile)
+  FzPlan P;
+  rc = fz_plan(dst, src, include, tolerance, reason, st, f, P);
+  if (rc) return rc;
+  if (P.ghosts > 0) { ts_set_error("fuse_update: dst holds %llu ghost blocks (a tiled map): not supported", P.ghosts); return TSLAM_E_INVALID; }
+  fz_settle(P, P.reason == FZ_INCR && P.cost > P.cost_full ? FZ_COST : P.reason);
+  rc = fz_execute(dst, src, f, P, nullptr, st);
+  if (rc) return rc;
+  unsigned long long ctr[8];
+  rc = fz_commit(dst, f, false, st, ctr);
+  if (rc) return rc;
+  fz_record(dst, src, P);
   z->gen = dst->write_gen;
-  if (stats8) {
-    stats8[0] = reason;
-    stats8[1] = n_add;
-    stats8[2] = n_move;
-    stats8[3] = n_remove;
-    stats8[4] = n_tol;
-    stats8[5] = (int64_t)ctr[1];
-    stats8[6] = (int64_t)ctr[2];
-    stats8[7] = (int64_t)(unsigned)ctr[4];
+  z->tiled = 0;
+  fz_stats(P, ctr, stats8);
+  return TSLAM_OK;
+}
+
+// ---------------------------------------------------------------------------
+// tiled updates (DESIGN.md section 6, "Incremental tiled fusion"; include/tslam.h)
+// ---------------------------------------------------------------------------
+static const char* const FZ_PHASE[] = {"none", "plan", "splat", "pack", "unpack"};
+
+static int fz_phase(tslam_tsdf* dst, int want, const char* what) {
+  const int ph = dst->fz ? dst->fz->phase : 0;
+  if (ph != want) {
+    ts_set_error("%s: called out of order (the last phase of this update was '%s', this call follows '%s')", what, FZ_PHASE[ph], FZ_PHASE[want]);
+    return TSLAM_E_INVALID;
   }
+  return TSLAM_OK;
+}
+
+// tiles3 / rank / world checks that need no handle (fill_tiling repeats them with the map's cuts)
+static int fz_check_tiles(const int32_t* tiles3, int32_t rank, int32_t world) {
+  if (!tiles3 || world < 1 || world > 24 || rank < 0 || rank >= world || tiles3[0] < 1 || tiles3[1] < 1 || tiles3[2] < 1 ||
+      tiles3[0] > TS_MAX_TILES_AXIS || tiles3[1] > TS_MAX_TILES_AXIS || tiles3[2] > TS_MAX_TILES_AXIS || tiles3[0] * tiles3[1] * tiles3[2] != world) {
+    ts_set_error("fuse_update_tiled: bad tiling %d x %d x %d for rank %d of world %d (1 <= world <= 24)", tiles3 ? tiles3[0] : -1, tiles3 ? tiles3[1] : -1,
+                 tiles3 ? tiles3[2] : -1, rank, world);
+    return TSLAM_E_INVALID;
+  }
+  return TSLAM_OK;
+}
+
+static int fz_tiling(tslam_tsdf* m, const int32_t* tiles3, int32_t rank, int32_t world, TsTiling* t) {
+  memset(t, 0, sizeof(*t));  // (the tiling is compared bytewise)
+  return fill_tiling(m, tiles3, rank, world, t);
+}
+
+extern "C" int tslam_tsdf_fuse_update_tiled_plan(tslam_tsdf_t* dst, tslam_tsdf_t* src, const int32_t* tiles3, int32_t rank, int32_t world,
+                                                 const uint8_t* include, float tolerance, int32_t full, int64_t* plan3, uint8_t* present,
+                                                 void* stream) {
+  int rc = fz_check_args(dst, src, tolerance);
+  if (rc) return rc;
+  if (!plan3 || !present) { ts_set_error("fuse_update_tiled_plan: NULL plan3 or present"); return TSLAM_E_INVALID; }
+  rc = fz_check_tiles(tiles3, rank, world);
+  if (rc) return rc;
+  rc = fz_check_maps(dst, src);
+  if (rc) return rc;
+  TsTiling t;
+  rc = fz_tiling(dst, tiles3, rank, world, &t);
+  if (rc) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  FzDev f;
+  rc = fz_open(dst, src, st, f);
+  if (rc) return rc;
+  TsFuse* z = dst->fz;
+  if (z->phase >= 2) z->valid = 0;  // an update abandoned after its splat left the sums part-way
+  z->phase = 0;
+  int reason = FZ_INCR;
+  if (full) reason = FZ_ASKED;
+  else if (!z->valid) reason = z->ever_valid ? FZ_INVALID : FZ_FIRST;
+  else if (z->src_serial != src->serial) reason = FZ_OTHER_SRC;
+  else if (z->gen != dst->write_gen - dst->ghost_gen) reason = FZ_DST_WRITTEN;  // owned content written; ghost imports are not
+  else if (!z->tiled || memcmp(&z->tiling, &t, sizeof(t))) reason = FZ_CUTS;
+  rc = fz_plan(dst, src, include, tolerance, reason, st, f, z->plan);
+  if (rc) return rc;
+  const FzPlan& P = z->plan;
+  for (int s = 0; s < dst->cfg.max_submaps; s++) present[s] = P.nblk[s] > 0;
+  plan3[0] = P.reason;
+  plan3[1] = P.cost;
+  plan3[2] = P.cost_full;
+  z->plan_src = src->serial;
+  z->plan_tiling = t;
+  z->phase = 1;
+  return TSLAM_OK;
+}
+
+extern "C" int tslam_tsdf_fuse_update_tiled_splat(tslam_tsdf_t* dst, tslam_tsdf_t* src, int32_t reason, void* stream) {
+  if (!dst || !src) { ts_set_error("fuse_update_tiled_splat: NULL handle"); return TSLAM_E_INVALID; }
+  if (reason < FZ_INCR || reason > FZ_INVALID) { ts_set_error("fuse_update_tiled_splat: reason %d outside [0, 8]", reason); return TSLAM_E_INVALID; }
+  int rc = fz_phase(dst, 1, "fuse_update_tiled_splat");
+  if (rc) return rc;
+  TsFuse* z = dst->fz;
+  if (src->serial != z->plan_src) { ts_set_error("fuse_update_tiled_splat: src is not the map the update was planned with"); return TSLAM_E_INVALID; }
+  if (reason == FZ_INCR && z->plan.reason != FZ_INCR) {
+    ts_set_error("fuse_update_tiled_splat: an incremental update where this rank's plan is full (reason %d)", z->plan.reason);
+    return TSLAM_E_INVALID;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  FzDev f;
+  fz_dev(z, f);  // (the plan sized it for src)
+  fz_settle(z->plan, reason);
+  z->phase = 2;  // (from here on a failure leaves the sums invalid)
+  return fz_execute(dst, src, f, z->plan, &z->plan_tiling, st);
+}
+
+extern "C" int tslam_tsdf_fuse_update_tiled_pack(tslam_tsdf_t* dst, const int32_t* tiles3, int32_t rank, int32_t world, const int32_t* counts,
+                                                 int64_t cap, int64_t* rows, void* stream) {
+  if (!dst || !counts || cap < 0 || (cap && !rows)) { ts_set_error("fuse_update_tiled_pack: NULL handle, counts or rows, or cap < 0"); return TSLAM_E_INVALID; }
+  int rc = fz_check_tiles(tiles3, rank, world);
+  if (rc) return rc;
+  rc = fz_phase(dst, 2, "fuse_update_tiled_pack");
+  if (rc) return rc;
+  TsFuse* z = dst->fz;
+  TsTiling t;
+  rc = fz_tiling(dst, tiles3, rank, world, &t);
+  if (rc) return rc;
+  if (!z->plan.full && memcmp(&t, &z->plan_tiling, sizeof(t))) {
+    ts_set_error("fuse_update_tiled_pack: the tiling changed during an incremental update (only a full update may move the cuts)");
+    return TSLAM_E_INVALID;
+  }
+  int h_off[24];
+  long long tot = 0;
+  for (int r = 0; r < world; r++) {
+    h_off[r] = (int)tot;
+    tot += counts[r] < 0 ? 0 : counts[r];
+  }
+  if (tot > cap) { ts_set_error("fuse_update_tiled_pack: %lld blocks to send, capacity %lld", tot, (long long)cap); return TSLAM_E_CAPACITY; }
+  cudaStream_t st = (cudaStream_t)stream;
+  if (z->sums) {
+    int* d_off = dst->scratch_i + 16;
+    int* d_cur = dst->scratch_i + 40;
+    TS_CUDA(cudaMemcpyAsync(d_off, h_off, world * sizeof(int), cudaMemcpyHostToDevice, st));
+    TS_CUDA(cudaMemsetAsync(d_cur, 0, 24 * sizeof(int), st));
+    const int planes = fz_planes(dst);
+    k_fz_pack<<<dst->sm_count * 4, 256, 0, st>>>(dst->g, t, fz_sums(z, planes), planes, d_off, d_cur, cap, (long long*)rows);
+    TS_LAUNCH_CHECK(dst);
+    TS_CUDA(cudaStreamSynchronize(st));  // h_off is on the stack
+  }
+  z->plan_tiling = t;
+  z->phase = 3;
+  return TSLAM_OK;
+}
+
+extern "C" int tslam_tsdf_fuse_update_tiled_unpack(tslam_tsdf_t* dst, int64_t n, const int64_t* rows, void* stream) {
+  if (!dst || n < 0 || (n && !rows)) { ts_set_error("fuse_update_tiled_unpack: NULL handle or rows, or n < 0"); return TSLAM_E_INVALID; }
+  int rc = fz_phase(dst, 3, "fuse_update_tiled_unpack");
+  if (rc) return rc;
+  TsFuse* z = dst->fz;
+  cudaStream_t st = (cudaStream_t)stream;
+  FzDev f;
+  fz_dev(z, f);
+  const int planes = fz_planes(dst);
+  if (n > 0) {
+    const long long rl = 1 + (long long)planes * TS_B3;
+    k_fz_unpack_alloc<<<(int)std::min<long long>((n + 255) / 256, dst->sm_count * 4), 256, 0, st>>>(dst->g, n, rl, (const long long*)rows);
+    TS_LAUNCH_CHECK(dst);
+    int nb = 0, err = 0;
+    TS_CUDA(cudaMemcpyAsync(&nb, dst->g.n_blocks, 4, cudaMemcpyDeviceToHost, st));
+    TS_CUDA(cudaMemcpyAsync(&err, dst->g.err, 4, cudaMemcpyDeviceToHost, st));
+    TS_CUDA(cudaStreamSynchronize(st));
+    if (err & ~TS_ERR_FUSE_MISSING) return ts_check_deferred(dst);  // pool exhausted on the owner
+    rc = fz_reserve_sums(dst, (size_t)std::min(nb, dst->g.max_blocks), st);
+    if (rc) return rc;
+    k_fz_unpack_add<<<(int)std::min<long long>(n, dst->sm_count * 4), 256, 0, st>>>(dst->g, fz_sums(z, planes), planes, n, (const long long*)rows);
+    TS_LAUNCH_CHECK(dst);
+  }
+  unsigned long long ctr[8];
+  rc = fz_commit(dst, f, true, st, ctr);
+  if (rc) return rc;
+  z->phase = 4;
+  return TSLAM_OK;
+}
+
+extern "C" int tslam_tsdf_fuse_update_tiled_finish(tslam_tsdf_t* dst, tslam_tsdf_t* src, int32_t ok, int64_t* stats8, void* stream) {
+  if (!dst || !src) { ts_set_error("fuse_update_tiled_finish: NULL handle"); return TSLAM_E_INVALID; }
+  TsFuse* z = dst->fz;
+  if (!z || z->phase == 0) { ts_set_error("fuse_update_tiled_finish: no tiled update is in progress"); return TSLAM_E_INVALID; }
+  if (!ok) {  // the update failed on some rank: a plan alone wrote nothing, anything later leaves the sums invalid
+    if (z->phase >= 2) z->valid = 0;
+    z->phase = 0;
+    return TSLAM_OK;
+  }
+  int rc = fz_phase(dst, 4, "fuse_update_tiled_finish");
+  if (rc) return rc;
+  if (src->serial != z->plan_src) { ts_set_error("fuse_update_tiled_finish: src is not the map the update was planned with"); return TSLAM_E_INVALID; }
+  FzDev f;
+  fz_dev(z, f);
+  unsigned long long ctr[8];
+  TS_CUDA(cudaMemcpyAsync(ctr, f.ctr, sizeof(ctr), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
+  TS_CUDA(cudaStreamSynchronize((cudaStream_t)stream));
+  fz_record(dst, src, z->plan);
+  z->gen = dst->write_gen - dst->ghost_gen;
+  z->tiled = 1;
+  z->tiling = z->plan_tiling;
+  z->phase = 0;
+  fz_stats(z->plan, ctr, stats8);
   return TSLAM_OK;
 }

@@ -638,6 +638,7 @@ struct tslam_tsdf {
   // the update compares both against what it recorded when it last ran.
   unsigned long long serial;        // process-unique number of the handle (an address can be reused by a new handle)
   unsigned long long write_gen;     // writes of the planes by any entry other than tslam_tsdf_fuse_update
+  unsigned long long ghost_gen;     // ... of which ghost imports (tslam_tsdf_ghost_unpack): the tiled update ignores them
   unsigned long long* content_ver;  // [max_submaps] host: writes of each submap's planes
   struct TsFuse* fz;                // state of this map as the destination of tslam_tsdf_fuse_update (first call allocates)
   int march_verify;    // TSLAM_MARCH_VERIFY=1: every fast-path index is re-computed exactly, mismatches counted
@@ -919,9 +920,28 @@ static cudaError_t ts_launch_pdl(void (*k)(KArgs...), dim3 grid, int block, size
   return cudaLaunchKernelEx(&cfg, k, std::forward<Args>(args)...);
 }
 
+// Tiling of a tiled global map over `world` ranks (tslam_dist.cu, and the tiled incremental fusion in tslam_fuse.cu)
+#define TS_MAX_TILES_AXIS 16
+struct TsTiling {
+  int tiles[3];
+  int rank, world;
+  int cuts[3][TS_MAX_TILES_AXIS + 1];  // tile k of axis a owns block coordinates [cuts[a][k], cuts[a][k+1])
+};
+
+__host__ __device__ __forceinline__ int tile_coord(const TsTiling& t, int axis, int b) {
+  int c = 0;
+  while (c + 1 < t.tiles[axis] && b >= t.cuts[axis][c + 1]) ++c;  // (blocks outside the cut range belong to the end tiles)
+  return c;
+}
+__host__ __device__ __forceinline__ int tile_owner(const TsTiling& t, int bx, int by, int bz) {
+  return (tile_coord(t, 0, bx) * t.tiles[1] + tile_coord(t, 1, by)) * t.tiles[2] + tile_coord(t, 2, bz);
+}
+
 // shared across translation units
+// tslam_dist.cu: the tiling of m for tiles3 / rank / world (its installed cuts when they match tiles3, else equal slices)
+int fill_tiling(tslam_tsdf* m, const int32_t* tiles3, int rank, int world, TsTiling* t);
 // tslam_integrate.cu
-int ts_integrate_init();                                 // once per process, before the first integrate launch
+int ts_integrate_init();                                // once per process, before the first integrate launch
 // commit if anything is pending; prof: the stamp row of the profiled integrate launch it belongs to, or null
 int ts_flush_pending(tslam_tsdf* m, cudaStream_t st, unsigned long long* prof = nullptr);
 // k_collect_dirty + commit of the dirty blocks

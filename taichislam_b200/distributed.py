@@ -76,6 +76,48 @@ def factor_tiles(world):
     return best
 
 
+def merge_fuse_plans(rows):
+    """Merge of the ranks' plans of a tiled incremental fusion (TiledGlobalMap.update_fused_submaps).  rows: int64
+    [world, 3 + 2 S], rank r's row = (full-update reason, cost, cost_full, present[S], include[S]) as
+    tslam_tsdf_fuse_update_tiled_plan reports them (present: the rank's collection holds blocks of the submap; include:
+    0/1 per submap, all 1 for None).  Returns the reason code every rank splats with: the smallest non-zero reason of
+    any rank, else 6 when the summed cost exceeds the summed cost_full (subtracting and re-adding would splat more
+    than a rebuild), else 0 (incremental).  Raises ValueError when a submap has blocks on two ranks, or when include
+    differs between ranks."""
+    rows = np.asarray(rows, dtype=np.int64)
+    if rows.ndim != 2 or rows.shape[1] < 3 or (rows.shape[1] - 3) % 2:
+        raise ValueError(f"plan rows of shape {rows.shape}: expected [world, 3 + 2 * max_submaps]")
+    S = (rows.shape[1] - 3) // 2
+    present, include = rows[:, 3:3 + S], rows[:, 3 + S:]
+    shared = np.flatnonzero((present != 0).sum(0) > 1)
+    if shared.size:
+        ranks = [np.flatnonzero(present[:, s]).tolist() for s in shared[:4]]
+        raise ValueError(f"tiled fusion: submaps {shared.tolist()} have blocks on several ranks (ranks {ranks}); a submap is "
+                         "contributed by one rank")
+    if np.any(include != include[:1]):
+        raise ValueError("tiled fusion: include differs between ranks (submaps "
+                         f"{np.flatnonzero(np.any(include != include[:1], 0)).tolist()}); every rank must pass the same")
+    reasons = rows[:, 0]
+    if np.any(reasons != 0):
+        return int(reasons[reasons != 0].min())
+    return 6 if int(rows[:, 1].sum()) > int(rows[:, 2].sum()) else 0
+
+
+# counters of the tiled incremental fusion, summed over the ranks
+_UPDATE_SUMS = ("added", "moved", "removed", "within_tolerance", "voxels_splatted", "voxels_skipped", "blocks_committed",
+                "foreign_blocks_sent", "foreign_blocks_received", "bytes_sent")
+
+
+def _attempt(fn, *args):
+    """(0, fn(*args)), or (error code, message) when the library refuses or fails: a phase that fails on one rank must
+    still reach the collective where the ranks agree on it."""
+    from . import _capi as capi
+    try:
+        return 0, fn(*args)
+    except capi.TslamError as e:
+        return e.code, str(e)
+
+
 def submap_owner(submap_id, world):
     return int(submap_id) % int(world)
 
@@ -256,6 +298,105 @@ class TiledGlobalMap:
         recv = exchange_counts(self.dist, send, dev)
         rbufs = tuple(exchange_rows(self.dist, b, send, recv) for b in bufs)
         self.fusion_unpack(rbufs)
+
+    # ---- incremental fusion with exact integer sums, phase by phase (csrc/tslam_fuse.cu) -------------------------
+    # The contract is tslam_tsdf_fuse_update_tiled_plan's (include/tslam.h, DESIGN.md section 6): the sums of a block live
+    # on its owner, the other ranks send integer deltas, so the union of the tiles is bit for bit the single-map
+    # tslam_tsdf_fuse_update of every rank's submaps.  update_fused_submaps (NCCL / gloo) and
+    # run_local_update_fused_submaps (LocalGroup) run the same phases.
+    def update_plan(self, submaps, include=None, tolerance=0.0, full=False):
+        """Phase 1: this rank's plan row (merge_fuse_plans) for its submap collection `submaps`."""
+        submaps._flush()
+        h = self.m._h
+        plan, present = h.fuse_update_tiled_plan(submaps._h, self.tiles, self.rank, self.world, include, tolerance, full)
+        inc = h.include_u8(include)
+        inc = np.ones(present.shape[0], np.int64) if inc is None else inc.astype(np.int64)
+        return np.concatenate([plan, present.astype(np.int64), inc])
+
+    def update_splat(self, submaps, reason):
+        """Phase 2: splat with the merged reason.  A full update with balanced cuts returns the marginal histograms of
+        the blocks its additions activated (to be summed over the ranks for balanced_tiling), else None."""
+        from . import _capi as capi
+        self.m._h.fuse_update_tiled_splat(submaps._h, reason)
+        if not (reason and self.balance):
+            return None
+        hist = np.zeros((3, 1024), np.int32)
+        capi.check(self._L().tslam_tsdf_dirty_hist(self._h(), capi.np_ptr(hist), capi.stream_ptr()))
+        return hist
+
+    def update_pack(self):
+        """Phase 3: the sum rows of the foreign blocks -> (send counts, (rows,)) grouped by owner."""
+        send, rows = self.m._h.fuse_update_tiled_pack(self.tiles, self.rank, self.world)
+        self.last_exchange = {"foreign_blocks_sent": int(send.sum()), "bytes_sent": int(rows.numel()) * 8}
+        return send, (rows,)
+
+    def update_unpack(self, bufs):
+        """Phase 4: add the received rows into the owned sums and commit the touched blocks."""
+        self.m._h.fuse_update_tiled_unpack(bufs[0])
+        self.last_exchange["foreign_blocks_received"] = int(bufs[0].shape[0])
+
+    def update_finish(self, submaps, ok):
+        """Phase 5: record the update (ok: every rank's phases succeeded) -> this rank's statistics, or None."""
+        self._halo_current = False
+        st = self.m._h.fuse_update_tiled_finish(submaps._h, ok)
+        if st is not None:
+            for k in ("foreign_blocks_sent", "foreign_blocks_received", "bytes_sent"):
+                st[k] = int(self.last_exchange.get(k, 0))
+        return st
+
+    def _agree(self, submaps, rc, msg, dev):
+        """Every rank learns whether a phase failed anywhere; if so every rank abandons the update and raises."""
+        import torch
+        from . import _capi as capi
+        t = torch.tensor([int(rc)], dtype=torch.int64, device=dev)
+        self.dist.all_reduce(t, op=self.dist.ReduceOp.MIN)
+        worst = int(t.item())
+        if worst:
+            self.update_finish(submaps, False)
+            raise capi.TslamError(worst, msg if rc else "tiled fusion update failed on another rank")
+
+    def update_fused_submaps(self, submaps, include=None, tolerance=0.0, full=False):
+        """Incremental fusion of every rank's submaps into the tiled global map (collective; the tiled counterpart of
+        TsdfHandle.fuse_update).  `submaps` = this rank's submap collection, include / tolerance / full as fuse_update's
+        (include must be the same on every rank); the pose table of every rank's global map holds the poses of all
+        submaps.  Afterwards the union of the ranks' tiles is bit for bit the single-map fuse_update of all submaps.
+        Only a full update with balanced cuts moves the cuts.  Returns fuse_update's statistics summed over the ranks
+        (reason: the same on every rank) plus foreign_blocks_sent / _received and bytes_sent."""
+        import torch
+        from . import _capi as capi
+        dev = torch.device("cuda", torch.cuda.current_device())
+        self.last_exchange = {}
+        width = 3 + 2 * int(self.m._h.cfg.max_submaps)
+        rc, row = _attempt(self.update_plan, submaps, include, tolerance, full)
+        mine = torch.as_tensor(np.concatenate([[rc], row if rc == 0 else np.zeros(width, np.int64)]), dtype=torch.int64, device=dev)
+        parts = [torch.empty_like(mine) for _ in range(self.world)]
+        self.dist.all_gather(parts, mine)
+        rows = torch.stack(parts).cpu().numpy()
+        if np.any(rows[:, 0] != 0):
+            self.update_finish(submaps, False)
+            raise capi.TslamError(int(rows[:, 0].min()), row if rc else "tiled fusion plan failed on another rank")
+        try:
+            reason = merge_fuse_plans(rows[:, 1:])
+        except ValueError:
+            self.update_finish(submaps, False)
+            raise
+        rc, hist = _attempt(self.update_splat, submaps, reason)
+        self._agree(submaps, rc, hist, dev)
+        if hist is not None:
+            ht = torch.as_tensor(hist.astype(np.int64), device=dev)
+            self.dist.all_reduce(ht)
+            self.set_tiling(*balanced_tiling(ht.cpu().numpy(), self.world))
+        rc, packed = _attempt(self.update_pack)
+        self._agree(submaps, rc, packed, dev)
+        send, bufs = packed
+        recv = exchange_counts(self.dist, send, dev)
+        rc, msg = _attempt(self.update_unpack, tuple(exchange_rows(self.dist, b, send, recv) for b in bufs))
+        self._agree(submaps, rc, msg, dev)
+        st = self.update_finish(submaps, True)
+        tot = torch.tensor([st[k] for k in _UPDATE_SUMS], dtype=torch.int64, device=dev)
+        self.dist.all_reduce(tot)
+        st.update(zip(_UPDATE_SUMS, (int(x) for x in tot.cpu().numpy())))
+        return st
 
     # ---- halo + mesh --------------------------------------------------------------------------------------
     def halo_pack(self):
@@ -671,6 +812,45 @@ def run_local_fusion(tiled, submaps):
     routed, _ = _route([p[1] for p in packed], [p[0] for p in packed], world)
     for t, bufs in zip(tiled, routed):
         t.fusion_unpack(bufs)
+
+
+def run_local_update_fused_submaps(tiled, submaps, include=None, tolerance=0.0, full=False):
+    """TiledGlobalMap.update_fused_submaps on `world` virtual ranks in one process: tiled[r] / submaps[r] = rank r's
+    global map wrapper and submap collection, the all-to-all replaced by slicing.  Returns the statistics summed over
+    the ranks."""
+    from . import _capi as capi
+    world = len(tiled)
+    for t in tiled:
+        t.last_exchange = {}
+
+    def agree(res):
+        bad = [(rc, msg) for rc, msg in res if rc]
+        if bad:
+            for t, s in zip(tiled, submaps):
+                t.update_finish(s, False)
+            raise capi.TslamError(min(rc for rc, _ in bad), bad[0][1])
+        return [r for _, r in res]
+
+    rows = agree([_attempt(t.update_plan, s, include, tolerance, full) for t, s in zip(tiled, submaps)])
+    try:
+        reason = merge_fuse_plans(np.stack(rows))
+    except ValueError:
+        for t, s in zip(tiled, submaps):
+            t.update_finish(s, False)
+        raise
+    hists = agree([_attempt(t.update_splat, s, reason) for t, s in zip(tiled, submaps)])
+    if hists[0] is not None:
+        tiles, cuts = balanced_tiling(np.sum([h.astype(np.int64) for h in hists], axis=0), world)
+        for t in tiled:
+            t.set_tiling(tiles, cuts)
+    packed = agree([_attempt(t.update_pack) for t in tiled])
+    routed, _ = _route([p[1] for p in packed], [p[0] for p in packed], world)
+    agree([_attempt(t.update_unpack, b) for t, b in zip(tiled, routed)])
+    stats = [t.update_finish(s, True) for t, s in zip(tiled, submaps)]
+    out = dict(stats[0])
+    for k in _UPDATE_SUMS:
+        out[k] = sum(st[k] for st in stats)
+    return out
 
 
 def run_local_mesh(tiled, meshers, step=1):

@@ -188,19 +188,61 @@ class TsdfHandle:
         afterwards this map is the exact-sum fusion of the included submaps at their fused poses.  include: None (all) or
         bools / 0-1 per submap (up to max_submaps); tolerance: how far (metres, translation + angle x radius) a fused
         submap may move before it is re-splatted; full=True forces a rebuild.  -> dict of the call's statistics."""
-        inc = None
-        if include is not None:
-            n = int(self.cfg.max_submaps)
-            a = np.asarray(include).reshape(-1).astype(bool)
-            assert a.shape[0] <= n, "include has more entries than max_submaps"
-            inc = np.zeros(n, np.uint8)
-            inc[:a.shape[0]] = a
+        inc = self.include_u8(include)
         st = np.zeros(8, np.int64)
         capi.check(self.L.tslam_tsdf_fuse_update(self.h, src.h, capi.np_ptr(inc) if inc is not None else None, float(tolerance),
                                                  int(bool(full)), capi.np_ptr(st), capi.stream_ptr()))
-        return dict(full=bool(st[0] != 0), reason=capi.FUSE_REASONS[int(st[0])], added=int(st[1]), moved=int(st[2]),
-                    removed=int(st[3]), within_tolerance=int(st[4]), voxels_splatted=int(st[5]), voxels_skipped=int(st[6]),
-                    blocks_committed=int(st[7]))
+        return _fuse_stats(st, capi.FUSE_REASONS)
+
+    def include_u8(self, include):
+        """include of the fusion updates (None or bools / 0-1 per submap) -> None or u8[max_submaps]."""
+        if include is None:
+            return None
+        n = int(self.cfg.max_submaps)
+        a = np.asarray(include).reshape(-1).astype(bool)
+        assert a.shape[0] <= n, "include has more entries than max_submaps"
+        inc = np.zeros(n, np.uint8)
+        inc[:a.shape[0]] = a
+        return inc
+
+    # -- incremental fusion of a tiled global map, phase by phase (tslam_tsdf_fuse_update_tiled_*) ------------------
+    # distributed.TiledGlobalMap.update_fused_submaps drives these on every rank; each raises capi.TslamError.
+    def fuse_update_tiled_plan(self, src, tiles, rank, world, include=None, tolerance=0.0, full=False):
+        """-> (plan int64[3] = this rank's full-update reason, cost, cost_full; present bool[max_submaps])."""
+        inc = self.include_u8(include)
+        plan = np.zeros(3, np.int64)
+        present = np.zeros(int(self.cfg.max_submaps), np.uint8)
+        t = (C.c_int32 * 3)(*tiles)
+        capi.check(self.L.tslam_tsdf_fuse_update_tiled_plan(self.h, src.h, t, int(rank), int(world), capi.np_ptr(inc) if inc is not None else None,
+                                                            float(tolerance), int(bool(full)), capi.np_ptr(plan), capi.np_ptr(present),
+                                                            capi.stream_ptr()))
+        return plan, present.astype(bool)
+
+    def fuse_update_tiled_splat(self, src, reason):
+        capi.check(self.L.tslam_tsdf_fuse_update_tiled_splat(self.h, src.h, int(reason), capi.stream_ptr()))
+
+    def fuse_update_tiled_pack(self, tiles, rank, world):
+        """-> (rows per destination rank int32[world], rows int64[n, 1 + planes * 4096] torch CUDA, grouped by destination)."""
+        torch = self.torch
+        t = (C.c_int32 * 3)(*tiles)
+        send = np.zeros(int(world), np.int32)
+        capi.check(self.L.tslam_tsdf_foreign_count(self.h, t, int(rank), int(world), capi.np_ptr(send), capi.stream_ptr()))
+        n = int(send.sum())
+        planes = 6 if self.texture_enabled else 3
+        rows = torch.empty((max(n, 1), 1 + planes * 4096), dtype=torch.int64, device=torch.device("cuda", torch.cuda.current_device()))
+        capi.check(self.L.tslam_tsdf_fuse_update_tiled_pack(self.h, t, int(rank), int(world), capi.np_ptr(send), n, capi.tptr(rows),
+                                                            capi.stream_ptr()))
+        return send, rows[:n]
+
+    def fuse_update_tiled_unpack(self, rows):
+        rows = rows.contiguous()
+        capi.check(self.L.tslam_tsdf_fuse_update_tiled_unpack(self.h, rows.shape[0], capi.tptr(rows), capi.stream_ptr()))
+
+    def fuse_update_tiled_finish(self, src, ok):
+        """-> this rank's statistics (as fuse_update's) when ok, else None."""
+        st = np.zeros(8, np.int64)
+        capi.check(self.L.tslam_tsdf_fuse_update_tiled_finish(self.h, src.h, int(bool(ok)), capi.np_ptr(st), capi.stream_ptr()))
+        return _fuse_stats(st, capi.TILED_FUSE_REASONS) if ok else None
 
     def extract_surface(self, submap, xyz, rgb, count):
         """Append to torch CUDA buffers xyz/rgb f32[cap,3]; count: int32[1] device counter."""
@@ -532,3 +574,8 @@ class TsdfHandle:
         capi.check(self.L.tslam_tsdf_get_march_stats2(self.h, capi.np_ptr(o)))
         return dict(n_segs=int(o[0]), n_items=int(o[1]), n_slow=int(o[2]), n_fallback=int(o[3]), n_generic=int(o[4]),
                     n_verify_bad=int(o[5]), n_seg_guard=int(o[6]))
+
+
+def _fuse_stats(st, reasons):
+    return dict(full=bool(st[0] != 0), reason=reasons[int(st[0])], added=int(st[1]), moved=int(st[2]), removed=int(st[3]),
+                within_tolerance=int(st[4]), voxels_splatted=int(st[5]), voxels_skipped=int(st[6]), blocks_committed=int(st[7]))

@@ -9,7 +9,9 @@ foreign blocks travel in one NCCL all-to-all, the boundary layer is exchanged as
 locally and the triangle soup is all-gathered.  Then the tiled ESDF of the fused map (exchange rounds of boundary-block
 ESDF until no rank sends) and routed ESDF queries (2^20 uniform points per rank, answered by the owning ranks), a
 routed raycast (2^16 rays per rank, 4 m, handed across tile seams; rounds and forwarded rays reported beside the
-time) and one TopoGraphGen run on the tiled map, all ranks in lockstep.
+time) and one TopoGraphGen run on the tiled map, all ranks in lockstep.  Last, the incremental tiled fusion
+(TiledGlobalMap.update_fused_submaps): its first update (a full one), then one submap moved 5 cm (incremental: only
+that submap's integer deltas travel to the tile owners).
 Prints one JSON line on rank 0, with the GPU model and its power limit beside the figures."""
 import json, os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -105,6 +107,18 @@ def main():
     n_nodes = topo.generate_topo_graph(np.array([0.0, 0.0, 1.0]), max_nodes=20)
     torch.cuda.synchronize(); dist.barrier()
     t_topo = time.perf_counter() - t0
+    # incremental tiled fusion: the first update is full, then one submap moves 5 cm
+    t0 = time.perf_counter()
+    tiled.update_fused_submaps(sub)
+    torch.cuda.synchronize(); dist.barrier()
+    t_upd_full = time.perf_counter() - t0
+    a = 0.0
+    glo.set_base_pose_submap(0, np.array([[np.cos(a), -np.sin(a), 0], [np.sin(a), np.cos(a), 0], [0, 0, 1.0]]),
+                             np.array([6.0 * (0 - 3.5) + 0.05, 6.0 * (0 - 3.5), 0.0]))
+    t0 = time.perf_counter()
+    upd = tiled.update_fused_submaps(sub)
+    torch.cuda.synchronize(); dist.barrier()
+    t_upd_move = time.perf_counter() - t0
     esx = torch.tensor([es["blocks_sent"], es["bytes_sent"], int(vq.sum().item())], dtype=torch.float64, device="cuda")
     dist.all_reduce(esx)
     own = torch.tensor([glo.count_active(), sum(sub._h.count_active(s) for s in mine), x["fusion_blocks_sent"], x.get("halo_blocks_sent", 0),
@@ -122,6 +136,8 @@ def main():
                           "query_Gpoints_per_s": world * (1 << 20) / t_query / 1e9, "query_valid": int(esx[2].item()),
                           "raycast_rays_per_rank": 1 << 16, "raycast_ms": 1e3 * t_ray, "raycast_rounds": rq["rounds"],
                           "raycast_rays_forwarded": rq["rays_forwarded"], "topo_ms": 1e3 * t_topo, "topo_nodes": int(n_nodes),
+                          "update_full_ms": 1e3 * t_upd_full, "update_move1_ms": 1e3 * t_upd_move, "update_move1_reason": upd["reason"],
+                          "update_move1_blocks_sent": upd["foreign_blocks_sent"], "update_move1_MB_sent": upd["bytes_sent"] / 1e6,
                           "gpu": torch.cuda.get_device_name(local), "power_limit_W": _power_limit(local)}))
     dist.destroy_process_group()
 

@@ -184,6 +184,37 @@ int tslam_tsdf_fuse(tslam_tsdf_t* dst, tslam_tsdf_t* src, void* stream);
  * Synchronises with `stream`. */
 int tslam_tsdf_fuse_update(tslam_tsdf_t* dst, tslam_tsdf_t* src, const uint8_t* include, float tolerance, int32_t full,
                            int64_t* stats8, void* stream);
+/* Reclaim pool blocks (DESIGN.md section 7, "Reclaiming pool blocks"): drop blocks and compact the pool in place.
+ * Queued frames are integrated and pending sums committed first.  A block is a candidate when submaps[s] != 0 for its
+ * submap s (submaps: host, max_submaps bytes; NULL = every submap).  A candidate is dropped when
+ *   TSLAM_RECLAIM_ALL is set, or
+ *   TSLAM_RECLAIM_EMPTY is set and the block is empty: no voxel has obs != 0, no commit is pending for it, and, on a
+ *     fusion destination whose sums are valid, every sum word of the block is zero (obs 0 with a non-zero sum is kept), or
+ *   TSLAM_RECLAIM_OUTSIDE is set and the block lies outside the sphere (center3, radius): with the voxel positions
+ *     p = (double)((float)i * vs) of the frame the map stores the submap in (the map frame of a global map; the submap's
+ *     own frame, before its base pose, in a collection), the block (b, voxels 16 b .. 16 b + 15 per axis) is outside iff
+ *     (d_x^2 + d_y^2) + d_z^2 > radius^2 in f64, d = c - clamp(c, p(16 b), p(16 b + 15)) per axis.  A block that touches
+ *     the sphere exactly is kept.
+ * Compaction: n_keep = kept blocks.  Holes (dropped slots below n_keep) and movers (kept slots at or above n_keep) are
+ * paired in ascending order, and the k-th mover moves to the k-th hole with every per-block state: key, acc, tw, obs,
+ * occ, colour word and colour, ESDF, dirty flags, commit stamp and the fusion sum planes.  Kept blocks below n_keep stay
+ * put.  [n_keep, n_old) of every plane is zeroed, n_blocks = n_keep, and the hash table is rebuilt from the kept keys
+ * (keys that failed on a full pool can allocate again).  When a block was dropped, the next tslam_mesh_update and ESDF
+ * update are full ones, and every submap that lost a non-empty block counts as written for tslam_tsdf_fuse_update
+ * (dropping empty blocks does not; an EMPTY reclaim of a fusion destination keeps its next update incremental).  When
+ * nothing is dropped, nothing is moved or invalidated.
+ * stats6 (host, may be NULL): blocks before, candidates, dropped, dropped non-empty, moved, blocks after.
+ * Refused (TSLAM_E_INVALID, nothing written, before the handle is read): rules 0 or with unknown bits; with OUTSIDE a
+ * radius that is negative or not finite, or a NULL or non-finite centre; a NULL handle.  Then: a tiled map (tile cuts
+ * set, or ghost blocks), an open tiled ESDF exchange, a tiled fusion update in progress.  Synchronises with `stream`. */
+#define TSLAM_RECLAIM_ALL 1
+#define TSLAM_RECLAIM_EMPTY 2
+#define TSLAM_RECLAIM_OUTSIDE 4
+int tslam_tsdf_reclaim(tslam_tsdf_t* m, int32_t rules, const uint8_t* submaps, const double* center3, double radius,
+                       int64_t* stats6, void* stream);
+/* The pool in slot order: keys4 (DEVICE int32[cap, 4]) row b = (submap, bx, by, bz) of pool block b, b < n_blocks.
+ * Pending work is flushed first.  *n_out = n_blocks; TSLAM_E_CAPACITY (rows saturated) when it exceeds cap.  Synchronises. */
+int tslam_tsdf_block_keys(tslam_tsdf_t* m, int64_t cap, int32_t* keys4, int64_t* n_out, void* stream);
 /* cvt_TSDF_surface_to_voxels_kernel (dense_tsdf.py:339-365): append |TSDF|<1.8*vs
  * voxels of `submap` to xyz/rgb f32[cap,3] (DEVICE) starting at *count_dev (DEVICE
  * int32 counter, incremented; entries beyond cap are counted but not written). */

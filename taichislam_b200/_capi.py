@@ -22,6 +22,7 @@ RENDER_MAX_SAMPLES = 65536
 ABI_VERSION = 6
 FUSE_REASONS = ("incremental", "first call", "full requested", "other source", "destination written", "content changed",
                 "cheaper than subtract and re-add")
+RECLAIM_ALL, RECLAIM_EMPTY, RECLAIM_OUTSIDE = 1, 2, 4
 TILED_FUSE_REASONS = FUSE_REASONS + ("tile cuts changed", "sums not valid")  # tslam_tsdf_fuse_update_tiled_*
 
 
@@ -200,6 +201,8 @@ SIGNATURES = {
     "tslam_tsdf_place_describe": (C.c_int, [_vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "tslam_place_match": (C.c_int, [_i32, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _i32, _i64, _i64, _vp, _vp, _vp]),
     "tslam_tsdf_fuse_update": (C.c_int, [_vp, _vp, _vp, _f32, _i32, _vp, _vp]),
+    "tslam_tsdf_reclaim": (C.c_int, [_vp, _i32, _vp, _vp, C.c_double, _vp, _vp]),
+    "tslam_tsdf_block_keys": (C.c_int, [_vp, _i64, _vp, C.POINTER(_i64), _vp]),
     "tslam_tsdf_fuse_update_tiled_plan": (C.c_int, [_vp, _vp, _vp, _i32, _i32, _vp, _f32, _i32, _vp, _vp, _vp]),
     "tslam_tsdf_fuse_update_tiled_splat": (C.c_int, [_vp, _vp, _i32, _vp]),
     "tslam_tsdf_fuse_update_tiled_pack": (C.c_int, [_vp, _vp, _i32, _i32, _vp, _i64, _vp, _vp]),

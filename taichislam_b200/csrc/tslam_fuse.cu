@@ -121,6 +121,17 @@ void ts_fuse_free(tslam_tsdf* m) {
   }
 }
 
+TsFuseView ts_fuse_view(tslam_tsdf* m) {
+  TsFuseView v = {nullptr, 0, m->g.col ? 6 : 3, 0, 0};
+  if (m->fz) {
+    v.sums = (long long*)m->fz->sums;
+    v.cap_blocks = v.sums ? m->fz->cap_blocks : 0;
+    v.valid = m->fz->valid;
+    v.phase = m->fz->phase;
+  }
+  return v;
+}
+
 void ts_map_written(tslam_tsdf* m, int submap) {
   m->write_gen++;
   if (!m->content_ver) return;

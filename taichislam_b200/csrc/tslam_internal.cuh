@@ -170,6 +170,19 @@ __device__ __forceinline__ int ts_get_or_alloc(const G& g, unsigned long long ke
   return -1;
 }
 
+// Insert `key` at pool slot `slot` into a table that does not hold it: the rebuild of the table after a compaction of
+// the pool (tslam_reclaim.cu), between launches, so ts_get_or_alloc_cached's L1 argument still holds.  False when the
+// table is full.
+template <class G>
+__device__ __forceinline__ bool ts_insert_slot(const G& g, unsigned long long key, int slot) {
+  uint32_t h = ts_hash(key) & g.table_mask;
+  for (uint32_t probe = 0; probe <= g.table_mask; ++probe) {
+    if (atomicCAS(&g.table[h], TS_EMPTY, (key << 24) | (unsigned long long)slot) == TS_EMPTY) return true;
+    h = (h + 1) & g.table_mask;
+  }
+  return false;
+}
+
 // Touched blocks are flagged with a fire-and-forget store (no load on the ray-march critical
 // path); k_collect_dirty compacts the flags into dirty_list before a commit.
 __device__ __forceinline__ void ts_mark_dirty(const TsGrid& g, int blk) { g.dirty_flag[blk] = 1; }
@@ -633,6 +646,8 @@ struct tslam_tsdf {
   size_t render_jobs_bytes;
   void* traj_mem;      // inputs, outputs and solver work of tslam_esdf_trajectory (tslam_traj.cuh), grown geometrically
   size_t traj_mem_bytes;
+  void* rc_mem;        // keep flags, scan, hole / mover lists and counters of tslam_tsdf_reclaim (tslam_reclaim.cu), grown geometrically
+  size_t rc_bytes;
   // Change tracking of the incremental global fusion (tslam_tsdf_fuse_update, tslam_fuse.cu).  Every entry that writes a
   // submap's planes calls ts_map_written, which bumps that submap's content version and the map's write generation;
   // the update compares both against what it recorded when it last ran.
@@ -957,6 +972,15 @@ int ts_integrate_depth_impl(tslam_tsdf_t* m, const uint16_t* depth, int mem, int
 int ts_fuse_init(tslam_tsdf* m);                         // at create: serial and content versions
 void ts_fuse_free(tslam_tsdf* m);                        // at destroy
 void ts_map_written(tslam_tsdf* m, int submap);          // submap's planes were written (submap < 0: every submap)
+// the fusion sum planes of m as a destination (tslam_reclaim.cu moves them with their blocks): sums = null when none
+struct TsFuseView {
+  long long* sums;    // planes x cap_blocks x 4096 int64, plane after plane
+  size_t cap_blocks;  // pool blocks the planes cover
+  int planes;         // 3, or 6 on textured maps
+  int valid;          // the sums describe the map (the last update completed)
+  int phase;          // phase of a tiled update in progress, 0 none
+};
+TsFuseView ts_fuse_view(tslam_tsdf* m);
 // tslam_integrate.cu: k_collect_dirty on st (dirty_flag -> dirty_list, n_dirty)
 int ts_collect_dirty(tslam_tsdf* m, cudaStream_t st, unsigned long long* prof = nullptr);
 // tslam_register.cu: *p holds at least `need` bytes: reallocated (contents dropped) to max(need, 2 x the old size) when smaller

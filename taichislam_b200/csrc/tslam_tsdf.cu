@@ -264,6 +264,7 @@ extern "C" int tslam_tsdf_destroy(tslam_tsdf_t* m) {
   if (m->reg_pts) cudaFree(m->reg_pts);
   if (m->render_jobs) cudaFree(m->render_jobs);
   if (m->traj_mem) cudaFree(m->traj_mem);
+  if (m->rc_mem) cudaFree(m->rc_mem);
   if (g.cword) cudaFree(g.cword);
   if (g.col) cudaFree(g.col);
   if (m->tex_stage) cudaFree(m->tex_stage);

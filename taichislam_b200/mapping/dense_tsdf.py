@@ -194,6 +194,14 @@ class DenseTSDF(BaseMap):
         submaps._flush()
         return self._h.fuse_update(submaps._h, include=include, tolerance=tolerance, full=full)
 
+    def reclaim(self, submaps=None, all_blocks=False, empty=False, center=None, radius=None):
+        """Give pool blocks back (TsdfHandle.reclaim): the blocks of `submaps` (None: all) that all_blocks, empty (no
+        observed voxel) or the sphere (center, radius) select are dropped and the pool is compacted.  `center` is in
+        the frame this map stores its submaps in (the map frame of a global map, a submap's own frame before its base
+        pose).  Queued frames are integrated first.  -> dict of the call's statistics."""
+        self._flush()
+        return self._h.reclaim(submaps=submaps, all_blocks=all_blocks, empty=empty, center=center, radius=radius)
+
     # ------------------------------------------------------------------ exporters (:320-389)
     def _active(self):
         return 0 if self.is_global_map else self.active_submap_id[None]

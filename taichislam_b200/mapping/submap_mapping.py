@@ -14,6 +14,8 @@ set_frame_poses and input_remote_submap refresh the global map (its mesh and the
 submap is left out of the global map in that mode: the reference fuses at the switch, when the active submap is
 empty, and its global-mode exporters add the active submap separately.  One deviation: when a remote submap arrives
 in the middle of a submap, the reference's rebuild also fuses the local active submap; the incremental mode does not.
+reclaim_empty=True (incremental mode only) gives the global map's blocks that a move or removal left empty back to the
+pool after each such update, so loop closures do not grow the global map.
 """
 import io
 import time
@@ -37,14 +39,18 @@ _COMMON = dict(voxel_scale=0.05, texture_enabled=False, min_ray_length=0.3, max_
 
 class SubmapMapping:
     def __init__(self, submap_type=DenseTSDF, keyframe_step=20, sub_opts={}, global_opts={}, autosave_path=None,
-                 global_fusion="rebuild", fusion_tolerance=0.0):
+                 global_fusion="rebuild", fusion_tolerance=0.0, reclaim_empty=False):
         if global_fusion not in ("rebuild", "incremental"):
             raise ValueError(f"global_fusion must be 'rebuild' or 'incremental', not {global_fusion!r}")
         if global_fusion == "incremental" and submap_type is not DenseTSDF:
             raise ValueError("global_fusion='incremental' needs TSDF submaps")
+        if reclaim_empty and global_fusion != "incremental":
+            raise ValueError("reclaim_empty needs global_fusion='incremental' (a rebuild resets the global map anyway)")
         self.global_fusion = global_fusion
         self.fusion_tolerance = float(fusion_tolerance)
+        self.reclaim_empty = bool(reclaim_empty)
         self.last_fusion_stats = None  # statistics of the last incremental update
+        self.last_reclaim_stats = None  # statistics of the last reclaim of the global map (reclaim_empty)
         self.submap_type = submap_type
         self.keyframe_step = keyframe_step
         self.autosave_path = autosave_path
@@ -204,7 +210,11 @@ class SubmapMapping:
             sc = self.submap_collection
             include = np.ones(sc.max_submap_num, bool)
             include[sc.get_active_submap_id()] = False  # the growing submap is exported separately (see above)
-            self.last_fusion_stats = self.global_map.update_fused_submaps(sc, include=include, tolerance=self.fusion_tolerance)
+            st = self.global_map.update_fused_submaps(sc, include=include, tolerance=self.fusion_tolerance)
+            self.last_fusion_stats = st
+            if self.reclaim_empty and (st["moved"] > 0 or st["removed"] > 0):
+                # blocks the old poses covered are left empty by the subtraction: give them back to the pool
+                self.last_reclaim_stats = self.global_map.reclaim(empty=True)
         else:
             self.global_map.fuse_submaps(self.submap_collection)
         if self.post_local_to_global_callback is not None:

@@ -194,6 +194,51 @@ class TsdfHandle:
                                                  int(bool(full)), capi.np_ptr(st), capi.stream_ptr()))
         return _fuse_stats(st, capi.FUSE_REASONS)
 
+    def reclaim(self, submaps=None, all_blocks=False, empty=False, center=None, radius=None):
+        """Drop pool blocks and compact the pool in place (tslam_tsdf_reclaim).  Candidates are the blocks of `submaps`
+        (None: every submap; else ids or bools / 0-1 per submap); a candidate is dropped when all_blocks, when empty and
+        it holds no observed voxel, or when center / radius are given and it lies outside that sphere (metres, in the
+        frame the map stores its submaps in).  -> dict of the call's statistics."""
+        rules = (capi.RECLAIM_ALL if all_blocks else 0) | (capi.RECLAIM_EMPTY if empty else 0)
+        c = None
+        if center is not None or radius is not None:
+            assert center is not None and radius is not None, "OUTSIDE needs both center and radius"
+            rules |= capi.RECLAIM_OUTSIDE
+            c = np.ascontiguousarray(np.asarray(center, np.float64).reshape(3))
+        mask = self.submap_mask_u8(submaps)
+        st = np.zeros(6, np.int64)
+        capi.check(self.L.tslam_tsdf_reclaim(self.h, rules, capi.np_ptr(mask) if mask is not None else None,
+                                             capi.np_ptr(c) if c is not None else None, float(radius) if c is not None else 0.0,
+                                             capi.np_ptr(st), capi.stream_ptr()))
+        return dict(blocks_before=int(st[0]), candidates=int(st[1]), dropped=int(st[2]), dropped_nonempty=int(st[3]),
+                    moved=int(st[4]), blocks_after=int(st[5]))
+
+    def submap_mask_u8(self, submaps):
+        """None, submap ids, or bools / 0-1 per submap -> None or u8[max_submaps]."""
+        if submaps is None:
+            return None
+        a = np.asarray(submaps).reshape(-1)
+        if a.dtype == bool:
+            return self.include_u8(a)
+        n = int(self.cfg.max_submaps)
+        ids = a.astype(np.int64)
+        assert np.all((ids >= 0) & (ids < n)), "submap id out of range"
+        mask = np.zeros(n, np.uint8)
+        mask[ids] = 1
+        return mask
+
+    def block_keys(self):
+        """The pool in slot order: int32[n_blocks, 4] rows (submap, bx, by, bz)."""
+        torch = self.torch
+        n = C.c_int64(0)
+        rc = self.L.tslam_tsdf_block_keys(self.h, 0, None, C.byref(n), capi.stream_ptr())  # the count
+        if rc != capi.E_CAPACITY:
+            capi.check(rc)
+        cap = int(n.value)
+        keys = torch.empty((max(cap, 1), 4), dtype=torch.int32, device=torch.device("cuda", torch.cuda.current_device()))
+        capi.check(self.L.tslam_tsdf_block_keys(self.h, cap, capi.tptr(keys), C.byref(n), capi.stream_ptr()))
+        return keys[:cap].cpu().numpy()
+
     def include_u8(self, include):
         """include of the fusion updates (None or bools / 0-1 per submap) -> None or u8[max_submaps]."""
         if include is None:

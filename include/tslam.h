@@ -528,6 +528,51 @@ int tslam_octo_extract(tslam_octo_t* m, int32_t submap, int32_t level, int64_t c
                        void* stream);
 /* fuse_submaps_kernel (taichi_octomap.py:171-189) after reset(). */
 int tslam_octo_fuse(tslam_octo_t* dst, tslam_octo_t* src, void* stream);
+/* Incremental fusion of the submaps of `src` into the Octomap global map `dst` (DESIGN.md section 7, "Incremental
+ * Octomap fusion"), hit counters and log-odds maps alike: an opt-in alternative to tslam_octo_fuse that re-places only
+ * the submaps a call added, moved or removed.
+ * Result: after the call every voxel word (cnt plane) and colour word of dst is bit for bit what tslam_octo_fuse gives
+ * when src holds only the submaps s with include[s] != 0 (include: host, max_submaps bytes; NULL = all), each at its
+ * fused pose, with k_octo_fuse's placement and dst's rule (hit threshold / l_occ).  Pool order may differ (it does
+ * between two tslam_octo_fuse calls too): compare sorted gathered rows (ijk, word, colour).  An allocated block whose
+ * words are all zero (left so by removals) reads like an absent one to every reader: gather, extract, queries, raycast,
+ * the occupancy ESDF and the frontiers.
+ * Fused pose of s: dst's pose-table row of s, unless s was fused before with the same content and
+ * |T - T0| + angle(R0^T R) * r_s <= tolerance (r_s: farthest allocated 8^3 block corner of s from its origin; tolerance 0:
+ * iff the pose bits are unchanged) - tslam_tsdf_fuse_update's rule.  The result does not depend on the history of calls.
+ * Hit counter: dst.cnt = u32 sum (mod 2^32) of c over contributing source voxels (c > min_occupy_thres); removals
+ * subtract in the cnt plane, exact under wrapping.
+ * Log-odds: one int64 sum word per voxel, count * 2^32 + sum L (4 KB per 8^3 block, grown geometrically with the pool
+ * blocks in use, log-odds dst only); a touched voxel reads count > 0 ? lo_word(clamp(sum L, l_min, l_max)) : 0.
+ * Bound: a rigid placement puts at most 27 source voxels into one dst cell (27 sub-cubes of side vs / 3, plus f32
+ * rounding, each of diameter < vs), so a cell takes at most 27 * max_submaps contributions and |sum L| <= 27 *
+ * max_submaps * max(|l_min|, l_max) of src; the call refuses maps where that reaches 2^30 (OctoMap's defaults with 1024
+ * submaps: 27 * 1024 * 3595 < 2^27).  Then count and sum L fit their 32-bit halves, and the readout equals
+ * k_octo_fuse's: its wrapped u32 sum of L << 1 is 2 sum L exactly (|2 sum L| < 2^31, low bit 0), the OR'd known bit
+ * makes it lo_word(sum L), and k_octo_lo_clamp clamps it once, as the readout does.
+ * Colour (textured maps): additions raise colour words with a max, as k_octo_fuse does; every dst block a removal (or
+ * the old pose of a move) touches has its colour words cleared and raised again from the included submaps at their
+ * fused poses that can reach it (host filter on each submap's placed bounding sphere).
+ * Plan: unchanged or moved within tolerance: nothing; newly included: add; excluded or now empty: subtract; moved:
+ * subtract then add.  A full update (reset dst, then add every included submap) runs on the first call, when full != 0,
+ * for another src, after any other write of dst (integrate, reset, tslam_octo_fuse into it), when a fused submap's
+ * content changed (integrate into it, reset or tslam_octo_fuse of src), and when subtracting and re-adding would place
+ * more source blocks than a rebuild; both paths give the same bits.
+ * Trackers: an incremental update flags every dst block it touched for the next occupancy-ESDF and frontier update
+ * (which stay incremental, and readable as of their last update); a full update resets dst and so invalidates them.
+ * stats8 (may be NULL; tslam_tsdf_fuse_update's layout): full-update reason (0 incremental, 1 first call, 2 full
+ * requested, 3 other src, 4 dst written, 5 content changed, 6 cheaper than subtract and re-add), submaps added, moved,
+ * removed, left within tolerance, source voxels placed (adds + subtracts), voxels recoloured, dst blocks committed.
+ * Refused (TSLAM_E_INVALID, nothing written), before the handles are looked at: tolerance not finite or < 0, a NULL
+ * handle, dst == src; then maps that differ in occupancy model, max_submaps, voxel size or texture setting, and the
+ * log-odds bound above.  N / Nz may differ (a large global map of small submaps): placement tests only dst's bounds, as
+ * tslam_octo_fuse does.  An error flag of earlier work on dst is reported first.  TSLAM_E_POOL_FULL when dst's pool runs
+ * out, with nothing added: an incremental update returns before any sum or word changes (dst as before the call); a
+ * full update has already reset dst, which comes back empty.  Either way the next call is a full update.  TSLAM_E_CUDA
+ * when the sums cannot grow; a removal that finds no dst block is reported as TSLAM_E_INVALID and makes the next call
+ * full.  Synchronises. */
+int tslam_octo_fuse_update(tslam_octo_t* dst, tslam_octo_t* src, const uint8_t* include, float tolerance, int32_t full,
+                           int64_t* stats8, void* stream);
 /* Octomap.is_occupy (taichi_octomap.py:86-88: occupy > min_occupy_thres) for points, and BaseMap.raycast. */
 int tslam_octo_query_points(tslam_octo_t* m, int32_t submap, int64_t n, const float* xyz, uint8_t* flags, void* stream);
 int tslam_octo_raycast(tslam_octo_t* m, int32_t submap, int64_t n, const float* pos, const float* dir, float max_dist, uint8_t* hit,

@@ -163,6 +163,7 @@ SIGNATURES = {
     "tslam_octo_gather": (C.c_int, [_vp, _i32, _i64, _vp, _vp, C.POINTER(_i64), _vp]),
     "tslam_octo_extract": (C.c_int, [_vp, _i32, _i32, _i64, _vp, _vp, _vp]),
     "tslam_octo_fuse": (C.c_int, [_vp, _vp, _vp]),
+    "tslam_octo_fuse_update": (C.c_int, [_vp, _vp, _vp, _f32, _i32, _vp, _vp]),
     "tslam_octo_set_color_intrinsics": (C.c_int, [_vp, C.c_double, C.c_double, C.c_double, C.c_double, C.c_int]),
     "tslam_octo_integrate_points_rgb": (C.c_int, [_vp, _vp, _vp, C.c_int, _i32, _vp, _vp, _i32, _vp]),
     "tslam_octo_integrate_depth_tex": (C.c_int, [_vp, _vp, _vp, C.c_int, _i32, _i32, _i32, _i32, _vp, _vp, _i32, _vp]),

@@ -33,21 +33,12 @@
 #include <cstring>
 #include <vector>
 #include "tslam_internal.cuh"
+#include "tslam_fuse_plan.cuh"
 
 #define FZ_Q 16777216.0             // 2^24: quantum of the sums
 #define FZ_FMAX 8388608.0f          // 2^23: terms at or above this magnitude are skipped
 #define TS_ERR_FUSE_MISSING 16      // g.err: a removal found no dst block (the sums and the pool disagree)
 
-// full-update reasons (stats8[0]; 0 = incremental)
-// 7, 8: tiled updates only (tslam_tsdf_fuse_update_tiled_*)
-enum { FZ_INCR = 0, FZ_FIRST = 1, FZ_ASKED = 2, FZ_OTHER_SRC = 3, FZ_DST_WRITTEN = 4, FZ_CONTENT = 5, FZ_COST = 6, FZ_CUTS = 7,
-       FZ_INVALID = 8 };
-enum { FZ_NONE = 0, FZ_ADD, FZ_REMOVE, FZ_MOVE, FZ_KEEP };  // what an update does with a submap
-
-struct FzJob {        // one placement of one submap: sign +1 adds, -1 removes
-  float R[9], T[3];
-  int sign, pad;
-};
 struct FzSums {       // sum planes, [cap blocks * 4096] int64 each
   long long* wt;      // S_wT
   long long* w;       // S_w
@@ -65,21 +56,6 @@ struct FzDev {        // device scratch of one update (TsFuse::dev)
                             // [5] voxels whose count decodes as negative (tiled updates)
 };
 
-struct FzSub {        // what a submap contributes to dst (TsFuse::sub)
-  int fused;          // 1: its voxels are in the sums, at (R, T)
-  float R[9], T[3];
-  unsigned long long ver;  // src content version at that time
-  int nblk;           // its non-ghost source blocks then
-};
-struct FzPlan {        // one update, from its plan to its record
-  int reason;         // FZ_*
-  bool full;
-  std::vector<unsigned char> want, act;  // per submap: included with source blocks; FZ_NONE .. FZ_KEEP
-  std::vector<int> nblk;
-  std::vector<float> rad, pR, pT;        // radius, dst pose table
-  long long n_add, n_move, n_remove, n_tol, cost, cost_full;  // cost: source blocks an incremental update splats
-  unsigned long long ghosts;             // dst ghost blocks
-};
 struct TsFuse {
   int valid;          // the sums describe dst (cleared by a failed update)
   unsigned long long src_serial, gen;  // src handle and dst write generation of the last update (tiled: write_gen - ghost_gen)
@@ -101,8 +77,10 @@ struct TsFuse {
 
 static unsigned long long g_serial = 0;  // handle numbers (create is not called concurrently with itself here)
 
+unsigned long long ts_next_serial() { return __atomic_add_fetch(&g_serial, 1ull, __ATOMIC_RELAXED); }
+
 int ts_fuse_init(tslam_tsdf* m) {
-  m->serial = __atomic_add_fetch(&g_serial, 1ull, __ATOMIC_RELAXED);
+  m->serial = ts_next_serial();
   m->write_gen = 0;
   m->ghost_gen = 0;
   m->content_ver = new unsigned long long[m->cfg.max_submaps]();
@@ -463,16 +441,6 @@ static TsTiling* fz_dev_tiling(TsFuse* z) {
   return (TsTiling*)((char*)z->dev + 8 * 8 + 2 * S * sizeof(FzJob) + S * (8 + 4 + 4) + (size_t)z->dev_blocks * 4);
 }
 
-// rotation angle of R0^T R (row-major 3x3), in double
-static double fz_angle(const float* R0, const float* R) {
-  double tr = 0.0;
-  for (int i = 0; i < 3; i++)
-    for (int k = 0; k < 3; k++) tr += (double)R0[3 * k + i] * (double)R[3 * k + i];  // trace(R0^T R) = sum R0_ki R_ki
-  double c = (tr - 1.0) * 0.5;
-  c = c > 1.0 ? 1.0 : (c < -1.0 ? -1.0 : c);
-  return std::acos(c);
-}
-
 // Refusals that need no handle contents (TSLAM_E_INVALID, nothing written)
 static int fz_check_args(tslam_tsdf* dst, tslam_tsdf* src, float tolerance) {
   if (!std::isfinite(tolerance) || tolerance < 0.0f) { ts_set_error("fuse_update: tolerance %g must be finite and >= 0", (double)tolerance); return TSLAM_E_INVALID; }
@@ -534,51 +502,8 @@ static int fz_plan(tslam_tsdf* dst, tslam_tsdf* src, const uint8_t* include, flo
   TS_CUDA(cudaStreamSynchronize(st));
   P.ghosts = ctr0[3];
 
-  P.want.assign(S, 0);
-  P.act.assign(S, FZ_NONE);
-  P.n_add = P.n_move = P.n_remove = P.n_tol = P.cost = P.cost_full = 0;
-  const std::vector<int>& nblk = P.nblk;
-  for (int s = 0; s < S; s++) {
-    const bool want = (!include || include[s]) && nblk[s] > 0;
-    P.want[s] = want;
-    if (want) P.cost_full += nblk[s];
-    if (reason != FZ_INCR) continue;
-    const FzSub& r = z->sub[s];
-    if (!r.fused) {
-      if (want) { P.act[s] = FZ_ADD; P.cost += nblk[s]; }
-      continue;
-    }
-    if (r.ver != src->content_ver[s]) { reason = FZ_CONTENT; continue; }  // its old content is gone: cannot be subtracted
-    if (!want) { P.act[s] = FZ_REMOVE; P.cost += r.nblk; continue; }
-    const float* R = &P.pR[(size_t)9 * s];
-    const float* T = &P.pT[(size_t)3 * s];
-    if (!memcmp(R, r.R, 36) && !memcmp(T, r.T, 12)) { P.act[s] = FZ_KEEP; continue; }
-    if (tolerance > 0.0f) {
-      const double dx = (double)T[0] - r.T[0], dy = (double)T[1] - r.T[1], dz = (double)T[2] - r.T[2];
-      const double move = std::sqrt(dx * dx + dy * dy + dz * dz) + fz_angle(r.R, R) * (double)P.rad[s];
-      if (move <= (double)tolerance) { P.act[s] = FZ_KEEP; P.n_tol++; continue; }
-    }
-    P.act[s] = FZ_MOVE;
-    P.cost += r.nblk + nblk[s];
-  }
-  P.reason = reason;
+  fz_decide(P, z->sub, src->content_ver, include, tolerance, reason);
   return TSLAM_OK;
-}
-
-// the update's final reason: a full update adds every included submap
-static void fz_settle(FzPlan& P, int reason) {
-  P.reason = reason;
-  P.full = reason != FZ_INCR;
-  if (P.full) {
-    P.n_tol = 0;
-    for (size_t s = 0; s < P.act.size(); s++) P.act[s] = P.want[s] ? FZ_ADD : FZ_NONE;
-  }
-  P.n_add = P.n_move = P.n_remove = 0;
-  for (size_t s = 0; s < P.act.size(); s++) {
-    P.n_add += P.act[s] == FZ_ADD;
-    P.n_move += P.act[s] == FZ_MOVE;
-    P.n_remove += P.act[s] == FZ_REMOVE;
-  }
 }
 
 // Splat the plan into the sums: a full update resets dst and zeroes the sums first.  Tiled (t: the tiling, else null):
@@ -684,18 +609,7 @@ static int fz_commit(tslam_tsdf* dst, const FzDev& f, bool check_negative, cudaS
 // the submaps' new state after a successful update
 static void fz_record(tslam_tsdf* dst, tslam_tsdf* src, const FzPlan& P) {
   TsFuse* z = dst->fz;
-  for (int s = 0; s < dst->cfg.max_submaps; s++) {
-    FzSub& r = z->sub[s];
-    if (P.full) r.fused = 0;
-    if (P.act[s] == FZ_REMOVE) r.fused = 0;
-    if (P.act[s] == FZ_ADD || P.act[s] == FZ_MOVE) {
-      r.fused = 1;
-      memcpy(r.R, &P.pR[(size_t)9 * s], 36);
-      memcpy(r.T, &P.pT[(size_t)3 * s], 12);
-      r.ver = src->content_ver[s];
-      r.nblk = P.nblk[s];
-    }
-  }
+  fz_record_subs(z->sub, P, src->content_ver);
   // voxels that lose their last contribution become unobserved, which the incremental ESDF does not undo
   if (P.n_remove + P.n_move > 0) dst->esdf_full_needed = 1;
   z->valid = 1;

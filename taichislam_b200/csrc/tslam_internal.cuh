@@ -690,6 +690,15 @@ struct OcGrid {
 __device__ __forceinline__ int oc_voxel_off(int i, int j, int k) {
   return (((i & OC_BMASK) << OC_BSHIFT) | (j & OC_BMASK)) << OC_BSHIFT | (k & OC_BMASK);
 }
+// Placement of source voxel v of block (bx, by, bz) of a submap at pose (R, T) by the Octomap fusions (k_octo_fuse and
+// the incremental update, tslam_octo_fuse.cu; taichi_octomap.py:182-186): x = R (i vs, j vs, k vs) + T lands in the
+// nearest dst cell (int)roundf(x / vs) per axis.  Both call this one helper, so they place every voxel alike.
+__device__ __forceinline__ void oc_fuse_cell(const float* R, const float* T, int bx, int by, int bz, int v, float vs, int& i, int& j,
+                                             int& k) {
+  float x, y, z;
+  pose_apply(R, T, (float)(bx * OC_B + (v >> 6)) * vs, (float)(by * OC_B + ((v >> 3) & 7)) * vs, (float)(bz * OC_B + (v & 7)) * vs, x, y, z);
+  i = (int)roundf(x / vs); j = (int)roundf(y / vs); k = (int)roundf(z / vs);
+}
 // Log-odds occupancy (tslam_octo_create_logodds, DESIGN.md section 7): the cnt plane holds w = (L << 1) | 1 for a
 // known voxel and 0 for an unknown one, so a zeroed block reads unknown.  L is Q10 fixed point, clamped to
 // [l_min, l_max] after every update.
@@ -747,7 +756,9 @@ struct OcLo {             // per-frame workspace of a log-odds map (allocated in
   int l_hit, l_miss, l_min, l_max, l_occ;
 };
 // What a tracker of a log-odds map (occupancy ESDF, frontiers, travel-cost fields) kept can be read for `submap` iff an
-// update for that submap has completed and no reset, fusion or failed update came after it (oc_track_readable).
+// update for that submap has completed and no reset, fusion (tslam_octo_fuse, or a full tslam_octo_fuse_update) or
+// failed update came after it (oc_track_readable).  Integration and an incremental tslam_octo_fuse_update leave it
+// readable: readers answer as of their last update, and both flag the blocks they change for the next incremental one.
 struct OcTrack {
   int ready;   // set when an update completes; cleared when one begins, and by reset and fusion (oc_track_invalidate_all)
   int submap;  // submap of that update
@@ -804,8 +815,16 @@ struct tslam_octo {
   // inputs, outputs and solver work of tslam_octo_esdf_trajectory (tslam_traj.cuh), grown geometrically
   void* traj_mem;
   size_t traj_mem_bytes;
+  // change tracking of the incremental Octomap fusion (tslam_octo_fuse_update, tslam_octo_fuse.cu)
+  unsigned long long serial;        // process-unique handle number
+  unsigned long long write_gen;     // writes of the map by any entry other than tslam_octo_fuse_update
+  unsigned long long* content_ver;  // [max_submaps] host: writes of each submap's voxels
+  struct OcFuse* ofz;               // state of this map as a fusion destination; NULL until its first update
 };
 int oc_esdf_free(tslam_octo* m);      // tslam_octo_esdf.cu
+// tslam_octo_fuse.cu: submap's voxels were written (submap < 0: every submap); free the fusion state at destroy
+void oc_map_written(tslam_octo* m, int submap);
+void oc_fuse_free(tslam_octo* m);
 int oc_frontier_free(tslam_octo* m);  // tslam_octo_frontier.cu
 int oc_view_free(tslam_octo* m);      // tslam_octo_view.cu
 int oc_travel_free(tslam_octo* m);    // tslam_octo_travel.cu
@@ -843,6 +862,7 @@ int oc_frontier_records(tslam_octo* m, int64_t* rec16, cudaStream_t st);
 #define OC_ERR_VIEW_WINDOW 16  // g.err: a viewpoint-gain walk left its view's bitmap window (tslam_octo_view.cu)
 #define OC_ERR_TRAVEL_PATH 32  // g.err: a travel path found no predecessor (impossible at the field's fixed point; tslam_octo_travel.cu)
 #define OC_ERR_TRAVEL_SOURCE 64  // g.err: a many-source travel path named a source outside [0, S) (tslam_octo_travel.cu)
+#define OC_ERR_FUSE_MISSING 128  // g.err: a removal of tslam_octo_fuse_update found no dst block (tslam_octo_fuse.cu)
 
 // Amanatides-Woo traversal of the log-odds map in voxel units (DESIGN.md section 7, "Traversal"): p0 = origin / vs,
 // p1 = endpoint / vs, cells c = round_half_away(p).  The k-th boundary crossing of axis a is at
@@ -1011,6 +1031,9 @@ int ts_march_launch(tslam_tsdf* m, cudaStream_t st, const TsBatch& batch, uint32
 int oc_logodds_submap(tslam_octo* m, int32_t submap, const char* what, const char* feature);
 // the state kept in t can be read for `submap` (see OcTrack); `update` names the entry point that computes it
 int oc_track_readable(tslam_octo* m, const OcTrack& t, int32_t submap, const char* what, const char* update);
+// reads and clears the device error flags (synchronous): TSLAM_E_POOL_FULL for a pool / table bit, else TSLAM_E_INVALID
+// naming every tracker bit that is set
+int oc_deferred(tslam_octo* m);
 // reset and fusion recycle pool slots: no tracker's kept state describes the map any more
 void oc_track_invalidate_all(tslam_octo* m);
 // *p holds at least `need` bytes: reallocated to exactly `need` when smaller (the contents are not kept)

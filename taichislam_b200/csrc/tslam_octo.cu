@@ -5,6 +5,7 @@
 #include <cstring>
 #include <string>
 #include "tslam_internal.cuh"
+#include "tslam_fuse_plan.cuh"
 
 __device__ __forceinline__ int oc_iroundf(float x) { return (int)roundf(x); }
 
@@ -145,10 +146,8 @@ __global__ void __launch_bounds__(256) k_octo_fuse(OcGrid dst, OcGrid src, Rule 
     const int b = (int)(e >> 9), v = (int)(e & 511);
     int s, bx, by, bz;
     ts_unpack_key(src.block_key[b], s, bx, by, bz);
-    float x, y, z;
-    pose_apply(pR + 9 * s, pT + 3 * s, (float)(bx * OC_B + (v >> 6)) * vs, (float)(by * OC_B + ((v >> 3) & 7)) * vs,
-               (float)(bz * OC_B + (v & 7)) * vs, x, y, z);  // :182
-    const int i = oc_iroundf(x / vs), j = oc_iroundf(y / vs), k = oc_iroundf(z / vs);  // :183-186
+    int i, j, k;
+    oc_fuse_cell(pR + 9 * s, pT + 3 * s, bx, by, bz, v, vs, i, j, k);  // :182-186
     if (!ts_in_bounds(dst, i, j, k)) continue;
     const int blk = ts_get_or_alloc(dst, ts_pack_key(0, i >> OC_BSHIFT, j >> OC_BSHIFT, k >> OC_BSHIFT));
     if (blk < 0) continue;
@@ -380,6 +379,7 @@ static int oc_create(const tslam_octo_config_t* cfg, const tslam_octo_logodds_t*
   tslam_octo* m = new tslam_octo();
   memset(m, 0, sizeof(*m));
   m->cfg = *cfg;
+  m->serial = ts_next_serial();
   int dev = 0;
   TS_CUDA(cudaGetDevice(&dev));
   cudaDeviceProp prop;
@@ -390,6 +390,7 @@ static int oc_create(const tslam_octo_config_t* cfg, const tslam_octo_logodds_t*
   if (m->cfg.max_points <= 0) m->cfg.max_points = 1 << 20;
   if (m->cfg.max_blocks <= 0) m->cfg.max_blocks = 1 << 18;  // 262144 blocks x 2 KB = 512 MB
   if (m->cfg.max_blocks > TS_MAX_BLOCKS) m->cfg.max_blocks = TS_MAX_BLOCKS;
+  m->content_ver = new unsigned long long[m->cfg.max_submaps]();
   m->in.fx = (float)cfg->fx; m->in.fy = (float)cfg->fy; m->in.cx = (float)cfg->cx; m->in.cy = (float)cfg->cy;
   m->in.dmin_mm = (float)(cfg->min_ray_length * 1000.0);
   m->in.dmax_mm = (float)(cfg->max_ray_length * 1000.0);
@@ -473,6 +474,8 @@ extern "C" int tslam_octo_destroy(tslam_octo_t* m) {
   oc_view_free(m);
   oc_travel_free(m);
   if (m->traj_mem) cudaFree(m->traj_mem);
+  oc_fuse_free(m);
+  delete[] m->content_ver;
   delete m;
   return TSLAM_OK;
 }
@@ -489,6 +492,7 @@ extern "C" int tslam_octo_reset(tslam_octo_t* m, void* stream) {
   if (nb && m->g.cw) TS_CUDA(cudaMemsetAsync(m->g.cw, 0, (size_t)nb * OC_B3 * 8, st));
   TS_CUDA(cudaMemsetAsync(m->scratch_i, 0, 4 * 4, st));
   oc_track_invalidate_all(m);
+  oc_map_written(m, -1);
   return TSLAM_OK;
 }
 
@@ -576,7 +580,7 @@ static int oc_lo_finish(tslam_octo* m, const TsFrame& fr, int n_max, cudaStream_
 
 // Reads and clears the device error flags.  A pool or table bit means hits were dropped: TSLAM_E_POOL_FULL.  Otherwise
 // one message names every tracker bit that is set: TSLAM_E_INVALID.
-static int oc_deferred(tslam_octo* m) {
+int oc_deferred(tslam_octo* m) {
   int err = 0;
   TS_CUDA(cudaMemcpy(&err, m->g.err, 4, cudaMemcpyDeviceToHost));
   if (!err) return TSLAM_OK;
@@ -585,7 +589,9 @@ static int oc_deferred(tslam_octo* m) {
   static const struct { int bit; const char* msg; } flags[] = {
       {OC_ERR_VIEW_WINDOW, "octo view gain: a walk left its view's bitmap window (is every view's R a rotation?): gains are invalid"},
       {OC_ERR_TRAVEL_PATH, "octo travel path: a cell of the field had no predecessor: paths are invalid"},
-      {OC_ERR_TRAVEL_SOURCE, "octo travel multi path: a source index was outside [0, n_starts): those paths have len 0"}};
+      {OC_ERR_TRAVEL_SOURCE, "octo travel multi path: a source index was outside [0, n_starts): those paths have len 0"},
+      {OC_ERR_FUSE_MISSING, "octo fuse_update: a removal found no block of dst (the map and its fusion record disagree): the next update is a "
+                            "full one"}};
   int tracker = 0;
   for (const auto& f : flags) tracker |= f.bit;
   if (err & ~tracker) {
@@ -624,11 +630,13 @@ extern "C" int tslam_octo_integrate_points_rgb(tslam_octo_t* m, const float* xyz
   oc_fill_frame(m, fr, R9, T3, submap);
   if (m->logodds) {
     if (n > m->ray_cap) { ts_set_error("n=%d exceeds the ray records of a log-odds map (%d)", n, m->ray_cap); return TSLAM_E_INVALID; }
+    oc_map_written(m, submap);
     TS_CUDA(cudaMemsetAsync(m->lo.ctr, 0, 8, st));
     k_octo_lo_points<<<(n + 255) / 256, 256, 0, st>>>(m->g, m->lo, src, n, fr, m->in.vs, csrc);
     TS_LAUNCH_CHECK(m);
     return oc_lo_finish(m, fr, n, st);
   }
+  oc_map_written(m, submap);
   k_octo_points<<<(n + 255) / 256, 256, 0, st>>>(m->g, src, n, fr, m->in.vs, csrc);
   TS_LAUNCH_CHECK(m);
   return TSLAM_OK;
@@ -662,6 +670,7 @@ extern "C" int tslam_octo_integrate_depth_tex(tslam_octo_t* m, const uint16_t* d
   }
   TsFrame fr;
   oc_fill_frame(m, fr, R9, T3, submap);
+  oc_map_written(m, submap);
   if (m->logodds) {
     TS_CUDA(cudaMemsetAsync(m->lo.ctr, 0, 8, st));
     k_octo_lo_depth<<<(hh * ww + 255) / 256, 256, 0, st>>>(m->g, m->lo, src, h, w, hh, ww, fr, m->in, tsrc, th, tw);

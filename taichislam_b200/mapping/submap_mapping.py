@@ -8,14 +8,15 @@ scripts/taichislam_node.py can drive it unchanged.  Differences, all fixes of re
 `recast_depth_to_map(R, T, ...)` works (the reference calls need_create_new_submap with the wrong arity,
 :195-196), send handles are optional.
 
-global_fusion="incremental" (TSDF submaps only) keeps the global map with DenseTSDF.update_fused_submaps instead of
-rebuilding it at every submap switch: only submaps that were added, moved or removed are re-splatted, so
+global_fusion="incremental" keeps the global map with DenseTSDF.update_fused_submaps (TSDF submaps) or
+Octomap.update_fused_submaps (Octomap submaps, either occupancy model) instead of rebuilding it at every submap switch:
+only submaps that were added, moved or removed are placed again, so
 set_frame_poses and input_remote_submap refresh the global map (its mesh and the callback) at once.  The active
 submap is left out of the global map in that mode: the reference fuses at the switch, when the active submap is
 empty, and its global-mode exporters add the active submap separately.  One deviation: when a remote submap arrives
 in the middle of a submap, the reference's rebuild also fuses the local active submap; the incremental mode does not.
-reclaim_empty=True (incremental mode only) gives the global map's blocks that a move or removal left empty back to the
-pool after each such update, so loop closures do not grow the global map.
+reclaim_empty=True (incremental mode with TSDF submaps only; the Octomap has no reclaim) gives the global map's blocks
+that a move or removal left empty back to the pool after each such update, so loop closures do not grow the global map.
 """
 import io
 import time
@@ -42,10 +43,12 @@ class SubmapMapping:
                  global_fusion="rebuild", fusion_tolerance=0.0, reclaim_empty=False):
         if global_fusion not in ("rebuild", "incremental"):
             raise ValueError(f"global_fusion must be 'rebuild' or 'incremental', not {global_fusion!r}")
-        if global_fusion == "incremental" and submap_type is not DenseTSDF:
-            raise ValueError("global_fusion='incremental' needs TSDF submaps")
+        if global_fusion == "incremental" and submap_type not in (DenseTSDF, Octomap):
+            raise ValueError("global_fusion='incremental' needs DenseTSDF or Octomap submaps")
         if reclaim_empty and global_fusion != "incremental":
             raise ValueError("reclaim_empty needs global_fusion='incremental' (a rebuild resets the global map anyway)")
+        if reclaim_empty and submap_type is not DenseTSDF:
+            raise ValueError("reclaim_empty needs TSDF submaps: the Octomap has no block reclaim")
         self.global_fusion = global_fusion
         self.fusion_tolerance = float(fusion_tolerance)
         self.reclaim_empty = bool(reclaim_empty)

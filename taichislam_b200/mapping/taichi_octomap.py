@@ -148,6 +148,12 @@ class Octomap(BaseMap):
         print(f"[OctoMap] Fuse submaps {(time.time() - t) * 1000:.1f}ms, active local: {submaps.active_submap_id[None]} "
               f"remote: {submaps.remote_submap_num[None]}")
 
+    def update_fused_submaps(self, submaps, include=None, tolerance=0.0, full=False):
+        """Keep this global map equal to fuse_submaps of `submaps` (an Octomap collection of the same occupancy model),
+        placing again only the submaps that were added, moved or removed since the last call (OctoHandle.fuse_update):
+        bit for bit what fuse_submaps gives for the included submaps.  -> dict of the call's statistics."""
+        return self._h.fuse_update(submaps._h, include=include, tolerance=tolerance, full=full)
+
     # planner queries (mapping_common.py:165-204; is_occupy :86-88; the reference's Octomap has no is_unobserved)
     def _query_raycast(self, pos, dir, max_dist):
         return self._h.raycast(pos, dir, max_dist, submap=self._active())

@@ -444,6 +444,25 @@ class OctoHandle:
     def fuse_from(self, src):
         capi.check(self.L.tslam_octo_fuse(self.h, src.h, capi.stream_ptr()))
 
+    def fuse_update(self, src, include=None, tolerance=0.0, full=False):
+        """Incremental fusion of the submaps of `src` (an OctoHandle of the same occupancy model) into this global map
+        (tslam_octo_fuse_update): afterwards this map is bit for bit fuse_from of the included submaps at their fused
+        poses.  include: None (all) or bools / 0-1 per submap (up to max_submaps); tolerance: how far (metres,
+        translation + angle x radius) a fused submap may move before it is placed again; full=True forces a rebuild.
+        -> dict of the call's statistics (TsdfHandle.fuse_update's keys; voxels_skipped counts recoloured voxels)."""
+        from .tsdf_handle import _fuse_stats
+        inc = None
+        if include is not None:
+            n = int(self.cfg.max_submaps) if 0 < int(self.cfg.max_submaps) <= 1024 else 1024
+            a = np.asarray(include).reshape(-1).astype(bool)
+            assert a.shape[0] <= n, "include has more entries than max_submaps"
+            inc = np.zeros(n, np.uint8)
+            inc[:a.shape[0]] = a
+        st = np.zeros(8, np.int64)
+        capi.check(self.L.tslam_octo_fuse_update(self.h, src.h, capi.np_ptr(inc) if inc is not None else None, float(tolerance),
+                                                 int(bool(full)), capi.np_ptr(st), capi.stream_ptr()))
+        return _fuse_stats(st, capi.FUSE_REASONS)
+
     def sync(self):
         capi.check(self.L.tslam_octo_sync(self.h, capi.stream_ptr()))
 

@@ -1017,6 +1017,67 @@ int tslam_esdf_trajectory(tslam_tsdf_t* m, int32_t submap, int32_t T, const int3
 int tslam_octo_esdf_trajectory(tslam_octo_t* m, int32_t submap, int32_t T, const int32_t* n_ctrl, const double* ctrl_in,
                                const tslam_traj_params_t* params, double* ctrl_out, double* cost, int32_t* info, void* stream);
 
+/* ----------------------------------------------------------------------------
+ * Submap pose-graph optimisation (DESIGN.md section 7, "Pose-graph optimisation"; tests/pose_graph_reference.py states
+ * the same contract in numpy).  Stateless: no handle.  All arithmetic is f64.
+ *   nodes      X_i = (R_i, t_i), i < N, maps submap-local coordinates to world coordinates.  fixed[i] != 0 marks a node
+ *              that never moves (the gauge); it is returned bit-identical to its input.
+ *   edges      edge k = (i, j, Z_k, Omega_k, c_k), i != j.  Z_k = (R, t) maps i-local to j-local: tslam_tsdf_register's
+ *              T with i = reference and j = reading submap, detect_loops' with i = query and j = match.  Omega_k is 6x6 in
+ *              xi = (rho, phi) order; only its upper triangle is read, and it may be rank-deficient (registration on one
+ *              plane gives rank 3).  c_k >= 0 is the Cauchy scale, 0 for plain least squares.
+ *   residual   e_k = Log(X_j^-1 X_i Z_k^-1), Log the exact inverse of registration's exponential R' = Exp(phi) R,
+ *              t' = Exp(phi) t + V(phi) rho: theta = atan2(|w| / 2, (tr R - 1) / 2), w = vee(R - R^T); phi = theta w /
+ *              (2 sin theta) when cos theta >= 0, else theta times the unit axis u of the symmetric part
+ *              (R + R^T) / 2 - cos theta I = (1 - cos theta) u u^T (largest diagonal first), signed so that u . w >= 0;
+ *              rho = V(phi)^-1 t.  Every angle coefficient (sin th / th, (1 - cos th) / th^2, (th - sin th) / th^3,
+ *              (1 - (th / 2) cot(th / 2)) / th^2 and Barfoot's two Q coefficients) is its series through th^4 below
+ *              theta = 1e-2.  If the measurement were exp(xi) Z for the true relative pose, e = xi exactly, so
+ *              registration's H (for the left perturbation T <- exp(xi) T) is the information of e as it stands.
+ *   cost       s_k = e_k^T Omega_k e_k; rho_k(s) = s when c_k = 0, else c_k^2 log1p(s / c_k^2); F = 1/2 sum rho_k(s_k),
+ *              summed in edge order within chunks of 256 edges and then over the chunk sums in chunk order.  IRLS weight
+ *              w_k = rho_k'(s_k) = 1 / (1 + s_k / c_k^2) (1 when c_k = 0).
+ *   update     left perturbation in the world frame X_i <- exp(delta_i) X_i for free nodes.  J_i = de/ddelta_i =
+ *              Jl^-1(e) Ad(X_j^-1) (Jl^-1 the closed-form inverse left Jacobian of SE(3)), J_j = -J_i, both exact.
+ *              A = sum w J^T Omega J over free nodes, g = sum w J^T Omega e.
+ *   solver     Levenberg-Marquardt with registration's schedule: (A + lam diag(max(A_ii, 1e-9 max_j A_jj))) delta = -g,
+ *              lam from 1e-4; a step is accepted when F decreases (lam / 10), else rejected (poses kept, lam * 10).
+ *              Converged when an accepted step has max |rho| < eps_t and max |phi| < eps_r.  Also stops after max_iters
+ *              evaluations, when lam > 1e16 (no progress), or when a damped 6x6 diagonal block is not positive definite.
+ *              max_iters = 0 evaluates F, s_k and w_k at the input and moves nothing.
+ *   linear     preconditioned conjugate gradients (6x6 block-Jacobi preconditioner, Cholesky of the damped diagonal
+ *              blocks) from x0 = 0, stopped when |r|_2 <= cg_tol |g|_2 or after max_cg iterations (or when p^T A p <= 0).
+ *              A step from a CG run that hit max_cg is still tried: LM's acceptance test guards it.  One cooperative
+ *              launch runs every CG iteration; its dot products sum fixed chunks of 32 free nodes in chunk order.
+ * Determinism: two identical calls give the same bits, whatever the grid size (pcg_grid) or the SM count.
+ * Inputs (HOST): R f64[N,9] row-major, T f64[N,3], fixed u8[N], ij int32[E,2], ZR f64[E,9], ZT f64[E,3], omega f64[E,36]
+ * row-major, cauchy f64[E].  Outputs (HOST): R_out f64[N,9], T_out f64[N,3] (final poses), chi2 f64[E] (s_k) and weight
+ * f64[E] (w_k) at the final poses, f3 f64[3] (F initial, F final, the largest final relative CG residual |r| / |g|),
+ * info5 int64[5] (LM evaluations, accepted steps, CG iterations in all, converged, status: 0 converged, 1 max_iters
+ * evaluations, 2 no progress, 3 damped block not positive definite).
+ * Refused (TSLAM_E_INVALID, nothing written), in this order, before any device work: N outside [2, 4096] or E outside
+ * [1, 65536]; a NULL array or params; eps_t or eps_r not finite or < 0, cg_tol not finite or outside [0, 1), max_iters
+ * outside [0, TSLAM_PG_MAX_ITERS], max_cg outside [1, TSLAM_PG_MAX_ITERS], pcg_grid < 0; then per node in order a
+ * non-finite pose, a rotation with max |R^T R - I| > 1e-6; then per edge in order an endpoint out of range or i == j, a
+ * non-finite measurement, upper-triangle Omega entry or c_k, c_k < 0, a measured rotation with max |R^T R - I| > 1e-6, a
+ * negative diagonal entry of Omega; then a connected component with no fixed node (union-find on the host: without one
+ * the damped system has no gauge).
+ * Uploads the graph once into stream-ordered scratch (about 600 B per edge, 700 B per free node, 200 B per node) and
+ * synchronises `stream` once per LM evaluation. */
+typedef struct {
+  double eps_t;       /* convergence: max |rho| of an accepted step below this (m) */
+  double eps_r;       /* convergence: max |phi| of an accepted step below this (rad) */
+  double cg_tol;      /* CG stops at |r|_2 <= cg_tol |g|_2 */
+  int32_t max_iters;  /* LM evaluations at most (0: evaluate the input only) */
+  int32_t max_cg;     /* CG iterations per step at most */
+  int32_t pcg_grid;   /* CTAs of the CG launch: 0 sizes it from the graph, clamped to the co-resident maximum */
+} tslam_pg_params_t;
+#define TSLAM_PG_MAX_ITERS 100000
+int tslam_pose_graph_solve(int32_t n_nodes, const double* R, const double* T, const uint8_t* fixed, int32_t n_edges,
+                           const int32_t* ij, const double* ZR, const double* ZT, const double* omega, const double* cauchy,
+                           const tslam_pg_params_t* params, double* R_out, double* T_out, double* chi2, double* weight,
+                           double* f3, int64_t* info5, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -70,6 +70,12 @@ class ViewCamera(C.Structure):
                 ("height", C.c_int32), ("step", C.c_int32), ("max_range", C.c_float)]
 
 
+class PgParams(C.Structure):
+    """tslam_pg_params_t"""
+    _fields_ = [("eps_t", C.c_double), ("eps_r", C.c_double), ("cg_tol", C.c_double), ("max_iters", C.c_int32),
+                ("max_cg", C.c_int32), ("pcg_grid", C.c_int32)]
+
+
 _vp, _i32, _i64, _f32 = C.c_void_p, C.c_int32, C.c_int64, C.c_float
 
 # name -> (restype, argtypes).  Every symbol declared in include/tslam.h appears here
@@ -212,6 +218,8 @@ SIGNATURES = {
     "tslam_tsdf_render": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _f32, _f32, _f32, _vp, _vp, _vp, _vp, _vp]),
     "tslam_esdf_trajectory": (C.c_int, [_vp, _i32, _i32, _vp, _vp, C.POINTER(TrajParams), _vp, _vp, _vp, _vp]),
     "tslam_octo_esdf_trajectory": (C.c_int, [_vp, _i32, _i32, _vp, _vp, C.POINTER(TrajParams), _vp, _vp, _vp, _vp]),
+    "tslam_pose_graph_solve": (C.c_int, [_i32, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, C.POINTER(PgParams), _vp, _vp, _vp,
+                                         _vp, _vp, _vp, _vp]),
 }
 
 class PlaceParams(C.Structure):

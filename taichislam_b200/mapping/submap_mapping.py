@@ -20,6 +20,7 @@ that a move or removal left empty back to the pool after each such update, so lo
 """
 import io
 import time
+import warnings
 import zlib
 
 import numpy as np
@@ -36,6 +37,15 @@ def _merged(defaults, overrides):
 
 _COMMON = dict(voxel_scale=0.05, texture_enabled=False, min_ray_length=0.3, max_ray_length=3.0,
                max_disp_particles=1024 * 1024)
+
+
+# optimize_poses defaults: odometry (sigma_t m, sigma_r degrees) and the Cauchy scale c of loop edges (sqrt(chi2) units).
+# Registration's H sums tens of thousands of points, so a loop that is not applied has a chi2 of 1e7 or more, and its
+# Cauchy cost c^2 log1p(chi2 / c^2) caps what it can buy in odometry chi2: about 1400 at c = 10.  The loop world of the
+# tests needs about 200 to close its true loop; a loop 1 m and 20 degrees off is applied at c = 30 and rejected at c = 10.
+# Picked there, not measured on real data.
+ODOMETRY_SIGMA = (0.05, 1.0)
+LOOP_ROBUST = 10.0
 
 
 class SubmapMapping:
@@ -69,6 +79,7 @@ class SubmapMapping:
         self.set_exporting_global()
         self.ego_motion_poses = {}
         self.pgo_poses = {}
+        self.submap_odometry = {}    # submap id -> the pose odometry reported at its creation frame (optimize_poses)
         self.last_frame_id = None
         self.active_submap_frame_id = 0
         self.enable_texture = self.global_map.enable_texture
@@ -173,6 +184,102 @@ class SubmapMapping:
             out[(frame_id, frame_of[c["match"]])] = c
         return out
 
+    def optimize_poses(self, loops, odometry_sigma=ODOMETRY_SIGMA, loop_sigma=None, loop_robust=LOOP_ROBUST, apply=True,
+                       **solver):
+        """Optimise the submap pose graph (pose_graph.optimize) and, with apply=True, move the submaps to the result.
+        Nodes: the submaps at the global map's base poses; the lowest submap id is fixed, and submaps outside its
+        connected component are left out (reported in "not_moved").  Edges: odometry between consecutive local submaps,
+        from the odometry poses of their creation frames, information diag(sigma_t^-2 I, sigma_r^-2 I) (odometry_sigma =
+        (sigma_t m, sigma_r degrees)), no robust kernel; and one loop per entry of `loops`, a dict keyed by (frame_id,
+        matched frame_id) of detect_loops dicts (accumulated across calls by the caller), i = query, j = match, Z = (R,
+        T), Omega = H / loop_sigma^2 (default half a voxel), Cauchy scale loop_robust.  When both (a, b) and (b, a) are
+        given, only the first in key order is used: they come from the same pair of submaps.  The defaults were picked on the
+        loop world of the tests, not measured on real data.  apply=True hands the moved submaps to set_frame_poses (which
+        moves them in the global map) and carries the active submap's correction C = X_new X_old^-1 into its base poses
+        and pgo_poses, so the next frames and submaps continue from the corrected pose.  solver: pose_graph.DEFAULTS.
+        Returns dict(poses {frame_id: (R, T)}, edges [(kind, frame_i, frame_j)], chi2, weight, rejected (loop keys whose
+        final weight is below 0.1), not_moved (frame ids), converged, info (the solver's result)).  A solve that does not
+        converge warns (RuntimeWarning): its poses and weights are those of the last accepted step."""
+        from .. import pose_graph
+        g = self.global_map
+        frame_of = {s: f for f, s in self.submaps.items()}
+        sids = sorted(frame_of)
+        if len(sids) < 2:
+            return dict(poses={}, edges=[], chi2=np.zeros(0), weight=np.zeros(0), rejected=[], not_moved=list(self.submaps),
+                        info=None)
+        vs = float(g.voxel_scale)
+        loop_sigma = 0.5 * vs if loop_sigma is None else float(loop_sigma)
+        st, sr = float(odometry_sigma[0]), np.deg2rad(float(odometry_sigma[1]))
+        O_odo = np.diag([st ** -2] * 3 + [sr ** -2] * 3)
+        pairs, Zs, Os, cs, kinds = [], [], [], [], []
+        local = [s for s in sids if s in self.submap_odometry]
+        for a, b in zip(local[:-1], local[1:]):
+            (Ra, Ta), (Rb, Tb) = self.submap_odometry[a], self.submap_odometry[b]
+            pairs.append((a, b)), Zs.append((Rb.T @ Ra, Rb.T @ (Ta - Tb))), Os.append(O_odo), cs.append(0.0)
+            kinds.append(("odometry", frame_of[a], frame_of[b]))
+        seen = set()
+        for (fq, fd), c in sorted(loops.items(), key=lambda kv: kv[0]):
+            if frozenset((fq, fd)) in seen:  # (a, b) and (b, a) from the same registration data: count it once
+                continue
+            seen.add(frozenset((fq, fd)))
+            pairs.append((self.submaps[fq], self.submaps[fd]))
+            Zs.append((np.asarray(c["R"], np.float64), np.asarray(c["T"], np.float64)))
+            Os.append(np.asarray(c["H"], np.float64).reshape(6, 6) / loop_sigma ** 2)
+            cs.append(float(loop_robust))
+            kinds.append(("loop", fq, fd))
+        parent = {s: s for s in sids}
+
+        def find(a):
+            while parent[a] != a:
+                a = parent[a]
+            return a
+        for a, b in pairs:
+            parent[find(a)] = find(b)
+        gauge = sids[0]
+        nodes = [s for s in sids if find(s) == find(gauge)]
+        keep = [k for k, (a, b) in enumerate(pairs) if find(a) == find(gauge)]
+        if len(nodes) < 2 or not keep:
+            return dict(poses={}, edges=[], chi2=np.zeros(0), weight=np.zeros(0), rejected=[], not_moved=list(self.submaps),
+                        info=None)
+        at = {s: n for n, s in enumerate(nodes)}
+        R0 = np.stack([np.asarray(g.submaps_base_R_np[s], np.float64) for s in nodes])
+        T0 = np.stack([np.asarray(g.submaps_base_T_np[s], np.float64) for s in nodes])
+        edges = dict(ij=np.array([(at[pairs[k][0]], at[pairs[k][1]]) for k in keep]), R=np.stack([Zs[k][0] for k in keep]),
+                     T=np.stack([Zs[k][1] for k in keep]), omega=np.stack([Os[k] for k in keep]),
+                     cauchy=np.array([cs[k] for k in keep]))
+        res = pose_graph.optimize(R0, T0, np.array([s == gauge for s in nodes]), edges, **solver)
+        if not res["converged"]:
+            warnings.warn(f"optimize_poses: the pose graph did not converge ({res['status_name']} after "
+                          f"{res['evaluations']} evaluations, largest CG residual {res['cg_residual']:.2g})",
+                          RuntimeWarning, stacklevel=2)
+        kinds = [kinds[k] for k in keep]
+        poses = {frame_of[s]: (res["R"][at[s]], res["T"][at[s]]) for s in nodes}
+        out = dict(poses=poses, edges=kinds, chi2=res["chi2"], weight=res["weight"],
+                   rejected=[(fi, fj) for (kd, fi, fj), w in zip(kinds, res["weight"]) if kd == "loop" and w < 0.1],
+                   not_moved=[frame_of[s] for s in sids if s not in at], converged=res["converged"], info=res)
+        if apply:
+            act = self.submap_collection.get_active_submap_id()
+            fa = frame_of.get(act)
+            moved = {f: p for f, p in poses.items() if self.submaps[f] != act and self.submaps[f] != gauge}
+            if moved:
+                self.set_frame_poses(moved)
+            if fa is not None and act in at and act != gauge:
+                Rn, Tn = poses[fa]
+                Ro, To = R0[at[act]], T0[at[act]]
+                Rc = Rn @ Ro.T
+                Tc = Tn - Rc @ To
+                g.set_base_pose_submap(act, Rn, Tn)
+                self.submap_collection.set_base_pose_submap(act, Rn, Tn)
+                if self.last_frame_id is None or self.last_frame_id <= fa:
+                    self.pgo_poses[fa] = (Rn, Tn)
+                    if fa in self.ego_motion_poses:
+                        self.last_frame_id = fa
+                else:
+                    Rl, Tl = self.pgo_poses[self.last_frame_id]
+                    self.pgo_poses[self.last_frame_id] = (Rc @ Rl, Rc @ Tl + Tc)
+                self.send_traj({fa: (Rn, Tn)})  # peers learn the active submap's pose as set_frame_poses tells them the others
+        return out
+
     def convert_by_pgo(self, frame_id, R, T):  # :162-169
         self.ego_motion_poses[frame_id] = (R, T)
         if self.last_frame_id is None:
@@ -202,6 +309,9 @@ class SubmapMapping:
         self.submap_collection.set_base_pose_submap(sid, R, T)
         self.submaps[frame_id] = sid
         self.pgo_poses[frame_id] = (R, T)
+        # odometry edges come from these, not from the base poses, so that a second optimisation does not anchor the first
+        odo = self.ego_motion_poses.get(frame_id, (R, T))
+        self.submap_odometry[sid] = (np.array(odo[0], np.float64), np.array(odo[1], np.float64))
         self.active_submap_frame_id = frame_id
         print(f"[SubmapMapping] Created new submap on frame {frame_id}, now have {sid + 1} submaps")
         if self.autosave_path and sid % 2 == 0:

@@ -476,7 +476,7 @@ extern "C" int tslam_tsdf_foreign_pack2(tslam_tsdf_t* m, const int32_t* tiles3, 
   TS_CUDA(cudaMemcpyAsync(d_off, h_off, world * sizeof(int), cudaMemcpyHostToDevice, st));
   TS_CUDA(cudaMemsetAsync(d_cur, 0, 24 * sizeof(int), st));
   m->mesh_epoch++;  // the packed blocks' obs / col planes are cleared without a stamp
-  ts_map_written(m, -1);
+  fz_written(m->ver, -1);
   k_foreign_pack<<<m->sm_count * 4, 256, 0, st>>>(m->g, t, d_off, d_cur, cap, (long long*)keys, (float2*)acc, obs, occ, (float4*)col);
   TS_LAUNCH_CHECK(m);
   TS_CUDA(cudaStreamSynchronize(st));  // h_off is on the stack
@@ -494,7 +494,7 @@ extern "C" int tslam_tsdf_unpack_add2(tslam_tsdf_t* m, int64_t n, const int64_t*
   if (n == 0) return TSLAM_OK;
   cudaStream_t st = (cudaStream_t)stream;
   m->mesh_epoch++;  // obs / col change before the fused commit stamps the blocks
-  ts_map_written(m, -1);
+  fz_written(m->ver, -1);
   k_unpack_add<<<(int)(n < m->sm_count * 4 ? n : m->sm_count * 4), 256, 0, st>>>(m->g, n, (const long long*)keys, (const float2*)acc, obs, occ, (const float4*)col);
   TS_LAUNCH_CHECK(m);
   return TSLAM_OK;
@@ -551,7 +551,7 @@ extern "C" int tslam_tsdf_ghost_unpack2(tslam_tsdf_t* m, int64_t n, const int64_
   if (col && !m->g.col) { ts_set_error("colour plane given to an untextured map"); return TSLAM_E_INVALID; }
   if (n == 0) return TSLAM_OK;
   cudaStream_t st = (cudaStream_t)stream;
-  ts_map_written(m, -1);
+  fz_written(m->ver, -1);
   m->ghost_gen++;
   m->esdf_full_needed = 1;
   const unsigned long long seq = ++m->commit_seq;  // the imported ghosts are stamped like committed blocks (incremental mesh)

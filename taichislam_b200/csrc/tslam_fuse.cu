@@ -20,10 +20,11 @@
 // re-addition are both in flight still ends on the exact total.  Because every sum is exact and order-free, dst does
 // not depend on the history of updates: any sequence of calls ends bit for bit where one call on a fresh map would.
 //
-// An update plans on the host (per-submap block counts and radii from k_fz_plan), lists the source blocks of the
-// submaps with work (k_fz_list), activates the dst blocks the additions need (k_fz_splat<0>), grows the sum planes
-// to the pool blocks in use, splats (k_fz_splat<1>: removals at the old pose, additions at the new one) and reads the
-// touched blocks out of the sums (k_fz_commit), stamping them for the incremental mesh and the ESDF.
+// An update plans and lists the source blocks of the submaps with work as the Octomap's does (tslam_fuse_plan.cuh: the
+// plan rule, fusion state, scratch, sum storage, k_fz_plan / k_fz_list and the host steps around them), activates the
+// dst blocks the additions need (k_fz_splat<0>), grows the sum planes to the pool blocks in use, splats
+// (k_fz_splat<1>: removals at the old pose, additions at the new one) and reads the touched blocks out of the sums
+// (k_fz_commit), stamping them for the incremental mesh and the ESDF.
 //
 // Tiled global maps (tslam_tsdf_fuse_update_tiled_*, DESIGN.md section 6) run the same plan, splat and commit per rank:
 // the sums of a block live on its owner, the other ranks pack the sum rows of their foreign blocks (k_fz_pack) and the
@@ -46,25 +47,16 @@ struct FzSums {       // sum planes, [cap blocks * 4096] int64 each
   long long* c;       // textured maps: 3 planes S_c (c + p * stride), else null
   size_t stride;      // elements per plane
 };
-struct FzDev {        // device scratch of one update (TsFuse::dev)
-  int* nblk;          // [max_submaps] non-ghost source blocks per submap (k_fz_plan)
-  unsigned* rbits;    // [max_submaps] float bits of the farthest block corner from the submap origin (k_fz_plan)
-  int2* job_of;       // [max_submaps] (removal job, addition job), -1 none
-  FzJob* jobs;        // [2 * max_submaps]
-  int* list;          // [src max_blocks] source blocks with work
-  unsigned long long* ctr;  // [0] list length, [1] voxels splatted, [2] voxels skipped, [3] dst ghost blocks, [4] dirty blocks,
-                            // [5] voxels whose count decodes as negative (tiled updates)
+// Device scratch of one update.  ctr: [0] list length, [1] voxels splatted, [2] voxels skipped, [3] dst ghost blocks,
+// [4] dirty blocks, [5] voxels whose count decodes as negative (tiled updates).
+struct TsDev : FzDev {
+  TsTiling* tiling;   // a tiled update's tiling (k_fz_splat indexes its cuts: as a kernel parameter they would be
+                      // copied to the stack)
+  void carve_tail(FzCarve& c, int) { tiling = c.take<TsTiling>(1); }
 };
 
-struct TsFuse {
-  int valid;          // the sums describe dst (cleared by a failed update)
-  unsigned long long src_serial, gen;  // src handle and dst write generation of the last update (tiled: write_gen - ghost_gen)
-  std::vector<FzSub> sub;
-  void* sums;         // sum planes (grown geometrically, never shrunk)
-  size_t cap_blocks;
-  void* dev;          // FzDev arrays
-  size_t dev_bytes;
-  int dev_submaps, dev_blocks;
+// (FzState::gen of a tiled update: write_gen - ghost_gen, as ghost imports are not writes of dst's own content)
+struct TsFuse : FzState {
   // tiled updates (tslam_tsdf_fuse_update_tiled_*)
   int ever_valid;     // the sums were valid once: invalid sums read "sums not valid", not "first call"
   int tiled;          // the last update was tiled, with this tiling (world 0 for a single-map update)
@@ -77,32 +69,34 @@ struct TsFuse {
 
 static unsigned long long g_serial = 0;  // handle numbers (create is not called concurrently with itself here)
 
-unsigned long long ts_next_serial() { return __atomic_add_fetch(&g_serial, 1ull, __ATOMIC_RELAXED); }
-
-int ts_fuse_init(tslam_tsdf* m) {
-  m->serial = ts_next_serial();
-  m->write_gen = 0;
-  m->ghost_gen = 0;
-  m->content_ver = new unsigned long long[m->cfg.max_submaps]();
-  m->fz = nullptr;
-  return TSLAM_OK;
+void fz_ver_init(FzVer& v, int max_submaps) {
+  v.serial = __atomic_add_fetch(&g_serial, 1ull, __ATOMIC_RELAXED);
+  v.write_gen = 0;
+  v.content_ver = new unsigned long long[max_submaps]();
+  v.n = max_submaps;
 }
 
-void ts_fuse_free(tslam_tsdf* m) {
-  delete[] m->content_ver;
-  m->content_ver = nullptr;
-  if (m->fz) {
-    if (m->fz->sums) cudaFree(m->fz->sums);
-    if (m->fz->dev) cudaFree(m->fz->dev);
-    delete m->fz;
-    m->fz = nullptr;
+void fz_ver_free(FzVer& v) {
+  delete[] v.content_ver;
+  v.content_ver = nullptr;
+}
+
+void fz_written(FzVer& v, int submap) {
+  v.write_gen++;
+  if (!v.content_ver) return;
+  if (submap < 0) {
+    for (int s = 0; s < v.n; s++) v.content_ver[s]++;
+  } else if (submap < v.n) {
+    v.content_ver[submap]++;
   }
 }
+
+void ts_fuse_free(tslam_tsdf* m) { fz_free(m->fz); }
 
 TsFuseView ts_fuse_view(tslam_tsdf* m) {
   TsFuseView v = {nullptr, 0, m->g.col ? 6 : 3, 0, 0};
   if (m->fz) {
-    v.sums = (long long*)m->fz->sums;
+    v.sums = m->fz->sums;
     v.cap_blocks = v.sums ? m->fz->cap_blocks : 0;
     v.valid = m->fz->valid;
     v.phase = m->fz->phase;
@@ -110,57 +104,9 @@ TsFuseView ts_fuse_view(tslam_tsdf* m) {
   return v;
 }
 
-void ts_map_written(tslam_tsdf* m, int submap) {
-  m->write_gen++;
-  if (!m->content_ver) return;
-  if (submap < 0) {
-    for (int s = 0; s < m->cfg.max_submaps; s++) m->content_ver[s]++;
-  } else if (submap < m->cfg.max_submaps) {
-    m->content_ver[submap]++;
-  }
-}
-
 // ---------------------------------------------------------------------------
 // kernels
 // ---------------------------------------------------------------------------
-// non-ghost blocks and radius per source submap; ghost blocks of dst
-__global__ void __launch_bounds__(256) k_fz_plan(TsGrid src, TsGrid dst, float vs, FzDev f) {
-  const int nb = min(*src.n_blocks, src.max_blocks);
-  for (int b = blockIdx.x * blockDim.x + threadIdx.x; b < nb; b += gridDim.x * blockDim.x) {
-    if (src.ghost[b]) continue;
-    int s, bx, by, bz;
-    ts_unpack_key(src.block_key[b], s, bx, by, bz);
-    const float ex = fmaxf(fabsf((float)(bx * TS_B) * vs), fabsf((float)(bx * TS_B + TS_B) * vs));
-    const float ey = fmaxf(fabsf((float)(by * TS_B) * vs), fabsf((float)(by * TS_B + TS_B) * vs));
-    const float ez = fmaxf(fabsf((float)(bz * TS_B) * vs), fabsf((float)(bz * TS_B + TS_B) * vs));
-    atomicAdd(&f.nblk[s], 1);
-    atomicMax(&f.rbits[s], __float_as_uint(sqrtf(ex * ex + ey * ey + ez * ez)));  // non-negative floats order as uints
-  }
-  const int nd = min(*dst.n_blocks, dst.max_blocks);
-  unsigned ng = 0;
-  for (int b = blockIdx.x * blockDim.x + threadIdx.x; b < nd; b += gridDim.x * blockDim.x) ng += dst.ghost[b] != 0;
-  if (ng) atomicAdd(&f.ctr[3], (unsigned long long)ng);
-}
-
-// the non-ghost source blocks of submaps with a job
-__global__ void __launch_bounds__(256) k_fz_list(TsGrid src, FzDev f) {
-  const int nb = min(*src.n_blocks, src.max_blocks);
-  const int stride = gridDim.x * blockDim.x;
-  const int iters = (nb + stride - 1) / stride;
-  for (int it = 0; it < iters; ++it) {
-    const int b = it * stride + blockIdx.x * blockDim.x + threadIdx.x;
-    bool want = false;
-    if (b < nb && !src.ghost[b]) {
-      int s, bx, by, bz;
-      ts_unpack_key(src.block_key[b], s, bx, by, bz);
-      const int2 j = f.job_of[s];
-      want = j.x >= 0 || j.y >= 0;
-    }
-    const long long row = warp_append_u64(want, &f.ctr[0]);
-    if (want) f.list[row] = b;
-  }
-}
-
 __device__ __forceinline__ bool fz_term_ok(float x) { return fabsf(x) < FZ_FMAX; }  // false for NaN and +-inf too
 __device__ __forceinline__ long long fz_q(float x) { return __double2ll_rn((double)x * FZ_Q); }
 
@@ -365,7 +311,7 @@ static int fz_planes(const tslam_tsdf* m) { return m->g.col ? 6 : 3; }
 static FzSums fz_sums(const TsFuse* z, int planes) {
   FzSums S;
   const size_t n = z->cap_blocks * TS_B3;
-  long long* p = (long long*)z->sums;
+  long long* p = z->sums;
   S.stride = n;
   S.wt = p;
   S.w = p + n;
@@ -374,79 +320,9 @@ static FzSums fz_sums(const TsFuse* z, int planes) {
   return S;
 }
 
-// sum planes for at least `need` pool blocks: grown to max(need, 2 x cap) (at most max_blocks), the old sums kept
-static int fz_reserve_sums(tslam_tsdf* m, size_t need, cudaStream_t st) {
-  TsFuse* z = m->fz;
-  if (need <= z->cap_blocks) return TSLAM_OK;
-  size_t cap = std::max(need, 2 * z->cap_blocks);
-  if (cap > (size_t)m->g.max_blocks) cap = (size_t)m->g.max_blocks;
-  const int planes = fz_planes(m);
-  const size_t bytes = cap * TS_B3 * 8 * planes;
-  void* p = nullptr;
-  cudaError_t e = cudaMalloc(&p, bytes);
-  if (e != cudaSuccess) {
-    cudaGetLastError();
-    ts_set_error("fuse_update: cannot allocate %zu bytes of sum planes (%zu pool blocks x %d planes x 32 KiB): %s", bytes, cap, planes,
-                 cudaGetErrorString(e));
-    return TSLAM_E_CUDA;
-  }
-  const size_t old_n = z->cap_blocks * TS_B3, n = cap * TS_B3;
-  for (int k = 0; k < planes; k++) {
-    long long* dstp = (long long*)p + k * n;
-    if (old_n) TS_CUDA(cudaMemcpyAsync(dstp, (long long*)z->sums + k * old_n, old_n * 8, cudaMemcpyDeviceToDevice, st));
-    TS_CUDA(cudaMemsetAsync(dstp + old_n, 0, (n - old_n) * 8, st));
-  }
-  if (z->sums) {
-    TS_CUDA(cudaStreamSynchronize(st));
-    TS_CUDA(cudaFree(z->sums));
-  }
-  z->sums = p;
-  z->cap_blocks = cap;
-  return TSLAM_OK;
-}
-
-static void fz_dev(TsFuse* z, FzDev& f);
-static int fz_reserve_dev(tslam_tsdf* dst, tslam_tsdf* src, FzDev& f) {
-  TsFuse* z = dst->fz;
-  const int S = dst->cfg.max_submaps, B = src->g.max_blocks;
-  if (!z->dev || z->dev_submaps != S || z->dev_blocks < B) {
-    if (z->dev) TS_CUDA(cudaFree(z->dev));
-    z->dev = nullptr;
-    const size_t bytes = (size_t)S * (4 + 4 + 8) + (size_t)2 * S * sizeof(FzJob) + (size_t)B * 4 + 8 * 8 + sizeof(TsTiling) + 256;
-    TS_CUDA(cudaMalloc(&z->dev, bytes));
-    z->dev_bytes = bytes;
-    z->dev_submaps = S;
-    z->dev_blocks = B;
-  }
-  fz_dev(z, f);
-  return TSLAM_OK;
-}
-
-// the FzDev arrays in z->dev (as the last fz_reserve_dev sized them)
-static void fz_dev(TsFuse* z, FzDev& f) {
-  const int S = z->dev_submaps;
-  char* p = (char*)z->dev;
-  f.ctr = (unsigned long long*)p; p += 8 * 8;
-  f.jobs = (FzJob*)p; p += (size_t)2 * S * sizeof(FzJob);
-  f.job_of = (int2*)p; p += (size_t)S * 8;
-  f.nblk = (int*)p; p += (size_t)S * 4;
-  f.rbits = (unsigned*)p; p += (size_t)S * 4;
-  f.list = (int*)p;
-}
-
-// device copy of a tiled update's tiling, after the FzDev arrays (k_fz_splat indexes its cuts: as a kernel parameter
-// they would be copied to the stack)
-static TsTiling* fz_dev_tiling(TsFuse* z) {
-  const size_t S = (size_t)z->dev_submaps;
-  return (TsTiling*)((char*)z->dev + 8 * 8 + 2 * S * sizeof(FzJob) + S * (8 + 4 + 4) + (size_t)z->dev_blocks * 4);
-}
-
-// Refusals that need no handle contents (TSLAM_E_INVALID, nothing written)
-static int fz_check_args(tslam_tsdf* dst, tslam_tsdf* src, float tolerance) {
-  if (!std::isfinite(tolerance) || tolerance < 0.0f) { ts_set_error("fuse_update: tolerance %g must be finite and >= 0", (double)tolerance); return TSLAM_E_INVALID; }
-  if (!dst || !src) { ts_set_error("fuse_update: NULL handle"); return TSLAM_E_INVALID; }
-  if (dst == src) { ts_set_error("fuse_update: dst == src (a map cannot be fused into itself)"); return TSLAM_E_INVALID; }
-  return TSLAM_OK;
+// sum planes for at least `need` pool blocks (fz_reserve_sums)
+static int fz_reserve_planes(tslam_tsdf* m, size_t need, cudaStream_t st) {
+  return fz_reserve_sums(*m->fz, need, (size_t)m->g.max_blocks, TS_B3, fz_planes(m), "fuse_update", st);
 }
 
 static int fz_check_maps(tslam_tsdf* dst, tslam_tsdf* src) {
@@ -459,99 +335,39 @@ static int fz_check_maps(tslam_tsdf* dst, tslam_tsdf* src) {
   return TSLAM_OK;
 }
 
-// flush both maps' pending work, create dst's fusion state, reserve its device scratch
-static int fz_open(tslam_tsdf* dst, tslam_tsdf* src, cudaStream_t st, FzDev& f) {
+// flush both maps' pending work, then dst's fusion state and device scratch (fz_open)
+static int fz_begin(tslam_tsdf* dst, tslam_tsdf* src, cudaStream_t st, TsDev& f) {
   int rc = ts_flush_pending(src, st);
   if (rc) return rc;
   rc = ts_flush_pending(dst, st);
   if (rc) return rc;
-  if (!dst->fz) {
-    dst->fz = new TsFuse();
-    dst->fz->valid = 0;
-    dst->fz->sums = nullptr;
-    dst->fz->cap_blocks = 0;
-    dst->fz->dev = nullptr;
-    dst->fz->sub.assign(dst->cfg.max_submaps, FzSub());
-  }
-  return fz_reserve_dev(dst, src, f);
-}
-
-// The plan of an update (k_fz_plan: source blocks and radius per submap, dst ghosts; dst's pose table).  `reason` is the
-// full-update reason found from the host state; when it is FZ_INCR the per-submap actions of an incremental update are
-// planned, which may still find a fused submap whose content changed (FZ_CONTENT).  The cost rule and the switch to
-// a full update's actions are the caller's (fz_settle), as a tiled update decides them over all ranks.
-static int fz_plan(tslam_tsdf* dst, tslam_tsdf* src, const uint8_t* include, float tolerance, int reason, cudaStream_t st, const FzDev& f,
-                   FzPlan& P) {
-  TsFuse* z = dst->fz;
-  const int S = dst->cfg.max_submaps;
-  TS_CUDA(cudaMemsetAsync(f.ctr, 0, 8 * 8, st));
-  TS_CUDA(cudaMemsetAsync(f.nblk, 0, (size_t)S * 8, st));  // nblk and rbits
-  const int gp = src->sm_count * 4;
-  k_fz_plan<<<gp, 256, 0, st>>>(src->g, dst->g, src->in.vs, f);
-  TS_LAUNCH_CHECK(dst);
-  P.nblk.assign(S, 0);
-  P.rad.assign(S, 0.0f);
-  P.pR.assign((size_t)S * 9, 0.0f);
-  P.pT.assign((size_t)S * 3, 0.0f);
-  unsigned long long ctr0[8];
-  TS_CUDA(cudaMemcpyAsync(P.nblk.data(), f.nblk, (size_t)S * 4, cudaMemcpyDeviceToHost, st));
-  TS_CUDA(cudaMemcpyAsync(P.rad.data(), f.rbits, (size_t)S * 4, cudaMemcpyDeviceToHost, st));
-  TS_CUDA(cudaMemcpyAsync(ctr0, f.ctr, sizeof(ctr0), cudaMemcpyDeviceToHost, st));
-  TS_CUDA(cudaMemcpyAsync(P.pR.data(), dst->pose_R, (size_t)S * 36, cudaMemcpyDeviceToHost, st));
-  TS_CUDA(cudaMemcpyAsync(P.pT.data(), dst->pose_T, (size_t)S * 12, cudaMemcpyDeviceToHost, st));
-  TS_CUDA(cudaStreamSynchronize(st));
-  P.ghosts = ctr0[3];
-
-  fz_decide(P, z->sub, src->content_ver, include, tolerance, reason);
-  return TSLAM_OK;
+  return fz_open(dst->fz, dst->cfg.max_submaps, src->g.max_blocks, 0, f);
 }
 
 // Splat the plan into the sums: a full update resets dst and zeroes the sums first.  Tiled (t: the tiling, else null):
 // removals also activate their foreign blocks.  Invalidates the sums until the update is recorded.
-static int fz_execute(tslam_tsdf* dst, tslam_tsdf* src, const FzDev& f, const FzPlan& P, const TsTiling* t, cudaStream_t st) {
+static int fz_execute(tslam_tsdf* dst, tslam_tsdf* src, const TsDev& f, const FzPlan& P, const TsTiling* t, cudaStream_t st) {
   TsFuse* z = dst->fz;
-  const int S = dst->cfg.max_submaps;
-  std::vector<FzJob> jobs;
-  std::vector<int2> job_of(S, make_int2(-1, -1));
-  for (int s = 0; s < S; s++) {
-    if (P.act[s] == FZ_REMOVE || P.act[s] == FZ_MOVE) {
-      FzJob j;
-      memcpy(j.R, z->sub[s].R, 36); memcpy(j.T, z->sub[s].T, 12);
-      j.sign = -1; j.pad = 0;
-      job_of[s].x = (int)jobs.size();
-      jobs.push_back(j);
-    }
-    if (P.act[s] == FZ_ADD || P.act[s] == FZ_MOVE) {
-      FzJob j;
-      memcpy(j.R, &P.pR[(size_t)9 * s], 36); memcpy(j.T, &P.pT[(size_t)3 * s], 12);
-      j.sign = 1; j.pad = 0;
-      job_of[s].y = (int)jobs.size();
-      jobs.push_back(j);
-    }
-  }
-
+  const FzJobs J = fz_jobs(P, z->sub);
   const int planes = fz_planes(dst);
   z->valid = 0;  // until this update completes
   if (P.full) {
-    const unsigned long long gen = dst->write_gen;
+    const unsigned long long gen = dst->ver.write_gen;
     int rc = tslam_tsdf_reset(dst, (void*)st);  // also compacts the pool: blocks left empty by removals are dropped
     if (rc) return rc;
-    dst->write_gen = gen;
+    dst->ver.write_gen = gen;
     // every plane in full: a reset of dst since the last update left the pool empty but not the sums (at most 2x the
     // blocks in use: the planes grow geometrically)
     if (z->sums) TS_CUDA(cudaMemsetAsync(z->sums, 0, z->cap_blocks * TS_B3 * 8 * planes, st));
   }
-  if (!jobs.empty()) {
-    TS_CUDA(cudaMemcpyAsync(f.jobs, jobs.data(), jobs.size() * sizeof(FzJob), cudaMemcpyHostToDevice, st));
-    TS_CUDA(cudaMemcpyAsync(f.job_of, job_of.data(), (size_t)S * 8, cudaMemcpyHostToDevice, st));
-    const int gl = std::max(1, std::min((src->g.max_blocks + 255) / 256, src->sm_count * 4));
-    k_fz_list<<<gl, 256, 0, st>>>(src->g, f);
-    TS_LAUNCH_CHECK(dst);
+  if (!J.jobs.empty()) {
+    int rc = fz_list(dst, src, f, J, st);
+    if (rc) return rc;
     const int gs = dst->sm_count * 8;
     if (P.n_add + P.n_move > 0 || (t && P.n_remove > 0)) {
       TsTiling* td = nullptr;
       if (t) {
-        td = fz_dev_tiling(z);
+        td = f.tiling;
         TS_CUDA(cudaMemcpyAsync(td, t, sizeof(TsTiling), cudaMemcpyHostToDevice, st));
       }
       k_fz_splat<0><<<gs, 256, 0, st>>>(dst->g, src->g, f, FzSums{}, dst->in.vs, td);
@@ -562,7 +378,7 @@ static int fz_execute(tslam_tsdf* dst, tslam_tsdf* src, const FzDev& f, const Fz
     TS_CUDA(cudaMemcpyAsync(&err, dst->g.err, 4, cudaMemcpyDeviceToHost, st));
     TS_CUDA(cudaStreamSynchronize(st));
     if (err) return ts_check_deferred(dst);  // pool exhausted: nothing was added; the next update is a full one
-    int rc = fz_reserve_sums(dst, (size_t)std::min(nb, dst->g.max_blocks), st);
+    rc = fz_reserve_planes(dst, (size_t)std::min(nb, dst->g.max_blocks), st);
     if (rc) return rc;
     k_fz_splat<1><<<gs, 256, 0, st>>>(dst->g, src->g, f, fz_sums(z, planes), dst->in.vs, nullptr);
     TS_LAUNCH_CHECK(dst);
@@ -607,47 +423,34 @@ static int fz_commit(tslam_tsdf* dst, const FzDev& f, bool check_negative, cudaS
 }
 
 // the submaps' new state after a successful update
-static void fz_record(tslam_tsdf* dst, tslam_tsdf* src, const FzPlan& P) {
-  TsFuse* z = dst->fz;
-  fz_record_subs(z->sub, P, src->content_ver);
+static void ts_fz_record(tslam_tsdf* dst, tslam_tsdf* src, const FzPlan& P) {
+  fz_record(*dst->fz, P, src->ver);
   // voxels that lose their last contribution become unobserved, which the incremental ESDF does not undo
   if (P.n_remove + P.n_move > 0) dst->esdf_full_needed = 1;
-  z->valid = 1;
-  z->ever_valid = 1;
-  z->src_serial = src->serial;
+  dst->fz->ever_valid = 1;
 }
 
-static void fz_stats(const FzPlan& P, const unsigned long long* ctr, int64_t* stats8) {
-  if (!stats8) return;
-  stats8[0] = P.reason;
-  stats8[1] = P.n_add;
-  stats8[2] = P.n_move;
-  stats8[3] = P.n_remove;
-  stats8[4] = P.n_tol;
-  stats8[5] = (int64_t)ctr[1];
-  stats8[6] = (int64_t)ctr[2];
-  stats8[7] = (int64_t)(unsigned)ctr[4];
+// stats8 of a completed update: voxels splatted, skipped, blocks committed
+static void ts_fz_stats(const FzPlan& P, const unsigned long long* ctr, int64_t* stats8) {
+  fz_stats(P, (int64_t)ctr[1], (int64_t)ctr[2], (int64_t)(unsigned)ctr[4], stats8);
 }
 
 extern "C" int tslam_tsdf_fuse_update(tslam_tsdf_t* dst, tslam_tsdf_t* src, const uint8_t* include, float tolerance, int32_t full,
                                       int64_t* stats8, void* stream) {
-  int rc = fz_check_args(dst, src, tolerance);
+  int rc = fz_check_args(dst, src, tolerance, "fuse_update");
   if (rc) return rc;
   rc = fz_check_maps(dst, src);
   if (rc) return rc;
   if (dst->tile_cuts_set) { ts_set_error("fuse_update: dst is a tiled map (tile cuts set): not supported"); return TSLAM_E_INVALID; }
   cudaStream_t st = (cudaStream_t)stream;
-  FzDev f;
-  rc = fz_open(dst, src, st, f);
+  TsDev f;
+  rc = fz_begin(dst, src, st, f);
   if (rc) return rc;
   TsFuse* z = dst->fz;
-  int reason = FZ_INCR;
-  if (full) reason = FZ_ASKED;
-  else if (!z->valid) reason = FZ_FIRST;
-  else if (z->src_serial != src->serial) reason = FZ_OTHER_SRC;
-  else if (z->gen != dst->write_gen || z->tiled) reason = FZ_DST_WRITTEN;  // (sums of a tiled update hold one tile)
+  // (the sums of a tiled update hold one tile)
+  const int reason = fz_reason(*z, full, FZ_FIRST, src->ver.serial, z->gen != dst->ver.write_gen || z->tiled);
   FzPlan P;
-  rc = fz_plan(dst, src, include, tolerance, reason, st, f, P);
+  rc = fz_plan(dst, src, f, include, tolerance, reason, st, P);
   if (rc) return rc;
   if (P.ghosts > 0) { ts_set_error("fuse_update: dst holds %llu ghost blocks (a tiled map): not supported", P.ghosts); return TSLAM_E_INVALID; }
   fz_settle(P, P.reason == FZ_INCR && P.cost > P.cost_full ? FZ_COST : P.reason);
@@ -656,10 +459,10 @@ extern "C" int tslam_tsdf_fuse_update(tslam_tsdf_t* dst, tslam_tsdf_t* src, cons
   unsigned long long ctr[8];
   rc = fz_commit(dst, f, false, st, ctr);
   if (rc) return rc;
-  fz_record(dst, src, P);
-  z->gen = dst->write_gen;
+  ts_fz_record(dst, src, P);
+  z->gen = dst->ver.write_gen;
   z->tiled = 0;
-  fz_stats(P, ctr, stats8);
+  ts_fz_stats(P, ctr, stats8);
   return TSLAM_OK;
 }
 
@@ -696,7 +499,7 @@ static int fz_tiling(tslam_tsdf* m, const int32_t* tiles3, int32_t rank, int32_t
 extern "C" int tslam_tsdf_fuse_update_tiled_plan(tslam_tsdf_t* dst, tslam_tsdf_t* src, const int32_t* tiles3, int32_t rank, int32_t world,
                                                  const uint8_t* include, float tolerance, int32_t full, int64_t* plan3, uint8_t* present,
                                                  void* stream) {
-  int rc = fz_check_args(dst, src, tolerance);
+  int rc = fz_check_args(dst, src, tolerance, "fuse_update");
   if (rc) return rc;
   if (!plan3 || !present) { ts_set_error("fuse_update_tiled_plan: NULL plan3 or present"); return TSLAM_E_INVALID; }
   rc = fz_check_tiles(tiles3, rank, world);
@@ -707,26 +510,23 @@ extern "C" int tslam_tsdf_fuse_update_tiled_plan(tslam_tsdf_t* dst, tslam_tsdf_t
   rc = fz_tiling(dst, tiles3, rank, world, &t);
   if (rc) return rc;
   cudaStream_t st = (cudaStream_t)stream;
-  FzDev f;
-  rc = fz_open(dst, src, st, f);
+  TsDev f;
+  rc = fz_begin(dst, src, st, f);
   if (rc) return rc;
   TsFuse* z = dst->fz;
   if (z->phase >= 2) z->valid = 0;  // an update abandoned after its splat left the sums part-way
   z->phase = 0;
-  int reason = FZ_INCR;
-  if (full) reason = FZ_ASKED;
-  else if (!z->valid) reason = z->ever_valid ? FZ_INVALID : FZ_FIRST;
-  else if (z->src_serial != src->serial) reason = FZ_OTHER_SRC;
-  else if (z->gen != dst->write_gen - dst->ghost_gen) reason = FZ_DST_WRITTEN;  // owned content written; ghost imports are not
-  else if (!z->tiled || memcmp(&z->tiling, &t, sizeof(t))) reason = FZ_CUTS;
-  rc = fz_plan(dst, src, include, tolerance, reason, st, f, z->plan);
+  // owned content written; ghost imports are not
+  int reason = fz_reason(*z, full, z->ever_valid ? FZ_INVALID : FZ_FIRST, src->ver.serial, z->gen != dst->ver.write_gen - dst->ghost_gen);
+  if (reason == FZ_INCR && (!z->tiled || memcmp(&z->tiling, &t, sizeof(t)))) reason = FZ_CUTS;
+  rc = fz_plan(dst, src, f, include, tolerance, reason, st, z->plan);
   if (rc) return rc;
   const FzPlan& P = z->plan;
   for (int s = 0; s < dst->cfg.max_submaps; s++) present[s] = P.nblk[s] > 0;
   plan3[0] = P.reason;
   plan3[1] = P.cost;
   plan3[2] = P.cost_full;
-  z->plan_src = src->serial;
+  z->plan_src = src->ver.serial;
   z->plan_tiling = t;
   z->phase = 1;
   return TSLAM_OK;
@@ -738,14 +538,14 @@ extern "C" int tslam_tsdf_fuse_update_tiled_splat(tslam_tsdf_t* dst, tslam_tsdf_
   int rc = fz_phase(dst, 1, "fuse_update_tiled_splat");
   if (rc) return rc;
   TsFuse* z = dst->fz;
-  if (src->serial != z->plan_src) { ts_set_error("fuse_update_tiled_splat: src is not the map the update was planned with"); return TSLAM_E_INVALID; }
+  if (src->ver.serial != z->plan_src) { ts_set_error("fuse_update_tiled_splat: src is not the map the update was planned with"); return TSLAM_E_INVALID; }
   if (reason == FZ_INCR && z->plan.reason != FZ_INCR) {
     ts_set_error("fuse_update_tiled_splat: an incremental update where this rank's plan is full (reason %d)", z->plan.reason);
     return TSLAM_E_INVALID;
   }
   cudaStream_t st = (cudaStream_t)stream;
-  FzDev f;
-  fz_dev(z, f);  // (the plan sized it for src)
+  TsDev f;
+  fz_dev(*z, f);  // (the plan sized it for src)
   fz_settle(z->plan, reason);
   z->phase = 2;  // (from here on a failure leaves the sums invalid)
   return fz_execute(dst, src, f, z->plan, &z->plan_tiling, st);
@@ -795,8 +595,8 @@ extern "C" int tslam_tsdf_fuse_update_tiled_unpack(tslam_tsdf_t* dst, int64_t n,
   if (rc) return rc;
   TsFuse* z = dst->fz;
   cudaStream_t st = (cudaStream_t)stream;
-  FzDev f;
-  fz_dev(z, f);
+  TsDev f;
+  fz_dev(*z, f);
   const int planes = fz_planes(dst);
   if (n > 0) {
     const long long rl = 1 + (long long)planes * TS_B3;
@@ -807,7 +607,7 @@ extern "C" int tslam_tsdf_fuse_update_tiled_unpack(tslam_tsdf_t* dst, int64_t n,
     TS_CUDA(cudaMemcpyAsync(&err, dst->g.err, 4, cudaMemcpyDeviceToHost, st));
     TS_CUDA(cudaStreamSynchronize(st));
     if (err & ~TS_ERR_FUSE_MISSING) return ts_check_deferred(dst);  // pool exhausted on the owner
-    rc = fz_reserve_sums(dst, (size_t)std::min(nb, dst->g.max_blocks), st);
+    rc = fz_reserve_planes(dst, (size_t)std::min(nb, dst->g.max_blocks), st);
     if (rc) return rc;
     k_fz_unpack_add<<<(int)std::min<long long>(n, dst->sm_count * 4), 256, 0, st>>>(dst->g, fz_sums(z, planes), planes, n, (const long long*)rows);
     TS_LAUNCH_CHECK(dst);
@@ -830,17 +630,17 @@ extern "C" int tslam_tsdf_fuse_update_tiled_finish(tslam_tsdf_t* dst, tslam_tsdf
   }
   int rc = fz_phase(dst, 4, "fuse_update_tiled_finish");
   if (rc) return rc;
-  if (src->serial != z->plan_src) { ts_set_error("fuse_update_tiled_finish: src is not the map the update was planned with"); return TSLAM_E_INVALID; }
-  FzDev f;
-  fz_dev(z, f);
+  if (src->ver.serial != z->plan_src) { ts_set_error("fuse_update_tiled_finish: src is not the map the update was planned with"); return TSLAM_E_INVALID; }
+  TsDev f;
+  fz_dev(*z, f);
   unsigned long long ctr[8];
   TS_CUDA(cudaMemcpyAsync(ctr, f.ctr, sizeof(ctr), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
   TS_CUDA(cudaStreamSynchronize((cudaStream_t)stream));
-  fz_record(dst, src, z->plan);
-  z->gen = dst->write_gen - dst->ghost_gen;
+  ts_fz_record(dst, src, z->plan);
+  z->gen = dst->ver.write_gen - dst->ghost_gen;
   z->tiled = 1;
   z->tiling = z->plan_tiling;
   z->phase = 0;
-  fz_stats(z->plan, ctr, stats8);
+  ts_fz_stats(z->plan, ctr, stats8);
   return TSLAM_OK;
 }

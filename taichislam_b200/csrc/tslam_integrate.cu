@@ -795,7 +795,7 @@ static void ts_fill_frame(tslam_tsdf* m, TsFrame& fr, const float* R9, const flo
   memcpy(fr.R, R9, 36);
   memcpy(fr.T, T3, 12);
   fr.submap = submap;
-  ts_map_written(m, submap);
+  fz_written(m->ver, submap);
   m->frame_seq++;  // 1, 2, ... (texture: later frames win); < 2^22 - TSLAM_MAX_BATCH (ts_seq_renorm runs before that)
   fr.seq = m->frame_seq;
 }

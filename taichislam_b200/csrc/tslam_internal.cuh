@@ -560,6 +560,20 @@ struct TsMarchWs {
   float near_eps;      // |frac - 0.5| below this -> exact index path
 };
 
+// Change tracking of a map as a source or destination of the incremental fusions (tslam_tsdf_fuse_update,
+// tslam_octo_fuse_update).  Every entry that writes a submap's voxels calls fz_written, which bumps that submap's content
+// version and the map's write generation; an update compares both against what it recorded when it last ran.
+struct FzVer {
+  unsigned long long serial;        // process-unique number of the handle (an address can be reused by a new handle)
+  unsigned long long write_gen;     // writes of the map by any entry other than the incremental fusion into it
+  unsigned long long* content_ver;  // [n] host: writes of each submap's voxels
+  int n;                            // max_submaps
+};
+// tslam_fuse.cu: at create (a fresh serial, versions zero) and destroy
+void fz_ver_init(FzVer& v, int max_submaps);
+void fz_ver_free(FzVer& v);
+void fz_written(FzVer& v, int submap);  // submap's voxels were written (submap < 0: every submap)
+
 // host-side handle
 struct tslam_tsdf {
   tslam_tsdf_config_t cfg;
@@ -648,13 +662,8 @@ struct tslam_tsdf {
   size_t traj_mem_bytes;
   void* rc_mem;        // keep flags, scan, hole / mover lists and counters of tslam_tsdf_reclaim (tslam_reclaim.cu), grown geometrically
   size_t rc_bytes;
-  // Change tracking of the incremental global fusion (tslam_tsdf_fuse_update, tslam_fuse.cu).  Every entry that writes a
-  // submap's planes calls ts_map_written, which bumps that submap's content version and the map's write generation;
-  // the update compares both against what it recorded when it last ran.
-  unsigned long long serial;        // process-unique number of the handle (an address can be reused by a new handle)
-  unsigned long long write_gen;     // writes of the planes by any entry other than tslam_tsdf_fuse_update
+  FzVer ver;                        // change tracking of the incremental fusion (writes of the tw / obs / occ / col planes)
   unsigned long long ghost_gen;     // ... of which ghost imports (tslam_tsdf_ghost_unpack): the tiled update ignores them
-  unsigned long long* content_ver;  // [max_submaps] host: writes of each submap's planes
   struct TsFuse* fz;                // state of this map as the destination of tslam_tsdf_fuse_update (first call allocates)
   int march_verify;    // TSLAM_MARCH_VERIFY=1: every fast-path index is re-computed exactly, mismatches counted
   bool clamp_on_commit;
@@ -815,16 +824,10 @@ struct tslam_octo {
   // inputs, outputs and solver work of tslam_octo_esdf_trajectory (tslam_traj.cuh), grown geometrically
   void* traj_mem;
   size_t traj_mem_bytes;
-  // change tracking of the incremental Octomap fusion (tslam_octo_fuse_update, tslam_octo_fuse.cu)
-  unsigned long long serial;        // process-unique handle number
-  unsigned long long write_gen;     // writes of the map by any entry other than tslam_octo_fuse_update
-  unsigned long long* content_ver;  // [max_submaps] host: writes of each submap's voxels
-  struct OcFuse* ofz;               // state of this map as a fusion destination; NULL until its first update
+  FzVer ver;                        // change tracking of the incremental fusion (writes of the cnt / cw planes)
+  struct FzState* fz;               // state of this map as the destination of tslam_octo_fuse_update (first call allocates)
 };
 int oc_esdf_free(tslam_octo* m);      // tslam_octo_esdf.cu
-// tslam_octo_fuse.cu: submap's voxels were written (submap < 0: every submap); free the fusion state at destroy
-void oc_map_written(tslam_octo* m, int submap);
-void oc_fuse_free(tslam_octo* m);
 int oc_frontier_free(tslam_octo* m);  // tslam_octo_frontier.cu
 int oc_view_free(tslam_octo* m);      // tslam_octo_view.cu
 int oc_travel_free(tslam_octo* m);    // tslam_octo_travel.cu
@@ -988,10 +991,7 @@ int ts_check_tex(tslam_tsdf* m, const uint8_t* tex, int th, int tw);  // a colou
 int ts_integrate_depth_impl(tslam_tsdf_t* m, const uint16_t* depth, int mem, int32_t n_frames, int32_t h, int32_t w, const float* R9s,
                             const float* T3s, const int32_t* submap_ids, int flags, void* stream, const uint8_t* tex = nullptr, int th = 0,
                             int tw = 0);
-// tslam_fuse.cu: change tracking of the incremental global fusion (tslam_tsdf::serial, write_gen, content_ver)
-int ts_fuse_init(tslam_tsdf* m);                         // at create: serial and content versions
-void ts_fuse_free(tslam_tsdf* m);                        // at destroy
-void ts_map_written(tslam_tsdf* m, int submap);          // submap's planes were written (submap < 0: every submap)
+void ts_fuse_free(tslam_tsdf* m);                        // tslam_fuse.cu: the fusion state, at destroy
 // the fusion sum planes of m as a destination (tslam_reclaim.cu moves them with their blocks): sums = null when none
 struct TsFuseView {
   long long* sums;    // planes x cap_blocks x 4096 int64, plane after plane

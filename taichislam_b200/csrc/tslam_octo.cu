@@ -379,7 +379,6 @@ static int oc_create(const tslam_octo_config_t* cfg, const tslam_octo_logodds_t*
   tslam_octo* m = new tslam_octo();
   memset(m, 0, sizeof(*m));
   m->cfg = *cfg;
-  m->serial = ts_next_serial();
   int dev = 0;
   TS_CUDA(cudaGetDevice(&dev));
   cudaDeviceProp prop;
@@ -390,7 +389,7 @@ static int oc_create(const tslam_octo_config_t* cfg, const tslam_octo_logodds_t*
   if (m->cfg.max_points <= 0) m->cfg.max_points = 1 << 20;
   if (m->cfg.max_blocks <= 0) m->cfg.max_blocks = 1 << 18;  // 262144 blocks x 2 KB = 512 MB
   if (m->cfg.max_blocks > TS_MAX_BLOCKS) m->cfg.max_blocks = TS_MAX_BLOCKS;
-  m->content_ver = new unsigned long long[m->cfg.max_submaps]();
+  fz_ver_init(m->ver, m->cfg.max_submaps);
   m->in.fx = (float)cfg->fx; m->in.fy = (float)cfg->fy; m->in.cx = (float)cfg->cx; m->in.cy = (float)cfg->cy;
   m->in.dmin_mm = (float)(cfg->min_ray_length * 1000.0);
   m->in.dmax_mm = (float)(cfg->max_ray_length * 1000.0);
@@ -474,8 +473,8 @@ extern "C" int tslam_octo_destroy(tslam_octo_t* m) {
   oc_view_free(m);
   oc_travel_free(m);
   if (m->traj_mem) cudaFree(m->traj_mem);
-  oc_fuse_free(m);
-  delete[] m->content_ver;
+  fz_free(m->fz);
+  fz_ver_free(m->ver);
   delete m;
   return TSLAM_OK;
 }
@@ -492,7 +491,7 @@ extern "C" int tslam_octo_reset(tslam_octo_t* m, void* stream) {
   if (nb && m->g.cw) TS_CUDA(cudaMemsetAsync(m->g.cw, 0, (size_t)nb * OC_B3 * 8, st));
   TS_CUDA(cudaMemsetAsync(m->scratch_i, 0, 4 * 4, st));
   oc_track_invalidate_all(m);
-  oc_map_written(m, -1);
+  fz_written(m->ver, -1);
   return TSLAM_OK;
 }
 
@@ -630,13 +629,13 @@ extern "C" int tslam_octo_integrate_points_rgb(tslam_octo_t* m, const float* xyz
   oc_fill_frame(m, fr, R9, T3, submap);
   if (m->logodds) {
     if (n > m->ray_cap) { ts_set_error("n=%d exceeds the ray records of a log-odds map (%d)", n, m->ray_cap); return TSLAM_E_INVALID; }
-    oc_map_written(m, submap);
+    fz_written(m->ver, submap);
     TS_CUDA(cudaMemsetAsync(m->lo.ctr, 0, 8, st));
     k_octo_lo_points<<<(n + 255) / 256, 256, 0, st>>>(m->g, m->lo, src, n, fr, m->in.vs, csrc);
     TS_LAUNCH_CHECK(m);
     return oc_lo_finish(m, fr, n, st);
   }
-  oc_map_written(m, submap);
+  fz_written(m->ver, submap);
   k_octo_points<<<(n + 255) / 256, 256, 0, st>>>(m->g, src, n, fr, m->in.vs, csrc);
   TS_LAUNCH_CHECK(m);
   return TSLAM_OK;
@@ -670,7 +669,7 @@ extern "C" int tslam_octo_integrate_depth_tex(tslam_octo_t* m, const uint16_t* d
   }
   TsFrame fr;
   oc_fill_frame(m, fr, R9, T3, submap);
-  oc_map_written(m, submap);
+  fz_written(m->ver, submap);
   if (m->logodds) {
     TS_CUDA(cudaMemsetAsync(m->lo.ctr, 0, 8, st));
     k_octo_lo_depth<<<(hh * ww + 255) / 256, 256, 0, st>>>(m->g, m->lo, src, h, w, hh, ww, fr, m->in, tsrc, th, tw);

@@ -320,7 +320,7 @@ static int ts_queue_end(tslam_tsdf* m, const float* R9, const float* T3, int32_t
   memcpy(m->q_R + 9 * q, R9, 36);
   memcpy(m->q_T + 3 * q, T3, 12);
   m->q_s[q] = submap;
-  ts_map_written(m, submap);
+  fz_written(m->ver, submap);
   m->q_n = q + 1;
   if (m->q_n >= m->queue_launch[m->q_phase]) {
     const int ph = m->q_phase;

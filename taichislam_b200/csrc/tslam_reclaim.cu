@@ -298,7 +298,7 @@ extern "C" int tslam_tsdf_reclaim(tslam_tsdf_t* m, int32_t rules, const uint8_t*
     m->mesh_epoch++;
     m->esdf_full_needed = 1;
     for (int s = 0; s < S; s++)
-      if (h_ne[s]) ts_map_written(m, s);  // lost observed content; empty blocks are no content change
+      if (h_ne[s]) fz_written(m->ver, s);  // lost observed content; empty blocks are no content change
   }
   if (stats6) {
     stats6[0] = nb;

@@ -245,7 +245,7 @@ extern "C" int tslam_tsdf_create(const tslam_tsdf_config_t* cfg, tslam_tsdf_t** 
   // (the workspace of the block-binned march - ~2 GB for 640x480 frames - is allocated by the first integrate launch:
   // global maps that are only ever fused into never pay for it)
   { int rci = ts_integrate_init(); if (rci) return rci; }
-  { int rcf = ts_fuse_init(m); if (rcf) return rcf; }
+  fz_ver_init(m->ver, m->cfg.max_submaps);
   TS_CUDA(cudaDeviceSynchronize());
   *out = m;
   return TSLAM_OK;
@@ -276,6 +276,7 @@ extern "C" int tslam_tsdf_destroy(tslam_tsdf_t* m) {
   if (m->bcnt) cudaFree(m->bcnt);
   cudaFree(m->depth_stage); cudaFree(m->points_stage);
   ts_queue_free(m);
+  fz_ver_free(m->ver);
   ts_fuse_free(m);
   if (m->mw.rays) ts_march_free(m);
   cudaFree(m->counters); cudaFree(m->pose_R); cudaFree(m->pose_T); cudaFree(m->colormap);
@@ -294,7 +295,7 @@ extern "C" int tslam_tsdf_reset(tslam_tsdf_t* m, void* stream) {
   m->mesh_epoch++;           // ... and the incremental mesh (planes cleared and pool slots recycled without stamps)
   m->q_n = 0;                // ... and so are queued frames
   m->q_gathered = 0;
-  ts_map_written(m, -1);     // ... and every submap's content
+  fz_written(m->ver, -1);    // ... and every submap's content
   TS_CUDA(cudaMemcpyAsync(&nb, g.n_blocks, 4, cudaMemcpyDeviceToHost, st));
   TS_CUDA(cudaStreamSynchronize(st));
   if (nb > g.max_blocks) nb = g.max_blocks;
@@ -450,7 +451,7 @@ extern "C" int tslam_tsdf_scatter2(tslam_tsdf_t* m, int32_t submap, int64_t n, c
   if (grid > m->sm_count * 32) grid = m->sm_count * 32;
   m->esdf_full_needed = 1;  // bulk load: values change without a commit
   m->mesh_epoch++;          // (same for the incremental mesh)
-  ts_map_written(m, submap);
+  fz_written(m->ver, submap);
   k_scatter<<<grid, 256, 0, st>>>(m->g, submap, n, idx, tsdf, w, occ, color);
   TS_LAUNCH_CHECK(m);
   return TSLAM_OK;

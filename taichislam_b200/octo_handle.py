@@ -450,14 +450,9 @@ class OctoHandle:
         poses.  include: None (all) or bools / 0-1 per submap (up to max_submaps); tolerance: how far (metres,
         translation + angle x radius) a fused submap may move before it is placed again; full=True forces a rebuild.
         -> dict of the call's statistics (TsdfHandle.fuse_update's keys; voxels_skipped counts recoloured voxels)."""
-        from .tsdf_handle import _fuse_stats
-        inc = None
-        if include is not None:
-            n = int(self.cfg.max_submaps) if 0 < int(self.cfg.max_submaps) <= 1024 else 1024
-            a = np.asarray(include).reshape(-1).astype(bool)
-            assert a.shape[0] <= n, "include has more entries than max_submaps"
-            inc = np.zeros(n, np.uint8)
-            inc[:a.shape[0]] = a
+        from .tsdf_handle import _fuse_stats, _include_u8
+        n = int(self.cfg.max_submaps)
+        inc = _include_u8(include, n if 0 < n <= 1024 else 1024)  # the table size the map was created with
         st = np.zeros(8, np.int64)
         capi.check(self.L.tslam_octo_fuse_update(self.h, src.h, capi.np_ptr(inc) if inc is not None else None, float(tolerance),
                                                  int(bool(full)), capi.np_ptr(st), capi.stream_ptr()))

@@ -241,14 +241,7 @@ class TsdfHandle:
 
     def include_u8(self, include):
         """include of the fusion updates (None or bools / 0-1 per submap) -> None or u8[max_submaps]."""
-        if include is None:
-            return None
-        n = int(self.cfg.max_submaps)
-        a = np.asarray(include).reshape(-1).astype(bool)
-        assert a.shape[0] <= n, "include has more entries than max_submaps"
-        inc = np.zeros(n, np.uint8)
-        inc[:a.shape[0]] = a
-        return inc
+        return _include_u8(include, int(self.cfg.max_submaps))
 
     # -- incremental fusion of a tiled global map, phase by phase (tslam_tsdf_fuse_update_tiled_*) ------------------
     # distributed.TiledGlobalMap.update_fused_submaps drives these on every rank; each raises capi.TslamError.
@@ -619,6 +612,17 @@ class TsdfHandle:
         capi.check(self.L.tslam_tsdf_get_march_stats2(self.h, capi.np_ptr(o)))
         return dict(n_segs=int(o[0]), n_items=int(o[1]), n_slow=int(o[2]), n_fallback=int(o[3]), n_generic=int(o[4]),
                     n_verify_bad=int(o[5]), n_seg_guard=int(o[6]))
+
+
+def _include_u8(include, n):
+    """include of the fusion updates (None or bools / 0-1 per submap) -> None or u8[n], n the submap table size."""
+    if include is None:
+        return None
+    a = np.asarray(include).reshape(-1).astype(bool)
+    assert a.shape[0] <= n, "include has more entries than max_submaps"
+    inc = np.zeros(n, np.uint8)
+    inc[:a.shape[0]] = a
+    return inc
 
 
 def _fuse_stats(st, reasons):

@@ -16,6 +16,8 @@ import ctypes as C
 
 import numpy as np
 
+from . import _capi as capi
+
 
 def balanced_tiling(hist, world):
     """Data-driven tiling: `hist` = int[3,1024] marginal histograms of the occupied block coordinates (+512), summed over
@@ -111,7 +113,6 @@ _UPDATE_SUMS = ("added", "moved", "removed", "within_tolerance", "voxels_splatte
 def _attempt(fn, *args):
     """(0, fn(*args)), or (error code, message) when the library refuses or fails: a phase that fails on one rank must
     still reach the collective where the ranks agree on it."""
-    from . import _capi as capi
     try:
         return 0, fn(*args)
     except capi.TslamError as e:
@@ -220,14 +221,12 @@ class TiledGlobalMap:
         return self.m._h.h
 
     def owner_of_block(self, bx, by, bz):
-        from . import _capi as capi
         o = C.c_int32(0)
         capi.check(self._L().tslam_tiling_owner(self._h(), self._tiles_c, self.world, int(bx), int(by), int(bz), C.byref(o)))
         return int(o.value)
 
     def set_tiling(self, tiles, cuts):
         """Install a tiling on this rank (every rank must install the same one)."""
-        from . import _capi as capi
         self.tiles = tuple(int(t) for t in tiles)
         self._tiles_c = (C.c_int32 * 3)(*self.tiles)
         self.cuts = cuts
@@ -240,7 +239,6 @@ class TiledGlobalMap:
     # ---- fusion, phase by phase -------------------------------------------------------------------------
     def fusion_splat(self, submaps):
         """Phase 1: splat this rank's submaps (sums pending) and return the marginal histograms of the touched blocks."""
-        from . import _capi as capi
         L, h, st = self._L(), self._h(), capi.stream_ptr()
         submaps._flush()
         capi.check(L.tslam_tsdf_fuse_pending(h, submaps._h.h, st))  # (resets the global map first, dense_tsdf.py:313)
@@ -251,28 +249,21 @@ class TiledGlobalMap:
     def fusion_pack(self):
         """Phase 2: blocks that fell into a foreign tile -> (send counts, (keys, acc, obs, occ[, col])) grouped by owner."""
         import torch
-        from . import _capi as capi
         L, h, st = self._L(), self._h(), capi.stream_ptr()
-        dev = torch.device("cuda", torch.cuda.current_device())
-        send = np.zeros(self.world, np.int32)
-        capi.check(L.tslam_tsdf_foreign_count(h, self._tiles_c, self.rank, self.world, capi.np_ptr(send), st))
-        n_send = int(send.sum())
-        keys = torch.empty(max(n_send, 1), dtype=torch.int64, device=dev)
-        acc = torch.empty((max(n_send, 1), 4096, 2), dtype=torch.float32, device=dev)
-        obs = torch.empty((max(n_send, 1), 4096), dtype=torch.uint8, device=dev)
-        occ = torch.empty((max(n_send, 1), 4096), dtype=torch.int8, device=dev)
         tex = bool(getattr(self.m, "enable_texture", False))
-        col = torch.empty((max(n_send, 1), 4096, 4), dtype=torch.float32, device=dev) if tex else None
-        capi.check(L.tslam_tsdf_foreign_pack2(h, self._tiles_c, self.rank, self.world, capi.np_ptr(send), n_send, capi.tptr(keys),
-                                              capi.tptr(acc), capi.tptr(obs), capi.tptr(occ), capi.tptr(col), st))
-        bufs = (keys[:n_send], acc[:n_send], obs[:n_send], occ[:n_send]) + ((col[:n_send],) if tex else ())
+        send, bufs = capi.pack(
+            lambda send: L.tslam_tsdf_foreign_count(h, self._tiles_c, self.rank, self.world, send, st),
+            lambda send, n, keys, acc, obs, occ, col=None: L.tslam_tsdf_foreign_pack2(h, self._tiles_c, self.rank, self.world, send, n,
+                                                                                       keys, acc, obs, occ, col, st),
+            self.world, ((), torch.int64), ((4096, 2), torch.float32), ((4096,), torch.uint8), ((4096,), torch.int8),
+            *([((4096, 4), torch.float32)] if tex else []))
+        n_send = int(send.sum())
         self.last_exchange = {"fusion_blocks_sent": n_send, "fusion_bytes_sent": n_send * (8 + 4096 * (10 + (16 if tex else 0)))}
         return send, bufs
 
     def fusion_unpack(self, bufs):
         """Phase 3: add the received blocks, commit this rank's tile."""
         import torch
-        from . import _capi as capi
         L, h, st = self._L(), self._h(), capi.stream_ptr()
         n_recv = int(bufs[0].shape[0])
         col = bufs[4] if len(bufs) > 4 else None
@@ -287,7 +278,7 @@ class TiledGlobalMap:
         """fuse_submaps (dense_tsdf.py:312-318) with the result tiled over the ranks.  `submaps` = this rank's
         submap collection; the pose table of the global map must hold the poses of the submaps it contains."""
         import torch
-        dev = torch.device("cuda", torch.cuda.current_device())
+        dev = capi.device()
         hist = self.fusion_splat(submaps)
         if self.balance:
             ht = torch.as_tensor(hist.astype(np.int64), device=dev)
@@ -316,7 +307,6 @@ class TiledGlobalMap:
     def update_splat(self, submaps, reason):
         """Phase 2: splat with the merged reason.  A full update with balanced cuts returns the marginal histograms of
         the blocks its additions activated (to be summed over the ranks for balanced_tiling), else None."""
-        from . import _capi as capi
         self.m._h.fuse_update_tiled_splat(submaps._h, reason)
         if not (reason and self.balance):
             return None
@@ -347,7 +337,6 @@ class TiledGlobalMap:
     def _agree(self, submaps, rc, msg, dev):
         """Every rank learns whether a phase failed anywhere; if so every rank abandons the update and raises."""
         import torch
-        from . import _capi as capi
         t = torch.tensor([int(rc)], dtype=torch.int64, device=dev)
         self.dist.all_reduce(t, op=self.dist.ReduceOp.MIN)
         worst = int(t.item())
@@ -363,10 +352,9 @@ class TiledGlobalMap:
         Only a full update with balanced cuts moves the cuts.  Returns fuse_update's statistics summed over the ranks
         (reason: the same on every rank) plus foreign_blocks_sent / _received and bytes_sent."""
         import torch
-        from . import _capi as capi
-        dev = torch.device("cuda", torch.cuda.current_device())
+        dev = capi.device()
         self.last_exchange = {}
-        width = 3 + 2 * int(self.m._h.cfg.max_submaps)
+        width = 3 + 2 * capi.submap_table(self.m._h.cfg.max_submaps)
         rc, row = _attempt(self.update_plan, submaps, include, tolerance, full)
         mine = torch.as_tensor(np.concatenate([[rc], row if rc == 0 else np.zeros(width, np.int64)]), dtype=torch.int64, device=dev)
         parts = [torch.empty_like(mine) for _ in range(self.world)]
@@ -401,25 +389,18 @@ class TiledGlobalMap:
     # ---- halo + mesh --------------------------------------------------------------------------------------
     def halo_pack(self):
         import torch
-        from . import _capi as capi
         L, h, st = self._L(), self._h(), capi.stream_ptr()
-        dev = torch.device("cuda", torch.cuda.current_device())
-        send = np.zeros(self.world, np.int32)
-        capi.check(L.tslam_tsdf_halo_count(h, self._tiles_c, self.rank, self.world, capi.np_ptr(send), st))
-        n_send = int(send.sum())
-        keys = torch.empty(max(n_send, 1), dtype=torch.int64, device=dev)
-        tw = torch.empty((max(n_send, 1), 4096, 2), dtype=torch.float32, device=dev)
-        obs = torch.empty((max(n_send, 1), 4096), dtype=torch.uint8, device=dev)
         tex = bool(getattr(self.m, "enable_texture", False))
-        col = torch.empty((max(n_send, 1), 4096, 4), dtype=torch.float32, device=dev) if tex else None
-        capi.check(L.tslam_tsdf_halo_pack2(h, self._tiles_c, self.rank, self.world, capi.np_ptr(send), n_send, capi.tptr(keys),
-                                           capi.tptr(tw), capi.tptr(obs), capi.tptr(col), st))
-        self.last_exchange["halo_blocks_sent"] = n_send
-        return send, (keys[:n_send], tw[:n_send], obs[:n_send]) + ((col[:n_send],) if tex else ())
+        send, bufs = capi.pack(
+            lambda send: L.tslam_tsdf_halo_count(h, self._tiles_c, self.rank, self.world, send, st),
+            lambda send, n, keys, tw, obs, col=None: L.tslam_tsdf_halo_pack2(h, self._tiles_c, self.rank, self.world, send, n, keys, tw,
+                                                                              obs, col, st),
+            self.world, ((), torch.int64), ((4096, 2), torch.float32), ((4096,), torch.uint8), *([((4096, 4), torch.float32)] if tex else []))
+        self.last_exchange["halo_blocks_sent"] = int(send.sum())
+        return send, bufs
 
     def halo_unpack(self, bufs):
         import torch
-        from . import _capi as capi
         L, h, st = self._L(), self._h(), capi.stream_ptr()
         n_recv = int(bufs[0].shape[0])
         col = bufs[3] if len(bufs) > 3 else None
@@ -429,8 +410,7 @@ class TiledGlobalMap:
         self._halo_current = True
 
     def exchange_halo(self):
-        import torch
-        dev = torch.device("cuda", torch.cuda.current_device())
+        dev = capi.device()
         send, bufs = self.halo_pack()
         recv = exchange_counts(self.dist, send, dev)
         self.halo_unpack(tuple(exchange_rows(self.dist, b, send, recv) for b in bufs))
@@ -462,18 +442,13 @@ class TiledGlobalMap:
     def esdf_halo_pack(self):
         """Owned boundary blocks whose ESDF changed since they were last packed -> (send counts, (keys, esdf))."""
         import torch
-        from . import _capi as capi
         L, h, st = self._L(), self._h(), capi.stream_ptr()
-        dev = torch.device("cuda", torch.cuda.current_device())
-        send = np.zeros(self.world, np.int32)
-        capi.check(L.tslam_esdf_halo_count(h, self._tiles_c, self.rank, self.world, capi.np_ptr(send), st))
-        n_send = int(send.sum())
-        keys = torch.empty(max(n_send, 1), dtype=torch.int64, device=dev)
-        esdf = torch.empty((max(n_send, 1), 4096), dtype=torch.float32, device=dev)
-        capi.check(L.tslam_esdf_halo_pack(h, self._tiles_c, self.rank, self.world, capi.np_ptr(send), n_send, capi.tptr(keys),
-                                          capi.tptr(esdf), st))
-        self.last_exchange["esdf_blocks_sent"] = self.last_exchange.get("esdf_blocks_sent", 0) + n_send
-        return send, (keys[:n_send], esdf[:n_send])
+        send, bufs = capi.pack(
+            lambda send: L.tslam_esdf_halo_count(h, self._tiles_c, self.rank, self.world, send, st),
+            lambda send, n, keys, esdf: L.tslam_esdf_halo_pack(h, self._tiles_c, self.rank, self.world, send, n, keys, esdf, st),
+            self.world, ((), torch.int64), ((4096,), torch.float32))
+        self.last_exchange["esdf_blocks_sent"] = self.last_exchange.get("esdf_blocks_sent", 0) + int(send.sum())
+        return send, bufs
 
     def esdf_halo_unpack(self, bufs):
         import torch
@@ -491,7 +466,7 @@ class TiledGlobalMap:
         rank; rounds = exchange rounds in which some rank sent a block.  Runs a TSDF halo exchange first unless one
         has run since the last fusion.  Raises after `max_rounds` rounds."""
         import torch
-        dev = torch.device("cuda", torch.cuda.current_device())
+        dev = capi.device()
         if not self._halo_current:
             self.exchange_halo()
         self.last_exchange["esdf_blocks_sent"] = 0
@@ -515,18 +490,11 @@ class TiledGlobalMap:
     def _query_dest(self, xyz):
         """Points f32[n,3] on the device and the rank that answers each: the owner of the block holding its low
         interpolation corner; this rank for points no tile holds (they come out invalid anywhere)."""
-        import torch
-        from . import _capi as capi
-        x = self.m._h._dev_f32(xyz).reshape(-1, 3)
-        owner = torch.empty(x.shape[0], dtype=torch.int32, device=x.device)
-        capi.check(self._L().tslam_tiling_owner_points(self._h(), self._tiles_c, self.world, x.shape[0], capi.tptr(x), capi.tptr(owner),
-                                                       capi.stream_ptr()))
-        return x, torch.where(owner < 0, torch.full_like(owner, self.rank), owner).long()
+        return capi.owner_ranks(self._L().tslam_tiling_owner_points, self._h(), self._tiles_c, self.world, self.rank, xyz)
 
     def _esdf_answer(self, pts):
         """tslam_esdf_query on points routed here -> (dist|grad f32[n,4], valid u8[n])."""
         import torch
-        from . import _capi as capi
         n = pts.shape[0]
         dg = torch.empty((n, 4), dtype=torch.float32, device=pts.device)
         dist = torch.empty(n, dtype=torch.float32, device=pts.device)
@@ -551,7 +519,7 @@ class TiledGlobalMap:
     def esdf_slice_local(self, z):
         """This rank's part of the ESDF slice at height z: (xyz f32[n,3], ESDF f32[n]) torch CUDA tensors."""
         import torch
-        dev = torch.device("cuda", torch.cuda.current_device())
+        dev = capi.device()
         _, xyz, val = self.m._h.esdf_slice(z, submap=self.esdf_submap)
         return torch.from_numpy(xyz).to(dev), torch.from_numpy(val).to(dev)
 
@@ -579,8 +547,7 @@ class TiledGlobalMap:
     def _ray_rows(self, pos, dir, max_dist):
         """Rays f32[n,8] (pos, dir, max_dist, next sample 0) and their tags row * world + rank (int64[n])."""
         import torch
-        p = self.m._h._dev_f32(pos).reshape(-1, 3)
-        d = self.m._h._dev_f32(dir).reshape(-1, 3)
+        p, d = capi.to_device(pos, (-1, 3)), capi.to_device(dir, (-1, 3))
         rays = torch.zeros((p.shape[0], 8), dtype=torch.float32, device=p.device)  # (j = 0: int32 0 has the bits of 0.0f)
         rays[:, :3] = p
         rays[:, 3:6] = d
@@ -591,7 +558,6 @@ class TiledGlobalMap:
         """One round of tslam_tsdf_raycast_tiled on the rays held here -> (dest int64[n], answer f32[n,5] = hit,
         xyz, len; meaningful where dest < 0)."""
         import torch
-        from . import _capi as capi
         n, dev = rays.shape[0], rays.device
         dest = torch.empty(n, dtype=torch.int32, device=dev)
         hit = torch.empty(n, dtype=torch.uint8, device=dev)
@@ -604,18 +570,11 @@ class TiledGlobalMap:
     def _cell_dest(self, xyz):
         """Points f32[n,3] on the device and the rank that answers each: the owner of the block holding its cell; this
         rank for cells outside the volume (occupied and unobserved anywhere)."""
-        import torch
-        from . import _capi as capi
-        x = self.m._h._dev_f32(xyz).reshape(-1, 3)
-        owner = torch.empty(x.shape[0], dtype=torch.int32, device=x.device)
-        capi.check(self._L().tslam_tiling_owner_cells(self._h(), self._tiles_c, self.world, x.shape[0], capi.tptr(x), capi.tptr(owner),
-                                                      capi.stream_ptr()))
-        return x, torch.where(owner < 0, torch.full_like(owner, self.rank), owner).long()
+        return capi.owner_ranks(self._L().tslam_tiling_owner_cells, self._h(), self._tiles_c, self.world, self.rank, xyz)
 
     def _points_answer(self, pts):
         """tslam_tsdf_query_points on points routed here -> (flags u8[n],)."""
         import torch
-        from . import _capi as capi
         f = torch.empty(pts.shape[0], dtype=torch.uint8, device=pts.device)
         capi.check(self._L().tslam_tsdf_query_points(self._h(), self.m._active(), pts.shape[0], capi.tptr(pts), capi.tptr(f), capi.stream_ptr()))
         return (f,)
@@ -623,7 +582,6 @@ class TiledGlobalMap:
     def _near_answer(self, pts, voxel):
         """tslam_tsdf_query_near_occupy_tiled (reads ghosts) on points routed here -> (u8[n],)."""
         import torch
-        from . import _capi as capi
         f = torch.empty(pts.shape[0], dtype=torch.uint8, device=pts.device)
         capi.check(self._L().tslam_tsdf_query_near_occupy_tiled(self._h(), self.m._active(), pts.shape[0], capi.tptr(pts), int(voxel), capi.tptr(f),
                                                                 capi.stream_ptr()))
@@ -818,7 +776,6 @@ def run_local_update_fused_submaps(tiled, submaps, include=None, tolerance=0.0, 
     """TiledGlobalMap.update_fused_submaps on `world` virtual ranks in one process: tiled[r] / submaps[r] = rank r's
     global map wrapper and submap collection, the all-to-all replaced by slicing.  Returns the statistics summed over
     the ranks."""
-    from . import _capi as capi
     world = len(tiled)
     for t in tiled:
         t.last_exchange = {}

@@ -47,16 +47,7 @@ class MeshCache:
         first_tri int64 [n], n_tri int32 [n], full).  A superset of the blocks whose triangles changed; n_tri 0 means
         the block's mesh is now empty; full = the last update rebuilt everything (drop what was kept)."""
         import torch
-        dev = torch.device("cuda", torch.cuda.current_device())
-        n, full = C.c_int64(0), C.c_int32(0)
-        rc = self.L.tslam_mesh_updated_blocks(self.h, 0, None, None, None, C.byref(n), C.byref(full), capi.stream_ptr())
-        if rc != capi.E_CAPACITY:  # (the count alone: capacity 0)
-            capi.check(rc)
-        k = int(n.value)
-        blk = torch.empty((max(k, 1), 4), dtype=torch.int32, device=dev)
-        first = torch.empty(max(k, 1), dtype=torch.int64, device=dev)
-        cnt = torch.empty(max(k, 1), dtype=torch.int32, device=dev)
-        rc = self.L.tslam_mesh_updated_blocks(self.h, k, capi.tptr(blk), capi.tptr(first), capi.tptr(cnt), C.byref(n), C.byref(full),
-                                              capi.stream_ptr())
-        capi.check(rc)
-        return dict(blocks=blk[:k], first_tri=first[:k], n_tri=cnt[:k], full=bool(full.value))
+        full = C.c_int32(0)
+        blk, first, cnt = capi.count_fill(lambda cap, n, blk, first, cnt: self.L.tslam_mesh_updated_blocks(
+            self.h, cap, blk, first, cnt, n, C.byref(full), capi.stream_ptr()), ((4,), torch.int32), ((), torch.int64), ((), torch.int32))
+        return dict(blocks=blk, first_tri=first, n_tri=cnt, full=bool(full.value))

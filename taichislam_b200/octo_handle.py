@@ -58,98 +58,38 @@ class OctoHandle:
         capi.check(self.L.tslam_octo_set_color_intrinsics(self.h, K9[0], K9[4], K9[2], K9[5], int(bool(color_same_proj))))
 
     def integrate_points(self, xyz, R, T, submap=0, rgb=None):
-        torch = self.torch
-        if isinstance(xyz, torch.Tensor):
-            assert xyz.is_cuda and xyz.dtype == torch.float32 and xyz.is_contiguous()
-            mem, ptr, n = capi.MEM_DEVICE, capi.tptr(xyz), xyz.shape[0]
-        else:
-            xyz = np.ascontiguousarray(xyz, dtype=np.float32)
-            mem, ptr, n = capi.MEM_HOST, capi.np_ptr(xyz), xyz.shape[0]
+        xyz, mem, ptr, shape = capi.source(xyz, np.float32, (self.torch.float32,), (-1, 3))
+        n = shape[0]
         R, T = capi.f32c(R).reshape(9), capi.f32c(T).reshape(3)
-        cptr = None
+        rgb, cptr = capi.companion(rgb, mem)
         if rgb is not None:
-            if isinstance(rgb, torch.Tensor):
-                assert mem == capi.MEM_DEVICE and rgb.is_cuda and rgb.dtype == torch.uint8 and rgb.is_contiguous()
-                cptr = capi.tptr(rgb)
-            else:
-                assert mem == capi.MEM_HOST
-                rgb = np.ascontiguousarray(rgb, dtype=np.uint8)
-                cptr = capi.np_ptr(rgb)
             assert tuple(rgb.shape) == (n, 3)
         capi.check(self.L.tslam_octo_integrate_points_rgb(self.h, ptr, cptr, mem, n, capi.np_ptr(R), capi.np_ptr(T), int(submap),
                                                           capi.stream_ptr()))
         if mem == capi.MEM_HOST:
-            torch.cuda.current_stream().synchronize()  # pageable host source must outlive the copy
+            self.torch.cuda.current_stream().synchronize()  # pageable host source must outlive the copy
 
     def integrate_depth(self, depth, R, T, submap=0, texture=None):
-        torch = self.torch
-        if isinstance(depth, torch.Tensor):
-            mem, ptr, (h, w) = capi.MEM_DEVICE, capi.tptr(depth), depth.shape
-        else:
-            depth = np.ascontiguousarray(depth, dtype=np.uint16)
-            mem, ptr, (h, w) = capi.MEM_HOST, capi.np_ptr(depth), depth.shape
+        depth, mem, ptr, (h, w) = capi.source(depth, np.uint16, (self.torch.uint16, self.torch.int16))
         R, T = capi.f32c(R).reshape(9), capi.f32c(T).reshape(3)
-        tptr, th, tw = None, 0, 0
-        if texture is not None:
-            if isinstance(texture, torch.Tensor):
-                assert mem == capi.MEM_DEVICE and texture.is_cuda and texture.dtype == torch.uint8 and texture.is_contiguous()
-                tptr = capi.tptr(texture)
-            else:
-                assert mem == capi.MEM_HOST
-                texture = np.ascontiguousarray(texture, dtype=np.uint8)
-                tptr = capi.np_ptr(texture)
-            th, tw = int(texture.shape[0]), int(texture.shape[1])
+        texture, tptr = capi.companion(texture, mem)
+        th, tw = (0, 0) if texture is None else (int(texture.shape[0]), int(texture.shape[1]))
         capi.check(self.L.tslam_octo_integrate_depth_tex(self.h, ptr, tptr, mem, h, w, th, tw, capi.np_ptr(R), capi.np_ptr(T),
                                                          int(submap), capi.stream_ptr()))
         if mem == capi.MEM_HOST:
-            torch.cuda.current_stream().synchronize()
-
-    def _count_fill(self, call, *alloc, cap=None):
-        """The two-call protocol of a count-then-fill reader.  call(cap, n_ref, *ptrs) makes the C call; a probe with
-        cap 0 and NULL buffers gives the count n (unless cap is given).  Without alloc that count is the result; else
-        each (trailing shape, torch dtype) of alloc becomes a device tensor [max(n, 1), *shape], the second call fills
-        them, and they come back sliced to the rows written."""
-        torch = self.torch
-        n = C.c_int64(0)
-        if cap is None:
-            rc = call(0, C.byref(n), *(None for _ in alloc))
-            if rc not in (capi.TSLAM_OK, capi.E_CAPACITY):
-                capi.check(rc)
-            cap = int(n.value)
-            if not alloc:
-                return cap
-        dev = torch.device("cuda", torch.cuda.current_device())
-        out = [torch.empty((max(cap, 1),) + tuple(shape), dtype=dt, device=dev) for shape, dt in alloc]
-        capi.check(call(cap, C.byref(n), *(capi.tptr(t) for t in out)))
-        k = int(n.value)
-        return tuple(t[:k] for t in out)
-
-    def _input(self, a, shape, dtype="float32"):
-        """a as a contiguous CUDA tensor of `dtype` and `shape`: a torch tensor is converted on the device (no host
-        synchronisation), anything else through numpy"""
-        torch = self.torch
-        dev = torch.device("cuda", torch.cuda.current_device())
-        if isinstance(a, torch.Tensor):
-            return a.to(device=dev, dtype=getattr(torch, dtype)).reshape(shape).contiguous()
-        return torch.from_numpy(np.ascontiguousarray(np.asarray(a, dtype).reshape(shape))).to(dev)
-
-    @staticmethod
-    def _out(as_torch, *tensors):
-        """torch in -> the CUDA tensors, numpy in -> numpy arrays (one value for one tensor, else a tuple)"""
-        r = tensors if as_torch else tuple(t.cpu().numpy() for t in tensors)
-        return r if len(r) > 1 else r[0]
+            self.torch.cuda.current_stream().synchronize()
 
     def gather_device(self, submap=0, cap=None, color=False):
         torch = self.torch
         alloc = [((3,), torch.int32), ((), torch.int32)] + ([((3,), torch.float32)] if color else [])
-        return self._count_fill(lambda cap, n, idx, cnt, col=None: self.L.tslam_octo_gather2(
+        return capi.count_fill(lambda cap, n, idx, cnt, col=None: self.L.tslam_octo_gather2(
             self.h, int(submap), cap, idx, cnt, col, n, capi.stream_ptr()), *alloc, cap=cap)
 
     def gather_logodds_device(self, submap=0, color=False):
         """(idx int32[n,3], L int32[n][, color f32[n,3]]) of the known voxels of a log-odds map, on the device."""
         torch = self.torch
         alloc = [((3,), torch.int32), ((), torch.int32)] + ([((3,), torch.float32)] if color else [])
-        return self._count_fill(lambda cap, n, idx, lo, col=None: self.L.tslam_octo_gather_logodds(
+        return capi.count_fill(lambda cap, n, idx, lo, col=None: self.L.tslam_octo_gather_logodds(
             self.h, int(submap), cap, idx, lo, col, n, capi.stream_ptr()), *alloc)
 
     def gather(self, submap=0, color=False):
@@ -166,24 +106,13 @@ class OctoHandle:
                                               capi.tptr(rgb) if rgb is not None else None, capi.tptr(count), capi.stream_ptr()))
 
     def export(self, level=1, submap=0, cap=1 << 22, color=False):
-        torch = self.torch
-        dev = torch.device("cuda", torch.cuda.current_device())
-        xyz = torch.empty((cap, 3), dtype=torch.float32, device=dev)
-        rgb = torch.zeros((cap, 3), dtype=torch.float32, device=dev) if color else None
-        cnt = torch.zeros(1, dtype=torch.int32, device=dev)
-        self.extract(submap, level, xyz, cnt, rgb)
-        n = int(cnt.item())
-        if color:
-            return n, xyz[:min(n, cap)].cpu().numpy(), rgb[:min(n, cap)].cpu().numpy()
-        return n, xyz[:min(n, cap)].cpu().numpy()
+        f32 = self.torch.float32
+        alloc = [((3,), f32)] + ([((3,), f32, True)] if color else [])  # rgb stays 0 where the map has no colour
+        return capi.extract(lambda cnt, xyz, rgb=None: self.extract(submap, level, xyz, cnt, rgb), cap, *alloc)
 
     def query_flags(self, xyz, submap=0):
         """uint8 flags per point: bit0 occupied, bit1 unknown (log-odds maps; always 0 for a hit counter)."""
-        torch = self.torch
-        x = torch.from_numpy(np.ascontiguousarray(xyz, dtype=np.float32).reshape(-1, 3)).cuda()
-        f = torch.empty(x.shape[0], dtype=torch.uint8, device=x.device)
-        capi.check(self.L.tslam_octo_query_points(self.h, int(submap), x.shape[0], capi.tptr(x), capi.tptr(f), capi.stream_ptr()))
-        return f.cpu().numpy()
+        return capi.query_flags(self.L.tslam_octo_query_points, self.h, xyz, submap)
 
     def query_points(self, xyz, submap=0):
         """occupied per point; a log-odds map returns (occupied, unknown)."""
@@ -194,12 +123,7 @@ class OctoHandle:
 
     def query_near(self, xyz, voxel, submap=0):
         """is_near_pos_occupy: any occupied cell in [-voxel, voxel)^3 around each point's cell."""
-        torch = self.torch
-        x = torch.from_numpy(np.ascontiguousarray(xyz, dtype=np.float32).reshape(-1, 3)).cuda()
-        o = torch.empty(x.shape[0], dtype=torch.uint8, device=x.device)
-        capi.check(self.L.tslam_octo_query_near_occupy(self.h, int(submap), x.shape[0], capi.tptr(x), int(voxel), capi.tptr(o),
-                                                       capi.stream_ptr()))
-        return o.cpu().numpy().astype(bool)
+        return capi.near_occupy(self.L.tslam_octo_query_near_occupy, self.h, xyz, voxel, submap)
 
     def stats(self, clear=False):
         """Log-odds counters since the last clear: rays cast, in-volume miss-cell visits, hit voxels, voxels updated."""
@@ -221,22 +145,14 @@ class OctoHandle:
         """(idx int32[n,3], ESDF f32[n]) of the voxels known at the last esdf_update: numpy arrays, or torch CUDA tensors
         with as_torch."""
         torch = self.torch
-        return self._out(as_torch, *self._count_fill(lambda cap, n, idx, e: self.L.tslam_octo_esdf_gather(
+        return capi.results(as_torch, *capi.count_fill(lambda cap, n, idx, e: self.L.tslam_octo_esdf_gather(
             self.h, int(submap), cap, idx, e, n, capi.stream_ptr()), ((3,), torch.int32), ((), torch.float32)))
 
     def esdf_query(self, xyz, submap=0):
         """Trilinear ESDF and its exact gradient at points [n,3] of the submap's map frame, as of the last esdf_update:
         (dist f32[n], grad f32[n,3], valid bool[n]); dist and grad are NaN where valid is False.  A torch CUDA tensor in
         -> torch CUDA tensors out, without a host synchronisation; a numpy array in -> numpy arrays out."""
-        torch = self.torch
-        x = self._input(xyz, (-1, 3))
-        n = x.shape[0]
-        dist = torch.empty(n, dtype=torch.float32, device=x.device)
-        grad = torch.empty((n, 3), dtype=torch.float32, device=x.device)
-        valid = torch.empty(n, dtype=torch.uint8, device=x.device)
-        capi.check(self.L.tslam_octo_esdf_query(self.h, int(submap), n, capi.tptr(x), capi.tptr(dist), capi.tptr(grad),
-                                                capi.tptr(valid), capi.stream_ptr()))
-        return self._out(isinstance(xyz, torch.Tensor), dist, grad, valid.view(torch.bool))  # the kernel writes 0 / 1
+        return capi.esdf_query(self.L.tslam_octo_esdf_query, self.h, xyz, submap)
 
     def esdf_trajectory(self, ctrls, clearance, submap=0, **settings):
         """Optimise uniform cubic B-splines (control points f[N,3] each, the submap's map frame) against the occupancy
@@ -257,13 +173,13 @@ class OctoHandle:
         """(idx int32[n,3], cluster int32[n]) of the frontier voxels of the last frontier_update; cluster is the ordinal in
         frontier_clusters.  numpy arrays, or torch CUDA tensors with as_torch."""
         torch = self.torch
-        return self._out(as_torch, *self._count_fill(lambda cap, n, idx, cl: self.L.tslam_octo_frontier_gather(
+        return capi.results(as_torch, *capi.count_fill(lambda cap, n, idx, cl: self.L.tslam_octo_frontier_gather(
             self.h, int(submap), cap, idx, cl, n, capi.stream_ptr()), ((3,), torch.int32), ((), torch.int32)))
 
     def frontier_clusters(self, submap=0, as_torch=False):
         """int64[n,16] cluster records of the last frontier_update in label order (label, voxels, sum i / j / k, min i / j
         / k, max i / j / k, faces, sum of the unit offsets towards UNKNOWN x / y / z, 0)."""
-        return self._out(as_torch, *self._count_fill(self._clusters_call(submap), ((16,), self.torch.int64)))
+        return capi.results(as_torch, *capi.count_fill(self._clusters_call(submap), ((16,), self.torch.int64)))
 
     def _clusters_call(self, submap):
         return lambda cap, n, rec=None: self.L.tslam_octo_frontier_clusters(self.h, int(submap), cap, rec, n, capi.stream_ptr())
@@ -277,7 +193,7 @@ class OctoHandle:
 
     def _views(self, pos, R):
         """(as_torch, pos f32 [n,3], R f32 [n,9]) as contiguous CUDA tensors"""
-        p, r = self._input(pos, (-1, 3)), self._input(R, (-1, 9))
+        p, r = capi.to_device(pos, (-1, 3)), capi.to_device(R, (-1, 9))
         assert p.shape[0] == r.shape[0], "pos [n,3] and R [n,3,3] need the same n"
         return isinstance(pos, self.torch.Tensor), p, r
 
@@ -296,7 +212,7 @@ class OctoHandle:
                                                        capi.tptr(gain), capi.stream_ptr()))
         if not as_torch:
             self.sync()
-        return self._out(as_torch, valid.view(torch.bool), gain)
+        return capi.results(as_torch, valid.view(torch.bool), gain)
 
     def view_gain_frontier(self, pos, R, cam, submap=0):
         """Frontier gain of n views against the frontier set of the last frontier_update -> (valid bool[n], total int32[n],
@@ -305,7 +221,7 @@ class OctoHandle:
         torch = self.torch
         as_torch, p, r = self._views(pos, R)
         n = p.shape[0]
-        nc = self._count_fill(self._clusters_call(submap))
+        nc = capi.count_fill(self._clusters_call(submap))
         valid = torch.empty(n, dtype=torch.uint8, device=p.device)
         total = torch.empty(n, dtype=torch.int32, device=p.device)
         per = torch.empty((n, nc), dtype=torch.int32, device=p.device)
@@ -313,7 +229,7 @@ class OctoHandle:
         capi.check(self.L.tslam_octo_view_gain_frontier(self.h, int(submap), n, capi.tptr(p), capi.tptr(r), C.byref(c), nc,
                                                         capi.tptr(valid), capi.tptr(total), capi.tptr(per) if nc else None,
                                                         capi.stream_ptr()))
-        return self._out(as_torch, valid.view(torch.bool), total, per)
+        return capi.results(as_torch, valid.view(torch.bool), total, per)
 
     def frontier_viewpoints(self, offsets, cam, clearance=0.0, min_visible=1, top_k=1, submap=0):
         """The best top_k candidate views per frontier cluster of the last frontier_update (DESIGN.md section 7, "Frontier
@@ -324,9 +240,9 @@ class OctoHandle:
         R f32[nc,top_k,3,3]), rows in cluster ordinal order, slots at and beyond count[c] hold sample -1 and zeros.
         Torch in -> torch out without a host synchronisation; numpy in -> numpy out."""
         torch = self.torch
-        off = self._input(offsets, (-1, 3))
+        off = capi.to_device(offsets, (-1, 3))
         S, k = off.shape[0], int(top_k)
-        nc = self._count_fill(self._clusters_call(submap))
+        nc = capi.count_fill(self._clusters_call(submap))
         dev = off.device
         count = torch.empty(nc, dtype=torch.int32, device=dev)
         sample = torch.empty((nc, max(k, 0)), dtype=torch.int32, device=dev)
@@ -338,7 +254,7 @@ class OctoHandle:
         capi.check(self.L.tslam_octo_frontier_viewpoints(self.h, int(submap), C.byref(c), S, capi.tptr(off), float(clearance),
                                                          int(min_visible), k, nc, ptr(count), ptr(sample), ptr(visible), ptr(pos),
                                                          ptr(R), capi.stream_ptr()))
-        return self._out(isinstance(offsets, torch.Tensor), count, sample, visible, pos, R)
+        return capi.results(isinstance(offsets, torch.Tensor), count, sample, visible, pos, R)
 
     # -- travel cost on a log-odds map (tslam_octo_travel_*, DESIGN.md section 7) --------------------------------------
     def travel_limit(self):
@@ -360,25 +276,25 @@ class OctoHandle:
         """(idx int32[n,3], cost f32[n]) of the cells reachable at the last travel_update: numpy arrays, or torch CUDA
         tensors with as_torch."""
         torch = self.torch
-        return self._out(as_torch, *self._count_fill(lambda cap, n, idx, g: self.L.tslam_octo_travel_gather(
+        return capi.results(as_torch, *capi.count_fill(lambda cap, n, idx, g: self.L.tslam_octo_travel_gather(
             self.h, int(submap), cap, idx, g, n, capi.stream_ptr()), ((3,), torch.int32), ((), torch.float32)))
 
     def travel_query(self, xyz, submap=0):
         """Travel cost f32[n] of the cells of points [n,3] as of the last travel_update (+inf where unreachable).  A torch
         CUDA tensor in -> a torch CUDA tensor out, without a host synchronisation; a numpy array in -> a numpy array out."""
         torch = self.torch
-        x = self._input(xyz, (-1, 3))
+        x = capi.to_device(xyz, (-1, 3))
         n = x.shape[0]
         cost = torch.empty(n, dtype=torch.float32, device=x.device)
         capi.check(self.L.tslam_octo_travel_query(self.h, int(submap), n, capi.tptr(x), capi.tptr(cost), capi.stream_ptr()))
-        return self._out(isinstance(xyz, torch.Tensor), cost)
+        return capi.results(isinstance(xyz, torch.Tensor), cost)
 
     def travel_path(self, xyz, submap=0, max_len=4096):
         """Paths from the cells of targets [n,3] back to the start of the last travel_update -> (cells int32[n,max_len,3]
         target -> start, len int32[n]: the full cell count, 0 when unreachable; rows beyond min(len, max_len) are
         undefined).  Torch in -> torch out without a host synchronisation; numpy in -> numpy out."""
         torch = self.torch
-        as_torch, x = isinstance(xyz, torch.Tensor), self._input(xyz, (-1, 3))
+        as_torch, x = isinstance(xyz, torch.Tensor), capi.to_device(xyz, (-1, 3))
         n = x.shape[0]
         cells = torch.empty((n, int(max_len), 3), dtype=torch.int32, device=x.device)
         ln = torch.empty(n, dtype=torch.int32, device=x.device)
@@ -386,7 +302,7 @@ class OctoHandle:
                                                  capi.stream_ptr()))
         if not as_torch:
             self.sync()
-        return self._out(as_torch, cells, ln)
+        return capi.results(as_torch, cells, ln)
 
     def travel_multi_update(self, submap, starts, clearance=0.0, max_cost=None):
         """Travel-cost fields of `submap` from each of S starts [S,3] (metres, submap frame; 1 <= S <= 1024) in one update,
@@ -408,11 +324,11 @@ class OctoHandle:
         unreachable); the starts themselves give the S x S matrix.  Torch in -> torch out without a host
         synchronisation; numpy in -> numpy out."""
         torch = self.torch
-        x = self._input(xyz, (-1, 3))
+        x = capi.to_device(xyz, (-1, 3))
         n = x.shape[0]
         cost = torch.empty((getattr(self, "_travel_multi_S", 0), n), dtype=torch.float32, device=x.device)
         capi.check(self.L.tslam_octo_travel_multi_query(self.h, int(submap), n, capi.tptr(x), capi.tptr(cost), capi.stream_ptr()))
-        return self._out(isinstance(xyz, torch.Tensor), cost)
+        return capi.results(isinstance(xyz, torch.Tensor), cost)
 
     def travel_multi_path(self, source, xyz, submap=0, max_len=4096):
         """Paths of pairs (source[q], xyz[q]) from the cell of the target back to starts[source[q]] of the last
@@ -420,26 +336,17 @@ class OctoHandle:
         [0, S) gets len 0 and the next sync() raises.  Torch in -> torch out without a host synchronisation; numpy in ->
         numpy out."""
         torch = self.torch
-        x, src = self._input(xyz, (-1, 3)), self._input(source, (-1,), "int32")
+        x, src = capi.to_device(xyz, (-1, 3)), capi.to_device(source, (-1,), "int32")
         n = x.shape[0]
         assert src.shape[0] == n, "source [n] and xyz [n,3] need the same n"
         cells = torch.empty((n, int(max_len), 3), dtype=torch.int32, device=x.device)
         ln = torch.empty(n, dtype=torch.int32, device=x.device)
         capi.check(self.L.tslam_octo_travel_multi_path(self.h, int(submap), n, capi.tptr(src), capi.tptr(x), int(max_len), capi.tptr(cells),
                                                        capi.tptr(ln), capi.stream_ptr()))
-        return self._out(isinstance(xyz, torch.Tensor), cells, ln)
+        return capi.results(isinstance(xyz, torch.Tensor), cells, ln)
 
     def raycast(self, pos, direction, max_dist, submap=0):
-        torch = self.torch
-        p = torch.from_numpy(np.ascontiguousarray(pos, dtype=np.float32)).cuda()
-        d = torch.from_numpy(np.ascontiguousarray(direction, dtype=np.float32)).cuda()
-        n = p.shape[0]
-        hit = torch.empty(n, dtype=torch.uint8, device=p.device)
-        xyz = torch.empty((n, 3), dtype=torch.float32, device=p.device)
-        ln = torch.empty(n, dtype=torch.float32, device=p.device)
-        capi.check(self.L.tslam_octo_raycast(self.h, int(submap), n, capi.tptr(p), capi.tptr(d), float(max_dist), capi.tptr(hit), capi.tptr(xyz),
-                                             capi.tptr(ln), capi.stream_ptr()))
-        return hit.cpu().numpy().astype(bool), xyz.cpu().numpy(), ln.cpu().numpy()
+        return capi.raycast(self.L.tslam_octo_raycast, self.h, pos, direction, max_dist, submap)
 
     def fuse_from(self, src):
         capi.check(self.L.tslam_octo_fuse(self.h, src.h, capi.stream_ptr()))
@@ -450,13 +357,7 @@ class OctoHandle:
         poses.  include: None (all) or bools / 0-1 per submap (up to max_submaps); tolerance: how far (metres,
         translation + angle x radius) a fused submap may move before it is placed again; full=True forces a rebuild.
         -> dict of the call's statistics (TsdfHandle.fuse_update's keys; voxels_skipped counts recoloured voxels)."""
-        from .tsdf_handle import _fuse_stats, _include_u8
-        n = int(self.cfg.max_submaps)
-        inc = _include_u8(include, n if 0 < n <= 1024 else 1024)  # the table size the map was created with
-        st = np.zeros(8, np.int64)
-        capi.check(self.L.tslam_octo_fuse_update(self.h, src.h, capi.np_ptr(inc) if inc is not None else None, float(tolerance),
-                                                 int(bool(full)), capi.np_ptr(st), capi.stream_ptr()))
-        return _fuse_stats(st, capi.FUSE_REASONS)
+        return capi.fuse_update(self.L.tslam_octo_fuse_update, self, src, include, tolerance, full)
 
     def sync(self):
         capi.check(self.L.tslam_octo_sync(self.h, capi.stream_ptr()))

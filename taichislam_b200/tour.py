@@ -22,8 +22,7 @@ def solve_open_tour(C, restarts=64, seed=0, max_passes=None):
             raise ValueError("solve_open_tour needs a CUDA tensor or a numpy array")
         c = C.detach().to(torch.float32).contiguous()
     else:
-        c = torch.from_numpy(np.ascontiguousarray(np.asarray(C, np.float32))).to(
-            torch.device("cuda", torch.cuda.current_device()))
+        c = torch.from_numpy(np.ascontiguousarray(np.asarray(C, np.float32))).to(capi.device())
     if c.dim() != 2 or c.shape[0] != c.shape[1]:
         raise ValueError(f"the cost matrix must be [n, n], not {tuple(c.shape)}")
     n, R = int(c.shape[0]), int(restarts)

@@ -61,13 +61,7 @@ class TsdfHandle:
     def integrate_depth(self, depth, Rs, Ts, submaps=None, commit=True, texture=None):
         """depth: uint16 [n,h,w] (or [h,w]) numpy (host) or torch CUDA tensor; Rs [n,3,3]; Ts [n,3];
         texture: uint8 [n,th,tw,3] in the same memory space as depth (textured maps)."""
-        torch = self.torch
-        if isinstance(depth, torch.Tensor):
-            assert depth.is_cuda and depth.dtype in (torch.uint16, torch.int16) and depth.is_contiguous()
-            mem, ptr, shape = capi.MEM_DEVICE, capi.tptr(depth), tuple(depth.shape)
-        else:
-            depth = np.ascontiguousarray(depth, dtype=np.uint16)
-            mem, ptr, shape = capi.MEM_HOST, capi.np_ptr(depth), depth.shape
+        depth, mem, ptr, shape = capi.source(depth, np.uint16, (self.torch.uint16, self.torch.int16))
         if len(shape) == 2:
             shape = (1,) + tuple(shape)
         n, h, w = shape
@@ -76,48 +70,26 @@ class TsdfHandle:
         sm = None
         if submaps is not None:
             sm = np.ascontiguousarray(np.broadcast_to(np.asarray(submaps, dtype=np.int32), (n,)))
+        texture, tptr = capi.companion(texture, mem)
+        tshape = (0, 0, 0, 3)
         if texture is not None:
-            if isinstance(texture, torch.Tensor):
-                assert mem == capi.MEM_DEVICE and texture.is_cuda and texture.dtype == torch.uint8 and texture.is_contiguous()
-                tptr, tshape = capi.tptr(texture), tuple(texture.shape)
-            else:
-                assert mem == capi.MEM_HOST
-                texture = np.ascontiguousarray(texture, dtype=np.uint8)
-                tptr, tshape = capi.np_ptr(texture), texture.shape
+            tshape = tuple(texture.shape)
             if len(tshape) == 3:
-                tshape = (1,) + tuple(tshape)
+                tshape = (1,) + tshape
             assert tshape[0] == n and tshape[3] == 3
-            capi.check(self.L.tslam_tsdf_integrate_depth_tex(self.h, ptr, tptr, mem, n, h, w, tshape[1], tshape[2], capi.np_ptr(Rs),
-                                                             capi.np_ptr(Ts), capi.np_ptr(sm) if sm is not None else None,
-                                                             capi.F_COMMIT if commit else 0, capi.stream_ptr()))
-            return
-        capi.check(self.L.tslam_tsdf_integrate_depth(self.h, ptr, mem, n, h, w, capi.np_ptr(Rs), capi.np_ptr(Ts),
-                                                     capi.np_ptr(sm) if sm is not None else None,
-                                                     capi.F_COMMIT if commit else 0, capi.stream_ptr()))
+        capi.check(self.L.tslam_tsdf_integrate_depth_tex(self.h, ptr, tptr, mem, n, h, w, tshape[1], tshape[2], capi.np_ptr(Rs),
+                                                         capi.np_ptr(Ts), capi.np_ptr(sm) if sm is not None else None,
+                                                         capi.F_COMMIT if commit else 0, capi.stream_ptr()))
 
     def integrate_points(self, xyz, R, T, submap=0, commit=True, rgb=None):
-        torch = self.torch
-        if isinstance(xyz, torch.Tensor):
-            assert xyz.is_cuda and xyz.dtype == torch.float32 and xyz.is_contiguous()
-            mem, ptr, n = capi.MEM_DEVICE, capi.tptr(xyz), xyz.shape[0]
-        else:
-            xyz = np.ascontiguousarray(xyz, dtype=np.float32)
-            mem, ptr, n = capi.MEM_HOST, capi.np_ptr(xyz), xyz.shape[0]
+        xyz, mem, ptr, shape = capi.source(xyz, np.float32, (self.torch.float32,), (-1, 3))
+        n = shape[0]
         R, T = capi.f32c(R).reshape(9), capi.f32c(T).reshape(3)
+        rgb, cptr = capi.companion(rgb, mem)
         if rgb is not None:
-            if isinstance(rgb, torch.Tensor):
-                assert mem == capi.MEM_DEVICE and rgb.is_cuda and rgb.dtype == torch.uint8 and rgb.is_contiguous()
-                cptr = capi.tptr(rgb)
-            else:
-                assert mem == capi.MEM_HOST
-                rgb = np.ascontiguousarray(rgb, dtype=np.uint8)
-                cptr = capi.np_ptr(rgb)
             assert tuple(rgb.shape) == (n, 3)
-            capi.check(self.L.tslam_tsdf_integrate_points_rgb(self.h, ptr, cptr, mem, n, capi.np_ptr(R), capi.np_ptr(T), int(submap),
-                                                              capi.F_COMMIT if commit else 0, capi.stream_ptr()))
-            return
-        capi.check(self.L.tslam_tsdf_integrate_points(self.h, ptr, mem, n, capi.np_ptr(R), capi.np_ptr(T), int(submap),
-                                                      capi.F_COMMIT if commit else 0, capi.stream_ptr()))
+        capi.check(self.L.tslam_tsdf_integrate_points_rgb(self.h, ptr, cptr, mem, n, capi.np_ptr(R), capi.np_ptr(T), int(submap),
+                                                          capi.F_COMMIT if commit else 0, capi.stream_ptr()))
 
     def commit(self):
         capi.check(self.L.tslam_tsdf_commit(self.h, capi.stream_ptr()))
@@ -138,47 +110,23 @@ class TsdfHandle:
         torch = self.torch
         if cap is None:
             cap = self.count_active(submap)
-        dev = torch.device("cuda", torch.cuda.current_device())
-        idx = torch.empty((max(cap, 1), 3), dtype=torch.int32, device=dev)
-        t = torch.empty(max(cap, 1), dtype=torch.float32, device=dev)
-        w = torch.empty(max(cap, 1), dtype=torch.float32, device=dev)
-        occ = torch.empty(max(cap, 1), dtype=torch.int8, device=dev)
-        n = C.c_int64(0)
-        if color:
-            col = torch.empty((max(cap, 1), 3), dtype=torch.float32, device=dev)
-            capi.check(self.L.tslam_tsdf_gather2(self.h, int(submap), cap, capi.tptr(idx), capi.tptr(t), capi.tptr(w),
-                                                 capi.tptr(occ), capi.tptr(col), C.byref(n), capi.stream_ptr()))
-            k = int(n.value)
-            return idx[:k], t[:k], w[:k], occ[:k], col[:k]
-        capi.check(self.L.tslam_tsdf_gather(self.h, int(submap), cap, capi.tptr(idx), capi.tptr(t), capi.tptr(w),
-                                            capi.tptr(occ), C.byref(n), capi.stream_ptr()))
-        k = int(n.value)
-        return idx[:k], t[:k], w[:k], occ[:k]
+        alloc = [((3,), torch.int32), ((), torch.float32), ((), torch.float32), ((), torch.int8)] + ([((3,), torch.float32)] if color else [])
+        return capi.count_fill(lambda cap, n, idx, t, w, occ, col=None: self.L.tslam_tsdf_gather2(
+            self.h, int(submap), cap, idx, t, w, occ, col, n, capi.stream_ptr()), *alloc, cap=cap)
 
     def gather(self, submap=0, color=False):
         return tuple(a.cpu().numpy() for a in self.gather_device(submap, color=color))
 
     def scatter(self, submap, idx, tsdf, w, occ, color=None):
-        torch = self.torch
-        dev = torch.device("cuda", torch.cuda.current_device())
-
-        def dv(a, dt):
-            if isinstance(a, torch.Tensor):
-                return a.to(device=dev, dtype=dt).contiguous()
-            return torch.from_numpy(np.ascontiguousarray(a)).to(device=dev).to(dt).contiguous()
-
-        idx = dv(idx, torch.int32)
-        tsdf, w = dv(tsdf, torch.float32), dv(w, torch.float32)
-        occ = dv(occ, torch.int8)
+        idx = capi.to_device(idx, (-1, 3), "int32")
         n = idx.shape[0]
+        tsdf, w = capi.to_device(tsdf, (-1,)), capi.to_device(w, (-1,))
+        occ = capi.to_device(occ, (-1,), "int8")
         if color is not None:
-            color = dv(color, torch.float32).reshape(n, 3)
-            capi.check(self.L.tslam_tsdf_scatter2(self.h, int(submap), n, capi.tptr(idx), capi.tptr(tsdf), capi.tptr(w),
-                                                  capi.tptr(occ), capi.tptr(color), capi.stream_ptr()))
-        else:
-            capi.check(self.L.tslam_tsdf_scatter(self.h, int(submap), n, capi.tptr(idx), capi.tptr(tsdf), capi.tptr(w),
-                                                 capi.tptr(occ), capi.stream_ptr()))
-        torch.cuda.current_stream().synchronize()  # the temporaries above must outlive the kernel
+            color = capi.to_device(color, (n, 3))
+        capi.check(self.L.tslam_tsdf_scatter2(self.h, int(submap), n, capi.tptr(idx), capi.tptr(tsdf), capi.tptr(w), capi.tptr(occ),
+                                              capi.tptr(color), capi.stream_ptr()))
+        self.torch.cuda.current_stream().synchronize()  # the temporaries above must outlive the kernel
 
     def fuse_from(self, src):
         capi.check(self.L.tslam_tsdf_fuse(self.h, src.h, capi.stream_ptr()))
@@ -188,11 +136,7 @@ class TsdfHandle:
         afterwards this map is the exact-sum fusion of the included submaps at their fused poses.  include: None (all) or
         bools / 0-1 per submap (up to max_submaps); tolerance: how far (metres, translation + angle x radius) a fused
         submap may move before it is re-splatted; full=True forces a rebuild.  -> dict of the call's statistics."""
-        inc = self.include_u8(include)
-        st = np.zeros(8, np.int64)
-        capi.check(self.L.tslam_tsdf_fuse_update(self.h, src.h, capi.np_ptr(inc) if inc is not None else None, float(tolerance),
-                                                 int(bool(full)), capi.np_ptr(st), capi.stream_ptr()))
-        return _fuse_stats(st, capi.FUSE_REASONS)
+        return capi.fuse_update(self.L.tslam_tsdf_fuse_update, self, src, include, tolerance, full)
 
     def reclaim(self, submaps=None, all_blocks=False, empty=False, center=None, radius=None):
         """Drop pool blocks and compact the pool in place (tslam_tsdf_reclaim).  Candidates are the blocks of `submaps`
@@ -214,13 +158,13 @@ class TsdfHandle:
                     moved=int(st[4]), blocks_after=int(st[5]))
 
     def submap_mask_u8(self, submaps):
-        """None, submap ids, or bools / 0-1 per submap -> None or u8[max_submaps]."""
+        """None, submap ids, or bools / 0-1 per submap -> None or u8[submap table size]."""
         if submaps is None:
             return None
         a = np.asarray(submaps).reshape(-1)
         if a.dtype == bool:
             return self.include_u8(a)
-        n = int(self.cfg.max_submaps)
+        n = capi.submap_table(self.cfg.max_submaps)
         ids = a.astype(np.int64)
         assert np.all((ids >= 0) & (ids < n)), "submap id out of range"
         mask = np.zeros(n, np.uint8)
@@ -229,27 +173,21 @@ class TsdfHandle:
 
     def block_keys(self):
         """The pool in slot order: int32[n_blocks, 4] rows (submap, bx, by, bz)."""
-        torch = self.torch
-        n = C.c_int64(0)
-        rc = self.L.tslam_tsdf_block_keys(self.h, 0, None, C.byref(n), capi.stream_ptr())  # the count
-        if rc != capi.E_CAPACITY:
-            capi.check(rc)
-        cap = int(n.value)
-        keys = torch.empty((max(cap, 1), 4), dtype=torch.int32, device=torch.device("cuda", torch.cuda.current_device()))
-        capi.check(self.L.tslam_tsdf_block_keys(self.h, cap, capi.tptr(keys), C.byref(n), capi.stream_ptr()))
-        return keys[:cap].cpu().numpy()
+        (keys,) = capi.count_fill(lambda cap, n, keys: self.L.tslam_tsdf_block_keys(self.h, cap, keys, n, capi.stream_ptr()),
+                                  ((4,), self.torch.int32))
+        return keys.cpu().numpy()
 
     def include_u8(self, include):
-        """include of the fusion updates (None or bools / 0-1 per submap) -> None or u8[max_submaps]."""
-        return _include_u8(include, int(self.cfg.max_submaps))
+        """include of the fusion updates (None or bools / 0-1 per submap) -> None or u8[submap table size]."""
+        return capi.include_u8(include, capi.submap_table(self.cfg.max_submaps))
 
     # -- incremental fusion of a tiled global map, phase by phase (tslam_tsdf_fuse_update_tiled_*) ------------------
     # distributed.TiledGlobalMap.update_fused_submaps drives these on every rank; each raises capi.TslamError.
     def fuse_update_tiled_plan(self, src, tiles, rank, world, include=None, tolerance=0.0, full=False):
-        """-> (plan int64[3] = this rank's full-update reason, cost, cost_full; present bool[max_submaps])."""
+        """-> (plan int64[3] = this rank's full-update reason, cost, cost_full; present bool[submap table size])."""
         inc = self.include_u8(include)
         plan = np.zeros(3, np.int64)
-        present = np.zeros(int(self.cfg.max_submaps), np.uint8)
+        present = np.zeros(capi.submap_table(self.cfg.max_submaps), np.uint8)
         t = (C.c_int32 * 3)(*tiles)
         capi.check(self.L.tslam_tsdf_fuse_update_tiled_plan(self.h, src.h, t, int(rank), int(world), capi.np_ptr(inc) if inc is not None else None,
                                                             float(tolerance), int(bool(full)), capi.np_ptr(plan), capi.np_ptr(present),
@@ -261,16 +199,14 @@ class TsdfHandle:
 
     def fuse_update_tiled_pack(self, tiles, rank, world):
         """-> (rows per destination rank int32[world], rows int64[n, 1 + planes * 4096] torch CUDA, grouped by destination)."""
-        torch = self.torch
         t = (C.c_int32 * 3)(*tiles)
-        send = np.zeros(int(world), np.int32)
-        capi.check(self.L.tslam_tsdf_foreign_count(self.h, t, int(rank), int(world), capi.np_ptr(send), capi.stream_ptr()))
-        n = int(send.sum())
         planes = 6 if self.texture_enabled else 3
-        rows = torch.empty((max(n, 1), 1 + planes * 4096), dtype=torch.int64, device=torch.device("cuda", torch.cuda.current_device()))
-        capi.check(self.L.tslam_tsdf_fuse_update_tiled_pack(self.h, t, int(rank), int(world), capi.np_ptr(send), n, capi.tptr(rows),
-                                                            capi.stream_ptr()))
-        return send, rows[:n]
+        send, (rows,) = capi.pack(
+            lambda send: self.L.tslam_tsdf_foreign_count(self.h, t, int(rank), int(world), send, capi.stream_ptr()),
+            lambda send, n, rows: self.L.tslam_tsdf_fuse_update_tiled_pack(self.h, t, int(rank), int(world), send, n, rows,
+                                                                          capi.stream_ptr()),
+            world, ((1 + planes * 4096,), self.torch.int64))
+        return send, rows
 
     def fuse_update_tiled_unpack(self, rows):
         rows = rows.contiguous()
@@ -280,7 +216,7 @@ class TsdfHandle:
         """-> this rank's statistics (as fuse_update's) when ok, else None."""
         st = np.zeros(8, np.int64)
         capi.check(self.L.tslam_tsdf_fuse_update_tiled_finish(self.h, src.h, int(bool(ok)), capi.np_ptr(st), capi.stream_ptr()))
-        return _fuse_stats(st, capi.TILED_FUSE_REASONS) if ok else None
+        return capi.fuse_stats(st, capi.TILED_FUSE_REASONS) if ok else None
 
     def extract_surface(self, submap, xyz, rgb, count):
         """Append to torch CUDA buffers xyz/rgb f32[cap,3]; count: int32[1] device counter."""
@@ -292,40 +228,22 @@ class TsdfHandle:
                                                    capi.tptr(val), capi.tptr(rgb), capi.tptr(count), capi.stream_ptr()))
 
     def surface(self, submap=0, cap=1 << 22):
-        torch = self.torch
-        dev = torch.device("cuda", torch.cuda.current_device())
-        xyz = torch.empty((cap, 3), dtype=torch.float32, device=dev)
-        rgb = torch.empty((cap, 3), dtype=torch.float32, device=dev)
-        cnt = torch.zeros(1, dtype=torch.int32, device=dev)
-        self.extract_surface(submap, xyz, rgb, cnt)
-        n = int(cnt.item())
-        k = min(n, cap)
-        return n, xyz[:k].cpu().numpy(), rgb[:k].cpu().numpy()
+        f32 = self.torch.float32
+        return capi.extract(lambda cnt, xyz, rgb: self.extract_surface(submap, xyz, rgb, cnt), cap, ((3,), f32), ((3,), f32))
 
     def slice(self, z, dz=0.5, submap=0, cap=1 << 22):
-        torch = self.torch
-        dev = torch.device("cuda", torch.cuda.current_device())
-        xyz = torch.empty((cap, 3), dtype=torch.float32, device=dev)
-        val = torch.empty(cap, dtype=torch.float32, device=dev)
-        cnt = torch.zeros(1, dtype=torch.int32, device=dev)
-        self.extract_slice(submap, z, dz, xyz, val, None, cnt)
-        n = int(cnt.item())
-        k = min(n, cap)
-        return n, xyz[:k].cpu().numpy(), val[:k].cpu().numpy()
+        f32 = self.torch.float32
+        return capi.extract(lambda cnt, xyz, val: self.extract_slice(submap, z, dz, xyz, val, None, cnt), cap, ((3,), f32), ((), f32))
 
     def marching_cubes(self, step=1, thres=0.1, cap_tri=1 << 21, color=False):
         torch = self.torch
-        dev = torch.device("cuda", torch.cuda.current_device())
+        dev = capi.device()
         v = torch.empty((3 * cap_tri, 3), dtype=torch.float32, device=dev)
         nrm = torch.empty((3 * cap_tri, 3), dtype=torch.float32, device=dev)
+        col = torch.empty((3 * cap_tri, 3), dtype=torch.float32, device=dev) if color else None
         n = C.c_int64(0)
-        if color:
-            col = torch.empty((3 * cap_tri, 3), dtype=torch.float32, device=dev)
-            rc = self.L.tslam_mc_generate2(self.h, int(step), float(thres), cap_tri, capi.tptr(v), capi.tptr(nrm), capi.tptr(col),
-                                           C.byref(n), capi.stream_ptr())
-        else:
-            rc = self.L.tslam_mc_generate(self.h, int(step), float(thres), cap_tri, capi.tptr(v), capi.tptr(nrm), C.byref(n),
-                                          capi.stream_ptr())
+        rc = self.L.tslam_mc_generate2(self.h, int(step), float(thres), cap_tri, capi.tptr(v), capi.tptr(nrm), capi.tptr(col), C.byref(n),
+                                       capi.stream_ptr())
         if rc != capi.E_CAPACITY:
             capi.check(rc)
         k = min(int(n.value), cap_tri)
@@ -334,39 +252,17 @@ class TsdfHandle:
         return int(n.value), v[:3 * k].cpu().numpy(), nrm[:3 * k].cpu().numpy()
 
     # -- planner queries (batched @ti.func helpers of BaseMap, mapping_common.py:165-204) ------------------
-    def _dev_f32(self, a):
-        torch = self.torch
-        if isinstance(a, torch.Tensor):
-            return a.to(device="cuda", dtype=torch.float32).contiguous()
-        return torch.from_numpy(np.ascontiguousarray(a, dtype=np.float32)).cuda()
-
     def query_points(self, xyz, submap=0):
         """(is_pos_occupy, is_pos_unobserved) per point."""
-        torch = self.torch
-        x = self._dev_f32(xyz)
-        f = torch.empty(x.shape[0], dtype=torch.uint8, device=x.device)
-        capi.check(self.L.tslam_tsdf_query_points(self.h, int(submap), x.shape[0], capi.tptr(x), capi.tptr(f), capi.stream_ptr()))
-        f = f.cpu().numpy()
+        f = capi.query_flags(self.L.tslam_tsdf_query_points, self.h, xyz, submap)
         return (f & 1).astype(bool), (f & 2).astype(bool)
 
     def query_near_occupy(self, xyz, voxel, submap=0):
-        torch = self.torch
-        x = self._dev_f32(xyz)
-        f = torch.empty(x.shape[0], dtype=torch.uint8, device=x.device)
-        capi.check(self.L.tslam_tsdf_query_near_occupy(self.h, int(submap), x.shape[0], capi.tptr(x), int(voxel), capi.tptr(f), capi.stream_ptr()))
-        return f.cpu().numpy().astype(bool)
+        return capi.near_occupy(self.L.tslam_tsdf_query_near_occupy, self.h, xyz, voxel, submap)
 
     def raycast(self, pos, direction, max_dist, submap=0):
         """BaseMap.raycast for a batch of rays: (hit, last position, length)."""
-        torch = self.torch
-        p, d = self._dev_f32(pos), self._dev_f32(direction)
-        n = p.shape[0]
-        hit = torch.empty(n, dtype=torch.uint8, device=p.device)
-        xyz = torch.empty((n, 3), dtype=torch.float32, device=p.device)
-        ln = torch.empty(n, dtype=torch.float32, device=p.device)
-        capi.check(self.L.tslam_tsdf_raycast(self.h, int(submap), n, capi.tptr(p), capi.tptr(d), float(max_dist), capi.tptr(hit), capi.tptr(xyz),
-                                             capi.tptr(ln), capi.stream_ptr()))
-        return hit.cpu().numpy().astype(bool), xyz.cpu().numpy(), ln.cpu().numpy()
+        return capi.raycast(self.L.tslam_tsdf_raycast, self.h, pos, direction, max_dist, submap)
 
     def esdf_update(self, submap=0):
         sw = C.c_int32(0)
@@ -403,33 +299,16 @@ class TsdfHandle:
     def esdf_gather(self, submap=0):
         torch = self.torch
         cap = self.count_active(submap)
-        dev = torch.device("cuda", torch.cuda.current_device())
-        idx = torch.empty((max(cap, 1), 3), dtype=torch.int32, device=dev)
-        e = torch.empty(max(cap, 1), dtype=torch.float32, device=dev)
-        n = C.c_int64(0)
-        capi.check(self.L.tslam_esdf_gather(self.h, int(submap), cap, capi.tptr(idx), capi.tptr(e), C.byref(n),
-                                            capi.stream_ptr()))
-        k = int(n.value)
-        return idx[:k].cpu().numpy(), e[:k].cpu().numpy()
+        idx, e = capi.count_fill(lambda cap, n, idx, e: self.L.tslam_esdf_gather(self.h, int(submap), cap, idx, e, n, capi.stream_ptr()),
+                                 ((3,), torch.int32), ((), torch.float32), cap=cap)
+        return idx.cpu().numpy(), e.cpu().numpy()
 
     def esdf_query(self, xyz, submap=0):
         """Trilinear ESDF and its exact gradient at points [n,3] of the submap's map frame, as of the last esdf_update of
         `submap`: (dist f32[n], grad f32[n,3], valid bool[n]); dist and grad are NaN where valid is False.
         A torch CUDA tensor in -> torch CUDA tensors out, enqueued on the current stream without a host synchronisation
         (a planner's torch loop can call it); a numpy array in -> numpy arrays out."""
-        torch = self.torch
-        as_torch = isinstance(xyz, torch.Tensor)
-        x = self._dev_f32(xyz).reshape(-1, 3)
-        n = x.shape[0]
-        dist = torch.empty(n, dtype=torch.float32, device=x.device)
-        grad = torch.empty((n, 3), dtype=torch.float32, device=x.device)
-        valid = torch.empty(n, dtype=torch.uint8, device=x.device)
-        capi.check(self.L.tslam_esdf_query(self.h, int(submap), n, capi.tptr(x), capi.tptr(dist), capi.tptr(grad), capi.tptr(valid),
-                                           capi.stream_ptr()))
-        valid = valid.view(torch.bool)  # the kernel writes 0 / 1
-        if as_torch:
-            return dist, grad, valid
-        return dist.cpu().numpy(), grad.cpu().numpy(), valid.cpu().numpy()
+        return capi.esdf_query(self.L.tslam_esdf_query, self.h, xyz, submap)
 
     def trajectory(self, ctrls, clearance, submap=0, **settings):
         """Optimise uniform cubic B-splines (control points f[N,3] each, the submap's map frame) against the ESDF of
@@ -445,15 +324,8 @@ class TsdfHandle:
 
     def esdf_slice(self, z, submap=0, cap=1 << 22):
         """cvt_ESDF_to_voxels_slice (dense_esdf.py:498-509) as of the last esdf_update: (demand, xyz, ESDF) numpy."""
-        torch = self.torch
-        dev = torch.device("cuda", torch.cuda.current_device())
-        xyz = torch.empty((max(cap, 1), 3), dtype=torch.float32, device=dev)
-        val = torch.empty(max(cap, 1), dtype=torch.float32, device=dev)
-        cnt = torch.zeros(1, dtype=torch.int32, device=dev)
-        self.esdf_extract_slice(submap, z, xyz[:cap], val[:cap], cnt)
-        n = int(cnt.item())
-        k = min(n, cap)
-        return n, xyz[:k].cpu().numpy(), val[:k].cpu().numpy()
+        f32 = self.torch.float32
+        return capi.extract(lambda cnt, xyz, val: self.esdf_extract_slice(submap, z, xyz, val, cnt), cap, ((3,), f32), ((), f32))
 
     # -- SDF-to-SDF registration of submap pairs (tslam_tsdf_register) -------------------------------------
     def register(self, reading, ref_submaps, read_submaps, R0, T0, band, min_weight=0.0, huber=None, max_iters=20,
@@ -487,7 +359,7 @@ class TsdfHandle:
         n = sm.shape[0]
         M9 = np.ascontiguousarray(np.asarray(M, dtype=np.float64).reshape(n, 9).astype(np.float32))
         params = capi.PlaceParams(float(r_max), float(h_min), float(band), float(min_weight))
-        dev = torch.device("cuda", torch.cuda.current_device())
+        dev = capi.device()
         rows = max(n, 1)
         sc = torch.empty((rows, 20, 60), dtype=torch.float32, device=dev)
         ring = torch.empty((rows, 20), dtype=torch.float32, device=dev)
@@ -521,13 +393,7 @@ class TsdfHandle:
         frame's points lie on the zero level.  depth: uint16 [n,h,w] (or [h,w]) numpy (host) or torch CUDA tensor; Rs
         [n,3,3], Ts [n,3]: initial poses (f64, the frame of integrate_depth's Rs, Ts); submaps: per frame (default 0);
         step defaults to recast_step, huber to the voxel scale.  -> dict of numpy arrays keyed like register()."""
-        torch = self.torch
-        if isinstance(depth, torch.Tensor):
-            assert depth.is_cuda and depth.dtype in (torch.uint16, torch.int16) and depth.is_contiguous()
-            mem, ptr, shape = capi.MEM_DEVICE, capi.tptr(depth), tuple(depth.shape)
-        else:
-            depth = np.ascontiguousarray(depth, dtype=np.uint16)
-            mem, ptr, shape = capi.MEM_HOST, capi.np_ptr(depth), depth.shape
+        depth, mem, ptr, shape = capi.source(depth, np.uint16, (self.torch.uint16, self.torch.int16))
         if len(shape) == 2:
             shape = (1,) + tuple(shape)
         n, h, w = shape
@@ -540,14 +406,8 @@ class TsdfHandle:
         """Track one point cloud xyz [n,3] (sensor frame; numpy or torch CUDA f32) against submap `submap`: points that are
         not finite or whose range lies outside [min_ray_length, max_ray_length) are dropped.  R [3,3], T [3]: initial pose
         (f64).  -> dict of numpy arrays keyed like register(), one row."""
-        torch = self.torch
-        if isinstance(xyz, torch.Tensor):
-            assert xyz.is_cuda and xyz.dtype == torch.float32 and xyz.is_contiguous()
-            mem, ptr, n = capi.MEM_DEVICE, capi.tptr(xyz), xyz.shape[0]
-        else:
-            xyz = np.ascontiguousarray(np.asarray(xyz, dtype=np.float32).reshape(-1, 3))
-            mem, ptr, n = capi.MEM_HOST, capi.np_ptr(xyz), xyz.shape[0]
-        return self._track("tslam_tsdf_track_points", 1, ((ptr, mem, n, int(submap)), ()), R, T, huber, max_iters, min_points)
+        xyz, mem, ptr, shape = capi.source(xyz, np.float32, (self.torch.float32,), (-1, 3))
+        return self._track("tslam_tsdf_track_points", 1, ((ptr, mem, shape[0], int(submap)), ()), R, T, huber, max_iters, min_points)
 
     # -- rendering (tslam_tsdf_render) -----------------------------------------------------
     def render(self, Rs, Ts, height, width, K9, submaps=None, z_min=None, z_max=None, step=None, normals=True, color=False):
@@ -565,7 +425,7 @@ class TsdfHandle:
         z_min = float(self.cfg.min_ray_length) if z_min is None else float(z_min)
         z_max = float(self.cfg.max_ray_length) if z_max is None else float(z_max)
         step = float(self.cfg.voxel_scale) if step is None else float(step)
-        dev = torch.device("cuda", torch.cuda.current_device())
+        dev = capi.device()
         h, w = int(height), int(width)
         depth = torch.empty((n, h, w), dtype=torch.float32, device=dev)
         status = torch.empty((n, h, w), dtype=torch.uint8, device=dev)
@@ -612,19 +472,3 @@ class TsdfHandle:
         capi.check(self.L.tslam_tsdf_get_march_stats2(self.h, capi.np_ptr(o)))
         return dict(n_segs=int(o[0]), n_items=int(o[1]), n_slow=int(o[2]), n_fallback=int(o[3]), n_generic=int(o[4]),
                     n_verify_bad=int(o[5]), n_seg_guard=int(o[6]))
-
-
-def _include_u8(include, n):
-    """include of the fusion updates (None or bools / 0-1 per submap) -> None or u8[n], n the submap table size."""
-    if include is None:
-        return None
-    a = np.asarray(include).reshape(-1).astype(bool)
-    assert a.shape[0] <= n, "include has more entries than max_submaps"
-    inc = np.zeros(n, np.uint8)
-    inc[:a.shape[0]] = a
-    return inc
-
-
-def _fuse_stats(st, reasons):
-    return dict(full=bool(st[0] != 0), reason=reasons[int(st[0])], added=int(st[1]), moved=int(st[2]), removed=int(st[3]),
-                within_tolerance=int(st[4]), voxels_splatted=int(st[5]), voxels_skipped=int(st[6]), blocks_committed=int(st[7]))

@@ -312,6 +312,17 @@ def test_refusals():
     assert same(w.union(), before)
 
 
+def test_plan_present_has_the_c_side_submap_table():
+    """max_submaps = 0 gives the C side's 1024-entry table: the plan's present array has 1024 entries."""
+    from taichislam_b200.tsdf_handle import TsdfHandle
+    src = TsdfHandle(128, 128, voxel_scale=0.05, K=K, max_ray_length=3.0, max_submaps=0)
+    dst = TsdfHandle(256, 256, voxel_scale=0.05, K=K, max_ray_length=3.0, is_global_map=True, max_submaps=0)
+    src.integrate_depth(DEPTH, np.eye(3)[None], np.zeros((1, 3)), submaps=[3])
+    plan, present = dst.fuse_update_tiled_plan(src, (1, 1, 1), 0, 1)
+    assert present.shape == (1024,) and np.flatnonzero(present).tolist() == [3]
+    dst.fuse_update_tiled_finish(src, False)
+
+
 def test_pool_exhaustion_on_an_owner_fails_every_rank_and_the_next_update_is_full():
     # rank 1 contributes nothing, so its pool fills only with the blocks it receives: size it between what the first
     # and the second update need

@@ -383,6 +383,22 @@ def test_pool_exhaustion_is_reported():
     assert e.value.code == capi.E_POOL_FULL
 
 
+def test_submap_table_outside_the_limit_sizes_include_like_the_c_side():
+    """max_submaps = 0 gives the C side's 1024-entry table, so include masks take 1024 entries, as on a 1024 pair."""
+    include = [True, False, True]
+    out = []
+    for m in (0, 1024):
+        src, dst = handle(128, False, max_submaps=m), handle(256, True, max_submaps=m)
+        for s in range(3):
+            add_sphere(src, s)
+        set_poses(dst, {s: pose_of(s) for s in range(3)})
+        out.append((dst.fuse_update(src, include=include), rows(dst)))
+        src.close()
+        dst.close()
+    assert out[0][0] == out[1][0] and out[0][0]["added"] == 2
+    assert same(out[0][1], out[1][1]) and out[0][1][0].shape[0] > 0
+
+
 def test_refusals_that_need_handles():
     import torch
     src, dst = handle(128, False), handle(256, True)
